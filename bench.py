@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- FAcodec encode -> quantize -> decode throughput on B200 (BASELINE.json metric).
+"""bench.py -- FAcodec encode -> quantize -> decode throughput on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path (encoder -> quantizer(n_c=2, codes) -> decoder) over one
 batch of synthetic 4 s 24 kHz utterances (PseudoDataset law, meldataset.py:67-68); the workload
@@ -9,14 +9,16 @@ is BASELINE configs[1]: 32 utterances per GPU (weak scaling: every rank gets its
 Prints ONE JSON line on rank 0 (contract in the task statement):
   value      = audio-seconds per second, whole job, inputs resident in HBM (CUDA events, max over ranks)
   e2e        = same metric through Codec.forward_host: pinned HOST buffers, H2D + D2H inside the timed region
-  roofline   = dominant kernel family (the two tcgen05 conv kernels conv_tc_kernel + conv_tcp_kernel, ~80 % of a step):
+  roofline   = dominant kernel family (the wgmma conv kernel conv_tc_kernel, plain and promoted launches):
                algorithmic FLOPs / device time, from CUDA events recorded around every launch in a separate
-               instrumented pass (fac_profile_*); traffic = DRAM bytes per launch of that family from the committed
-               ncu launch list (profiles/roofline_r02.json)
+               instrumented pass (fac_profile_*)
   cpu_baseline = the oracle port (oracle/facodec_oracle.py = the reference's own ATen call sequence)
                timed on this box's host cores on a bounded sample
---impl reference times that CPU path alone (the reference is 100% Python/PyTorch; /root/reference is
-not on the GPU box, so the validated restatement stands in: kind "port").
+--impl reference times that CPU path alone (the reference is 100% Python/PyTorch; the validated restatement
+stands in for it: kind "port").
+--dump-outputs DIR writes what the last timed step of the codec workload returned (y, the three code tensors, timbre)
+as DIR/<name>.npy (float32; codes as float64), so that two builds can be compared output for output: the inputs are
+seeded and identical from run to run.
 """
 import argparse
 import json
@@ -46,7 +48,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- never reached, an upper bound only
+    return dict(hbm_gbs=3350.0, tflops=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -96,6 +99,17 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
+def dump_outputs(out_dir, outputs):
+    """The codec step's outputs (y, [codes_p, codes_c, codes_r], timbre) as <name>.npy: float32, codes as float64."""
+    import numpy as np
+    y, codes, timbre = outputs
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"y": y.float(), "codes_p": codes[0].double(), "codes_c": codes[1].double(), "codes_r": codes[2].double(),
+              "timbre": timbre.float()}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
+
+
 def usable_cores():
     """Host threads this process may actually use: min(cpu_count, affinity mask, cgroup CPU quota)."""
     n = os.cpu_count() or 1
@@ -133,7 +147,7 @@ def cpu_reference_run(steps, warmup, sample_utts=4):
 
 def library_baseline(x, dev, steps=2):
     """SURVEY.md 8(d) "library" baseline: the reference's ATen call sequence (the oracle restatement = what the reference's
-    nn.Modules execute: cuDNN convs / LSTM, cuBLAS, cuFFT) run by PyTorch eager on the same B200, fp32 with TF32 disabled,
+    nn.Modules execute: cuDNN convs / LSTM, cuBLAS, cuFFT) run by PyTorch eager on the same GPU, fp32 with TF32 disabled,
     on one configs[1] batch.  Returns None when it cannot run (e.g. out of memory)."""
     import torch
     from facodec_b200 import synth
@@ -219,7 +233,7 @@ def vq_bench(args, rank, local_rank, world):
                           "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32 / int64", "data": "synthetic",
                           "config": {"workload": "BASELINE configs[3]: FVQ+RVQ codebook-distance microbench, 1024-dim latents x 4 codebooks "
                                                  "x 1024 entries, 2^20 frames per GPU (B=1024, T=1024), channels-last",
-                                     "l2": "8.6 GB of input + output per step >> 126 MB L2"},
+                                     "l2": "8.6 GB of input + output per step >> 50 MB L2"},
                           "roofline": {"kernel": "rvq_kernel (warp per frame)", "bound": "hbm", "achieved": gbs, "peak": peaks["hbm_gbs"],
                                        "unit": "GB/s", "frac": gbs / peaks["hbm_gbs"], "traffic": None,
                                        "algorithmic_bytes_per_frame": bytes_per_frame, "peak_source": peaks["source"]},
@@ -233,7 +247,7 @@ def trainfwd_bench(args, rank, local_rank, world):
     """BASELINE configs[4], the part of it this repo builds: the training step's FORWARD (encoder -> quantizer n_c=2 ->
     decoder, train.py:265-272, eval-mode arithmetic) plus the forward of the reference's own reconstruction loss
     (losses.py:65-89) between input and reconstruction, fp32-faithful, 8 utterances x 4 s per GPU (batch 64 on 8 GPUs).
-    No backward, no discriminators, no audiotools losses (DESIGN.md section 0, row f3).  Parity: the loss value of the first
+    No backward, no discriminators, no audiotools losses.  Parity: the loss value of the first
     timed batch against the CPU oracle fed with the GPU's reconstruction."""
     import torch
     import torch.distributed as dist
@@ -321,7 +335,13 @@ def main():
     ap.add_argument("--workload", default="codec", choices=["codec", "vq", "trainfwd"],
                     help="codec = BASELINE configs[1] (the headline); vq = configs[3] FVQ/RVQ codebook-distance microbench; "
                          "trainfwd = the forward half of configs[4] (codec forward + losses.reconstruction_loss)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (codec workload, --impl ours)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "codec" or args.impl != "ours"):
+        ap.error("--dump-outputs applies to the codec workload with --impl ours")
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -330,7 +350,7 @@ def main():
                           "forward (encoder -> quantizer n_c=2 with codes -> decoder), reference config.yml geometry",
               "utterances_per_gpu": BATCH_PER_GPU, "utterance_samples": UTT_SAMPLES,
               "parallelism": f"dp{world} (utterance sharding, replicas, no hot-path collective)",
-              "l2": "per-step working set (~10 GB of activations) >> 126 MB L2; inputs rotate over 4 distinct batches"}
+              "l2": "per-step working set (~10 GB of activations) >> 50 MB L2; inputs rotate over 4 distinct batches"}
 
     if args.workload == "vq":
         return vq_bench(args, rank, local_rank, world)
@@ -410,8 +430,15 @@ def main():
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    ms_total = timed(lambda i: codec.forward(xs[i % nrot], n_c=2), args.steps)
+    last = [None]
+
+    def step(i):
+        last[0] = codec.forward(xs[i % nrot], n_c=2)
+
+    ms_total = timed(step, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0])
     launches = codec.launch_count() * args.steps
     audio_s = world * BATCH_PER_GPU * UTT_SECONDS * args.steps
     value = audio_s / (ms_total * 1e-3)
@@ -439,41 +466,31 @@ def main():
     torch.cuda.synchronize()
     L.fac_profile_enable(h, 0)
     fam = {}
-    for name in ("conv_tc", "conv_tcp", "conv_tt", "conv", "lstm_rec", "fa_quantize"):
+    for name in ("conv_tc", "conv_tcp", "conv", "lstm_rec", "fa_quantize"):
         ms, fl, by, n = ctypes.c_double(), ctypes.c_double(), ctypes.c_double(), ctypes.c_longlong()
         L.fac_profile_get(h, name.encode(), ctypes.byref(ms), ctypes.byref(fl), ctypes.byref(by), ctypes.byref(n))
         fam[name] = dict(ms=ms.value / nprof, flops=fl.value / nprof, bytes=by.value / nprof, launches=n.value // nprof)
     L.fac_profile_reset(h)
-    # dominant kernels: the two tcgen05 conv kernels (same mainloop; conv_tcp adds register promotion)
-    conv = {k: fam["conv_tc"][k] + fam["conv_tcp"][k] + fam["conv_tt"][k] for k in ("ms", "flops", "bytes", "launches")}
+    # dominant kernels: the wgmma conv kernel (conv_tcp = its promoted launches)
+    conv = {k: fam["conv_tc"][k] + fam["conv_tcp"][k] for k in ("ms", "flops", "bytes", "launches")}
     conv_tflops = conv["flops"] / (conv["ms"] * 1e-3) / 1e12 if conv["ms"] > 0 else 0.0
-    traffic, traffic_src = None, None
-    try:
-        rj = json.load(open(os.path.join(ROOT, "profiles", "roofline_r02.json")))
-        traffic = rj["conv_family"]["dram_bytes_per_launch"]
-        traffic_src = rj["conv_family"]["source"]
-    except Exception:
-        pass
-    pipe_ops = 3.0 * fam["conv_tc"]["flops"] + 6.0 * fam["conv_tcp"]["flops"] + 3.0 * fam["conv_tt"]["flops"]   # bf16-equivalent tensor work issued
-    roofline = {"kernel": "tcgen05 conv family: conv_tc_kernel (kind::f16, bf16 hi/lo split, layers downstream of the VQ) + "
-                          "conv_tt_kernel (transposed formulation, time = MMA N = 256, fp16 hi + scaled-lo split with "
-                          "register-promoted accumulation, layers upstream of the VQ; conv_tcp_kernel is its TF32 fallback): all "
-                          "eligible Conv1d/ConvTranspose1d/Linear layers",
-                "family_ms_per_step": {k: fam[k]["ms"] for k in ("conv_tc", "conv_tcp", "conv_tt")},
+    pipe_ops = 3.0 * fam["conv_tc"]["flops"] + 3.0 * fam["conv_tcp"]["flops"]   # 16-bit-equivalent tensor work issued (3-pass splits)
+    roofline = {"kernel": "wgmma conv family: conv_tc_kernel (bf16 hi/lo split or one fp16 pass, layers downstream of the VQ; "
+                          "fp16 hi + scaled-lo split with register-promoted accumulation upstream of the VQ): all eligible "
+                          "Conv1d/ConvTranspose1d/Linear layers",
+                "family_ms_per_step": {k: fam[k]["ms"] for k in ("conv_tc", "conv_tcp")},
                 "bound": "tensor", "achieved": conv_tflops, "peak": peaks["tflops"], "unit": "TFLOP/s",
-                "frac": conv_tflops / peaks["tflops"], "traffic": traffic, "traffic_source": traffic_src,
-                "peak_source": f"{peaks['source']} bf16 dense sustained (MEASURED_PEAKS.json)",
+                "frac": conv_tflops / peaks["tflops"],
+                "peak_source": f"{peaks['source']} bf16 dense",
                 "note": "achieved counts ALGORITHMIC fp32 FLOPs (2*MACs) per launch / mean launch time; an fp32-faithful "
-                        "product costs 3 MMAs (bf16 / fp16 splits; 3 half-rate MMAs for the TF32 fallback), so the tensor pipe does >= 3x "
-                        "this work; traffic is DRAM read+write bytes per launch (ncu), to compare with "
-                        "per_launch.algorithmic_gb_per_step / launches_per_step",
+                        "product costs 3 MMAs (bf16 / fp16 splits), so the tensor pipe does up to 3x this work",
                 "tensor_pipe_frac_est": pipe_ops / (conv["ms"] * 1e-3) / 1e12 / peaks["tflops"] if conv["ms"] > 0 else 0.0,
                 "per_launch": {"launches_per_step": conv["launches"], "avg_ms": conv["ms"] / max(1, conv["launches"]),
                                "algorithmic_gflop_per_step": conv["flops"] / 1e9,
                                "algorithmic_gb_per_step": conv["bytes"] / 1e9,
                                "achieved_gbs": conv["bytes"] / (conv["ms"] * 1e-3) / 1e9 if conv["ms"] > 0 else 0.0},
                 "share_of_step": conv["ms"] / (ms_total / args.steps),
-                "other_families_ms_per_step": {k: v["ms"] for k, v in fam.items() if k not in ("conv_tc", "conv_tcp", "conv_tt")},
+                "other_families_ms_per_step": {k: v["ms"] for k, v in fam.items() if k not in ("conv_tc", "conv_tcp")},
                 "whole_path": {"hbm_roofline_audio_s_per_s": peaks["hbm_gbs"] * 1e3 / MB_PER_AUDIO_S,
                                "tensor_roofline_audio_s_per_s": peaks["tflops"] * 1e3 / GFLOP_PER_AUDIO_S,
                                "frac_of_hbm_roofline": value / world / (peaks["hbm_gbs"] * 1e3 / MB_PER_AUDIO_S),

@@ -1,4 +1,4 @@
-"""facodec_b200 -- B200-native FAcodec encode -> quantize -> decode hot path (sm_100a CUDA
+"""facodec_b200 -- H100-native FAcodec encode -> quantize -> decode hot path (sm_90a CUDA
 behind the reference's model.encoder / model.quantizer / model.decoder call surface)."""
 from .modules import (Activation1d, CNNLSTM, Codec, CodecStream, Decoder, Encoder, Engine, FApredictors, FAquantizer, Munch,  # noqa: F401
                       Redecoder, ResidualVQ, VoiceConverter, build_model)

@@ -1,6 +1,6 @@
-// Shared device helpers for the FAcodec sm_100a hot path.
+// Shared device helpers for the FAcodec sm_90a hot path.
 // Activations are CHANNELS-LAST fp32: a tensor the reference calls [B, C, T] lives in HBM as
-// [B][T][C] ("frames x channels"); see DESIGN.md "Data layout in HBM".
+// [B][T][C] ("frames x channels").
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

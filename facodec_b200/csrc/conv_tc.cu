@@ -1,4 +1,4 @@
-// Channels-last 1-D convolution on the 5th-gen tensor cores (tcgen05, sm_100a), fp32-faithful.
+// Channels-last 1-D convolution on the Hopper tensor cores (wgmma, sm_90a), fp32-faithful.
 //
 // Same contract as conv_simt.cu (SConv1d / SConvTranspose1d / Linear call sites of the
 // reference), restricted to stride-1 convs in "rows" (a strided down-conv with kernel 2s is a
@@ -9,33 +9,26 @@
 // Precision: bit-exact VQ indices need fp32-faithful sums (SURVEY.md 0.5), so every product is
 // formed as 3 MMAs over split operands (x = hi + lo):
 //   a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi     (dropped term a_lo*b_lo ~ 2^-22 |ab|)
-// with fp32 accumulation in TMEM.  Weights are split offline; activations are split in-kernel.
-// Split classes: TF32 pairs (kind::tf32, K = 8) upstream of the VQ; bf16 pairs (kind::f16, K = 16) downstream;
-// experimental fp16 hi + 2^11-scaled fp16 lo upstream (conv_tcp_kernel<true>).
+// Weights are split offline (tc_pack_blob); activations are split in-kernel.  Split classes:
+//   TF32 pairs (k = 8 MMAs); bf16 pairs (k = 16) downstream of the VQ; ONE fp16 pass (g1f16: the k = 7 convs
+//   downstream of the VQ); fp16 hi + 2^11-scaled fp16 lo (f16x2, promoted only).
+// Promoted layers (upstream of the VQ, long K loops) accumulate each window of <= 48 chained MMAs in fresh
+// registers and add it to an fp32 master accumulator, so the sum is not one long tensor-core accumulation chain.
 //
-// Two kernels share the operand pipeline:
-//   conv_tc_kernel<FUSED, BF16, G1F16, NW, NG>  accumulates in TMEM only (decoder, short K loops); 2 control warps + NW = 8
-//                                worker warps, planned for two CTAs per SM wherever the tile fits 256 TMEM columns / 112 KB,
-//                                or NW = 16 when a tile owns the SM; NG = 2 producer groups on alternate chunks where a
-//                                group covers a chunk in <= 5 pieces per thread; FUSED = a whole ResidualUnit; G1F16 = the
-//                                layer's own GEMM in ONE fp16 pass (k = 7 convs downstream of the VQ).
-//   conv_tcp_kernel<F16>         promotes TMEM accumulators into fp32 registers every <= 48 MMAs (everything upstream of
-//                                the VQ with a long K loop); 20 warps re-allocated with setmaxnreg, persistent.
-// Roles in conv_tc_kernel (the promoted kernel splits the last group into producers and accumulators):
-//   warp 0    : weight producer -- one elected lane streams pre-arranged [tap][16 ci] weight
-//               blobs (hi|lo, already in the UMMA K-major core-matrix layout) with 1-D bulk
-//               TMA copies (cp.async.bulk, UBLKCP) into an mbarrier ring of 2-4 slots; a slot holds every tap of
-//               `cps` consecutive chunks (tc_conv_plan).
-//   warp 1    : TMEM allocator + MMA issuer -- converged warp, every tcgen05.mma / tcgen05.commit predicated by
-//               elect.sync inside its asm block; slot > chunk > tap loop nest with the taps unrolled and every invariant
-//               pinned in a register (issue_taps): ~27 instructions per tap instead of ~440 cycles of dependent scalar work.
-//   warps 2.. : activation producers, then epilogue.  Per 16-channel chunk they load the UNION
-//               of the rows all taps need (128*MT + (K-1)*dil rows) once from HBM with 16-byte
-//               loads (reflect/zero padding = index map, no padded copy), apply Snake, split into
-//               hi/lo and store them in a no-swizzle K-major layout whose row pitch is a uniform
-//               16 bytes, so each tap is just a descriptor start-address offset of tap*dil rows
-//               (taps are never re-loaded or im2col'ed).  Epilogue: tcgen05.ld -> shared-memory transpose ->
-//               bias -> Snake/tanh/Mish -> residual -> coalesced 128-byte row segments.
+// CTA = two warpgroups over a tile of 128 rows x N channels (each warpgroup 64 rows) or 64 rows x N channels (each
+// warpgroup N/2 channels).  Per 16-channel chunk:
+//   weights: one thread streams the chunk's pre-arranged [tap][hi|lo][k-piece][N][16 B] blob with ONE 1-D bulk copy
+//            (cp.async.bulk, completion on an mbarrier) into a ring of 1-2 slots;
+//   activations: all 256 threads load the UNION of the rows all taps need (rows + (K-1)*dil) once with 16-byte loads
+//            (reflect / zero padding = index map, no padded copy), apply Snake, split into hi/lo and store them in a
+//            no-swizzle K-major layout whose row pitch is a uniform 16 bytes, so each tap is just a descriptor
+//            start-address offset of tap*dil rows (taps are never re-loaded or im2col'ed);
+//   the next chunk's activations are produced while this chunk's wgmma run (double-buffered operand).
+// Fused mode (a whole ResidualUnit, conv7 -> +b7 -> Snake -> 1x1 conv -> +b1 -> +x): GEMM 1's accumulators go through
+// bias + Snake + split straight into a resident shared-memory operand for GEMM 2.
+// Epilogue from the accumulator registers: bias -> Snake/tanh/Mish -> residual -> 8-byte stores.
+// Variants: tiles planned for two resident CTAs per SM (option "tc_occ2_maxn"), and the transposed formulation of the
+// promoted fp16 class (option "encoder_tt": weights as the wgmma A operand, time as wgmma N).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -48,1031 +41,357 @@
 
 namespace fac {
 
-// Kernel-tuning aid (fac_debug_tc_phase_clocks).  conv_tc_kernel: phase timestamps (clock64) of one probe CTA of the last
-// launch.  conv_tcp_kernel (persistent): totals over CTA 3's whole tile list -- [0] cycles the CTA ran, [1] producers waiting
-// for a free operand buffer, [2]/[3]/[4] MMA warp waiting for operands / weights / a free TMEM buffer, [5] accumulators
-// waiting for MMAs, [6] accumulators in the epilogue, [7] tiles processed.
-__device__ long long g_tc_phase_clock[8];
-// conv_tc_kernel, probe producer thread, totals over the tile's chunks: [0] waiting for a free operand buffer, [1] waiting
-// for the chunk's global loads to land, [2] Snake + split + stores + arrive, [3] chunks
-__device__ long long g_tc_prod_clock[4];
-// per-chunk timeline of the probe CTA (absolute clock64, same SM): [0][c] MMA warp saw chunk c's operands, [1][c] MMA warp
-// done issuing chunk c (MMAs + commits), [2][c] producer thread 0 saw buffer free for chunk c, [3][c] producer thread 0
-// arrived for chunk c, [4][c] cycles the MMA warp waited for weights inside chunk c
-__device__ long long g_tc_trace[5][16];
+namespace {
 
+using namespace tc;
 
-// One chunk of the K loop issued by the (converged) MMA warp: KR taps x MT accumulators x NPASS split passes x K steps.
-// Every operand is a pre-pinned register; a tap is +dil rows on the A descriptor and +b1_16 on the B descriptor.
-__device__ __forceinline__ void pin_u(uint32_t& v) { v = __shfl_sync(0xffffffffu, v, 0); }
-__device__ __forceinline__ void pin_i(int& v) { v = __shfl_sync(0xffffffffu, v, 0); }
-struct IssueCtx {
-    uint32_t idesc, a_half16, b_half16, a_lbo16, b_lbo16, b1_16, dil, N;
-    int MT;
+enum Prec { P_TF32 = 0, P_BF16 = 1, P_F16S = 2, P_F16X2 = 3, P_NONE = -1 };
+
+template <int P> struct PrecT {
+    static constexpr int KG = P == P_TF32 ? 4 : 2;           // 16-byte k-pieces per 16-channel chunk and plane
+    static constexpr int planes = P == P_F16S ? 1 : 2;       // hi (+ lo)
+    static constexpr int ksteps = P == P_TF32 ? 2 : 1;       // MMAs per chunk, tap and split pass
+    static constexpr int kind = P == P_TF32 ? WG_TF32 : (P == P_BF16 ? WG_BF16 : WG_F16);
 };
-template <bool BF16, int NPASS, int KR>
-__device__ __forceinline__ void issue_taps(const IssueCtx& ic, uint32_t d_tmem0, uint32_t a_w, uint32_t b_w, bool first) {
-    constexpr int KSTEPS = BF16 ? 1 : 2;
+
+__host__ __device__ constexpr int prec_kg(int P) { return P == P_TF32 ? 4 : 2; }
+__host__ __device__ constexpr int prec_planes(int P) { return P == P_F16S ? 1 : 2; }
+
+template <int NI, int NS>
+__device__ __forceinline__ void zero_acc(float (&a)[NS][NI / 2]) {
 #pragma unroll
-    for (int tap = 0; tap < KR; ++tap) {
-        uint32_t a_t = a_w + (uint32_t)tap * ic.dil, d_t = d_tmem0;
-        const uint32_t b_t = b_w + (uint32_t)tap * ic.b1_16;
-#pragma unroll 1
-        for (int mt = 0; mt < ic.MT; ++mt, a_t += 128, d_t += ic.N) {
+    for (int s = 0; s < NS; ++s)
 #pragma unroll
-            for (int pass = 0; pass < NPASS; ++pass) {
-                const uint32_t aa = a_t + (pass == 2 ? ic.a_half16 : 0u);
-                const uint32_t bb = b_t + (pass == 1 ? ic.b_half16 : 0u);
+        for (int i = 0; i < NI / 2; ++i) a[s][i] = 0.f;
+}
+
+// One operand pair (A rows x K-pieces, B channels x K-pieces) of one chunk, all sub-tiles of this warpgroup.
+template <int P, int NI, int NS>
+__device__ __forceinline__ void mma_pass(float (&acc)[NS][NI / 2], int nsub, uint32_t a_addr, uint32_t a_lbo, uint32_t b_addr,
+                                         uint32_t b_lbo) {
 #pragma unroll
-                for (int ks = 0; ks < KSTEPS; ++ks) {
-                    const uint32_t accum = (tap | pass | ks) != 0 ? 1u : (first ? 0u : 1u);
-                    uint64_t da, db;
-                    asm("mov.b64 %0, {%1, %2};" : "=l"(da) : "r"(aa + ks * 2 * ic.a_lbo16), "r"(0x4008u));
-                    asm("mov.b64 %0, {%1, %2};" : "=l"(db) : "r"(bb + ks * 2 * ic.b_lbo16), "r"(0x4008u));
-                    tc::umma<BF16>(d_t, da, db, ic.idesc, accum);
-                }
+    for (int ks = 0; ks < PrecT<P>::ksteps; ++ks) {
+        const uint64_t da = gdesc(a_addr + ks * 2 * a_lbo, a_lbo, 128);
+#pragma unroll
+        for (int s = 0; s < NS; ++s)
+            if (s < nsub) wgmma_ss<NI, PrecT<P>::kind>(acc[s], da, gdesc(b_addr + ks * 2 * b_lbo + s * NI * 16, b_lbo, 128));
+    }
+}
+
+struct Tile {
+    int row0, col0, nsub;     // this warpgroup's first tile row / channel, NI-wide sub-tiles
+    int warp, lane;
+};
+
+// Accumulator fragment of wgmma m64nNI: register 4j + 2h + e of sub-tile s holds row 16*warp + lane/4 + 8h,
+// column s*NI + 8j + 2*(lane%4) + e.
+template <int NI, int NS, typename F>
+__device__ __forceinline__ void for_each_pair(const Tile& tl, const float (&acc)[NS][NI / 2], F&& f) {
+#pragma unroll
+    for (int s = 0; s < NS; ++s) {
+        if (s >= tl.nsub) break;
+#pragma unroll
+        for (int j = 0; j < NI / 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = tl.row0 + 16 * tl.warp + (tl.lane >> 2) + 8 * h;
+                const int col = tl.col0 + s * NI + 8 * j + 2 * (tl.lane & 3);
+                f(row, col, acc[s][4 * j + 2 * h], acc[s][4 * j + 2 * h + 1]);
             }
-        }
     }
 }
 
-// GEMM-2 operand of a fused unit (see conv_tc_kernel): this warp's CW columns of every 16-channel chunk of D1, + b7, Snake,
-// hi/lo split, stored K-major into the resident operand; the TMEM load of chunk c2 + 1 stays in flight behind the
-// arithmetic on chunk c2.
-template <int CW>
-__device__ __forceinline__ void tmem_ldw_issue(uint32_t taddr, uint32_t (&v)[CW]) {
-    if constexpr (CW == 16) {
-        tc::tmem_ld16_issue(taddr, v);
-    } else if constexpr (CW == 8) {
-        tc::tmem_ld8_issue(taddr, v);
-    } else {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(taddr));
-    }
-}
-template <int CW>
-__device__ __forceinline__ void tmem_ldw_wait(uint32_t (&v)[CW]) {
-    if constexpr (CW == 16) {
-        tc::tmem_ld_wait16(v);
-    } else if constexpr (CW == 8) {
-        tc::tmem_ld_wait8(v);
-    } else {
-        asm volatile("tcgen05.wait::ld.sync.aligned;" : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]) :: "memory");
-    }
-}
-// One mbarrier arrival per WARP: every lane has fenced its own stores (fence.proxy.async), the warp converges, lane 0
-// arrives.  With one arrival per thread a chunk hand-off was 256-512 serialised shared-memory atomics.
-__device__ __forceinline__ void warp_arrive(uint64_t* bar) {
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) tc::mbar_arrive(bar);
-}
-// wait for two TMEM loads in flight (tcgen05.wait::ld covers every outstanding load of the thread; both register sets are
-// named so that no read of either can move above the wait)
-template <int CW>
-__device__ __forceinline__ void tmem_ldw_wait2(uint32_t (&a)[CW], uint32_t (&b)[CW]) {
-    static_assert(CW == 4 || CW == 8, "paired wait");
-    if constexpr (CW == 4) {
-        asm volatile("tcgen05.wait::ld.sync.aligned;"
-                     : "+r"(a[0]), "+r"(a[1]), "+r"(a[2]), "+r"(a[3]), "+r"(b[0]), "+r"(b[1]), "+r"(b[2]), "+r"(b[3]) :: "memory");
-    } else {
-        asm volatile("tcgen05.wait::ld.sync.aligned;"
-                     : "+r"(a[0]), "+r"(a[1]), "+r"(a[2]), "+r"(a[3]), "+r"(a[4]), "+r"(a[5]), "+r"(a[6]), "+r"(a[7]),
-                       "+r"(b[0]), "+r"(b[1]), "+r"(b[2]), "+r"(b[3]), "+r"(b[4]), "+r"(b[5]), "+r"(b[6]), "+r"(b[7]) :: "memory");
-    }
-}
-// one chunk's share of this warp: + b7, Snake, hi/lo split, K-major stores
-template <int CW, bool BF16>
-__device__ __forceinline__ void a2_transform(const TcConvParams& p, const uint32_t (&v)[CW], int c2, int arow, int pc0, int Rpad2,
-                                             uint8_t* a2_base, uint32_t a2_half) {
-    using namespace tc;
-    uint8_t* ahi = a2_base + (size_t)c2 * 2 * a2_half;
-    uint8_t* alo = ahi + a2_half;
-#pragma unroll
-    for (int pp = 0; pp < CW / 4; ++pp) {
-        const int pc = pc0 + pp;
-        const int co = c2 * 16 + pc * 4;
-        float4 bi = __ldg(reinterpret_cast<const float4*>(p.bias + co));
-        float4 al = __ldg(reinterpret_cast<const float4*>(p.out_alpha + co));
-        float4 ia = __ldg(reinterpret_cast<const float4*>(p.out_inv_alpha + co));
-        float4 x4 = make_float4(__uint_as_float(v[pp * 4 + 0]) + bi.x, __uint_as_float(v[pp * 4 + 1]) + bi.y,
-                                __uint_as_float(v[pp * 4 + 2]) + bi.z, __uint_as_float(v[pp * 4 + 3]) + bi.w);
-        x4 = snake4_sel<BF16>(x4, al, ia);
-        split_store<BF16>(x4, pc, arow, Rpad2, ahi, alo);
-    }
-}
-template <int CW, bool BF16>
-__device__ __forceinline__ void a2_phase(const TcConvParams& p, tc::Smem* sm, uint32_t taddr0, int arow, int pc0,
-                                         uint8_t* a2_base, uint32_t a2_half) {
-    using namespace tc;
-    const int Rpad2 = p.R2pad;
-    if constexpr (CW <= 8) {
-        // Two chunks per step when the warp's share is small (4 / 8 columns): a chunk is one dependent chain (TMEM load ->
-        // Snake -> split -> stores -> proxy fence -> arrive), so pairing them halves the fence / arrive round trips.
-        if ((p.nchunk2 & 1) == 0 && !(p.dbg & 8)) {
-            uint32_t v0[CW], v1[CW], n0[CW], n1[CW];
-            tmem_ldw_issue<CW>(taddr0, v0);
-            tmem_ldw_issue<CW>(taddr0 + 16u, v1);
-            tmem_ldw_wait2<CW>(v0, v1);
-#pragma unroll 1
-            for (int c2 = 0; c2 < p.nchunk2; c2 += 2) {
-                const bool more = c2 + 2 < p.nchunk2;
-                if (more) {
-                    tmem_ldw_issue<CW>(taddr0 + (uint32_t)((c2 + 2) * 16), n0);
-                    tmem_ldw_issue<CW>(taddr0 + (uint32_t)((c2 + 3) * 16), n1);
-                }
-                a2_transform<CW, BF16>(p, v0, c2, arow, pc0, Rpad2, a2_base, a2_half);
-                a2_transform<CW, BF16>(p, v1, c2 + 1, arow, pc0, Rpad2, a2_base, a2_half);
-                fence_proxy_async();
-                __syncwarp();
-                if ((threadIdx.x & 31) == 0) { mbar_arrive(&sm->a2_full[c2]); mbar_arrive(&sm->a2_full[c2 + 1]); }
-                if (more) {
-                    tmem_ldw_wait2<CW>(n0, n1);
-#pragma unroll
-                    for (int i = 0; i < CW; ++i) { v0[i] = n0[i]; v1[i] = n1[i]; }
-                }
-            }
-            return;
-        }
-    }
-    uint32_t v[CW], vn[CW];
-    tmem_ldw_issue<CW>(taddr0, v);
-    tmem_ldw_wait<CW>(v);
-#pragma unroll 1
-    for (int c2 = 0; c2 < p.nchunk2; ++c2) {
-        const bool more = c2 + 1 < p.nchunk2;
-        if (more) tmem_ldw_issue<CW>(taddr0 + (uint32_t)((c2 + 1) * 16), vn);
-        a2_transform<CW, BF16>(p, v, c2, arow, pc0, Rpad2, a2_base, a2_half);
-        fence_proxy_async();
-        warp_arrive(&sm->a2_full[c2]);
-        if (more) {
-            tmem_ldw_wait<CW>(vn);
-#pragma unroll
-            for (int i = 0; i < CW; ++i) v[i] = vn[i];
-        }
-    }
+template <bool FAST>
+__device__ __forceinline__ float act_out(int act, float v, float al, float ia) {
+    if (act == ACT_SNAKE) return FAST ? fmaf(ia, sin2_mufu(al * v), v) : snake_fast(v, al, ia);
+    if (act == ACT_TANH) return tanhf(v);
+    if (act == ACT_MISH) return mish_f(v);
+    return v;
 }
 
+// P1: split class of the layer's own GEMM; P2: of the fused GEMM 2 (P_NONE = not fused); NI: wgmma N per instruction;
+// MINB = 2: planned for two resident CTAs per SM (<= 128 registers, <= 64 accumulator columns per warpgroup);
+// TT: transposed formulation -- the weights are the wgmma A operand (64 output channels per warpgroup) and time is the
+// wgmma N dimension; the operand buffers and the weight blob are the same K-major layouts as the plain formulation.
+template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false>
+__global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p) {
+    constexpr bool FUSED = P2 != P_NONE;
+    static_assert(!TT || (NI == 64 && !FUSED), "transposed tiles: <= 64 channels x 64 time steps per warpgroup");
+    constexpr int NS = (PROMO || MINB == 2 ? 64 : 128) / NI;   // sub-tiles per warpgroup (registers: <= 64 / 128 floats)
+    constexpr bool F16X2 = P1 == P_F16X2;
+    constexpr bool DEC = P1 == P_BF16 || P1 == P_F16S;      // downstream of the VQ: SFU-sine Snake class
+    using T1 = PrecT<P1>;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem);
 
-// FUSED = true runs a whole ResidualUnit (dac.py:25-42) in one launch when all its channels fit one CTA:
-//   y = x + W1 . snake2(conv7_d(snake1(x)) + b7) + b1
-// GEMM 1 (the dilated conv) accumulates D1 in TMEM columns [0, MT*N); the worker warps then read D1 back
-// 16 columns at a time (tcgen05.ld), add b7, apply Snake, split hi/lo and write it as the K-major A operand
-// of GEMM 2 (the 1x1 conv) into the same double-buffered activation ring; D2 accumulates in TMEM columns
-// [MT*N, 2*MT*N).  The 96/192-channel intermediate never goes to HBM and the K=1 launch disappears.
-// BF16 = true (decoder only): operands split into bf16 hi + bf16 lo instead of tf32 hi + tf32 lo, issued as
-// tcgen05.mma.kind::f16 with K = 16.  Half the MMA instructions and half the shared-memory operand bytes
-// per channel (the SS-mode TF32 MMAs are shared-memory-bandwidth bound for N <= 192); 16 mantissa bits
-// keep the waveform error at ~1e-5 RMS, well inside the 1e-4 bar, but not VQ-exact -- never used upstream.
-// G1F16 = true (with BF16, downstream only): the layer's own GEMM (GEMM 1 when FUSED) takes ONE fp16 pass -- the operand
-// ring holds a single fp16 plane, the weight tiles are hi-only, a third of the MMAs.  On the oracle this moves the
-// reconstructed waveform by 1.4e-5 RMS when applied to every k = 7 conv of the decoder (scripts/cpu_decoder_precision.py;
-// bar 1e-4); GEMM 2 of a fused unit keeps the bf16 hi/lo class.
-// NW = worker warps (producers, then GEMM-2 operand, then epilogue): 8 for tiles planned for two CTAs per SM; 16 for tiles
-// that own a whole SM (fused C = 192: D1 + D2 = 384 TMEM columns) -- with one CTA of 8 workers an SM had 2 warps per
-// scheduler and every SIMT phase ran latency-bound while the MMA warp starved (profiles/r02 phase clocks).
-template <bool FUSED, bool BF16, bool G1F16 = false, int NW = 8, int NG = (NW == 16 ? 2 : 1)>
-__global__ void __launch_bounds__(64 + 32 * NW, NW == 8 ? 2 : 1) conv_tc_kernel(TcConvParams p) {
-    static_assert(!G1F16 || BF16, "the one-pass fp16 class shares the 16-bit operand layout");
-    static_assert(NW == 8 || NW == 16, "worker warps");
-    using namespace tc;
-    constexpr int NWT = NW * 32;                            // worker threads
-    constexpr int NSUB = NW / 4;                            // worker warps per TMEM lane quarter
-    // NG = 2: the workers produce as TWO groups on alternate chunks into a 4-deep operand ring: a group's chunk is one
-    // dependent chain (loads -> Snake -> split -> stores -> proxy fence -> arrive, ~1.5 k cycles whatever the thread count),
-    // so two chunks in flight is what shortens the K loop, not more threads per chunk.  Always with 16 workers; with 8
-    // workers when a group of 4 warps covers a chunk in <= PIPE_P pieces per thread (128-row tiles of 1- and 2-tap layers
-    // and of the k = 7 convs with dilation 1 / 3).
-    static_assert(NG == 1 || NG == 2, "producer groups");
-    constexpr int NBUF = 2 * NG;
-    constexpr int GT = NWT / NG;                            // producer threads per group
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    Smem* sm = reinterpret_cast<Smem*>(smem_raw);
-    constexpr int KG = BF16 ? 2 : 4;                        // 16-byte k-groups per 16-channel chunk
-    constexpr int KSTEPS = BF16 ? 1 : 2;                    // MMAs per chunk and pass (K = 16 / K = 8)
-    const int N = p.N, MT = p.MT;
-    const int R = 128 * MT + (p.Kr - 1) * p.dil;            // union of rows all taps touch
-    const int Rpad = p.Rpad;                                // R rounded so that Rpad % 8 == 2
-    const uint32_t a_half = (uint32_t)Rpad * 16 * KG;       // bytes of one hi (or lo) A buffer
-    const uint32_t b_half = (uint32_t)N * 16 * KG;          // bytes of one hi (or lo) weight tile
-    const uint32_t a_slot = (G1F16 ? 1u : 2u) * a_half;     // one operand buffer: hi (+ lo) planes
-    const uint32_t b_slot = (uint32_t)p.b_slot;             // one weight-ring slot: p.tpt GEMM-1 tiles (or p.tpt2 GEMM-2 tiles)
-    const uint32_t b1_bytes = (G1F16 ? 1u : 2u) * b_half;   // bytes of one GEMM-1 weight tile
-    const int TPT = p.tpt, TPT2 = p.tpt2;                   // tiles per bulk copy: a 3-12 KB tile per round trip left the MMA warp
-                                                            // waiting on L2 latency (~500 cycles per tap for N = 96)
-    uint8_t* a_base = smem_raw + kSmemHdr;                  // [2 bufs][hi|lo][4 k4][Rpad][16B]
-    uint8_t* b_base = a_base + NBUF * a_slot;               // [S][hi|lo][4 k4][N][16B]
-    const int S = p.stagesB;
-    // fused: resident GEMM-2 operand, [nchunk2][hi|lo][KG][R2pad][16B]
-    const uint32_t a2_half = (uint32_t)p.R2pad * 16 * KG;
-    uint8_t* a2_base = b_base + (size_t)S * b_slot;
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int t0 = blockIdx.x * 128 * MT;
-    const int ntile = blockIdx.y;
-    const int b = blockIdx.z;
-    const int nchunk = p.nchunk, Kr = p.Kr;
-    const uint32_t ncols = p.tmem_cols;
+    const int tid = threadIdx.x, wg = tid >> 7;
+    const int BM = 64 * p.MT;                               // MT = 2: warpgroups split rows; 1: they split channels
+    const int N = p.N, NW = p.MT == 2 ? N : N / 2;
+    Tile tl;
+    tl.row0 = p.MT == 2 ? 64 * wg : 0;
+    tl.col0 = p.MT == 2 ? 0 : wg * NW;
+    tl.nsub = TT ? 1 : NW / NI;                             // transposed: one 64-step time sub-tile
+    tl.warp = (tid >> 5) & 3;
+    tl.lane = tid & 31;
+    const int t0 = blockIdx.x * BM, ntile = blockIdx.y, b = blockIdx.z;
+    const int Kr = p.Kr, dil = p.dil, Rpad = p.Rpad, nchunk = p.nchunk, S = p.stagesB;
+    const int R = BM + (Kr - 1) * dil;
+    const uint32_t a_plane = (uint32_t)T1::KG * Rpad * 16, a_bytes = a_plane * T1::planes;
+    uint8_t* abuf = smem + kSmemHdr;
+    uint8_t* wbuf = abuf + 2 * (size_t)a_bytes;
+    uint8_t* a2buf = wbuf + (size_t)S * p.b_slot;
+    const uint32_t w_unit1 = (uint32_t)Kr * T1::planes * T1::KG * N * 16;
+    const uint32_t w_unit2 = FUSED ? (uint32_t)prec_planes(P2) * prec_kg(P2) * N * 16 : 0;
+    const int units = nchunk + (FUSED ? p.nchunk2 : 0);
 
     if (tid == 0) {
-        for (int i = 0; i < kMaxStagesB; ++i) { mbar_init(&sm->b_full[i], 1); mbar_init(&sm->b_empty[i], 1); }
-        for (int i = 0; i < NBUF; ++i) { mbar_init(&sm->a_full[i], NW / NG); mbar_init(&sm->a_empty[i], 1); }
-        mbar_init(&sm->acc_full, 1);
-        mbar_init(&sm->acc2_full, 1);
-        if (FUSED) for (int i = 0; i < 16; ++i) mbar_init(&sm->a2_full[i], NW);
+        for (int i = 0; i < S; ++i) mbar_init(&full[i], 1);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(&sm->tmem_base, ncols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sm->tmem_base;
+    auto issue_w = [&](int u) {
+        uint64_t* bar = &full[u % S];
+        uint8_t* dst = wbuf + (size_t)(u % S) * p.b_slot;
+        const uint8_t* src;
+        uint32_t bytes;
+        if (u < nchunk) { src = reinterpret_cast<const uint8_t*>(p.wblob) + ((size_t)ntile * nchunk + u) * w_unit1; bytes = w_unit1; }
+        else { src = reinterpret_cast<const uint8_t*>(p.wblob2) + (size_t)(u - nchunk) * w_unit2; bytes = w_unit2; }
+        mbar_arrive_expect_tx(bar, bytes);
+        bulk_g2s(dst, src, bytes, bar);
+    };
+    if (tid == 0)
+        for (int u = 0; u < S - 1 && u < units; ++u) issue_w(u);
 
-    if (warp == 0) {
-        // ================= weight producer =================
-        if (lane == 0) {
-            const float* wsrc = p.wblob + (size_t)ntile * nchunk * Kr * (size_t)(b1_bytes / 4);
-            // the blob is [chunk][tap] tiles back to back: TPT consecutive tiles travel as one bulk copy
-            const int ntiles = nchunk * Kr;
-            uint32_t ws = 0, wph = 1;                // slot, parity of the EMPTY barrier to wait for (first round passes)
-            int tr = 0;
-            for (int it0 = 0; it0 < ntiles; it0 += TPT, ++tr) {
-                const uint32_t bytes = (uint32_t)(ntiles - it0 < TPT ? ntiles - it0 : TPT) * b1_bytes;
-                mbar_wait(&sm->b_empty[ws], wph);
-                if ((p.dbg & 1) && tr >= S) {           // TIMING EXPERIMENT: stale weights
-                    mbar_arrive(&sm->b_full[ws]);
+    const PadMap pm = PadMap::make(p.Tin, p.pad_left_s, p.pad_right_s, p.reflect);
+    const float* __restrict__ xb = p.x + (size_t)b * p.x_bstride;
+    auto produce = [&](int c) {
+        uint8_t* ahi = abuf + (size_t)(c & 1) * a_bytes;
+        if constexpr (P1 == P_TF32) produce_chunk<kThreads, false>(p, pm, xb, c, t0, R, Rpad, ahi, ahi + a_plane, tid);
+        else if constexpr (P1 == P_BF16) produce_chunk<kThreads, true>(p, pm, xb, c, t0, R, Rpad, ahi, ahi + a_plane, tid);
+        else if constexpr (P1 == P_F16S) produce_chunk<kThreads, true, 4, false, false, true>(p, pm, xb, c, t0, R, Rpad, ahi, ahi, tid);
+        else produce_chunk<kThreads, false, 4, false, true>(p, pm, xb, c, t0, R, Rpad, ahi, ahi + a_plane, tid);
+        fence_proxy_async();    // make the generic-proxy stores visible to the tensor core
+    };
+    produce(0);
+
+    float acc[NS][NI / 2];
+    float tmp[PROMO ? NS : 1][PROMO ? NI / 2 : 1];
+    float crs[F16X2 ? NS : 1][F16X2 ? NI / 2 : 1];
+    zero_acc<NI, NS>(acc);
+    if constexpr (PROMO) zero_acc<NI, NS>(tmp);
+    if constexpr (F16X2) zero_acc<NI, NS>(crs);
+    const uint32_t a_lbo = (uint32_t)Rpad * 16, b_lbo = (uint32_t)N * 16;
+    const uint32_t abase = smem_u32(abuf), wbase = smem_u32(wbuf), a2base = smem_u32(a2buf);
+    const int BM2 = BM;
+
+    auto promote = [&]() {
+        if constexpr (PROMO) {
+#pragma unroll
+            for (int s = 0; s < NS; ++s)
+#pragma unroll
+                for (int i = 0; i < NI / 2; ++i) {
+                    if constexpr (F16X2) { acc[s][i] += tmp[s][i] + crs[s][i] * kLoUnscale; crs[s][i] = 0.f; }
+                    else acc[s][i] += tmp[s][i];
+                    tmp[s][i] = 0.f;
+                }
+        }
+    };
+
+#pragma unroll 1
+    for (int u = 0; u < units; ++u) {
+        __syncthreads();                     // operand u ready in every thread's view; the slot refilled below is idle
+        if (tid == 0 && u + S - 1 < units) issue_w(u + S - 1);
+        mbar_wait(&full[u % S], (uint32_t)(u / S) & 1u);
+        const uint32_t wslot = wbase + (uint32_t)(u % S) * p.b_slot;
+        wg_fence();
+        if (u < nchunk) {
+            const uint32_t a0 = abase + (uint32_t)(u & 1) * a_bytes + (uint32_t)tl.row0 * 16;
+            const uint32_t b0 = wslot + (uint32_t)tl.col0 * 16;
+#pragma unroll 1
+            for (int tap = 0; tap < Kr; ++tap) {
+                const uint32_t ahi = a0 + (uint32_t)(tap * dil) * 16, alo = ahi + a_plane;
+                const uint32_t bhi = b0 + (uint32_t)tap * T1::planes * T1::KG * b_lbo, blo = bhi + T1::KG * b_lbo;
+                if constexpr (TT) {         // D[channel][time]: weights are the A operand, activations the B operand
+                    mma_pass<P1, NI, NS>(tmp, 1, bhi, b_lbo, ahi, a_lbo);
+                    mma_pass<P1, NI, NS>(crs, 1, bhi, b_lbo, alo, a_lbo);
+                    mma_pass<P1, NI, NS>(crs, 1, blo, b_lbo, ahi, a_lbo);
+                } else if constexpr (P1 == P_F16S) {
+                    mma_pass<P1, NI, NS>(acc, tl.nsub, ahi, a_lbo, bhi, b_lbo);
+                } else if constexpr (F16X2) {
+                    mma_pass<P1, NI, NS>(tmp, tl.nsub, ahi, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI, NS>(crs, tl.nsub, ahi, a_lbo, blo, b_lbo);
+                    mma_pass<P1, NI, NS>(crs, tl.nsub, alo, a_lbo, bhi, b_lbo);
+                } else if constexpr (PROMO) {
+                    mma_pass<P1, NI, NS>(tmp, tl.nsub, ahi, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI, NS>(tmp, tl.nsub, ahi, a_lbo, blo, b_lbo);
+                    mma_pass<P1, NI, NS>(tmp, tl.nsub, alo, a_lbo, bhi, b_lbo);
                 } else {
-                    mbar_arrive_expect_tx(&sm->b_full[ws], bytes);
-                    bulk_g2s(b_base + (size_t)ws * b_slot, wsrc + (size_t)it0 * (b1_bytes / 4), bytes, &sm->b_full[ws]);
-                }
-                if (++ws == (uint32_t)S) { ws = 0; wph ^= 1; }
-            }
-            if (FUSED) {
-                for (int c20 = 0; c20 < p.nchunk2; c20 += TPT2) {
-                    const uint32_t bytes = (uint32_t)(p.nchunk2 - c20 < TPT2 ? p.nchunk2 - c20 : TPT2) * 2 * b_half;
-                    mbar_wait(&sm->b_empty[ws], wph);
-                    mbar_arrive_expect_tx(&sm->b_full[ws], bytes);
-                    bulk_g2s(b_base + (size_t)ws * b_slot, p.wblob2 + (size_t)c20 * (2 * b_half / 4), bytes, &sm->b_full[ws]);
-                    if (++ws == (uint32_t)S) { ws = 0; wph ^= 1; }
+                    mma_pass<P1, NI, NS>(acc, tl.nsub, ahi, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI, NS>(acc, tl.nsub, ahi, a_lbo, blo, b_lbo);
+                    mma_pass<P1, NI, NS>(acc, tl.nsub, alo, a_lbo, bhi, b_lbo);
                 }
             }
-        }
-    } else if (warp == 1) {
-        // ================= MMA issuer (whole warp converged, see umma_tf32) =================
-        {
-            // instruction descriptor: D=f32, A=B=tf32, K-major both, N>>3, M=128>>4
-            const uint32_t fmt = BF16 ? 1u : 2u;   // F16F32Format: F16 = 0, BF16 = 1, TF32 = 2
-            const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t idesc1 = G1F16 ? ((1u << 4) | ((uint32_t)(N >> 3) << 17) | ((128u >> 4) << 24)) : idesc;
-            constexpr int NPASS1 = G1F16 ? 1 : 3;
-            const uint32_t a_slot16 = a_slot >> 4, b_slot16 = b_slot >> 4;
-            // everything below is in 16-byte units and warp-uniform
-            const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem, 0);
-            const uint32_t a_base16 = __shfl_sync(0xffffffffu, smem_u32(a_base), 0) >> 4;
-            const uint32_t b_base16 = __shfl_sync(0xffffffffu, smem_u32(b_base), 0) >> 4;
-            const uint32_t a_lbo16 = (uint32_t)Rpad, b_lbo16 = (uint32_t)N;
-            const uint32_t a_half16 = a_half >> 4, b_half16 = b_half >> 4;
-            const uint32_t b1_16 = b1_bytes >> 4;
-            const bool mprobe = blockIdx.x == 3 && blockIdx.y == 0 && blockIdx.z == 0;   // [6]/[7]: cycles waiting for operands / weights
-            long long w_a = 0, w_b = 0;
-            const long long t_m0 = mprobe ? clock64() : 0;
-            uint32_t rs = 0, rph = 0;               // weight ring: slot, phase parity
-            if (p.cps > 0) {
-                // Slot-structured issue loop: a weight-ring slot holds ALL taps of `cps` consecutive chunks, so the loop nest
-                // is slot > chunk > tap (unrolled for Kr = 1 / 2 / 7) with no per-tap ring bookkeeping.  The generic loop
-                // below spent ~440 cycles of dependent scalar work per tap (two integer divisions per slot, parameters
-                // re-read from the constant bank, descriptor arithmetic) against 120-155 cycles of tensor-pipe time for the
-                // one MMA of a one-pass tap: the issuing warp, not the tensor pipe, set the pace of every N <= 192 layer
-                // (profiles/r02 per-chunk trace).
-                IssueCtx ic;
-                ic.idesc = idesc1; ic.a_half16 = a_half16; ic.b_half16 = b_half16; ic.a_lbo16 = a_lbo16; ic.b_lbo16 = b_lbo16;
-                ic.b1_16 = b1_16; ic.dil = (uint32_t)p.dil; ic.MT = MT; ic.N = (uint32_t)N;
-                uint32_t a_w0 = a_base16 + (a_lbo16 << 16), b_w0 = b_base16 + (b_lbo16 << 16);
-                uint32_t a_slot16r = a_slot16, b_slot16r = b_slot16, Sr = (uint32_t)S;
-                int cps = p.cps, nch = nchunk, kr = Kr;
-                // pin the loop invariants in registers: a shuffle is opaque to ptxas, which otherwise re-reads kernel
-                // parameters from the constant bank (LDC + dependent use, ~40 cycles each) inside the tap loop
-                pin_u(ic.idesc); pin_u(ic.a_half16); pin_u(ic.b_half16); pin_u(ic.a_lbo16); pin_u(ic.b_lbo16); pin_u(ic.b1_16);
-                pin_u(ic.dil); pin_i(ic.MT); pin_u(ic.N); pin_u(a_w0); pin_u(b_w0); pin_u(a_slot16r); pin_u(b_slot16r); pin_u(Sr);
-                pin_i(cps); pin_i(nch); pin_i(kr);
-                const uint32_t kstride = (uint32_t)kr * ic.b1_16;
-                for (int c0 = 0; c0 < nch; c0 += cps) {
-                    long long tq2 = mprobe ? clock64() : 0;
-                    mbar_wait(&sm->b_full[rs], rph);
-                    if (mprobe) w_b += clock64() - tq2;
-                    uint32_t b_w = b_w0 + rs * b_slot16r;
-                    const int ce = c0 + cps < nch ? c0 + cps : nch;
-                    for (int c = c0; c < ce; ++c, b_w += kstride) {
-                        const int buf = c % NBUF;
-                        long long tq = mprobe ? clock64() : 0;
-                        mbar_wait(&sm->a_full[buf], (c / NBUF) & 1);
-                        if (mprobe) { w_a += clock64() - tq; if (lane == 0 && c < 16) { g_tc_trace[0][c] = clock64(); g_tc_trace[4][c] = 0; } }
-                        tc_fence_after();
-                        const uint32_t a_w = a_w0 + (uint32_t)buf * a_slot16r;
-                        if (kr == 7) issue_taps<BF16, NPASS1, 7>(ic, tmem_u, a_w, b_w, c == 0);
-                        else if (kr == 2) issue_taps<BF16, NPASS1, 2>(ic, tmem_u, a_w, b_w, c == 0);
-                        else issue_taps<BF16, NPASS1, 1>(ic, tmem_u, a_w, b_w, c == 0);
-                        umma_commit(&sm->a_empty[buf]);         // activation buffer free
-                        if (mprobe && lane == 0 && c < 16) g_tc_trace[1][c] = clock64();
-                    }
-                    umma_commit(&sm->b_empty[rs]);              // weight slot free once these MMAs retire
-                    if (++rs == Sr) { rs = 0; rph ^= 1; }
-                }
-            } else {
-            int it = 0, tr = -1, s = 0, sub = 0;
-            const int ntiles = nchunk * Kr;
-            for (int c = 0; c < nchunk; ++c) {
-                const int buf = c % NBUF;
-                long long tq = mprobe ? clock64() : 0;
-                mbar_wait(&sm->a_full[buf], (c / NBUF) & 1);
-                if (mprobe) { w_a += clock64() - tq; if (lane == 0 && c < 16) { g_tc_trace[0][c] = clock64(); g_tc_trace[4][c] = -w_b; } }
-                const uint32_t a_hi = a_base16 + (uint32_t)buf * a_slot16;
-                const uint32_t a_lo = a_hi + a_half16;
-                for (int tap = 0; tap < Kr; ++tap, ++it) {
-                    if (sub == 0) {
-                        ++tr;
-                        s = tr % S;
-                        long long tq2 = mprobe ? clock64() : 0;
-                        mbar_wait(&sm->b_full[s], (tr / S) & 1);
-                        if (mprobe) w_b += clock64() - tq2;
-                    }
-                    tc_fence_after();
-                    const uint32_t b_hi = b_base16 + (uint32_t)s * b_slot16 + (uint32_t)sub * b1_16;
-                    const uint32_t b_lo = b_hi + b_half16;
-                    for (int mt = 0; mt < MT; ++mt) {
-                        const uint32_t row_off = (uint32_t)(mt * 128 + tap * p.dil);
-                        const uint32_t d_tmem = tmem_u + (uint32_t)(mt * N);
-#pragma unroll
-                        for (int pass = 0; pass < NPASS1; ++pass) {
-                            const uint32_t aa = (pass == 2 ? a_lo : a_hi) + row_off;
-                            const uint32_t bb = (pass == 1 ? b_lo : b_hi);
-#pragma unroll
-                            for (int ks = 0; ks < KSTEPS; ++ks) {
-                                uint32_t accum = (c | tap | pass | ks) != 0;
-                                umma<BF16>(d_tmem, desc_u(aa + ks * 2 * a_lbo16, a_lbo16), desc_u(bb + ks * 2 * b_lbo16, b_lbo16), idesc1, accum);
-                            }
+            wg_commit();
+            if (u + 1 < nchunk) produce(u + 1);         // overlaps the MMAs in flight
+            wg_wait_all();
+            if (PROMO && ((u + 1) % p.promote_every == 0 || u + 1 == nchunk)) promote();
+            if constexpr (FUSED) {
+                if (u + 1 == nchunk) {
+                    // GEMM-2 operand snake2(D1 + b7), split, K-major [plane][k-piece][BM rows][16 B]
+                    constexpr int KG2 = prec_kg(P2 < 0 ? 0 : P2);
+                    const uint32_t a2_plane = (uint32_t)(p.nchunk2 * KG2) * BM2 * 16;
+                    for_each_pair<NI, NS>(tl, acc, [&](int row, int col, float v0, float v1) {
+                        const float2 bi = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                        const float2 al = __ldg(reinterpret_cast<const float2*>(p.out_alpha + col));
+                        const float2 ia = __ldg(reinterpret_cast<const float2*>(p.out_inv_alpha + col));
+                        v0 = act_out<DEC>(ACT_SNAKE, v0 + bi.x, al.x, ia.x);
+                        v1 = act_out<DEC>(ACT_SNAKE, v1 + bi.y, al.y, ia.y);
+                        if constexpr (P2 == P_BF16) {
+                            __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1);
+                            float2 hf = __bfloat1622float2(h);
+                            __nv_bfloat162 l = __floats2bfloat162_rn(v0 - hf.x, v1 - hf.y);
+                            const uint32_t off = ((uint32_t)(col >> 3) * BM2 + row) * 16 + (col & 7) * 2;
+                            *reinterpret_cast<__nv_bfloat162*>(a2buf + off) = h;
+                            *reinterpret_cast<__nv_bfloat162*>(a2buf + a2_plane + off) = l;
+                        } else {
+                            const float h0 = to_tf32(v0), h1 = to_tf32(v1);
+                            const uint32_t off = ((uint32_t)(col >> 2) * BM2 + row) * 16 + (col & 3) * 4;
+                            *reinterpret_cast<float2*>(a2buf + off) = make_float2(h0, h1);
+                            *reinterpret_cast<float2*>(a2buf + a2_plane + off) = make_float2(to_tf32(v0 - h0), to_tf32(v1 - h1));
                         }
-                    }
-                    if (++sub == TPT || it == ntiles - 1) {
-                        umma_commit(&sm->b_empty[s]);   // weight slot free once these MMAs retire
-                        sub = 0;
-                    }
+                    });
+                    fence_proxy_async();
+                    zero_acc<NI, NS>(acc);
                 }
-                umma_commit(&sm->a_empty[buf]);         // activation buffer free
-                if (mprobe && lane == 0 && c < 16) { g_tc_trace[1][c] = clock64(); g_tc_trace[4][c] += w_b; }
             }
-            const uint32_t trn = (uint32_t)(tr + 1);
-            rs = trn % (uint32_t)S; rph = (trn / (uint32_t)S) & 1u;
-            }
-            umma_commit(&sm->acc_full);
-            if (mprobe && lane == 0) { g_tc_phase_clock[6] = clock64() - t_m0; g_tc_phase_clock[7] = w_b + w_a; }
-            if (FUSED) {
-                // GEMM 2 (the 1x1 conv): resident operand chunks, weight slots of TPT2 chunk tiles (hi|lo)
-                IssueCtx ic;
-                ic.idesc = idesc; ic.a_half16 = a2_half >> 4; ic.b_half16 = b_half16; ic.a_lbo16 = (uint32_t)p.R2pad; ic.b_lbo16 = b_lbo16;
-                ic.b1_16 = 2 * b_half16; ic.dil = 0; ic.MT = MT; ic.N = (uint32_t)N;
-                const uint32_t a2_base16 = __shfl_sync(0xffffffffu, smem_u32(a2_base), 0) >> 4;
-                uint32_t a_w0 = a2_base16 + (ic.a_lbo16 << 16), b_w0 = b_base16 + (b_lbo16 << 16);
-                uint32_t b_slot16r = b_slot16, Sr = (uint32_t)S;
-                const uint32_t a2_chunk16 = 2 * ic.a_half16;
-                int nch2 = p.nchunk2, tpt2 = TPT2;
-                pin_u(ic.idesc); pin_u(ic.a_half16); pin_u(ic.b_half16); pin_u(ic.a_lbo16); pin_u(ic.b_lbo16); pin_u(ic.b1_16);
-                pin_i(ic.MT); pin_u(ic.N); pin_u(a_w0); pin_u(b_w0); pin_u(b_slot16r); pin_u(Sr); pin_i(nch2); pin_i(tpt2);
-                const uint32_t d2 = tmem_u + (uint32_t)(MT * N);
-                for (int c20 = 0; c20 < nch2; c20 += tpt2) {
-                    mbar_wait(&sm->b_full[rs], rph);
-                    uint32_t b_w = b_w0 + rs * b_slot16r;
-                    const int ce = c20 + tpt2 < nch2 ? c20 + tpt2 : nch2;
-                    for (int c2 = c20; c2 < ce; ++c2, b_w += ic.b1_16) {
-                        mbar_wait(&sm->a2_full[c2], 0);
-                        tc_fence_after();
-                        issue_taps<BF16, 3, 1>(ic, d2, a_w0 + (uint32_t)c2 * a2_chunk16, b_w, c2 == 0);
-                    }
-                    umma_commit(&sm->b_empty[rs]);
-                    if (++rs == Sr) { rs = 0; rph ^= 1; }
-                }
-                umma_commit(&sm->acc2_full);
-            }
-        }
-    } else {
-        // ================= activation producers (warps 2..NW+1) =================
-        const int ptid = tid - 64;                                  // 0..NWT-1
-        const bool probe = (ptid == 0 && blockIdx.x == 3 && blockIdx.y == 0 && blockIdx.z == 0);
-        if (probe) g_tc_phase_clock[0] = clock64();
-        const PadMap pm = PadMap::make(p.Tin, p.pad_left_s, p.pad_right_s, p.reflect);
-        const float* __restrict__ xb = p.x + (size_t)b * p.x_bstride;
-        // interior tile: every row of the union exists in the input (no padding, no tail) and a row is one sample
-        const int vrow0 = t0 - p.PLr;
-        const bool interior = p.vf == 1 && vrow0 >= 0 && vrow0 + R <= p.Tin && vrow0 + R <= p.Tout + (Kr - 1) * p.dil;
-        const int grp = ptid / GT, gtid = ptid - grp * GT;           // producer group (chunks grp, grp + NG, ...) and thread in it
-        const float* __restrict__ isrc = interior ? xb + (size_t)(vrow0 + (gtid >> 2)) * p.ldx + (gtid & 3) * 4 : xb;
-        const size_t pstride = (size_t)(GT / 4) * p.ldx;
-        long long pw_e = 0, pw_l = 0, pw_x = 0;
-        if (R <= PIPE_P * (GT / 4)) {
-            // <= 5 pieces per thread: keep the group's next chunk's loads in flight while transforming this one
-            ChunkRegs cur, nxt = {};
-            const int npc = (R - (gtid >> 2) + GT / 4 - 1) / (GT / 4);     // this thread's pieces per chunk
-            if (grp < nchunk) {
-                if (interior) load_chunk_interior<GT>(isrc + grp * kChunk, pstride, npc, cur);
-                else load_chunk_regs<GT>(p, pm, xb, grp, t0, R, gtid, cur);
-            }
-            for (int c = grp; c < nchunk; c += NG) {
-                const int buf = c % NBUF;
-                if (c + NG < nchunk && !(p.dbg & 2)) {   // dbg bit 2, TIMING EXPERIMENT: the first chunk's values for every chunk
-                    if (interior) load_chunk_interior<GT>(isrc + (c + NG) * kChunk, pstride, npc, nxt);
-                    else load_chunk_regs<GT>(p, pm, xb, c + NG, t0, R, gtid, nxt);
-                }
-                long long tq = probe ? clock64() : 0;
-                mbar_wait(&sm->a_empty[buf], ((c / NBUF) & 1) ^ 1);   // polled: a 200 ns parked wait here measured +1 ms/step
-                if (probe) {
-                    long long t1 = clock64();
-                    pw_e += t1 - tq;
-                    if (c < 16) g_tc_trace[2][c] = t1;
-                    float sacc = 0.f;
-#pragma unroll
-                    for (int u = 0; u < PIPE_P; ++u) sacc += cur.v[u].x + cur.v[u].w;
-                    if (sacc == 1.2345e-33f) pw_e += 1;     // a real use of the loaded registers: stalls until they land
-                    tq = clock64();
-                    pw_l += tq - t1;
-                }
-                uint8_t* ahi = a_base + (size_t)buf * a_slot;
-                if (interior) store_chunk_interior<GT, BF16, G1F16>(p, c, npc, Rpad, ahi, ahi + a_half, gtid, cur);
-                else store_chunk_regs<GT, BF16, G1F16>(p, c, R, Rpad, ahi, ahi + a_half, gtid, cur);
-                fence_proxy_async();    // make the generic-proxy stores visible to the tensor core
-                warp_arrive(&sm->a_full[buf]);
-                if (probe) { pw_x += clock64() - tq; if (c < 16) g_tc_trace[3][c] = clock64(); }
-                if (!(p.dbg & 2)) cur = nxt;
-            }
-        } else {
-            for (int c = grp; c < nchunk; c += NG) {
-                const int buf = c % NBUF;
-                long long tq = probe ? clock64() : 0;
-                mbar_wait(&sm->a_empty[buf], ((c / NBUF) & 1) ^ 1);   // polled: a 200 ns parked wait here measured +1 ms/step
-                if (probe) { long long t1 = clock64(); pw_e += t1 - tq; tq = t1; }
-                uint8_t* ahi = a_base + (size_t)buf * a_slot;
-                if (interior) produce_chunk_interior<GT, BF16, G1F16>(p, isrc + c * kChunk, pstride, c, R, Rpad, ahi, ahi + a_half, gtid);
-                else produce_chunk<GT, BF16, 4, false, false, G1F16>(p, pm, xb, c, t0, R, Rpad, ahi, ahi + a_half, gtid);
-                fence_proxy_async();
-                warp_arrive(&sm->a_full[buf]);
-                if (probe) pw_x += clock64() - tq;
-            }
-        }
-        if (probe) { g_tc_prod_clock[0] = pw_e; g_tc_prod_clock[1] = pw_l; g_tc_prod_clock[2] = pw_x; g_tc_prod_clock[3] = nchunk; }
-        // ================= epilogue =================
-        if (probe) g_tc_phase_clock[1] = clock64();                 // all activation chunks produced
-        mbar_wait_relaxed(&sm->acc_full, 0);
-        tc_fence_after();
-        if (probe) g_tc_phase_clock[2] = clock64();                 // GEMM 1 retired
-        const int q = warp & 3;                                     // TMEM lane quarter of this warp
-        const int h = (warp - 2) >> 2;                              // NSUB warps per quarter split the columns
-        const int half = h & 1;
-        uint32_t d_base = tmem;                                     // accumulator the final epilogue reads
-        const float* ep_bias = p.bias;
-        int ep_act = p.out_act;
-        if (FUSED) {
-            // ---- GEMM-2 operand: snake2(D1 + b7), 16 channels per chunk, straight from TMEM ----
-            // The whole operand stays resident (no ring, no waits): the MMA warp starts chunk c2 as soon as it is
-            // complete while the workers already transform the next ones.  The NSUB warps of a lane quarter share the
-            // MT * 16 columns of a chunk: CW = 16 * MT / NSUB columns each (accumulator am, column offset coff).
-            const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-            const int CW = 16 * MT / NSUB;
-            const int am = (h * CW) >> 4, coff = (h * CW) & 15;
-            const int arow = am * 128 + q * 32 + lane;
-            const uint32_t taddr0 = lane_addr + (uint32_t)(am * N + coff);
-            if (CW == 16) a2_phase<16, BF16>(p, sm, taddr0, arow, coff >> 2, a2_base, a2_half);
-            else if (CW == 8) a2_phase<8, BF16>(p, sm, taddr0, arow, coff >> 2, a2_base, a2_half);
-            else a2_phase<4, BF16>(p, sm, taddr0, arow, coff >> 2, a2_base, a2_half);
-            tc_fence_before();
-            if (probe) g_tc_phase_clock[3] = clock64();             // GEMM-2 operand produced
-            mbar_wait_relaxed(&sm->acc2_full, 0);
-            tc_fence_after();
-            if (probe) g_tc_phase_clock[4] = clock64();             // GEMM 2 retired
-            d_base = tmem + (uint32_t)(MT * N);
-            ep_bias = p.bias2;
-            ep_act = ACT_NONE;
-        }
-        const int csplit = ((N / 2 + 15) / 16) * 16;
-        const int cbeg = half ? csplit : 0, cend = half ? N : csplit;
-        const int row = q * 32 + lane;
-        float* __restrict__ yb = p.y + (size_t)b * p.y_bstride;
-        const float* __restrict__ rb = p.res ? p.res + (size_t)b * p.y_bstride : nullptr;
-        if ((N & 31) == 0) {
-            // coalesced path: 32-column groups through the (now idle) activation buffers as transpose stage
-            float* stage = reinterpret_cast<float*>(a_base) + (size_t)(warp - 2) * (32 * 36);
-            // the MT * N/32 column groups of a lane quarter are dealt to its NSUB warps in contiguous runs
-            const int ng = N / 32, items = MT * ng;
-            const int ibeg = h * items / NSUB, iend = (h + 1) * items / NSUB;
-#pragma unroll 1
-            for (int item = ibeg; item < iend; ++item) {
-                const int mt = item / ng, g = item - mt * ng;
-                uint32_t acc[32];
-                tmem_ld32(d_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * N + g * 32), acc);
-                float v[32];
-#pragma unroll
-                for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(acc[i]);
-                epilogue_tile32<true, BF16>(p, ep_bias, ep_act, v, stage, lane, t0 + mt * 128 + q * 32, ntile * N + g * 32, yb, rb);
-            }
-            if (probe) g_tc_phase_clock[5] = clock64();
-        } else {
-        // flat loop over (mt, 16-column group); the residual of group g+1 is fetched while group g is
-        // drained from TMEM and stored, so its DRAM latency is off the critical path
-        const int ngrp = (cend - cbeg) / 16;
-        const int total = MT * ngrp;
-        const bool has_res = rb != nullptr;
-        float4 rcur[4], rnxt[4];
-        auto fetch_res = [&](int g, float4 (&dst)[4]) {
-            const int mt = g / ngrp, c0 = cbeg + (g - mt * ngrp) * 16;
-            const int t = t0 + mt * 128 + row;
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) dst[j4] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (has_res && t < p.Tout) {
-                const float* rrow = rb + (size_t)t * p.ldy + ntile * N + c0;
-#pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4) dst[j4] = *reinterpret_cast<const float4*>(rrow + j4 * 4);
-            }
-        };
-        constexpr int GSTEP = NSUB / 2;                             // NW = 16: the two warps of a column half alternate groups
-        const int g0 = h >> 1;
-        if (g0 < total) fetch_res(g0, rcur);
-#pragma unroll 1
-        for (int g = g0; g < total; g += GSTEP) {
-            const int mt = g / ngrp, c0 = cbeg + (g - mt * ngrp) * 16;
-            const int t = t0 + mt * 128 + row;
-            if (g + GSTEP < total) fetch_res(g + GSTEP, rnxt);
-            uint32_t acc[16];
-            tmem_ld16(d_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * N + c0), acc);
-            if (t < p.Tout) {
-                float* yrow = yb + (size_t)t * p.ldy;
-                const int co0 = ntile * N + c0;
-#pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4)
-                    epilogue_store4(p, ep_bias, ep_act, __uint_as_float(acc[j4 * 4 + 0]), __uint_as_float(acc[j4 * 4 + 1]),
-                                    __uint_as_float(acc[j4 * 4 + 2]), __uint_as_float(acc[j4 * 4 + 3]), co0 + j4 * 4, yrow,
-                                    has_res, rcur[j4]);
-            }
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) rcur[j4] = rnxt[j4];
-        }
-        if (probe) g_tc_phase_clock[5] = clock64();                 // epilogue done
+        } else if constexpr (FUSED) {
+            constexpr int P2x = P2 < 0 ? 0 : P2;
+            constexpr int KG2 = prec_kg(P2x);
+            const int c2 = u - nchunk;
+            const uint32_t a2_plane = (uint32_t)(p.nchunk2 * KG2) * BM2 * 16, a2_lbo = (uint32_t)BM2 * 16;
+            const uint32_t ahi = a2base + ((uint32_t)(c2 * KG2) * BM2 + tl.row0) * 16, alo = ahi + a2_plane;
+            const uint32_t bhi = wslot + (uint32_t)tl.col0 * 16, blo = bhi + KG2 * b_lbo;
+            mma_pass<P2x, NI, NS>(acc, tl.nsub, ahi, a2_lbo, bhi, b_lbo);
+            mma_pass<P2x, NI, NS>(acc, tl.nsub, ahi, a2_lbo, blo, b_lbo);
+            mma_pass<P2x, NI, NS>(acc, tl.nsub, alo, a2_lbo, bhi, b_lbo);
+            wg_commit();
+            wg_wait_all();
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, ncols);
+
+    // ================= epilogue =================
+    const float* __restrict__ bias = FUSED ? p.bias2 : p.bias;
+    const int act = FUSED ? ACT_NONE : p.out_act;
+    float* __restrict__ yb = p.y + (size_t)b * p.y_bstride + (size_t)ntile * N;
+    const float* __restrict__ rb = p.res ? p.res + (size_t)b * p.y_bstride + (size_t)ntile * N : nullptr;
+    const float* al_p = act == ACT_SNAKE ? p.out_alpha + (size_t)ntile * N : nullptr;
+    const float* ia_p = act == ACT_SNAKE ? p.out_inv_alpha + (size_t)ntile * N : nullptr;
+    const float* bi_p = bias ? bias + (size_t)ntile * N : nullptr;
+    if constexpr (TT) {
+        // fragment row = output channel, column = time step
+        for_each_pair<NI, NS>(tl, acc, [&](int r, int c, float v0, float v1) {
+            if (r - tl.row0 >= NW) return;           // A-operand rows past this warpgroup's channels
+            const int co = tl.col0 + (r - tl.row0), tf = tl.row0 + (c - tl.col0);
+            const float bi = bi_p ? __ldg(bi_p + co) : 0.f;
+            const float al = act == ACT_SNAKE ? __ldg(al_p + co) : 0.f, ia = act == ACT_SNAKE ? __ldg(ia_p + co) : 0.f;
+            const float v[2] = {v0, v1};
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int t = t0 + tf + e;
+                if (t >= p.Tout) continue;
+                float o = act_out<DEC>(act, v[e] + bi, al, ia);
+                if (rb) o += rb[(size_t)t * p.ldy + co];
+                yb[(size_t)t * p.ldy + co] = o;
+            }
+        });
+        return;
+    }
+    for_each_pair<NI, NS>(tl, acc, [&](int row, int col, float v0, float v1) {
+        const int t = t0 + row;
+        if (t >= p.Tout) return;
+        if (bi_p) { const float2 bi = __ldg(reinterpret_cast<const float2*>(bi_p + col)); v0 += bi.x; v1 += bi.y; }
+        if (act == ACT_SNAKE) {
+            const float2 al = __ldg(reinterpret_cast<const float2*>(al_p + col));
+            const float2 ia = __ldg(reinterpret_cast<const float2*>(ia_p + col));
+            v0 = act_out<DEC>(ACT_SNAKE, v0, al.x, ia.x);
+            v1 = act_out<DEC>(ACT_SNAKE, v1, al.y, ia.y);
+        } else if (act != ACT_NONE) {
+            v0 = act_out<DEC>(act, v0, 0.f, 0.f);
+            v1 = act_out<DEC>(act, v1, 0.f, 0.f);
+        }
+        if (rb) { const float2 r = *reinterpret_cast<const float2*>(rb + (size_t)t * p.ldy + col); v0 += r.x; v1 += r.y; }
+        *reinterpret_cast<float2*>(yb + (size_t)t * p.ldy + col) = make_float2(v0, v1);
+    });
 }
 
-
-// ================================================================================================
-// conv_tcp_kernel: same math, with PROMOTED accumulation for the layers upstream of the VQ.
-//
-// The tensor core adds into its fp32 TMEM accumulator with truncation (measured: ~0.5 ulp of
-// one-sided error per chained MMA, i.e. ~1e-5 relative after a few hundred MMAs), which is enough
-// to flip near-tied VQ decisions.  Here each TMEM accumulator only lives for `promote_every`
-// chunks (~48 MMAs); 8 worker warps then pull it out with tcgen05.ld and add it into fp32
-// REGISTER accumulators with round-to-nearest (128 registers per thread hold the 128 x 256 tile),
-// while the MMA warp already fills the other TMEM buffer.
-// Warp-specialised with register re-allocation (setmaxnreg): 20 warps launch with 96 registers each;
-// the 4 control warps drop to 48, the 8 activation-producer warps to 56, and the 8 accumulator warps
-// grow to 160, so producing, MMA issue and promotion/epilogue all overlap instead of taking turns on
-// the same warps (measured before the split: produce 39 %, wait 19 %, promote 5 %, epilogue 36 % of
-// a CTA, serially).
-// ================================================================================================
-namespace tc {
-// role wait-time probes of conv_tcp_kernel (fac_debug_tc_phase_clocks): compile with -DFAC_TCP_PROBE=1 to measure; the
-// counters cost registers in the 32-register MMA warp and the 160-register accumulators (spills: +20 % on conv7 layers)
-#ifndef FAC_TCP_PROBE
-#define FAC_TCP_PROBE 0
-#endif
-constexpr bool kTcpProbe = FAC_TCP_PROBE != 0;
-constexpr int kThreadsP = 640;     // warps 0-3: control (weights, MMA, 2 idle); 4-11: producers; 12-19: accumulators
-constexpr int kMaxStagesP = 4;     // weight ring depth of the persistent kernel.  The MMA warp waits for weights ~10 % of the
-                                   // time (probes), but a 6-8 deep ring measured SLOWER (conv7 C=128: 1.98 -> 2.23 ms), so 4
-struct SmemP {
-    uint64_t b_full[kMaxStagesP];
-    uint64_t b_empty[kMaxStagesP];
-    uint64_t a_full[2];
-    uint64_t a_empty[2];
-    uint64_t acc_ready[2];
-    uint64_t acc_free[2];
-    uint32_t tmem_base;
-    uint32_t pad;
-};
-static_assert(sizeof(SmemP) <= kSmemHdr, "SmemP header");
-}  // namespace tc
-
-// F16 = true: fp16 hi + scaled-lo split (see split_store_f16): kind::f16 MMAs with K = 16; per accumulator TWO TMEM
-// regions -- D0 += a_hi * b_hi (promoted to registers every <= 48 MMAs like before, double-buffered per group) and
-// D1 += a_hi * b_lo' + a_lo' * b_hi (2^11-scaled cross terms: their accumulation error is 2^-11 of D0's, so D1 lives
-// in TMEM for the whole tile, double-buffered per tile, and is added once, times 2^-11, after the last group).
-// TMEM map (MT * N <= 128): D0[g & 1] at columns (g & 1) * MT*N, D1[tile & 1] at (2 + (tile & 1)) * MT*N.
-template <bool F16>
-__global__ void __launch_bounds__(tc::kThreadsP, 1) conv_tcp_kernel(TcConvParams p) {
-    constexpr int KG = F16 ? 2 : 4;                         // 16-byte k-groups per 16-channel chunk
-    constexpr int KSTEPS = F16 ? 1 : 2;                     // MMAs per chunk, tap and pass
-    constexpr int ACC = F16 ? 64 : 128;                     // fp32 register accumulators per accumulator thread
-    using namespace tc;
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    SmemP* sm = reinterpret_cast<SmemP*>(smem_raw);
-    const int N = p.N, MT = p.MT;
-    const int ncols = MT * N;                               // <= 256 (F16: 128) columns per TMEM region
-    const int R = 128 * MT + (p.Kr - 1) * p.dil;
-    const int Rpad = p.Rpad;
-    const uint32_t a_half = (uint32_t)Rpad * 16 * KG;
-    const uint32_t b_half = (uint32_t)N * 16 * KG;
-    uint8_t* a_base = smem_raw + kSmemHdr;
-    uint8_t* b_base = a_base + 4 * a_half;
-    const int S = p.stagesB;
-    const int P = p.promote_every;
-    float* stage_base = reinterpret_cast<float*>(b_base + (size_t)S * 2 * b_half);   // [8 warps][32][36] epilogue transpose stage
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int nchunk = p.nchunk, Kr = p.Kr;
-    // PERSISTENT: one CTA per SM walks the tile list L = blockIdx.x, += gridDim.x.  L -> (time tile, channel tile, batch),
-    // time fastest.  Every role keeps its ring / phase counters running across tiles, so the producers and the MMA warp
-    // are already two chunks (and two TMEM buffers) into tile i+1 while the accumulator warps still run the epilogue of
-    // tile i (measured before: accumulators idle 2/3 of a CTA's life, producers idle during the epilogue).
-    const int gx = (p.Tout + 128 * MT - 1) / (128 * MT), gy = p.Cout / N;
-    const int ntiles = gx * gy * p.B;
-    const int G = (nchunk + P - 1) / P;
-
-    if (tid == 0) {
-        for (int i = 0; i < kMaxStagesP; ++i) { mbar_init(&sm->b_full[i], 1); mbar_init(&sm->b_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&sm->a_full[i], 256); mbar_init(&sm->a_empty[i], 1);
-            mbar_init(&sm->acc_ready[i], 1); mbar_init(&sm->acc_free[i], 256);
-        }
-        fence_mbar_init();
-    }
-    if (warp == 1) tmem_alloc(&sm->tmem_base, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sm->tmem_base;
-
-    if (warp < 4) reg_dec<48>();      // whole control warpgroup at one program point (4*32*48 + 8*32*56 + 8*32*160 == 640*96)
-    if (warp == 0) {
-        if (lane == 0) {
-            int it = 0;
-            for (int L = blockIdx.x; L < ntiles; L += gridDim.x) {
-                const int ntile = (L / gx) % gy;
-                const float* wsrc = p.wblob + (size_t)ntile * nchunk * Kr * (size_t)(2 * b_half / 4);
-                for (int j = 0; j < nchunk * Kr; ++j, ++it) {
-                    int s = it % S;
-                    mbar_wait(&sm->b_empty[s], ((it / S) & 1) ^ 1);
-                    mbar_arrive_expect_tx(&sm->b_full[s], 2 * b_half);
-                    bulk_g2s(b_base + (size_t)s * 2 * b_half, wsrc + (size_t)j * (2 * b_half / 4), 2 * b_half, &sm->b_full[s]);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        {   // whole warp converged; tcgen05 instructions are elect-predicated inside their asm blocks
-            const uint32_t fmt = F16 ? 0u : 2u;          // A/B format: F16 = 0, TF32 = 2
-            const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem, 0);
-            const uint32_t a_base16 = __shfl_sync(0xffffffffu, smem_u32(a_base), 0) >> 4;
-            const uint32_t b_base16 = __shfl_sync(0xffffffffu, smem_u32(b_base), 0) >> 4;
-            const uint32_t a_lbo16 = (uint32_t)Rpad, b_lbo16 = (uint32_t)N;
-            const uint32_t a_half16 = a_half >> 4, b_half16 = b_half >> 4;
-            int it = 0, cg = 0, gg = 0, tl = 0;
-            const bool mprobe = kTcpProbe && blockIdx.x == 3;
-            long long w_a = 0, w_b = 0, w_acc = 0, tq;
-            for (int L = blockIdx.x; L < ntiles; L += gridDim.x, ++tl) {
-                for (int g = 0; g < G; ++g, ++gg) {
-                    const int abuf = gg & 1;
-                    if (mprobe) tq = clock64();
-                    mbar_wait(&sm->acc_free[abuf], ((gg >> 1) & 1) ^ 1);
-                    if (mprobe) w_acc += clock64() - tq;
-                    tc_fence_after();
-                    const int c_begin = g * P, c_end = (c_begin + P < nchunk) ? c_begin + P : nchunk;
-                    for (int c = c_begin; c < c_end; ++c, ++cg) {
-                        const int buf = cg & 1;
-                        if (mprobe) tq = clock64();
-                        mbar_wait(&sm->a_full[buf], (cg >> 1) & 1);
-                        if (mprobe) w_a += clock64() - tq;
-                        const uint32_t a_hi = a_base16 + (uint32_t)buf * 2 * a_half16;
-                        const uint32_t a_lo = a_hi + a_half16;
-                        for (int tap = 0; tap < Kr; ++tap, ++it) {
-                            const int s = it % S;
-                            if (mprobe) tq = clock64();
-                            mbar_wait(&sm->b_full[s], (it / S) & 1);
-                            if (mprobe) w_b += clock64() - tq;
-                            tc_fence_after();
-                            const uint32_t b_hi = b_base16 + (uint32_t)s * 2 * b_half16;
-                            const uint32_t b_lo = b_hi + b_half16;
-                            for (int mt = 0; mt < MT; ++mt) {
-                                const uint32_t row_off = (uint32_t)(mt * 128 + tap * p.dil);
-                                if constexpr (F16) {
-                                    const uint32_t d0 = tmem_u + (uint32_t)(abuf * ncols + mt * N);
-                                    const uint32_t d1 = tmem_u + (uint32_t)((2 + (tl & 1)) * ncols + mt * N);
-                                    const uint32_t first0 = ((c - c_begin) | tap) != 0, first1 = (g | (c - c_begin) | tap) != 0;
-                                    umma_bf16(d0, desc_u(a_hi + row_off, a_lbo16), desc_u(b_hi, b_lbo16), idesc, first0);
-                                    umma_bf16(d1, desc_u(a_hi + row_off, a_lbo16), desc_u(b_lo, b_lbo16), idesc, first1);
-                                    umma_bf16(d1, desc_u(a_lo + row_off, a_lbo16), desc_u(b_hi, b_lbo16), idesc, 1u);
-                                } else {
-                                    const uint32_t d_tmem = tmem_u + (uint32_t)(abuf * 256 + mt * N);
-#pragma unroll
-                                    for (int pass = 0; pass < 3; ++pass) {
-                                        const uint32_t aa = (pass == 2 ? a_lo : a_hi) + row_off;
-                                        const uint32_t bb = (pass == 1 ? b_lo : b_hi);
-#pragma unroll
-                                        for (int ks = 0; ks < KSTEPS; ++ks) {
-                                            uint32_t accum = ((c - c_begin) | tap | pass | ks) != 0;
-                                            umma_tf32(d_tmem, desc_u(aa + ks * 2 * a_lbo16, a_lbo16), desc_u(bb + ks * 2 * b_lbo16, b_lbo16), idesc, accum);
-                                        }
-                                    }
-                                }
-                            }
-                            umma_commit(&sm->b_empty[s]);
-                        }
-                        umma_commit(&sm->a_empty[buf]);
-                    }
-                    umma_commit(&sm->acc_ready[abuf]);
-                }
-            }
-            if (mprobe && lane == 0) { g_tc_phase_clock[2] = w_a; g_tc_phase_clock[3] = w_b; g_tc_phase_clock[4] = w_acc; }
-        }
-    } else if (warp >= 4 && warp < 12) {
-        // ================= activation producers (warps 4..11, 56 registers each) =================
-        reg_dec<56>();
-        const int wtid = tid - 128;                                 // 0..255
-        const bool probe = kTcpProbe && (wtid == 0 && blockIdx.x == 3);
-        const long long t_start = probe ? clock64() : 0;
-        long long w_ae = 0, tq = 0;
-        const PadMap pm = PadMap::make(p.Tin, p.pad_left_s, p.pad_right_s, p.reflect);
-        int cg = 0;
-        for (int L = blockIdx.x; L < ntiles; L += gridDim.x) {
-            const int t0 = (L % gx) * 128 * MT;
-            const int b = L / (gx * gy);
-            const float* __restrict__ xb = p.x + (size_t)b * p.x_bstride;
-            for (int c = 0; c < nchunk; ++c, ++cg) {
-                const int buf = cg & 1;
-                uint8_t* ahi = a_base + (size_t)buf * 2 * a_half;
-                if (probe) tq = clock64();
-                mbar_wait(&sm->a_empty[buf], ((cg >> 1) & 1) ^ 1);
-                if (probe) w_ae += clock64() - tq;
-                produce_chunk<256, false, 4, true, F16>(p, pm, xb, c, t0, R, Rpad, ahi, ahi + a_half, wtid);
-                fence_proxy_async();
-                mbar_arrive(&sm->a_full[buf]);
-            }
-        }
-        if (probe) { g_tc_phase_clock[0] = clock64() - t_start; g_tc_phase_clock[1] = w_ae; g_tc_phase_clock[7] = (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x; }
-    } else if (warp >= 12) {
-        // ================= accumulators (warps 12..19, 160 registers each): promote + epilogue =================
-        reg_inc<160>();
-        const int q = warp & 3;                                     // TMEM lane quarter
-        const int half = (warp - 12) >> 2;                          // column half of the tile set
-        int split = ((ncols / 2 + 15) / 16) * 16;
-        if (split > ncols) split = ncols;
-        const int mycol0 = half ? split : 0;
-        const int mycols = half ? ncols - split : split;
-        float* stage = stage_base + (size_t)(warp - 12) * (32 * 36);
-        const int c4 = lane & 7, rsub = lane >> 3;
-        const int act = p.out_act;
-        const bool aprobe = kTcpProbe && (tid == 12 * 32 && blockIdx.x == 3);
-        int gg = 0, tl = 0;
-        long long w_ar = 0, t_ep = 0, tq = 0;
-        for (int L = blockIdx.x; L < ntiles; L += gridDim.x, ++tl) {
-            const int t0 = (L % gx) * 128 * MT;
-            const int ntile = (L / gx) % gy;
-            const int b = L / (gx * gy);
-            float acc[ACC];
-#pragma unroll
-            for (int i = 0; i < ACC; ++i) acc[i] = 0.f;
-            for (int g = 0; g < G; ++g, ++gg) {
-                const int abuf = gg & 1;
-                if (aprobe) tq = clock64();
-                mbar_wait(&sm->acc_ready[abuf], (gg >> 1) & 1);   // on the critical path (2 TMEM buffers): polled, not parked
-                if (aprobe) w_ar += clock64() - tq;
-                tc_fence_after();
-                const uint32_t tbase = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(abuf * (F16 ? ncols : 256) + mycol0);
-#pragma unroll
-                for (int grp = 0; grp < ACC / 16; ++grp) {
-                    if (grp * 16 < mycols) {
-                        uint32_t v[16];
-                        tmem_ld16(tbase + grp * 16, v);
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) acc[grp * 16 + i] += __uint_as_float(v[i]);
-                    }
-                }
-                if constexpr (F16) {
-                    if (g == G - 1) {
-                        // the last group's commit covers every MMA of the tile: add the scaled cross terms, then release
-                        // (acc_free of this group also tells the MMA warp that D1[tile & 1] may be overwritten two tiles on)
-                        const uint32_t t1 = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)((2 + (tl & 1)) * ncols + mycol0);
-#pragma unroll
-                        for (int grp = 0; grp < ACC / 16; ++grp) {
-                            if (grp * 16 < mycols) {
-                                uint32_t v[16];
-                                tmem_ld16(t1 + grp * 16, v);
-#pragma unroll
-                                for (int i = 0; i < 16; ++i) acc[grp * 16 + i] = fmaf(__uint_as_float(v[i]), kLoUnscale, acc[grp * 16 + i]);
-                            }
-                        }
-                    }
-                }
-                tc_fence_before();
-                mbar_arrive(&sm->acc_free[abuf]);
-            }
-            // ---- epilogue.  The TMEM buffers are already released, so the MMA warp and the producers work on the next
-            // tile meanwhile.  32-column slabs of the register tile go through a private [32][36] shared-memory
-            // transpose stage (conflict-free both ways) and leave coalesced (8 lanes = 128 contiguous bytes of a row).
-            // The slab loop is ROLLED on purpose (the fully unrolled register epilogue was 20k SASS instructions and ran
-            // out of the instruction cache); only the register -> stage copy is selected by a switch.
-            float* __restrict__ yb = p.y + (size_t)b * p.y_bstride;
-            const float* __restrict__ rb = p.res ? p.res + (size_t)b * p.y_bstride : nullptr;
-            if (aprobe) tq = clock64();
-#pragma unroll 1
-            for (int sl = 0; sl * 32 < mycols; ++sl) {
-#define FAC_PARK(S0)                                                                                              \
-    _Pragma("unroll") for (int j = 0; j < 8; ++j)                                                                \
-        *reinterpret_cast<float4*>(stage + lane * 36 + j * 4) =                                                  \
-            make_float4(acc[(S0) + j * 4], acc[(S0) + j * 4 + 1], acc[(S0) + j * 4 + 2], acc[(S0) + j * 4 + 3]);
-                if constexpr (F16) {
-                    switch (sl) {
-                        case 0: FAC_PARK(0) break;
-                        default: FAC_PARK(32) break;
-                    }
-                } else {
-                    switch (sl) {
-                        case 0: FAC_PARK(0) break;
-                        case 1: FAC_PARK(32) break;
-                        case 2: FAC_PARK(64) break;
-                        default: FAC_PARK(96) break;
-                    }
-                }
-#undef FAC_PARK
-                __syncwarp();
-                const int jc = sl * 32 + c4 * 4;                        // column inside my range handled by this lane
-                if (jc < mycols) {
-                    const int jflat = mycol0 + jc;
-                    const int mt = jflat / N, col = jflat - mt * N;
-                    const int co = ntile * N + col;
-                    float4 bi = make_float4(0.f, 0.f, 0.f, 0.f), al = bi, ia = bi;
-                    if (p.bias) bi = __ldg(reinterpret_cast<const float4*>(p.bias + co));
-                    if (act == ACT_SNAKE) {
-                        al = __ldg(reinterpret_cast<const float4*>(p.out_alpha + co));
-                        ia = __ldg(reinterpret_cast<const float4*>(p.out_inv_alpha + co));
-                    }
-                    const int tbase_row = t0 + mt * 128 + q * 32;
-#pragma unroll 2
-                    for (int i = 0; i < 8; ++i) {
-                        const int row = 4 * i + rsub;
-                        const int t = tbase_row + row;
-                        if (t >= p.Tout) continue;
-                        float4 o = *reinterpret_cast<const float4*>(stage + row * 36 + c4 * 4);
-                        o.x += bi.x; o.y += bi.y; o.z += bi.z; o.w += bi.w;
-                        if (act == ACT_SNAKE) {
-                            o = snake4<true>(o, al, ia);
-                        } else if (act == ACT_TANH) {
-                            o.x = tanhf(o.x); o.y = tanhf(o.y); o.z = tanhf(o.z); o.w = tanhf(o.w);
-                        } else if (act == ACT_MISH) {
-                            o.x = mish_f(o.x); o.y = mish_f(o.y); o.z = mish_f(o.z); o.w = mish_f(o.w);
-                        }
-                        if (rb) {
-                            float4 r1 = *reinterpret_cast<const float4*>(rb + (size_t)t * p.ldy + co);
-                            o.x += r1.x; o.y += r1.y; o.z += r1.z; o.w += r1.w;
-                        }
-                        *reinterpret_cast<float4*>(yb + (size_t)t * p.ldy + co) = o;
-                    }
-                }
-                __syncwarp();
-            }
-            if (aprobe) t_ep += clock64() - tq;
-        }
-        if (aprobe) { g_tc_phase_clock[5] = w_ar; g_tc_phase_clock[6] = t_ep; }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, 512);
-}
+}  // namespace
 
 // ---- host side ---------------------------------------------------------------------------------
-int g_tc_dbg = 0;       // fac_set_option "tc_dbg": timing experiments with WRONG results (bit 0: stale weights, bit 1: stale activations)
-int g_tc_groups_ok = 1; // fac_set_option "tc_groups": 0 = one producer group on 8-worker tiles (A/B aid, process-wide)
-int g_tc_wide_ok = 1;
-int g_tc_slot_issue = 1;   // fac_set_option "tc_slot_issue": 0 = legacy per-tap weight-ring bookkeeping in the MMA warp (A/B aid)   // fac_set_option "tc_wide": 0 plans every conv_tc tile with 8 worker warps (A/B aid, process-wide)
+namespace {
+constexpr size_t kSmemCap = 227 * 1024;        // dynamic shared memory per block (sm_90)
+constexpr size_t kSmemCap2 = 113 * 1024;       // per block with two resident blocks (228 KB per SM, 1 KB reserved each)
+int plan_prec(const TcConvParams& p) {
+    return p.g1f16 ? P_F16S : (p.f16x2 ? P_F16X2 : (p.bf16 ? P_BF16 : P_TF32));
+}
+}  // namespace
 
 bool tc_conv_plan(TcConvParams& p) {
-    p.wide = 0; p.ng = 1;
-    p.cps = 0;
-    // p.Cin, p.vf, p.Kr, p.dil, p.Cout, p.promoted must be set; fills N, MT, nchunk, Rpad, stagesB, ...
-    if ((p.Cin % 4) != 0 || ((p.Cin * p.vf) % tc::kChunk) != 0 || (p.Cout % 16) != 0) return false;
-    int N = 0;
-    for (int cand = p.promoted ? 128 : 256; cand >= 16; cand -= 16)
-        if (p.Cout % cand == 0) { N = cand; break; }
-    if (N < 32) return false;
-    p.N = N;
-    const int KG = p.bf16 ? 2 : 4;
+    // p.Cin, p.vf, p.Kr, p.dil, p.Cout, p.promoted (+ bf16 / g1f16 / f16x2 / fused / tt / occ2_maxn) must be set; fills N,
+    // MT, nchunk, Rpad, stagesB, b_slot, smem_bytes, promote_every, occ2
+    if ((p.Cin % 4) != 0 || ((p.Cin * p.vf) % kChunk) != 0 || (p.Cout % 16) != 0) return false;
     if (p.bf16 && p.promoted) return false;
     if (p.f16x2 && !p.promoted) return false;
     if (p.g1f16 && !p.bf16) return false;
-    if (p.fused && (N != p.Cout || p.Cin != p.Cout || p.vf != 1 || N > 256)) return false;
-    p.nchunk = p.Cin * p.vf / tc::kChunk;
-    p.nchunk2 = p.fused ? p.Cout / tc::kChunk : 0;
-    // rows the tile grid actually covers for a given MT: short sequences (T' = 320 stages) waste up to 37 % of the MMAs in
-    // the padded tail of a 256-row tile, so MT is halved while that saves more than 10 % (only when the caller set Tout)
-    auto padded_rows = [&](int mt) { const long long tile = 128LL * mt; return (p.Tout + tile - 1) / tile * tile; };
-    auto trim_mt = [&](int mt) {
-        if (p.Tout > 0)
-            while (mt > 1 && padded_rows(mt) * 10 > padded_rows(mt / 2) * 11) mt >>= 1;
-        return mt;
-    };
-    if (p.promoted) {
-        const int KGp = p.f16x2 ? 2 : 4;
-        if (p.f16x2) {
-            // fp16 hi + scaled-lo: four TMEM regions of MT*N <= 128 columns; one MMA per chunk and tap into D0
-            p.MT = trim_mt(N <= 32 ? 4 : (N <= 64 ? 2 : 1));
-            p.promote_every = 48 / p.Kr < 1 ? 1 : 48 / p.Kr;
-        } else {
-            p.MT = trim_mt((N <= 64) ? 4 : 2);     // MT * N <= 256 columns per TMEM buffer
-            p.promote_every = 8 / p.Kr < 1 ? 1 : 8 / p.Kr;
-        }
-        int R = 128 * p.MT + (p.Kr - 1) * p.dil, Rpad = R;
-        while (Rpad % 8 != 2) ++Rpad;
-        p.Rpad = Rpad;
-        p.tmem_cols = 512;
-        size_t a_bytes = (size_t)4 * Rpad * 16 * KGp, b_stage = (size_t)2 * N * 16 * KGp;
-        const size_t stage_bytes = (size_t)8 * 32 * 36 * 4;     // accumulator warps' private epilogue transpose stage
-        int S = tc::kMaxStagesP;
-        while (S > 2 && tc::kSmemHdr + a_bytes + S * b_stage + stage_bytes > 225 * 1024) --S;
-        if (tc::kSmemHdr + a_bytes + S * b_stage + stage_bytes > 225 * 1024) return false;
-        p.stagesB = S;
-        p.smem_bytes = tc::kSmemHdr + a_bytes + S * b_stage + stage_bytes;
-        return true;
+    if (p.tt && !p.f16x2) return false;
+    if (p.fused && (p.promoted || p.Cin != p.Cout || p.vf != 1 || p.Cout > 256)) return false;
+    const int P1 = plan_prec(p), P2 = p.fused ? (p.bf16 ? P_BF16 : P_TF32) : P_NONE;
+    p.nchunk = p.Cin * p.vf / kChunk;
+    p.nchunk2 = p.fused ? p.Cout / kChunk : 0;
+    p.promote_every = p.promoted ? (p.f16x2 ? (48 / p.Kr < 1 ? 1 : 48 / p.Kr) : (8 / p.Kr < 1 ? 1 : 8 / p.Kr)) : 1;
+    const int nw_max = p.promoted ? 64 : 128;      // accumulator registers per thread: NW / 2 (x 3 when promoted)
+    // N depends on the layer's shape and split class only (never on dil, Tout, tt or occ2_maxn): the weight blob is laid
+    // out for it once (tc_pack_blob) and every later plan of the layer must find the same N.  It is the widest tile whose
+    // weight slot and fused GEMM-2 operand leave kAReserve bytes for the activation buffers; a fused unit needs N = C.
+    constexpr size_t kAReserve = 40 * 1024;
+    int N = 0;
+    for (int cand = p.fused ? p.Cout : 256; cand >= 16 && N == 0; cand -= 16) {
+        const bool rows_split = cand <= nw_max, cols_split = (cand / 2) % 16 == 0 && cand / 2 <= nw_max;
+        if (p.Cout % cand || !(rows_split || cols_split)) continue;
+        size_t slot = (size_t)p.Kr * prec_planes(P1) * prec_kg(P1) * cand * 16, a2 = 0;
+        if (P2 != P_NONE) a2 = (size_t)prec_planes(P2) * p.nchunk2 * prec_kg(P2) * 64 * 16;
+        if (kSmemHdr + kAReserve + slot + a2 <= kSmemCap) N = cand;
+        else if (p.fused) return false;
     }
-    // conv_tc_kernel.  A tile is MT accumulators of 128 rows x N columns (x2 when fused: D1 and D2) sharing every weight
-    // tile.  Two candidate residencies: two CTAs per SM (<= 256 TMEM columns, <= 112 KB smem each; one CTA's produce and
-    // epilogue phases hide behind the other's MMAs) when the caller allows it for this N, else one CTA per SM.
-    const int per = (p.fused ? 2 : 1) * N;
-    for (int pass = (p.occ2_maxn > 0 && N <= p.occ2_maxn) ? 0 : 1; pass < 2; ++pass) {
-        const int colcap = pass == 0 ? 256 : 512;
-        const size_t smemcap = pass == 0 ? 112 * 1024 : 225 * 1024;
-        int MT = colcap / per;
-        MT = MT >= 4 ? 4 : (MT >= 2 ? 2 : MT);
-        if (p.fused && MT > 2) MT = 2;
-        if (MT >= 1) MT = trim_mt(MT);
-        // a tile that owns the SM (one CTA resident) runs 16 worker warps in two producer groups over a 4-deep operand ring
-        // (bf16-class kernels only); if that does not fit, 8 workers and 2 buffers
-        const bool want_wide = pass == 1 && g_tc_wide_ok && p.bf16 && (N % 32) == 0;
-        for (; MT >= 1; MT >>= 1)
-        for (int wide = want_wide ? 1 : 0; wide >= 0; --wide)
-        for (int ng = 2; ng >= 1; --ng) {
-            int R = 128 * MT + (p.Kr - 1) * p.dil, Rpad = R;
-            while (Rpad % 8 != 2) ++Rpad;
-            // producer groups: 16 workers always run two; 8 workers when a 4-warp group covers a chunk in <= PIPE_P (5)
-            // pieces per thread (R <= 160 rows), bf16-class kernels only
-            if (wide && ng == 1) continue;
-            if (!wide && ng == 2 && !(g_tc_groups_ok && p.bf16 && R <= 5 * 32)) continue;
-            int cols = MT * per, pow2 = 32;
-            while (pow2 < cols) pow2 <<= 1;
-            size_t a_bytes = (size_t)ng * (p.g1f16 ? 2 : 4) * Rpad * 16 * KG;   // 2 (4) bufs x (hi,lo) [hi only: one fp16 pass]
-            const size_t tile1 = (size_t)(p.g1f16 ? 1 : 2) * N * 16 * KG, tile2 = (size_t)2 * N * 16 * KG;
-            // fused: the whole GEMM-2 operand snake2(D1 + b7) stays resident: nchunk2 chunks of (hi,lo) x KG x R2pad x 16 B
-            const int R2pad = 128 * MT + 2;
-            size_t a2_bytes = p.fused ? (size_t)p.nchunk2 * 2 * KG * R2pad * 16 : 0;
-            if (tc::kSmemHdr + a_bytes + a2_bytes + 2 * (p.fused && tile2 > tile1 ? tile2 : tile1) > smemcap) continue;
-            // weight ring: S slots of `tpt` consecutive (chunk, tap) tiles each, one bulk copy per slot.  Small copies leave
-            // the MMA warp waiting on L2 round trips, so take the slot/stage combination with the most bytes in flight
-            // (capped: beyond ~96 KB nothing is gained), preferring more stages on ties.
-            const size_t avail = smemcap - tc::kSmemHdr - a_bytes - a2_bytes;
-            const int ntiles = p.nchunk * p.Kr;
-            int S = 0, tpt = 1, cps = 0;
-            size_t best = 0;
-            // preferred: a slot = every tap of `c` consecutive chunks (slot-structured issue loop, unrolled taps)
-            if (g_tc_slot_issue && (p.Kr == 1 || p.Kr == 2 || p.Kr == 7))
-                for (int c = 1; c <= 16 && c <= p.nchunk; ++c) {
-                    size_t slot = (size_t)c * p.Kr * tile1;
-                    if (p.fused && slot < tile2) slot = tile2;
-                    int s_max = (int)(avail / slot);
-                    if (s_max > tc::kMaxStagesB) s_max = tc::kMaxStagesB;
-                    if (s_max < 2) break;
-                    size_t flight = (size_t)s_max * slot;
-                    if (flight > 96 * 1024) flight = 96 * 1024;
-                    if (flight > best || (flight == best && s_max > S)) { best = flight; S = s_max; tpt = c * p.Kr; cps = c; }
+    if (N == 0) return false;
+    // Two resident CTAs per SM (tiles of N <= occ2_maxn, plain accumulation only): one CTA's operand production and
+    // epilogue overlap the other's MMAs; each gets half the shared memory and <= 128 registers per thread.
+    const bool want2 = p.occ2_maxn > 0 && N <= p.occ2_maxn && !p.promoted;
+    for (int two = want2 ? 1 : 0; two >= 0; --two) {
+        const size_t cap = two ? kSmemCap2 : kSmemCap;
+        const int nwl = two ? 64 : nw_max;
+        for (int S = 2; S >= 1; --S)
+            for (int MT = 2; MT >= 1; --MT) {
+                const int NW = MT == 2 ? N : N / 2;
+                if (NW > nwl || NW % 16) continue;
+                const int BM = 64 * MT;
+                int Rpad = BM + (p.Kr - 1) * p.dil;
+                while (Rpad % 8 != 2) ++Rpad;               // conflict-free 16-byte producer stores
+                const size_t a_bytes = (size_t)prec_planes(P1) * prec_kg(P1) * Rpad * 16;
+                size_t slot = (size_t)p.Kr * prec_planes(P1) * prec_kg(P1) * N * 16;
+                size_t a2 = 0;
+                if (P2 != P_NONE) {
+                    const size_t slot2 = (size_t)prec_planes(P2) * prec_kg(P2) * N * 16;
+                    if (slot2 > slot) slot = slot2;
+                    a2 = (size_t)prec_planes(P2) * p.nchunk2 * prec_kg(P2) * BM * 16;
                 }
-            if (S < 2)
-            for (int cand = 1; cand <= 16 && cand <= ntiles; ++cand) {
-                size_t slot = cand * tile1;
-                if (p.fused && slot < tile2) slot = tile2;
-                int s_max = (int)(avail / slot);
-                if (s_max > tc::kMaxStagesB) s_max = tc::kMaxStagesB;
-                if (s_max < 2) break;
-                size_t flight = (size_t)s_max * slot;
-                if (flight > 96 * 1024) flight = 96 * 1024;
-                if (flight > best || (flight == best && s_max > S)) { best = flight; S = s_max; tpt = cand; }
+                // transposed: a warpgroup's A operand is always 64 channel rows; rows past its NW read (and discard)
+                // whatever follows the weight slot, so the buffer ends with 64 rows of slack
+                const size_t total = kSmemHdr + 2 * a_bytes + S * slot + a2 + (p.tt ? 64 * 16 : 0);
+                if (total > cap) continue;
+                p.N = N; p.MT = MT; p.Rpad = Rpad; p.R2pad = BM; p.stagesB = S; p.b_slot = (int)slot; p.smem_bytes = total;
+                p.occ2 = two;
+                return true;
             }
-            if (S < 2) continue;
-            size_t b_stage = tpt * tile1;
-            if (p.fused && b_stage < tile2) b_stage = tile2;
-            p.tpt = tpt; p.cps = cps; p.b_slot = (int)b_stage;
-            p.tpt2 = p.fused ? (int)(b_stage / tile2) : 1;
-            if (p.tpt2 < 1) p.tpt2 = 1;
-            size_t total = tc::kSmemHdr + a_bytes + S * b_stage + a2_bytes;
-            p.wide = wide; p.ng = ng;
-            const size_t stage = (size_t)(p.wide ? 16 : 8) * 32 * 36 * 4 + tc::kSmemHdr;   // epilogue transpose stage (one [32][36] float tile per worker warp)
-            if (total < stage) total = stage;
-            p.MT = MT; p.Rpad = Rpad; p.R2pad = R2pad; p.tmem_cols = pow2; p.stagesB = S; p.smem_bytes = total;
-            return true;
-        }
     }
     return false;
 }
@@ -1178,90 +497,57 @@ void tc_pack_blob(const TcConvParams& p, const float* wp, int ldw, float* blob) 
                             }
 }
 
-cudaError_t tc_read_phase_clocks(long long* out8) {
-    return cudaMemcpyFromSymbol(out8, g_tc_phase_clock, sizeof(long long) * 8);
-}
-cudaError_t tc_read_producer_clocks(long long* out4) {
-    return cudaMemcpyFromSymbol(out4, g_tc_prod_clock, sizeof(long long) * 4);
-}
-cudaError_t tc_read_trace(long long* out80) {
-    return cudaMemcpyFromSymbol(out80, g_tc_trace, sizeof(long long) * 80);
-}
-
-// Function attributes (the > 48 KB dynamic shared-memory opt-in) and the SM count are PER DEVICE: a process may hold
-// handles on several GPUs (fac_create(out, device)), so both are tracked per device id under a mutex.
 namespace {
-struct DevCfg { bool done = false; int sm_count = 0; };
-DevCfg g_devcfg[64];
-std::mutex g_devcfg_mu;
-cudaError_t ensure_device_config(int& sm_count) {
+template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false>
+cudaError_t launch_one(const TcConvParams& p, dim3 grid, cudaStream_t st) {
+    // the > 48 KB dynamic shared-memory opt-in is per device and per kernel
+    static bool done[64] = {};
+    static std::mutex mu;
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
     if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-    std::lock_guard<std::mutex> lk(g_devcfg_mu);
-    DevCfg& d = g_devcfg[dev];
-    if (!d.done) {
-        const int cap = 225 * 1024;
-        e = cudaFuncSetAttribute(conv_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<false, true, false, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, true, false, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<false, true, true, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, true, true, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<false, true, false, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, true, false, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<false, true, true, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, true, true, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tcp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tcp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-        if (e != cudaSuccess) return e;
-        if (cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sm_count <= 0) d.sm_count = 148;
-        d.done = true;
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        if (!done[dev]) {
+            e = cudaFuncSetAttribute(conv_tc_kernel<P1, P2, PROMO, NI, MINB, TT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)kSmemCap);
+            if (e != cudaSuccess) return e;
+            done[dev] = true;
+        }
     }
-    sm_count = d.sm_count;
-    return cudaSuccess;
+    conv_tc_kernel<P1, P2, PROMO, NI, MINB, TT><<<grid, kThreads, p.smem_bytes, st>>>(p);
+    return cudaGetLastError();
+}
+template <int P1, int P2, bool PROMO, int MINB = 1>
+cudaError_t launch_ni(const TcConvParams& p, dim3 grid, cudaStream_t st) {
+    const int NW = p.MT == 2 ? p.N : p.N / 2;
+    if (NW % 64 == 0) return launch_one<P1, P2, PROMO, 64, MINB>(p, grid, st);
+    if (NW % 32 == 0) return launch_one<P1, P2, PROMO, 32, MINB>(p, grid, st);
+    return launch_one<P1, P2, PROMO, 16, MINB>(p, grid, st);
+}
+template <int P1, int P2>
+cudaError_t launch_occ(const TcConvParams& p, dim3 grid, cudaStream_t st) {
+    return p.occ2 ? launch_ni<P1, P2, false, 2>(p, grid, st) : launch_ni<P1, P2, false, 1>(p, grid, st);
 }
 }  // namespace
 
-cudaError_t launch_conv_tc(const TcConvParams& p_in, cudaStream_t st) {
-    if (p_in.Tout <= 0 || p_in.B <= 0) return cudaSuccess;
-    TcConvParams p = p_in;
-    p.dbg = g_tc_dbg;
-    int sm_count = 148;
-    cudaError_t e0 = ensure_device_config(sm_count);
-    if (e0 != cudaSuccess) return e0;
-    dim3 grid((p.Tout + 128 * p.MT - 1) / (128 * p.MT), p.Cout / p.N, p.B);
-    if (p.promoted) {
-        const long long ntiles = (long long)grid.x * grid.y * grid.z;
-        const unsigned nctas = (unsigned)(ntiles < sm_count ? ntiles : sm_count);   // persistent: one CTA per SM
-        if (p.f16x2) conv_tcp_kernel<true><<<dim3(nctas), tc::kThreadsP, p.smem_bytes, st>>>(p);
-        else conv_tcp_kernel<false><<<dim3(nctas), tc::kThreadsP, p.smem_bytes, st>>>(p);
-    } else {
-        if (grid.y > 65535 || grid.z > 65535) return cudaErrorInvalidValue;
-        constexpr int kThreadsW = 64 + 32 * 16;
-        if (p.wide && !p.bf16) return cudaErrorInvalidValue;
-        if (p.wide && p.fused && p.g1f16) conv_tc_kernel<true, true, true, 16><<<grid, kThreadsW, p.smem_bytes, st>>>(p);
-        else if (p.wide && p.g1f16) conv_tc_kernel<false, true, true, 16><<<grid, kThreadsW, p.smem_bytes, st>>>(p);
-        else if (p.wide && p.fused) conv_tc_kernel<true, true, false, 16><<<grid, kThreadsW, p.smem_bytes, st>>>(p);
-        else if (p.wide) conv_tc_kernel<false, true, false, 16><<<grid, kThreadsW, p.smem_bytes, st>>>(p);
-        else if (p.ng == 2 && !p.bf16) return cudaErrorInvalidValue;
-        else if (p.ng == 2 && p.fused && p.g1f16) conv_tc_kernel<true, true, true, 8, 2><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else if (p.ng == 2 && p.g1f16) conv_tc_kernel<false, true, true, 8, 2><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else if (p.ng == 2 && p.fused) conv_tc_kernel<true, true, false, 8, 2><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else if (p.ng == 2) conv_tc_kernel<false, true, false, 8, 2><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else if (p.fused && p.bf16 && p.g1f16) conv_tc_kernel<true, true, true><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else if (p.bf16 && p.g1f16) conv_tc_kernel<false, true, true><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else if (p.fused && p.bf16) conv_tc_kernel<true, true><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else if (p.fused) conv_tc_kernel<true, false><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else if (p.bf16) conv_tc_kernel<false, true><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
-        else conv_tc_kernel<false, false><<<grid, tc::kThreads, p.smem_bytes, st>>>(p);
+cudaError_t launch_conv_tc(const TcConvParams& p, cudaStream_t st) {
+    if (p.Tout <= 0 || p.B <= 0) return cudaSuccess;
+    const int BM = 64 * p.MT;
+    dim3 grid((p.Tout + BM - 1) / BM, p.Cout / p.N, p.B);
+    if (grid.y > 65535 || grid.z > 65535) return cudaErrorInvalidValue;
+    const int P1 = plan_prec(p);
+    if (p.fused) {
+        if (P1 == P_F16S) return launch_occ<P_F16S, P_BF16>(p, grid, st);
+        if (P1 == P_BF16) return launch_occ<P_BF16, P_BF16>(p, grid, st);
+        return launch_occ<P_TF32, P_TF32>(p, grid, st);
     }
-    return cudaGetLastError();
+    if (p.tt) return launch_one<P_F16X2, P_NONE, true, 64, 1, true>(p, grid, st);
+    if (p.promoted) return P1 == P_F16X2 ? launch_ni<P_F16X2, P_NONE, true>(p, grid, st) : launch_ni<P_TF32, P_NONE, true>(p, grid, st);
+    if (P1 == P_F16S) return launch_occ<P_F16S, P_NONE>(p, grid, st);
+    if (P1 == P_BF16) return launch_occ<P_BF16, P_NONE>(p, grid, st);
+    return launch_occ<P_TF32, P_NONE>(p, grid, st);
 }
 
 }  // namespace fac

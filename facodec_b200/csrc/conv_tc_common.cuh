@@ -1,5 +1,5 @@
-// tcgen05 / mbarrier / bulk-TMA primitives and the activation-operand producer shared by the tensor-core conv kernels
-// (conv_tc.cu: conv_tc_kernel, conv_tcp_kernel; conv_tt.cu: conv_tt_kernel).  Device code only.
+// mbarrier / bulk-copy / wgmma primitives and the activation-operand producer of the tensor-core conv kernel
+// (conv_tc.cu).  Device code only.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -11,10 +11,9 @@ namespace fac {
 
 namespace tc {
 
-constexpr int kThreads = 320;      // warp 0: weights, warp 1: MMA, warps 2..9: activation producers + epilogue
+constexpr int kThreads = 256;     // two warpgroups: both produce operands, each issues wgmma for its share of the tile
 constexpr int kChunk = 16;        // K elements (channels) per pipeline chunk
-constexpr int kMaxStagesB = 4;
-constexpr int kSmemHdr = 384;     // barriers + TMEM base at the start of dynamic shared memory
+constexpr int kSmemHdr = 128;     // mbarriers at the start of dynamic shared memory
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -27,13 +26,8 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// Two flavours of waiting.  The hand-offs on the critical path (weight ring, operand ring, TMEM buffers seen from the
-// MMA warp and the producers) poll try_wait back to back.  Warps that wait for a long time for something that is not
-// latency critical (accumulator / epilogue warps waiting for a whole GEMM group) pass a suspend-time hint, which parks
-// the thread in hardware: polled, those ~8 warps took a measurable share of the issue slots (ncu: ~60k warp-instructions
-// of spinning per 512-row tile next to 160k of useful work) -- but a parked thread seems to wake at the END of the hint
-// rather than when the phase completes (a 4 us hint made every group hand-off ~8k cycles late: +30 % on layers with
-// short groups), so the hint is kept short (0.4 us) and never used on the critical hand-offs.
+// Two flavours of waiting: polled back to back (RELAXED = false), or with a short suspend-time hint (0.4 us) that parks
+// the thread in hardware between polls.
 template <bool RELAXED>
 __device__ __forceinline__ bool mbar_try_wait_t(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
@@ -74,129 +68,70 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols));
-}
-// The MMA warp runs its loop CONVERGED (all 32 lanes); each tcgen05 instruction is issued by the lane
-// elect.sync picks, inside the same asm block.  (Issuing from an `if (lane == 0)` region made the compiler
-// wrap every UTCHMMA in an ELECT / BRA.U.ANY serialisation loop: ~75 extra cycles per MMA, measured.)
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
-}
-template <bool BF16>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    if constexpr (BF16) umma_bf16(tmem_d, adesc, bdesc, idesc, accum);
-    else umma_tf32(tmem_d, adesc, bdesc, idesc, accum);
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {   // converged warp; one elected lane commits
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-        ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Split issue / wait so that a TMEM load can stay in flight behind arithmetic on the previous one.  The wait names the
-// destination registers as in/out operands: the compiler then cannot move a read of them above the wait.
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait16(uint32_t (&v)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                   "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15])
-                 :: "memory");
-}
-__device__ __forceinline__ void tmem_ld8_issue(uint32_t taddr, uint32_t (&v)[8]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait8(uint32_t (&v)[8]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7])
-                 :: "memory");
-}
-
-// UMMA shared-memory descriptor, K-major, SWIZZLE_NONE: core matrix = 8 rows x 16 bytes stored as
-// 128 contiguous bytes; SBO = byte pitch between 8-row groups, LBO = byte pitch between the two
-// 16-byte K halves of one K=8 (tf32) MMA; version = 1 (sm_100).
-__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// ---- wgmma (sm_90a) ------------------------------------------------------------------------------
+// Shared-memory matrix descriptor, K-major, no swizzle: core matrix = 8 rows x 16 bytes stored as 128 contiguous
+// bytes; LBO = byte pitch between core matrices adjacent in K, SBO = byte pitch between 8-row groups.
+__device__ __forceinline__ uint64_t gdesc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// Same descriptor from warp-uniform pieces: lo = (address >> 4) + (LBO/16 << 16), hi = SBO/16 (= 8) | version bit 46.
-// The MMA warp keeps every ingredient warp-uniform (values broadcast with __shfl_sync, loop counters, kernel
-// parameters) so the descriptor arithmetic runs on the uniform datapath instead of R2UR round trips: the single
-// issuing warp was the critical resource for N <= 128 tiles (measured ~88 cycles per MMA issued, 35 on the tensor pipe).
-__device__ __forceinline__ uint64_t desc_u(uint32_t addr16, uint32_t lbo16) {
-    uint64_t d;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(addr16 + (lbo16 << 16)), "r"(0x4008u));
-    return d;
+enum WgKind { WG_TF32 = 0, WG_BF16 = 1, WG_F16 = 2 };
+
+#define FAC_R16(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
+    "+f"(d[o + 6]), "+f"(d[o + 7]), "+f"(d[o + 8]), "+f"(d[o + 9]), "+f"(d[o + 10]), "+f"(d[o + 11]), "+f"(d[o + 12]), \
+    "+f"(d[o + 13]), "+f"(d[o + 14]), "+f"(d[o + 15])
+#define FAC_R8(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
+    "+f"(d[o + 6]), "+f"(d[o + 7])
+#define FAC_D8 "{%0, %1, %2, %3, %4, %5, %6, %7}"
+#define FAC_D16 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}"
+#define FAC_D32 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+
+// D[64 x NI] += A[64 x K] * B[NI x K]^T, both operands K-major in shared memory; K = 16 (f16 / bf16) or 8 (tf32).
+template <int NI, int KIND>
+__device__ __forceinline__ void wgmma_ss(float (&d)[NI / 2], uint64_t da, uint64_t db) {
+    static_assert(NI == 16 || NI == 32 || NI == 64, "instruction N");
+    if constexpr (NI == 64 && KIND == WG_TF32)
+        asm volatile("wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " FAC_D32 ", %32, %33, 1, 1, 1;"
+                     : FAC_R16(0), FAC_R16(16) : "l"(da), "l"(db));
+    else if constexpr (NI == 64 && KIND == WG_BF16)
+        asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " FAC_D32 ", %32, %33, 1, 1, 1, 0, 0;"
+                     : FAC_R16(0), FAC_R16(16) : "l"(da), "l"(db));
+    else if constexpr (NI == 64 && KIND == WG_F16)
+        asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " FAC_D32 ", %32, %33, 1, 1, 1, 0, 0;"
+                     : FAC_R16(0), FAC_R16(16) : "l"(da), "l"(db));
+    else if constexpr (NI == 32 && KIND == WG_TF32)
+        asm volatile("wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 " FAC_D16 ", %16, %17, 1, 1, 1;"
+                     : FAC_R16(0) : "l"(da), "l"(db));
+    else if constexpr (NI == 32 && KIND == WG_BF16)
+        asm volatile("wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 " FAC_D16 ", %16, %17, 1, 1, 1, 0, 0;"
+                     : FAC_R16(0) : "l"(da), "l"(db));
+    else if constexpr (NI == 32)
+        asm volatile("wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 " FAC_D16 ", %16, %17, 1, 1, 1, 0, 0;"
+                     : FAC_R16(0) : "l"(da), "l"(db));
+    else if constexpr (KIND == WG_TF32)
+        asm volatile("wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 " FAC_D8 ", %8, %9, 1, 1, 1;"
+                     : FAC_R8(0) : "l"(da), "l"(db));
+    else if constexpr (KIND == WG_BF16)
+        asm volatile("wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 " FAC_D8 ", %8, %9, 1, 1, 1, 0, 0;"
+                     : FAC_R8(0) : "l"(da), "l"(db));
+    else
+        asm volatile("wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 " FAC_D8 ", %8, %9, 1, 1, 1, 0, 0;"
+                     : FAC_R8(0) : "l"(da), "l"(db));
 }
+#undef FAC_R8
+#undef FAC_D8
+#undef FAC_R16
+#undef FAC_D16
+#undef FAC_D32
 
 __device__ __forceinline__ float to_tf32(float x) {
     uint32_t r;
@@ -308,225 +243,6 @@ __device__ __forceinline__ void produce_chunk(const TcConvParams& p, const PadMa
     }
 }
 
-// Software-pipelined variant for tiles with at most PIPE_P pieces per thread (MT <= 2): the loads
-// of chunk c+1 are issued into registers BEFORE chunk c is transformed, so two chunks of HBM
-// reads are in flight per thread and the load latency hides behind the transform + barrier wait.
-constexpr int PIPE_P = 5;
-struct ChunkRegs { float4 v[PIPE_P]; };
-
-template <int NT>
-__device__ __forceinline__ void load_chunk_regs(const TcConvParams& p, const PadMap& pm, const float* __restrict__ xb,
-                                                int c, int t0, int R, int ptid, ChunkRegs& cr) {
-    const int pc = ptid & 3;
-    const int j = c * kChunk + pc * 4;
-    const int soff = j / p.Cin, ci = j - soff * p.Cin;
-    constexpr int RSTEP = NT / 4;
-    const int row_limit = p.Tout + (p.Kr - 1) * p.dil;
-    const int vrow0 = t0 - p.PLr;
-    const float* __restrict__ xcol = xb + ci;
-#pragma unroll
-    for (int u = 0; u < PIPE_P; ++u) {
-        const int rr = (ptid >> 2) + u * RSTEP;
-        cr.v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        const int vrow = vrow0 + rr;
-        if (rr < R && vrow < row_limit) {
-            const int src = pm.src(vrow * p.vf + soff);
-            if (src >= 0) cr.v[u] = __ldg(reinterpret_cast<const float4*>(xcol + (size_t)src * p.ldx));
-        }
-    }
-}
-
-template <int NT, bool BF16, bool SINGLE = false>
-__device__ __forceinline__ void store_chunk_regs(const TcConvParams& p, int c, int R, int Rpad, uint8_t* ahi, uint8_t* alo,
-                                                 int ptid, const ChunkRegs& cr) {
-    const int pc = ptid & 3;
-    const int j = c * kChunk + pc * 4;
-    const int soff = j / p.Cin, ci = j - soff * p.Cin;
-    const bool has_alpha = p.in_alpha != nullptr;
-    float4 al = make_float4(0.f, 0.f, 0.f, 0.f), ia = al;
-    if (has_alpha) {
-        al = __ldg(reinterpret_cast<const float4*>(p.in_alpha + ci));
-        ia = __ldg(reinterpret_cast<const float4*>(p.in_inv_alpha + ci));
-    }
-    constexpr int RSTEP = NT / 4;
-#pragma unroll
-    for (int u = 0; u < PIPE_P; ++u) {
-        const int rr = (ptid >> 2) + u * RSTEP;
-        if (rr < R) {
-            float4 x4 = cr.v[u];
-            if (has_alpha) x4 = snake4_sel<BF16>(x4, al, ia);
-            if constexpr (SINGLE) store_f16_single(x4, pc, rr, Rpad, ahi);
-            else split_store<BF16>(x4, pc, rr, Rpad, ahi, alo);
-        }
-    }
-}
-
-// ---- interior tiles (conv_tc_kernel) -------------------------------------------------------------
-// A tile whose union of rows lies inside the input (no padding, no tail, vf == 1) needs no index map: thread `ptid` owns
-// 16-byte piece pc = ptid & 3 of rows ptid/4 + u * NT/4, i.e. ONE pointer + u * constant stride, + 16 floats per chunk.
-// The generic path spent more instructions on the map, the bounds and the channel arithmetic than on Snake + split
-// (measured on the fused 192-channel unit: ~1.1 k of a 3.3 k-cycle chunk period in load issue alone).
-template <int NT>
-__device__ __forceinline__ void load_chunk_interior(const float* __restrict__ src /* row ptid/4, piece pc, chunk c */, size_t pstride,
-                                                    int npc, ChunkRegs& cr) {
-#pragma unroll
-    for (int u = 0; u < PIPE_P; ++u)
-        if (u < npc) cr.v[u] = __ldg(reinterpret_cast<const float4*>(src + (size_t)u * pstride));
-}
-template <int NT, bool BF16, bool SINGLE>
-__device__ __forceinline__ void store_chunk_interior(const TcConvParams& p, int c, int npc, int Rpad, uint8_t* ahi, uint8_t* alo,
-                                                     int ptid, const ChunkRegs& cr) {
-    const int pc = ptid & 3;
-    const int ci = c * kChunk + pc * 4;
-    const bool has_alpha = p.in_alpha != nullptr;
-    float4 al = make_float4(0.f, 0.f, 0.f, 0.f), ia = al;
-    if (has_alpha) {
-        al = __ldg(reinterpret_cast<const float4*>(p.in_alpha + ci));
-        ia = __ldg(reinterpret_cast<const float4*>(p.in_inv_alpha + ci));
-    }
-    constexpr int RSTEP = NT / 4;
-#pragma unroll
-    for (int u = 0; u < PIPE_P; ++u) {
-        if (u < npc) {
-            float4 x4 = cr.v[u];
-            if (has_alpha) x4 = snake4_sel<BF16>(x4, al, ia);
-            const int rr = (ptid >> 2) + u * RSTEP;
-            if constexpr (SINGLE) store_f16_single(x4, pc, rr, Rpad, ahi);
-            else split_store<BF16>(x4, pc, rr, Rpad, ahi, alo);
-        }
-    }
-}
-// tiles with more than PIPE_P pieces per thread: BATCH loads in flight, then their transforms
-template <int NT, bool BF16, bool SINGLE, int BATCH = 4>
-__device__ __forceinline__ void produce_chunk_interior(const TcConvParams& p, const float* __restrict__ src, size_t pstride, int c,
-                                                       int R, int Rpad, uint8_t* ahi, uint8_t* alo, int ptid) {
-    const int pc = ptid & 3;
-    const int ci = c * kChunk + pc * 4;
-    const bool has_alpha = p.in_alpha != nullptr;
-    float4 al = make_float4(0.f, 0.f, 0.f, 0.f), ia = al;
-    if (has_alpha) {
-        al = __ldg(reinterpret_cast<const float4*>(p.in_alpha + ci));
-        ia = __ldg(reinterpret_cast<const float4*>(p.in_inv_alpha + ci));
-    }
-    constexpr int RSTEP = NT / 4;
-#pragma unroll 1
-    for (int r = ptid >> 2; r < R; r += RSTEP * BATCH, src += (size_t)BATCH * pstride) {
-        float4 v[BATCH];
-#pragma unroll
-        for (int u = 0; u < BATCH; ++u)
-            if (r + u * RSTEP < R) v[u] = __ldg(reinterpret_cast<const float4*>(src + (size_t)u * pstride));
-#pragma unroll
-        for (int u = 0; u < BATCH; ++u) {
-            const int rr = r + u * RSTEP;
-            if (rr < R) {
-                float4 x4 = v[u];
-                if (has_alpha) x4 = snake4_sel<BF16>(x4, al, ia);
-                if constexpr (SINGLE) store_f16_single(x4, pc, rr, Rpad, ahi);
-                else split_store<BF16>(x4, pc, rr, Rpad, ahi, alo);
-            }
-        }
-    }
-}
-
-// ---- epilogue for 4 consecutive output channels of one row --------------------------------------
-__device__ __forceinline__ void epilogue_store4(const TcConvParams& p, const float* __restrict__ bias, int act, float o0,
-                                                float o1, float o2, float o3, int co, float* __restrict__ yrow,
-                                                bool has_res, float4 rr) {
-    if (bias) {
-        float4 bi = __ldg(reinterpret_cast<const float4*>(bias + co));
-        o0 += bi.x; o1 += bi.y; o2 += bi.z; o3 += bi.w;
-    }
-    if (act == ACT_SNAKE) {
-        float4 al = __ldg(reinterpret_cast<const float4*>(p.out_alpha + co));
-        float4 ia = __ldg(reinterpret_cast<const float4*>(p.out_inv_alpha + co));
-        o0 = snake_fast(o0, al.x, ia.x);
-        o1 = snake_fast(o1, al.y, ia.y);
-        o2 = snake_fast(o2, al.z, ia.z);
-        o3 = snake_fast(o3, al.w, ia.w);
-    } else if (act == ACT_TANH) {
-        o0 = tanhf(o0); o1 = tanhf(o1); o2 = tanhf(o2); o3 = tanhf(o3);
-    } else if (act == ACT_MISH) {
-        o0 = mish_f(o0); o1 = mish_f(o1); o2 = mish_f(o2); o3 = mish_f(o3);
-    }
-    if (has_res) { o0 += rr.x; o1 += rr.y; o2 += rr.z; o3 += rr.w; }
-    *reinterpret_cast<float4*>(yrow + co) = make_float4(o0, o1, o2, o3);
-}
-
-// ---- coalesced epilogue of one warp tile -------------------------------------------------------
-// tcgen05.ld hands every lane one ROW (32 consecutive channels of its time step).  Storing that
-// directly touches 32 different 128-byte lines per instruction (measured: ~3000 cycles per
-// 16-column group, the epilogue was 30-50 % of a CTA).  Instead the warp parks its 32x32 tile in
-// shared memory (row pitch 36 floats: conflict-free 16-byte accesses both ways) and reads it back
-// so that 8 lanes cover 128 contiguous bytes of one row: every global load/store instruction
-// (residual in, result out) then touches 4 full lines instead of 32 partial ones.
-template <bool PREFETCH_RES = true, bool MUFU = false>
-__device__ __forceinline__ void epilogue_tile32(const TcConvParams& p, const float* __restrict__ bias, int act,
-                                                const float (&v)[32], float* stage /* [32][36] per warp */, int lane,
-                                                int t_first /* time step of tile row 0 */, int co0 /* channel of col 0 */,
-                                                float* __restrict__ yb, const float* __restrict__ rb) {
-    const int c4 = lane & 7, rsub = lane >> 3;
-    const int co = co0 + c4 * 4;
-    // residual rows for this lane's 8 (row, 16-byte column chunk) slots: issued first, consumed last
-    float4 rr[PREFETCH_RES ? 8 : 1];
-    if constexpr (PREFETCH_RES) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const int t = t_first + 4 * i + rsub;
-            rr[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (rb && t < p.Tout) rr[i] = *reinterpret_cast<const float4*>(rb + (size_t)t * p.ldy + co);
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float4*>(stage + lane * 36 + j * 4) = make_float4(v[j * 4], v[j * 4 + 1], v[j * 4 + 2], v[j * 4 + 3]);
-    __syncwarp();
-    float4 bi = make_float4(0.f, 0.f, 0.f, 0.f), al = bi, ia = bi;
-    if (bias) bi = __ldg(reinterpret_cast<const float4*>(bias + co));
-    if (act == ACT_SNAKE) {
-        al = __ldg(reinterpret_cast<const float4*>(p.out_alpha + co));
-        ia = __ldg(reinterpret_cast<const float4*>(p.out_inv_alpha + co));
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int row = 4 * i + rsub;
-        const int t = t_first + row;
-        float4 o = *reinterpret_cast<const float4*>(stage + row * 36 + c4 * 4);
-        o.x += bi.x; o.y += bi.y; o.z += bi.z; o.w += bi.w;
-        if (act == ACT_SNAKE) {
-            o = snake4_sel<MUFU>(o, al, ia);
-        } else if (act == ACT_TANH) {
-            o.x = tanhf(o.x); o.y = tanhf(o.y); o.z = tanhf(o.z); o.w = tanhf(o.w);
-        } else if (act == ACT_MISH) {
-            o.x = mish_f(o.x); o.y = mish_f(o.y); o.z = mish_f(o.z); o.w = mish_f(o.w);
-        }
-        if constexpr (PREFETCH_RES) {
-            o.x += rr[i].x; o.y += rr[i].y; o.z += rr[i].z; o.w += rr[i].w;
-        } else if (rb && t < p.Tout) {      // low-register variant (promoted kernel): residual fetched in place
-            float4 r1 = *reinterpret_cast<const float4*>(rb + (size_t)t * p.ldy + co);
-            o.x += r1.x; o.y += r1.y; o.z += r1.z; o.w += r1.w;
-        }
-        if (t < p.Tout) *reinterpret_cast<float4*>(yb + (size_t)t * p.ldy + co) = o;
-    }
-    __syncwarp();
-}
-
-struct Smem {
-    uint64_t b_full[kMaxStagesB];
-    uint64_t b_empty[kMaxStagesB];
-    uint64_t a_full[4];            // operand ring: 2 buffers (8 workers) or 4 (16 workers in two producer groups)
-    uint64_t a_empty[4];
-    uint64_t acc_full;
-    uint64_t acc2_full;
-    uint64_t a2_full[16];          // fused: GEMM-2 operand chunk c2 written (256 worker arrivals)
-    uint32_t tmem_base;
-    uint32_t pad;
-};
-static_assert(sizeof(Smem) <= kSmemHdr, "Smem header");
-
-template <int R>
-__device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int R>
-__device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 }  // namespace tc
 
 }  // namespace fac

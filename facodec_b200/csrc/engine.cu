@@ -40,7 +40,6 @@ struct ConvW {
     bool promoted = false;   // blob built for conv_tcp_kernel (layers upstream of the VQ)
     bool has16 = false; size_t tcw16 = 0;   // 16-bit-operand blob: bf16 hi/lo (non-promoted layers) or fp16 hi / scaled lo (promoted)
     bool has_f16s = false; size_t tcw_f16s = 0;   // hi-only fp16 blob: the one-pass class of the k = 7 convs downstream of the VQ
-    bool has_tt = false; size_t tcw_tt = 0; // transposed-formulation blob (conv_tt_kernel, promoted layers): [co tile of 128][chunk][tap][hi|lo']
 };
 struct SnakeW { size_t a = 0, ia = 0; int C = 0; };
 struct LstmW { ConvW ih[2]; size_t whh[2] = {0, 0}; size_t whh16[2] = {0, 0}; bool has16 = false; int H = 0, U = 0, G = 0;
@@ -93,19 +92,18 @@ struct fac_handle {
     std::vector<HeadSet*> heads;
     char* ws = nullptr; size_t ws_bytes = 0;
     int launches = 0;
-    // tcgen05 3xTF32 path (fac_set_option "tensor_cores"): 0 = never, 1 = layers downstream of the VQ only
+    // tensor-core path (fac_set_option "tensor_cores"): 0 = never, 1 = layers downstream of the VQ only
     // (decoder, timbre branch), 2 = every eligible layer (default; promoted accumulation upstream of the VQ)
     int use_tc = 2;
     int fuse_res = 1;               // fused ResidualUnit launches (fac_set_option "fuse_resunit"); 2 = only where the
                                     // fused tile still allows two CTAs per SM (C <= 128)
     int lstm_v2 = 1;                // fac_set_option "lstm_v2": resident-W fp16 recurrence kernel (lstm2.cu); 0 = round-1 kernel
     int dec_lstm_fp16 = 1;          // fac_set_option "decoder_lstm_fp16": downstream LSTMs run ONE fp16 pass (0 = bf16 hi/lo 3-pass)
-    int enc_mufu = 0;               // fac_set_option "encoder_snake_mufu" (experiment)
     int attn_stream = 0;            // fac_set_option "attention_stream": 1 forces the recomputing attention kernel (test aid)
     int dec_c7_f16 = 1;             // fac_set_option "decoder_conv7_fp16": k = 7 convs downstream of the VQ take ONE fp16 pass (0 = bf16 hi/lo 3-pass)
-    int enc_tt = 1;                 // fac_set_option "encoder_tt": promoted layers run the transposed kernel (conv_tt_kernel)
-    int enc_f16 = 0;                // fac_set_option "encoder_f16x2": promoted layers use the fp16 hi + scaled-lo split
-    int tc_occ2 = 256;              // fac_set_option "tc_occ2_maxn": conv_tc tiles with N <= this are planned for two CTAs per SM (0 = off)
+    int enc_f16 = 1;                // fac_set_option "encoder_f16x2": promoted layers use the fp16 hi + scaled-lo split (0 = 3xTF32)
+    int enc_tt = 0;                 // fac_set_option "encoder_tt": those layers use the transposed formulation (time = wgmma N)
+    int tc_occ2 = 0;                // fac_set_option "tc_occ2_maxn": tiles with N <= this are planned for two CTAs per SM (0 = off)
     bool dec_bf16 = true;           // decoder-side layers use the bf16x3 split (fac_set_option "decoder_bf16")
     // second stream for the waveform-only half of the quantizer (fac_set_option "overlap_front")
     int overlap_front = 1; cudaStream_t side = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -203,7 +201,7 @@ std::vector<float> folded_weight(fac_handle* h, int m, const std::string& prefix
     return w;
 }
 
-// Builds the tcgen05 weight blob for a packed conv (stride-1 in rows; `stride` > 1 means the
+// Builds the tensor-core weight blob for a packed conv (stride-1 in rows; `stride` > 1 means the
 // kernel-2*stride down-conv viewed as a 2-tap conv over rows of `stride` samples).
 void attach_tc(fac_handle* h, ConvW& c, int stride, bool promoted) {
     TcConvParams tp;
@@ -218,15 +216,9 @@ void attach_tc(fac_handle* h, ConvW& c, int stride, bool promoted) {
     tc_pack_blob(tp, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw);
     c.tc = true;
     if (promoted) {
-        TcConvParams tt = tp;
-        if (tt_conv_plan(tt)) {
-            c.tcw_tt = pack_alloc(h, tt_blob_floats(tt));
-            tt_pack_blob(tt, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw_tt);
-            c.has_tt = true;
-        }
         TcConvParams t16 = tp;
         t16.f16x2 = 1;
-        if (tc_conv_plan(t16) && t16.N == tp.N) {
+        if (tc_conv_plan(t16)) {
             c.tcw16 = pack_alloc(h, tc_blob_floats(t16));
             tc_pack_blob(t16, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw16);
             c.has16 = true;
@@ -234,7 +226,7 @@ void attach_tc(fac_handle* h, ConvW& c, int stride, bool promoted) {
     } else {
         TcConvParams t16 = tp;
         t16.bf16 = 1;
-        if (tc_conv_plan(t16) && t16.N == tp.N) {
+        if (tc_conv_plan(t16)) {
             c.tcw16 = pack_alloc(h, tc_blob_floats(t16));
             tc_pack_blob(t16, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw16);
             c.has16 = true;
@@ -248,7 +240,7 @@ void attach_f16_single(fac_handle* h, ConvW& c) {
     if (!c.tc || c.promoted || !c.has16 || c.vf != 1) return;
     TcConvParams t1;
     t1.Cin = c.Cin; t1.Cout = c.Cout; t1.dil = 1; t1.vf = 1; t1.Kr = c.K; t1.bf16 = 1; t1.g1f16 = 1;
-    if (!tc_conv_plan(t1) || t1.N != c.tcN) return;
+    if (!tc_conv_plan(t1)) return;
     c.tcw_f16s = pack_alloc(h, tc_blob_floats(t1));
     tc_pack_blob(t1, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw_f16s);
     c.has_f16s = true;
@@ -687,10 +679,13 @@ void run_conv(Ctx& c, const ConvW& w, const float* x, float* y, int B, int Tin, 
         tp.f16x2 = (tp.promoted && c.h->enc_f16 && w.has16) ? 1 : 0;
         tp.occ2_maxn = c.h->tc_occ2;
         tp.Tout = Tout;
-        const bool use_tt = tp.promoted && c.h->enc_tt && w.has_tt;
-        tp.snake_mufu = c.h->enc_mufu;
-        if (use_tt ? tt_conv_plan(tp) : tc_conv_plan(tp)) {
-            tp.x = x; tp.y = y; tp.wblob = c.W(use_tt ? w.tcw_tt : (tp.g1f16 ? w.tcw_f16s : ((tp.bf16 || tp.f16x2) ? w.tcw16 : w.tcw))); tp.bias = c.W(w.b);
+        if (tp.f16x2 && c.h->enc_tt) {
+            TcConvParams t2 = tp;
+            t2.tt = 1;
+            if (tc_conv_plan(t2)) tp = t2;
+        }
+        if (tc_conv_plan(tp)) {
+            tp.x = x; tp.y = y; tp.wblob = c.W(tp.g1f16 ? w.tcw_f16s : ((tp.bf16 || tp.f16x2) ? w.tcw16 : w.tcw)); tp.bias = c.W(w.b);
             if (o.in_snake) { tp.in_alpha = c.W(o.in_snake->a); tp.in_inv_alpha = c.W(o.in_snake->ia); }
             tp.out_act = o.act;
             if (o.out_snake) { tp.out_act = ACT_SNAKE; tp.out_alpha = c.W(o.out_snake->a); tp.out_inv_alpha = c.W(o.out_snake->ia); }
@@ -704,9 +699,9 @@ void run_conv(Ctx& c, const ConvW& w, const float* x, float* y, int B, int Tin, 
             double bytes = 4.0 * ((double)B * Tin * w.Cin + (double)B * Tout * w.Cout * (o.res ? 2 : 1) + (double)w.K * w.Cin * w.Cout);
             char det[96];
             snprintf(det, sizeof det, "%s Cin%d Cout%d K%d d%d T%d", name, w.Cin, w.Cout, w.K, o.dil, Tout);
-            c.begin(use_tt ? "conv_tt" : (tp.promoted ? "conv_tcp" : "conv_tc"), flops, bytes, det);
+            c.begin(tp.promoted ? "conv_tcp" : "conv_tc", flops, bytes, det);
             (void)short_chain;
-            c.check(use_tt ? launch_conv_tt(tp, c.st) : launch_conv_tc(tp, c.st), name);
+            c.check(launch_conv_tc(tp, c.st), name);
             c.end();
             return;
         }
@@ -751,7 +746,7 @@ int sconv(Ctx& c, const ConvW& w, const float* x, float* y, int B, int T, int di
     return Tout;
 }
 
-// Whole ResidualUnit in one tcgen05 launch (conv_tc_kernel<true>) when every channel fits one CTA tile.
+// Whole ResidualUnit in one tensor-core launch (conv_tc_kernel<true>) when every channel fits one CTA tile.
 bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B, int T, bool causal) {
     if (c.h->use_tc < 1 || !c.h->fuse_res || c.vq_critical || !r.c7.tc || !r.c1.tc || r.c7.promoted || r.c1.promoted ||
         r.c7.Cin != r.c7.Cout || r.c1.K != 1 || r.c7.vf != 1)
@@ -764,6 +759,10 @@ bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B,
     tp.Tout = T;
     if (c.h->fuse_res == 2 && r.c7.Cout > 128) return false;
     if (!tc_conv_plan(tp)) return false;
+    // the unit's weight blobs were laid out by the unfused plans of the same split classes: their tile must be N = C too
+    TcConvParams q7 = tp, q1 = tp;
+    q7.fused = 0; q1.fused = 0; q1.Kr = 1; q1.g1f16 = 0;
+    if (!tc_conv_plan(q7) || !tc_conv_plan(q1) || q7.N != tp.N || q1.N != tp.N) return false;
     if (c.dry) return true;
     const int k_eff = (r.c7.K - 1) * r.dil + 1;
     tp.x = x; tp.y = y; tp.res = x;
@@ -1002,7 +1001,7 @@ float* mel_forward(Ctx& c, const float* wave, int B, int T, int Tm, const MelW* 
     MelW q;
     if (mw) q = *mw; else { q.dft = &c.h->qw.dft; q.dft_tc = &c.h->qw.dft_tc; q.fb = c.h->qw.fb; }
     if (c.h->use_tc >= 2 && q.dft_tc->tc) {
-        // frames gather + K=1 GEMM on the promoted tcgen05 kernel (the mel feeds the prosody VQ: fp32-grade sums)
+        // frames gather + K=1 GEMM on the promoted tensor-core kernel (the mel feeds the prosody VQ: fp32-grade sums)
         float* frames = c.alloc<float>((size_t)B * Tm * WIN);
         float* spec = c.alloc<float>((size_t)B * Tm * SPEC_TC_LD);
         float* mel = c.alloc<float>((size_t)B * Tm * N_MELS);
@@ -2238,20 +2237,13 @@ int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, i
 int fac_set_option(fac_handle* h, const char* name, int value) {
     if (!h || !name) return FAC_ERR_INVALID;
     if (std::string(name) == "fuse_resunit") { h->fuse_res = value < 0 ? 0 : (value > 2 ? 2 : value); return FAC_OK; }
-    if (std::string(name) == "tc_dbg") { g_tc_dbg = value; return FAC_OK; }
-    if (std::string(name) == "tc_slot_issue") { g_tc_slot_issue = value != 0; return FAC_OK; }
-    if (std::string(name) == "tt_pair") { g_tt_pair_ok = value != 0; return FAC_OK; }
-    if (std::string(name) == "tc_groups") { g_tc_groups_ok = value != 0; return FAC_OK; }
-    if (std::string(name) == "tc_wide") { g_tc_wide_ok = value != 0; return FAC_OK; }
-    if (std::string(name) == "tc_occ2_maxn") { h->tc_occ2 = value < 0 ? 0 : value; return FAC_OK; }
     if (std::string(name) == "encoder_f16x2") { h->enc_f16 = value != 0; return FAC_OK; }
-    if (std::string(name) == "decoder_conv7_fp16") { h->dec_c7_f16 = value != 0; return FAC_OK; }
     if (std::string(name) == "encoder_tt") { h->enc_tt = value != 0; return FAC_OK; }
-    if (std::string(name) == "encoder_snake_mufu") { h->enc_mufu = value != 0; return FAC_OK; }
+    if (std::string(name) == "tc_occ2_maxn") { h->tc_occ2 = value < 0 ? 0 : value; return FAC_OK; }
+    if (std::string(name) == "decoder_conv7_fp16") { h->dec_c7_f16 = value != 0; return FAC_OK; }
     if (std::string(name) == "overlap_front") { h->overlap_front = value != 0; return FAC_OK; }
     if (std::string(name) == "lstm_v2") { h->lstm_v2 = value != 0; return FAC_OK; }
     if (std::string(name) == "decoder_lstm_fp16") { h->dec_lstm_fp16 = value != 0; return FAC_OK; }
-    if (std::string(name) == "tt_probe") { g_tt_probe_on = value != 0; return FAC_OK; }
     if (std::string(name) == "attention_stream") { h->attn_stream = value != 0; return FAC_OK; }
     if (std::string(name) == "decoder_bf16") { h->dec_bf16 = value != 0; return FAC_OK; }
     if (std::string(name) == "tensor_cores") { h->use_tc = value < 0 ? 0 : (value > 2 ? 2 : value); return FAC_OK; }
@@ -2267,27 +2259,27 @@ int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const 
     cudaSetDevice(h->device);
     cudaStream_t st = (cudaStream_t)stream;
     TcConvParams tp;
-    tp.Cin = Cin; tp.Cout = Cout; tp.promoted = (promoted == 1 || promoted == 3) ? 1 : 0; tp.bf16 = (promoted == 2 || promoted == 5) ? 1 : 0;
-    tp.f16x2 = promoted == 3 ? 1 : 0;
+    tp.Cin = Cin; tp.Cout = Cout; tp.promoted = (promoted == 1 || promoted == 3 || promoted == 4) ? 1 : 0;
+    tp.bf16 = (promoted == 2 || promoted == 5) ? 1 : 0;
+    tp.f16x2 = (promoted == 3 || promoted == 4) ? 1 : 0;
+    tp.tt = promoted == 4 ? 1 : 0;         // 4 = the transposed formulation of class 3
     tp.g1f16 = promoted == 5 ? 1 : 0;      // 5 = the one-pass fp16 class of conv_tc_kernel
-    const bool use_tt = promoted == 4;
     tp.occ2_maxn = h->tc_occ2;
     tp.Tout = Tout;
     if (stride == 1) { tp.vf = 1; tp.Kr = K; tp.dil = dil; }
     else if (K == 2 * stride && dil == 1) { tp.vf = stride; tp.Kr = 2; tp.dil = 1; }
     else { h->err = "fac_debug_conv_tc: unsupported stride/kernel"; return FAC_ERR_UNSUPPORTED; }
-    if (!(use_tt ? tt_conv_plan(tp) : tc_conv_plan(tp))) { h->err = "fac_debug_conv_tc: layer not eligible for the tensor-core path"; return FAC_ERR_UNSUPPORTED; }
+    if (promoted < 0 || promoted > 5 || !tc_conv_plan(tp)) { h->err = "fac_debug_conv_tc: layer not eligible for the tensor-core path"; return FAC_ERR_UNSUPPORTED; }
     int ldw = (Cout + 3) / 4 * 4;
     std::vector<float> gen((size_t)K * Cin * ldw, 0.f);
     for (int co = 0; co < Cout; ++co)
         for (int ci = 0; ci < Cin; ++ci)
             for (int k = 0; k < K; ++k) gen[((size_t)k * Cin + ci) * ldw + co] = w_host[((size_t)co * Cin + ci) * K + k];
-    size_t nb = use_tt ? tt_blob_floats(tp) : tc_blob_floats(tp);
+    size_t nb = tc_blob_floats(tp);
     auto al4 = [](size_t v) { return (v + 3) / 4 * 4; };
     size_t o_b = al4(nb), o_ia = al4(o_b + Cout), o_iia = al4(o_ia + Cin), o_oa = al4(o_iia + Cin), o_oia = al4(o_oa + Cout);
     std::vector<float> pk(o_oia + Cout + 16, 0.f);
-    if (use_tt) tt_pack_blob(tp, gen.data(), ldw, pk.data());
-    else tc_pack_blob(tp, gen.data(), ldw, pk.data());
+    tc_pack_blob(tp, gen.data(), ldw, pk.data());
     for (int i = 0; i < Cout; ++i) pk[o_b + i] = bias_host ? bias_host[i] : 0.f;
     for (int i = 0; i < Cin; ++i) { pk[o_ia + i] = in_alpha_host ? in_alpha_host[i] : 1.f; pk[o_iia + i] = 1.0f / (pk[o_ia + i] + 1e-9f); }
     for (int i = 0; i < Cout; ++i) { pk[o_oa + i] = out_alpha_host ? out_alpha_host[i] : 1.f; pk[o_oia + i] = 1.0f / (pk[o_oa + i] + 1e-9f); }
@@ -2305,7 +2297,7 @@ int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const 
     tp.pad_left_s = pad_left; tp.pad_right_s = pad_right; tp.reflect = reflect;
     tp.Tout = Tout; tp.ldy = Cout;
     tp.x_bstride = (size_t)Tin * Cin; tp.y_bstride = (size_t)Tout * Cout;
-    e = use_tt ? launch_conv_tt(tp, st) : launch_conv_tc(tp, st);
+    e = launch_conv_tc(tp, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     cudaFree(d);
     if (e != cudaSuccess) { h->err = std::string("fac_debug_conv_tc: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
@@ -2318,7 +2310,7 @@ int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const
     if (!h || !x || !y || !w7_host || !w1_host) return FAC_ERR_INVALID;
     fac_handle tmp;
     tmp.device = h->device;
-    tmp.use_tc = mode == 0 ? 0 : 1;          // 0: fp32 FMA, 1: two tcgen05 launches, 2: fused launch; 3/4 = 1/2 with bf16 split;
+    tmp.use_tc = mode == 0 ? 0 : 1;          // 0: fp32 FMA, 1: two tensor-core launches, 2: fused launch; 3/4 = 1/2 with bf16 split;
                                              // 5/6 = 3/4 with the k = 7 conv in one fp16 pass
     tmp.fuse_res = (mode == 2 || mode == 4 || mode == 6) ? 1 : 0;
     tmp.dec_bf16 = mode >= 3;
@@ -2427,7 +2419,7 @@ int fac_debug_pad_map(int L, int pad_left, int pad_right, int reflect, int* out,
     return FAC_OK;
 }
 
-// Host-only: the tile plan the tcgen05 conv kernels would use for a layer geometry (no GPU, no handle).
+// Host-only: the tile plan the tensor-core conv kernel would use for a layer geometry (no GPU, no handle).
 int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* out8) {
     if (!out8 || Cin <= 0 || Cout <= 0 || K <= 0 || dil <= 0 || stride <= 0 || mode < 0 || mode > 6) return FAC_ERR_INVALID;
     TcConvParams tp;
@@ -2436,19 +2428,12 @@ int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, i
     tp.bf16 = (mode == 2 || mode == 4) ? 1 : 0;
     tp.f16x2 = mode == 3 ? 1 : 0;
     tp.fused = (mode == 4 || mode == 5) ? 1 : 0;
+    if (mode == 6) { tp.promoted = 1; tp.f16x2 = 1; tp.tt = 1; }     // 6: transposed formulation of mode 3
     if (stride == 1) { tp.vf = 1; tp.Kr = K; tp.dil = dil; }
     else if (K == 2 * stride && dil == 1) { tp.vf = stride; tp.Kr = 2; tp.dil = 1; }
     else return FAC_ERR_UNSUPPORTED;
-    if (mode == 6) {
-        tp.promoted = 0; tp.bf16 = 0; tp.f16x2 = 0; tp.fused = 0;
-        if (!tt_conv_plan(tp)) return FAC_ERR_UNSUPPORTED;
-        out8[0] = tp.N * (tp.pair ? 2 : 1);   // output channels per CTA tile: 128, or 256 in PAIR mode (two weight tiles)
-        out8[1] = tp.NT; out8[2] = tp.nchunk; out8[3] = tp.stagesB; out8[4] = tp.tmem_cols;
-        out8[5] = (int)tp.smem_bytes; out8[6] = tp.Rpad; out8[7] = tp.promote_every;
-        return FAC_OK;
-    }
     if (!tc_conv_plan(tp)) return FAC_ERR_UNSUPPORTED;
-    out8[0] = tp.N; out8[1] = tp.MT; out8[2] = tp.nchunk; out8[3] = tp.stagesB; out8[4] = tp.tmem_cols;
+    out8[0] = tp.N; out8[1] = tp.MT; out8[2] = tp.nchunk; out8[3] = tp.stagesB; out8[4] = 64 * tp.MT;
     out8[5] = (int)tp.smem_bytes; out8[6] = tp.Rpad; out8[7] = tp.promote_every;
     return FAC_OK;
 }
@@ -2457,54 +2442,41 @@ int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, i
 // floats (32-bit words) of the blob, writes it when blob_out has room.
 long long fac_debug_tc_pack(const float* w_host, int Cin, int Cout, int K, int stride, int mode, float* blob_out,
                             long long capacity_floats) {
-    if (!w_host || Cin <= 0 || Cout <= 0 || K <= 0 || stride <= 0 || mode < 0 || mode > 4) return FAC_ERR_INVALID;
+    if (!w_host || Cin <= 0 || Cout <= 0 || K <= 0 || stride <= 0 || mode < 0 || mode > 3) return FAC_ERR_INVALID;
     TcConvParams tp;
     tp.Cin = Cin; tp.Cout = Cout; tp.dil = 1;
     tp.promoted = (mode == 1 || mode == 3) ? 1 : 0; tp.bf16 = mode == 2 ? 1 : 0; tp.f16x2 = mode == 3 ? 1 : 0;
     if (stride == 1) { tp.vf = 1; tp.Kr = K; }
     else if (K == 2 * stride) { tp.vf = stride; tp.Kr = 2; }
     else return FAC_ERR_UNSUPPORTED;
-    const bool use_tt = mode == 4;
-    if (use_tt) { tp.promoted = 0; tp.bf16 = 0; tp.f16x2 = 0; }
-    if (!(use_tt ? tt_conv_plan(tp) : tc_conv_plan(tp))) return FAC_ERR_UNSUPPORTED;
-    const long long n = (long long)(use_tt ? tt_blob_floats(tp) : tc_blob_floats(tp));
+    if (!tc_conv_plan(tp)) return FAC_ERR_UNSUPPORTED;
+    const long long n = (long long)tc_blob_floats(tp);
     if (!blob_out || capacity_floats < n) return n;
     const int ldw = (Cout + 3) / 4 * 4;
     std::vector<float> gen((size_t)K * Cin * ldw, 0.f);      // generic packed layout [K*Cin][ldw]
     for (int co = 0; co < Cout; ++co)
         for (int ci = 0; ci < Cin; ++ci)
             for (int k = 0; k < K; ++k) gen[((size_t)k * Cin + ci) * ldw + co] = w_host[((size_t)co * Cin + ci) * K + k];
-    if (use_tt) tt_pack_blob(tp, gen.data(), ldw, blob_out);
-    else tc_pack_blob(tp, gen.data(), ldw, blob_out);
+    tc_pack_blob(tp, gen.data(), ldw, blob_out);
     return n;
 }
 
 int fac_debug_tc_phase_clocks(fac_handle* h, long long* out8) {
     if (!h || !out8) return FAC_ERR_INVALID;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    cudaError_t e = g_tt_probe_on ? tt_read_probe(out8) : tc_read_phase_clocks(out8);
-
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return FAC_ERR_CUDA; }
-    return FAC_OK;
+    h->err = "fac_debug_tc_phase_clocks: the tensor-core conv kernel records no timing probes";
+    return FAC_ERR_UNSUPPORTED;
 }
 
 int fac_debug_tc_trace(fac_handle* h, long long* out80) {
     if (!h || !out80) return FAC_ERR_INVALID;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    cudaError_t e = tc_read_trace(out80);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return FAC_ERR_CUDA; }
-    return FAC_OK;
+    h->err = "fac_debug_tc_trace: the tensor-core conv kernel records no timing probes";
+    return FAC_ERR_UNSUPPORTED;
 }
 
 int fac_debug_tc_producer_clocks(fac_handle* h, long long* out4) {
     if (!h || !out4) return FAC_ERR_INVALID;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    cudaError_t e = tc_read_producer_clocks(out4);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return FAC_ERR_CUDA; }
-    return FAC_OK;
+    h->err = "fac_debug_tc_producer_clocks: the tensor-core conv kernel records no timing probes";
+    return FAC_ERR_UNSUPPORTED;
 }
 
 int fac_debug_lstm_phase_clocks(fac_handle* h, long long* out4) {

@@ -45,7 +45,7 @@ __global__ void __launch_bounds__(128) mel_from_spec_kernel(const float* __restr
 }
 
 // Frame gather for the tensor-core DFT: frames[b][f][j] = wave[b][reflect(f*hop - pad + j)], j < win.  The hop (300) is
-// not a multiple of the 16-channel chunk of the tcgen05 conv, so the strided "conv" view of the STFT cannot feed it
+// not a multiple of the 16-channel chunk of the tensor-core conv, so the strided "conv" view of the STFT cannot feed it
 // directly; the explicit [B*F][1200] matrix (49 MB at B=32) can, as a plain K=1 GEMM against the folded basis.
 __global__ void __launch_bounds__(256) stft_frames_kernel(const float* __restrict__ wave, float* __restrict__ frames, int T,
                                                           int F, int hop, int win, int pad) {

@@ -25,10 +25,10 @@ struct ConvParams {
 };
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t st);
 
-// ---- tcgen05 tensor-core conv (conv_tc.cu) ---------------------------------------------------
+// ---- wgmma tensor-core conv (conv_tc.cu) -----------------------------------------------------
 struct TcConvParams {
     const float* x = nullptr;          // [B][Tin][ldx] channels-last samples
-    const float* wblob = nullptr;      // [ntile][chunk][tap][hi|lo][4][N][4] (tc_pack_blob)
+    const float* wblob = nullptr;      // [ntile][chunk][tap][hi|lo][k-piece][N][16 B] (tc_pack_blob)
     const float* bias = nullptr;
     const float* in_alpha = nullptr;   // [Cin] Snake on the input or null
     const float* in_inv_alpha = nullptr;
@@ -42,33 +42,24 @@ struct TcConvParams {
     int pad_left_s = 0, pad_right_s = 0, reflect = 0;   // sample-level padding (PadMap)
     int Tout = 0, Cout = 0, ldy = 0;
     int out_act = 0;
-    int promoted = 0;                  // 1 = conv_tcp_kernel (register-promoted accumulation)
-    int bf16 = 0;                      // 1 = bf16 hi/lo split (kind::f16, K = 16) instead of tf32 hi/lo; decoder only
+    int promoted = 0;                  // 1 = register-promoted accumulation (layers upstream of the VQ)
+    int bf16 = 0;                      // 1 = bf16 hi/lo split (K = 16 MMAs) instead of tf32 hi/lo; downstream of the VQ only
     int g1f16 = 0;                     // with bf16 = 1 (downstream only): the layer's own GEMM (the k-tap conv; GEMM 1 of a fused unit) takes
                                        // ONE fp16 pass (10-bit operands, fp32 accumulation) instead of the 3-pass bf16 hi/lo split
-    int f16x2 = 0;                     // promoted only: fp16 hi + 2^11-scaled fp16 lo split (kind::f16, K = 16) instead of tf32 hi/lo
-    int tt = 0;                        // 1 = conv_tt_kernel: transposed formulation (weights = MMA A operand, M = 128 output
-                                       // channels; time = N = NT <= 256), fp16 hi + scaled-lo split, promoted (tt_conv_plan)
-    int pair = 0;                      // tt (plan): 1 = PAIR mode, a CTA tile is two 128-channel weight tiles x NT <= 128 time steps
-    int NT = 0;                        // tt: time steps per tile
-    int snake_mufu = 0;                // tt, EXPERIMENT: Snake via the SFU sine (abs error ~4e-7 instead of 2.5e-7)
+    int f16x2 = 0;                     // promoted only: fp16 hi + 2^11-scaled fp16 lo split (K = 16 MMAs) instead of tf32 hi/lo
     int fused = 0;                     // 1 = whole ResidualUnit: conv7 -> +b7 -> Snake -> 1x1 conv -> +b1 -> +x
+    int tt = 0;                        // f16x2 only: transposed formulation (weights = wgmma A operand, time = wgmma N)
+    int occ2_maxn = 0;                 // > 0: tiles with N <= occ2_maxn are planned for two resident CTAs per SM
     const float* wblob2 = nullptr;     // 1x1 conv weight blob (same tile N), when fused
     const float* bias2 = nullptr;
     int nchunk2 = 0;
-    int occ2_maxn = 0;                 // > 0: tiles with N <= occ2_maxn are planned for TWO resident CTAs per SM
-                                       // (<= 256 TMEM columns, <= 112 KB smem each) so one CTA's MMAs overlap the other's
-                                       // produce / epilogue phases
     // plan (tc_conv_plan)
-    int promote_every = 1;
-    int N = 0, MT = 0, nchunk = 0, Rpad = 0, stagesB = 0, tmem_cols = 0;
-    int cps = 0;                       // conv_tc_kernel: > 0 = a weight-ring slot holds every tap of `cps` consecutive chunks (tpt = Kr * cps)
-    int tpt = 1, tpt2 = 1;             // conv_tc_kernel: weight tiles ((chunk, tap) / GEMM-2 chunk) per bulk copy into one ring slot
+    int promote_every = 1;             // promoted: chunks per accumulation window
+    int N = 0, nchunk = 0, Rpad = 0, stagesB = 0;
+    int MT = 2;                        // 2: tile = 128 rows x N (warpgroups split rows); 1: 64 rows x N (they split channels)
     int b_slot = 0;                    // bytes of one weight-ring slot
-    int R2pad = 0;                     // fused: row pitch (rows) of the resident GEMM-2 operand chunks
-    int dbg = 0;                       // conv_tc_kernel timing experiments (g_tc_dbg); results are wrong when non-zero
-    int ng = 1;                        // conv_tc_kernel: producer groups (2 = alternate chunks over a 4-deep operand ring)
-    int wide = 0;                      // conv_tc_kernel: 1 = 16 worker warps (tile planned for one CTA per SM), 0 = 8
+    int occ2 = 0;                      // planned for two resident CTAs per SM
+    int R2pad = 0;                     // fused: row pitch (rows) of the resident GEMM-2 operand
     size_t smem_bytes = 0;
     size_t x_bstride = 0, y_bstride = 0;
 };
@@ -76,20 +67,6 @@ bool tc_conv_plan(TcConvParams& p);
 size_t tc_blob_floats(const TcConvParams& p);
 void tc_pack_blob(const TcConvParams& p, const float* wp, int ldw, float* blob);
 cudaError_t launch_conv_tc(const TcConvParams& p, cudaStream_t st);
-bool tt_conv_plan(TcConvParams& p);                 // conv_tt.cu
-size_t tt_blob_floats(const TcConvParams& p);
-void tt_pack_blob(const TcConvParams& p, const float* wp, int ldw, float* blob);
-cudaError_t launch_conv_tt(const TcConvParams& p, cudaStream_t st);
-extern int g_tc_dbg;
-extern int g_tc_slot_issue;
-extern int g_tc_groups_ok;
-extern int g_tc_wide_ok;                             // conv_tc.cu: 0 = never plan 16-worker tiles (A/B aid)
-extern int g_tt_pair_ok;                             // conv_tt.cu: 0 = never plan PAIR-mode tiles
-extern int g_tt_probe_on;                            // 1 = launch the probing variant (process-wide test aid)
-cudaError_t tt_read_probe(long long* out8);
-cudaError_t tc_read_trace(long long* out80);          // per-chunk timeline of the probe CTA (conv_tc.cu g_tc_trace)
-cudaError_t tc_read_producer_clocks(long long* out4); // probe producer thread of the last conv_tc_kernel
-cudaError_t tc_read_phase_clocks(long long* out8);   // probe-CTA phase timestamps of the last conv_tc_kernel
 
 // ---- LSTM recurrence (lstm.cu) -----------------------------------------------------------
 // One nn.LSTM layer over all T steps for up to 32 sequences (dac/model/encodec.py:272-288).

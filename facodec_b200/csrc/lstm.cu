@@ -11,7 +11,7 @@
 // linear) and of h_{t-1} through private multi-stage cp.async rings, and feed them to the tensor
 // cores as mma.sync m16n8k8 TF32 tiles with the same fp32-faithful 3xTF32 split as the convs
 // (hi/lo formed in registers; 48-72 chained MMAs per accumulator, then an fp32 cross-warp sum).
-// A 32 x 4U x H product per step is far too small for a tcgen05/TMEM tile pipeline.  Measured per
+// A 32 x 4U x H product per step is far too small for a wgmma tile pipeline.  Measured per
 // step (clock64 probe, fac_debug_lstm_phase_clocks): barrier wait ~2.0k cycles, K loop 12k (H=1024) /
 // 23.5k (H=1536), reduce+gates 1.4-2.6k, publish 1.4k.  The K loop is bound by the legacy HMMA.1688
 // TF32 rate of this chip (~1 per 32 cycles per SM sub-partition == the fp32 FMA rate: the earlier FMA

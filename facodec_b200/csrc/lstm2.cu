@@ -18,9 +18,8 @@
 //     W_hh and h of the decoder's LSTM to fp16 moves the reconstructed waveform by 1.9e-7 RMS (bar 1e-4; bf16 hi+lo kept
 //     as "decoder_lstm_fp16" = 0).
 //
-// Why not tcgen05 here (VERDICT r1 item 3): scripts/mma_probe.cu measured a fixed >= 110 cycles per tcgen05.mma in one issue
-// stream whatever its size (N = 32: 122 cycles, profiles/r02/mma_probe_r02.log).  A step needs H/16 k-steps x passes =
-// 96-192 dependent-issue MMAs per CTA whatever M is, i.e. >= 10-21 k cycles per step against ~5 k for this mma.sync loop.
+// A step needs H/16 k-steps x passes = 96-192 dependent MMAs per CTA on a 32-row tile: warp-level mma.sync keeps that
+// latency chain short; an asynchronous warpgroup MMA pipeline only pays off on tiles far larger than one step.
 #include <cooperative_groups.h>
 #include <cuda_fp16.h>
 

@@ -1,4 +1,4 @@
-"""Training-side losses of the reference, forward values only, on the B200 front-end kernels: ``reconstruction_loss``
+"""Training-side losses of the reference, forward values only, on the front-end kernels: ``reconstruction_loss``
 (losses.py:65-89) and the ``dac/nn/loss.py`` criteria train.py:153-164 builds (``MultiScaleSTFTLoss``, ``MelSpectrogramLoss``,
 ``L1Loss``; their audiotools / librosa arithmetic is restated from the published semantics -- parity unpinned, see the classes).
 

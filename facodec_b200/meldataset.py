@@ -1,4 +1,4 @@
-"""Dataset-side mel of the reference's training input pipeline (meldataset.py:29-71), computed by the B200 front-end
+"""Dataset-side mel of the reference's training input pipeline (meldataset.py:29-71), computed by the front-end
 kernels (frame gather + tensor-core DFT + mel filterbank) through ``fac_dataset_mel``.
 
 ``preprocess(wave)`` mirrors meldataset.py:42-47: torchaudio ``MelSpectrogram(n_mels=80, n_fft=2048, win_length=1200,

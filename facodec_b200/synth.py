@@ -4,7 +4,7 @@ trained checkpoint; SURVEY.md section 8c/8d).
 ``synth_state_dicts(seed)`` returns ``{'encoder': sd, 'quantizer': sd, 'decoder': sd}``
 with exactly the key names / shapes / dtypes of the reference checkpoints
 (``reconstruct.py:30-34`` loads ``ckpt[key]`` per module; keys listed in
-``docs`` of DESIGN.md).  Values are drawn from ``numpy.random.RandomState`` so
+the reference state_dicts).  Values are drawn from ``numpy.random.RandomState`` so
 that the same seed gives bit-identical tensors on any machine, following the
 default PyTorch initialisers of each layer family so activations have
 reference-like statistics:

@@ -177,24 +177,25 @@ int fac_head_finalize(fac_handle* h, int head_id, int indim, int outdim, int nhe
 int fac_head_forward(fac_handle* h, int head_id, const float* x, int B, int T, float* const* outs, void* stream);
 int fac_add3(fac_handle* h, const float* a, const float* b, const float* c, long long n, float* out, void* stream);
 
-/* Engine options.  "tensor_cores": 0 = fp32 FMA kernels everywhere; 1 = tcgen05 3xTF32
+/* Engine options.  "tensor_cores": 0 = fp32 FMA kernels everywhere; 1 = wgmma split-operand
  * kernel for every eligible layer downstream of the VQ (decoder, timbre branch), fp32 FMA upstream
- * (encoder, prosody branch); 2 (default) = tcgen05 everywhere, with the register-promoted accumulation
+ * (encoder, prosody branch); 2 (default) = wgmma everywhere, with the register-promoted accumulation
  * variant upstream of the VQ where the bit-exact argmin needs fp32-grade sums.
  * "fuse_resunit": 1 (default) runs each decoder ResidualUnit whose channels fit one CTA tile as a single
- * fused launch (conv7 -> Snake -> 1x1 conv -> +x with the intermediate kept in TMEM/SMEM); 0 = two launches;
- * 2 = fuse only units of at most 128 channels (the ones whose fused tile still allows two CTAs per SM).
+ * fused launch (conv7 -> Snake -> 1x1 conv -> +x with the intermediate kept in shared memory); 0 = two launches;
+ * 2 = fuse only units of at most 128 channels.
  * "decoder_bf16": 1 (default) = layers downstream of the VQ split operands into bf16 hi + bf16 lo
- * (tcgen05.mma.kind::f16, K = 16: half the MMAs and half the operand bytes of the TF32 split; waveform error
- * ~1e-5 RMS against the 1e-4 bar), evaluate Snake with the SFU sine and run the LSTM recurrence on bf16 hi/lo
+ * (K = 16 MMAs: half the MMAs and half the operand bytes of the TF32 split; waveform error
+ * ~1e-5 RMS against the 1e-4 bar, measured on the oracle), evaluate Snake with the SFU sine and run the LSTM recurrence on bf16 hi/lo
  * mma.sync tiles; 0 = TF32 hi/lo everywhere.  Never applied upstream of the VQ.
- * "encoder_f16x2": 0 (default) / 1 = EXPERIMENTAL: layers upstream of the VQ split operands into fp16 hi + fp16 lo
- * scaled by 2^11 (kind::f16, K = 16, cross terms in their own TMEM accumulator, scaled back at promotion) instead of
- * the TF32 pair: same 22 mantissa bits and bit-exact codes on every fixture, but operands must stay below fp16's
- * 65504, and the measured gain is only 5-11 % on the k=7 encoder convs (one MMA stream per SM runs kind::f16 at
- * about half rate for N <= 128), so it is off by default.
- * "tc_occ2_maxn": channel tiles of at most this width (default 256; 0 = off) are planned for TWO resident CTAs per
- * SM (<= 256 TMEM columns, <= 112 KB shared memory each) so one CTA's MMAs overlap the other's produce/epilogue. */
+ * "encoder_f16x2": 1 (default) = layers upstream of the VQ split operands into fp16 hi + fp16 lo scaled by 2^11
+ * (K = 16 MMAs at twice the TF32 rate, cross terms in their own accumulator, scaled back at promotion): the same
+ * 22 mantissa bits as the TF32 pair, but operands must stay below fp16's 65504; 0 = TF32 hi/lo pairs.
+ * "encoder_tt": 0 (default) / 1 = those layers in the transposed formulation (weights as the wgmma A operand, time as
+ * wgmma N); same arithmetic, another tiling.
+ * "tc_occ2_maxn": tiles of at most this many channels with plain accumulation are planned for TWO resident CTAs per SM
+ * (<= 113 KB shared memory, <= 128 registers per thread) so one CTA's MMAs overlap the other's operand production and
+ * epilogue; 0 (default) = off. */
 int fac_set_option(fac_handle* h, const char* name, int value);
 
 size_t fac_workspace_bytes(const fac_handle* h);

@@ -24,19 +24,19 @@ int fac_debug_conv(fac_handle* h, const float* x, const float* w_host, const flo
                    int Cin, int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
                    const float* in_alpha_host, const float* out_alpha_host, int act, const float* res,
                    float* y, int Tout, void* stream);
-/* Same contract as fac_debug_conv, forced through the tcgen05 kernels: promoted = 0 -> conv_tc_kernel
- * (3xTF32, accumulates in TMEM only), 1 -> conv_tcp_kernel (3xTF32, TMEM accumulators promoted to fp32
- * registers every ~48 MMAs; the variant used upstream of the VQ), 2 -> conv_tc_kernel with the bf16 hi/lo
- * split (decoder-only precision class), 3 -> conv_tcp_kernel with the fp16 hi + 2^11-scaled fp16 lo split
- * (experimental "encoder_f16x2" class).  Returns FAC_ERR_UNSUPPORTED when
- * the layer geometry is not eligible (Cin % 16, Cout % 16, stride). */
+/* Same contract as fac_debug_conv, forced through the wgmma conv kernel: promoted = 0 -> 3xTF32, one accumulator,
+ * 1 -> 3xTF32 with each window of <= 48 chained MMAs promoted into an fp32 master accumulator, 2 -> bf16 hi/lo split
+ * (decoder-only precision class), 3 -> promoted fp16 hi + 2^11-scaled fp16 lo split (the class used upstream of the
+ * VQ), 4 -> 3 in the transposed formulation (weights as the wgmma A operand, time as wgmma N), 5 -> ONE fp16 pass (the
+ * k = 7 convs downstream of the VQ).  The handle's "tc_occ2_maxn" applies.  Returns FAC_ERR_UNSUPPORTED when the layer
+ * geometry is not eligible (Cin % 16, Cout % 16, stride) and for any other mode. */
 int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin,
                       int Cin, int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
                       const float* in_alpha_host, const float* out_alpha_host, int act, const float* res,
                       float* y, int Tout, int promoted, void* stream);
 /* One ResidualUnit (dac/model/dac.py:25-42) y = x + conv1(snake(conv7_d(snake(x)))) on DEVICE channels-last
- * x, y [B,T,C] with HOST folded weights w7 [C,C,7], w1 [C,C,1].  mode 0: fp32 FMA kernels, 1: two tcgen05
- * launches, 2: the single fused tcgen05 launch (FAC_ERR_UNSUPPORTED if the geometry cannot be fused);
+ * x, y [B,T,C] with HOST folded weights w7 [C,C,7], w1 [C,C,1].  mode 0: fp32 FMA kernels, 1: two tensor-core
+ * launches, 2: the single fused tensor-core launch (FAC_ERR_UNSUPPORTED if the geometry cannot be fused);
  * 3 / 4: as 1 / 2 with the bf16 hi/lo split. */
 int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const float* b7_host, const float* w1_host,
                       const float* b1_host, const float* alpha1_host, const float* alpha2_host, int B, int T, int C,
@@ -63,12 +63,11 @@ long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out
  * (dac/model/encodec.py:96-113 pad1d incl. the short-input branch): out[i] = source row of padded position
  * i - pad_left, or -1 where the padded value is zero; n must be pad_left + L + pad_right. */
 int fac_debug_pad_map(int L, int pad_left, int pad_right, int reflect, int* out, int n);
-/* Host-only (no GPU, no handle): the tile plan of the tcgen05 conv kernels for one layer geometry.  mode: 0 conv_tc TF32,
- * 1 conv_tcp (promoted) TF32, 2 conv_tc bf16, 3 conv_tcp fp16 hi + scaled lo, 4 fused ResidualUnit bf16, 5 fused TF32,
- * 6 conv_tt (transposed: out8[0] = output channels per CTA tile -- 128, or 256 in PAIR mode where two weight tiles share one
- * produced operand --, out8[1] = time steps per tile).
- * Tout may be 0 (unknown).  out8 = {N, MT, K chunks, weight-ring stages, TMEM columns, dynamic shared-memory bytes,
- * padded rows of the operand buffer, chunks per promotion}.  FAC_ERR_UNSUPPORTED when the layer is not eligible. */
+/* Host-only (no GPU, no handle): the tile plan of the wgmma conv kernel for one layer geometry.  mode: 0 TF32,
+ * 1 promoted TF32, 2 bf16, 3 promoted fp16 hi + scaled lo, 4 fused ResidualUnit bf16, 5 fused TF32, 6 mode 3 in the
+ * transposed formulation.  occ2_maxn as the "tc_occ2_maxn" option.  Tout may be 0 (unknown).  out8 = {N, MT (2: warpgroups split 128 rows, 1: they split N over 64 rows),
+ * K chunks, weight-ring stages, rows per tile, dynamic shared-memory bytes, padded rows of the operand buffer,
+ * chunks per promotion}.  FAC_ERR_UNSUPPORTED when the layer is not eligible. */
 int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* out8);
 /* Host-only: packs nn.Conv1d weights [Cout][Cin][K] (HOST) into the tensor-core blob of mode 0..3 (see
  * fac_debug_tc_plan): [Cout/N][K chunks][taps][hi|lo][k-groups][N][16 bytes], hi|lo = TF32 pair (4 k-groups of 4 fp32
@@ -92,7 +91,7 @@ int fac_debug_tap(fac_handle* h, const char* name, float* dst, size_t capacity_f
 
 /* Per-kernel-family device timing for bench.py's roofline object: when enabled, every launch of
  * the forward paths is bracketed by CUDA events on the launching stream.  Families: "conv"
- * (conv_cl_kernel, fp32 FMA), "conv_tc" (conv_tc_kernel, tcgen05 3xTF32), "lstm_rec", "fa_quantize".  fac_profile_get returns
+ * (conv_cl_kernel, fp32 FMA), "conv_tc" / "conv_tcp" (conv_tc_kernel, plain / promoted), "lstm_rec", "fa_quantize".  fac_profile_get returns
  * the accumulated device milliseconds, ALGORITHMIC flops (2*MACs) and bytes (in + out + weights
  * once) and launch count since the last fac_profile_reset (it synchronises the device). */
 int fac_profile_enable(fac_handle* h, int on);

@@ -1,6 +1,6 @@
-"""TEST INFRASTRUCTURE ONLY -- imports the *unmodified* reference from /root/reference.
+"""TEST INFRASTRUCTURE ONLY -- imports the *unmodified* reference from FACODEC_REFERENCE_ROOT.
 
-Only usable inside the build container (the GPU box has no /root/reference).
+Only usable where the reference tree is present; tests use the fixtures oracle/make_golden.py made from it.
 It is used to (1) validate the restatement in ``oracle/facodec_oracle.py``
 bit-for-bit and (2) generate the committed fixtures under ``tests/golden/``
 (``oracle/make_golden.py``).
@@ -21,7 +21,7 @@ import types
 import torch
 from torch import nn
 
-REFERENCE_ROOT = os.environ.get("FACODEC_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("FACODEC_REFERENCE_ROOT", "")   # the reference tree, when present
 
 
 class _Anything(types.ModuleType):
@@ -100,7 +100,7 @@ def _install_stubs():
 
 
 def available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "dac"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "dac"))
 
 
 def recursive_munch(d):

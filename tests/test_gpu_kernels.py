@@ -142,9 +142,9 @@ TC_CASES = [
     (1, 300, 384, 1920, 2, 1, 1, 1, 0, 0, 1, 0, 0, 0),    # up-conv 384 -> 5*384, N=240
     (2, 64, 1024, 1024, 3, 1, 1, 2, 0, 1, 1, 0, 0, 0),    # encoder conv_out geometry
     (1, 640, 1024, 4096, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),   # LSTM input projection geometry
-    (2, 320, 256, 512, 5, 1, 1, 4, 0, 1, 0, 0, 0, 0),     # WN in_layer geometry, T' = 320 (time tile 160 in the transposed kernel)
+    (2, 320, 256, 512, 5, 1, 1, 4, 0, 1, 0, 0, 0, 0),     # WN in_layer geometry, T' = 320
     (1, 1000, 128, 128, 7, 3, 1, 18, 0, 1, 1, 1, 0, 1),   # several time tiles + residual + both Snakes
-    (2, 700, 256, 256, 1, 1, 1, 0, 0, 1, 0, 0, 0, 1),     # encoder 1x1 + residual: conv_tt PAIR mode (two channel tiles x 128 steps), ragged tail
+    (2, 700, 256, 256, 1, 1, 1, 0, 0, 1, 0, 0, 0, 1),     # encoder 1x1 + residual, two channel tiles, ragged tail
     (1, 1000, 64, 512, 3, 1, 1, 2, 0, 1, 1, 1, 0, 0),     # 3 taps, 4 channel tiles (two pairs), both Snakes, several time tiles
 ]
 
@@ -153,15 +153,15 @@ TC_CASES = [
 @pytest.mark.parametrize("promoted", [0, 1, 2, 3, 4, 5])
 @pytest.mark.parametrize("case", TC_CASES)
 def test_conv_tc_kernel_vs_torch(case, promoted, occ2, built_lib):
-    """tcgen05 3xTF32 conv vs fp32 torch.  Operands are split exactly (hi + lo), but the tensor core adds
-    into its fp32 TMEM accumulator with truncation, so the error grows ~0.5 ulp per chained MMA
-    (measured ~1e-5 relative after 168 MMAs); tolerance 6e-5 * scale.  promoted=1 is the variant that
-    drains TMEM into fp32 registers every ~48 MMAs: held to 4e-6 * scale like the fp32 FMA kernel."""
+    """wgmma 3xTF32 conv vs fp32 torch.  Operands are split exactly (hi + lo), but the tensor core adds into its fp32
+    accumulator with truncation, so the error grows with the number of chained MMAs; tolerance 6e-5 * scale.
+    promoted=1 adds each window of <= 48 chained MMAs into an fp32 master accumulator: held to 4e-6 * scale like the
+    fp32 FMA kernel."""
     B, T, Cin, Cout, K, dil, stride, pl, pr, reflect, ins, outs, act, res = case
     if occ2 and promoted in (1, 3, 4):
         pytest.skip("the promoted kernel has a single residency plan")
     e = _engine()
-    e.set_option("tc_occ2_maxn", occ2)      # 256: tiles planned for two resident CTAs per SM (MT * N <= 256)
+    e.set_option("tc_occ2_maxn", occ2)      # 256: tiles planned for two resident CTAs per SM
     g = torch.Generator().manual_seed(hash(case) % 1000 + 7)
     x = torch.randn(B, Cin, T, generator=g) * 0.5
     w = torch.randn(Cout, Cin, K, generator=g) / math.sqrt(Cin * K)
@@ -183,8 +183,8 @@ def test_conv_tc_kernel_vs_torch(case, promoted, occ2, built_lib):
     scale = ref.abs().max().item()
     rel_rms = ((y - ref).double().pow(2).mean().sqrt() / ref.double().pow(2).mean().sqrt()).item()
     print(f"TCERR promoted={promoted} occ2={occ2} case={case} maxerr={err:.3e} scale={scale:.3f} rel_rms={rel_rms:.3e}")
-    # TMEM-truncating 3xTF32 / promoted (fp32-grade) / bf16 hi+lo / promoted with the fp16 hi + scaled-lo split (fp32-grade)
-    # 4 = the transposed formulation (conv_tt_kernel): same fp16 hi + scaled-lo split and promotion as 3, time as MMA N
+    # 3xTF32 / promoted (fp32-grade) / bf16 hi+lo / promoted with the fp16 hi + scaled-lo split (fp32-grade)
+    # 4 = the transposed formulation of 3: weights as the wgmma A operand, time as wgmma N
     # 5 = ONE fp16 pass (the k = 7 convs downstream of the VQ): 10-bit operands, error ~2e-4 of the output's RMS
     tol = {0: 6e-5, 1: 4e-6, 2: 2e-4, 3: 4e-6, 4: 4e-6, 5: 2e-3}[promoted]
     assert err <= tol * max(scale, 1.0), f"max err {err} (scale {scale})"
@@ -195,7 +195,7 @@ def test_conv_tc_kernel_vs_torch(case, promoted, occ2, built_lib):
 @pytest.mark.parametrize("B,T,C,dil", [(2, 300, 96, 1), (1, 520, 96, 9), (2, 200, 192, 3), (1, 130, 256, 1), (2, 40, 96, 9),
                                        (1, 700, 64, 3)])
 def test_residual_unit_modes(B, T, C, dil, mode, occ2, built_lib):
-    """ResidualUnit (dac.py:25-42) through the fp32 FMA path (0), two tcgen05 launches (1 tf32, 3 bf16 split), and the
+    """ResidualUnit (dac.py:25-42) through the fp32 FMA path (0), two tensor-core launches (1 tf32, 3 bf16 split), and the
     fused launch (2 tf32, 4 bf16 split), 5/6 = 3/4 with the k = 7 conv in ONE fp16 pass (the product's default downstream of
     the VQ); occ2 = tiles planned for two CTAs per SM."""
     from oracle import facodec_oracle as O
@@ -219,8 +219,8 @@ def test_residual_unit_modes(B, T, C, dil, mode, occ2, built_lib):
     rc = e.L.fac_debug_resunit(e.handle, _p(xd), _p(w7.contiguous()), _p(b7), _p(w1.contiguous()), _p(b1), _p(a1), _p(a2),
                                B, T, C, dil, mode, _p(yd), None)
     if mode == 2 and C > 128:
-        # the fused kernel keeps the whole GEMM-2 operand in shared memory: with the tf32 split that only fits up to
-        # C = 128 (the product runs fused units with the bf16 split, mode 4)
+        # the fused kernel keeps the whole GEMM-2 operand and a chunk's weights in shared memory: with the tf32 split
+        # that only fits up to C = 128 (the product runs fused units with the bf16 split, mode 4)
         assert rc != 0
         return
     assert rc == 0, e.L.fac_last_error(e.handle)

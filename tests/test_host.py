@@ -120,13 +120,29 @@ def _plan(L, Cin, Cout, K, dil, stride, Tout, mode, occ2):
     import ctypes
     out = (ctypes.c_int * 8)()
     rc = L.fac_debug_tc_plan(Cin, Cout, K, dil, stride, Tout, mode, occ2, out)
-    return rc, dict(zip(("N", "MT", "nchunk", "stages", "tmem_cols", "smem", "Rpad", "promote_every"), list(out)))
+    return rc, dict(zip(("N", "MT", "nchunk", "stages", "rows", "smem", "Rpad", "promote_every"), list(out)))
 
 
-def test_tcgen05_tile_plans_respect_hardware_limits(built_lib):
-    """Host logic of the tensor-core path (no GPU): every layer geometry of the model gets a plan inside the SM's
-    limits -- TMEM <= 512 columns (<= 256 for the two-CTA plan), dynamic shared memory <= 225 KB (<= 112 KB), N | Cout,
-    promotion window <= 48 chained MMAs -- and ineligible layers are refused."""
+SMEM_CAP = 227 * 1024     # dynamic shared memory per block on sm_90
+
+
+def _check_plan(p, Cout, mode, K, stride):
+    """A plan the wgmma kernel can run: N | Cout in 16-channel steps, a tile of 128 rows (warpgroups split rows) or 64 rows
+    (they split channels), per-warpgroup accumulators of <= 128 floats (<= 64 when promoted: master + window registers),
+    1-2 weight stages, shared memory within the SM, promotion windows of <= 48 chained MMAs."""
+    assert Cout % p["N"] == 0 and p["N"] % 16 == 0
+    assert p["rows"] == 64 * p["MT"] and p["MT"] in (1, 2)
+    nw = p["N"] if p["MT"] == 2 else p["N"] // 2
+    assert nw % 16 == 0 and nw <= (64 if mode in (1, 3) else 128)
+    assert 1 <= p["stages"] <= 2 and p["smem"] <= SMEM_CAP
+    if mode in (1, 3):
+        Kr = K if stride == 1 else 2
+        assert p["promote_every"] * Kr * (1 if mode == 3 else 6) <= 48 or p["promote_every"] == 1
+
+
+def test_tensor_core_tile_plans_respect_hardware_limits(built_lib):
+    """Host logic of the tensor-core path (no GPU): every layer geometry of the model gets a plan inside the SM's limits
+    (_check_plan) and ineligible layers are refused."""
     from facodec_b200 import _lib
     L = _lib.load()
     enc = [(64, 64, 7, d, 1, 96000) for d in (1, 3, 9)] + [(128, 128, 7, 9, 1, 48000), (256, 256, 7, 9, 1, 9600),
@@ -135,34 +151,20 @@ def test_tcgen05_tile_plans_respect_hardware_limits(built_lib):
            (256, 512, 5, 1, 1, 320), (512, 1024, 5, 1, 1, 320)]
     for (Cin, Cout, K, dil, stride, T) in enc:
         for mode in (1, 3):
-            rc, p = _plan(L, Cin, Cout, K, dil, stride, T, mode, 256)
+            rc, p = _plan(L, Cin, Cout, K, dil, stride, T, mode, 0)
             assert rc == 0, (Cin, Cout, K, mode)
-            assert Cout % p["N"] == 0 and p["N"] % 16 == 0 and p["N"] <= 128
-            assert p["MT"] * p["N"] <= (128 if mode == 3 else 256) and p["tmem_cols"] == 512
-            assert p["smem"] <= 225 * 1024 and 2 <= p["stages"] <= 8
-            Kr = K if stride == 1 else 2
-            chain = p["promote_every"] * Kr * (1 if mode == 3 else 6)
-            assert chain <= 48 or p["promote_every"] == 1
+            _check_plan(p, Cout, mode, K, stride)
     dec = [(1024, 1536, 7, 1, 1, 320), (1536, 6144, 1, 1, 1, 10240), (768, 768, 7, 9, 1, 1920), (384, 384, 7, 3, 1, 9600),
            (384, 384, 1, 1, 1, 9600), (192, 192, 2, 1, 1, 48000), (1536, 4608, 2, 1, 1, 320)]
     for (Cin, Cout, K, dil, stride, T) in dec:
-        for occ2 in (0, 256):
-            rc, p = _plan(L, Cin, Cout, K, dil, stride, T, 2, occ2)
-            assert rc == 0
-            assert Cout % p["N"] == 0 and p["N"] <= 256 and p["MT"] * p["N"] <= p["tmem_cols"] <= 512
-            if occ2:
-                assert p["tmem_cols"] <= 256 and p["smem"] <= 112 * 1024      # two CTAs per SM
-            assert p["smem"] <= 225 * 1024
-    # fused ResidualUnits: C = 96 fits the two-CTA plan, C = 192 needs 384 TMEM columns -> one CTA per SM
-    rc, p96 = _plan(L, 96, 96, 7, 9, 1, 96000, 4, 256)
-    rc2, p192 = _plan(L, 192, 192, 7, 9, 1, 48000, 4, 256)
-    assert rc == 0 and rc2 == 0
-    assert p96["tmem_cols"] <= 256 and p96["smem"] <= 112 * 1024
-    assert p192["MT"] == 1 and p192["tmem_cols"] == 512
-    # short sequences: MT trimmed so the padded tail of the tile grid stays small
-    _, long_t = _plan(L, 512, 512, 7, 1, 1, 1920, 1, 0)
-    _, short_t = _plan(L, 512, 512, 7, 1, 1, 320, 1, 0)
-    assert long_t["MT"] == 2 and short_t["MT"] == 1
+        rc, p = _plan(L, Cin, Cout, K, dil, stride, T, 2, 0)
+        assert rc == 0
+        _check_plan(p, Cout, 2, K, stride)
+    # fused ResidualUnits keep every channel in one tile: N = C
+    for C in (96, 192, 256):
+        rc, p = _plan(L, C, C, 7, 9, 1, 48000, 4, 0)
+        assert rc == 0 and p["N"] == C
+        _check_plan(p, C, 4, 7, 1)
     # not eligible: Cin not a multiple of 16 per row, odd strides, fused with Cin != Cout
     assert _plan(L, 20, 256, 1, 1, 1, 320, 1, 0)[0] != 0
     assert _plan(L, 64, 64, 7, 1, 3, 100, 0, 0)[0] != 0
@@ -172,7 +174,7 @@ def test_tcgen05_tile_plans_respect_hardware_limits(built_lib):
 @pytest.mark.parametrize("mode", [0, 1, 2, 3])
 @pytest.mark.parametrize("geom", [(64, 64, 7, 1), (128, 256, 10, 5), (96, 96, 1, 1), (32, 48, 3, 1)])
 def test_tensor_core_weight_blob_layout_and_split(geom, mode, built_lib):
-    """Host logic (no GPU): the UMMA weight blob.  Decodes [ntile][chunk][tap][hi|lo][k-group][N][16 B] back to W and
+    """Host logic (no GPU): the tensor-core weight blob.  Decodes [ntile][chunk][tap][hi|lo][k-group][N][16 B] back to W and
     checks the split classes: TF32 pair / bf16 pair / fp16 hi + 2^11-scaled lo reconstruct w to their mantissa budget
     and each half is exactly representable in its format."""
     import ctypes
@@ -294,7 +296,7 @@ int main(void) {
     int plan[8];
     int pad[9];
     if (fac_abi_version() != 2) return 2;
-    if (fac_debug_tc_plan(192, 192, 7, 9, 1, 48000, 4, 256, plan) != FAC_OK) return 3;
+    if (fac_debug_tc_plan(192, 192, 7, 9, 1, 48000, 4, 0, plan) != FAC_OK) return 3;
     if (fac_debug_pad_map(3, 6, 0, 1, pad, 9) != FAC_OK) return 4;
     if (fac_encode_frames(96000) != 320) return 5;
     printf("%d %d %d %d\n", plan[0], plan[1], plan[4], pad[0]);
@@ -308,50 +310,7 @@ int main(void) {
     env = dict(os.environ)
     env["LD_LIBRARY_PATH"] = "/usr/local/cuda/lib64:" + env.get("LD_LIBRARY_PATH", "")
     out = subprocess.check_output([str(exe)], env=env, text=True).split()
-    assert out[:3] == ["192", "1", "512"]        # fused C = 192 unit: N = 192, MT = 1, 512 TMEM columns
-
-
-@pytest.mark.parametrize("geom", [(64, 64, 7, 1), (128, 256, 10, 5), (96, 200, 3, 1), (512, 2176, 1, 1)])
-def test_transposed_kernel_weight_blob(geom, built_lib):
-    """Host logic (no GPU): conv_tt_kernel's A-operand blob [co tile of 128][chunk][tap][hi|lo'][k8][128 rows][8 fp16]
-    decodes back to W (fp16 hi + lo'/2^11 to 2^-20), rows beyond Cout are zero, and the plan puts time on MMA N."""
-    import ctypes
-    import numpy as np
-    from facodec_b200 import _lib
-    L = _lib.load()
-    Cin, Cout, K, stride = geom
-    rng = np.random.RandomState(Cin + Cout)
-    w = (rng.randn(Cout, Cin, K) / np.sqrt(Cin * K)).astype(np.float32)
-    P = lambda a: ctypes.c_void_p(a.ctypes.data)
-    n = L.fac_debug_tc_pack(P(w), Cin, Cout, K, stride, 4, None, 0)
-    assert n > 0
-    blob = np.zeros(n, np.float32)
-    assert L.fac_debug_tc_pack(P(w), Cin, Cout, K, stride, 4, P(blob), n) == n
-    out = (ctypes.c_int * 8)()
-    assert L.fac_debug_tc_plan(Cin, Cout, K, 1, stride, 96000, 6, 0, out) == 0
-    Kr, vf = (K, 1) if stride == 1 else (2, stride)
-    # PAIR mode (two 128-channel weight tiles share one produced operand of <= 128 time steps) for short-tap layers with an
-    # even number of channel tiles; everything else: one tile x 256 time steps
-    pair = Kr <= 3 and ((Cout + 127) // 128) % 2 == 0
-    assert out[0] == (256 if pair else 128) and out[1] == (128 if pair else 256) and out[4] == 512 and out[5] <= 225 * 1024
-    assert out[7] * Kr <= 48
-    assert L.fac_debug_tc_plan(Cin, Cout, K, 1, stride, 320, 6, 0, out) == 0
-    assert out[1] == (112 if pair else 160)      # T' = 320: three tiles of 112 / two full tiles of 160
-    nchunk = out[2]
-    Wg = np.zeros((Kr, vf * Cin, Cout), np.float32)
-    for k in range(K):
-        Wg[k // vf, (k % vf) * Cin:(k % vf + 1) * Cin, :] = w[:, :, k].T
-    nt = (Cout + 127) // 128
-    h16 = blob.view(np.float16).reshape(nt, nchunk, Kr, 2, 2, 128, 8)          # [..][hl][k8][row][e]
-    dec = lambda a: a.transpose(0, 1, 2, 4, 3, 5).reshape(nt, nchunk, Kr, 128, 16).astype(np.float64)
-    rec = dec(h16[:, :, :, 0]) + dec(h16[:, :, :, 1]) / 2048.0                    # [nt][chunk][tap][row][kk]
-    ref = np.zeros((nt, nchunk, Kr, 128, 16))
-    for t in range(nt):
-        rows = min(128, Cout - t * 128)
-        ref[t, :, :, :rows] = Wg[:, :, t * 128:t * 128 + rows].reshape(Kr, nchunk, 16, rows).transpose(1, 0, 3, 2)
-    assert np.abs(rec - ref).max() <= 2.0 ** -20 * np.abs(ref).max()
-    if Cout % 128:
-        assert not rec[-1, :, :, Cout % 128:].any()
+    assert out[:3] == ["192", "1", "64"]         # fused C = 192 unit: N = 192, warpgroups split channels, 64-row tiles
 
 
 @pytest.mark.parametrize("H,mode", [(1024, 3), (1024, 2), (1536, 2)])
@@ -482,13 +441,13 @@ def test_fa_predictors_state_dict_surface():
 
 
 def test_tile_plans_of_every_codec_layer_fit_the_sm(built_lib):
-    """Host logic (no GPU): the tensor-core tile plans of every conv geometry of config.yml's encoder (transposed kernel, incl.
-    PAIR mode) and decoder (conv_tc bf16 / fused units) at the benchmark lengths stay inside one SM: <= 225 KB of dynamic
-    shared memory (<= 112 KB when two CTAs share the SM), <= 512 TMEM columns, time tiles of 16..256 steps."""
+    """Host logic (no GPU): the tensor-core tile plans of every conv geometry of config.yml's encoder (promoted, fp16 hi +
+    scaled-lo split) and decoder (bf16 split / fused units) at the benchmark lengths stay inside one SM (_check_plan)."""
     import ctypes
     from facodec_b200 import _lib
     L = _lib.load()
     out = (ctypes.c_int * 8)()
+    keys = ("N", "MT", "nchunk", "stages", "rows", "smem", "Rpad", "promote_every")
     enc = []                                    # (Cin, Cout, K, dil, stride, Tout)
     T, c = 96000, 64
     for s in (2, 5, 5, 6):
@@ -499,10 +458,8 @@ def test_tile_plans_of_every_codec_layer_fit_the_sm(built_lib):
         c *= 2
     enc += [(1024, 4096, 1, 1, 1, 320 * 32), (1024, 1024, 3, 1, 1, 320)]
     for (ci, co, k, d, st, to) in enc:
-        assert L.fac_debug_tc_plan(ci, co, k, d, st, to, 6, 0, out) == 0, (ci, co, k)
-        chans, nt, smem, cols = out[0], out[1], out[5], out[4]
-        assert chans in (128, 256) and 16 <= nt <= 256 and nt % 16 == 0 and (chans == 128 or nt <= 128)
-        assert smem <= 225 * 1024 and cols <= 512
+        assert L.fac_debug_tc_plan(ci, co, k, d, st, to, 3, 0, out) == 0, (ci, co, k)
+        _check_plan(dict(zip(keys, list(out))), co, 3, k, st)
     dec = []
     T, c = 320, 1536
     for s in (6, 5, 5, 2):
@@ -516,8 +473,5 @@ def test_tile_plans_of_every_codec_layer_fit_the_sm(built_lib):
                 dec += [(c, c, 7, d, 1, T, 2), (c, c, 1, 1, 1, T, 2)]
     dec += [(1024, 1536, 7, 1, 1, 320, 2), (1536, 6144, 1, 1, 1, 320 * 32, 2)]
     for (ci, co, k, d, st, to, mode) in dec:
-        for occ2 in (0, 256):
-            assert L.fac_debug_tc_plan(ci, co, k, d, st, to, mode, occ2, out) == 0, (ci, co, k, mode)
-            n, mt, smem, cols = out[0], out[1], out[5], out[4]
-            assert co % n == 0 and mt in (1, 2, 4) and cols <= 512 and (mode == 4 or mt * n <= cols) and (mode != 4 or 2 * mt * n <= cols)
-            assert smem <= (112 * 1024 if (occ2 and cols <= 256) else 225 * 1024)
+        assert L.fac_debug_tc_plan(ci, co, k, d, st, to, mode, 0, out) == 0, (ci, co, k, mode)
+        _check_plan(dict(zip(keys, list(out))), co, mode, k, st)

@@ -1,5 +1,6 @@
-"""CPU: the oracle restatement against (a) the committed golden fixtures generated from the
-imported unmodified reference and (b) the imported reference itself when /root/reference exists."""
+"""CPU: the oracle restatement against the committed golden fixtures generated from the imported unmodified
+reference (oracle/make_golden.py): whole-model cases (tests/golden/<case>.npz) and the module-level pins
+(tests/golden/pin_*.npz)."""
 import hashlib
 import os
 
@@ -13,10 +14,23 @@ from oracle import ref_import
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-# Bit-exact in the build container (same CPU, same ATen kernels as when the fixtures were made);
-# on another host CPU oneDNN may pick other kernels, so floats get a tight tolerance there.
+# Bit-exact where the fixtures were made (same CPU, same ATen kernels); on another host CPU oneDNN may pick
+# other kernels, so floats get a tight tolerance there.
 SAME_HOST = ref_import.available()
 ATOL = 0.0 if SAME_HOST else 2e-5
+
+
+def _pin(name):
+    return dict(np.load(os.path.join(ROOT, "tests", "golden", "pin_" + name + ".npz")))
+
+
+def _pinned_params(pin, seed):
+    """The seeded parameters (oracle/make_golden.py seeded_params) and stored buffers the pinned module ran with."""
+    from oracle import make_golden
+    shapes = {k[len("shape/"):]: v for k, v in pin.items() if k.startswith("shape/")}
+    sd = make_golden.seeded_params(shapes, seed)
+    sd.update({k[len("buffer/"):]: torch.from_numpy(v) for k, v in pin.items() if k.startswith("buffer/")})
+    return sd
 
 
 def _close(a, b, name):
@@ -72,53 +86,38 @@ def test_oracle_matches_golden(name):
             _close(t, g[k], k)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 def test_oracle_matches_imported_reference():
-    """Pins the restatement to the real thing: bit-identical tensors from the unmodified reference."""
-    import warnings
-    warnings.simplefilter("ignore")
-    model = ref_import.build_reference_model(0)
+    """Pins the restatement to the real thing: the unmodified reference's tensors for this case (pin_codec.npz)."""
+    g = _pin("codec")
     sds = state_dicts(1)
-    for k in ("encoder", "quantizer", "decoder"):
-        model[k].load_state_dict(sds[k])
     x, _ = case_inputs(dict(B=2, T=4500, xseed=21))
     with torch.no_grad():
-        z = model.encoder(x)
-        q = model.quantizer(z, x, n_c=2, return_codes=True)
-        y = model.decoder(q[0])
         z2, q2, y2 = O.codec_forward(sds, x, n_c=2)
-    assert torch.equal(z, z2) and torch.equal(q[0], q2[0]) and torch.equal(y, y2)
-    assert torch.equal(q[4], q2[4])
-    for a, b in zip(q[5], q2[5]):
-        assert torch.equal(a, b)
-    for a, b in zip(q[1], q2[1]):
-        assert torch.equal(a, b)
-    assert float(q[2]) == float(q2[2]) and float(q[3]) == float(q2[3])
+    for k, t in (("z", z2), ("outs", q2[0]), ("y", y2), ("timbre", q2[4]), ("z_p", q2[1][0]), ("z_c", q2[1][1]), ("z_r", q2[1][2])):
+        _close(t, g[k], k)
+    for k, t in zip(("codes_p", "codes_c", "codes_r"), q2[5]):
+        assert np.array_equal(t.numpy(), g[k]), k
+    _close(float(q2[2]), g["commitment"], "commitment")
+    _close(float(q2[3]), g["codebook"], "codebook")
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 def test_fvq_rvq_and_alias_free_match_reference():
-    import sys
-    import warnings
-    warnings.simplefilter("ignore")
-    ref_import.import_reference()
-    from quantize.rvq import ResidualVQ as RefRVQ
-    from alias_free_torch import Activation1d as RefAct
-    torch.manual_seed(3)
-    rvq = RefRVQ(num_quantizers=4, codebook_size=10, dim=1024, codebook_dim=8, commitment=0.25).eval()
-    x = torch.randn(2, 1024, 17)
-    layers = []
-    for l in rvq.layers:
-        layers.append(dict(in_w=l.in_proj.weight.detach(), in_b=l.in_proj.bias.detach(),
-                           out_w=l.out_proj.weight.detach(), out_b=l.out_proj.bias.detach(),
-                           codebook=l.codebook.weight.detach()))
+    g = _pin("rvq_act")
+    sd = _pinned_params(g, 3)
+    def wn(p):      # the projections are weight-normed (dim 0), as the reference module folds them
+        return torch._weight_norm(sd[p + ".weight_v"], sd[p + ".weight_g"], 0)
+    layers = [dict(in_w=wn(f"layers.{i}.in_proj"), in_b=sd[f"layers.{i}.in_proj.bias"],
+                   out_w=wn(f"layers.{i}.out_proj"), out_b=sd[f"layers.{i}.out_proj.bias"],
+                   codebook=sd[f"layers.{i}._codebook.weight"]) for i in range(4)]
+    gen = torch.Generator().manual_seed(3)
+    x = torch.randn(2, 1024, 17, generator=gen)
     with torch.no_grad():
-        a = rvq(x)
         b = O.fvq_residual_vq(layers, x)
-    assert torch.equal(a[1], b[1]) and torch.equal(a[0], b[0]) and torch.equal(a[3], b[3])
-    act = RefAct(activation=torch.nn.Identity())
-    xx = torch.randn(2, 5, 50)
-    assert torch.allclose(act(xx), O.alias_free_act(xx, lambda u: u), atol=0, rtol=0)
+    assert np.array_equal(b[1].numpy(), g["idx"])
+    _close(b[0], g["q"], "q")
+    _close(b[3], g["allq"], "allq")
+    xx = torch.randn(2, 5, 50, generator=gen)
+    _close(O.alias_free_act(xx, lambda u: u), g["act_y"], "alias-free")
 
 
 def test_reflect_pad_short_branch():
@@ -157,127 +156,92 @@ def test_redecoder_oracle_matches_golden(name):
     _close(y, g["y"], "y")
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 def test_redecoder_oracle_matches_imported_reference():
-    """modules/redecoder.py:35-48 + the non-causal, LSTM-free Decoder of build_model(stage='redecoder'): bit-identical."""
-    import warnings
-    warnings.simplefilter("ignore")
+    """modules/redecoder.py:35-48 + the non-causal, LSTM-free Decoder of build_model(stage='redecoder') (pin_redecoder.npz)."""
     from facodec_b200 import synth
-    model = ref_import.build_reference_redecoder(0)
+    pin = _pin("redecoder")
     sds = synth.synth_redecoder_state_dicts(2)
-    for k in ("encoder", "decoder"):
-        model[k].load_state_dict(sds[k])
     g = torch.Generator().manual_seed(5)
     cp = torch.randint(0, 1024, (2, 1, 13), generator=g)
     cc = torch.randint(0, 1024, (2, 2, 13), generator=g)
     timbre = torch.randn(2, 1024, generator=g)
     for use_p, n_c in ((False, 1), (True, 2)):
         with torch.no_grad():
-            z = model.encoder(cp, cc, timbre, use_p_code=use_p, n_c=n_c)
-            y = model.decoder(z)
             z2 = O.redecoder_forward(sds["encoder"], cp, cc, timbre, use_p_code=use_p, n_c=n_c)
             y2 = O.decoder_forward(sds["decoder"], z2, causal=False, lstm=0)
-        assert torch.equal(z, z2) and torch.equal(y, y2)
+        _close(z2, pin[f"z_{int(use_p)}{n_c}"], "z")
+        _close(y2, pin[f"y_{int(use_p)}{n_c}"], "y")
 
-
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 def test_predictor_heads_and_snakebeta_match_imported_reference():
-    """SnakeBeta (modules/quantize.py:29-88) inside Activation1d, the heads' ResidualUnit (:90-104) and CNNLSTM (:106-125),
-    imported unmodified: the restatement is bit-identical (round 1 pinned the alias-free activation with Identity only)."""
-    import warnings
-    warnings.simplefilter("ignore")
+    """SnakeBeta (modules/quantize.py:29-88) inside Activation1d, the heads' ResidualUnit (:90-104) and CNNLSTM (:106-125)
+    of the unmodified reference (pin_heads.npz)."""
     from facodec_b200 import synth
-    ref_import.import_reference()
-    from modules.quantize import CNNLSTM, SnakeBeta
-    from alias_free_torch import Activation1d as RefAct
+    pin = _pin("heads")
     g = torch.Generator().manual_seed(9)
-    sb = SnakeBeta(6, alpha_logscale=True)
-    with torch.no_grad():
-        sb.alpha.copy_(torch.randn(6, generator=g) * 0.3)
-        sb.beta.copy_(torch.randn(6, generator=g) * 0.3)
+    alpha = torch.randn(6, generator=g) * 0.3
+    beta = torch.randn(6, generator=g) * 0.3
     x = torch.randn(2, 6, 40, generator=g)
     with torch.no_grad():
-        assert torch.equal(sb(x), O.snake_beta(x, sb.alpha, sb.beta))
-        act = RefAct(activation=sb)
-        assert torch.equal(act(x), O.alias_free_act(x, lambda u: O.snake_beta(u, sb.alpha, sb.beta)))
-    for (indim, outdim, heads, glob) in ((64, 10, 2, False), (32, 7, 1, True)):
-        m = CNNLSTM(indim, outdim, heads, global_pred=glob).eval()
+        _close(O.snake_beta(x, alpha, beta), pin["snakebeta"], "snakebeta")
+        _close(O.alias_free_act(x, lambda u: O.snake_beta(u, alpha, beta)), pin["act"], "act")
+    for j, (indim, outdim, heads, glob) in enumerate(((64, 10, 2, False), (32, 7, 1, True))):
         sd = synth.synth_cnnlstm(3, indim, outdim, heads)
-        missing, unexpected = m.load_state_dict(sd, strict=False)
-        assert not unexpected and all(k.endswith("filter") for k in missing)      # only the registered filter buffers
         xx = torch.randn(2, indim, 33, generator=g)
         with torch.no_grad():
-            a = m(xx)
             b = O.cnnlstm_forward(sd, xx, heads, global_pred=glob)
-        assert len(a) == len(b) == heads
-        for u, v in zip(a, b):
-            assert torch.equal(u, v)
+        assert len(b) == heads
+        for h, v in enumerate(b):
+            _close(v, pin[f"cnnlstm{j}_head{h}"], f"cnnlstm{j} head {h}")
 
-
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 def test_dataset_mel_matches_imported_meldataset():
-    """meldataset.py:37-47 preprocess (torchaudio MelSpectrogram with its default sample_rate = 16000) imported unmodified
-    (soundfile / librosa stubbed: file I/O only), against the restatement fed with synth's host-independent window and
-    16 kHz filterbank."""
-    import warnings
-    warnings.simplefilter("ignore")
+    """meldataset.py:37-47 preprocess (torchaudio MelSpectrogram with its default sample_rate = 16000) of the unmodified
+    reference (pin_dataset_mel.npz: output, window, filterbank), against the restatement fed with the reference's window
+    and filterbank and with synth's host-independent ones."""
     from facodec_b200 import synth
-    ref_import.import_reference()
-    import meldataset
+    pin = _pin("dataset_mel")
     w = synth.synth_waves(1, 5000, seed=3)[0, 0]
+    ref = torch.from_numpy(pin["mel"])
+    fb_ref, win_ref = torch.from_numpy(pin["fb"]), torch.from_numpy(pin["window"])
     with torch.no_grad():
-        ref = meldataset.preprocess(w.numpy())
-        fb_ref = meldataset.to_mel.mel_scale.fb
-        win_ref = meldataset.to_mel.spectrogram.window
-        got_same = O.dataset_mel(w, win_ref, fb_ref)
-        assert torch.equal(ref, got_same)
+        _close(O.dataset_mel(w, win_ref, fb_ref), pin["mel"], "mel")
         fb = synth.melscale_fbanks_htk(sample_rate=16000, f_max=8000.0)
         assert float((fb - fb_ref).abs().max()) <= 1e-5      # fp64-then-round vs torchaudio fp32 evaluation
         got = O.dataset_mel(w, synth.hann_window_periodic(1200), fb)
     assert tuple(ref.shape) == (1, 80, 5000 // 300 + 1)
     assert float((got - ref).abs().max()) <= 2e-5
 
-
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 def test_dac_code_file_matches_imported_dacfile(tmp_path):
-    """dac/model/base.py:15-54: files written here are byte-identical to the reference class's, and each side loads the
-    other's (codes, every metadata field)."""
+    """dac/model/base.py:15-54: files written here are byte-identical to the reference class's (pin_dacfile.npz), and the
+    reference's file loads here (codes, every metadata field)."""
     from facodec_b200 import codefile
-    ref_import.import_reference()
-    from dac.model.base import DACFile as RefFile
+    ref_bytes = _pin("dacfile")["bytes"].tobytes()
     g = torch.Generator().manual_seed(9)
     codes = [torch.randint(0, 1024, (2, n, 37), generator=g) for n in (1, 2, 3)]
     mine = codefile.from_forward(codes, original_length=37 * 300, input_db=torch.tensor([-23.5, -17.25]))
-    ref = RefFile(codes=codefile.pack_codes(codes), chunk_length=37, original_length=37 * 300,
-                  input_db=torch.tensor([-23.5, -17.25]), channels=1, sample_rate=24000, padding=True, dac_version="1.0.0")
-    pa, pb = mine.save(tmp_path / "mine"), ref.save(tmp_path / "ref")
-    assert pa.suffix == ".dac" and open(pa, "rb").read() == open(pb, "rb").read()
-    a, b = RefFile.load(pa), codefile.DACFile.load(pb)
-    for f in (a, b):
-        assert torch.equal(f.codes, codefile.pack_codes(codes))
-        assert (f.chunk_length, f.original_length, f.channels, f.sample_rate, f.padding, f.dac_version) == (37, 11100, 1, 24000, True, "1.0.0")
-        assert np.array_equal(np.asarray(f.input_db), np.array([-23.5, -17.25], np.float32))
+    pa = mine.save(tmp_path / "mine")
+    assert pa.suffix == ".dac" and open(pa, "rb").read() == ref_bytes
+    pb = tmp_path / "ref.dac"
+    pb.write_bytes(ref_bytes)
+    b = codefile.DACFile.load(pb)
+    assert torch.equal(b.codes, codefile.pack_codes(codes))
+    assert (b.chunk_length, b.original_length, b.channels, b.sample_rate, b.padding, b.dac_version) == (37, 11100, 1, 24000, True, "1.0.0")
+    assert np.array_equal(np.asarray(b.input_db), np.array([-23.5, -17.25], np.float32))
     for u, v in zip(codefile.unpack_codes(b.codes, n_c=2), codes):
         assert torch.equal(u, v)
-
 
 def _loss_signals(B=2, T=4800, seed=11):
     from facodec_b200 import synth
     return synth.synth_loss_pair(B, T, seed)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 def test_reconstruction_loss_matches_imported_losses_py():
-    """losses.py:65-89 imported unmodified (torchaudio is installed) against the restatement: same scalar, bit for bit."""
-    import warnings
-    warnings.simplefilter("ignore")
-    ref_import.import_reference()
-    import losses as ref_losses
-    x, G_x = _loss_signals()
+    """losses.py:65-89 of the unmodified reference (recon_loss.npz) against the restatement: the same scalar."""
+    gold = np.load(os.path.join(ROOT, "tests", "golden", "recon_loss.npz"))
+    x, G_x = _loss_signals(int(gold["B"]), int(gold["T"]), int(gold["seed"]))
     with torch.no_grad():
-        ref = ref_losses.reconstruction_loss(x, G_x)
         got = O.reconstruction_loss(x, G_x)
-    assert ref.dim() == 0 and torch.equal(ref, got)
+    assert got.dim() == 0
+    _close(np.float32(got), gold["loss"], "loss")
 
 
 def test_reconstruction_loss_golden():
@@ -296,39 +260,35 @@ FAP_FLAGS = dict(use_gr_content_f0=False, use_gr_prosody_phone=False, use_gr_res
                  use_gr_timbre_content=True, use_gr_timbre_prosody=False, use_gr_x_timbre=True, norm_f0=True)   # modules/commons.py:311-322 + config.yml
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 @pytest.mark.parametrize("timbre_norm", [True, False])
 def test_fa_predictors_match_imported_reference(timbre_norm):
-    """FApredictors (modules/quantize.py:456-619) imported unmodified with build_model's flags, both forward variants:
-    the restatement over its state_dict is bit-identical, output by output."""
-    import warnings
-    warnings.simplefilter("ignore")
-    ref_import.import_reference()
-    from modules.quantize import FApredictors
-    torch.manual_seed(4)
-    m = FApredictors(in_dim=32, timbre_norm=timbre_norm, use_gr_content_global_f0=True, **FAP_FLAGS).eval()
-    sd = {k: v.detach() for k, v in m.state_dict().items()}
+    """FApredictors (modules/quantize.py:456-619) of the unmodified reference with build_model's flags, both forward
+    variants (pin_fa_predictors_*.npz: seeded parameters, sampled outputs): the restatement, output by output."""
+    from oracle import make_golden
+    pin = _pin(f"fa_predictors_{int(timbre_norm)}")
+    sd = _pinned_params(pin, 4)
     g = torch.Generator().manual_seed(6)
     lat = [torch.randn(2, 32, 19, generator=g) for _ in range(3 if timbre_norm else 4)]
     with torch.no_grad():
-        if timbre_norm:
-            timbre = torch.randn(2, 32, generator=g)
-            ref = m(lat, timbre)
-            got = O.fa_predictors_forward(sd, lat, timbre, timbre_norm=True, **FAP_FLAGS)
-        else:
-            ref = m(lat)
-            got = O.fa_predictors_forward(sd, lat, None, timbre_norm=False, **FAP_FLAGS)
-    for a, b in zip(ref, got):
-        assert a.keys() == b.keys()
-        for k in a:
-            if a[k] is None or b[k] is None:
-                assert a[k] is None and b[k] is None, k
-            elif a[k].shape[-1] == 1:
-                # 1-wide nn.Linear heads (f0 / uv): torch's CPU F.linear takes another kernel for weights that do not require
-                # grad (the oracle works on detached state_dict tensors, the module on Parameters): 1-2 ulp apart
-                assert float((a[k] - b[k]).abs().max()) <= 5e-7 * max(1.0, float(a[k].abs().max())), k
-            else:
-                assert torch.equal(a[k], b[k]), k
+        timbre = torch.randn(2, 32, generator=g) if timbre_norm else None
+        got = O.fa_predictors_forward(sd, lat, timbre, timbre_norm=timbre_norm, **FAP_FLAGS)
+    keys = {k for k in pin if k.startswith("out") and not k.startswith("outshape")}
+    seen = set()
+    for i, b in enumerate(got):
+        for k, v in b.items():
+            name = f"out{i}/{k}"
+            if v is None:
+                assert name not in pin, name
+                continue
+            assert tuple(v.shape) == tuple(pin[f"outshape{i}/{k}"]), name
+            idx = torch.from_numpy(make_golden.sample_positions(v.numel()))
+            # 1-wide nn.Linear heads (f0 / uv): torch's CPU F.linear takes another kernel for weights that do not require
+            # grad (the oracle works on detached state_dict tensors, the module on Parameters): 1-2 ulp apart
+            tol = 5e-7 if v.shape[-1] == 1 else ATOL
+            a, r = v.reshape(-1)[idx].numpy(), pin[name]
+            assert np.abs(a - r).max() <= tol * max(1.0, np.abs(r).max()), name
+            seen.add(name)
+    assert seen == keys
 
 
 def test_slaney_mel_filterbank_against_torchaudio():

@@ -1,5 +1,5 @@
 """Library baseline (SURVEY.md 8d): the reference's own ATen call sequence (the oracle restatement, i.e. what the
-reference's nn.Modules execute) run by PyTorch eager on the same B200 in fp32 with TF32 disabled, at BASELINE
+reference's nn.Modules execute) run by PyTorch eager on the same GPU in fp32 with TF32 disabled, at BASELINE
 configs[1] (32 x 4 s), timed beside this repo's path.  Informational numbers are printed (pytest -s); the assertions
 only pin that both paths agree (cuDNN picks its own summation orders, so a handful of near-tied VQ decisions may differ
 between eager-GPU and the CPU reference -- this repo matches the CPU reference bit for bit, see test_gpu_parity.py).
