@@ -2234,6 +2234,54 @@ int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, i
     return rc;
 }
 
+int fac_debug_fa_quantize(fac_handle* h, const float* f0, const float* z, const float* const vq_host[6][5],
+                          const float* gamma_beta, int n_c, int B, int Tq, int Tz, int Tf0, float* outs, float* zp,
+                          float* zc, float* zr, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* sqerr,
+                          float* losses2, void* stream) {
+    if (!h || !f0 || !z || !vq_host || !gamma_beta || !outs || !codes_p || !codes_c || !codes_r || !sqerr || !losses2)
+        return FAC_ERR_INVALID;
+    if (n_c < 1 || n_c > 2 || B <= 0 || Tq <= 0 || Tz < Tq || Tf0 < Tq) return FAC_ERR_INVALID;
+    for (int i = 0; i < 6; ++i)
+        for (int j = 0; j < 5; ++j)
+            if (!vq_host[i][j]) return FAC_ERR_INVALID;
+    std::vector<float> pack;
+    VqW v[6];
+    for (int i = 0; i < 6; ++i) v[i] = pack_vq_raw(pack, vq_host[i][0], vq_host[i][1], vq_host[i][2], vq_host[i][3], vq_host[i][4]);
+    cudaSetDevice(h->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* d = nullptr;
+    cudaError_t e = cudaMalloc(&d, pack.size() * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemcpy(d, pack.data(), pack.size() * sizeof(float), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); cudaFree(d); return FAC_ERR_CUDA; }
+    FaqParams fp;
+    fp.f0 = f0; fp.z = z;
+    for (int i = 0; i < 6; ++i)
+        fp.vq[i] = VqWeights{d + v[i].w_in, d + v[i].b_in, d + v[i].cb, d + v[i].cbn, d + v[i].cbn2, d + v[i].w_out, d + v[i].b_out};
+    fp.n_c = n_c;
+    fp.gamma_beta = gamma_beta;
+    fp.outs = outs; fp.zp = zp; fp.zc = zc; fp.zr = zr;
+    fp.codes_p = codes_p; fp.codes_c = codes_c; fp.codes_r = codes_r;
+    fp.sqerr = sqerr;
+    fp.B = B; fp.Tq = Tq; fp.Tz = Tz; fp.Tf0 = Tf0;
+    e = launch_fa_quantize(fp, st);
+    if (e == cudaSuccess) e = launch_vq_loss_reduce(sqerr, 6, B, Tq, losses2, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    cudaFree(d);
+    if (e != cudaSuccess) { h->err = std::string("fac_debug_fa_quantize: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
+    return FAC_OK;
+}
+
+int fac_debug_attention(fac_handle* h, const float* q, const float* k, const float* v, float* o, int B, int T,
+                        int heads, const int* valid_len, int force_stream, void* stream) {
+    if (!h || !q || !k || !v || !o || B <= 0 || T <= 0 || heads <= 0) return FAC_ERR_INVALID;
+    cudaSetDevice(h->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    cudaError_t e = launch_attention(q, k, v, o, B, T, heads, 256, valid_len, st, force_stream ? 1 : 0);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { h->err = std::string("fac_debug_attention: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
+    return FAC_OK;
+}
+
 int fac_set_option(fac_handle* h, const char* name, int value) {
     if (!h || !name) return FAC_ERR_INVALID;
     if (std::string(name) == "fuse_resunit") { h->fuse_res = value < 0 ? 0 : (value > 2 ? 2 : value); return FAC_OK; }

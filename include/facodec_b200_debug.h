@@ -84,6 +84,23 @@ long long fac_debug_convtr_pack(const float* w_host, int Cin, int Cout, int stri
                                 long long capacity_floats);
 int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, float* y,
                     void* stream);
+/* fa_quantize_kernel + vq_loss_reduce_kernel on caller-given features, the six VectorQuantizes and the AdaLN of
+ * FAquantizer.forward_v2 (synchronous).  DEVICE f0 [B][Tf0][1024], z [B][Tz][1024] (Tf0, Tz >= Tq: frame t of
+ * utterance b is row b*Tf0 + t / b*Tz + t), gamma_beta [B][2048].  vq_host[i] = HOST {in_w [8][1024], in_b [8],
+ * out_w [1024][8], out_b [1024], codebook [1024][8]} of VQ i = prosody, content 0, content 1, residual 0..2 (weights
+ * already weight-normed), packed as the product packs them.  DEVICE outputs as FaqParams: outs / zp / zc / zr
+ * [B][Tq][1024] (zp, zc, zr may be NULL), codes_p [B][1][Tq], codes_c [B][n_c][Tq], codes_r [B][3][Tq] int64,
+ * sqerr [6][B*Tq], losses2 [2]. */
+int fac_debug_fa_quantize(fac_handle* h, const float* f0, const float* z, const float* const vq_host[6][5],
+                          const float* gamma_beta, int n_c, int B, int Tq, int Tz, int Tf0, float* outs, float* zp,
+                          float* zc, float* zr, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* sqerr,
+                          float* losses2, void* stream);
+/* The StyleEncoder's self-attention (launch_attention, synchronous) on DEVICE channels-last q, k, v, o
+ * [B][T][heads*256]; valid_len DEVICE int [B] (keys and queries t >= valid_len[b] masked) or NULL.
+ * force_stream = 0 keeps launch_attention's choice (stored scores up to 200 KB of shared memory), 1 forces the
+ * kernel that recomputes the scores. */
+int fac_debug_attention(fac_handle* h, const float* q, const float* k, const float* v, float* o, int B, int T,
+                        int heads, const int* valid_len, int force_stream, void* stream);
 /* Registers (dst != NULL) or clears a named tap: the next forward copies that channels-last
  * intermediate into dst (DEVICE, up to capacity_floats).  Names: enc_conv0, enc_block1..4,
  * enc_lstm, mel80, f0_input, gamma_beta, dec_conv0, dec_lstm, dec_block1..4. */
