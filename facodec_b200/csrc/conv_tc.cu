@@ -57,47 +57,43 @@ template <int P> struct PrecT {
 __host__ __device__ constexpr int prec_kg(int P) { return P == P_TF32 ? 4 : 2; }
 __host__ __device__ constexpr int prec_planes(int P) { return P == P_F16S ? 1 : 2; }
 
-template <int NI, int NS>
-__device__ __forceinline__ void zero_acc(float (&a)[NS][NI / 2]) {
+template <int NI>
+__device__ __forceinline__ void zero_acc(float (&a)[NI / 2]) {
 #pragma unroll
-    for (int s = 0; s < NS; ++s)
-#pragma unroll
-        for (int i = 0; i < NI / 2; ++i) a[s][i] = 0.f;
+    for (int i = 0; i < NI / 2; ++i) a[i] = 0.f;
 }
 
-// One operand pair (A rows x K-pieces, B channels x K-pieces) of one chunk, all sub-tiles of this warpgroup.
-template <int P, int NI, int NS>
-__device__ __forceinline__ void mma_pass(float (&acc)[NS][NI / 2], int nsub, uint32_t a_addr, uint32_t a_lbo, uint32_t b_addr,
+// One operand pair (A rows x K-pieces, B channels x K-pieces) of one chunk: one wgmma per k-step over the warpgroup's
+// whole width.  No runtime condition may guard these: ptxas then fences every wgmma with its own warpgroup.arrive and
+// wait, and the chunk's MMAs run one after another instead of as one chained batch.
+template <int P, int NI>
+__device__ __forceinline__ void mma_pass(float (&acc)[NI / 2], uint32_t a_addr, uint32_t a_lbo, uint32_t b_addr,
                                          uint32_t b_lbo) {
 #pragma unroll
-    for (int ks = 0; ks < PrecT<P>::ksteps; ++ks) {
-        const uint64_t da = gdesc(a_addr + ks * 2 * a_lbo, a_lbo, 128);
-#pragma unroll
-        for (int s = 0; s < NS; ++s)
-            if (s < nsub) wgmma_ss<NI, PrecT<P>::kind>(acc[s], da, gdesc(b_addr + ks * 2 * b_lbo + s * NI * 16, b_lbo, 128));
-    }
+    for (int ks = 0; ks < PrecT<P>::ksteps; ++ks)
+        wgmma_ss<NI, PrecT<P>::kind>(acc, gdesc(a_addr + ks * 2 * a_lbo, a_lbo, 128), gdesc(b_addr + ks * 2 * b_lbo, b_lbo, 128));
 }
 
 struct Tile {
-    int row0, col0, nsub;     // this warpgroup's first tile row / channel, NI-wide sub-tiles
+    int row0, col0, nw;       // this warpgroup's first tile row / channel, its channel width NW
     int warp, lane;
 };
 
-// Accumulator fragment of wgmma m64nNI: register 4j + 2h + e of sub-tile s holds row 16*warp + lane/4 + 8h,
-// column s*NI + 8j + 2*(lane%4) + e.
-template <int NI, int NS, typename F>
-__device__ __forceinline__ void for_each_pair(const Tile& tl, const float (&acc)[NS][NI / 2], F&& f) {
+// Accumulator fragment of wgmma m64nNI: register 4j + 2h + e holds row 16*warp + lane/4 + 8h, column 8j + 2*(lane%4) + e.
+// GROUP < NI cuts the unrolled loop into blocks of GROUP columns at a branch on the runtime width, never taken (the
+// launcher picks NI == NW).  ptxas schedules each block on its own: the fused GEMM-1 epilogue (a Snake per element)
+// takes 224 registers at NI = 128 as one block, and <= 128 in blocks of 32 columns.
+template <int NI, int GROUP = NI, typename F>
+__device__ __forceinline__ void for_each_pair(const Tile& tl, const float (&acc)[NI / 2], F&& f) {
 #pragma unroll
-    for (int s = 0; s < NS; ++s) {
-        if (s >= tl.nsub) break;
+    for (int j = 0; j < NI / 8; ++j) {
+        if (j > 0 && (8 * j) % GROUP == 0 && 8 * j >= tl.nw) break;
 #pragma unroll
-        for (int j = 0; j < NI / 8; ++j)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = tl.row0 + 16 * tl.warp + (tl.lane >> 2) + 8 * h;
-                const int col = tl.col0 + s * NI + 8 * j + 2 * (tl.lane & 3);
-                f(row, col, acc[s][4 * j + 2 * h], acc[s][4 * j + 2 * h + 1]);
-            }
+        for (int h = 0; h < 2; ++h) {
+            const int row = tl.row0 + 16 * tl.warp + (tl.lane >> 2) + 8 * h;
+            const int col = tl.col0 + 8 * j + 2 * (tl.lane & 3);
+            f(row, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
     }
 }
 
@@ -109,15 +105,17 @@ __device__ __forceinline__ float act_out(int act, float v, float al, float ia) {
     return v;
 }
 
-// P1: split class of the layer's own GEMM; P2: of the fused GEMM 2 (P_NONE = not fused); NI: wgmma N per instruction;
-// MINB = 2: planned for two resident CTAs per SM (<= 128 registers, <= 64 accumulator columns per warpgroup);
+// P1: split class of the layer's own GEMM; P2: of the fused GEMM 2 (P_NONE = not fused); NI: wgmma N, the warpgroup's
+// whole channel width NW (NI / 2 accumulator registers per thread; NI <= 64 when promoted or MINB = 2, else <= 128);
+// MINB = 2: planned for two resident CTAs per SM (<= 128 registers);
 // TT: transposed formulation -- the weights are the wgmma A operand (64 output channels per warpgroup) and time is the
-// wgmma N dimension; the operand buffers and the weight blob are the same K-major layouts as the plain formulation.
+// wgmma N dimension (NI = 64 time steps); the operand buffers and the weight blob are the same K-major layouts as the
+// plain formulation.
 template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false>
 __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p) {
     constexpr bool FUSED = P2 != P_NONE;
     static_assert(!TT || (NI == 64 && !FUSED), "transposed tiles: <= 64 channels x 64 time steps per warpgroup");
-    constexpr int NS = (PROMO || MINB == 2 ? 64 : 128) / NI;   // sub-tiles per warpgroup (registers: <= 64 / 128 floats)
+    static_assert(NI % 16 == 0 && NI <= (PROMO || MINB == 2 ? 64 : 128), "accumulator registers: <= 64 / 128 columns");
     constexpr bool F16X2 = P1 == P_F16X2;
     constexpr bool DEC = P1 == P_BF16 || P1 == P_F16S;      // downstream of the VQ: SFU-sine Snake class
     using T1 = PrecT<P1>;
@@ -130,7 +128,7 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
     Tile tl;
     tl.row0 = p.MT == 2 ? 64 * wg : 0;
     tl.col0 = p.MT == 2 ? 0 : wg * NW;
-    tl.nsub = TT ? 1 : NW / NI;                             // transposed: one 64-step time sub-tile
+    tl.nw = NW;
     tl.warp = (tid >> 5) & 3;
     tl.lane = tid & 31;
     const int t0 = blockIdx.x * BM, ntile = blockIdx.y, b = blockIdx.z;
@@ -174,12 +172,12 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
     };
     produce(0);
 
-    float acc[NS][NI / 2];
-    float tmp[PROMO ? NS : 1][PROMO ? NI / 2 : 1];
-    float crs[F16X2 ? NS : 1][F16X2 ? NI / 2 : 1];
-    zero_acc<NI, NS>(acc);
-    if constexpr (PROMO) zero_acc<NI, NS>(tmp);
-    if constexpr (F16X2) zero_acc<NI, NS>(crs);
+    float acc[NI / 2];
+    float tmp[PROMO ? NI / 2 : 1];
+    float crs[F16X2 ? NI / 2 : 1];
+    zero_acc<NI>(acc);
+    if constexpr (PROMO) zero_acc<NI>(tmp);
+    if constexpr (F16X2) zero_acc<NI>(crs);
     const uint32_t a_lbo = (uint32_t)Rpad * 16, b_lbo = (uint32_t)N * 16;
     const uint32_t abase = smem_u32(abuf), wbase = smem_u32(wbuf), a2base = smem_u32(a2buf);
     const int BM2 = BM;
@@ -187,13 +185,11 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
     auto promote = [&]() {
         if constexpr (PROMO) {
 #pragma unroll
-            for (int s = 0; s < NS; ++s)
-#pragma unroll
-                for (int i = 0; i < NI / 2; ++i) {
-                    if constexpr (F16X2) { acc[s][i] += tmp[s][i] + crs[s][i] * kLoUnscale; crs[s][i] = 0.f; }
-                    else acc[s][i] += tmp[s][i];
-                    tmp[s][i] = 0.f;
-                }
+            for (int i = 0; i < NI / 2; ++i) {
+                if constexpr (F16X2) { acc[i] += tmp[i] + crs[i] * kLoUnscale; crs[i] = 0.f; }
+                else acc[i] += tmp[i];
+                tmp[i] = 0.f;
+            }
         }
     };
 
@@ -212,23 +208,23 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
                 const uint32_t ahi = a0 + (uint32_t)(tap * dil) * 16, alo = ahi + a_plane;
                 const uint32_t bhi = b0 + (uint32_t)tap * T1::planes * T1::KG * b_lbo, blo = bhi + T1::KG * b_lbo;
                 if constexpr (TT) {         // D[channel][time]: weights are the A operand, activations the B operand
-                    mma_pass<P1, NI, NS>(tmp, 1, bhi, b_lbo, ahi, a_lbo);
-                    mma_pass<P1, NI, NS>(crs, 1, bhi, b_lbo, alo, a_lbo);
-                    mma_pass<P1, NI, NS>(crs, 1, blo, b_lbo, ahi, a_lbo);
+                    mma_pass<P1, NI>(tmp, bhi, b_lbo, ahi, a_lbo);
+                    mma_pass<P1, NI>(crs, bhi, b_lbo, alo, a_lbo);
+                    mma_pass<P1, NI>(crs, blo, b_lbo, ahi, a_lbo);
                 } else if constexpr (P1 == P_F16S) {
-                    mma_pass<P1, NI, NS>(acc, tl.nsub, ahi, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI>(acc, ahi, a_lbo, bhi, b_lbo);
                 } else if constexpr (F16X2) {
-                    mma_pass<P1, NI, NS>(tmp, tl.nsub, ahi, a_lbo, bhi, b_lbo);
-                    mma_pass<P1, NI, NS>(crs, tl.nsub, ahi, a_lbo, blo, b_lbo);
-                    mma_pass<P1, NI, NS>(crs, tl.nsub, alo, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI>(tmp, ahi, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI>(crs, ahi, a_lbo, blo, b_lbo);
+                    mma_pass<P1, NI>(crs, alo, a_lbo, bhi, b_lbo);
                 } else if constexpr (PROMO) {
-                    mma_pass<P1, NI, NS>(tmp, tl.nsub, ahi, a_lbo, bhi, b_lbo);
-                    mma_pass<P1, NI, NS>(tmp, tl.nsub, ahi, a_lbo, blo, b_lbo);
-                    mma_pass<P1, NI, NS>(tmp, tl.nsub, alo, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI>(tmp, ahi, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI>(tmp, ahi, a_lbo, blo, b_lbo);
+                    mma_pass<P1, NI>(tmp, alo, a_lbo, bhi, b_lbo);
                 } else {
-                    mma_pass<P1, NI, NS>(acc, tl.nsub, ahi, a_lbo, bhi, b_lbo);
-                    mma_pass<P1, NI, NS>(acc, tl.nsub, ahi, a_lbo, blo, b_lbo);
-                    mma_pass<P1, NI, NS>(acc, tl.nsub, alo, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI>(acc, ahi, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI>(acc, ahi, a_lbo, blo, b_lbo);
+                    mma_pass<P1, NI>(acc, alo, a_lbo, bhi, b_lbo);
                 }
             }
             wg_commit();
@@ -240,7 +236,7 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
                     // GEMM-2 operand snake2(D1 + b7), split, K-major [plane][k-piece][BM rows][16 B]
                     constexpr int KG2 = prec_kg(P2 < 0 ? 0 : P2);
                     const uint32_t a2_plane = (uint32_t)(p.nchunk2 * KG2) * BM2 * 16;
-                    for_each_pair<NI, NS>(tl, acc, [&](int row, int col, float v0, float v1) {
+                    for_each_pair<NI, 32>(tl, acc, [&](int row, int col, float v0, float v1) {
                         const float2 bi = __ldg(reinterpret_cast<const float2*>(p.bias + col));
                         const float2 al = __ldg(reinterpret_cast<const float2*>(p.out_alpha + col));
                         const float2 ia = __ldg(reinterpret_cast<const float2*>(p.out_inv_alpha + col));
@@ -261,7 +257,7 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
                         }
                     });
                     fence_proxy_async();
-                    zero_acc<NI, NS>(acc);
+                    zero_acc<NI>(acc);
                 }
             }
         } else if constexpr (FUSED) {
@@ -271,9 +267,9 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
             const uint32_t a2_plane = (uint32_t)(p.nchunk2 * KG2) * BM2 * 16, a2_lbo = (uint32_t)BM2 * 16;
             const uint32_t ahi = a2base + ((uint32_t)(c2 * KG2) * BM2 + tl.row0) * 16, alo = ahi + a2_plane;
             const uint32_t bhi = wslot + (uint32_t)tl.col0 * 16, blo = bhi + KG2 * b_lbo;
-            mma_pass<P2x, NI, NS>(acc, tl.nsub, ahi, a2_lbo, bhi, b_lbo);
-            mma_pass<P2x, NI, NS>(acc, tl.nsub, ahi, a2_lbo, blo, b_lbo);
-            mma_pass<P2x, NI, NS>(acc, tl.nsub, alo, a2_lbo, bhi, b_lbo);
+            mma_pass<P2x, NI>(acc, ahi, a2_lbo, bhi, b_lbo);
+            mma_pass<P2x, NI>(acc, ahi, a2_lbo, blo, b_lbo);
+            mma_pass<P2x, NI>(acc, alo, a2_lbo, bhi, b_lbo);
             wg_commit();
             wg_wait_all();
         }
@@ -289,7 +285,7 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
     const float* bi_p = bias ? bias + (size_t)ntile * N : nullptr;
     if constexpr (TT) {
         // fragment row = output channel, column = time step
-        for_each_pair<NI, NS>(tl, acc, [&](int r, int c, float v0, float v1) {
+        for_each_pair<NI>(tl, acc, [&](int r, int c, float v0, float v1) {
             if (r - tl.row0 >= NW) return;           // A-operand rows past this warpgroup's channels
             const int co = tl.col0 + (r - tl.row0), tf = tl.row0 + (c - tl.col0);
             const float bi = bi_p ? __ldg(bi_p + co) : 0.f;
@@ -306,7 +302,7 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
         });
         return;
     }
-    for_each_pair<NI, NS>(tl, acc, [&](int row, int col, float v0, float v1) {
+    for_each_pair<NI>(tl, acc, [&](int row, int col, float v0, float v1) {
         const int t = t0 + row;
         if (t >= p.Tout) return;
         if (bi_p) { const float2 bi = __ldg(reinterpret_cast<const float2*>(bi_p + col)); v0 += bi.x; v1 += bi.y; }
@@ -519,16 +515,18 @@ cudaError_t launch_one(const TcConvParams& p, dim3 grid, cudaStream_t st) {
     conv_tc_kernel<P1, P2, PROMO, NI, MINB, TT><<<grid, kThreads, p.smem_bytes, st>>>(p);
     return cudaGetLastError();
 }
-template <int P1, int P2, bool PROMO, int MINB = 1>
-cudaError_t launch_ni(const TcConvParams& p, dim3 grid, cudaStream_t st) {
+// The kernel's wgmma N is the warpgroup's whole channel width NW, so there is one instantiation per width tc_conv_plan
+// can return for the class: 16, 32, ..., 128, or up to 64 when promoted or planned for two CTAs per SM.
+template <int P1, int P2, bool PROMO, int MINB = 1, int NI = (PROMO || MINB == 2 ? 64 : 128)>
+cudaError_t launch_nw(const TcConvParams& p, dim3 grid, cudaStream_t st) {
     const int NW = p.MT == 2 ? p.N : p.N / 2;
-    if (NW % 64 == 0) return launch_one<P1, P2, PROMO, 64, MINB>(p, grid, st);
-    if (NW % 32 == 0) return launch_one<P1, P2, PROMO, 32, MINB>(p, grid, st);
-    return launch_one<P1, P2, PROMO, 16, MINB>(p, grid, st);
+    if (NW == NI) return launch_one<P1, P2, PROMO, NI, MINB>(p, grid, st);
+    if constexpr (NI > 16) return launch_nw<P1, P2, PROMO, MINB, NI - 16>(p, grid, st);
+    else return cudaErrorInvalidValue;
 }
 template <int P1, int P2>
 cudaError_t launch_occ(const TcConvParams& p, dim3 grid, cudaStream_t st) {
-    return p.occ2 ? launch_ni<P1, P2, false, 2>(p, grid, st) : launch_ni<P1, P2, false, 1>(p, grid, st);
+    return p.occ2 ? launch_nw<P1, P2, false, 2>(p, grid, st) : launch_nw<P1, P2, false, 1>(p, grid, st);
 }
 }  // namespace
 
@@ -544,7 +542,7 @@ cudaError_t launch_conv_tc(const TcConvParams& p, cudaStream_t st) {
         return launch_occ<P_TF32, P_TF32>(p, grid, st);
     }
     if (p.tt) return launch_one<P_F16X2, P_NONE, true, 64, 1, true>(p, grid, st);
-    if (p.promoted) return P1 == P_F16X2 ? launch_ni<P_F16X2, P_NONE, true>(p, grid, st) : launch_ni<P_TF32, P_NONE, true>(p, grid, st);
+    if (p.promoted) return P1 == P_F16X2 ? launch_nw<P_F16X2, P_NONE, true>(p, grid, st) : launch_nw<P_TF32, P_NONE, true>(p, grid, st);
     if (P1 == P_F16S) return launch_occ<P_F16S, P_NONE>(p, grid, st);
     if (P1 == P_BF16) return launch_occ<P_BF16, P_NONE>(p, grid, st);
     return launch_occ<P_TF32, P_NONE>(p, grid, st);

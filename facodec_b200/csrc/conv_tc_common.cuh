@@ -85,53 +85,71 @@ __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.s
 
 enum WgKind { WG_TF32 = 0, WG_BF16 = 1, WG_F16 = 2 };
 
-#define FAC_R16(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
-    "+f"(d[o + 6]), "+f"(d[o + 7]), "+f"(d[o + 8]), "+f"(d[o + 9]), "+f"(d[o + 10]), "+f"(d[o + 11]), "+f"(d[o + 12]), \
-    "+f"(d[o + 13]), "+f"(d[o + 14]), "+f"(d[o + 15])
-#define FAC_R8(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
-    "+f"(d[o + 6]), "+f"(d[o + 7])
-#define FAC_D8 "{%0, %1, %2, %3, %4, %5, %6, %7}"
-#define FAC_D16 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}"
-#define FAC_D32 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
-    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
-
 // D[64 x NI] += A[64 x K] * B[NI x K]^T, both operands K-major in shared memory; K = 16 (f16 / bf16) or 8 (tf32).
+// Defined for NI = 16, 32, ..., 128 by FAC_WGMMA_SS below; any other NI fails to compile.
 template <int NI, int KIND>
 __device__ __forceinline__ void wgmma_ss(float (&d)[NI / 2], uint64_t da, uint64_t db) {
-    static_assert(NI == 16 || NI == 32 || NI == 64, "instruction N");
-    if constexpr (NI == 64 && KIND == WG_TF32)
-        asm volatile("wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " FAC_D32 ", %32, %33, 1, 1, 1;"
-                     : FAC_R16(0), FAC_R16(16) : "l"(da), "l"(db));
-    else if constexpr (NI == 64 && KIND == WG_BF16)
-        asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " FAC_D32 ", %32, %33, 1, 1, 1, 0, 0;"
-                     : FAC_R16(0), FAC_R16(16) : "l"(da), "l"(db));
-    else if constexpr (NI == 64 && KIND == WG_F16)
-        asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " FAC_D32 ", %32, %33, 1, 1, 1, 0, 0;"
-                     : FAC_R16(0), FAC_R16(16) : "l"(da), "l"(db));
-    else if constexpr (NI == 32 && KIND == WG_TF32)
-        asm volatile("wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 " FAC_D16 ", %16, %17, 1, 1, 1;"
-                     : FAC_R16(0) : "l"(da), "l"(db));
-    else if constexpr (NI == 32 && KIND == WG_BF16)
-        asm volatile("wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 " FAC_D16 ", %16, %17, 1, 1, 1, 0, 0;"
-                     : FAC_R16(0) : "l"(da), "l"(db));
-    else if constexpr (NI == 32)
-        asm volatile("wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 " FAC_D16 ", %16, %17, 1, 1, 1, 0, 0;"
-                     : FAC_R16(0) : "l"(da), "l"(db));
-    else if constexpr (KIND == WG_TF32)
-        asm volatile("wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 " FAC_D8 ", %8, %9, 1, 1, 1;"
-                     : FAC_R8(0) : "l"(da), "l"(db));
-    else if constexpr (KIND == WG_BF16)
-        asm volatile("wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 " FAC_D8 ", %8, %9, 1, 1, 1, 0, 0;"
-                     : FAC_R8(0) : "l"(da), "l"(db));
-    else
-        asm volatile("wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 " FAC_D8 ", %8, %9, 1, 1, 1, 0, 0;"
-                     : FAC_R8(0) : "l"(da), "l"(db));
+    static_assert(NI < 0, "wgmma_ss: instruction N must be a multiple of 16 in [16, 128]");
 }
+
+// The m64nNI accumulator is NI/2 registers per thread, listed in groups of 8: FAC_Sg is the asm operand list
+// "%0, ..., %(8g-1)" and FAC_Cg the matching "+f" constraints on d[0 .. 8g-1].
+#define FAC_S1 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define FAC_S2 FAC_S1 ", %8, %9, %10, %11, %12, %13, %14, %15"
+#define FAC_S3 FAC_S2 ", %16, %17, %18, %19, %20, %21, %22, %23"
+#define FAC_S4 FAC_S3 ", %24, %25, %26, %27, %28, %29, %30, %31"
+#define FAC_S5 FAC_S4 ", %32, %33, %34, %35, %36, %37, %38, %39"
+#define FAC_S6 FAC_S5 ", %40, %41, %42, %43, %44, %45, %46, %47"
+#define FAC_S7 FAC_S6 ", %48, %49, %50, %51, %52, %53, %54, %55"
+#define FAC_S8 FAC_S7 ", %56, %57, %58, %59, %60, %61, %62, %63"
+#define FAC_R8(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
+    "+f"(d[o + 6]), "+f"(d[o + 7])
+#define FAC_C1 FAC_R8(0)
+#define FAC_C2 FAC_C1, FAC_R8(8)
+#define FAC_C3 FAC_C2, FAC_R8(16)
+#define FAC_C4 FAC_C3, FAC_R8(24)
+#define FAC_C5 FAC_C4, FAC_R8(32)
+#define FAC_C6 FAC_C5, FAC_R8(40)
+#define FAC_C7 FAC_C6, FAC_R8(48)
+#define FAC_C8 FAC_C7, FAC_R8(56)
+// One specialization per kind for N = 16 * G; the descriptors are operands %(8G) and %(8G + 1), spelled out as DESC.
+#define FAC_WGMMA_KIND(N, G, DESC, KIND, SHAPE, TAIL)                                                                   \
+    template <>                                                                                                      \
+    __device__ __forceinline__ void wgmma_ss<N, KIND>(float (&d)[N / 2], uint64_t da, uint64_t db) {                  \
+        asm volatile("wgmma.mma_async.sync.aligned.m64n" #N SHAPE " {" FAC_S##G "}, " DESC ", " TAIL ";"              \
+                     : FAC_C##G : "l"(da), "l"(db));                                                                 \
+    }
+#define FAC_WGMMA_SS(N, G, DESC)                                                                                     \
+    FAC_WGMMA_KIND(N, G, DESC, WG_TF32, "k8.f32.tf32.tf32", "1, 1, 1")                                                \
+    FAC_WGMMA_KIND(N, G, DESC, WG_BF16, "k16.f32.bf16.bf16", "1, 1, 1, 0, 0")                                         \
+    FAC_WGMMA_KIND(N, G, DESC, WG_F16, "k16.f32.f16.f16", "1, 1, 1, 0, 0")
+FAC_WGMMA_SS(16, 1, "%8, %9")
+FAC_WGMMA_SS(32, 2, "%16, %17")
+FAC_WGMMA_SS(48, 3, "%24, %25")
+FAC_WGMMA_SS(64, 4, "%32, %33")
+FAC_WGMMA_SS(80, 5, "%40, %41")
+FAC_WGMMA_SS(96, 6, "%48, %49")
+FAC_WGMMA_SS(112, 7, "%56, %57")
+FAC_WGMMA_SS(128, 8, "%64, %65")
+#undef FAC_WGMMA_SS
+#undef FAC_WGMMA_KIND
 #undef FAC_R8
-#undef FAC_D8
-#undef FAC_R16
-#undef FAC_D16
-#undef FAC_D32
+#undef FAC_S1
+#undef FAC_S2
+#undef FAC_S3
+#undef FAC_S4
+#undef FAC_S5
+#undef FAC_S6
+#undef FAC_S7
+#undef FAC_S8
+#undef FAC_C1
+#undef FAC_C2
+#undef FAC_C3
+#undef FAC_C4
+#undef FAC_C5
+#undef FAC_C6
+#undef FAC_C7
+#undef FAC_C8
 
 __device__ __forceinline__ float to_tf32(float x) {
     uint32_t r;
