@@ -59,6 +59,12 @@ class DACFile:
             raise RuntimeError(f"Given file {path} can't be loaded with this version of descript-audio-codec.")
         return cls(codes=torch.from_numpy(blob["codes"].astype(int)), **meta)
 
+    def unpack(self):
+        """The [codes_p, codes_c, codes_r] list (int64, CPU) that ``Codec.decode`` takes, via :func:`unpack_codes`; the
+        number of content rows follows from the codebook axis (1 + n_c + 3).  The timbre is not part of the format: it
+        travels with the caller."""
+        return unpack_codes(self.codes.to(torch.int64), self.codes.shape[1] - 4)
+
 
 def pack_codes(codes: Sequence[torch.Tensor]) -> torch.Tensor:
     """[codes_p [B,1,T'], codes_c [B,n_c,T'], codes_r [B,3,T']] -> one ``[B, 1 + n_c + 3, T']`` int64 tensor."""

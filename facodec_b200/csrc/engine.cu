@@ -1075,6 +1075,19 @@ struct QuantOut {
 // StyleEncoder -> timbre_linear) and the prosody features (mel[:, :20] -> melspec_linear -> WN -> melspec_linear2).  Nothing
 // here reads the encoder's latents, so fac_codec_forward runs it on a second stream beside the encoder.
 struct QuantFront { float* gb; float* f0; int Tm; };
+
+// gamma | beta = timbre_linear(timbre) (modules/quantize.py:444-445): [B][2048] in workspace.  Run with the promoted
+// quantizer-side kernel, so that decoding from codes sees the same gamma / beta as the forward.
+float* timbre_gamma_beta(Ctx& c, const float* timbre, int B) {
+    const bool was_critical = c.vq_critical;
+    c.vq_critical = true;
+    float* gb = c.alloc<float>((size_t)B * 2048);
+    run_conv(c, c.h->qw.timbre_linear, timbre, gb, 1, B, B, ConvOpts(), "timbre_linear");
+    c.tap("gamma_beta", gb, (size_t)B * 2048);
+    c.vq_critical = was_critical;
+    return gb;
+}
+
 QuantFront quantizer_front(Ctx& c, const float* wave, int B, int T, const float* full_waves, int T_full, const int64_t* wave_lens,
                            float* timbre) {
     const QuantW& q = c.h->qw;
@@ -1097,9 +1110,7 @@ QuantFront quantizer_front(Ctx& c, const float* wave, int B, int T, const float*
     } else {
         style_encoder(c, mel, B, Tm, nullptr, timbre);
     }
-    float* gb = c.alloc<float>((size_t)B * 2048);
-    run_conv(c, q.timbre_linear, timbre, gb, 1, B, B, ConvOpts(), "timbre_linear");
-    c.tap("gamma_beta", gb, (size_t)B * 2048);
+    float* gb = timbre_gamma_beta(c, timbre, B);
     // --- prosody branch: mel[:, :20] -> melspec_linear -> WN -> melspec_linear2 ---
     float* px = c.alloc<float>((size_t)B * Tm * 256);
     float* pin = c.alloc<float>((size_t)B * Tm * 512);
@@ -1172,6 +1183,38 @@ QuantOut quantizer_forward(Ctx& c, const float* z_cl, const float* wave, int B, 
     c.check(launch_fa_quantize(fp, c.st), "fa_quantize");
     c.end();
     c.check(launch_vq_loss_reduce(sqerr, 6, B, Tq, losses2 ? losses2 : loss_ws, c.st), "vq_loss");
+    return out;
+}
+
+// FAquantizer from codes (the composition of ResidualVectorQuantize.from_codes, dac/nn/quantize.py:200-220, per RVQ and
+// the AdaLN of modules/quantize.py:444-449): codes_p [B][1][T], codes_c [B][n_c][T], codes_r [B][n_r][T] int64 (device),
+// timbre [B][1024] -> channels-last outs [B][T][1024] in workspace; the parts too when want_parts.
+QuantOut dequantize_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes_c, int n_c, const int64_t* codes_r, int n_r,
+                            const float* timbre, int B, int T, bool want_parts) {
+    const QuantW& q = c.h->qw;
+    float* gb = timbre_gamma_beta(c, timbre, B);
+    QuantOut out;
+    out.Tq = T;
+    out.outs_cl = c.alloc<float>((size_t)B * T * 1024);
+    out.zp_cl = want_parts ? c.alloc<float>((size_t)B * T * 1024) : nullptr;
+    out.zc_cl = want_parts ? c.alloc<float>((size_t)B * T * 1024) : nullptr;
+    out.zr_cl = want_parts ? c.alloc<float>((size_t)B * T * 1024) : nullptr;
+    if (c.dry) return out;
+    DeqParams dp;
+    dp.codes_p = codes_p; dp.codes_c = codes_c; dp.codes_r = codes_r;
+    dp.n_c = n_c; dp.n_r = n_r;
+    for (int i = 0; i < 6; ++i) {
+        const VqW& v = q.vq[i];
+        dp.vq[i] = VqWeights{c.W(v.w_in), c.W(v.b_in), c.W(v.cb), c.W(v.cbn), c.W(v.cbn2), c.W(v.w_out), c.W(v.b_out)};
+    }
+    dp.gamma_beta = gb;
+    dp.outs = out.outs_cl; dp.zp = out.zp_cl; dp.zc = out.zc_cl; dp.zr = out.zr_cl;
+    dp.B = B; dp.T = T;
+    // codes in + outs out; the 6 x 32 KB of out_proj weights and the gathered codebook rows stay cache-resident
+    const double frames = (double)B * T, ncodes = 1 + n_c + n_r;
+    c.begin("dequantize", 2.0 * frames * ncodes * 8.0 * 1024, frames * (8.0 * ncodes + 4.0 * 1024 * (want_parts ? 4 : 1)));
+    c.check(launch_dequantize(dp, c.st), "dequantize");
+    c.end();
     return out;
 }
 
@@ -1375,21 +1418,85 @@ int fac_quantize(fac_handle* h, const float* z, const float* wave, int B, int T,
     });
 }
 
+}  // extern "C"
+
+namespace {
+// The compress half of reconstruct.py:56-61: encoder -> quantizer(n_c), with the waveform-only quantizer front forked
+// beside the encoder.  Returns the channels-last AdaLN output the decoder reads.
+QuantOut codec_encode(Ctx& c, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r,
+                      float* timbre) {
+    int Tz = fac_encode_frames(T);
+    float* zcl = c.alloc<float>((size_t)B * Tz * LATENT);
+    float* timbre_buf = timbre ? timbre : c.alloc<float>((size_t)B * 1024);
+    QuantFront fr;
+    const bool forked = fork_front(c, fr, x, B, T, timbre_buf);
+    encoder_forward(c, x, B, T, zcl, false);
+    if (forked) join_front(c);
+    return quantizer_forward(c, zcl, x, B, T, Tz, n_c, nullptr, 0, nullptr, nullptr, timbre_buf, codes_p, codes_c, codes_r,
+                             false, forked ? &fr : nullptr);
+}
+
+// Arguments of the decode-from-codes entry points: 1 prosody row, 1..2 content rows, 0..3 residual rows (codes_r unread
+// when there are none), timbre [B][1024].
+bool bad_codes_args(const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r, int n_r_rows,
+                    const float* timbre, int B, int T) {
+    return !codes_p || !codes_c || !timbre || n_c_rows < 1 || n_c_rows > 2 || n_r_rows < 0 || n_r_rows > 3 ||
+           (n_r_rows > 0 && !codes_r) || B <= 0 || T <= 0;
+}
+}  // namespace
+
+extern "C" {
+
 int fac_codec_forward(fac_handle* h, const float* x, int B, int T, int n_c, float* y, int64_t* codes_p,
                       int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream) {
     for (int m = 0; m < 3; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
     if (!x || !y || B <= 0 || T <= N_FFT / 2 || n_c < 1 || n_c > 2) { h->err = "fac_codec_forward: bad arguments"; return FAC_ERR_INVALID; }
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-        int Tz = fac_encode_frames(T);
-        float* zcl = c.alloc<float>((size_t)B * Tz * LATENT);
-        float* timbre_buf = timbre ? timbre : c.alloc<float>((size_t)B * 1024);
-        QuantFront fr;
-        const bool forked = fork_front(c, fr, x, B, T, timbre_buf);
-        encoder_forward(c, x, B, T, zcl, false);
-        if (forked) join_front(c);
-        QuantOut o = quantizer_forward(c, zcl, x, B, T, Tz, n_c, nullptr, 0, nullptr, nullptr, timbre_buf, codes_p,
-                                       codes_c, codes_r, false, forked ? &fr : nullptr);
+        QuantOut o = codec_encode(c, x, B, T, n_c, codes_p, codes_c, codes_r, timbre);
         decoder_forward(c, h->dec, o.outs_cl, B, o.Tq, y);
+    });
+}
+
+int fac_codec_encode(fac_handle* h, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
+                     int64_t* codes_r, float* timbre, void* stream) {
+    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    if (!x || !codes_p || !codes_c || !codes_r || B <= 0 || T <= N_FFT / 2 || n_c < 1 || n_c > 2) {
+        h->err = "fac_codec_encode: bad arguments";
+        return FAC_ERR_INVALID;
+    }
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { codec_encode(c, x, B, T, n_c, codes_p, codes_c, codes_r, timbre); });
+}
+
+int fac_dequantize(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
+                   int n_r_rows, const float* timbre, int B, int T, float* outs, float* zp, float* zc, float* zr, void* stream) {
+    int rc = check_ready(h, FAC_QUANTIZER);
+    if (rc) return rc;
+    if (!outs || bad_codes_args(codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T)) {
+        h->err = "fac_dequantize: bad arguments (1 <= content rows <= 2, 0 <= residual rows <= 3)";
+        return FAC_ERR_INVALID;
+    }
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        QuantOut o = dequantize_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T, zp || zc || zr);
+        if (c.dry) return;
+        c.check(launch_transpose(o.outs_cl, outs, B, T, LATENT, c.st), "deq.outs_T");
+        if (zp) c.check(launch_transpose(o.zp_cl, zp, B, T, LATENT, c.st), "deq.zp_T");
+        if (zc) c.check(launch_transpose(o.zc_cl, zc, B, T, LATENT, c.st), "deq.zc_T");
+        if (zr) c.check(launch_transpose(o.zr_cl, zr, B, T, LATENT, c.st), "deq.zr_T");
+    });
+}
+
+int fac_codes_decode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
+                     int n_r_rows, const float* timbre, int B, int T, float* y, void* stream) {
+    int rc = check_ready(h, FAC_QUANTIZER);
+    if (!rc) rc = check_ready(h, FAC_DECODER);
+    if (rc) return rc;
+    if (!y || bad_codes_args(codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T)) {
+        h->err = "fac_codes_decode: bad arguments (1 <= content rows <= 2, 0 <= residual rows <= 3)";
+        return FAC_ERR_INVALID;
+    }
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        QuantOut o = dequantize_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T, false);
+        decoder_forward(c, h->dec, o.outs_cl, B, T, y);
     });
 }
 
@@ -1580,18 +1687,23 @@ int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float
     return rc;
 }
 
-int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, float* y, void* stream) {
+}  // extern "C"
+
+namespace {
+// The body of fac_stream_decode / fac_stream_decode_codes: `latents(c, B)` returns the chunk's channels-last latents
+// [B][Fc][1024] (transposed from the caller's z, or dequantized from codes); the stream state is the same either way.
+template <typename F>
+int stream_decode(fac_handle* h, int stream_id, int Fc, float* y, void* stream, const char* who, F latents) {
     int rc = check_ready(h, FAC_DECODER);
     if (rc) return rc;
-    if (stream_id < 0 || stream_id >= (int)h->streams.size() || !h->streams[stream_id]->alive || !z || !y) { h->err = "fac_stream_decode: bad arguments"; return FAC_ERR_INVALID; }
+    if (stream_id < 0 || stream_id >= (int)h->streams.size() || !h->streams[stream_id]->alive || !y) { h->err = std::string(who) + ": bad arguments"; return FAC_ERR_INVALID; }
     fac_handle::Stream& s = *h->streams[stream_id];
-    if (Fc <= 0 || (s.dec_frames == 0 && Fc < kStreamMinFirst)) { h->err = "fac_stream_decode: the first chunk needs at least 10 frames"; return FAC_ERR_INVALID; }
-    if (!h->lstm_v2 || !h->dec_bf16 || !h->dec_lstm_fp16 || !h->dec.lstm.has2[0]) { h->err = "fac_stream_decode: needs the resident-W LSTM kernel"; return FAC_ERR_UNSUPPORTED; }
+    if (Fc <= 0 || (s.dec_frames == 0 && Fc < kStreamMinFirst)) { h->err = std::string(who) + ": the first chunk needs at least 10 frames"; return FAC_ERR_INVALID; }
+    if (!h->lstm_v2 || !h->dec_bf16 || !h->dec_lstm_fp16 || !h->dec.lstm.has2[0]) { h->err = std::string(who) + ": needs the resident-W LSTM kernel"; return FAC_ERR_UNSUPPORTED; }
     const int B = s.B, zh = s.z_hist_len, dh = s.dy_hist_len;
     rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
         const DecW& d = h->dec;
-        float* znew = c.alloc<float>((size_t)B * Fc * LATENT);
-        if (!c.dry) c.check(launch_transpose(z, znew, B, LATENT, Fc, c.st), "dec.z_transpose");
+        const float* znew = latents(c, B);
         float* zw = c.alloc<float>((size_t)B * (zh + Fc) * LATENT);
         copy_rows(c, zw, zh + Fc, s.z_hist, 6, 0, zh, LATENT, B, "stream.zh");
         copy_rows(c, zw + (size_t)zh * LATENT, zh + Fc, znew, Fc, 0, Fc, LATENT, B, "stream.zc");
@@ -1626,6 +1738,34 @@ int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, floa
         s.dec_frames += Fc;
     }
     return rc;
+}
+}  // namespace
+
+extern "C" {
+
+int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, float* y, void* stream) {
+    int rc = check_ready(h, FAC_DECODER);
+    if (rc) return rc;
+    if (!z) { h->err = "fac_stream_decode: bad arguments"; return FAC_ERR_INVALID; }
+    return stream_decode(h, stream_id, Fc, y, stream, "fac_stream_decode", [&](Ctx& c, int B) {
+        float* znew = c.alloc<float>((size_t)B * Fc * LATENT);
+        if (!c.dry) c.check(launch_transpose(z, znew, B, LATENT, Fc, c.st), "dec.z_transpose");
+        return znew;
+    });
+}
+
+int fac_stream_decode_codes(fac_handle* h, int stream_id, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows,
+                            const int64_t* codes_r, int n_r_rows, const float* timbre, int Fc, float* y, void* stream) {
+    int rc = check_ready(h, FAC_QUANTIZER);
+    if (rc) return rc;
+    if (stream_id < 0 || stream_id >= (int)h->streams.size() || !h->streams[stream_id]->alive ||
+        bad_codes_args(codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, h->streams[stream_id]->B, Fc)) {
+        h->err = "fac_stream_decode_codes: bad arguments (1 <= content rows <= 2, 0 <= residual rows <= 3)";
+        return FAC_ERR_INVALID;
+    }
+    return stream_decode(h, stream_id, Fc, y, stream, "fac_stream_decode_codes", [&](Ctx& c, int B) {
+        return (const float*)dequantize_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, Fc, false).outs_cl;
+    });
 }
 
 // meldataset.py:37-47 preprocess: torchaudio MelSpectrogram(n_mels=80, n_fft=2048, win_length=1200, hop_length=300) with

@@ -129,6 +129,19 @@ struct FaqParams {
     int B = 0, Tq = 0, Tz = 0, Tf0 = 0;   // Tz / Tf0 = frames per utterance of z / f0 (>= Tq)
 };
 cudaError_t launch_fa_quantize(const FaqParams& p, cudaStream_t st);
+// FAquantizer from codes: the same six VectorQuantizes' out_proj(codebook[code]) + the AdaLN, no search
+struct DeqParams {
+    const int64_t* codes_p = nullptr;   // [B][1][T]
+    const int64_t* codes_c = nullptr;   // [B][n_c][T], n_c = 1 or 2
+    const int64_t* codes_r = nullptr;   // [B][n_r][T], n_r = 0..3 (unread when 0)
+    int n_c = 1, n_r = 3;
+    VqWeights vq[6];                    // as FaqParams
+    const float* gamma_beta = nullptr;  // [B][2048] timbre_linear(timbre)
+    float* outs = nullptr;              // [B][T][1024]
+    float* zp = nullptr, *zc = nullptr, *zr = nullptr;  // [B][T][1024] each (may be null)
+    int B = 0, T = 0;
+};
+cudaError_t launch_dequantize(const DeqParams& p, cudaStream_t st);
 // losses[0] = commitment, losses[1] = codebook (identical in forward), from sqerr
 cudaError_t launch_vq_loss_reduce(const float* sqerr, int nq, int B, int Tq, float* losses2, cudaStream_t st);
 

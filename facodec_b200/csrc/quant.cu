@@ -31,6 +31,47 @@ __device__ __forceinline__ void store_frame(float* __restrict__ p, const float (
         *reinterpret_cast<float4*>(p + i * 128 + lane * 4) = make_float4(v[i * 4], v[i * 4 + 1], v[i * 4 + 2], v[i * 4 + 3]);
 }
 
+// out = b_out + w_out zq (the 8 -> 1024 out_proj): per channel one FMA chain over k = 0..7 starting from the bias.
+__device__ __forceinline__ void out_proj(const VqWeights& W, const float (&zq)[VQ_CD], float (&out)[32], int lane) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        float4 o = __ldg(reinterpret_cast<const float4*>(W.b_out + i * 128 + lane * 4));
+#pragma unroll
+        for (int k = 0; k < VQ_CD; ++k) {
+            float4 w = __ldg(reinterpret_cast<const float4*>(W.w_out + k * VQ_D + i * 128 + lane * 4));
+            o.x = fmaf(w.x, zq[k], o.x);
+            o.y = fmaf(w.y, zq[k], o.y);
+            o.z = fmaf(w.z, zq[k], o.z);
+            o.w = fmaf(w.w, zq[k], o.w);
+        }
+        out[i * 4] = o.x; out[i * 4 + 1] = o.y; out[i * 4 + 2] = o.z; out[i * 4 + 3] = o.w;
+    }
+}
+
+// In place: v = LayerNorm(v) * gamma + beta (timbre_norm = LayerNorm(1024, no affine), eps 1e-5; gb = [gamma | beta]).
+__device__ __forceinline__ void adaln(float (&v)[32], const float* __restrict__ gb, int lane) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s += v[i];
+    float mean = warp_sum(s) * (1.0f / VQ_D);
+    float var = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+        float d = v[i] - mean;
+        var = fmaf(d, d, var);
+    }
+    float rstd = rsqrtf(warp_sum(var) * (1.0f / VQ_D) + 1e-5f);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        float4 g = __ldg(reinterpret_cast<const float4*>(gb + i * 128 + lane * 4));
+        float4 be = __ldg(reinterpret_cast<const float4*>(gb + VQ_D + i * 128 + lane * 4));
+        v[i * 4 + 0] = (v[i * 4 + 0] - mean) * rstd * g.x + be.x;
+        v[i * 4 + 1] = (v[i * 4 + 1] - mean) * rstd * g.y + be.y;
+        v[i * 4 + 2] = (v[i * 4 + 2] - mean) * rstd * g.z + be.z;
+        v[i * 4 + 3] = (v[i * 4 + 3] - mean) * rstd * g.w + be.w;
+    }
+}
+
 // One VectorQuantize.forward on the frame held in r (channel c = i*128 + lane*4 + j <-> r[i*4+j]).
 // Writes out[] = out_proj(z_q), returns the code index; sqerr = sum_k (z_e - z_q)^2.
 __device__ __forceinline__ int vq_stage(const VqWeights& W, const float (&r)[32], float (&out)[32], float& sqerr,
@@ -98,19 +139,7 @@ __device__ __forceinline__ int vq_stage(const VqWeights& W, const float (&r)[32]
         zq[k] = ze[k] + (zq[k] - ze[k]);   // straight-through estimator, forward value
     }
     sqerr = se;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        float4 o = __ldg(reinterpret_cast<const float4*>(W.b_out + i * 128 + lane * 4));
-#pragma unroll
-        for (int k = 0; k < VQ_CD; ++k) {
-            float4 w = __ldg(reinterpret_cast<const float4*>(W.w_out + k * VQ_D + i * 128 + lane * 4));
-            o.x = fmaf(w.x, zq[k], o.x);
-            o.y = fmaf(w.y, zq[k], o.y);
-            o.z = fmaf(w.z, zq[k], o.z);
-            o.w = fmaf(w.w, zq[k], o.w);
-        }
-        out[i * 4] = o.x; out[i * 4 + 1] = o.y; out[i * 4 + 2] = o.z; out[i * 4 + 3] = o.w;
-    }
+    out_proj(W, zq, out, lane);
     return bidx;
 }
 
@@ -180,31 +209,10 @@ __global__ void __launch_bounds__(128) fa_quantize_kernel(FaqParams p) {
         }
     }
     if (p.zr) store_frame(p.zr + fo, zr, lane);
-    // outs = z_p + z_c + z_r ; timbre_norm = LayerNorm(1024, no affine), eps 1e-5 ; * gamma + beta
-    float s = 0.f;
+    // outs = LayerNorm(z_p + z_c + z_r) * gamma + beta
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-        out[i] = (zp[i] + zc[i]) + zr[i];
-        s += out[i];
-    }
-    float mean = warp_sum(s) * (1.0f / VQ_D);
-    float v = 0.f;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-        float d = out[i] - mean;
-        v = fmaf(d, d, v);
-    }
-    float rstd = rsqrtf(warp_sum(v) * (1.0f / VQ_D) + 1e-5f);
-    const float* gb = p.gamma_beta + (size_t)b * 2 * VQ_D;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        float4 g = __ldg(reinterpret_cast<const float4*>(gb + i * 128 + lane * 4));
-        float4 be = __ldg(reinterpret_cast<const float4*>(gb + VQ_D + i * 128 + lane * 4));
-        out[i * 4 + 0] = (out[i * 4 + 0] - mean) * rstd * g.x + be.x;
-        out[i * 4 + 1] = (out[i * 4 + 1] - mean) * rstd * g.y + be.y;
-        out[i * 4 + 2] = (out[i * 4 + 2] - mean) * rstd * g.z + be.z;
-        out[i * 4 + 3] = (out[i * 4 + 3] - mean) * rstd * g.w + be.w;
-    }
+    for (int i = 0; i < 32; ++i) out[i] = (zp[i] + zc[i]) + zr[i];
+    adaln(out, p.gamma_beta + (size_t)b * 2 * VQ_D, lane);
     store_frame(p.outs + fo, out, lane);
 }
 
@@ -212,6 +220,63 @@ cudaError_t launch_fa_quantize(const FaqParams& p, cudaStream_t st) {
     int nframes = p.B * p.Tq;
     if (nframes <= 0) return cudaSuccess;
     fa_quantize_kernel<<<(nframes + 3) / 4, 128, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
+// out = out_proj(codebook[idx]) for one code (VectorQuantize.decode_code + out_proj, dac/nn/quantize.py:211-218: the RAW
+// codebook row, not the straight-through value of the forward).  An index outside [0, 1024) reads nothing and gives NaN.
+__device__ __forceinline__ void code_stage(const VqWeights& W, long long idx, float (&out)[32], int lane) {
+    if (idx < 0 || idx >= VQ_N) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) out[i] = __int_as_float(0x7fc00000);
+        return;
+    }
+    float4 q0 = __ldg(reinterpret_cast<const float4*>(W.cb + idx * VQ_CD));
+    float4 q1 = __ldg(reinterpret_cast<const float4*>(W.cb + idx * VQ_CD + 4));
+    float zq[VQ_CD] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
+    out_proj(W, zq, out, lane);
+}
+
+// FAquantizer from codes per frame: ResidualVectorQuantize.from_codes (dac/nn/quantize.py:200-220, z_q = 0 + sum of the
+// stages in order) for the prosody, content and residual RVQs, outs = LayerNorm((z_p + z_c) + z_r) * gamma + beta
+// (modules/quantize.py:437-449).  n_r = 0 leaves z_r out (z_r = 0, as res_mask = 0 does).  One warp per frame, as above.
+__global__ void __launch_bounds__(128) dequantize_kernel(DeqParams p) {
+    const int lane = threadIdx.x & 31;
+    const int frame = blockIdx.x * 4 + (threadIdx.x >> 5);
+    const int nframes = p.B * p.T;
+    if (frame >= nframes) return;
+    const int b = frame / p.T, t = frame - b * p.T;
+    const size_t fo = (size_t)frame * VQ_D;
+
+    float zp[32], zc[32], zr[32], out[32];
+    code_stage(p.vq[0], p.codes_p[(size_t)b * p.T + t], zp, lane);
+    if (p.zp) store_frame(p.zp + fo, zp, lane);
+    code_stage(p.vq[1], p.codes_c[((size_t)b * p.n_c + 0) * p.T + t], zc, lane);
+    if (p.n_c > 1) {
+        code_stage(p.vq[2], p.codes_c[((size_t)b * p.n_c + 1) * p.T + t], out, lane);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) zc[i] += out[i];
+    }
+    if (p.zc) store_frame(p.zc + fo, zc, lane);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) zr[i] = 0.f;
+    for (int q = 0; q < p.n_r; ++q) {
+        code_stage(p.vq[3 + q], p.codes_r[((size_t)b * p.n_r + q) * p.T + t], out, lane);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) zr[i] += out[i];
+    }
+    if (p.zr) store_frame(p.zr + fo, zr, lane);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) out[i] = (zp[i] + zc[i]) + zr[i];
+    adaln(out, p.gamma_beta + (size_t)b * 2 * VQ_D, lane);
+    store_frame(p.outs + fo, out, lane);
+}
+
+cudaError_t launch_dequantize(const DeqParams& p, cudaStream_t st) {
+    const long long nframes = (long long)p.B * p.T;
+    if (nframes <= 0) return cudaSuccess;
+    if (nframes > 0x7fffffffLL) return cudaErrorInvalidValue;
+    dequantize_kernel<<<(unsigned)((nframes + 3) / 4), 128, 0, st>>>(p);
     return cudaGetLastError();
 }
 

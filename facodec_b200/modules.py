@@ -170,6 +170,35 @@ def _f32c(t):
     return t.detach().to(torch.float32).contiguous()
 
 
+def _codes_args(codes, timbre, check_devices):
+    """Validates the inputs of the decode-from-codes calls: ``codes`` = [codes_p [B,1,T], codes_c [B,1|2,T], codes_r
+    [B,0..3,T] or None] integer tensors and ``timbre`` [B,1024]; ``check_devices`` raises FacError for tensors off the
+    engine's device.  Returns (codes_p, codes_c, codes_r or None, residual rows, timbre, B, T) ready for the C call.
+    Out-of-range codes raise IndexError, as F.embedding does in the reference; that check is one device reduction and
+    one host synchronisation."""
+    if not isinstance(codes, (list, tuple)) or len(codes) != 3 or codes[0] is None or codes[1] is None or timbre is None:
+        raise ValueError("codes must be [codes_p, codes_c, codes_r or None] and timbre a [B, 1024] tensor")
+    check_devices([t for t in (*codes, timbre) if t is not None])
+    for t in codes:
+        if t is not None and (t.dim() != 3 or t.is_floating_point() or t.is_complex()):
+            raise ValueError("codes must be integer tensors [B, rows, T]; got %s %s" % (t.dtype, tuple(t.shape)))
+    cp, cc, cr = (None if t is None else t.detach().to(torch.int64).contiguous() for t in codes)
+    B, _, T = cp.shape
+    for name, t, rows in (("codes_p", cp, (1,)), ("codes_c", cc, (1, 2)), ("codes_r", cr, (0, 1, 2, 3))):
+        if t is not None and (t.shape[1] not in rows or t.shape[0] != B or t.shape[2] != T):
+            raise ValueError("%s: expected [%d, %s, %d], got %s" % (name, B, "|".join(map(str, rows)), T, tuple(t.shape)))
+    if B < 1 or T < 1:
+        raise ValueError("codes hold no frames: %s" % (tuple(cp.shape),))
+    if tuple(timbre.shape) != (B, 1024):
+        raise ValueError("timbre must be [%d, 1024], got %s" % (B, tuple(timbre.shape)))
+    if cr is not None and cr.shape[1] == 0:
+        cr = None
+    present = [t for t in (cp, cc, cr) if t is not None]
+    if bool(torch.stack([((t < 0) | (t >= 1024)).any() for t in present]).any()):
+        raise IndexError("codes must lie in [0, 1024)")
+    return cp, cc, cr, 0 if cr is None else cr.shape[1], _f32c(timbre), B, T
+
+
 class Encoder(_RefKeyModule):
     """dac/model/dac.py:69-104 Encoder(d_model=64, strides=[2,5,5,6], d_latent=1024, causal=True, lstm=2)."""
     _module_id = MOD_ENCODER
@@ -296,6 +325,22 @@ class FAquantizer(_RefKeyModule):
 
     forward_v2 = forward
 
+    def from_codes(self, codes, timbre):
+        """Latents from codes: ResidualVectorQuantize.from_codes (dac/nn/quantize.py:200-220) of the prosody, content and
+        residual quantizers, then outs = LayerNorm((z_p + z_c) + z_r) * gamma + beta with gamma | beta =
+        timbre_linear(timbre) (modules/quantize.py:437-449).  ``codes`` is the [codes_p, codes_c, codes_r] list
+        ``forward(..., return_codes=True)`` returns; codes_c may have 1 or 2 rows, codes_r 0..3 rows or be None (then z_r is
+        zeros and left out of outs).  ``timbre`` [B,1024] may come from another utterance.  Returns
+        (outs [B,1024,T], [z_p, z_c, z_r]).  Out-of-range codes raise IndexError (one device reduction + one host sync)."""
+        cp, cc, cr, n_r, tv, B, T = _codes_args(codes, timbre, lambda ts: self._prep(*ts))
+        L, h = self._engine.L, self._engine.handle
+        dev = cp.device
+        outs, zp, zc, zr = (torch.empty(B, 1024, T, device=dev) for _ in range(4))
+        rc = L.fac_dequantize(h, _ptr(cp), _ptr(cc), cc.shape[1], _ptr(cr), n_r, _ptr(tv), B, T, _ptr(outs), _ptr(zp), _ptr(zc),
+                              _ptr(zr), _stream(dev))
+        _lib.check(h, rc, "fac_dequantize")
+        return outs, [zp, zc, zr]
+
 
 class Munch(dict):
     """Attribute dict (the reference returns munch.Munch from build_model)."""
@@ -329,6 +374,41 @@ class Codec:
         rc = e.L.fac_codec_forward(e.handle, _ptr(x), B, T, n_c, _ptr(y), _ptr(cp), _ptr(cc), _ptr(cr), _ptr(timbre), _stream(dev))
         _lib.check(e.handle, rc, "fac_codec_forward")
         return y, [cp, cc, cr], timbre
+
+    def encode(self, x, n_c=2):
+        """Compress only: x [B,1,T] on the GPU -> ([codes_p, codes_c, codes_r], timbre), bit-identical to what forward()
+        returns, without running the decoder."""
+        e = self.engine
+        for m in (self.model.encoder, self.model.quantizer):
+            if m.training:
+                raise NotImplementedError("eval mode only")
+        e.sync_weights(x.device)
+        x = _f32c(x)
+        B, _, T = x.shape
+        Tq = min(T // 300, e.L.fac_encode_frames(T))
+        dev = x.device
+        cp = torch.empty(B, 1, Tq, device=dev, dtype=torch.int64)
+        cc = torch.empty(B, n_c, Tq, device=dev, dtype=torch.int64)
+        cr = torch.empty(B, 3, Tq, device=dev, dtype=torch.int64)
+        timbre = torch.empty(B, 1024, device=dev)
+        rc = e.L.fac_codec_encode(e.handle, _ptr(x), B, T, n_c, _ptr(cp), _ptr(cc), _ptr(cr), _ptr(timbre), _stream(dev))
+        _lib.check(e.handle, rc, "fac_codec_encode")
+        return [cp, cc, cr], timbre
+
+    def decode(self, codes, timbre):
+        """Decompress: codes ([codes_p, codes_c, codes_r] as forward()/encode() return them, or codefile.DACFile.unpack();
+        codes_r may have 0..3 rows or be None) + timbre [B,1024] on the GPU -> y [B,1,300*T].  A timbre from another
+        utterance gives that voice (FAquantizer.from_codes).  Out-of-range codes raise IndexError (one device reduction +
+        one host sync)."""
+        if self.model.decoder.training:
+            raise NotImplementedError("eval mode only")
+        cp, cc, cr, n_r, tv, B, T = _codes_args(codes, timbre, lambda ts: self.model.quantizer._prep(*ts))
+        e = self.engine
+        dev = cp.device
+        y = torch.empty(B, 1, T * 300, device=dev)
+        rc = e.L.fac_codes_decode(e.handle, _ptr(cp), _ptr(cc), cc.shape[1], _ptr(cr), n_r, _ptr(tv), B, T, _ptr(y), _stream(dev))
+        _lib.check(e.handle, rc, "fac_codes_decode")
+        return y
 
     def forward_host(self, x_host, n_c=2, out=None):
         """End-to-end with HOST tensors (pinned recommended): H2D, forward, D2H inside the call.
@@ -420,6 +500,23 @@ class CodecStream:
         y = torch.empty(B, 1, Fc * 300, device=z.device, dtype=torch.float32)
         e = self.engine
         _lib.check(e.handle, e.L.fac_stream_decode(e.handle, self.sid, _ptr(z), Fc, _ptr(y), _stream(z.device)), "fac_stream_decode")
+        return y
+
+    def decode_codes(self, codes, timbre):
+        """decode() from a chunk of codes ([codes_p, codes_c, codes_r] of Fc frames, as Codec.decode takes them) and the
+        utterance's timbre [B,1024] -> y chunk [B,1,300*Fc].  It advances the same decoder state as decode(): feed a stream
+        one or the other."""
+        def check(ts):
+            for t in ts:
+                self._check(t)
+        cp, cc, cr, n_r, tv, B, Fc = _codes_args(codes, timbre, check)
+        if B != self.batch:
+            raise ValueError("stream batch is %d, codes have %d utterances" % (self.batch, B))
+        y = torch.empty(B, 1, Fc * 300, device=cp.device, dtype=torch.float32)
+        e = self.engine
+        rc = e.L.fac_stream_decode_codes(e.handle, self.sid, _ptr(cp), _ptr(cc), cc.shape[1], _ptr(cr), n_r, _ptr(tv), Fc, _ptr(y),
+                                         _stream(cp.device))
+        _lib.check(e.handle, rc, "fac_stream_decode_codes")
         return y
 
     def close(self):

@@ -91,6 +91,27 @@ int fac_codec_forward(fac_handle* h, const float* x, int B, int T, int n_c, floa
 int fac_codec_forward_host(fac_handle* h, const float* x_host, int B, int T, int n_c, float* y_host,
                            int64_t* codes_p_host, int64_t* codes_c_host, int64_t* codes_r_host, void* stream);
 
+/* Compress only: fac_codec_forward without the decoder (encoder -> quantizer(n_c), the quantizer's waveform-only front
+ * forked beside the encoder): the same codes and timbre as fac_codec_forward, bit for bit.  codes_p [B,1,Tq],
+ * codes_c [B,n_c,Tq], codes_r [B,3,Tq] int64 are required; timbre [B,1024] may be NULL. */
+int fac_codec_encode(fac_handle* h, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
+                     int64_t* codes_r, float* timbre, void* stream);
+
+/* Decompress.  The reference has no single call for it (FAquantizer.decode, modules/quantize.py:245-254, needs the
+ * timbre quantizer that timbre_norm = True leaves out); it is ResidualVectorQuantize.from_codes (dac/nn/quantize.py:200-220:
+ * out_proj(codebook[code]) summed over a quantizer's rows) on the prosody, content and residual quantizers, then
+ * outs = LayerNorm((z_p + z_c) + z_r) * gamma + beta with gamma | beta = timbre_linear(timbre) (modules/quantize.py:437-449).
+ * codes_p [B,1,T], codes_c [B,n_c_rows,T] (n_c_rows = 1 or 2), codes_r [B,n_r_rows,T] (n_r_rows = 0..3; NULL allowed when
+ * 0: z_r is left out, as the training-time res_mask = 0 does) int64, timbre [B,1024] -- any utterance's timbre, so codes of
+ * one speaker decode in the voice of another.  A code outside [0, 1024) is never read past the codebook: it makes its
+ * frame's outputs NaN.
+ * fac_dequantize: outs [B,1024,T]; zp / zc / zr [B,1024,T] may be NULL.
+ * fac_codes_decode: the same, then the codec's decoder with the latents kept channels-last: y [B,1,300*T]. */
+int fac_dequantize(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
+                   int n_r_rows, const float* timbre, int B, int T, float* outs, float* zp, float* zc, float* zr, void* stream);
+int fac_codes_decode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
+                     int n_r_rows, const float* timbre, int B, int T, float* y, void* stream);
+
 /* Voice conversion (reconstruct_redecoder.py:108-122, webui.py:68-81).
  * fac_redecode = model.encoder(p_code, c_code, timbre, use_p_code, use_c_code, n_c) of the redecoder model,
  * modules/redecoder.py:35-48: codes_p [B,1,T], codes_c [B,n_c_rows,T] int64 (device; the codec's codes[0], codes[1]),
@@ -112,10 +133,14 @@ int fac_voice_convert(fac_handle* h, const int64_t* codes_p, const int64_t* code
  * fac_stream_encode: x_chunk [B,1,T] (device; T a multiple of 300, the first chunk >= 3000) -> z_chunk [B,1024,T/300].
  * fac_stream_decode: z_chunk [B,1024,Fc] (device; first chunk >= 10 frames) -> y_chunk [B,1,300*Fc].
  * The quantizer is not part of the stream: its timbre branch pools over the whole utterance (modules/quantize.py:375-454),
- * the VQ lookups themselves are per frame (fac_quantize on each z chunk is exact for the codes). */
+ * the VQ lookups themselves are per frame (fac_quantize on each z chunk is exact for the codes).
+ * fac_stream_decode_codes: fac_stream_decode on a chunk of codes (Fc frames, arguments as fac_codes_decode); it advances
+ * the same decoder state, so one stream should be fed either latents or codes. */
 int fac_stream_begin(fac_handle* h, int B);
 int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float* z, void* stream);
 int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, float* y, void* stream);
+int fac_stream_decode_codes(fac_handle* h, int stream_id, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows,
+                            const int64_t* codes_r, int n_r_rows, const float* timbre, int Fc, float* y, void* stream);
 int fac_stream_end(fac_handle* h, int stream_id);
 
 /* quantize/rvq.py:27-75 ResidualVQ.forward (eval) over quantize/fvq.py FactorizedVectorQuantize,

@@ -108,7 +108,8 @@ int fac_debug_tap(fac_handle* h, const char* name, float* dst, size_t capacity_f
 
 /* Per-kernel-family device timing for bench.py's roofline object: when enabled, every launch of
  * the forward paths is bracketed by CUDA events on the launching stream.  Families: "conv"
- * (conv_cl_kernel, fp32 FMA), "conv_tc" / "conv_tcp" (conv_tc_kernel, plain / promoted), "lstm_rec", "fa_quantize".  fac_profile_get returns
+ * (conv_cl_kernel, fp32 FMA), "conv_tc" / "conv_tcp" (conv_tc_kernel, plain / promoted), "lstm_rec", "fa_quantize",
+ * "dequantize" (decoding from codes).  fac_profile_get returns
  * the accumulated device milliseconds, ALGORITHMIC flops (2*MACs) and bytes (in + out + weights
  * once) and launch count since the last fac_profile_reset (it synchronises the device). */
 int fac_profile_enable(fac_handle* h, int on);
