@@ -13,7 +13,9 @@
 //   TF32 pairs (k = 8 MMAs); bf16 pairs (k = 16) downstream of the VQ; ONE fp16 pass (g1f16: the k = 7 convs
 //   downstream of the VQ); fp16 hi + 2^11-scaled fp16 lo (f16x2, promoted only).
 // Promoted layers (upstream of the VQ, long K loops) accumulate each window of <= 48 chained MMAs in fresh
-// registers and add it to an fp32 master accumulator, so the sum is not one long tensor-core accumulation chain.
+// registers and add it to an fp32 master accumulator, so the sum is not one long tensor-core accumulation chain.  The
+// master lives in shared memory, so the window registers are the only accumulators and the promoted class fits the
+// register budget of two resident CTAs per SM.
 //
 // CTA = two warpgroups over a tile of 128 rows x N channels (each warpgroup 64 rows) or 64 rows x N channels (each
 // warpgroup N/2 channels).  Per 16-channel chunk:
@@ -27,8 +29,9 @@
 // Fused mode (a whole ResidualUnit, conv7 -> +b7 -> Snake -> 1x1 conv -> +b1 -> +x): GEMM 1's accumulators go through
 // bias + Snake + split straight into a resident shared-memory operand for GEMM 2.
 // Epilogue from the accumulator registers: bias -> Snake/tanh/Mish -> residual -> 8-byte stores.
-// Variants: tiles planned for two resident CTAs per SM (option "tc_occ2_maxn"), and the transposed formulation of the
-// promoted fp16 class (option "encoder_tt": weights as the wgmma A operand, time as wgmma N).
+// Variants: tiles planned for two resident CTAs per SM (always tried for the promoted class; option "tc_occ2_maxn" for
+// the others), and the transposed formulation of the promoted fp16 class (option "encoder_tt": weights as the wgmma A
+// operand, time as wgmma N).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -56,6 +59,11 @@ template <int P> struct PrecT {
 
 __host__ __device__ constexpr int prec_kg(int P) { return P == P_TF32 ? 4 : 2; }
 __host__ __device__ constexpr int prec_planes(int P) { return P == P_F16S ? 1 : 2; }
+// Shared-memory master accumulator of a promoted layer: the NI / 2 accumulator floats of every thread, float4 q of
+// thread tid at q * kThreads + tid (lane-consecutive, so conflict-free).  A K loop of one window needs none.
+__host__ __device__ constexpr uint32_t master_bytes(bool promoted, int nchunk, int promote_every, int ni) {
+    return promoted && nchunk > promote_every ? (uint32_t)ni / 2 * 4 * kThreads : 0u;
+}
 
 template <int NI>
 __device__ __forceinline__ void zero_acc(float (&a)[NI / 2]) {
@@ -107,7 +115,8 @@ __device__ __forceinline__ float act_out(int act, float v, float al, float ia) {
 
 // P1: split class of the layer's own GEMM; P2: of the fused GEMM 2 (P_NONE = not fused); NI: wgmma N, the warpgroup's
 // whole channel width NW (NI / 2 accumulator registers per thread; NI <= 64 when promoted or MINB = 2, else <= 128);
-// MINB = 2: planned for two resident CTAs per SM (<= 128 registers);
+// MINB = 2: compiled for two resident CTAs per SM (<= 128 registers); the promoted class is only compiled so, and runs
+// one CTA per SM when its plan needs more than half the shared memory;
 // TT: transposed formulation -- the weights are the wgmma A operand (64 output channels per warpgroup) and time is the
 // wgmma N dimension (NI = 64 time steps); the operand buffers and the weight blob are the same K-major layouts as the
 // plain formulation.
@@ -136,7 +145,8 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
     const int R = BM + (Kr - 1) * dil;
     const uint32_t a_plane = (uint32_t)T1::KG * Rpad * 16, a_bytes = a_plane * T1::planes;
     uint8_t* abuf = smem + kSmemHdr;
-    uint8_t* wbuf = abuf + 2 * (size_t)a_bytes;
+    float4* master = reinterpret_cast<float4*>(abuf + 2 * (size_t)a_bytes);
+    uint8_t* wbuf = abuf + 2 * (size_t)a_bytes + master_bytes(PROMO, nchunk, p.promote_every, NI);
     uint8_t* a2buf = wbuf + (size_t)S * p.b_slot;
     const uint32_t w_unit1 = (uint32_t)Kr * T1::planes * T1::KG * N * 16;
     const uint32_t w_unit2 = FUSED ? (uint32_t)prec_planes(P2) * prec_kg(P2) * N * 16 : 0;
@@ -172,23 +182,34 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
     };
     produce(0);
 
-    float acc[NI / 2];
-    float tmp[PROMO ? NI / 2 : 1];
-    float crs[F16X2 ? NI / 2 : 1];
+    float acc[NI / 2];                   // promoted: the current window (f16x2: its hi*hi products)
+    float crs[F16X2 ? NI / 2 : 1];       // f16x2: the window's 2^11-scaled cross terms
     zero_acc<NI>(acc);
-    if constexpr (PROMO) zero_acc<NI>(tmp);
     if constexpr (F16X2) zero_acc<NI>(crs);
     const uint32_t a_lbo = (uint32_t)Rpad * 16, b_lbo = (uint32_t)N * 16;
     const uint32_t abase = smem_u32(abuf), wbase = smem_u32(wbuf), a2base = smem_u32(a2buf);
     const int BM2 = BM;
 
-    auto promote = [&]() {
+    // master += window (f16x2: hi*hi + cross * 2^-11), in fp32.  The first window adds to zero without reading the master;
+    // the last leaves the total in acc for the epilogue without writing it.  Thread-private slots need no barrier.
+    auto promote = [&](bool first, bool last) {
         if constexpr (PROMO) {
 #pragma unroll
-            for (int i = 0; i < NI / 2; ++i) {
-                if constexpr (F16X2) { acc[i] += tmp[i] + crs[i] * kLoUnscale; crs[i] = 0.f; }
-                else acc[i] += tmp[i];
-                tmp[i] = 0.f;
+            for (int q = 0; q < NI / 8; ++q) {
+                float w[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int i = 4 * q + e;
+                    if constexpr (F16X2) { w[e] = acc[i] + crs[i] * kLoUnscale; crs[i] = 0.f; }
+                    else w[e] = acc[i];
+                }
+                float4 m = first ? make_float4(0.f, 0.f, 0.f, 0.f) : master[q * kThreads + tid];
+                m.x += w[0]; m.y += w[1]; m.z += w[2]; m.w += w[3];
+                if (!last) master[q * kThreads + tid] = m;
+                acc[4 * q + 0] = last ? m.x : 0.f;
+                acc[4 * q + 1] = last ? m.y : 0.f;
+                acc[4 * q + 2] = last ? m.z : 0.f;
+                acc[4 * q + 3] = last ? m.w : 0.f;
             }
         }
     };
@@ -208,19 +229,15 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
                 const uint32_t ahi = a0 + (uint32_t)(tap * dil) * 16, alo = ahi + a_plane;
                 const uint32_t bhi = b0 + (uint32_t)tap * T1::planes * T1::KG * b_lbo, blo = bhi + T1::KG * b_lbo;
                 if constexpr (TT) {         // D[channel][time]: weights are the A operand, activations the B operand
-                    mma_pass<P1, NI>(tmp, bhi, b_lbo, ahi, a_lbo);
+                    mma_pass<P1, NI>(acc, bhi, b_lbo, ahi, a_lbo);
                     mma_pass<P1, NI>(crs, bhi, b_lbo, alo, a_lbo);
                     mma_pass<P1, NI>(crs, blo, b_lbo, ahi, a_lbo);
                 } else if constexpr (P1 == P_F16S) {
                     mma_pass<P1, NI>(acc, ahi, a_lbo, bhi, b_lbo);
                 } else if constexpr (F16X2) {
-                    mma_pass<P1, NI>(tmp, ahi, a_lbo, bhi, b_lbo);
+                    mma_pass<P1, NI>(acc, ahi, a_lbo, bhi, b_lbo);
                     mma_pass<P1, NI>(crs, ahi, a_lbo, blo, b_lbo);
                     mma_pass<P1, NI>(crs, alo, a_lbo, bhi, b_lbo);
-                } else if constexpr (PROMO) {
-                    mma_pass<P1, NI>(tmp, ahi, a_lbo, bhi, b_lbo);
-                    mma_pass<P1, NI>(tmp, ahi, a_lbo, blo, b_lbo);
-                    mma_pass<P1, NI>(tmp, alo, a_lbo, bhi, b_lbo);
                 } else {
                     mma_pass<P1, NI>(acc, ahi, a_lbo, bhi, b_lbo);
                     mma_pass<P1, NI>(acc, ahi, a_lbo, blo, b_lbo);
@@ -230,7 +247,7 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
             wg_commit();
             if (u + 1 < nchunk) produce(u + 1);         // overlaps the MMAs in flight
             wg_wait_all();
-            if (PROMO && ((u + 1) % p.promote_every == 0 || u + 1 == nchunk)) promote();
+            if (PROMO && ((u + 1) % p.promote_every == 0 || u + 1 == nchunk)) promote(u < p.promote_every, u + 1 == nchunk);
             if constexpr (FUSED) {
                 if (u + 1 == nchunk) {
                     // GEMM-2 operand snake2(D1 + b7), split, K-major [plane][k-piece][BM rows][16 B]
@@ -359,9 +376,10 @@ bool tc_conv_plan(TcConvParams& p) {
         else if (p.fused) return false;
     }
     if (N == 0) return false;
-    // Two resident CTAs per SM (tiles of N <= occ2_maxn, plain accumulation only): one CTA's operand production and
-    // epilogue overlap the other's MMAs; each gets half the shared memory and <= 128 registers per thread.
-    const bool want2 = p.occ2_maxn > 0 && N <= p.occ2_maxn && !p.promoted;
+    // Two resident CTAs per SM: one CTA's operand production, barriers, promotions and epilogue overlap the other's MMAs;
+    // each gets half the shared memory and <= 128 registers per thread.  Always tried for the promoted class, which loses
+    // no MMA width to it (NW <= 64 either way); for the others only for tiles of N <= occ2_maxn, which must halve NW.
+    const bool want2 = p.promoted ? !p.tt : (p.occ2_maxn > 0 && N <= p.occ2_maxn);
     for (int two = want2 ? 1 : 0; two >= 0; --two) {
         const size_t cap = two ? kSmemCap2 : kSmemCap;
         const int nwl = two ? 64 : nw_max;
@@ -382,7 +400,8 @@ bool tc_conv_plan(TcConvParams& p) {
                 }
                 // transposed: a warpgroup's A operand is always 64 channel rows; rows past its NW read (and discard)
                 // whatever follows the weight slot, so the buffer ends with 64 rows of slack
-                const size_t total = kSmemHdr + 2 * a_bytes + S * slot + a2 + (p.tt ? 64 * 16 : 0);
+                const size_t master = master_bytes(p.promoted, p.nchunk, p.promote_every, p.tt ? 64 : NW);
+                const size_t total = kSmemHdr + 2 * a_bytes + master + S * slot + a2 + (p.tt ? 64 * 16 : 0);
                 if (total > cap) continue;
                 p.N = N; p.MT = MT; p.Rpad = Rpad; p.R2pad = BM; p.stagesB = S; p.b_slot = (int)slot; p.smem_bytes = total;
                 p.occ2 = two;
@@ -516,7 +535,8 @@ cudaError_t launch_one(const TcConvParams& p, dim3 grid, cudaStream_t st) {
     return cudaGetLastError();
 }
 // The kernel's wgmma N is the warpgroup's whole channel width NW, so there is one instantiation per width tc_conv_plan
-// can return for the class: 16, 32, ..., 128, or up to 64 when promoted or planned for two CTAs per SM.
+// can return for the class: 16, 32, ..., 128, or up to 64 when promoted or planned for two CTAs per SM.  The promoted
+// class (TT aside) has only the MINB = 2 instantiations, whatever residency its plan allows.
 template <int P1, int P2, bool PROMO, int MINB = 1, int NI = (PROMO || MINB == 2 ? 64 : 128)>
 cudaError_t launch_nw(const TcConvParams& p, dim3 grid, cudaStream_t st) {
     const int NW = p.MT == 2 ? p.N : p.N / 2;
@@ -542,7 +562,8 @@ cudaError_t launch_conv_tc(const TcConvParams& p, cudaStream_t st) {
         return launch_occ<P_TF32, P_TF32>(p, grid, st);
     }
     if (p.tt) return launch_one<P_F16X2, P_NONE, true, 64, 1, true>(p, grid, st);
-    if (p.promoted) return P1 == P_F16X2 ? launch_nw<P_F16X2, P_NONE, true>(p, grid, st) : launch_nw<P_TF32, P_NONE, true>(p, grid, st);
+    if (p.promoted)
+        return P1 == P_F16X2 ? launch_nw<P_F16X2, P_NONE, true, 2>(p, grid, st) : launch_nw<P_TF32, P_NONE, true, 2>(p, grid, st);
     if (P1 == P_F16S) return launch_occ<P_F16S, P_NONE>(p, grid, st);
     if (P1 == P_BF16) return launch_occ<P_BF16, P_NONE>(p, grid, st);
     return launch_occ<P_TF32, P_NONE>(p, grid, st);

@@ -665,7 +665,7 @@ void run_conv(Ctx& c, const ConvW& w, const float* x, float* y, int B, int Tin, 
         TcConvParams tp;
         tp.Cin = w.Cin; tp.Cout = w.Cout; tp.vf = w.vf; tp.Kr = w.Kr; tp.promoted = w.promoted ? 1 : 0;
         // A layer whose whole K loop is at most one promotion window (<= 48 chained MMAs: the 1x1 convs of the 64- and
-        // 128-channel encoder stages) gains nothing from register promotion: same error class through conv_tc_kernel,
+        // 128-channel encoder stages) gains nothing from promotion: same error class through conv_tc_kernel,
         // which runs two CTAs per SM and prefetches the residual.
         bool short_chain = false;
         if (w.promoted && (w.Cin * w.vf / 16) * w.Kr * 6 <= 48) {

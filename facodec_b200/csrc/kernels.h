@@ -42,7 +42,7 @@ struct TcConvParams {
     int pad_left_s = 0, pad_right_s = 0, reflect = 0;   // sample-level padding (PadMap)
     int Tout = 0, Cout = 0, ldy = 0;
     int out_act = 0;
-    int promoted = 0;                  // 1 = register-promoted accumulation (layers upstream of the VQ)
+    int promoted = 0;                  // 1 = promoted accumulation, windows into a master in shared memory (upstream of the VQ)
     int bf16 = 0;                      // 1 = bf16 hi/lo split (K = 16 MMAs) instead of tf32 hi/lo; downstream of the VQ only
     int g1f16 = 0;                     // with bf16 = 1 (downstream only): the layer's own GEMM (the k-tap conv; GEMM 1 of a fused unit) takes
                                        // ONE fp16 pass (10-bit operands, fp32 accumulation) instead of the 3-pass bf16 hi/lo split

@@ -204,7 +204,7 @@ int fac_add3(fac_handle* h, const float* a, const float* b, const float* c, long
 
 /* Engine options.  "tensor_cores": 0 = fp32 FMA kernels everywhere; 1 = wgmma split-operand
  * kernel for every eligible layer downstream of the VQ (decoder, timbre branch), fp32 FMA upstream
- * (encoder, prosody branch); 2 (default) = wgmma everywhere, with the register-promoted accumulation
+ * (encoder, prosody branch); 2 (default) = wgmma everywhere, with the promoted accumulation
  * variant upstream of the VQ where the bit-exact argmin needs fp32-grade sums.
  * "fuse_resunit": 1 (default) runs each decoder ResidualUnit whose channels fit one CTA tile as a single
  * fused launch (conv7 -> Snake -> 1x1 conv -> +x with the intermediate kept in shared memory); 0 = two launches;
