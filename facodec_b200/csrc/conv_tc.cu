@@ -18,7 +18,9 @@
 // register budget of two resident CTAs per SM.
 //
 // CTA = two warpgroups over a tile of 128 rows x N channels (each warpgroup 64 rows) or 64 rows x N channels (each
-// warpgroup N/2 channels).  Per 16-channel chunk:
+// warpgroup N/2 channels).  A warpgroup spans at most 128 channels, except in the one-pass fp16 class: its tiles of the
+// decoder's C = 768 conv7 (N = 256) and C = 192 fused unit (N = 192) are 128 rows with each warpgroup over all N channels
+// (see tc_conv_plan).  Per 16-channel chunk:
 //   weights: one thread streams the chunk's pre-arranged [tap][hi|lo][k-piece][N][16 B] blob with ONE 1-D bulk copy
 //            (cp.async.bulk, completion on an mbarrier) into a ring of 1-2 slots;
 //   activations: all 256 threads load the UNION of the rows all taps need (rows + (K-1)*dil) once with 16-byte loads
@@ -114,7 +116,8 @@ __device__ __forceinline__ float act_out(int act, float v, float al, float ia) {
 }
 
 // P1: split class of the layer's own GEMM; P2: of the fused GEMM 2 (P_NONE = not fused); NI: wgmma N, the warpgroup's
-// whole channel width NW (NI / 2 accumulator registers per thread; NI <= 64 when promoted or MINB = 2, else <= 128);
+// whole channel width NW (NI / 2 accumulator registers per thread; NI <= 64 when promoted or MINB = 2, <= 256 in the
+// one-pass fp16 class, else <= 128);
 // MINB = 2: compiled for two resident CTAs per SM (<= 128 registers); the promoted class is only compiled so, and runs
 // one CTA per SM when its plan needs more than half the shared memory;
 // TT: transposed formulation -- the weights are the wgmma A operand (64 output channels per warpgroup) and time is the
@@ -124,7 +127,8 @@ template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false>
 __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p) {
     constexpr bool FUSED = P2 != P_NONE;
     static_assert(!TT || (NI == 64 && !FUSED), "transposed tiles: <= 64 channels x 64 time steps per warpgroup");
-    static_assert(NI % 16 == 0 && NI <= (PROMO || MINB == 2 ? 64 : 128), "accumulator registers: <= 64 / 128 columns");
+    static_assert(NI % 16 == 0 && NI <= (PROMO || MINB == 2 ? 64 : (P1 == P_F16S ? 256 : 128)),
+                  "accumulator registers: <= 64 / 128 columns (256 in the one-pass fp16 class at one CTA per SM)");
     constexpr bool F16X2 = P1 == P_F16X2;
     constexpr bool DEC = P1 == P_BF16 || P1 == P_F16S;      // downstream of the VQ: SFU-sine Snake class
     using T1 = PrecT<P1>;
@@ -346,6 +350,11 @@ constexpr size_t kSmemCap2 = 113 * 1024;       // per block with two resident bl
 int plan_prec(const TcConvParams& p) {
     return p.g1f16 ? P_F16S : (p.f16x2 ? P_F16X2 : (p.bf16 ? P_BF16 : P_TF32));
 }
+// Warpgroup width above 128 that the one-pass fp16 class is compiled for (launch_conv_tc): 256 for a plain conv (the
+// decoder's C = 768 conv7), 192 for a fused unit (the C = 192 ResidualUnit).  A plain N = 192 k = 7 conv fits two 64-row
+// CTAs per SM and keeps them (tc_conv_plan); a fused unit at C = 256 has no room for two weight slots next to its 128-row
+// GEMM-2 operand, and the 64-row plan with two slots comes first.
+constexpr int f16s_wide_nw(bool fused) { return fused ? 192 : 256; }
 }  // namespace
 
 bool tc_conv_plan(TcConvParams& p) {
@@ -379,6 +388,35 @@ bool tc_conv_plan(TcConvParams& p) {
     // Two resident CTAs per SM: one CTA's operand production, barriers, promotions and epilogue overlap the other's MMAs;
     // each gets half the shared memory and <= 128 registers per thread.  Always tried for the promoted class, which loses
     // no MMA width to it (NW <= 64 either way); for the others only for tiles of N <= occ2_maxn, which must halve NW.
+    // The one-pass fp16 class (g1f16) does ONE MMA per streamed weight element, against three in the split classes, so
+    // it needs three times the weight bytes per MMA clock.  Where its 64-row tile runs one CTA per SM anyway (more than
+    // half the shared memory), it takes the N of f16s_wide_nw as 128 rows with each warpgroup over all N channels (NW = N,
+    // m64n192 / m64n256 accumulators of 96 / 128 registers): both warpgroups then read every weight chunk, which halves
+    // the weight bytes per MMA, and the per-chunk barrier, weight wait and halo rows are amortized over twice the rows.
+    // A 64-row tile that fits two CTAs per SM (its kernel has <= 128 registers at NW <= 128) keeps them: the other CTA's
+    // MMAs then cover those same costs (the C = 384 conv7 at the bench workload: 2.2 ms in two 64-row CTAs per SM, 3.1 ms
+    // in one 128-row CTA; H100 80GB HBM3, 700 W, 1980 MHz max SM clock).  N itself is what the loop above found, so the
+    // weight blob does not change.
+    struct Layout { int Rpad; size_t slot, total; };
+    auto layout = [&](int S, int MT) {
+        const int NW = MT == 2 ? N : N / 2, BM = 64 * MT;
+        Layout l;
+        l.Rpad = BM + (p.Kr - 1) * p.dil;
+        while (l.Rpad % 8 != 2) ++l.Rpad;                   // conflict-free 16-byte producer stores
+        const size_t a_bytes = (size_t)prec_planes(P1) * prec_kg(P1) * l.Rpad * 16;
+        l.slot = (size_t)p.Kr * prec_planes(P1) * prec_kg(P1) * N * 16;
+        size_t a2 = 0;
+        if (P2 != P_NONE) {
+            const size_t slot2 = (size_t)prec_planes(P2) * prec_kg(P2) * N * 16;
+            if (slot2 > l.slot) l.slot = slot2;
+            a2 = (size_t)prec_planes(P2) * p.nchunk2 * prec_kg(P2) * BM * 16;
+        }
+        // transposed: a warpgroup's A operand is always 64 channel rows; rows past its NW read (and discard) whatever
+        // follows the weight slot, so the buffer ends with 64 rows of slack
+        const size_t master = master_bytes(p.promoted, p.nchunk, p.promote_every, p.tt ? 64 : NW);
+        l.total = kSmemHdr + 2 * a_bytes + master + S * l.slot + a2 + (p.tt ? 64 * 16 : 0);
+        return l;
+    };
     const bool want2 = p.promoted ? !p.tt : (p.occ2_maxn > 0 && N <= p.occ2_maxn);
     for (int two = want2 ? 1 : 0; two >= 0; --two) {
         const size_t cap = two ? kSmemCap2 : kSmemCap;
@@ -386,24 +424,13 @@ bool tc_conv_plan(TcConvParams& p) {
         for (int S = 2; S >= 1; --S)
             for (int MT = 2; MT >= 1; --MT) {
                 const int NW = MT == 2 ? N : N / 2;
-                if (NW > nwl || NW % 16) continue;
-                const int BM = 64 * MT;
-                int Rpad = BM + (p.Kr - 1) * p.dil;
-                while (Rpad % 8 != 2) ++Rpad;               // conflict-free 16-byte producer stores
-                const size_t a_bytes = (size_t)prec_planes(P1) * prec_kg(P1) * Rpad * 16;
-                size_t slot = (size_t)p.Kr * prec_planes(P1) * prec_kg(P1) * N * 16;
-                size_t a2 = 0;
-                if (P2 != P_NONE) {
-                    const size_t slot2 = (size_t)prec_planes(P2) * prec_kg(P2) * N * 16;
-                    if (slot2 > slot) slot = slot2;
-                    a2 = (size_t)prec_planes(P2) * p.nchunk2 * prec_kg(P2) * BM * 16;
-                }
-                // transposed: a warpgroup's A operand is always 64 channel rows; rows past its NW read (and discard)
-                // whatever follows the weight slot, so the buffer ends with 64 rows of slack
-                const size_t master = master_bytes(p.promoted, p.nchunk, p.promote_every, p.tt ? 64 : NW);
-                const size_t total = kSmemHdr + 2 * a_bytes + master + S * slot + a2 + (p.tt ? 64 * 16 : 0);
-                if (total > cap) continue;
-                p.N = N; p.MT = MT; p.Rpad = Rpad; p.R2pad = BM; p.stagesB = S; p.b_slot = (int)slot; p.smem_bytes = total;
+                const bool wide = !two && P1 == P_F16S && NW == f16s_wide_nw(p.fused);
+                if ((NW > nwl && !wide) || NW % 16) continue;
+                if (wide && layout(2, 1).total <= kSmemCap2) continue;
+                const Layout l = layout(S, MT);
+                if (l.total > cap) continue;
+                p.N = N; p.MT = MT; p.Rpad = l.Rpad; p.R2pad = 64 * MT; p.stagesB = S; p.b_slot = (int)l.slot;
+                p.smem_bytes = l.total;
                 p.occ2 = two;
                 return true;
             }
@@ -535,8 +562,9 @@ cudaError_t launch_one(const TcConvParams& p, dim3 grid, cudaStream_t st) {
     return cudaGetLastError();
 }
 // The kernel's wgmma N is the warpgroup's whole channel width NW, so there is one instantiation per width tc_conv_plan
-// can return for the class: 16, 32, ..., 128, or up to 64 when promoted or planned for two CTAs per SM.  The promoted
-// class (TT aside) has only the MINB = 2 instantiations, whatever residency its plan allows.
+// can return for the class: 16, 32, ..., 128, or up to 64 when promoted or planned for two CTAs per SM, plus
+// f16s_wide_nw in the one-pass fp16 class.  The promoted class (TT aside) has only the MINB = 2
+// instantiations, whatever residency its plan allows.
 template <int P1, int P2, bool PROMO, int MINB = 1, int NI = (PROMO || MINB == 2 ? 64 : 128)>
 cudaError_t launch_nw(const TcConvParams& p, dim3 grid, cudaStream_t st) {
     const int NW = p.MT == 2 ? p.N : p.N / 2;
@@ -546,7 +574,12 @@ cudaError_t launch_nw(const TcConvParams& p, dim3 grid, cudaStream_t st) {
 }
 template <int P1, int P2>
 cudaError_t launch_occ(const TcConvParams& p, dim3 grid, cudaStream_t st) {
-    return p.occ2 ? launch_nw<P1, P2, false, 2>(p, grid, st) : launch_nw<P1, P2, false, 1>(p, grid, st);
+    if (p.occ2) return launch_nw<P1, P2, false, 2>(p, grid, st);
+    if constexpr (P1 == P_F16S) {
+        constexpr int kWide = f16s_wide_nw(P2 != P_NONE);
+        if ((p.MT == 2 ? p.N : p.N / 2) == kWide) return launch_one<P1, P2, false, kWide>(p, grid, st);
+    }
+    return launch_nw<P1, P2, false, 1>(p, grid, st);
 }
 }  // namespace
 

@@ -86,10 +86,10 @@ __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.s
 enum WgKind { WG_TF32 = 0, WG_BF16 = 1, WG_F16 = 2 };
 
 // D[64 x NI] += A[64 x K] * B[NI x K]^T, both operands K-major in shared memory; K = 16 (f16 / bf16) or 8 (tf32).
-// Defined for NI = 16, 32, ..., 128 by FAC_WGMMA_SS below; any other NI fails to compile.
+// Defined for NI = 16, 32, ..., 256 by FAC_WGMMA_SS below; any other NI fails to compile.
 template <int NI, int KIND>
 __device__ __forceinline__ void wgmma_ss(float (&d)[NI / 2], uint64_t da, uint64_t db) {
-    static_assert(NI < 0, "wgmma_ss: instruction N must be a multiple of 16 in [16, 128]");
+    static_assert(NI < 0, "wgmma_ss: instruction N must be a multiple of 16 in [16, 256]");
 }
 
 // The m64nNI accumulator is NI/2 registers per thread, listed in groups of 8: FAC_Sg is the asm operand list
@@ -102,6 +102,14 @@ __device__ __forceinline__ void wgmma_ss(float (&d)[NI / 2], uint64_t da, uint64
 #define FAC_S6 FAC_S5 ", %40, %41, %42, %43, %44, %45, %46, %47"
 #define FAC_S7 FAC_S6 ", %48, %49, %50, %51, %52, %53, %54, %55"
 #define FAC_S8 FAC_S7 ", %56, %57, %58, %59, %60, %61, %62, %63"
+#define FAC_S9 FAC_S8 ", %64, %65, %66, %67, %68, %69, %70, %71"
+#define FAC_S10 FAC_S9 ", %72, %73, %74, %75, %76, %77, %78, %79"
+#define FAC_S11 FAC_S10 ", %80, %81, %82, %83, %84, %85, %86, %87"
+#define FAC_S12 FAC_S11 ", %88, %89, %90, %91, %92, %93, %94, %95"
+#define FAC_S13 FAC_S12 ", %96, %97, %98, %99, %100, %101, %102, %103"
+#define FAC_S14 FAC_S13 ", %104, %105, %106, %107, %108, %109, %110, %111"
+#define FAC_S15 FAC_S14 ", %112, %113, %114, %115, %116, %117, %118, %119"
+#define FAC_S16 FAC_S15 ", %120, %121, %122, %123, %124, %125, %126, %127"
 #define FAC_R8(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
     "+f"(d[o + 6]), "+f"(d[o + 7])
 #define FAC_C1 FAC_R8(0)
@@ -112,6 +120,14 @@ __device__ __forceinline__ void wgmma_ss(float (&d)[NI / 2], uint64_t da, uint64
 #define FAC_C6 FAC_C5, FAC_R8(40)
 #define FAC_C7 FAC_C6, FAC_R8(48)
 #define FAC_C8 FAC_C7, FAC_R8(56)
+#define FAC_C9 FAC_C8, FAC_R8(64)
+#define FAC_C10 FAC_C9, FAC_R8(72)
+#define FAC_C11 FAC_C10, FAC_R8(80)
+#define FAC_C12 FAC_C11, FAC_R8(88)
+#define FAC_C13 FAC_C12, FAC_R8(96)
+#define FAC_C14 FAC_C13, FAC_R8(104)
+#define FAC_C15 FAC_C14, FAC_R8(112)
+#define FAC_C16 FAC_C15, FAC_R8(120)
 // One specialization per kind for N = 16 * G; the descriptors are operands %(8G) and %(8G + 1), spelled out as DESC.
 #define FAC_WGMMA_KIND(N, G, DESC, KIND, SHAPE, TAIL)                                                                   \
     template <>                                                                                                      \
@@ -131,6 +147,14 @@ FAC_WGMMA_SS(80, 5, "%40, %41")
 FAC_WGMMA_SS(96, 6, "%48, %49")
 FAC_WGMMA_SS(112, 7, "%56, %57")
 FAC_WGMMA_SS(128, 8, "%64, %65")
+FAC_WGMMA_SS(144, 9, "%72, %73")
+FAC_WGMMA_SS(160, 10, "%80, %81")
+FAC_WGMMA_SS(176, 11, "%88, %89")
+FAC_WGMMA_SS(192, 12, "%96, %97")
+FAC_WGMMA_SS(208, 13, "%104, %105")
+FAC_WGMMA_SS(224, 14, "%112, %113")
+FAC_WGMMA_SS(240, 15, "%120, %121")
+FAC_WGMMA_SS(256, 16, "%128, %129")
 #undef FAC_WGMMA_SS
 #undef FAC_WGMMA_KIND
 #undef FAC_R8
@@ -142,6 +166,14 @@ FAC_WGMMA_SS(128, 8, "%64, %65")
 #undef FAC_S6
 #undef FAC_S7
 #undef FAC_S8
+#undef FAC_S9
+#undef FAC_S10
+#undef FAC_S11
+#undef FAC_S12
+#undef FAC_S13
+#undef FAC_S14
+#undef FAC_S15
+#undef FAC_S16
 #undef FAC_C1
 #undef FAC_C2
 #undef FAC_C3
@@ -150,6 +182,14 @@ FAC_WGMMA_SS(128, 8, "%64, %65")
 #undef FAC_C6
 #undef FAC_C7
 #undef FAC_C8
+#undef FAC_C9
+#undef FAC_C10
+#undef FAC_C11
+#undef FAC_C12
+#undef FAC_C13
+#undef FAC_C14
+#undef FAC_C15
+#undef FAC_C16
 
 __device__ __forceinline__ float to_tf32(float x) {
     uint32_t r;

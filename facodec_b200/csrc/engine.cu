@@ -2609,19 +2609,20 @@ int fac_debug_pad_map(int L, int pad_left, int pad_right, int reflect, int* out,
 
 // Host-only: the tile plan the tensor-core conv kernel would use for a layer geometry (no GPU, no handle).
 int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* out8) {
-    if (!out8 || Cin <= 0 || Cout <= 0 || K <= 0 || dil <= 0 || stride <= 0 || mode < 0 || mode > 6) return FAC_ERR_INVALID;
+    if (!out8 || Cin <= 0 || Cout <= 0 || K <= 0 || dil <= 0 || stride <= 0 || mode < 0 || mode > 8) return FAC_ERR_INVALID;
     TcConvParams tp;
     tp.Cin = Cin; tp.Cout = Cout; tp.Tout = Tout; tp.occ2_maxn = occ2_maxn;
     tp.promoted = (mode == 1 || mode == 3) ? 1 : 0;
-    tp.bf16 = (mode == 2 || mode == 4) ? 1 : 0;
+    tp.bf16 = (mode == 2 || mode == 4 || mode == 7 || mode == 8) ? 1 : 0;
     tp.f16x2 = mode == 3 ? 1 : 0;
-    tp.fused = (mode == 4 || mode == 5) ? 1 : 0;
+    tp.fused = (mode == 4 || mode == 5 || mode == 8) ? 1 : 0;
+    tp.g1f16 = (mode == 7 || mode == 8) ? 1 : 0;                     // 7 / 8: one-pass fp16 class, plain / fused
     if (mode == 6) { tp.promoted = 1; tp.f16x2 = 1; tp.tt = 1; }     // 6: transposed formulation of mode 3
     if (stride == 1) { tp.vf = 1; tp.Kr = K; tp.dil = dil; }
     else if (K == 2 * stride && dil == 1) { tp.vf = stride; tp.Kr = 2; tp.dil = 1; }
     else return FAC_ERR_UNSUPPORTED;
     if (!tc_conv_plan(tp)) return FAC_ERR_UNSUPPORTED;
-    out8[0] = tp.N; out8[1] = tp.MT; out8[2] = tp.nchunk; out8[3] = tp.stagesB; out8[4] = 64 * tp.MT;
+    out8[0] = tp.N; out8[1] = tp.MT; out8[2] = tp.nchunk; out8[3] = tp.stagesB; out8[4] = tp.R2pad;
     out8[5] = (int)tp.smem_bytes; out8[6] = tp.Rpad; out8[7] = tp.promote_every;
     return FAC_OK;
 }

@@ -65,7 +65,8 @@ long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out
 int fac_debug_pad_map(int L, int pad_left, int pad_right, int reflect, int* out, int n);
 /* Host-only (no GPU, no handle): the tile plan of the wgmma conv kernel for one layer geometry.  mode: 0 TF32,
  * 1 promoted TF32, 2 bf16, 3 promoted fp16 hi + scaled lo, 4 fused ResidualUnit bf16, 5 fused TF32, 6 mode 3 in the
- * transposed formulation.  occ2_maxn as the "tc_occ2_maxn" option.  Tout may be 0 (unknown).  out8 = {N, MT (2: warpgroups split 128 rows, 1: they split N over 64 rows),
+ * transposed formulation, 7 ONE fp16 pass (the k = 7 convs downstream of the VQ), 8 fused ResidualUnit with its k = 7
+ * conv in one fp16 pass.  occ2_maxn as the "tc_occ2_maxn" option.  Tout may be 0 (unknown).  out8 = {N, MT (2: warpgroups split 128 rows, 1: they split N over 64 rows),
  * K chunks, weight-ring stages, rows per tile, dynamic shared-memory bytes, padded rows of the operand buffer,
  * chunks per promotion}.  FAC_ERR_UNSUPPORTED when the layer is not eligible. */
 int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* out8);
