@@ -141,7 +141,15 @@ struct fac_handle::Stream {
     float* dy_hist = nullptr; int dy_hist_len = 0;          // [B][kDecCtx][1536] last decoder-LSTM output frames
     uint32_t* enc_h[2] = {nullptr, nullptr}; float* enc_c[2] = {nullptr, nullptr};
     uint32_t* dec_h[2] = {nullptr, nullptr}; float* dec_c[2] = {nullptr, nullptr};
-    void* all[12] = {nullptr};
+    // Compression to codes (fac_stream_encode_codes / fac_stream_finish_codes).  Mel frame t reads samples up to 300 t + 600,
+    // so the last frame seen is final only at the end of the stream: codes run one frame behind the encoder.
+    enum EncMode { kEncNone, kEncLatents, kEncCodes, kEncFinished };
+    int enc_mode = kEncNone;                                // which call feeds the encoder half
+    int n_c = 0;                                            // content codebooks of the codes calls
+    long long emitted = 0;                                  // frames of codes written so far
+    float* z_held = nullptr;                                // [B][1024] latent frame `emitted`, quantized by the next call
+    float* mel = nullptr; int mel_cap = 0;                  // [B][mel_cap][80] every mel80 row so far: the timbre pools them all
+    void* all[13] = {nullptr};
 };
 
 // One CNNLSTM predictor head (modules/quantize.py:106-125): 3 ResidualUnits (alias-free SnakeBeta, k7 conv dilation
@@ -997,17 +1005,22 @@ float* redecoder_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes_c,
 
 // mel [B][Tm][80] from wave [B][T] (Tm = T/300), preprocess modules/quantize.py:239-242
 struct MelW { const ConvW* dft; const ConvW* dft_tc; size_t fb; };
+// The tensor-core path: mel frames [f_first, f_first + F) of wave [B][T] (reflected at both ends of the T samples) ->
+// [B][F][80].  Frames gather + K=1 GEMM on the promoted tensor-core kernel (the mel feeds the prosody VQ: fp32-grade sums).
+float* mel_frames_tc(Ctx& c, const MelW& q, const float* wave, int B, int T, int f_first, int F) {
+    float* frames = c.alloc<float>((size_t)B * F * WIN);
+    float* spec = c.alloc<float>((size_t)B * F * SPEC_TC_LD);
+    float* mel = c.alloc<float>((size_t)B * F * N_MELS);
+    if (!c.dry) c.check(launch_stft_frames(wave, frames, B, T, F, HOP, WIN, N_FFT / 2 - (N_FFT - WIN) / 2, c.st, f_first), "mel.frames");
+    run_conv(c, *q.dft_tc, frames, spec, 1, B * F, B * F, ConvOpts(), "mel.dft");
+    if (!c.dry) c.check(launch_mel_from_spec(spec, SPEC_TC_LD, c.W(q.fb), mel, B, F, F, c.st), "mel.fb");
+    return mel;
+}
+MelW quantizer_mel(const fac_handle* h) { return MelW{&h->qw.dft, &h->qw.dft_tc, h->qw.fb}; }
 float* mel_forward(Ctx& c, const float* wave, int B, int T, int Tm, const MelW* mw = nullptr) {
-    MelW q;
-    if (mw) q = *mw; else { q.dft = &c.h->qw.dft; q.dft_tc = &c.h->qw.dft_tc; q.fb = c.h->qw.fb; }
+    const MelW q = mw ? *mw : quantizer_mel(c.h);
     if (c.h->use_tc >= 2 && q.dft_tc->tc) {
-        // frames gather + K=1 GEMM on the promoted tensor-core kernel (the mel feeds the prosody VQ: fp32-grade sums)
-        float* frames = c.alloc<float>((size_t)B * Tm * WIN);
-        float* spec = c.alloc<float>((size_t)B * Tm * SPEC_TC_LD);
-        float* mel = c.alloc<float>((size_t)B * Tm * N_MELS);
-        if (!c.dry) c.check(launch_stft_frames(wave, frames, B, T, Tm, HOP, WIN, N_FFT / 2 - (N_FFT - WIN) / 2, c.st), "mel.frames");
-        run_conv(c, *q.dft_tc, frames, spec, 1, B * Tm, B * Tm, ConvOpts(), "mel.dft");
-        if (!c.dry) c.check(launch_mel_from_spec(spec, SPEC_TC_LD, c.W(q.fb), mel, B, Tm, Tm, c.st), "mel.fb");
+        float* mel = mel_frames_tc(c, q, wave, B, T, 0, Tm);
         c.tap("mel80", mel, (size_t)B * Tm * N_MELS);
         return mel;
     }
@@ -1088,9 +1101,33 @@ float* timbre_gamma_beta(Ctx& c, const float* timbre, int B) {
     return gb;
 }
 
+// The prosody branch (modules/quantize.py:399-404): mel[:, :20] -> melspec_linear -> WN (8 causal k = 5 layers) ->
+// melspec_linear2.  mel [B][Tm][80] -> f0 [B][Tm][1024] in workspace; run with c.vq_critical set.
+float* prosody_forward(Ctx& c, const float* mel, int B, int Tm) {
+    const QuantW& q = c.h->qw;
+    float* px = c.alloc<float>((size_t)B * Tm * 256);
+    float* pin = c.alloc<float>((size_t)B * Tm * 512);
+    float* acts = c.alloc<float>((size_t)B * Tm * 256);
+    float* rs = c.alloc<float>((size_t)B * Tm * 512);
+    float* skip = c.alloc<float>((size_t)B * Tm * 256);
+    float* f0 = c.alloc<float>((size_t)B * Tm * 1024);
+    ConvW lin = q.mel_lin;
+    ConvOpts o;
+    o.ldx = N_MELS;
+    run_conv(c, lin, mel, px, B, Tm, Tm, o, "melspec_linear");
+    if (!c.dry) c.check_nk(cudaMemsetAsync(skip, 0, sizeof(float) * (size_t)B * Tm * 256, c.st), "wn.zero");
+    for (int i = 0; i < 8; ++i) {
+        sconv(c, q.wn_in[i], px, pin, B, Tm, 1, 1, ConvOpts(), "wn.in");
+        if (!c.dry) c.check(launch_wn_gate(pin, acts, (size_t)B * Tm, 256, c.st), "wn.gate");
+        sconv(c, q.wn_rs[i], acts, rs, B, Tm, 1, 1, ConvOpts(), "wn.rs");
+        if (!c.dry) c.check(launch_wn_update(rs, px, skip, (size_t)B * Tm, 256, i == 7, c.st), "wn.upd");
+    }
+    sconv(c, q.mel_lin2, skip, f0, B, Tm, 1, 1, ConvOpts(), "melspec_linear2");
+    return f0;
+}
+
 QuantFront quantizer_front(Ctx& c, const float* wave, int B, int T, const float* full_waves, int T_full, const int64_t* wave_lens,
                            float* timbre) {
-    const QuantW& q = c.h->qw;
     const int Tm = T / HOP;
     const bool was_critical = c.vq_critical;
     c.vq_critical = true;      // quantizer-side layers are tiny: all of them use the promoted kernel
@@ -1111,28 +1148,8 @@ QuantFront quantizer_front(Ctx& c, const float* wave, int B, int T, const float*
         style_encoder(c, mel, B, Tm, nullptr, timbre);
     }
     float* gb = timbre_gamma_beta(c, timbre, B);
-    // --- prosody branch: mel[:, :20] -> melspec_linear -> WN -> melspec_linear2 ---
-    float* px = c.alloc<float>((size_t)B * Tm * 256);
-    float* pin = c.alloc<float>((size_t)B * Tm * 512);
-    float* acts = c.alloc<float>((size_t)B * Tm * 256);
-    float* rs = c.alloc<float>((size_t)B * Tm * 512);
-    float* skip = c.alloc<float>((size_t)B * Tm * 256);
-    float* f0 = c.alloc<float>((size_t)B * Tm * 1024);
-    {
-        ConvW lin = q.mel_lin;
-        ConvOpts o;
-        o.ldx = N_MELS;
-        run_conv(c, lin, mel, px, B, Tm, Tm, o, "melspec_linear");
-        if (!c.dry) c.check_nk(cudaMemsetAsync(skip, 0, sizeof(float) * (size_t)B * Tm * 256, c.st), "wn.zero");
-        for (int i = 0; i < 8; ++i) {
-            sconv(c, q.wn_in[i], px, pin, B, Tm, 1, 1, ConvOpts(), "wn.in");
-            if (!c.dry) c.check(launch_wn_gate(pin, acts, (size_t)B * Tm, 256, c.st), "wn.gate");
-            sconv(c, q.wn_rs[i], acts, rs, B, Tm, 1, 1, ConvOpts(), "wn.rs");
-            if (!c.dry) c.check(launch_wn_update(rs, px, skip, (size_t)B * Tm, 256, i == 7, c.st), "wn.upd");
-        }
-        sconv(c, q.mel_lin2, skip, f0, B, Tm, 1, 1, ConvOpts(), "melspec_linear2");
-        c.tap("f0_input", f0, (size_t)B * Tm * 1024);
-    }
+    float* f0 = prosody_forward(c, mel, B, Tm);
+    c.tap("f0_input", f0, (size_t)B * Tm * 1024);
     c.vq_critical = was_critical;
     QuantFront fr;
     fr.gb = gb; fr.f0 = f0; fr.Tm = Tm;
@@ -1317,7 +1334,7 @@ int fac_destroy(fac_handle* h) {
     if (h->spec_arena) cudaFree(h->spec_arena);
     for (float* p : h->rvq_arenas) if (p) cudaFree(p);
     for (auto* hs : h->heads) { if (hs->arena) cudaFree(hs->arena); delete hs; }
-    for (auto* ss : h->streams) { for (void* p : ss->all) if (p) cudaFree(p); delete ss; }
+    for (auto* ss : h->streams) { for (void* p : ss->all) if (p) cudaFree(p); if (ss->mel) cudaFree(ss->mel); delete ss; }
     delete h;
     return FAC_OK;
 }
@@ -1588,12 +1605,13 @@ int fac_stream_begin(fac_handle* h, int B) {
     cudaSetDevice(h->device);
     auto* s = new fac_handle::Stream();
     s->B = B;
-    const size_t sizes[12] = {
+    const size_t sizes[13] = {
         sizeof(float) * (size_t)B * kEncCtx, sizeof(float) * (size_t)B * 2 * LATENT, sizeof(float) * (size_t)B * 6 * LATENT,
         sizeof(float) * (size_t)B * kDecCtx * 1536,
         sizeof(uint32_t) * 2 * 512 * 32, sizeof(uint32_t) * 2 * 512 * 32, sizeof(float) * 128 * 32 * 8, sizeof(float) * 128 * 32 * 8,
-        sizeof(uint32_t) * 768 * 32, sizeof(uint32_t) * 768 * 32, sizeof(float) * 128 * 32 * 12, sizeof(float) * 128 * 32 * 12};
-    for (int i = 0; i < 12; ++i) {
+        sizeof(uint32_t) * 768 * 32, sizeof(uint32_t) * 768 * 32, sizeof(float) * 128 * 32 * 12, sizeof(float) * 128 * 32 * 12,
+        sizeof(float) * (size_t)B * LATENT};
+    for (int i = 0; i < 13; ++i) {
         cudaError_t e = cudaMalloc(&s->all[i], sizes[i]);
         if (e == cudaSuccess) e = cudaMemset(s->all[i], 0, sizes[i]);
         if (e != cudaSuccess) {
@@ -1607,6 +1625,7 @@ int fac_stream_begin(fac_handle* h, int B) {
     s->x_hist = (float*)s->all[0]; s->ey_hist = (float*)s->all[1]; s->z_hist = (float*)s->all[2]; s->dy_hist = (float*)s->all[3];
     s->enc_h[0] = (uint32_t*)s->all[4]; s->enc_h[1] = (uint32_t*)s->all[5]; s->enc_c[0] = (float*)s->all[6]; s->enc_c[1] = (float*)s->all[7];
     s->dec_h[0] = (uint32_t*)s->all[8]; s->dec_h[1] = (uint32_t*)s->all[9]; s->dec_c[0] = (float*)s->all[10]; s->dec_c[1] = (float*)s->all[11];
+    s->z_held = (float*)s->all[12];
     s->alive = true;
     h->streams.push_back(s);
     return (int)h->streams.size() - 1;
@@ -1619,6 +1638,8 @@ int fac_stream_end(fac_handle* h, int stream_id) {
         cudaSetDevice(h->device);
         cudaDeviceSynchronize();
         for (void*& p : s->all) { if (p) cudaFree(p); p = nullptr; }
+        if (s->mel) cudaFree(s->mel);
+        s->mel = nullptr; s->mel_cap = 0;
         s->alive = false;
     }
     return FAC_OK;
@@ -1635,18 +1656,43 @@ void copy_rows(Ctx& c, float* dst, int dst_pitch_rows, const float* src, int src
 }
 }  // namespace
 
-int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float* z, void* stream) {
-    int rc = check_ready(h, FAC_ENCODER);
-    if (rc) return rc;
-    if (stream_id < 0 || stream_id >= (int)h->streams.size() || !h->streams[stream_id]->alive || !x || !z) { h->err = "fac_stream_encode: bad arguments"; return FAC_ERR_INVALID; }
-    fac_handle::Stream& s = *h->streams[stream_id];
+}  // extern "C"
+
+namespace {
+bool stream_alive(const fac_handle* h, int stream_id) {
+    return stream_id >= 0 && stream_id < (int)h->streams.size() && h->streams[stream_id]->alive;
+}
+
+// The chunk rules and the encoder-half state of fac_stream_encode (mode kEncLatents) / fac_stream_encode_codes (kEncCodes).
+int stream_encode_check(fac_handle* h, const fac_handle::Stream& s, int T, int mode, const char* who) {
+    using S = fac_handle::Stream;
     if (T <= 0 || T % HOP != 0 || (s.enc_samples == 0 && T < kStreamMinFirst * HOP)) {
-        h->err = "fac_stream_encode: chunks must be multiples of 300 samples, the first one at least 3000";
+        h->err = std::string(who) + ": chunks must be multiples of 300 samples, the first one at least 3000";
         return FAC_ERR_INVALID;
     }
-    if (!h->lstm_v2 || !h->enc.lstm.has2[1]) { h->err = "fac_stream_encode: needs the resident-W LSTM kernel"; return FAC_ERR_UNSUPPORTED; }
+    if (s.enc_mode == S::kEncFinished) {
+        h->err = std::string(who) + ": the stream's encoder was closed by fac_stream_finish_codes";
+        return FAC_ERR_STATE;
+    }
+    if (s.enc_mode != S::kEncNone && s.enc_mode != mode) {
+        h->err = std::string(who) + (mode == S::kEncCodes ? ": the stream is already fed by fac_stream_encode (latents)"
+                                                           : ": the stream is already fed by fac_stream_encode_codes");
+        return FAC_ERR_STATE;
+    }
+    if (!h->lstm_v2 || !h->enc.lstm.has2[1]) { h->err = std::string(who) + ": needs the resident-W LSTM kernel"; return FAC_ERR_UNSUPPORTED; }
+    return FAC_OK;
+}
+
+// What the encoder half of a chunk yields: the [x_hist | chunk] window xw [B][Tw] (global samples [enc_samples - hist,
+// enc_samples + T)) and the chunk's channels-last latents znew [B][T/300][1024], both in workspace.
+struct EncChunk { const float* xw; int Tw, hist; const float* znew; };
+
+// The body of fac_stream_encode / fac_stream_encode_codes (checked by stream_encode_check): advances the encoder state by one
+// chunk and hands the chunk to `tail(c, chunk)` inside the same launch sequence.
+template <typename F>
+int stream_encode(fac_handle* h, fac_handle::Stream& s, const float* x, int T, void* stream, int mode, F tail) {
     const int B = s.B, hist = s.x_hist_len, Tw = hist + T, Fc = T / HOP, Fh = hist / HOP;
-    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
         const EncW& e = h->enc;
         c.vq_critical = true;
         float* xw = c.alloc<float>((size_t)B * Tw);
@@ -1670,7 +1716,7 @@ int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float
         o.in_snake = &e.snake;
         sconv(c, e.conv_out, yw, zw, B, yh + Fc, 1, 1, o, "enc.conv_out");
         copy_rows(c, znew, Fc, zw, yh + Fc, yh, Fc, LATENT, B, "stream.znew");
-        if (!c.dry) c.check(launch_transpose(znew, z, B, Fc, LATENT, c.st), "enc.z_T");
+        tail(c, EncChunk{xw, Tw, hist, znew});
         // new histories: the last kEncCtx samples / 2 LSTM-output frames of what has been seen so far
         const int nh = Tw < kEncCtx ? Tw : kEncCtx, nyh = yh + Fc < 2 ? yh + Fc : 2;
         float* tmpx = c.alloc<float>((size_t)B * kEncCtx);
@@ -1683,8 +1729,163 @@ int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float
         s.x_hist_len = Tw < kEncCtx ? Tw : kEncCtx;
         s.ey_hist_len = s.ey_hist_len + Fc < 2 ? s.ey_hist_len + Fc : 2;
         s.enc_samples += T;
+        s.enc_mode = mode;
     }
     return rc;
+}
+
+// Codes of frames [E, E + Fq) (the kCodesOnly VQ kernel): the prosody net recomputed over the stream's mel rows
+// [max(0, E - 32), E + Fq) -- each of the WN's 8 causal k = 5 convs reflect-pads 4 frames at the window's left edge, so the
+// first 32 frames of a window are not those of the whole utterance unless the window starts at frame 0 -- and the latents
+// zq [B][Fq][1024] (row pitch zpitch frames).  Runs with c.vq_critical set, as the offline quantizer.
+void stream_codes(Ctx& c, const fac_handle::Stream& s, long long E, int Fq, const float* zq, int zpitch, int64_t* codes_p,
+                  int64_t* codes_c, int64_t* codes_r) {
+    constexpr int kWnCtx = 32;
+    const int B = s.B, lo = (int)(E > kWnCtx ? E - kWnCtx : 0), Fw = (int)(E + Fq - lo);
+    float* melw = c.alloc<float>((size_t)B * Fw * N_MELS);
+    copy_rows(c, melw, Fw, s.mel, s.mel_cap, lo, Fw, N_MELS, B, "stream.melw");
+    const float* f0 = prosody_forward(c, melw, B, Fw);
+    if (c.dry) return;
+    FaqParams fp;
+    fp.f0 = f0 + (size_t)(E - lo) * LATENT; fp.Tf0 = Fw;
+    fp.z = zq; fp.Tz = zpitch;
+    for (int i = 0; i < 6; ++i) {
+        const VqW& v = c.h->qw.vq[i];
+        fp.vq[i] = VqWeights{c.W(v.w_in), c.W(v.b_in), c.W(v.cb), c.W(v.cbn), c.W(v.cbn2), c.W(v.w_out), c.W(v.b_out)};
+    }
+    fp.n_c = s.n_c;
+    fp.codes_p = codes_p; fp.codes_c = codes_c; fp.codes_r = codes_r;
+    fp.B = B; fp.Tq = Fq;
+    c.check(launch_fa_codes(fp, c.st), "fa_codes");
+}
+
+// Grow-only (doubling) capacity of the stream's mel80 rows; the `emitted` rows written so far move along.
+int grow_mel(fac_handle* h, fac_handle::Stream& s, int rows, cudaStream_t st) {
+    if (rows <= s.mel_cap) return FAC_OK;
+    int cap = s.mel_cap > 0 ? s.mel_cap : 64;
+    while (cap < rows) cap *= 2;
+    cudaError_t e = cudaSetDevice(h->device);
+    float* p = nullptr;
+    if (e == cudaSuccess) e = cudaMalloc(&p, sizeof(float) * (size_t)s.B * cap * N_MELS);
+    if (e == cudaSuccess && s.mel) {
+        e = cudaMemcpy2DAsync(p, sizeof(float) * (size_t)cap * N_MELS, s.mel, sizeof(float) * (size_t)s.mel_cap * N_MELS,
+                              sizeof(float) * (size_t)s.emitted * N_MELS, s.B, cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    }
+    if (e != cudaSuccess) {
+        h->err = std::string("stream mel buffer: ") + cudaGetErrorString(e);
+        cudaGetLastError();
+        if (p) cudaFree(p);
+        return FAC_ERR_CUDA;
+    }
+    if (s.mel) cudaFree(s.mel);
+    s.mel = p; s.mel_cap = cap;
+    return FAC_OK;
+}
+
+// The compressor needs the mel frames cut explicitly (stft_frames, tensor_cores = 2): the FMA path's strided DFT conv
+// reflects at whatever window edge it is given.
+int stream_codes_supported(fac_handle* h, const char* who) {
+    if (h->use_tc >= 2 && h->qw.dft_tc.tc) return FAC_OK;
+    h->err = std::string(who) + ": needs tensor_cores = 2 (the mel path that frames the wave explicitly)";
+    return FAC_ERR_UNSUPPORTED;
+}
+}  // namespace
+
+extern "C" {
+
+int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float* z, void* stream) {
+    int rc = check_ready(h, FAC_ENCODER);
+    if (rc) return rc;
+    if (!stream_alive(h, stream_id) || !x || !z) { h->err = "fac_stream_encode: bad arguments"; return FAC_ERR_INVALID; }
+    fac_handle::Stream& s = *h->streams[stream_id];
+    rc = stream_encode_check(h, s, T, fac_handle::Stream::kEncLatents, "fac_stream_encode");
+    if (rc) return rc;
+    const int B = s.B, Fc = T / HOP;
+    return stream_encode(h, s, x, T, stream, fac_handle::Stream::kEncLatents, [&](Ctx& c, const EncChunk& ch) {
+        if (!c.dry) c.check(launch_transpose(ch.znew, z, B, Fc, LATENT, c.st), "enc.z_T");
+    });
+}
+
+int fac_stream_encode_codes(fac_handle* h, int stream_id, const float* x, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
+                            int64_t* codes_r, void* stream) {
+    using S = fac_handle::Stream;
+    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    const char* who = "fac_stream_encode_codes";
+    if (!stream_alive(h, stream_id) || !x || !codes_p || !codes_c || !codes_r || n_c < 1 || n_c > 2) {
+        h->err = "fac_stream_encode_codes: bad arguments (1 <= n_c <= 2)";
+        return FAC_ERR_INVALID;
+    }
+    S& s = *h->streams[stream_id];
+    int rc = stream_encode_check(h, s, T, S::kEncCodes, who);
+    if (rc) return rc;
+    if (s.enc_mode == S::kEncCodes && n_c != s.n_c) {
+        h->err = "fac_stream_encode_codes: n_c changed mid-stream (" + std::to_string(s.n_c) + " -> " + std::to_string(n_c) + ")";
+        return FAC_ERR_INVALID;
+    }
+    if ((rc = stream_codes_supported(h, who))) return rc;
+    // frames [E, N - 1) are final: frame N - 1 reads 300 samples past what has arrived (reflected only at the true end)
+    const int B = s.B, Fc = T / HOP, first = s.enc_samples == 0;
+    const long long N = (s.enc_samples + T) / HOP, E = s.emitted;
+    const int Fout = (int)(N - 1 - E);
+    if ((rc = grow_mel(h, s, (int)N, (cudaStream_t)stream))) return rc;
+    s.n_c = n_c;
+    rc = stream_encode(h, s, x, T, stream, S::kEncCodes, [&](Ctx& c, const EncChunk& ch) {
+        c.vq_critical = true;
+        const int f_first = (int)(E - (s.enc_samples - ch.hist) / HOP);   // frame E within the window
+        const float* mel = mel_frames_tc(c, quantizer_mel(h), ch.xw, B, ch.Tw, f_first, Fout);
+        copy_rows(c, s.mel + (size_t)E * N_MELS, s.mel_cap, mel, Fout, 0, Fout, N_MELS, B, "stream.mel");
+        // latents of frames [E, N - 1): the held frame (after the first chunk) then all but the chunk's last frame
+        const float* zq = ch.znew;
+        if (!first) {
+            float* zcat = c.alloc<float>((size_t)B * Fout * LATENT);
+            copy_rows(c, zcat, Fout, s.z_held, 1, 0, 1, LATENT, B, "stream.zheld");
+            copy_rows(c, zcat + LATENT, Fout, ch.znew, Fc, 0, Fc - 1, LATENT, B, "stream.zcat");
+            zq = zcat;
+        }
+        stream_codes(c, s, E, Fout, zq, first ? Fc : Fout, codes_p, codes_c, codes_r);
+        copy_rows(c, s.z_held, 1, ch.znew, Fc, Fc - 1, 1, LATENT, B, "stream.zhold");
+    });
+    if (rc == FAC_OK) s.emitted = N - 1;
+    return rc == FAC_OK ? Fout : rc;
+}
+
+int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre,
+                            void* stream) {
+    using S = fac_handle::Stream;
+    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    const char* who = "fac_stream_finish_codes";
+    if (!stream_alive(h, stream_id) || !codes_p || !codes_c || !codes_r) { h->err = "fac_stream_finish_codes: bad arguments"; return FAC_ERR_INVALID; }
+    S& s = *h->streams[stream_id];
+    if (s.enc_mode != S::kEncCodes) {
+        h->err = s.enc_mode == S::kEncFinished ? "fac_stream_finish_codes: the stream's encoder is already finished"
+                                               : "fac_stream_finish_codes: nothing was encoded with fac_stream_encode_codes";
+        return FAC_ERR_STATE;
+    }
+    int rc = stream_codes_supported(h, who);
+    if (rc) return rc;
+    const int B = s.B, hist = s.x_hist_len, N = (int)(s.enc_samples / HOP);
+    const long long E = s.emitted;   // == N - 1
+    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        c.vq_critical = true;
+        // frame N - 1 from the last `hist` samples, reflected at the utterance's true end
+        float* xw = c.alloc<float>((size_t)B * hist);
+        copy_rows(c, xw, hist, s.x_hist, kEncCtx, 0, hist, 1, B, "stream.xfin");
+        const float* mel = mel_frames_tc(c, quantizer_mel(h), xw, B, hist, (int)(E - (s.enc_samples - hist) / HOP), 1);
+        copy_rows(c, s.mel + (size_t)E * N_MELS, s.mel_cap, mel, 1, 0, 1, N_MELS, B, "stream.mel");
+        stream_codes(c, s, E, 1, s.z_held, 1, codes_p, codes_c, codes_r);
+        if (timbre) {
+            // the offline StyleEncoder input: every mel80 row of the utterance
+            float* melall = c.alloc<float>((size_t)B * N * N_MELS);
+            copy_rows(c, melall, N, s.mel, s.mel_cap, 0, N, N_MELS, B, "stream.melall");
+            style_encoder(c, melall, B, N, nullptr, timbre);
+        }
+        c.vq_critical = false;
+    });
+    if (rc != FAC_OK) return rc;
+    s.emitted = N;
+    s.enc_mode = S::kEncFinished;
+    return 1;
 }
 
 }  // extern "C"

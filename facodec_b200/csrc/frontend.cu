@@ -44,23 +44,27 @@ __global__ void __launch_bounds__(128) mel_from_spec_kernel(const float* __restr
     }
 }
 
-// Frame gather for the tensor-core DFT: frames[b][f][j] = wave[b][reflect(f*hop - pad + j)], j < win.  The hop (300) is
-// not a multiple of the 16-channel chunk of the tensor-core conv, so the strided "conv" view of the STFT cannot feed it
-// directly; the explicit [B*F][1200] matrix (49 MB at B=32) can, as a plain K=1 GEMM against the folded basis.
+// Frame gather for the tensor-core DFT: frames[b][f][j] = wave[b][reflect((f_first + f)*hop - pad + j)], j < win, f < F.  The hop
+// (300) is not a multiple of the 16-channel chunk of the tensor-core conv, so the strided "conv" view of the STFT cannot feed
+// it directly; the explicit [B*F][1200] matrix (49 MB at B=32) can, as a plain K=1 GEMM against the folded basis.
+// `wave` is [B][T] (row pitch T) and is reflected at both of its edges.  The streaming compressor passes a [history | chunk]
+// window of the utterance with f_first > 0: it only asks for a frame that reaches past a window edge when that edge is the
+// utterance's true start or end, so the reflection is the offline one.
 __global__ void __launch_bounds__(256) stft_frames_kernel(const float* __restrict__ wave, float* __restrict__ frames, int T,
-                                                          int F, int hop, int win, int pad) {
+                                                          int F, int f_first, int hop, int win, int pad) {
     const int b = blockIdx.y, f = blockIdx.x;
     const PadMap pm = PadMap::make(T, pad, pad, 1);
     const float* w = wave + (size_t)b * T;
     float* o = frames + ((size_t)b * F + f) * win;
     for (int j = threadIdx.x; j < win; j += blockDim.x) {
-        const int src = pm.src(f * hop - pad + j);
+        const int src = pm.src((f_first + f) * hop - pad + j);
         o[j] = src >= 0 ? __ldg(w + src) : 0.f;
     }
 }
-cudaError_t launch_stft_frames(const float* wave, float* frames, int B, int T, int F, int hop, int win, int pad, cudaStream_t st) {
+cudaError_t launch_stft_frames(const float* wave, float* frames, int B, int T, int F, int hop, int win, int pad, cudaStream_t st,
+                               int f_first) {
     if (B <= 0 || F <= 0) return cudaSuccess;
-    stft_frames_kernel<<<dim3(F, B), 256, 0, st>>>(wave, frames, T, F, hop, win, pad);
+    stft_frames_kernel<<<dim3(F, B), 256, 0, st>>>(wave, frames, T, F, f_first, hop, win, pad);
     return cudaGetLastError();
 }
 

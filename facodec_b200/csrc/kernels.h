@@ -99,8 +99,9 @@ cudaError_t lstm_read_phase_clocks(long long* out4);   // CTA-0 accumulated phas
 
 // ---- mel front-end (frontend.cu) -----------------------------------------------------------
 // spec [B][F][ldspec] (re at 2*bin, im at 2*bin+1) -> mel [B][Tm][80] = (log(1e-5 + |.|^2 fb)+4)/4
+// frames [f_first, f_first + F) of the centred STFT of wave [B][T], reflected at both ends of the T samples
 cudaError_t launch_stft_frames(const float* wave, float* frames /*[B][F][win]*/, int B, int T, int F, int hop, int win, int pad,
-                               cudaStream_t st);
+                               cudaStream_t st, int f_first = 0);
 cudaError_t launch_mel_from_spec(const float* spec, int ldspec, const float* fb /*[1025][80]*/, float* mel,
                                  int B, int F, int Tm, cudaStream_t st);
 
@@ -129,6 +130,8 @@ struct FaqParams {
     int B = 0, Tq = 0, Tz = 0, Tf0 = 0;   // Tz / Tf0 = frames per utterance of z / f0 (>= Tq)
 };
 cudaError_t launch_fa_quantize(const FaqParams& p, cudaStream_t st);
+// the codes alone (f0, z, vq, n_c, codes_*, B, Tq, Tz, Tf0 read; gamma_beta, outs, the parts and sqerr neither read nor written)
+cudaError_t launch_fa_codes(const FaqParams& p, cudaStream_t st);
 // FAquantizer from codes: the same six VectorQuantizes' out_proj(codebook[code]) + the AdaLN, no search
 struct DeqParams {
     const int64_t* codes_p = nullptr;   // [B][1][T]

@@ -145,6 +145,9 @@ __device__ __forceinline__ int vq_stage(const VqWeights& W, const float (&r)[32]
 
 // FAquantizer.forward_v2 per frame (eval): prosody RVQ(1) on f0, content RVQ(n_c) on z,
 // residual RVQ(3) on z - z_p - z_c, outs = LN(z_p + z_c + z_r) * gamma + beta.
+// kCodesOnly: the codes alone (the streaming compressor): no AdaLN, no outs / part / sqerr stores, gamma_beta unread.  The
+// searches run the same instructions on the same values, so the codes are those of the full instantiation.
+template <bool kCodesOnly>
 __global__ void __launch_bounds__(128) fa_quantize_kernel(FaqParams p) {
     const int lane = threadIdx.x & 31;
     const int frame = blockIdx.x * 4 + (threadIdx.x >> 5);
@@ -160,9 +163,9 @@ __global__ void __launch_bounds__(128) fa_quantize_kernel(FaqParams p) {
     int idx = vq_stage(p.vq[0], r, zp, se, lane);
     if (lane == 0) {
         p.codes_p[(size_t)b * p.Tq + t] = idx;
-        p.sqerr[(size_t)0 * nframes + frame] = se;
+        if (!kCodesOnly) p.sqerr[(size_t)0 * nframes + frame] = se;
     }
-    if (p.zp) store_frame(p.zp + fo, zp, lane);
+    if (!kCodesOnly && p.zp) store_frame(p.zp + fo, zp, lane);
     // content
     float x[32];
     load_frame(p.z + ((size_t)b * p.Tz + t) * VQ_D, x, lane);
@@ -171,7 +174,7 @@ __global__ void __launch_bounds__(128) fa_quantize_kernel(FaqParams p) {
     idx = vq_stage(p.vq[1], r, zc, se, lane);
     if (lane == 0) {
         p.codes_c[((size_t)b * p.n_c + 0) * p.Tq + t] = idx;
-        p.sqerr[(size_t)1 * nframes + frame] = se;
+        if (!kCodesOnly) p.sqerr[(size_t)1 * nframes + frame] = se;
     }
     if (p.n_c > 1) {
 #pragma unroll
@@ -181,12 +184,12 @@ __global__ void __launch_bounds__(128) fa_quantize_kernel(FaqParams p) {
         for (int i = 0; i < 32; ++i) zc[i] += out[i];
         if (lane == 0) {
             p.codes_c[((size_t)b * p.n_c + 1) * p.Tq + t] = idx;
-            p.sqerr[(size_t)2 * nframes + frame] = se;
+            if (!kCodesOnly) p.sqerr[(size_t)2 * nframes + frame] = se;
         }
-    } else if (lane == 0) {
+    } else if (!kCodesOnly && lane == 0) {
         p.sqerr[(size_t)2 * nframes + frame] = 0.f;
     }
-    if (p.zc) store_frame(p.zc + fo, zc, lane);
+    if (!kCodesOnly && p.zc) store_frame(p.zc + fo, zc, lane);
     // residual feature = x - z_p - z_c
 #pragma unroll
     for (int i = 0; i < 32; ++i) r[i] = (x[i] - zp[i]) - zc[i];
@@ -194,7 +197,7 @@ __global__ void __launch_bounds__(128) fa_quantize_kernel(FaqParams p) {
     idx = vq_stage(p.vq[3], r, zr, se, lane);
     if (lane == 0) {
         p.codes_r[((size_t)b * 3 + 0) * p.Tq + t] = idx;
-        p.sqerr[(size_t)3 * nframes + frame] = se;
+        if (!kCodesOnly) p.sqerr[(size_t)3 * nframes + frame] = se;
     }
 #pragma unroll
     for (int q = 1; q < 3; ++q) {
@@ -205,9 +208,10 @@ __global__ void __launch_bounds__(128) fa_quantize_kernel(FaqParams p) {
         for (int i = 0; i < 32; ++i) zr[i] += out[i];
         if (lane == 0) {
             p.codes_r[((size_t)b * 3 + q) * p.Tq + t] = idx;
-            p.sqerr[(size_t)(3 + q) * nframes + frame] = se;
+            if (!kCodesOnly) p.sqerr[(size_t)(3 + q) * nframes + frame] = se;
         }
     }
+    if (kCodesOnly) return;
     if (p.zr) store_frame(p.zr + fo, zr, lane);
     // outs = LayerNorm(z_p + z_c + z_r) * gamma + beta
 #pragma unroll
@@ -219,7 +223,14 @@ __global__ void __launch_bounds__(128) fa_quantize_kernel(FaqParams p) {
 cudaError_t launch_fa_quantize(const FaqParams& p, cudaStream_t st) {
     int nframes = p.B * p.Tq;
     if (nframes <= 0) return cudaSuccess;
-    fa_quantize_kernel<<<(nframes + 3) / 4, 128, 0, st>>>(p);
+    fa_quantize_kernel<false><<<(nframes + 3) / 4, 128, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_fa_codes(const FaqParams& p, cudaStream_t st) {
+    int nframes = p.B * p.Tq;
+    if (nframes <= 0) return cudaSuccess;
+    fa_quantize_kernel<true><<<(nframes + 3) / 4, 128, 0, st>>>(p);
     return cudaGetLastError();
 }
 

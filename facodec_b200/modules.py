@@ -473,6 +473,7 @@ class CodecStream:
         sid = self.engine.L.fac_stream_begin(self.engine.handle, self.batch)
         _lib.check(self.engine.handle, sid, "fac_stream_begin")
         self.sid = sid
+        self._n_c = 0   # content codebooks of encode_codes (fixed by its first call)
 
     def _check(self, t):
         if t.device.type != "cuda" or (t.device.index if t.device.index is not None else torch.cuda.current_device()) != self.engine.device_index:
@@ -518,6 +519,46 @@ class CodecStream:
                                          _stream(cp.device))
         _lib.check(e.handle, rc, "fac_stream_decode_codes")
         return y
+
+    def encode_codes(self, x, n_c=2):
+        """Compress a chunk: x [B,1,T] (T a multiple of 300; first chunk >= 3000 samples) -> [codes_p [B,1,F], codes_c
+        [B,n_c,F], codes_r [B,3,F]] int64, F = T/300 - 1 on the first call and T/300 after it.  The codes run one frame
+        behind the samples (the last mel frame reads 300 samples past the chunk; finish_codes() emits it), and n_c is fixed
+        by the first call.  Concatenated with finish_codes(), the codes equal Codec.encode(x, n_c) on the whole utterance
+        bit for bit.  A stream is fed either encode() or encode_codes(); decode_codes() runs on its own decoder state and
+        may consume these codes as they come out (with any timbre)."""
+        self._check(x)
+        x = _f32c(x)
+        B, C, T = x.shape
+        assert C == 1 and B == self.batch
+        F = max(T // 300 - (self._n_c == 0), 1)      # the first call holds back one frame
+        dev = x.device
+        cp = torch.empty(B, 1, F, device=dev, dtype=torch.int64)
+        cc = torch.empty(B, n_c, F, device=dev, dtype=torch.int64)
+        cr = torch.empty(B, 3, F, device=dev, dtype=torch.int64)
+        e = self.engine
+        rc = e.L.fac_stream_encode_codes(e.handle, self.sid, _ptr(x), T, int(n_c), _ptr(cp), _ptr(cc), _ptr(cr), _stream(dev))
+        _lib.check(e.handle, rc, "fac_stream_encode_codes")
+        self._n_c = int(n_c)
+        return [cp, cc, cr]
+
+    def finish_codes(self):
+        """End of the utterance: ([codes_p, codes_c, codes_r] of the one held-back frame, timbre [B,1024]).  The timbre is
+        Codec.encode's, bit for bit (the StyleEncoder pools over every mel frame, so it exists only now).  Closes the
+        encoder half of the stream; the decoder half stays usable."""
+        if self.sid is None:
+            raise _lib.FacError("stream is closed")
+        e = self.engine
+        dev = self.device
+        B = self.batch
+        n_c = max(self._n_c, 1)
+        cp = torch.empty(B, 1, 1, device=dev, dtype=torch.int64)
+        cc = torch.empty(B, n_c, 1, device=dev, dtype=torch.int64)
+        cr = torch.empty(B, 3, 1, device=dev, dtype=torch.int64)
+        timbre = torch.empty(B, 1024, device=dev)
+        rc = e.L.fac_stream_finish_codes(e.handle, self.sid, _ptr(cp), _ptr(cc), _ptr(cr), _ptr(timbre), _stream(dev))
+        _lib.check(e.handle, rc, "fac_stream_finish_codes")
+        return [cp, cc, cr], timbre
 
     def close(self):
         if self.sid is not None and self.engine.handle is not None:

@@ -132,15 +132,34 @@ int fac_voice_convert(fac_handle* h, const int64_t* codes_p, const int64_t* code
  * fac_stream_begin(B <= 32) -> stream id (>= 0) or a negative status; one stream holds one encoder and one decoder state.
  * fac_stream_encode: x_chunk [B,1,T] (device; T a multiple of 300, the first chunk >= 3000) -> z_chunk [B,1024,T/300].
  * fac_stream_decode: z_chunk [B,1024,Fc] (device; first chunk >= 10 frames) -> y_chunk [B,1,300*Fc].
- * The quantizer is not part of the stream: its timbre branch pools over the whole utterance (modules/quantize.py:375-454),
- * the VQ lookups themselves are per frame (fac_quantize on each z chunk is exact for the codes).
+ * fac_quantize on each z chunk is NOT exact: only the content codes are per frame of z.  The prosody branch reads a centred
+ * STFT (600 samples of look-ahead per frame, reflected at the wave's ends) through an 8-layer causal WaveNet whose convs
+ * reflect-pad at their left edge, and the residual codes read z - z_p - z_c; the timbre pools over the whole utterance
+ * (modules/quantize.py:228-242, :375-454).  fac_stream_encode_codes / fac_stream_finish_codes carry what that needs.
  * fac_stream_decode_codes: fac_stream_decode on a chunk of codes (Fc frames, arguments as fac_codes_decode); it advances
- * the same decoder state, so one stream should be fed either latents or codes. */
+ * the same decoder state, so one stream should be fed either latents or codes.
+ *
+ * Compression to codes in chunks, with codes and timbre bit-identical to fac_codec_encode on the whole utterance:
+ * fac_stream_encode_codes: x_chunk [B,1,T] (chunk rules of fac_stream_encode), n_c = 1 or 2 for the whole stream ->
+ * codes_p [B,1,F_out], codes_c [B,n_c,F_out], codes_r [B,3,F_out] int64 (device), F_out = T/300 - 1 on the first call and
+ * T/300 after it; returns F_out.  The codes run ONE frame behind the samples: mel frame t reads samples up to 300 t + 600,
+ * so the last frame seen is final only when the stream ends.  fac_stream_finish_codes writes that held-back frame
+ * (codes [B,rows,1]) and, unless `timbre` is NULL, timbre [B,1024] (StyleEncoder over every mel frame of the utterance);
+ * returns 1 and closes the encoder half (the decoder half is untouched: fac_stream_decode_codes may run alongside).
+ * The stream keeps every mel80 row until fac_stream_end: 320 B per frame per utterance, ~92 MB per utterance-hour.
+ * Each chunk recomputes the encoder over a 6000-sample history and the prosody net over <= 32 frames of history.
+ * FAC_ERR_STATE: encode_codes on a stream fed by fac_stream_encode or the reverse, any encode after finish, finish with
+ * nothing encoded; FAC_ERR_INVALID: n_c changed mid-stream; FAC_ERR_UNSUPPORTED unless "tensor_cores" is 2 (the only mel
+ * path that cuts the STFT frames explicitly).  A rejected call leaves the stream as it was. */
 int fac_stream_begin(fac_handle* h, int B);
 int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float* z, void* stream);
 int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, float* y, void* stream);
 int fac_stream_decode_codes(fac_handle* h, int stream_id, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows,
                             const int64_t* codes_r, int n_r_rows, const float* timbre, int Fc, float* y, void* stream);
+int fac_stream_encode_codes(fac_handle* h, int stream_id, const float* x, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
+                            int64_t* codes_r, void* stream);
+int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre,
+                            void* stream);
 int fac_stream_end(fac_handle* h, int stream_id);
 
 /* quantize/rvq.py:27-75 ResidualVQ.forward (eval) over quantize/fvq.py FactorizedVectorQuantize,
