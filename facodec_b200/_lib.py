@@ -82,7 +82,7 @@ def load():
         "fac_debug_tc_pack": ([fp, i32, i32, i32, i32, i32, fp, _c.c_longlong], _c.c_longlong),
         "fac_debug_lstm_phase_clocks": ([vp, _c.POINTER(_c.c_longlong)], i32),
         "fac_set_option": ([vp, _c.c_char_p, i32], i32),
-        "fac_debug_slstm": ([vp, fp, _c.POINTER(vp), i32, i32, i32, fp, vp], i32),
+        "fac_debug_slstm": ([vp, fp, _c.POINTER(vp), i32, i32, i32, i32, _c.POINTER(_c.c_int), i32, fp, vp], i32),
         "fac_debug_fa_quantize": ([vp, fp, fp, _c.POINTER(vp), fp, i32, i32, i32, i32, i32, fp, fp, fp, fp, i64p, i64p, i64p,
                                    fp, fp, vp], i32),
         "fac_debug_attention": ([vp, fp, fp, fp, fp, i32, i32, i32, _c.c_void_p, i32, vp], i32),

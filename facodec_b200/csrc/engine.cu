@@ -808,6 +808,15 @@ void residual_unit(Ctx& c, const ResW& r, const float* x, float* tmp, float* y, 
 // Carried state of one 2-layer SLSTM (streaming): h in the kernel's published fp16 layout, c per CTA.
 struct LstmState { uint32_t* h[2] = {nullptr, nullptr}; float* c[2] = {nullptr, nullptr}; };
 
+// Precision class of slstm's recurrence: 3-pass fp32-faithful upstream of the VQ (and when "decoder_bf16" is off), one fp16
+// pass downstream.
+int lstm_pass3(const Ctx& c) { return (c.vq_critical || !c.h->dec_bf16) ? 1 : 0; }
+// Whether slstm runs the resident-W kernel (lstm2.cu), the only one that can carry a stream's state.
+bool lstm_resident(const Ctx& c, const LstmW& L) {
+    const int pass3 = lstm_pass3(c);
+    return c.h->lstm_v2 && L.has2[pass3] && (pass3 || c.h->dec_lstm_fp16);
+}
+
 // SLSTM (encodec.py:272-288) on channels-last x [B][T][H]; y = lstm2(lstm1(x)) + x.  st (streaming, B <= 32, resident-W
 // kernel only): initial state read from / final state written to st.
 void slstm(Ctx& c, const LstmW& L, const float* x, float* y, int B, int T, LstmState* st = nullptr) {
@@ -822,9 +831,8 @@ void slstm(Ctx& c, const LstmW& L, const float* x, float* y, int B, int T, LstmS
         ConvOpts o;
         run_conv(c, L.ih[l], in, xg, 1, B * T, B * T, o, "lstm.ih");
         if (c.dry) continue;
-        // precision class: 3-pass fp32-faithful upstream of the VQ (and when "decoder_bf16" is off), one fp16 pass downstream
-        const int pass3 = (c.vq_critical || !c.h->dec_bf16) ? 1 : 0;
-        const bool v2 = c.h->lstm_v2 && L.has2[pass3] && (pass3 || c.h->dec_lstm_fp16);
+        const int pass3 = lstm_pass3(c);
+        const bool v2 = lstm_resident(c, L);
         for (int b0 = 0; b0 < B; b0 += 32) {
             int nb = B - b0 < 32 ? B - b0 : 32;
             LstmParams p;
@@ -1605,11 +1613,15 @@ int fac_stream_begin(fac_handle* h, int B) {
     cudaSetDevice(h->device);
     auto* s = new fac_handle::Stream();
     s->B = B;
+    // LSTM states: the encoder's LSTM (H = 1024) runs the 3-pass recurrence, the decoder's (H = 1536) one fp16 pass
+    size_t enc_hw, enc_cf, dec_hw, dec_cf;
+    lstm2_state_sizes(LATENT, lstm_units_per_cta(LATENT), 1, &enc_hw, &enc_cf);
+    lstm2_state_sizes(1536, lstm_units_per_cta(1536), 0, &dec_hw, &dec_cf);
     const size_t sizes[13] = {
         sizeof(float) * (size_t)B * kEncCtx, sizeof(float) * (size_t)B * 2 * LATENT, sizeof(float) * (size_t)B * 6 * LATENT,
         sizeof(float) * (size_t)B * kDecCtx * 1536,
-        sizeof(uint32_t) * 2 * 512 * 32, sizeof(uint32_t) * 2 * 512 * 32, sizeof(float) * 128 * 32 * 8, sizeof(float) * 128 * 32 * 8,
-        sizeof(uint32_t) * 768 * 32, sizeof(uint32_t) * 768 * 32, sizeof(float) * 128 * 32 * 12, sizeof(float) * 128 * 32 * 12,
+        sizeof(uint32_t) * enc_hw, sizeof(uint32_t) * enc_hw, sizeof(float) * enc_cf, sizeof(float) * enc_cf,
+        sizeof(uint32_t) * dec_hw, sizeof(uint32_t) * dec_hw, sizeof(float) * dec_cf, sizeof(float) * dec_cf,
         sizeof(float) * (size_t)B * LATENT};
     for (int i = 0; i < 13; ++i) {
         cudaError_t e = cudaMalloc(&s->all[i], sizes[i]);
@@ -2538,11 +2550,24 @@ int fac_debug_conv(fac_handle* h, const float* x, const float* w_host, const flo
     return FAC_OK;
 }
 
-int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, float* y, void* stream) {
-    if (!h || !x || !w_host || !y || B <= 0 || T <= 0) return FAC_ERR_INVALID;
-    // build a private handle holding only this LSTM, reuse the packing + slstm code path
+int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, int upstream,
+                    const int* chunks, int n_chunks, float* y, void* stream) {
+    if (!h || !x || !w_host || !y || B <= 0 || T <= 0 || n_chunks < 0) return FAC_ERR_INVALID;
+    const bool chunked = chunks && n_chunks > 0;
+    if (chunked) {
+        long long sum = 0;
+        for (int i = 0; i < n_chunks; ++i) {
+            if (chunks[i] <= 0) { h->err = "fac_debug_slstm: chunk lengths must be positive"; return FAC_ERR_INVALID; }
+            sum += chunks[i];
+        }
+        if (sum != T) { h->err = "fac_debug_slstm: chunk lengths must sum to T"; return FAC_ERR_INVALID; }
+    }
+    // build a private handle holding only this LSTM with the caller's precision options, reuse the packing + slstm code path
     fac_handle tmp;
     tmp.device = h->device;
+    tmp.use_tc = h->use_tc; tmp.enc_f16 = h->enc_f16; tmp.enc_tt = h->enc_tt; tmp.tc_occ2 = h->tc_occ2;
+    tmp.dec_bf16 = h->dec_bf16; tmp.dec_c7_f16 = h->dec_c7_f16;
+    tmp.lstm_v2 = h->lstm_v2; tmp.dec_lstm_fp16 = h->dec_lstm_fp16;
     const char* names[8] = {"weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0", "weight_ih_l1", "weight_hh_l1", "bias_ih_l1", "bias_hh_l1"};
     for (int i = 0; i < 8; ++i) {
         HostTensor t;
@@ -2551,24 +2576,46 @@ int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, i
         t.data.assign(w_host[i], w_host[i] + t.numel());
         tmp.host[0][std::string("l.") + names[i]] = std::move(t);
     }
-    tmp.dec_bf16 = h->dec_bf16;     // decoder-class precision (bf16 hi/lo) unless the caller switched it off
-    tmp.lstm_v2 = h->lstm_v2; tmp.dec_lstm_fp16 = h->dec_lstm_fp16;
+    // upstream: packed and run as the encoder's LSTM (promoted input projection, under vq_critical); else as the decoder's
     LstmW L;
-    try { L = pack_lstm(&tmp, 0, "l"); } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_UNSUPPORTED; }
+    try { L = pack_lstm(&tmp, 0, "l", upstream != 0); } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_UNSUPPORTED; }
+    cudaStream_t st = (cudaStream_t)stream;
+    size_t hw = 0, cf = 0;
+    if (chunked) {
+        Ctx probe{&tmp, st, true};
+        probe.vq_critical = upstream != 0;
+        if (B > 32 || !lstm_resident(probe, L)) {
+            h->err = "fac_debug_slstm: chunks need B <= 32 and the resident-W LSTM kernel";
+            return FAC_ERR_UNSUPPORTED;
+        }
+        lstm2_state_sizes(H, L.U, lstm_pass3(probe), &hw, &cf);
+    }
     cudaSetDevice(h->device);
     cudaError_t e = cudaMalloc(&tmp.warena, (tmp.pack.size() + 64) * sizeof(float));
     if (e == cudaSuccess) e = cudaMemcpy(tmp.warena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
-    cudaStream_t st = (cudaStream_t)stream;
-    Ctx dry{&tmp, st, true};
-    slstm(dry, L, x, y, B, T);
-    int rc = ensure_ws(&tmp, dry.off);
-    if (rc == FAC_OK) {
-        Ctx c{&tmp, st, false};
-        slstm(c, L, x, y, B, T);
-        rc = finish(&tmp, c);
-        cudaStreamSynchronize(st);
-    }
+    int rc = two_pass(&tmp, st, [&](Ctx& c) {
+        c.vq_critical = upstream != 0;
+        if (!chunked) { slstm(c, L, x, y, B, T); return; }
+        // chunk by chunk with the state carried as fac_stream_encode / fac_stream_decode do, from a zero state
+        LstmState s;
+        for (int l = 0; l < 2; ++l) {
+            s.h[l] = c.alloc<uint32_t>(hw);
+            s.c[l] = c.alloc<float>(cf);
+            if (c.dry) continue;
+            c.check_nk(cudaMemsetAsync(s.h[l], 0, sizeof(uint32_t) * hw, c.st), "slstm.state_h");
+            c.check_nk(cudaMemsetAsync(s.c[l], 0, sizeof(float) * cf, c.st), "slstm.state_c");
+        }
+        for (int i = 0, t0 = 0; i < n_chunks; t0 += chunks[i++]) {
+            const int n = chunks[i];
+            float* xc = c.alloc<float>((size_t)B * n * H);
+            float* yc = c.alloc<float>((size_t)B * n * H);
+            copy_rows(c, xc, n, x, T, t0, n, H, B, "slstm.xc");
+            slstm(c, L, xc, yc, B, n, &s);
+            copy_rows(c, y + (size_t)t0 * H, T, yc, n, 0, n, H, B, "slstm.yc");
+        }
+    });
+    cudaStreamSynchronize(st);
     if (rc != FAC_OK) h->err = tmp.err;
     cudaFree(tmp.warena);
     if (tmp.ws) cudaFree(tmp.ws);

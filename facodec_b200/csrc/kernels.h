@@ -93,6 +93,8 @@ cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st);   // lstm2
 size_t lstm2_pack_words(int H, int U, int pass3);
 void lstm2_pack(const float* whh, int H, int U, int pass3, uint32_t* out);
 size_t lstm2_smem_bytes(int H, int U, int pass3);
+// sizes of one layer's carried stream state: state_h words and state_c floats
+void lstm2_state_sizes(int H, int U, int pass3, size_t* h_words, size_t* c_floats);
 cudaError_t lstm2_read_phase_clocks(long long* out4);
 int lstm_units_per_cta(int H);
 cudaError_t lstm_read_phase_clocks(long long* out4);   // CTA-0 accumulated phase clocks of the last launch  // U such that H % U == 0 and H / U <= resident CTAs

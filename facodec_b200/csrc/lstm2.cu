@@ -292,6 +292,12 @@ size_t lstm2_smem_bytes(int H, int U, int pass3) {
     return sizeof(uint32_t) * ((size_t)(H / 16) * PL * 8 * R + (size_t)L2_WARPS * depth * PL * 8 * L2_BT) + sizeof(float) * L2_BT * U;
 }
 
+// state_h: [planes][H/2 k pairs][32] words, the layout the kernel publishes h in; state_c: [G][32][U] (per-CTA cell state)
+void lstm2_state_sizes(int H, int U, int pass3, size_t* h_words, size_t* c_floats) {
+    *h_words = (size_t)(pass3 ? 2 : 1) * (H / 2) * L2_BT;
+    *c_floats = (size_t)(H / U) * L2_BT * U;
+}
+
 template <int U, bool PASS3>
 static cudaError_t launch2_u(const LstmParams& p, cudaStream_t st) {
     const size_t smem = lstm2_smem_bytes(p.H, U, PASS3 ? 1 : 0);

@@ -83,8 +83,13 @@ int fac_debug_lstm_phase_clocks(fac_handle* h, long long* out4);
  * non-causal -> 3 taps, out [taps][Cin][s*Cout] (phase-major channels); returns the float count. */
 long long fac_debug_convtr_pack(const float* w_host, int Cin, int Cout, int stride, int causal, float* out,
                                 long long capacity_floats);
-int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, float* y,
-                    void* stream);
+/* fac_debug_slstm (synchronous) runs the LSTM with the precision options set on h.  upstream = 1: packed and run as the
+ * encoder's LSTM (promoted input projection, 3-pass recurrence); 0: as the decoder's.  chunks = NULL or n_chunks = 0: one
+ * pass over all T.  Otherwise chunks (HOST, n_chunks lengths summing to T) runs T chunk by chunk, carrying the LSTM state
+ * from a zero state as the streaming calls do: needs B <= 32 and the resident-W kernel (FAC_ERR_UNSUPPORTED otherwise).
+ * Bad chunk lists return FAC_ERR_INVALID.  Both errors are returned before anything is launched. */
+int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, int upstream,
+                    const int* chunks, int n_chunks, float* y, void* stream);
 /* fa_quantize_kernel + vq_loss_reduce_kernel on caller-given features, the six VectorQuantizes and the AdaLN of
  * FAquantizer.forward_v2 (synchronous).  DEVICE f0 [B][Tf0][1024], z [B][Tz][1024] (Tf0, Tz >= Tq: frame t of
  * utterance b is row b*Tf0 + t / b*Tz + t), gamma_beta [B][2048].  vq_host[i] = HOST {in_w [8][1024], in_b [8],

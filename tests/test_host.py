@@ -316,7 +316,8 @@ int main(void) {
 @pytest.mark.parametrize("H,mode", [(1024, 3), (1024, 2), (1536, 2)])
 def test_lstm2_resident_weight_words(H, mode, built_lib):
     """Host logic (no GPU): lstm2.cu's resident W_hh layout -- fp16 pairs of consecutive k per 32-bit word, XOR-swizzled
-    columns -- decodes back to W_hh (one pass: fp16 rounding 2^-11; three-pass: hi + lo'/2^11 to 2^-20), and every
+    columns -- holds round-to-nearest fp16 planes bit for bit (the rounding test_gpu_lstm.py's emulation assumes), decodes
+    back to W_hh (one pass: fp16 rounding 2^-11; three-pass: hi + lo'/2^11 to 2^-20), and every
     mma.sync fragment load (4 k pairs x 8 rows per instruction) touches 32 distinct shared-memory banks."""
     import ctypes
     import numpy as np
@@ -334,17 +335,23 @@ def test_lstm2_resident_weight_words(H, mode, built_lib):
     assert L.fac_debug_lstm_pack(P(w), H, mode, P(words), n, info) == n
     wv = words.view(np.uint32).reshape(G, H // 16, PL, 8, R)
     swz = (lambda k2: (k2 & 3) << 3) if R == 32 else (lambda k2: ((k2 >> 1) & 1) << 3)
-    ref = w.reshape(4, G, U, H).transpose(1, 0, 2, 3).reshape(G, R, H).astype(np.float64)      # [g][r = gate*U + u][k]
+    w32 = w.reshape(4, G, U, H).transpose(1, 0, 2, 3).reshape(G, R, H)                        # [g][r = gate*U + u][k]
+    ref = w32.astype(np.float64)
+    # the planes bit for bit: hi = rn_f16(w), lo' = rn_f16((w - hi) * 2^11) (numpy's float16 casts round to nearest even)
+    hi_ref = w32.astype(np.float16)
+    planes = [hi_ref, ((w32 - hi_ref.astype(np.float32)) * np.float32(2048)).astype(np.float16)]
     rec = np.zeros((G, R, H))
     for k2 in range(8):
         cols = np.arange(R) ^ swz(k2)
         for pl in range(PL):
             wd = wv[:, :, pl, k2, :][:, :, cols]                                               # [g][sub][r]
-            lo16 = (wd & 0xFFFF).astype(np.uint16).view(np.float16).astype(np.float64)
-            hi16 = (wd >> 16).astype(np.uint16).view(np.float16).astype(np.float64)
+            lo16 = (wd & 0xFFFF).astype(np.uint16).view(np.float16)
+            hi16 = (wd >> 16).astype(np.uint16).view(np.float16)
+            assert np.array_equal(lo16.transpose(0, 2, 1).view(np.uint16), planes[pl][:, :, 2 * k2::16].view(np.uint16))
+            assert np.array_equal(hi16.transpose(0, 2, 1).view(np.uint16), planes[pl][:, :, 2 * k2 + 1::16].view(np.uint16))
             sc = 1.0 if pl == 0 else 1.0 / 2048.0
-            rec[:, :, 2 * k2::16] += sc * lo16.transpose(0, 2, 1)
-            rec[:, :, 2 * k2 + 1::16] += sc * hi16.transpose(0, 2, 1)
+            rec[:, :, 2 * k2::16] += sc * lo16.astype(np.float64).transpose(0, 2, 1)
+            rec[:, :, 2 * k2 + 1::16] += sc * hi16.astype(np.float64).transpose(0, 2, 1)
     tol = 2.0 ** -20 if mode == 3 else 2.0 ** -11
     assert np.abs(rec - ref).max() <= tol * np.abs(ref).max()
     # bank check of one A-fragment load instruction: lanes (fg = row 0..7, ft = k pair 0..3) -> word address ft*R + (row ^ swz)
