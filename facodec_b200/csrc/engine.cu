@@ -88,6 +88,8 @@ struct fac_handle {
     std::vector<RvqSet> rvqs; std::vector<float*> rvq_arenas;
     struct Stream;                  // chunked (streaming) encoder / decoder state (fac_stream_*)
     std::vector<Stream*> streams;
+    struct VcStream;                // chunked voice conversion through the redecoder (fac_vc_stream_*)
+    std::vector<VcStream*> vc_streams;
     struct HeadSet;                 // modules/quantize.py:106-125 CNNLSTM instances (fac_head_*)
     std::vector<HeadSet*> heads;
     char* ws = nullptr; size_t ws_bytes = 0;
@@ -150,6 +152,20 @@ struct fac_handle::Stream {
     float* z_held = nullptr;                                // [B][1024] latent frame `emitted`, quantized by the next call
     float* mel = nullptr; int mel_cap = 0;                  // [B][mel_cap][80] every mel80 row so far: the timbre pools them all
     void* all[13] = {nullptr};
+};
+
+// Streaming voice conversion: the redecoder and its decoder are non-causal but carry no LSTM, so a chunk's outputs depend
+// only on bounded windows of codes and latents on both sides (kVcRedCtx / kVcDecCtx frames, fac_vc_stream_lookahead).
+// Frames [0, Zf) of z and [0, Yf) of the output are final; the device keeps the codes [max(0, Zf - kVcRedCtx), N) and the
+// channels-last z [max(0, Yf - kVcDecCtx), Zf) those windows still need.
+struct fac_handle::VcStream {
+    int B = 0, use_p = 0, use_c = 0, n_c = 0;
+    bool alive = false, finished = false;
+    long long N = 0, Zf = 0, Yf = 0;        // code frames received, z frames final, output frames emitted
+    float* g = nullptr;                     // [B][2 * 512 * 16] cond_layer(timbre), computed once at begin
+    int64_t* codes = nullptr;               // [B][3][kVcCodesHist]: row 0 prosody, rows 1..2 content
+    float* z = nullptr;                     // [B][kVcZHist][1024]
+    void* all[3] = {nullptr, nullptr, nullptr};
 };
 
 // One CNNLSTM predictor head (modules/quantize.py:106-125): 3 ResidualUnits (alias-free SnakeBeta, k7 conv dilation
@@ -964,27 +980,44 @@ void decoder_forward(Ctx& c, const DecW& d, const float* z, int B, int Tf, float
     decoder_stack(c, d, buf[cur], cur, buf, B, t, y);
 }
 
-__global__ void embed_sum_kernel(const int64_t* __restrict__ codes_p, const int64_t* __restrict__ codes_c, int cc_stride,
-                                 const float* __restrict__ ep, const float* __restrict__ ec0, const float* __restrict__ ec1,
-                                 float* __restrict__ out, int T, int hidden, int use_p, int n_c) {
+constexpr int kRedCodes = 1024;   // rows of each embedding table (pack_redecoder)
+
+__global__ void embed_sum_kernel(const int64_t* __restrict__ codes_p, int cp_stride, const int64_t* __restrict__ codes_c,
+                                 int cc_stride, const float* __restrict__ ep, const float* __restrict__ ec0,
+                                 const float* __restrict__ ec1, float* __restrict__ out, int T, int hidden, int use_p, int n_c) {
     // one CTA per (b, t): out[b][t][:] = [use_p] E_p[codes_p[b,0,t]] + sum_{i < n_c} E_c[i][codes_c[b,i,t]]  (redecoder.py:36-46)
+    // codes_p / codes_c rows of utterance b start at b * cp_stride / b * cc_stride; content row i at + i * T.
+    // A code outside [0, kRedCodes) reads nothing and makes the frame's embedding NaN.
     const int bt = blockIdx.x, b = bt / T, t = bt - b * T;
-    const long long ip = use_p ? codes_p[(size_t)b * T + t] : -1;
-    const long long i0 = n_c > 0 ? codes_c[(size_t)b * cc_stride + t] : -1;
-    const long long i1 = n_c > 1 ? codes_c[(size_t)b * cc_stride + T + t] : -1;
+    const long long ip = use_p ? codes_p[(size_t)b * cp_stride + t] : 0;
+    const long long i0 = n_c > 0 ? codes_c[(size_t)b * cc_stride + t] : 0;
+    const long long i1 = n_c > 1 ? codes_c[(size_t)b * cc_stride + T + t] : 0;
+    const bool bad = ip < 0 || ip >= kRedCodes || i0 < 0 || i0 >= kRedCodes || i1 < 0 || i1 >= kRedCodes;
     for (int c = threadIdx.x; c < hidden; c += blockDim.x) {
-        float pe = 0.f, ce = 0.f;                 // the reference sums the prosody and the content embeddings apart
-        if (ip >= 0) pe += ep[(size_t)ip * hidden + c];
-        if (i0 >= 0) ce += ec0[(size_t)i0 * hidden + c];
-        if (i1 >= 0) ce += ec1[(size_t)i1 * hidden + c];
-        out[(size_t)bt * hidden + c] = pe + ce;
+        float v = __int_as_float(0x7fc00000);
+        if (!bad) {
+            float pe = 0.f, ce = 0.f;             // the reference sums the prosody and the content embeddings apart
+            if (use_p) pe += ep[(size_t)ip * hidden + c];
+            if (n_c > 0) ce += ec0[(size_t)i0 * hidden + c];
+            if (n_c > 1) ce += ec1[(size_t)i1 * hidden + c];
+            v = pe + ce;
+        }
+        out[(size_t)bt * hidden + c] = v;
     }
 }
 
-// Redecoder.forward (modules/redecoder.py:35-48): codes -> embeddings -> WN conditioned on the timbre -> conv_out.
-// codes_p [B][1][T], codes_c [B][ncc][T] int64 (device), timbre [B][1024]; returns channels-last z [B][T][1024] in workspace.
-float* redecoder_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes_c, int ncc, const float* timbre, int B, int T,
-                         int use_p, int use_c, int n_c) {
+// cond_layer(timbre) of the redecoder's WN (modules/wavenet.py:143-151): timbre [B][1024] -> g [B][2 * 512 * 16], every
+// layer's slice of the per-utterance conditioning (a Linear per utterance).
+void redecoder_cond(Ctx& c, const float* timbre, int B, float* g) {
+    run_conv(c, c.h->red.cond, timbre, g, 1, B, B, ConvOpts(), "red.cond");
+}
+size_t redecoder_cond_floats(const fac_handle* h, int B) { return (size_t)B * 2 * h->red.hidden * h->red.layers; }
+
+// Redecoder.forward (modules/redecoder.py:35-48) after the cond layer: codes -> embeddings -> WN conditioned on g
+// (redecoder_cond) -> conv_out.  codes_p row b at codes_p + b * cp_stride, codes_c rows at codes_c + b * cc_stride + i * T
+// (int64, device); returns channels-last z [B][T][1024] in workspace.
+float* redecoder_body(Ctx& c, const int64_t* codes_p, int cp_stride, const int64_t* codes_c, int cc_stride, const float* g,
+                      int B, int T, int use_p, int use_c, int n_c) {
     const RedW& r = c.h->red;
     const int Hd = r.hidden;
     float* x = c.alloc<float>((size_t)B * T * Hd);
@@ -992,14 +1025,12 @@ float* redecoder_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes_c,
     float* acts = c.alloc<float>((size_t)B * T * Hd);
     float* rs = c.alloc<float>((size_t)B * T * 2 * Hd);
     float* skip = c.alloc<float>((size_t)B * T * Hd);
-    float* g = c.alloc<float>((size_t)B * 2 * Hd * r.layers);
     float* z = c.alloc<float>((size_t)B * T * LATENT);
     if (!c.dry) {
-        embed_sum_kernel<<<B * T, 128, 0, c.st>>>(codes_p, codes_c, ncc * T, c.W(r.emb_p), c.W(r.emb_c[0]), c.W(r.emb_c[1]), x, T, Hd,
-                                                  use_p, use_c ? n_c : 0);
+        embed_sum_kernel<<<B * T, 128, 0, c.st>>>(codes_p, cp_stride, codes_c, cc_stride, c.W(r.emb_p), c.W(r.emb_c[0]),
+                                                  c.W(r.emb_c[1]), x, T, Hd, use_p ? 1 : 0, use_c ? n_c : 0);
         c.check(cudaGetLastError(), "red.embed");
     }
-    run_conv(c, r.cond, timbre, g, 1, B, B, ConvOpts(), "red.cond");        // cond_layer on g [B,1024,1]: a Linear per utterance
     if (!c.dry) c.check_nk(cudaMemsetAsync(skip, 0, sizeof(float) * (size_t)B * T * Hd, c.st), "red.zero");
     for (int i = 0; i < r.layers; ++i) {
         sconv(c, r.wn_in[i], x, pin, B, T, 1, 1, ConvOpts(), "red.in", false);
@@ -1009,6 +1040,15 @@ float* redecoder_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes_c,
     }
     run_conv(c, r.conv_out, skip, z, B, T, T, ConvOpts(), "red.conv_out");
     return z;
+}
+
+// Redecoder.forward (modules/redecoder.py:35-48): codes_p [B][1][T], codes_c [B][ncc][T] int64 (device), timbre [B][1024];
+// returns channels-last z [B][T][1024] in workspace.
+float* redecoder_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes_c, int ncc, const float* timbre, int B, int T,
+                         int use_p, int use_c, int n_c) {
+    float* g = c.alloc<float>(redecoder_cond_floats(c.h, B));
+    redecoder_cond(c, timbre, B, g);
+    return redecoder_body(c, codes_p, T, codes_c, ncc * T, g, B, T, use_p, use_c, n_c);
 }
 
 // mel [B][Tm][80] from wave [B][T] (Tm = T/300), preprocess modules/quantize.py:239-242
@@ -1343,6 +1383,7 @@ int fac_destroy(fac_handle* h) {
     for (float* p : h->rvq_arenas) if (p) cudaFree(p);
     for (auto* hs : h->heads) { if (hs->arena) cudaFree(hs->arena); delete hs; }
     for (auto* ss : h->streams) { for (void* p : ss->all) if (p) cudaFree(p); if (ss->mel) cudaFree(ss->mel); delete ss; }
+    for (auto* vs : h->vc_streams) { for (void* p : vs->all) if (p) cudaFree(p); delete vs; }
     delete h;
     return FAC_OK;
 }
@@ -1657,18 +1698,19 @@ int fac_stream_end(fac_handle* h, int stream_id) {
     return FAC_OK;
 }
 
+}  // extern "C"
+
 namespace {
-// dst[b][0..n) = src[b][off..off+n) for rows of `w` floats each (row pitches in rows)
-void copy_rows(Ctx& c, float* dst, int dst_pitch_rows, const float* src, int src_pitch_rows, int off_rows, int n_rows, int w, int B,
+// dst[b][0..n) = src[b][off..off+n) for rows of `w` elements each (row pitches in rows)
+template <typename E>
+void copy_rows(Ctx& c, E* dst, int dst_pitch_rows, const E* src, int src_pitch_rows, int off_rows, int n_rows, int w, int B,
                const char* what) {
     if (c.dry || n_rows <= 0) return;
-    c.check_nk(cudaMemcpy2DAsync(dst, sizeof(float) * (size_t)dst_pitch_rows * w, src + (size_t)off_rows * w,
-                                 sizeof(float) * (size_t)src_pitch_rows * w, sizeof(float) * (size_t)n_rows * w, B,
+    c.check_nk(cudaMemcpy2DAsync(dst, sizeof(E) * (size_t)dst_pitch_rows * w, src + (size_t)off_rows * w,
+                                 sizeof(E) * (size_t)src_pitch_rows * w, sizeof(E) * (size_t)n_rows * w, B,
                                  cudaMemcpyDeviceToDevice, c.st), what);
 }
 }  // namespace
-
-}  // extern "C"
 
 namespace {
 bool stream_alive(const fac_handle* h, int stream_id) {
@@ -1979,6 +2021,163 @@ int fac_stream_decode_codes(fac_handle* h, int stream_id, const int64_t* codes_p
     return stream_decode(h, stream_id, Fc, y, stream, "fac_stream_decode_codes", [&](Ctx& c, int B) {
         return (const float*)dequantize_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, Fc, false).outs_cl;
     });
+}
+
+}  // extern "C"
+
+// ---- streaming voice conversion (fac_vc_stream_*): codes -> redecoder -> non-causal decoder on windows ----
+namespace {
+// Reach of the redecoder in code frames: its 16 WN layers are non-causal k = 5 SConv1ds, each reflect-padding (5 - 1) / 2 = 2
+// frames on both sides; the embeddings, the 1x1 res/skip convs and conv_out are per frame.  So z frame t reads codes
+// [t - 32, t + 32], and a window edge that is not the utterance's own corrupts the 32 z frames next to it.
+constexpr int kVcRedCtx = 16 * (5 - 1) / 2;
+
+// Reach of the non-causal decoder in z frames.  z frame f reaches output samples [300 f + lo, 300 f + hi]: conv0 (k 7) reaches
+// +-3 frames; each DecoderBlock of stride s takes input position u through its 3-tap transposed conv (pack_convtr_noncausal:
+// phases r < s/2 also read x[t-1], phases r >= s/2 also read x[t+1]) to outputs [s u - s + s/2, s u + s + s/2 - 1], and its
+// ResidualUnits (k 7, dilations 1, 3, 9) add +-39; conv_out (k 7) adds +-3.  That gives [300 f - 3547, 300 f + 3834]: output
+// frame t (samples [300 t, 300 t + 300)) reads z frames [t - 12, t + 12], and a window edge corrupts the 12 frames next to it.
+constexpr int vc_decoder_reach() {
+    const int rates[4] = {6, 5, 5, 2};
+    int lo = -3, hi = 3;
+    for (int s : rates) { lo = s * lo - s + s / 2 - 39; hi = s * hi + s + s / 2 - 1 + 39; }
+    lo -= 3; hi += 3;
+    const int ahead = (HOP - 1 - lo) / HOP, behind = hi / HOP;
+    return ahead > behind ? ahead : behind;
+}
+constexpr int kVcDecCtx = vc_decoder_reach();
+// Stream state capacities: after every call the codes history is at most 2 * kVcRedCtx frames and the z history at most
+// 2 * kVcDecCtx.
+constexpr int kVcCodesHist = 2 * kVcRedCtx, kVcZHist = 2 * kVcDecCtx;
+
+fac_handle::VcStream* vc_stream(fac_handle* h, int id) {
+    return id >= 0 && id < (int)h->vc_streams.size() && h->vc_streams[id]->alive ? h->vc_streams[id] : nullptr;
+}
+
+// One step of a voice-conversion stream: append F code frames (codes_p [B][1][F], codes_c [B][n_c_rows][F]; F = 0 at
+// finish), make z final up to frame Zf1 and the output up to frame Yf1, and write output frames [Yf, Yf1) to y as
+// [B][1][300 (Yf1 - Yf)].  Both stages run the offline bodies on windows that reach kVcRedCtx / kVcDecCtx frames past the
+// rows they keep, so those rows never see a window edge except the utterance's own (frame 0, and frame N at finish).
+// The state (N, Zf, Yf) is the caller's to advance on success.
+int vc_step(fac_handle* h, fac_handle::VcStream& s, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, int F,
+            long long Zf1, long long Yf1, float* y, void* stream) {
+    auto floor0 = [](long long v) { return v > 0 ? v : 0; };
+    const int B = s.B;
+    const long long N1 = s.N + F, hc0 = floor0(s.Zf - kVcRedCtx), zh0 = floor0(s.Yf - kVcDecCtx);
+    const long long hc1 = floor0(Zf1 - kVcRedCtx), zh1 = floor0(Yf1 - kVcDecCtx);
+    const int Tw = (int)(N1 - hc0), hist = (int)(s.N - hc0), Tz = (int)(Zf1 - zh0), zhist = (int)(s.Zf - zh0);
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        // codes [hc0, N1) as [B][3][Tw]: the history, then the new frames
+        int64_t* cw = c.alloc<int64_t>((size_t)B * 3 * Tw);
+        copy_rows(c, cw, Tw, s.codes, kVcCodesHist, 0, hist, 1, 3 * B, "vc.codes_hist");
+        copy_rows(c, cw + hist, 3 * Tw, codes_p, F, 0, F, 1, B, "vc.codes_p");
+        for (int i = 0; i < s.n_c; ++i)
+            copy_rows(c, cw + (size_t)(1 + i) * Tw + hist, 3 * Tw, codes_c + (size_t)i * F, n_c_rows * F, 0, F, 1, B, "vc.codes_c");
+        if (Zf1 > s.Zf) {
+            // z over the codes window, of which rows [Zf, Zf1) are final; the decoder's window is z [zh0, Zf1)
+            float* zc = redecoder_body(c, cw, 3 * Tw, cw + Tw, 3 * Tw, s.g, B, Tw, s.use_p, s.use_c, s.n_c);
+            float* zw = c.alloc<float>((size_t)B * Tz * LATENT);
+            copy_rows(c, zw, Tz, s.z, kVcZHist, 0, zhist, LATENT, B, "vc.z_hist");
+            copy_rows(c, zw + (size_t)zhist * LATENT, Tz, zc, Tw, (int)(s.Zf - hc0), (int)(Zf1 - s.Zf), LATENT, B, "vc.z_new");
+            if (Yf1 > s.Yf) {
+                const int k = (int)(Yf1 - s.Yf);
+                float* yw = c.alloc<float>((size_t)B * Tz * HOP);
+                decoder_forward(c, h->dec2, zw, B, Tz, yw);
+                copy_rows(c, y, k * HOP, yw, Tz * HOP, (int)(s.Yf - zh0) * HOP, k * HOP, 1, B, "vc.y");
+            }
+            copy_rows(c, s.z, kVcZHist, zw, Tz, (int)(zh1 - zh0), (int)(Zf1 - zh1), LATENT, B, "vc.z_keep");
+        }
+        copy_rows(c, s.codes, kVcCodesHist, cw, Tw, (int)(hc1 - hc0), (int)(N1 - hc1), 1, 3 * B, "vc.codes_keep");
+    });
+}
+}  // namespace
+
+extern "C" {
+
+int fac_vc_stream_lookahead(void) { return kVcRedCtx + kVcDecCtx; }
+
+int fac_vc_stream_begin(fac_handle* h, int B, const float* timbre, int use_p_code, int use_c_code, int n_c, void* stream) {
+    int rc = check_ready(h, FAC_REDECODER);
+    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    if (rc) return rc;
+    if (!timbre || B < 1 || B > 32 || n_c < 0 || n_c > 2) {
+        h->err = "fac_vc_stream_begin: bad arguments (1 <= B <= 32, 0 <= n_c <= 2)";
+        return FAC_ERR_INVALID;
+    }
+    cudaSetDevice(h->device);
+    auto* s = new fac_handle::VcStream();
+    s->B = B; s->use_p = use_p_code ? 1 : 0; s->use_c = use_c_code ? 1 : 0; s->n_c = n_c;
+    const size_t sizes[3] = {sizeof(float) * redecoder_cond_floats(h, B), sizeof(int64_t) * (size_t)B * 3 * kVcCodesHist,
+                             sizeof(float) * (size_t)B * kVcZHist * LATENT};
+    for (int i = 0; i < 3 && rc == FAC_OK; ++i) {
+        cudaError_t e = cudaMalloc(&s->all[i], sizes[i]);
+        if (e != cudaSuccess) {
+            h->err = std::string("fac_vc_stream_begin: ") + cudaGetErrorString(e);
+            cudaGetLastError();
+            rc = FAC_ERR_CUDA;
+        }
+    }
+    s->g = (float*)s->all[0]; s->codes = (int64_t*)s->all[1]; s->z = (float*)s->all[2];
+    if (rc == FAC_OK) rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { redecoder_cond(c, timbre, B, s->g); });
+    if (rc != FAC_OK) {
+        for (void* p : s->all) if (p) cudaFree(p);
+        delete s;
+        return rc;
+    }
+    s->alive = true;
+    h->vc_streams.push_back(s);
+    return (int)h->vc_streams.size() - 1;
+}
+
+int fac_vc_stream_convert(fac_handle* h, int stream_id, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, int F,
+                          float* y, void* stream) {
+    int rc = check_ready(h, FAC_REDECODER);
+    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    if (rc) return rc;
+    fac_handle::VcStream* s = vc_stream(h, stream_id);
+    if (!s || !codes_p || !codes_c || !y || F <= 0 || n_c_rows < s->n_c || n_c_rows > 2) {
+        h->err = "fac_vc_stream_convert: bad arguments (F >= 1, n_c <= rows of codes_c <= 2)";
+        return FAC_ERR_INVALID;
+    }
+    if (s->finished) { h->err = "fac_vc_stream_convert: the stream was finished"; return FAC_ERR_STATE; }
+    const long long N1 = s->N + F;
+    const long long Zf1 = N1 - kVcRedCtx > s->Zf ? N1 - kVcRedCtx : s->Zf;
+    const long long Yf1 = Zf1 - kVcDecCtx > s->Yf ? Zf1 - kVcDecCtx : s->Yf;
+    rc = vc_step(h, *s, codes_p, codes_c, n_c_rows, F, Zf1, Yf1, y, stream);
+    if (rc != FAC_OK) return rc;
+    const int k = (int)(Yf1 - s->Yf);
+    s->N = N1; s->Zf = Zf1; s->Yf = Yf1;
+    return k;
+}
+
+int fac_vc_stream_finish(fac_handle* h, int stream_id, float* y, void* stream) {
+    int rc = check_ready(h, FAC_REDECODER);
+    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    if (rc) return rc;
+    fac_handle::VcStream* s = vc_stream(h, stream_id);
+    if (!s || !y) { h->err = "fac_vc_stream_finish: bad arguments"; return FAC_ERR_INVALID; }
+    if (s->finished || s->N == 0) {
+        h->err = s->finished ? "fac_vc_stream_finish: the stream was finished" : "fac_vc_stream_finish: no codes were received";
+        return FAC_ERR_STATE;
+    }
+    rc = vc_step(h, *s, nullptr, nullptr, 0, 0, s->N, s->N, y, stream);
+    if (rc != FAC_OK) return rc;
+    const int k = (int)(s->N - s->Yf);
+    s->Zf = s->Yf = s->N;
+    s->finished = true;
+    return k;
+}
+
+int fac_vc_stream_end(fac_handle* h, int stream_id) {
+    if (!h || stream_id < 0 || stream_id >= (int)h->vc_streams.size()) return FAC_ERR_INVALID;
+    fac_handle::VcStream* s = h->vc_streams[stream_id];
+    if (s->alive) {
+        cudaSetDevice(h->device);
+        cudaDeviceSynchronize();
+        for (void*& p : s->all) { if (p) cudaFree(p); p = nullptr; }
+        s->alive = false;
+    }
+    return FAC_OK;
 }
 
 // meldataset.py:37-47 preprocess: torchaudio MelSpectrogram(n_mels=80, n_fft=2048, win_length=1200, hop_length=300) with

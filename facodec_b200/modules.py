@@ -170,6 +170,16 @@ def _f32c(t):
     return t.detach().to(torch.float32).contiguous()
 
 
+def _engine_inputs(engine, tensors):
+    """Uploads the engine's weights to the first tensor's device if they changed, and raises FacError for any tensor that is
+    not on the engine's CUDA device (no CPU fallback, no cross-device copies)."""
+    engine.sync_weights(tensors[0].device)
+    for t in tensors:
+        if t.device.type != "cuda" or (t.device.index if t.device.index is not None else torch.cuda.current_device()) != engine.device_index:
+            raise _lib.FacError("all inputs must be on cuda:%d (no CPU fallback, no cross-device copies); got %s"
+                                % (engine.device_index, t.device))
+
+
 def _codes_args(codes, timbre, check_devices):
     """Validates the inputs of the decode-from-codes calls: ``codes`` = [codes_p [B,1,T], codes_c [B,1|2,T], codes_r
     [B,0..3,T] or None] integer tensors and ``timbre`` [B,1024]; ``check_devices`` raises FacError for tensors off the
@@ -261,11 +271,9 @@ class Redecoder(_RefKeyModule):
         self.encoder_type = "wavenet"
 
     def forward(self, p_code, c_code, timbre_vec, use_p_code=True, use_c_code=True, n_c=2):
-        L, h = self._prep(p_code, c_code, timbre_vec)
-        cp = p_code.detach().to(torch.int64).contiguous()
-        cc = c_code.detach().to(torch.int64).contiguous()
-        tv = _f32c(timbre_vec)
-        B, _, T = cp.shape
+        """Codes outside [0, 1024) raise IndexError, as F.embedding does (one device reduction + one host sync)."""
+        cp, cc, _, _, tv, B, T = _codes_args([p_code, c_code, None], timbre_vec, lambda ts: self._prep(*ts))
+        L, h = self._engine.L, self._engine.handle
         if cc.shape[1] < n_c:
             raise IndexError("c_code has %d codebooks, n_c = %d" % (cc.shape[1], n_c))
         z = torch.empty(B, 1024, T, device=cp.device, dtype=torch.float32)
@@ -581,18 +589,81 @@ class VoiceConverter:
         self.engine = model.encoder._engine
 
     def convert(self, codes, timbre, use_p_code=False, use_c_code=True, n_c=1):
+        """codes[0] [B,1,T], codes[1] [B,1|2,T] (codes[2] is not read), timbre [B,1024] -> y [B,1,300 T].  Codes outside
+        [0, 1024) raise IndexError, as F.embedding does (one device reduction + one host sync)."""
         e = self.engine
-        dev = codes[0].device
-        e.sync_weights(dev)
-        cp = codes[0].detach().to(torch.int64).contiguous()
-        cc = codes[1].detach().to(torch.int64).contiguous()
-        tv = _f32c(timbre)
-        B, _, T = cp.shape
+        cp, cc, _, _, tv, B, T = _codes_args([codes[0], codes[1], None], timbre, lambda ts: _engine_inputs(e, ts))
+        dev = cp.device
         y = torch.empty(B, 1, T * 300, device=dev)
         rc = e.L.fac_voice_convert(e.handle, _ptr(cp), _ptr(cc), cc.shape[1], _ptr(tv), B, T, int(bool(use_p_code)),
                                    int(bool(use_c_code)), int(n_c), _ptr(y), _stream(dev))
         _lib.check(e.handle, rc, "fac_voice_convert")
         return y
+
+
+class VoiceConversionStream:
+    """Voice conversion in chunks (reconstruct_redecoder.py:118-121 on a live signal): codes in, converted audio out, with
+    the concatenated output bit-identical to ONE VoiceConverter.convert(codes, timbre, use_p_code, use_c_code, n_c) on the
+    whole utterance.  ``redecoder_model`` is a build_model(stage='redecoder') Munch; ``timbre`` [batch, 1024] (the target
+    voice, e.g. Codec.encode of a reference clip) is fixed for the stream.  The redecoder and its decoder are non-causal, so
+    output frame t comes out once code frames up to t + lookahead_frames (44 frames, 550 ms) are in; finish() flushes the
+    rest.  The codes and latents those windows need live on the device between calls (fac_vc_stream_*)."""
+
+    def __init__(self, redecoder_model, batch, timbre, use_p_code=False, use_c_code=True, n_c=1):
+        self.model = redecoder_model
+        self.engine = e = redecoder_model.encoder._engine
+        self.sid = None
+        self.batch = int(batch)
+        _engine_inputs(e, [timbre])
+        self.device = torch.device("cuda", e.device_index)
+        self._timbre = _f32c(timbre)          # kept alive until the cond layer has read it; the shape check of convert()
+        if tuple(self._timbre.shape) != (self.batch, 1024):
+            raise ValueError("timbre must be [%d, 1024], got %s" % (self.batch, tuple(self._timbre.shape)))
+        self.lookahead_frames = e.L.fac_vc_stream_lookahead()
+        sid = e.L.fac_vc_stream_begin(e.handle, self.batch, _ptr(self._timbre), int(bool(use_p_code)), int(bool(use_c_code)),
+                                      int(n_c), _stream(self.device))
+        _lib.check(e.handle, sid, "fac_vc_stream_begin")
+        self.sid = sid
+
+    def _check(self, tensors):
+        if self.sid is None:
+            raise _lib.FacError("stream is closed")
+        _engine_inputs(self.engine, tensors)
+
+    def convert(self, codes):
+        """codes[0] [B,1,F] and codes[1] [B,1|2,F] (a chunk of CodecStream.encode_codes, or codes as VoiceConverter.convert
+        takes them; codes[2] is not read), F >= 1 -> y [B,1,300 k]: the next k converted frames, 0 <= k <= F (k = 0 until
+        lookahead_frames frames are in).  Codes outside [0, 1024) raise IndexError (one device reduction + one host sync)."""
+        if len(codes) < 2 or codes[0].dim() != 3 or codes[0].shape[0] != self.batch:
+            raise ValueError("codes must be [codes_p [%d, 1, F], codes_c [%d, 1|2, F], ...]" % (self.batch, self.batch))
+        cp, cc, _, _, _, B, F = _codes_args([codes[0], codes[1], None], self._timbre, self._check)
+        e = self.engine
+        y = torch.empty(B * 300 * F, device=self.device)
+        k = e.L.fac_vc_stream_convert(e.handle, self.sid, _ptr(cp), _ptr(cc), cc.shape[1], F, _ptr(y), _stream(self.device))
+        _lib.check(e.handle, k, "fac_vc_stream_convert")
+        return y[:B * 300 * k].view(B, 1, 300 * k)
+
+    def finish(self):
+        """End of the utterance -> y [B,1,300 k], the last k <= lookahead_frames frames."""
+        if self.sid is None:
+            raise _lib.FacError("stream is closed")
+        e = self.engine
+        B = self.batch
+        y = torch.empty(B * 300 * self.lookahead_frames, device=self.device)
+        k = e.L.fac_vc_stream_finish(e.handle, self.sid, _ptr(y), _stream(self.device))
+        _lib.check(e.handle, k, "fac_vc_stream_finish")
+        return y[:B * 300 * k].view(B, 1, 300 * k)
+
+    def close(self):
+        if self.sid is not None and self.engine.handle is not None:
+            self.engine.L.fac_vc_stream_end(self.engine.handle, self.sid)
+        self.sid = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 class _HeadLinear(nn.Module):

@@ -117,12 +117,37 @@ int fac_codes_decode(fac_handle* h, const int64_t* codes_p, const int64_t* codes
  * modules/redecoder.py:35-48: codes_p [B,1,T], codes_c [B,n_c_rows,T] int64 (device; the codec's codes[0], codes[1]),
  * timbre [B,1024] -> z [B,1024,T].  n_c <= n_c_rows <= 2 content codebooks are summed.
  * fac_redecoder_decode = that model's decoder (non-causal, no SLSTM: config_redecoder.yml decoder_causal / decoder_lstm),
- * z [B,1024,Tf] -> y [B,1,300*Tf].  fac_voice_convert runs both with the latents kept channels-last on the device. */
+ * z [B,1024,Tf] -> y [B,1,300*Tf].  fac_voice_convert runs both with the latents kept channels-last on the device.
+ * A code the call reads (codes_p when use_p_code, content rows < n_c when use_c_code) outside [0, 1024) is never read past the
+ * embedding tables: it makes its frame's embedding NaN, which the WN spreads to the z frames within 32 of it. */
 int fac_redecode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre,
                  int B, int T, int use_p_code, int use_c_code, int n_c, float* z, void* stream);
 int fac_redecoder_decode(fac_handle* h, const float* z, int B, int Tf, float* y, void* stream);
 int fac_voice_convert(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre,
                       int B, int T, int use_p_code, int use_c_code, int n_c, float* y, void* stream);
+
+/* Voice conversion in chunks, bit-identical to fac_voice_convert on the whole utterance.  The redecoder and its decoder are
+ * non-causal but hold no LSTM, so the output needs a fixed look-ahead and no recurrent state.  z frame t reads codes
+ * [t - 32, t + 32] (16 WN layers of k = 5 convs, reflect-padded 2 frames per side), and output frame t (samples
+ * [300 t, 300 t + 300)) reads z frames [t - 12, t + 12] (the decoder's centred convs and 3-tap transposed convs).  Output
+ * frame t is therefore final once codes up to frame t + 44 have arrived: fac_vc_stream_lookahead() = 44 frames, 550 ms at
+ * 24 kHz.  Each call recomputes the redecoder over <= 32 frames of code history plus 32 of look-ahead, and the decoder over
+ * <= 12 + 12 frames of z; windows reflect only at the utterance's true start (frame 0) and, at finish, its true end.
+ * fac_vc_stream_begin(B <= 32, timbre [B,1024] device, use_p_code, use_c_code, n_c <= 2) -> stream id (>= 0) or a negative
+ * status; the timbre's cond layer runs once here.
+ * fac_vc_stream_convert: codes_p [B,1,F], codes_c [B,n_c_rows,F] int64 (device; the codec's codes[0], codes[1], e.g. a chunk
+ * of fac_stream_encode_codes), F >= 1 new frames -> returns k (0 <= k <= F; 0 for the first 44 frames received) and writes the
+ * next k output frames to y as [B,1,300*k] (capacity B*300*F floats).
+ * fac_vc_stream_finish: the end of the utterance -> returns k <= 44 (k = min(N, 44) for N frames received) and writes the
+ * last k frames to y as [B,1,300*k] (capacity B*300*44 floats).  A stream shorter than the look-ahead emits everything here.
+ * FAC_ERR_STATE: convert after finish, finish twice, finish with nothing received; FAC_ERR_INVALID: bad B, F <= 0,
+ * n_c > n_c_rows.  A rejected call leaves the stream as it was.  Out-of-range codes behave as in fac_voice_convert. */
+int fac_vc_stream_lookahead(void);
+int fac_vc_stream_begin(fac_handle* h, int B, const float* timbre, int use_p_code, int use_c_code, int n_c, void* stream);
+int fac_vc_stream_convert(fac_handle* h, int stream_id, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, int F,
+                          float* y, void* stream);
+int fac_vc_stream_finish(fac_handle* h, int stream_id, float* y, void* stream);
+int fac_vc_stream_end(fac_handle* h, int stream_id);
 
 /* Streaming (SURVEY.md section 8f rank 4; README.md:105-107 "causal ... can be used for streaming"): the encoder and the codec's
  * decoder are causal, so a long utterance can be processed in chunks with the SAME results as one offline call
