@@ -2311,6 +2311,11 @@ int fac_reconstruction_loss(fac_handle* h, const float* x, const float* gx, int 
                 c.check(launch_strided_sum(tr, (long long)B * F, 2, 1.0 / ((double)B * F * 64.0), sums + 1 + 2 * i, c.st), "loss.l1");
                 c.check(launch_strided_sum(tr + 1, (long long)B * F, 2, 1.0 / ((double)B * F), sums + 2 + 2 * i, c.st), "loss.l2");
             }
+            // before the next scale reuses the scratch (the tap copies are ordered on c.st)
+            const std::string si = std::to_string(i);
+            c.tap(("recon.dft." + si).c_str(), spec, rows * L.ld);
+            c.tap(("recon.terms." + si).c_str(), tr, (size_t)B * F * 2);
+            c.tap(("recon.fb." + si).c_str(), c.W(L.fb), (size_t)L.nb * 64);
             if (c.off > peak) peak = c.off;
         }
         c.vq_critical = false;
@@ -2431,6 +2436,11 @@ int fac_spectral_loss(fac_handle* h, const float* x, const float* y, int B, int 
                 c.check(launch_strided_sum(tr, (long long)B * F, 2, inv, sums + 2 * i, c.st), "spec.mag");
                 c.check(launch_strided_sum(tr + 1, (long long)B * F, 2, inv, sums + 2 * i + 1, c.st), "spec.log");
             }
+            // before the next scale reuses the scratch (the tap copies are ordered on c.st)
+            const std::string si = std::to_string(i);
+            c.tap(("spec.dft." + si).c_str(), spec, rows * L.ld);
+            c.tap(("spec.terms." + si).c_str(), tr, (size_t)B * F * 2);
+            if (L.mel) c.tap(("spec.fb." + si).c_str(), c.W(L.fb), (size_t)L.nb * L.n_out);
             if (c.off > peak) peak = c.off;
         }
         c.vq_critical = false;

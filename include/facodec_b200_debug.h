@@ -109,7 +109,11 @@ int fac_debug_attention(fac_handle* h, const float* q, const float* k, const flo
                         int heads, const int* valid_len, int force_stream, void* stream);
 /* Registers (dst != NULL) or clears a named tap: the next forward copies that channels-last
  * intermediate into dst (DEVICE, up to capacity_floats).  Names: enc_conv0, enc_block1..4,
- * enc_lstm, mel80, f0_input, gamma_beta, dec_conv0, dec_lstm, dec_block1..4. */
+ * enc_lstm, mel80, f0_input, gamma_beta, dec_conv0, dec_lstm, dec_block1..4.
+ * Per scale i of fac_reconstruction_loss ("recon.") and fac_spectral_loss ("spec."): recon.dft.<i> / spec.dft.<i> the
+ * DFT GEMM output [2*B*F][ld] (rows [0, B*F) of x, then those of the second signal; Re at column 2k, Im at 2k + 1,
+ * columns >= 2*nb zero), recon.terms.<i> / spec.terms.<i> the per-frame terms [B*F][2], and recon.fb.<i> / spec.fb.<i>
+ * (mel scales only) the filterbank [nb][n_mels] as the terms kernel reads it. */
 int fac_debug_tap(fac_handle* h, const char* name, float* dst, size_t capacity_floats);
 
 /* Per-kernel-family device timing for bench.py's roofline object: when enabled, every launch of

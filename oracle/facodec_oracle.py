@@ -621,9 +621,10 @@ def reconstruction_loss(x, G_x, eps=1e-7, return_terms=False):
 # and neither audiotools nor librosa is installed or vendored (SURVEY.md 8c).  Their published semantics are restated here;
 # the Slaney filterbank is cross-checked against torchaudio's own Slaney implementation (tests/test_oracle.py).
 # ----------------------------------------------------------------------------
-def librosa_mel_filters(sr, n_fft, n_mels, fmin=0.0, fmax=None):
+def librosa_mel_filters(sr, n_fft, n_mels, fmin=0.0, fmax=None, dtype=torch.float32):
     """librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax) with its defaults (htk=False: Slaney mel scale; norm='slaney':
-    each triangle divided by half its width in Hz), evaluated in float64 and rounded to float32.  Returns [n_mels, 1 + n_fft // 2]."""
+    each triangle divided by half its width in Hz), evaluated in float64 and rounded to ``dtype`` (float32, as librosa
+    returns it; float64 keeps the unrounded values).  Returns [n_mels, 1 + n_fft // 2]."""
     import numpy as np
     fmax = sr / 2.0 if fmax is None else float(fmax)
     f_sp, min_log_hz = 200.0 / 3.0, 1000.0
@@ -638,7 +639,7 @@ def librosa_mel_filters(sr, n_fft, n_mels, fmin=0.0, fmax=None):
     for i in range(n_mels):
         w[i] = np.maximum(0.0, np.minimum(-ramps[i] / fdiff[i], ramps[i + 2] / fdiff[i + 1]))
     w *= (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None]
-    return torch.from_numpy(w.astype(np.float32))
+    return torch.from_numpy(w).to(dtype)
 
 
 def _audiotools_magnitude(x, w):
