@@ -116,8 +116,9 @@ struct fac_handle {
     // and the 64-band HTK filterbank [n_fft/2 + 1][64]; built on first use
     struct LossScale { ConvW dft; size_t fb = 0; int s = 0, nfft = 0, nb = 0, ld = 0; };
     float* loss_arena = nullptr; LossScale loss_scale[6];
-    // dac/nn/loss.py MultiScaleSTFTLoss / MelSpectrogramLoss: one cached configuration (rebuilt when the arguments change)
-    struct SpecScale { ConvW dft; size_t fb = 0; int w = 0, nb = 0, ld = 0, n_out = 0; bool mel = false; };
+    // dac/nn/loss.py MultiScaleSTFTLoss / MelSpectrogramLoss: one cached configuration (rebuilt when the arguments change);
+    // dftT is the same basis transposed ([ld][w]: the gradient GEMM dframes = dspec basis^T)
+    struct SpecScale { ConvW dft, dftT; size_t fb = 0; int w = 0, nb = 0, ld = 0, n_out = 0; bool mel = false; };
     float* spec_arena = nullptr; std::vector<SpecScale> spec_scales; std::vector<double> spec_key;
     // optional per-kernel-family timing (fac_profile_*): CUDA events around every launch
     bool profiling = false;
@@ -2353,9 +2354,13 @@ void slaney_mel_fb(double sr, int n_fft, int n_mels, double fmin, double fmax, s
 }
 }  // namespace
 
-int fac_spectral_loss(fac_handle* h, const float* x, const float* y, int B, int T, int sample_rate, int n_scales, const int* window_lengths,
-                      const int* n_mels, const float* mel_fmin, const float* mel_fmax, float clamp_eps, float mag_weight, float log_weight,
-                      float pw, float* loss, void* stream) {
+// dx / dy (either may be null): dL/dx, dL/dy [B][T].  Per scale, after the loss terms: spec_loss_grad_kernel turns the spec
+// rows of the requested signals into dL/d(Re, Im) in place, the transposed DFT GEMM (same fp32-faithful class) maps them to
+// dL/dframes over the frames buffer, and the overlap-add gather folds those into dx / dy (the first scale writes, the later
+// ones add, on one stream: bit-reproducible).  With both null this is the forward call, launch for launch.
+static int spectral_loss(fac_handle* h, const float* x, const float* y, int B, int T, int sample_rate, int n_scales, const int* window_lengths,
+                         const int* n_mels, const float* mel_fmin, const float* mel_fmax, float clamp_eps, float mag_weight, float log_weight,
+                         float pw, float* loss, float* dx, float* dy, void* stream) {
     if (!h || !x || !y || !loss || !window_lengths || B <= 0 || T <= 0 || n_scales < 1 || n_scales > 16 || sample_rate <= 0) return FAC_ERR_INVALID;
     if (B > 32767) { h->err = "fac_spectral_loss: B > 32767"; return FAC_ERR_UNSUPPORTED; }
     std::vector<double> key{(double)sample_rate, (double)n_scales};
@@ -2395,6 +2400,14 @@ int fac_spectral_loss(fac_handle* h, const float* x, const float* y, int B, int 
                     }
                 }
                 attach_tc(&tmp, d, 1, true);
+                ConvW& dt = L.dftT;
+                dt = ConvW();
+                dt.Cin = L.ld; dt.Cout = L.w; dt.K = 1; dt.ldw = L.w;
+                dt.w = pack_alloc(&tmp, (size_t)L.ld * L.w);
+                dt.b = pack_alloc(&tmp, L.w);
+                for (int n = 0; n < L.w; ++n)
+                    for (int col = 0; col < 2 * L.nb; ++col) tmp.pack[dt.w + (size_t)col * L.w + n] = tmp.pack[d.w + (size_t)n * L.ld + col];
+                attach_tc(&tmp, dt, 1, true);
                 if (L.mel) {
                     std::vector<float> fb;
                     slaney_mel_fb((double)sample_rate, L.w, nm, key[2 + 4 * i + 2], key[2 + 4 * i + 3], fb);
@@ -2441,6 +2454,27 @@ int fac_spectral_loss(fac_handle* h, const float* x, const float* y, int B, int 
             c.tap(("spec.dft." + si).c_str(), spec, rows * L.ld);
             c.tap(("spec.terms." + si).c_str(), tr, (size_t)B * F * 2);
             if (L.mel) c.tap(("spec.fb." + si).c_str(), c.W(L.fb), (size_t)L.nb * L.n_out);
+            if (dx || dy) {
+                // rows of the signals whose gradient is asked for: [0, B*F) x, [B*F, 2*B*F) y
+                const size_t r0 = dx ? 0 : (size_t)B * F, nr = (dx && dy) ? rows : (size_t)B * F;
+                float* inv = c.alloc<float>(rows);                   // per-row inverse scales of the gradient rows
+                if (!c.dry) {
+                    const double n_el = (double)B * F * L.n_out;
+                    c.check(launch_spec_loss_grad(spec, L.ld, L.nb, L.mel ? c.W(L.fb) : nullptr, L.n_out, B, F, clamp_eps, pw,
+                                                  (float)(mag_weight / n_el), (float)(log_weight / n_el), dx != nullptr, dy != nullptr, inv,
+                                                  c.st),
+                            "spec.grad");
+                }
+                run_conv(c, L.dftT, spec + r0 * L.ld, frames + r0 * L.w, 1, (int)nr, (int)nr, ConvOpts(), "spec.dftT");
+                if (!c.dry) {
+                    if (dx) c.check(launch_stft_overlap_add_grad(frames, inv, dx, B, T, F, hop, L.w, L.w / 2, i > 0, c.st), "spec.ola");
+                    if (dy) c.check(launch_stft_overlap_add_grad(frames + (size_t)B * F * L.w, inv + (size_t)B * F, dy, B, T, F, hop, L.w,
+                                                                 L.w / 2, i > 0, c.st),
+                                    "spec.ola");
+                }
+                c.tap(("spec.dframes." + si).c_str(), frames, rows * L.w);
+                c.tap(("spec.dscale." + si).c_str(), inv, rows);
+            }
             if (c.off > peak) peak = c.off;
         }
         c.vq_critical = false;
@@ -2451,8 +2485,23 @@ int fac_spectral_loss(fac_handle* h, const float* x, const float* y, int B, int 
     return rc;
 }
 
+int fac_spectral_loss(fac_handle* h, const float* x, const float* y, int B, int T, int sample_rate, int n_scales, const int* window_lengths,
+                      const int* n_mels, const float* mel_fmin, const float* mel_fmax, float clamp_eps, float mag_weight, float log_weight,
+                      float pw, float* loss, void* stream) {
+    return spectral_loss(h, x, y, B, T, sample_rate, n_scales, window_lengths, n_mels, mel_fmin, mel_fmax, clamp_eps, mag_weight,
+                         log_weight, pw, loss, nullptr, nullptr, stream);
+}
+
+int fac_spectral_loss_grad(fac_handle* h, const float* x, const float* y, int B, int T, int sample_rate, int n_scales,
+                           const int* window_lengths, const int* n_mels, const float* mel_fmin, const float* mel_fmax, float clamp_eps,
+                           float mag_weight, float log_weight, float pw, float* loss, float* dx, float* dy, void* stream) {
+    return spectral_loss(h, x, y, B, T, sample_rate, n_scales, window_lengths, n_mels, mel_fmin, mel_fmax, clamp_eps, mag_weight,
+                         log_weight, pw, loss, dx, dy, stream);
+}
+
 // dac/nn/loss.py:11-47 L1Loss on the waveforms: mean |x - y| over n floats
-int fac_l1_loss(fac_handle* h, const float* x, const float* y, long long n, float* loss, void* stream) {
+// (dx / dy: null, or dL/dx = sgn(x - y) / n and dL/dy = -dL/dx)
+static int l1_loss(fac_handle* h, const float* x, const float* y, long long n, float* loss, float* dx, float* dy, void* stream) {
     if (!h || !x || !y || !loss || n <= 0) return FAC_ERR_INVALID;
     cudaSetDevice(h->device);
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
@@ -2463,8 +2512,15 @@ int fac_l1_loss(fac_handle* h, const float* x, const float* y, long long n, floa
             c.check(launch_absdiff_partial(x, y, n, part, nblk, c.st), "l1.partial");
             c.check(launch_strided_sum(part, nblk, 1, 1.0 / (double)n, sum, c.st), "l1.sum");
             c.check(launch_spec_loss_combine(sum, 0, 0.f, 0.f, loss, c.st), "l1.out");
+            if (dx || dy) c.check(launch_l1_grad(x, y, n, (float)(1.0 / (double)n), dx, dy, c.st), "l1.grad");
         }
     });
+}
+int fac_l1_loss(fac_handle* h, const float* x, const float* y, long long n, float* loss, void* stream) {
+    return l1_loss(h, x, y, n, loss, nullptr, nullptr, stream);
+}
+int fac_l1_loss_grad(fac_handle* h, const float* x, const float* y, long long n, float* loss, float* dx, float* dy, void* stream) {
+    return l1_loss(h, x, y, n, loss, dx, dy, stream);
 }
 
 // ---- predictor heads (SURVEY.md 8f rank 1; training-side in the reference, forward only here) ----

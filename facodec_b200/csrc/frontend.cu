@@ -287,6 +287,181 @@ cudaError_t launch_absdiff_partial(const float* a, const float* b, long long n, 
     return cudaGetLastError();
 }
 
+// ---- gradients of the spectral losses (fac_spectral_loss_grad) -------------------------------------------------------
+// One CTA per (frame, utterance), run after spec_loss_terms_kernel has read `spec`.  Recomputes |X|, |Y| and (mel scales)
+// v = |.| @ fb with the terms kernel's arithmetic, so every sign below is the one the returned loss saw, then forms per
+// requested signal
+//   dL/dvx = mag_scale * sgn(vx - vy) + log_scale * sgn(log10 lx - log10 ly) * pw / (vx ln 10)   (log part only where vx >= eps)
+// (dL/dvy the same with the signs negated and vy; mag_scale = mag_weight / N, log_scale = log_weight / N, N = B * F * n_out:
+// the nn.L1Loss means), chains it through the filterbank transpose (d|X|_k = sum_o fb[k][o] dv_o, one warp per k, fixed
+// butterfly order) and the complex magnitude (dRe = d|X| Re / |X|, dIm = d|X| Im / |X|, 0 where |X| = 0, as torch's sgn),
+// and writes dRe, dIm in place over that signal's spec row; columns >= 2 * nb are zeroed.
+// Each row is written scaled by a power of two 2^k chosen from the frame's largest |dL/d|.||, which bounds every |dRe|,
+// |dIm| of the row: the scaled row's largest entry lies in [2^13, 2^14).  The gradients carry the loss's 1 / N mean factor
+// (1e-9 ... 1e-6 at the benchmark shape), below fp16's normal range, and the gradient GEMM's promoted class splits its
+// activations into fp16 hi + 2^11-scaled fp16 lo without a scale of its own; scaled, they keep its 22 significant bits.
+// inv_scale[row] = 2^-k (rows as in spec: x, then y) is applied by the overlap-add.  Both scalings are exact in fp32.
+__global__ void __launch_bounds__(128) spec_loss_grad_kernel(float* __restrict__ spec, int ldspec, int nb, const float* __restrict__ fb,
+                                                             int n_out, int B, int F, float eps, float pw, float mag_scale, float log_scale,
+                                                             int want_x, int want_y, float* __restrict__ inv_scale) {
+    extern __shared__ float sg[];
+    float* mg = sg;                                  // [2][nb] magnitudes
+    float* dv = sg + 2 * nb;                         // [2][n_out] dL/dv of x, y (no filterbank: dL/d|.| itself)
+    float* dm = fb ? dv + 2 * n_out : dv;            // [2][nb] dL/d|.|
+    const int b = blockIdx.y, f = blockIdx.x, tid = threadIdx.x;
+    float* rx = spec + ((size_t)b * F + f) * ldspec;
+    float* ry = spec + ((size_t)(B + b) * F + f) * ldspec;
+    for (int i = tid; i < nb; i += blockDim.x) {
+        const float2 cx = *reinterpret_cast<const float2*>(rx + 2 * i), cy = *reinterpret_cast<const float2*>(ry + 2 * i);
+        mg[i] = sqrtf(cx.x * cx.x + cx.y * cx.y);
+        mg[nb + i] = sqrtf(cy.x * cy.x + cy.y * cy.y);
+    }
+    __syncthreads();
+    const float inv_ln10 = 0.43429448190325182f;
+    for (int o = tid; o < n_out; o += blockDim.x) {
+        float vx, vy;
+        if (fb) {
+            float a0 = 0.f, a1 = 0.f, c0 = 0.f, c1 = 0.f;
+            int i = 0;
+            for (; i + 1 < nb; i += 2) {
+                const float w0 = __ldg(fb + (size_t)i * n_out + o), w1 = __ldg(fb + (size_t)(i + 1) * n_out + o);
+                a0 = fmaf(mg[i], w0, a0); a1 = fmaf(mg[i + 1], w1, a1);
+                c0 = fmaf(mg[nb + i], w0, c0); c1 = fmaf(mg[nb + i + 1], w1, c1);
+            }
+            if (i < nb) { const float w0 = __ldg(fb + (size_t)i * n_out + o); a0 = fmaf(mg[i], w0, a0); c0 = fmaf(mg[nb + i], w0, c0); }
+            vx = a0 + a1; vy = c0 + c1;
+        } else {
+            vx = mg[o]; vy = mg[nb + o];
+        }
+        float lx = fmaxf(vx, eps), ly = fmaxf(vy, eps);
+        if (pw == 2.0f) { lx *= lx; ly *= ly; }
+        else if (pw != 1.0f) { lx = powf(lx, pw); ly = powf(ly, pw); }
+        const float dl = log10f(lx) - log10f(ly);
+        const float s_mag = (float)((vx > vy) - (vx < vy)), s_log = (float)((dl > 0.f) - (dl < 0.f));
+        float gx = mag_scale * s_mag, gy = -gx;
+        if (vx >= eps) gx += log_scale * s_log * (pw * inv_ln10 / vx);
+        if (vy >= eps) gy -= log_scale * s_log * (pw * inv_ln10 / vy);
+        dv[o] = gx; dv[n_out + o] = gy;
+    }
+    __syncthreads();
+    if (fb) {
+        const int warp = tid >> 5, lane = tid & 31;
+        for (int k = warp; k < nb; k += blockDim.x >> 5) {
+            const float* row = fb + (size_t)k * n_out;
+            float ax = 0.f, ay = 0.f;
+            for (int o = lane; o < n_out; o += 32) {
+                const float w = __ldg(row + o);
+                ax = fmaf(w, dv[o], ax); ay = fmaf(w, dv[n_out + o], ay);
+            }
+            ax = warp_sum(ax); ay = warp_sum(ay);
+            if (lane == 0) { dm[k] = ax; dm[nb + k] = ay; }
+        }
+        __syncthreads();
+    }
+    // per-signal power-of-two row scale from max |dL/d|.||
+    __shared__ float red[4][2];
+    __shared__ float row_scale[2];
+    float mx = 0.f, my = 0.f;
+    for (int i = tid; i < nb; i += blockDim.x) { mx = fmaxf(mx, fabsf(dm[i])); my = fmaxf(my, fabsf(dm[nb + i])); }
+    for (int o = 16; o > 0; o >>= 1) {
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        my = fmaxf(my, __shfl_xor_sync(0xffffffffu, my, o));
+    }
+    if ((tid & 31) == 0) { red[tid >> 5][0] = mx; red[tid >> 5][1] = my; }
+    __syncthreads();
+    if (tid < 2) {
+        const float m = fmaxf(fmaxf(red[0][tid], red[1][tid]), fmaxf(red[2][tid], red[3][tid]));
+        int k = 0;
+        if (m > 0.f) {
+            int e;
+            frexpf(m, &e);                               // m in [2^(e-1), 2^e)
+            k = min(max(14 - e, -126), 126);
+        }
+        row_scale[tid] = ldexpf(1.f, k);
+        if ((tid == 0 && want_x) || (tid == 1 && want_y)) inv_scale[(size_t)(tid * B + b) * F + f] = ldexpf(1.f, -k);
+    }
+    __syncthreads();
+    const float sx = row_scale[0], sy = row_scale[1];
+    for (int i = tid; i < nb; i += blockDim.x) {
+        if (want_x) {
+            const float2 c = *reinterpret_cast<const float2*>(rx + 2 * i);
+            const float m = mg[i], g = dm[i] * sx;
+            *reinterpret_cast<float2*>(rx + 2 * i) = m > 0.f ? make_float2(g * (c.x / m), g * (c.y / m)) : make_float2(0.f, 0.f);
+        }
+        if (want_y) {
+            const float2 c = *reinterpret_cast<const float2*>(ry + 2 * i);
+            const float m = mg[nb + i], g = dm[nb + i] * sy;
+            *reinterpret_cast<float2*>(ry + 2 * i) = m > 0.f ? make_float2(g * (c.x / m), g * (c.y / m)) : make_float2(0.f, 0.f);
+        }
+    }
+    for (int j = 2 * nb + tid; j < ldspec; j += blockDim.x) {
+        if (want_x) rx[j] = 0.f;
+        if (want_y) ry[j] = 0.f;
+    }
+}
+cudaError_t launch_spec_loss_grad(float* spec, int ldspec, int nb, const float* fb, int n_out, int B, int F, float eps, float pw,
+                                  float mag_scale, float log_scale, int want_x, int want_y, float* inv_scale, cudaStream_t st) {
+    if (B <= 0 || F <= 0 || !(want_x || want_y)) return cudaSuccess;
+    if (B > 65535) return cudaErrorInvalidValue;
+    const size_t smem = (size_t)(2 * nb + 2 * n_out + (fb ? 2 * nb : 0)) * sizeof(float);
+    if (smem > 48 * 1024) return cudaErrorInvalidValue;
+    spec_loss_grad_kernel<<<dim3(F, B), 128, smem, st>>>(spec, ldspec, nb, fb, n_out, B, F, eps, pw, mag_scale, log_scale, want_x, want_y,
+                                                         inv_scale);
+    return cudaGetLastError();
+}
+
+// Adjoint of stft_frames_kernel (f_first = 0): a deterministic gather, no atomics.  out[b][t] is the sum of
+// dframes[b][f][j] * inv_scale[b][f] (the row scales of spec_loss_grad_kernel) over every (f, j) that read sample t: padded
+// position t + pad itself and, for the reflect padding, the mirrored positions pad - t (left edge, 1 <= t <= pad) and
+// pad + 2 (T - 1) - t (right edge, T - 1 - pad <= t <= T - 2), in that order, frames ascending -- the fold torch's
+// reflect-pad backward does.  accumulate = 0 writes, 1 adds (the later scales of one loss).
+__global__ void __launch_bounds__(256) stft_overlap_add_grad_kernel(const float* __restrict__ dframes, const float* __restrict__ inv_scale,
+                                                                    float* __restrict__ out, int T, int F, int hop, int win, int pad,
+                                                                    int accumulate) {
+    const int b = blockIdx.y, t = blockIdx.x * 256 + threadIdx.x;
+    if (t >= T) return;
+    const float* d = dframes + (size_t)b * F * win;
+    const float* is = inv_scale + (size_t)b * F;
+    int pos[3], n = 0;
+    pos[n++] = t + pad;
+    if (t >= 1 && t <= pad) pos[n++] = pad - t;
+    if (t >= T - 1 - pad && t <= T - 2) pos[n++] = pad + 2 * (T - 1) - t;
+    float s = 0.f;
+    for (int q = 0; q < n; ++q) {
+        const int P = pos[q];
+        const int f0 = P - win + 1 > 0 ? (P - win + hop) / hop : 0;     // first frame reaching P
+        const int f1 = P / hop < F - 1 ? P / hop : F - 1;               // last frame starting at or before P
+        for (int fr = f0; fr <= f1; ++fr) s += d[(size_t)fr * win + (P - fr * hop)] * __ldg(is + fr);
+    }
+    float* o = out + (size_t)b * T + t;
+    *o = accumulate ? *o + s : s;
+}
+cudaError_t launch_stft_overlap_add_grad(const float* dframes, const float* inv_scale, float* out, int B, int T, int F, int hop, int win,
+                                         int pad, int accumulate, cudaStream_t st) {
+    if (B <= 0 || T <= 0) return cudaSuccess;
+    if (B > 65535) return cudaErrorInvalidValue;
+    stft_overlap_add_grad_kernel<<<dim3((T + 255) / 256, B), 256, 0, st>>>(dframes, inv_scale, out, T, F, hop, win, pad, accumulate);
+    return cudaGetLastError();
+}
+
+// d/da mean |a - b| = sgn(a - b) / n (torch's sign: 0 where a == b); db = -da.  da / db may each be null.
+__global__ void __launch_bounds__(256) l1_grad_kernel(const float* __restrict__ a, const float* __restrict__ b, long long n, float inv_n,
+                                                      float* __restrict__ da, float* __restrict__ db) {
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const float d = a[i] - b[i];
+        const float g = d > 0.f ? inv_n : (d < 0.f ? -inv_n : 0.f);
+        if (da) da[i] = g;
+        if (db) db[i] = -g;
+    }
+}
+cudaError_t launch_l1_grad(const float* a, const float* b, long long n, float inv_n, float* da, float* db, cudaStream_t st) {
+    if (n <= 0 || !(da || db)) return cudaSuccess;
+    long long blocks = (n + 255) / 256;
+    if (blocks > 148 * 16) blocks = 148 * 16;
+    l1_grad_kernel<<<(unsigned)blocks, 256, 0, st>>>(a, b, n, inv_n, da, db);
+    return cudaGetLastError();
+}
+
 // loss = sum over scales of (log_weight * v[2i+1] + mag_weight * v[2i]) accumulated in fp32 in the reference's order
 // (dac/nn/loss.py:217-226: the log term first); n = 0: loss = (float)v[0] (L1Loss)
 __global__ void spec_loss_combine_kernel(const double* __restrict__ v, int n, float mag_weight, float log_weight, float* __restrict__ loss) {

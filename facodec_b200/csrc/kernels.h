@@ -173,6 +173,14 @@ cudaError_t launch_spec_loss_terms(const float* spec, int ldspec, int nb, const 
                                    float eps, float pw, float* terms /*[B*F][2]*/, cudaStream_t st);
 cudaError_t launch_absdiff_partial(const float* a, const float* b, long long n, float* part, int nblocks, cudaStream_t st);
 cudaError_t launch_spec_loss_combine(const double* v, int n, float mag_weight, float log_weight, float* loss, cudaStream_t st);
+// their gradients (fac_spectral_loss_grad / fac_l1_loss_grad): dL/d(Re, Im) in place over the spec rows of the requested
+// signals, each row scaled by a power of two whose inverse goes to inv_scale [2*B*F]; the adjoint of launch_stft_frames
+// (f_first = 0) over those scaled rows into out [B][T] (accumulate: add instead of write); sgn(a - b) / n
+cudaError_t launch_spec_loss_grad(float* spec, int ldspec, int nb, const float* fb, int n_out, int B, int F, float eps, float pw,
+                                  float mag_scale, float log_scale, int want_x, int want_y, float* inv_scale, cudaStream_t st);
+cudaError_t launch_stft_overlap_add_grad(const float* dframes /*[B][F][win]*/, const float* inv_scale /*[B][F]*/, float* out, int B, int T,
+                                         int F, int hop, int win, int pad, int accumulate, cudaStream_t st);
+cudaError_t launch_l1_grad(const float* a, const float* b, long long n, float inv_n, float* da, float* db, cudaStream_t st);
 cudaError_t launch_add3(const float* a, const float* b, const float* c /* or null */, long long n, float* out, cudaStream_t st);
 cudaError_t launch_loss_combine(const double* v13, float* loss, float* terms, cudaStream_t st);
 cudaError_t launch_transpose(const float* in, float* out, int B, int R, int C, cudaStream_t st);  // [B][R][C]->[B][C][R]

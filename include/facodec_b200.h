@@ -228,6 +228,15 @@ int fac_spectral_loss(fac_handle* h, const float* x, const float* y, int B, int 
                       const int* window_lengths, const int* n_mels, const float* mel_fmin, const float* mel_fmax, float clamp_eps,
                       float mag_weight, float log_weight, float pow, float* loss, void* stream);
 int fac_l1_loss(fac_handle* h, const float* x, const float* y, long long n, float* loss, void* stream);
+/* The same losses with their gradients for back-propagation: arguments and errors as above, plus dx / dy ([B,T] device, each
+ * may be NULL) receiving dL/dx and dL/dy (upstream gradient 1; L is a scalar, so a caller scales them by its own).  *loss is
+ * bit-identical to the forward call's; with dx = dy = NULL the call is the forward call.  Gradients are bit-reproducible
+ * (fixed summation orders, no atomics).  The spectral gradient follows torch autograd of the restated loss: sgn(0) = 0 in
+ * the L1 terms, clamp passes the gradient where v >= eps, d|z|/dz = 0 at z = 0, reflect padding folded back. */
+int fac_spectral_loss_grad(fac_handle* h, const float* x, const float* y, int B, int T, int sample_rate, int n_scales,
+                           const int* window_lengths, const int* n_mels, const float* mel_fmin, const float* mel_fmax, float clamp_eps,
+                           float mag_weight, float log_weight, float pow, float* loss, float* dx, float* dy, void* stream);
+int fac_l1_loss_grad(fac_handle* h, const float* x, const float* y, long long n, float* loss, float* dx, float* dy, void* stream);
 
 /* Predictor heads: modules/quantize.py:106-125 CNNLSTM(indim, outdim, head, global_pred) forward (3 ResidualUnits of
  * alias-free SnakeBeta + weight-normed Conv1d k7 (dilation 1, 2, 3, zero padding) / k1, a final alias-free SnakeBeta,

@@ -113,7 +113,10 @@ int fac_debug_attention(fac_handle* h, const float* q, const float* k, const flo
  * Per scale i of fac_reconstruction_loss ("recon.") and fac_spectral_loss ("spec."): recon.dft.<i> / spec.dft.<i> the
  * DFT GEMM output [2*B*F][ld] (rows [0, B*F) of x, then those of the second signal; Re at column 2k, Im at 2k + 1,
  * columns >= 2*nb zero), recon.terms.<i> / spec.terms.<i> the per-frame terms [B*F][2], and recon.fb.<i> / spec.fb.<i>
- * (mel scales only) the filterbank [nb][n_mels] as the terms kernel reads it. */
+ * (mel scales only) the filterbank [nb][n_mels] as the terms kernel reads it.  fac_spectral_loss_grad adds spec.dframes.<i>:
+ * the frames buffer [2*B*F][w] after the transposed DFT GEMM, whose rows of each signal with a requested gradient hold
+ * dL/dframes scaled by a per-row power of two (the other signal's rows still hold its frames), and spec.dscale.<i> [2*B*F]
+ * the inverse row scales: dL/dframes = row * dscale[row]. */
 int fac_debug_tap(fac_handle* h, const char* name, float* dst, size_t capacity_floats);
 
 /* Per-kernel-family device timing for bench.py's roofline object: when enabled, every launch of
