@@ -20,7 +20,7 @@
 // CTA = two warpgroups over a tile of 128 rows x N channels (each warpgroup 64 rows) or 64 rows x N channels (each
 // warpgroup N/2 channels).  A warpgroup spans at most 128 channels, except in the one-pass fp16 class: its tiles of the
 // decoder's C = 768 conv7 (N = 256) and C = 192 fused unit (N = 192) are 128 rows with each warpgroup over all N channels
-// (see tc_conv_plan).  Per 16-channel chunk:
+// (see tc_conv_plan).  Per step of `group` (1, 2 or 4) 16-channel chunks, 2-4 only on layers of 1-3 taps:
 //   weights: one thread streams the chunk's pre-arranged [tap][hi|lo][k-piece][N][16 B] blob with ONE 1-D bulk copy
 //            (cp.async.bulk, completion on an mbarrier) into a ring of 1-2 slots;
 //   activations: all 256 threads load the UNION of the rows all taps need (rows + (K-1)*dil) once with 16-byte loads
@@ -39,6 +39,7 @@
 
 #include <cstring>
 #include <mutex>
+#include <type_traits>
 
 #include "common.cuh"
 #include "conv_tc_common.cuh"
@@ -123,9 +124,17 @@ __device__ __forceinline__ float act_out(int act, float v, float al, float ia) {
 // TT: transposed formulation -- the weights are the wgmma A operand (64 output channels per warpgroup) and time is the
 // wgmma N dimension (NI = 64 time steps); the operand buffers and the weight blob are the same K-major layouts as the
 // plain formulation.
+// Grouping (p.group > 1, see tc_conv_plan) exists only in the instantiations that can plan it: not the one-pass fp16
+// class, fused units or the transposed formulation, which keep the one-chunk K loop and producer.  The others run the
+// grouped K loop at every G; they are register-bounded for two CTAs per SM at NI <= 128 (the grouped loop would take
+// some past 128), so a plan within half the shared memory keeps two CTAs per SM.
+template <int P1, int P2, bool TT>
+constexpr bool groupable() { return P1 != P_F16S && P2 == P_NONE && !TT; }
+
 template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false>
-__global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p) {
+__global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128 ? 2 : MINB) conv_tc_kernel(TcConvParams p) {
     constexpr bool FUSED = P2 != P_NONE;
+    constexpr bool GROUPABLE = groupable<P1, P2, TT>();
     static_assert(!TT || (NI == 64 && !FUSED), "transposed tiles: <= 64 channels x 64 time steps per warpgroup");
     static_assert(NI % 16 == 0 && NI <= (PROMO || MINB == 2 ? 64 : (P1 == P_F16S ? 256 : 128)),
                   "accumulator registers: <= 64 / 128 columns (256 in the one-pass fp16 class at one CTA per SM)");
@@ -146,15 +155,17 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
     tl.lane = tid & 31;
     const int t0 = blockIdx.x * BM, ntile = blockIdx.y, b = blockIdx.z;
     const int Kr = p.Kr, dil = p.dil, Rpad = p.Rpad, nchunk = p.nchunk, S = p.stagesB;
+    const int G = GROUPABLE ? p.group : 1;                   // chunks per GEMM-1 step: 1, 2 or 4
     const int R = BM + (Kr - 1) * dil;
-    const uint32_t a_plane = (uint32_t)T1::KG * Rpad * 16, a_bytes = a_plane * T1::planes;
+    const int nstep1 = G == 4 ? nchunk >> 2 : (G == 2 ? nchunk >> 1 : nchunk);     // GEMM-1 steps
+    const uint32_t a_plane = (uint32_t)G * T1::KG * Rpad * 16, a_bytes = a_plane * T1::planes;
     uint8_t* abuf = smem + kSmemHdr;
     float4* master = reinterpret_cast<float4*>(abuf + 2 * (size_t)a_bytes);
     uint8_t* wbuf = abuf + 2 * (size_t)a_bytes + master_bytes(PROMO, nchunk, p.promote_every, NI);
     uint8_t* a2buf = wbuf + (size_t)S * p.b_slot;
     const uint32_t w_unit1 = (uint32_t)Kr * T1::planes * T1::KG * N * 16;
     const uint32_t w_unit2 = FUSED ? (uint32_t)prec_planes(P2) * prec_kg(P2) * N * 16 : 0;
-    const int units = nchunk + (FUSED ? p.nchunk2 : 0);
+    const int units = nstep1 + (FUSED ? p.nchunk2 : 0);
 
     if (tid == 0) {
         for (int i = 0; i < S; ++i) mbar_init(&full[i], 1);
@@ -166,8 +177,10 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
         uint8_t* dst = wbuf + (size_t)(u % S) * p.b_slot;
         const uint8_t* src;
         uint32_t bytes;
-        if (u < nchunk) { src = reinterpret_cast<const uint8_t*>(p.wblob) + ((size_t)ntile * nchunk + u) * w_unit1; bytes = w_unit1; }
-        else { src = reinterpret_cast<const uint8_t*>(p.wblob2) + (size_t)(u - nchunk) * w_unit2; bytes = w_unit2; }
+        if (u < nstep1) {
+            src = reinterpret_cast<const uint8_t*>(p.wblob) + ((size_t)ntile * nchunk + (size_t)u * G) * w_unit1;
+            bytes = G * w_unit1;
+        } else { src = reinterpret_cast<const uint8_t*>(p.wblob2) + (size_t)(u - nstep1) * w_unit2; bytes = w_unit2; }
         mbar_arrive_expect_tx(bar, bytes);
         bulk_g2s(dst, src, bytes, bar);
     };
@@ -176,12 +189,22 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
 
     const PadMap pm = PadMap::make(p.Tin, p.pad_left_s, p.pad_right_s, p.reflect);
     const float* __restrict__ xb = p.x + (size_t)b * p.x_bstride;
-    auto produce = [&](int c) {
-        uint8_t* ahi = abuf + (size_t)(c & 1) * a_bytes;
-        if constexpr (P1 == P_TF32) produce_chunk<kThreads, false>(p, pm, xb, c, t0, R, Rpad, ahi, ahi + a_plane, tid);
-        else if constexpr (P1 == P_BF16) produce_chunk<kThreads, true>(p, pm, xb, c, t0, R, Rpad, ahi, ahi + a_plane, tid);
-        else if constexpr (P1 == P_F16S) produce_chunk<kThreads, true, 4, false, false, true>(p, pm, xb, c, t0, R, Rpad, ahi, ahi, tid);
-        else produce_chunk<kThreads, false, 4, false, true>(p, pm, xb, c, t0, R, Rpad, ahi, ahi + a_plane, tid);
+    auto produce = [&](int s) {              // the operand of GEMM-1 step s: chunks s*G .. s*G + G - 1
+        uint8_t* ahi = abuf + (size_t)(s & 1) * a_bytes;
+        auto run = [&](auto grouped) {
+            constexpr bool GR = decltype(grouped)::value;
+            const int c = GR ? s * G : s;
+            if constexpr (P1 == P_TF32) produce_chunk<kThreads, GR, false>(p, pm, xb, c, G, t0, R, Rpad, ahi, ahi + a_plane, tid);
+            else if constexpr (P1 == P_BF16) produce_chunk<kThreads, GR, true>(p, pm, xb, c, G, t0, R, Rpad, ahi, ahi + a_plane, tid);
+            else if constexpr (P1 == P_F16S) produce_chunk<kThreads, GR, true, 4, false, false, true>(p, pm, xb, c, G, t0, R, Rpad, ahi, ahi, tid);
+            else produce_chunk<kThreads, GR, false, 4, false, true>(p, pm, xb, c, G, t0, R, Rpad, ahi, ahi + a_plane, tid);
+        };
+        if constexpr (GROUPABLE) {
+            if (G > 1) run(std::true_type());
+            else run(std::false_type());
+        } else {
+            run(std::false_type());
+        }
         fence_proxy_async();    // make the generic-proxy stores visible to the tensor core
     };
     produce(0);
@@ -225,13 +248,11 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
         mbar_wait(&full[u % S], (uint32_t)(u / S) & 1u);
         const uint32_t wslot = wbase + (uint32_t)(u % S) * p.b_slot;
         wg_fence();
-        if (u < nchunk) {
+        if (u < nstep1) {
             const uint32_t a0 = abase + (uint32_t)(u & 1) * a_bytes + (uint32_t)tl.row0 * 16;
             const uint32_t b0 = wslot + (uint32_t)tl.col0 * 16;
-#pragma unroll 1
-            for (int tap = 0; tap < Kr; ++tap) {
-                const uint32_t ahi = a0 + (uint32_t)(tap * dil) * 16, alo = ahi + a_plane;
-                const uint32_t bhi = b0 + (uint32_t)tap * T1::planes * T1::KG * b_lbo, blo = bhi + T1::KG * b_lbo;
+            auto mma_tap = [&](uint32_t ahi, uint32_t bhi) {    // one tap of one chunk: every split pass
+                const uint32_t alo = ahi + a_plane, blo = bhi + T1::KG * b_lbo;
                 if constexpr (TT) {         // D[channel][time]: weights are the A operand, activations the B operand
                     mma_pass<P1, NI>(acc, bhi, b_lbo, ahi, a_lbo);
                     mma_pass<P1, NI>(crs, bhi, b_lbo, alo, a_lbo);
@@ -247,13 +268,29 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
                     mma_pass<P1, NI>(acc, ahi, a_lbo, blo, b_lbo);
                     mma_pass<P1, NI>(acc, alo, a_lbo, bhi, b_lbo);
                 }
+            };
+            // One MMA loop per instantiation: a second loop next to it makes ptxas fence every wgmma on its own.
+            if constexpr (GROUPABLE) {
+                // (chunk, tap) pairs in chunk-major order, so each output element sums its products as one-chunk steps do
+                uint32_t ac = a0, bc = b0, ahi = a0, bhi = b0;     // the chunk's and the tap's operand starts
+#pragma unroll 1
+                for (int i = 0, tap = 0; i < G * Kr; ++i) {
+                    mma_tap(ahi, bhi);
+                    if (++tap < Kr) { ahi += (uint32_t)dil * 16; bhi += T1::planes * T1::KG * b_lbo; }
+                    else { tap = 0; ac += T1::KG * a_lbo; bc += w_unit1; ahi = ac; bhi = bc; }
+                }
+            } else {
+#pragma unroll 1
+                for (int tap = 0; tap < Kr; ++tap)
+                    mma_tap(a0 + (uint32_t)(tap * dil) * 16, b0 + (uint32_t)tap * T1::planes * T1::KG * b_lbo);
             }
             wg_commit();
-            if (u + 1 < nchunk) produce(u + 1);         // overlaps the MMAs in flight
+            if (u + 1 < nstep1) produce(u + 1);         // overlaps the MMAs in flight
             wg_wait_all();
-            if (PROMO && ((u + 1) % p.promote_every == 0 || u + 1 == nchunk)) promote(u < p.promote_every, u + 1 == nchunk);
+            const int done = (u + 1) * G;               // chunks summed so far
+            if (PROMO && (done % p.promote_every == 0 || done == nchunk)) promote(done <= p.promote_every, done == nchunk);
             if constexpr (FUSED) {
-                if (u + 1 == nchunk) {
+                if (u + 1 == nstep1) {
                     // GEMM-2 operand snake2(D1 + b7), split, K-major [plane][k-piece][BM rows][16 B]
                     constexpr int KG2 = prec_kg(P2 < 0 ? 0 : P2);
                     const uint32_t a2_plane = (uint32_t)(p.nchunk2 * KG2) * BM2 * 16;
@@ -284,7 +321,7 @@ __global__ void __launch_bounds__(kThreads, MINB) conv_tc_kernel(TcConvParams p)
         } else if constexpr (FUSED) {
             constexpr int P2x = P2 < 0 ? 0 : P2;
             constexpr int KG2 = prec_kg(P2x);
-            const int c2 = u - nchunk;
+            const int c2 = u - nstep1;
             const uint32_t a2_plane = (uint32_t)(p.nchunk2 * KG2) * BM2 * 16, a2_lbo = (uint32_t)BM2 * 16;
             const uint32_t ahi = a2base + ((uint32_t)(c2 * KG2) * BM2 + tl.row0) * 16, alo = ahi + a2_plane;
             const uint32_t bhi = wslot + (uint32_t)tl.col0 * 16, blo = bhi + KG2 * b_lbo;
@@ -359,7 +396,7 @@ constexpr int f16s_wide_nw(bool fused) { return fused ? 192 : 256; }
 
 bool tc_conv_plan(TcConvParams& p) {
     // p.Cin, p.vf, p.Kr, p.dil, p.Cout, p.promoted (+ bf16 / g1f16 / f16x2 / fused / tt / occ2_maxn) must be set; fills N,
-    // MT, nchunk, Rpad, stagesB, b_slot, smem_bytes, promote_every, occ2
+    // MT, nchunk, Rpad, stagesB, b_slot, smem_bytes, promote_every, occ2, group
     if ((p.Cin % 4) != 0 || ((p.Cin * p.vf) % kChunk) != 0 || (p.Cout % 16) != 0) return false;
     if (p.bf16 && p.promoted) return false;
     if (p.f16x2 && !p.promoted) return false;
@@ -398,13 +435,18 @@ bool tc_conv_plan(TcConvParams& p) {
     // in one 128-row CTA; H100 80GB HBM3, 700 W, 1980 MHz max SM clock).  N itself is what the loop above found, so the
     // weight blob does not change.
     struct Layout { int Rpad; size_t slot, total; };
-    auto layout = [&](int S, int MT) {
+    auto layout = [&](int S, int MT, int G) {
         const int NW = MT == 2 ? N : N / 2, BM = 64 * MT;
         Layout l;
+        // Row pitch: one store phase of the producer (8 threads of 16-byte TF32 pieces, 16 threads of 8-byte 16-bit pieces)
+        // covers v rows x 8/v pitch-apart columns of 16 bytes, conflict-free when Rpad % 8 == v: v = 1 for TF32 at G > 1,
+        // 4/G in the 16-bit classes at G > 1.  G = 1 keeps Rpad % 8 == 2, right for TF32 (v = 2) and a 2-way conflict
+        // in the 16-bit classes (v = 4), as the one-chunk plans have always been laid out.
+        const int v = G == 1 ? 2 : (P1 == P_TF32 ? 1 : 4 / G);
         l.Rpad = BM + (p.Kr - 1) * p.dil;
-        while (l.Rpad % 8 != 2) ++l.Rpad;                   // conflict-free 16-byte producer stores
-        const size_t a_bytes = (size_t)prec_planes(P1) * prec_kg(P1) * l.Rpad * 16;
-        l.slot = (size_t)p.Kr * prec_planes(P1) * prec_kg(P1) * N * 16;
+        while (l.Rpad % 8 != v) ++l.Rpad;
+        const size_t a_bytes = (size_t)G * prec_planes(P1) * prec_kg(P1) * l.Rpad * 16;
+        l.slot = (size_t)G * p.Kr * prec_planes(P1) * prec_kg(P1) * N * 16;
         size_t a2 = 0;
         if (P2 != P_NONE) {
             const size_t slot2 = (size_t)prec_planes(P2) * prec_kg(P2) * N * 16;
@@ -417,6 +459,18 @@ bool tc_conv_plan(TcConvParams& p) {
         l.total = kSmemHdr + 2 * a_bytes + master + S * l.slot + a2 + (p.tt ? 64 * 16 : 0);
         return l;
     };
+    // Chunks per K-loop step G: every step pays a barrier, a weight wait, a global-load round trip for the next operand
+    // and a tensor-pipe drain, which a k = 7 conv's 7 taps of MMAs hide and a layer of 1-3 taps does not.  Such a layer
+    // streams G consecutive chunks per step (their weights are contiguous in the blob) into G-times larger operand and
+    // weight slots, as long as the plan keeps its residency: a plan within half the shared memory (two CTAs per SM, the
+    // register budget of every <= 128-column instantiation allows it) stays within it.  G divides the promotion window,
+    // so windows close at the same chunks; the transposed formulation keeps one chunk per step.
+    auto group = [&](int S, int MT, size_t cap) {
+        if (p.Kr > 3 || p.tt || p.fused || p.g1f16) return 1;     // the instantiations without the grouped loop
+        for (int G = 4; G > 1; G /= 2)
+            if (G <= p.max_group && p.nchunk % G == 0 && (!p.promoted || p.promote_every % G == 0) && layout(S, MT, G).total <= cap) return G;
+        return 1;
+    };
     const bool want2 = p.promoted ? !p.tt : (p.occ2_maxn > 0 && N <= p.occ2_maxn);
     for (int two = want2 ? 1 : 0; two >= 0; --two) {
         const size_t cap = two ? kSmemCap2 : kSmemCap;
@@ -426,10 +480,13 @@ bool tc_conv_plan(TcConvParams& p) {
                 const int NW = MT == 2 ? N : N / 2;
                 const bool wide = !two && P1 == P_F16S && NW == f16s_wide_nw(p.fused);
                 if ((NW > nwl && !wide) || NW % 16) continue;
-                if (wide && layout(2, 1).total <= kSmemCap2) continue;
-                const Layout l = layout(S, MT);
-                if (l.total > cap) continue;
+                if (wide && layout(2, 1, 1).total <= kSmemCap2) continue;
+                const Layout l1 = layout(S, MT, 1);
+                if (l1.total > cap) continue;
+                const int G = group(S, MT, l1.total <= kSmemCap2 ? kSmemCap2 : cap);
+                const Layout l = layout(S, MT, G);
                 p.N = N; p.MT = MT; p.Rpad = l.Rpad; p.R2pad = 64 * MT; p.stagesB = S; p.b_slot = (int)l.slot;
+                p.group = G;
                 p.smem_bytes = l.total;
                 p.occ2 = two;
                 return true;

@@ -254,14 +254,16 @@ __device__ __forceinline__ void store_f16_single(float4 x4, int pc, int row, int
     *reinterpret_cast<uint2*>(ahi + off) = hv;
 }
 
-// ---- activation producer shared by both kernels ------------------------------------------------
-// Thread `ptid` of NT producer threads owns 16-byte piece pc = ptid & 3 (4 input channels) of
-// rows ptid/4, ptid/4 + NT/4, ...: channel offset, Snake parameters and the smem column are
-// per-thread constants for the whole chunk; only the row varies.
-template <int NT, bool BF16, int BATCH = 4, bool INL = false, bool F16 = false, bool SINGLE = false>
+// ---- activation producer ----------------------------------------------------------------------
+// Chunks c .. c + G - 1 of the operand (GROUPED: G = 2 or 4; else the one chunk c): 4G 16-byte pieces (4 input channels
+// each) per row.  Thread `ptid` of NT producer threads owns piece pc = ptid % 4G of rows ptid/4G, ptid/4G + NT/4G, ...:
+// channel offset, Snake parameters and the smem column are per-thread constants for the whole call; only the row varies.
+// Piece pc lands in k-piece pc (TF32) or pc/2 (16-bit classes) of the buffer, so chunk c + s starts at k-piece s * KG.
+template <int NT, bool GROUPED, bool BF16, int BATCH = 4, bool INL = false, bool F16 = false, bool SINGLE = false>
 __device__ __forceinline__ void produce_chunk(const TcConvParams& p, const PadMap& pm, const float* __restrict__ xb,
-                                              int c, int t0, int R, int Rpad, uint8_t* ahi, uint8_t* alo, int ptid) {
-    const int pc = ptid & 3;
+                                              int c, int G, int t0, int R, int Rpad, uint8_t* ahi, uint8_t* alo, int ptid) {
+    const int lp = GROUPED ? (G == 4 ? 4 : 3) : 2;           // log2 of the pieces per row
+    const int pc = ptid & ((1 << lp) - 1);
     const int j = c * kChunk + pc * 4;
     const int soff = j / p.Cin, ci = j - soff * p.Cin;
     const bool has_alpha = p.in_alpha != nullptr;
@@ -270,12 +272,12 @@ __device__ __forceinline__ void produce_chunk(const TcConvParams& p, const PadMa
         al = __ldg(reinterpret_cast<const float4*>(p.in_alpha + ci));
         ia = __ldg(reinterpret_cast<const float4*>(p.in_inv_alpha + ci));
     }
-    constexpr int RSTEP = NT / 4;
+    const int RSTEP = NT >> lp;
     const int row_limit = p.Tout + (p.Kr - 1) * p.dil;
     const int vrow0 = t0 - p.PLr;
     const float* __restrict__ xcol = xb + ci;
 #pragma unroll 1
-    for (int r = ptid >> 2; r < R; r += RSTEP * BATCH) {
+    for (int r = ptid >> lp; r < R; r += RSTEP * BATCH) {
         float4 v[BATCH];
 #pragma unroll
         for (int u = 0; u < BATCH; ++u) {

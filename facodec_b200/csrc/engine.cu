@@ -2952,10 +2952,10 @@ int fac_set_option(fac_handle* h, const char* name, int value) {
     return FAC_ERR_INVALID;
 }
 
-int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin, int Cin,
-                      int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
-                      const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
-                      int Tout, int promoted, void* stream) {
+static int debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin, int Cin,
+                         int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
+                         const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
+                         int Tout, int promoted, void* stream, int* group_out) {
     if (!h || !x || !w_host || !y) return FAC_ERR_INVALID;
     cudaSetDevice(h->device);
     cudaStream_t st = (cudaStream_t)stream;
@@ -2971,6 +2971,11 @@ int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const 
     else if (K == 2 * stride && dil == 1) { tp.vf = stride; tp.Kr = 2; tp.dil = 1; }
     else { h->err = "fac_debug_conv_tc: unsupported stride/kernel"; return FAC_ERR_UNSUPPORTED; }
     if (promoted < 0 || promoted > 5 || !tc_conv_plan(tp)) { h->err = "fac_debug_conv_tc: layer not eligible for the tensor-core path"; return FAC_ERR_UNSUPPORTED; }
+    if (group_out) {                       // report the plan's chunks per step, run the one-chunk plan
+        *group_out = tp.group;
+        tp.max_group = 1;
+        if (!tc_conv_plan(tp)) { h->err = "fac_debug_conv_tc_group1: no one-chunk plan"; return FAC_ERR_UNSUPPORTED; }
+    }
     int ldw = (Cout + 3) / 4 * 4;
     std::vector<float> gen((size_t)K * Cin * ldw, 0.f);
     for (int co = 0; co < Cout; ++co)
@@ -3003,6 +3008,23 @@ int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const 
     cudaFree(d);
     if (e != cudaSuccess) { h->err = std::string("fac_debug_conv_tc: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
     return FAC_OK;
+}
+
+int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin, int Cin,
+                      int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
+                      const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
+                      int Tout, int promoted, void* stream) {
+    return debug_conv_tc(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
+                         in_alpha_host, out_alpha_host, act, res, y, Tout, promoted, stream, nullptr);
+}
+
+int fac_debug_conv_tc_group1(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin,
+                             int Cin, int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
+                             const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
+                             int Tout, int promoted, void* stream, int* group) {
+    if (!group) return FAC_ERR_INVALID;
+    return debug_conv_tc(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
+                         in_alpha_host, out_alpha_host, act, res, y, Tout, promoted, stream, group);
 }
 
 int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const float* b7_host, const float* w1_host,
@@ -3121,9 +3143,8 @@ int fac_debug_pad_map(int L, int pad_left, int pad_right, int reflect, int* out,
 }
 
 // Host-only: the tile plan the tensor-core conv kernel would use for a layer geometry (no GPU, no handle).
-int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* out8) {
-    if (!out8 || Cin <= 0 || Cout <= 0 || K <= 0 || dil <= 0 || stride <= 0 || mode < 0 || mode > 8) return FAC_ERR_INVALID;
-    TcConvParams tp;
+static int debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, TcConvParams& tp) {
+    if (Cin <= 0 || Cout <= 0 || K <= 0 || dil <= 0 || stride <= 0 || mode < 0 || mode > 8) return FAC_ERR_INVALID;
     tp.Cin = Cin; tp.Cout = Cout; tp.Tout = Tout; tp.occ2_maxn = occ2_maxn;
     tp.promoted = (mode == 1 || mode == 3) ? 1 : 0;
     tp.bf16 = (mode == 2 || mode == 4 || mode == 7 || mode == 8) ? 1 : 0;
@@ -3134,10 +3155,31 @@ int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, i
     if (stride == 1) { tp.vf = 1; tp.Kr = K; tp.dil = dil; }
     else if (K == 2 * stride && dil == 1) { tp.vf = stride; tp.Kr = 2; tp.dil = 1; }
     else return FAC_ERR_UNSUPPORTED;
-    if (!tc_conv_plan(tp)) return FAC_ERR_UNSUPPORTED;
+    return tc_conv_plan(tp) ? FAC_OK : FAC_ERR_UNSUPPORTED;
+}
+
+int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* out8) {
+    if (!out8) return FAC_ERR_INVALID;
+    TcConvParams tp;
+    const int rc = debug_tc_plan(Cin, Cout, K, dil, stride, Tout, mode, occ2_maxn, tp);
+    if (rc != FAC_OK) return rc;
     out8[0] = tp.N; out8[1] = tp.MT; out8[2] = tp.nchunk; out8[3] = tp.stagesB; out8[4] = tp.R2pad;
     out8[5] = (int)tp.smem_bytes; out8[6] = tp.Rpad; out8[7] = tp.promote_every;
     return FAC_OK;
+}
+
+int fac_debug_tc_plan_group(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* smem2) {
+    TcConvParams tp;
+    const int rc = debug_tc_plan(Cin, Cout, K, dil, stride, Tout, mode, occ2_maxn, tp);
+    if (rc != FAC_OK) return rc;
+    if (smem2) {
+        TcConvParams t1 = tp;
+        t1.max_group = 1;
+        if (!tc_conv_plan(t1)) return FAC_ERR_UNSUPPORTED;
+        smem2[0] = (int)tp.smem_bytes;
+        smem2[1] = (int)t1.smem_bytes;
+    }
+    return tp.group;
 }
 
 // Host-only: the tensor-core weight blob (tc_pack_blob) for nn.Conv1d weights [Cout][Cin][K]; returns the number of

@@ -50,12 +50,14 @@ struct TcConvParams {
     int fused = 0;                     // 1 = whole ResidualUnit: conv7 -> +b7 -> Snake -> 1x1 conv -> +b1 -> +x
     int tt = 0;                        // f16x2 only: transposed formulation (weights = wgmma A operand, time = wgmma N)
     int occ2_maxn = 0;                 // > 0: tiles with N <= occ2_maxn are planned for two resident CTAs per SM
+    int max_group = 4;                 // largest `group` the plan may take (1: the one-chunk reference of the tests)
     const float* wblob2 = nullptr;     // 1x1 conv weight blob (same tile N), when fused
     const float* bias2 = nullptr;
     int nchunk2 = 0;
     // plan (tc_conv_plan)
     int promote_every = 1;             // promoted: chunks per accumulation window
     int N = 0, nchunk = 0, Rpad = 0, stagesB = 0;
+    int group = 1;                     // 16-channel chunks per K-loop step (1, 2 or 4; divides nchunk and promote_every)
     int MT = 2;                        // 2: tile = 128 rows x N (warpgroups split rows); 1: 64 rows x N (they split channels)
     int b_slot = 0;                    // bytes of one weight-ring slot
     int occ2 = 0;                      // planned for two resident CTAs per SM

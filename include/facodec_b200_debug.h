@@ -34,6 +34,13 @@ int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const 
                       int Cin, int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
                       const float* in_alpha_host, const float* out_alpha_host, int act, const float* res,
                       float* y, int Tout, int promoted, void* stream);
+/* fac_debug_conv_tc with the layer's K loop stepped one 16-channel chunk at a time (the planner groups 2 or 4 chunks per
+ * step on layers of 1-3 taps): the reference a grouped launch must equal bit for bit.  *group receives the number of
+ * chunks per step the layer's own plan takes. */
+int fac_debug_conv_tc_group1(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin,
+                             int Cin, int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
+                             const float* in_alpha_host, const float* out_alpha_host, int act, const float* res,
+                             float* y, int Tout, int promoted, void* stream, int* group);
 /* One ResidualUnit (dac/model/dac.py:25-42) y = x + conv1(snake(conv7_d(snake(x)))) on DEVICE channels-last
  * x, y [B,T,C] with HOST folded weights w7 [C,C,7], w1 [C,C,1].  mode 0: fp32 FMA kernels, 1: two tensor-core
  * launches, 2: the single fused tensor-core launch (FAC_ERR_UNSUPPORTED if the geometry cannot be fused);
@@ -70,6 +77,9 @@ int fac_debug_pad_map(int L, int pad_left, int pad_right, int reflect, int* out,
  * K chunks, weight-ring stages, rows per tile, dynamic shared-memory bytes, padded rows of the operand buffer,
  * chunks per promotion}.  FAC_ERR_UNSUPPORTED when the layer is not eligible. */
 int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* out8);
+/* Host-only: 16-channel chunks per K-loop step (1, 2 or 4) of the same plan, or the negative status of fac_debug_tc_plan.
+ * smem2 (or NULL) receives the dynamic shared-memory bytes of that plan and of the layer's one-chunk-per-step plan. */
+int fac_debug_tc_plan_group(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* smem2);
 /* Host-only: packs nn.Conv1d weights [Cout][Cin][K] (HOST) into the tensor-core blob of mode 0..3 (see
  * fac_debug_tc_plan): [Cout/N][K chunks][taps][hi|lo][k-groups][N][16 bytes], hi|lo = TF32 pair (4 k-groups of 4 fp32
  * words), bf16 pair or fp16 hi / 2^11-scaled lo (2 k-groups of 8 halves).  Returns the blob size in 32-bit words (also
