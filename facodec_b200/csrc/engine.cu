@@ -5,6 +5,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
@@ -90,6 +91,10 @@ struct fac_handle {
     std::vector<Stream*> streams;
     struct VcStream;                // chunked voice conversion through the redecoder (fac_vc_stream_*)
     std::vector<VcStream*> vc_streams;
+    struct CodesPool;               // many B = 1 compression streams stepped in shared batches (fac_codes_pool_*)
+    std::vector<CodesPool*> codes_pools;
+    struct VcPool;                  // many B = 1 voice-conversion streams stepped in shared batches (fac_vc_pool_*)
+    std::vector<VcPool*> vc_pools;
     struct HeadSet;                 // modules/quantize.py:106-125 CNNLSTM instances (fac_head_*)
     std::vector<HeadSet*> heads;
     char* ws = nullptr; size_t ws_bytes = 0;
@@ -152,6 +157,7 @@ struct fac_handle::Stream {
     long long emitted = 0;                                  // frames of codes written so far
     float* z_held = nullptr;                                // [B][1024] latent frame `emitted`, quantized by the next call
     float* mel = nullptr; int mel_cap = 0;                  // [B][mel_cap][80] every mel80 row so far: the timbre pools them all
+    long long mel_base = 0;                                 // frame of mel row 0 (a pool's batch holds only the prosody window)
     void* all[13] = {nullptr};
 };
 
@@ -1385,6 +1391,8 @@ int fac_destroy(fac_handle* h) {
     for (auto* hs : h->heads) { if (hs->arena) cudaFree(hs->arena); delete hs; }
     for (auto* ss : h->streams) { for (void* p : ss->all) if (p) cudaFree(p); if (ss->mel) cudaFree(ss->mel); delete ss; }
     for (auto* vs : h->vc_streams) { for (void* p : vs->all) if (p) cudaFree(p); delete vs; }
+    for (int i = 0; i < (int)h->codes_pools.size(); ++i) fac_codes_pool_destroy(h, i);
+    for (int i = 0; i < (int)h->vc_pools.size(); ++i) fac_vc_pool_destroy(h, i);
     delete h;
     return FAC_OK;
 }
@@ -1648,10 +1656,13 @@ int fac_voice_convert(fac_handle* h, const int64_t* codes_p, const int64_t* code
 // Left context of the encoder's conv stack: 5581 samples (conv0 6 + stage 1 78 + down 3 + stage 2 156 + down 18 + stage 3 780
 // + down 90 + stage 4 3900 + down 550) -> 6000 (20 frames); of the decoder's stack after the LSTM: < 18 latent frames -> 20.
 constexpr int kEncCtx = 6000, kDecCtx = 20, kStreamMinFirst = 10;
+constexpr int kWnCtx = 32;   // mel frames of prosody-net history a codes window recomputes over (stream_codes)
 
-int fac_stream_begin(fac_handle* h, int B) {
-    if (!h || B < 1 || B > 32) { if (h) h->err = "fac_stream_begin: 1 <= B <= 32"; return FAC_ERR_INVALID; }
-    if (!h->finalized) { h->err = "module weights not loaded/finalized"; return FAC_ERR_STATE; }
+}  // extern "C"
+
+namespace {
+// Device state of a B-row stream (zeroed), or null with h->err set.
+fac_handle::Stream* alloc_stream(fac_handle* h, int B, const char* who) {
     cudaSetDevice(h->device);
     auto* s = new fac_handle::Stream();
     s->B = B;
@@ -1669,17 +1680,28 @@ int fac_stream_begin(fac_handle* h, int B) {
         cudaError_t e = cudaMalloc(&s->all[i], sizes[i]);
         if (e == cudaSuccess) e = cudaMemset(s->all[i], 0, sizes[i]);
         if (e != cudaSuccess) {
-            h->err = std::string("fac_stream_begin: ") + cudaGetErrorString(e);
+            h->err = std::string(who) + ": " + cudaGetErrorString(e);
             cudaGetLastError();
             for (void* p : s->all) if (p) cudaFree(p);
             delete s;
-            return FAC_ERR_CUDA;
+            return nullptr;
         }
     }
     s->x_hist = (float*)s->all[0]; s->ey_hist = (float*)s->all[1]; s->z_hist = (float*)s->all[2]; s->dy_hist = (float*)s->all[3];
     s->enc_h[0] = (uint32_t*)s->all[4]; s->enc_h[1] = (uint32_t*)s->all[5]; s->enc_c[0] = (float*)s->all[6]; s->enc_c[1] = (float*)s->all[7];
     s->dec_h[0] = (uint32_t*)s->all[8]; s->dec_h[1] = (uint32_t*)s->all[9]; s->dec_c[0] = (float*)s->all[10]; s->dec_c[1] = (float*)s->all[11];
     s->z_held = (float*)s->all[12];
+    return s;
+}
+}  // namespace
+
+extern "C" {
+
+int fac_stream_begin(fac_handle* h, int B) {
+    if (!h || B < 1 || B > 32) { if (h) h->err = "fac_stream_begin: 1 <= B <= 32"; return FAC_ERR_INVALID; }
+    if (!h->finalized) { h->err = "module weights not loaded/finalized"; return FAC_ERR_STATE; }
+    auto* s = alloc_stream(h, B, "fac_stream_begin");
+    if (!s) return FAC_ERR_CUDA;
     s->alive = true;
     h->streams.push_back(s);
     return (int)h->streams.size() - 1;
@@ -1795,10 +1817,9 @@ int stream_encode(fac_handle* h, fac_handle::Stream& s, const float* x, int T, v
 // zq [B][Fq][1024] (row pitch zpitch frames).  Runs with c.vq_critical set, as the offline quantizer.
 void stream_codes(Ctx& c, const fac_handle::Stream& s, long long E, int Fq, const float* zq, int zpitch, int64_t* codes_p,
                   int64_t* codes_c, int64_t* codes_r) {
-    constexpr int kWnCtx = 32;
     const int B = s.B, lo = (int)(E > kWnCtx ? E - kWnCtx : 0), Fw = (int)(E + Fq - lo);
     float* melw = c.alloc<float>((size_t)B * Fw * N_MELS);
-    copy_rows(c, melw, Fw, s.mel, s.mel_cap, lo, Fw, N_MELS, B, "stream.melw");
+    copy_rows(c, melw, Fw, s.mel, s.mel_cap, (int)(lo - s.mel_base), Fw, N_MELS, B, "stream.melw");
     const float* f0 = prosody_forward(c, melw, B, Fw);
     if (c.dry) return;
     FaqParams fp;
@@ -1862,34 +1883,36 @@ int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float
     });
 }
 
-int fac_stream_encode_codes(fac_handle* h, int stream_id, const float* x, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
-                            int64_t* codes_r, void* stream) {
+}  // extern "C"
+
+namespace {
+// The argument-independent rules of fac_stream_encode_codes on stream s (pointers and the stream id checked by the caller).
+int stream_encode_codes_check(fac_handle* h, const fac_handle::Stream& s, int T, int n_c, const char* who) {
     using S = fac_handle::Stream;
-    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
-    const char* who = "fac_stream_encode_codes";
-    if (!stream_alive(h, stream_id) || !x || !codes_p || !codes_c || !codes_r || n_c < 1 || n_c > 2) {
-        h->err = "fac_stream_encode_codes: bad arguments (1 <= n_c <= 2)";
-        return FAC_ERR_INVALID;
-    }
-    S& s = *h->streams[stream_id];
     int rc = stream_encode_check(h, s, T, S::kEncCodes, who);
     if (rc) return rc;
     if (s.enc_mode == S::kEncCodes && n_c != s.n_c) {
-        h->err = "fac_stream_encode_codes: n_c changed mid-stream (" + std::to_string(s.n_c) + " -> " + std::to_string(n_c) + ")";
+        h->err = std::string(who) + ": n_c changed mid-stream (" + std::to_string(s.n_c) + " -> " + std::to_string(n_c) + ")";
         return FAC_ERR_INVALID;
     }
-    if ((rc = stream_codes_supported(h, who))) return rc;
+    return stream_codes_supported(h, who);
+}
+
+// The launch sequence of fac_stream_encode_codes on a checked stream whose mel rows reach frame N - 1 (row r at s.mel +
+// (r - s.mel_base) * 80): advances the stream and returns the frames written, or a negative status.
+int stream_encode_codes(fac_handle* h, fac_handle::Stream& s, const float* x, int T, int n_c, int64_t* codes_p,
+                        int64_t* codes_c, int64_t* codes_r, void* stream) {
+    using S = fac_handle::Stream;
     // frames [E, N - 1) are final: frame N - 1 reads 300 samples past what has arrived (reflected only at the true end)
     const int B = s.B, Fc = T / HOP, first = s.enc_samples == 0;
     const long long N = (s.enc_samples + T) / HOP, E = s.emitted;
     const int Fout = (int)(N - 1 - E);
-    if ((rc = grow_mel(h, s, (int)N, (cudaStream_t)stream))) return rc;
     s.n_c = n_c;
-    rc = stream_encode(h, s, x, T, stream, S::kEncCodes, [&](Ctx& c, const EncChunk& ch) {
+    int rc = stream_encode(h, s, x, T, stream, S::kEncCodes, [&](Ctx& c, const EncChunk& ch) {
         c.vq_critical = true;
         const int f_first = (int)(E - (s.enc_samples - ch.hist) / HOP);   // frame E within the window
         const float* mel = mel_frames_tc(c, quantizer_mel(h), ch.xw, B, ch.Tw, f_first, Fout);
-        copy_rows(c, s.mel + (size_t)E * N_MELS, s.mel_cap, mel, Fout, 0, Fout, N_MELS, B, "stream.mel");
+        copy_rows(c, s.mel + (size_t)(E - s.mel_base) * N_MELS, s.mel_cap, mel, Fout, 0, Fout, N_MELS, B, "stream.mel");
         // latents of frames [E, N - 1): the held frame (after the first chunk) then all but the chunk's last frame
         const float* zq = ch.znew;
         if (!first) {
@@ -1905,23 +1928,23 @@ int fac_stream_encode_codes(fac_handle* h, int stream_id, const float* x, int T,
     return rc == FAC_OK ? Fout : rc;
 }
 
-int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre,
-                            void* stream) {
+int stream_finish_codes_check(fac_handle* h, const fac_handle::Stream& s, const char* who) {
     using S = fac_handle::Stream;
-    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
-    const char* who = "fac_stream_finish_codes";
-    if (!stream_alive(h, stream_id) || !codes_p || !codes_c || !codes_r) { h->err = "fac_stream_finish_codes: bad arguments"; return FAC_ERR_INVALID; }
-    S& s = *h->streams[stream_id];
     if (s.enc_mode != S::kEncCodes) {
-        h->err = s.enc_mode == S::kEncFinished ? "fac_stream_finish_codes: the stream's encoder is already finished"
-                                               : "fac_stream_finish_codes: nothing was encoded with fac_stream_encode_codes";
+        h->err = std::string(who) + (s.enc_mode == S::kEncFinished ? ": the stream's encoder is already finished"
+                                                                    : ": nothing was encoded with fac_stream_encode_codes");
         return FAC_ERR_STATE;
     }
-    int rc = stream_codes_supported(h, who);
-    if (rc) return rc;
+    return stream_codes_supported(h, who);
+}
+
+// The launch sequence of fac_stream_finish_codes on a checked stream whose mel rows start at frame 0.
+int stream_finish_codes(fac_handle* h, fac_handle::Stream& s, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r,
+                        float* timbre, void* stream) {
+    using S = fac_handle::Stream;
     const int B = s.B, hist = s.x_hist_len, N = (int)(s.enc_samples / HOP);
     const long long E = s.emitted;   // == N - 1
-    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
         c.vq_critical = true;
         // frame N - 1 from the last `hist` samples, reflected at the utterance's true end
         float* xw = c.alloc<float>((size_t)B * hist);
@@ -1941,6 +1964,34 @@ int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int6
     s.emitted = N;
     s.enc_mode = S::kEncFinished;
     return 1;
+}
+}  // namespace
+
+extern "C" {
+
+int fac_stream_encode_codes(fac_handle* h, int stream_id, const float* x, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
+                            int64_t* codes_r, void* stream) {
+    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    const char* who = "fac_stream_encode_codes";
+    if (!stream_alive(h, stream_id) || !x || !codes_p || !codes_c || !codes_r || n_c < 1 || n_c > 2) {
+        h->err = "fac_stream_encode_codes: bad arguments (1 <= n_c <= 2)";
+        return FAC_ERR_INVALID;
+    }
+    fac_handle::Stream& s = *h->streams[stream_id];
+    int rc = stream_encode_codes_check(h, s, T, n_c, who);
+    if (rc) return rc;
+    if ((rc = grow_mel(h, s, (int)((s.enc_samples + T) / HOP), (cudaStream_t)stream))) return rc;
+    return stream_encode_codes(h, s, x, T, n_c, codes_p, codes_c, codes_r, stream);
+}
+
+int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre,
+                            void* stream) {
+    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    if (!stream_alive(h, stream_id) || !codes_p || !codes_c || !codes_r) { h->err = "fac_stream_finish_codes: bad arguments"; return FAC_ERR_INVALID; }
+    fac_handle::Stream& s = *h->streams[stream_id];
+    int rc = stream_finish_codes_check(h, s, "fac_stream_finish_codes");
+    if (rc) return rc;
+    return stream_finish_codes(h, s, codes_p, codes_c, codes_r, timbre, stream);
 }
 
 }  // extern "C"
@@ -2051,6 +2102,13 @@ constexpr int kVcDecCtx = vc_decoder_reach();
 // 2 * kVcDecCtx.
 constexpr int kVcCodesHist = 2 * kVcRedCtx, kVcZHist = 2 * kVcDecCtx;
 
+// The frames a convert of F new code frames makes final: z up to Zf1, the output up to Yf1.
+void vc_targets(const fac_handle::VcStream& s, int F, long long* Zf1, long long* Yf1) {
+    const long long N1 = s.N + F;
+    *Zf1 = N1 - kVcRedCtx > s.Zf ? N1 - kVcRedCtx : s.Zf;
+    *Yf1 = *Zf1 - kVcDecCtx > s.Yf ? *Zf1 - kVcDecCtx : s.Yf;
+}
+
 fac_handle::VcStream* vc_stream(fac_handle* h, int id) {
     return id >= 0 && id < (int)h->vc_streams.size() && h->vc_streams[id]->alive ? h->vc_streams[id] : nullptr;
 }
@@ -2142,8 +2200,8 @@ int fac_vc_stream_convert(fac_handle* h, int stream_id, const int64_t* codes_p, 
     }
     if (s->finished) { h->err = "fac_vc_stream_convert: the stream was finished"; return FAC_ERR_STATE; }
     const long long N1 = s->N + F;
-    const long long Zf1 = N1 - kVcRedCtx > s->Zf ? N1 - kVcRedCtx : s->Zf;
-    const long long Yf1 = Zf1 - kVcDecCtx > s->Yf ? Zf1 - kVcDecCtx : s->Yf;
+    long long Zf1, Yf1;
+    vc_targets(*s, F, &Zf1, &Yf1);
     rc = vc_step(h, *s, codes_p, codes_c, n_c_rows, F, Zf1, Yf1, y, stream);
     if (rc != FAC_OK) return rc;
     const int k = (int)(Yf1 - s->Yf);
@@ -2179,6 +2237,552 @@ int fac_vc_stream_end(fac_handle* h, int stream_id) {
         s->alive = false;
     }
     return FAC_OK;
+}
+
+}  // extern "C"
+
+// ---- stream pools (fac_codes_pool_*, fac_vc_pool_*): many B = 1 streams stepped in shared batches ----
+// A session's state lives in slot arrays with the per-row content of a B = 1 stream, and is presented to the stream bodies
+// as a B = 1 Stream / VcStream whose pointers alias its slot (finishes run there directly).  A step groups its sessions by
+// every integer the launch sequence depends on, gathers each batch of <= 32 into the lanes of a B = 32 stream (pool.cu,
+// lstm2.cu), runs the stream body on it and scatters the state back.  Every lane of the batched kernels computes as a
+// B = 1 launch does (batch invariance), so a session's bits do not depend on who shares its launch.
+struct fac_handle::CodesPool {
+    int cap = 0, n_c = 0;
+    std::vector<Stream> slot;               // B = 1 views: x_hist / ey_hist / z_held alias the arrays below; mel is the slot's own
+    std::vector<char> used;
+    Stream* lanes = nullptr;                // the B = 32 batch
+    float *x_hist = nullptr, *ey_hist = nullptr, *z_held = nullptr;
+    uint32_t* carry = nullptr;              // [cap][2 layers][kCarryWords] encoder-LSTM (h, c) in lstm2_lane_map order
+    float* xin = nullptr; size_t xin_cap = 0;           // [32][T] gathered chunks
+    int64_t* cout = nullptr; size_t cout_cap = 0;       // [32][1 + n_c + 3][F] codes before the scatter
+};
+struct fac_handle::VcPool {
+    int cap = 0, use_p = 0, use_c = 0, n_c = 0;
+    std::vector<VcStream> slot;             // B = 1 views of the arrays below
+    std::vector<char> used;
+    VcStream* lanes = nullptr;
+    float* g = nullptr; int64_t* codes = nullptr; float* z = nullptr;
+    int64_t* cin = nullptr; size_t cin_cap = 0;         // [32][1 + n_c][F] gathered codes
+    float* yout = nullptr; size_t yout_cap = 0;         // [32][300 k] output before the scatter
+};
+
+namespace {
+constexpr int kCarryWords = 2 * (LATENT / 2) + LATENT;   // one encoder-LSTM layer of one lane: hi | lo h planes, c
+
+template <typename E>
+int dev_zeros(fac_handle* h, E*& p, size_t n, const char* who) {
+    cudaError_t e = cudaMalloc(&p, sizeof(E) * n);
+    if (e == cudaSuccess) e = cudaMemset(p, 0, sizeof(E) * n);
+    if (e != cudaSuccess) {
+        h->err = std::string(who) + ": " + cudaGetErrorString(e);
+        cudaGetLastError();
+        if (p) cudaFree(p);
+        p = nullptr;
+        return FAC_ERR_CUDA;
+    }
+    return FAC_OK;
+}
+
+// Grow-only scratch of a pool; the old buffer may still be read by queued work, so the stream is drained first.
+template <typename E>
+int grow_buf(fac_handle* h, E*& p, size_t& cap, size_t n, cudaStream_t st) {
+    if (n <= cap) return FAC_OK;
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess && p) { e = cudaFree(p); p = nullptr; cap = 0; }
+    if (e == cudaSuccess) e = cudaMalloc(&p, sizeof(E) * n);
+    if (e != cudaSuccess) {
+        h->err = std::string("pool scratch: ") + cudaGetErrorString(e);
+        cudaGetLastError();
+        p = nullptr; cap = 0;
+        return FAC_ERR_CUDA;
+    }
+    cap = n;
+    return FAC_OK;
+}
+
+// lane b of a batch of n: `words` 32-bit words from src(b) to dst(b)
+template <typename S, typename D>
+int lane_move(fac_handle* h, int n, long long words, S src, D dst, cudaStream_t st, const char* what) {
+    LaneCopyParams p;
+    p.n = n; p.words = words;
+    for (int b = 0; b < n; ++b) { p.src[b] = (const uint32_t*)src(b); p.dst[b] = (uint32_t*)dst(b); }
+    cudaError_t e = launch_lane_copy(p, st);
+    if (e != cudaSuccess) { h->err = std::string(what) + ": " + cudaGetErrorString(e); return FAC_ERR_CUDA; }
+    return FAC_OK;
+}
+
+// Batches of one pool step: sessions with equal keys form a group (groups in order of first appearance, members in input
+// order), each group cut into batches of at most kLaneMax.  group[i] / batch[i] (optional) receive input i's.
+std::vector<std::vector<int>> pool_plan(const std::vector<std::vector<long long>>& keys, int* group, int* batch) {
+    std::map<std::vector<long long>, int> index;
+    std::vector<std::vector<int>> groups, batches;
+    for (int i = 0; i < (int)keys.size(); ++i) {
+        auto it = index.find(keys[i]);
+        int g = it != index.end() ? it->second : (index[keys[i]] = (int)groups.size());
+        if (g == (int)groups.size()) groups.emplace_back();
+        groups[g].push_back(i);
+        if (group) group[i] = g;
+    }
+    for (const auto& g : groups)
+        for (size_t o = 0; o < g.size(); o += kLaneMax) {
+            batches.emplace_back(g.begin() + o, g.begin() + (o + kLaneMax < g.size() ? o + kLaneMax : g.size()));
+            if (batch) for (int i : batches.back()) batch[i] = (int)batches.size() - 1;
+        }
+    return batches;
+}
+
+// Every integer the launch sequence of stream_encode_codes depends on, for a stream at (enc_samples, x_hist_len,
+// ey_hist_len, emitted) fed T samples: T, hist, yh, first chunk, f_first, Fout, the prosody window's E - lo and Fw.
+std::vector<long long> codes_key(long long enc_samples, int hist, int yh, long long E, int T) {
+    const long long N = (enc_samples + T) / HOP, Fout = N - 1 - E, lo = E > kWnCtx ? E - kWnCtx : 0;
+    return {T, hist, yh, enc_samples == 0, E - (enc_samples - hist) / HOP, Fout, E - lo, E + Fout - lo};
+}
+
+// ... of vc_step for a stream at (N, Zf, Yf) fed F frames: F, Tw, hist, Tz, zhist and the copy offsets and lengths.
+std::vector<long long> vc_key(long long N, long long Zf, long long Yf, int F) {
+    auto floor0 = [](long long v) { return v > 0 ? v : 0; };
+    fac_handle::VcStream s;
+    s.N = N; s.Zf = Zf; s.Yf = Yf;
+    long long Zf1, Yf1;
+    vc_targets(s, F, &Zf1, &Yf1);
+    const long long N1 = N + F, hc0 = floor0(Zf - kVcRedCtx), zh0 = floor0(Yf - kVcDecCtx);
+    const long long hc1 = floor0(Zf1 - kVcRedCtx), zh1 = floor0(Yf1 - kVcDecCtx);
+    return {F, N1 - hc0, N - hc0, Zf1 - zh0, Zf - zh0, Zf1 - Zf, Yf1 - Yf, Yf - zh0, zh1 - zh0, Zf1 - zh1, hc1 - hc0, N1 - hc1};
+}
+
+fac_handle::CodesPool* codes_pool(fac_handle* h, int id) {
+    return h && id >= 0 && id < (int)h->codes_pools.size() ? h->codes_pools[id] : nullptr;
+}
+fac_handle::VcPool* vc_pool(fac_handle* h, int id) {
+    return h && id >= 0 && id < (int)h->vc_pools.size() ? h->vc_pools[id] : nullptr;
+}
+
+// The sessions of one step: each open and named once.
+template <typename P>
+int check_sessions(fac_handle* h, const P& pool, int n, const int* sessions, const char* who) {
+    std::vector<char> seen(pool.cap, 0);
+    for (int i = 0; i < n; ++i) {
+        const int sid = sessions[i];
+        if (sid < 0 || sid >= pool.cap || !pool.used[sid]) {
+            h->err = std::string(who) + ": session " + std::to_string(sid) + " is not open";
+            return FAC_ERR_INVALID;
+        }
+        if (seen[sid]++) {
+            h->err = std::string(who) + ": session " + std::to_string(sid) + " is named twice";
+            return FAC_ERR_INVALID;
+        }
+    }
+    return FAC_OK;
+}
+
+void free_codes_pool(fac_handle::CodesPool* P) {
+    if (P->lanes) { for (void* p : P->lanes->all) if (p) cudaFree(p); if (P->lanes->mel) cudaFree(P->lanes->mel); delete P->lanes; }
+    for (auto& s : P->slot) if (s.mel) cudaFree(s.mel);
+    for (void* p : {(void*)P->x_hist, (void*)P->ey_hist, (void*)P->z_held, (void*)P->carry, (void*)P->xin, (void*)P->cout})
+        if (p) cudaFree(p);
+    delete P;
+}
+
+void free_vc_pool(fac_handle::VcPool* P) {
+    if (P->lanes) { for (void* p : P->lanes->all) if (p) cudaFree(p); delete P->lanes; }
+    for (void* p : {(void*)P->g, (void*)P->codes, (void*)P->z, (void*)P->cin, (void*)P->yout}) if (p) cudaFree(p);
+    delete P;
+}
+
+// Moves the encoder-LSTM carries of a batch between the sessions' slots and the lanes' state tiles.
+int codes_pool_carry(fac_handle* h, fac_handle::CodesPool& P, const std::vector<int>& slots, int to_lanes, cudaStream_t st) {
+    for (int l = 0; l < 2; ++l) {
+        LaneCarryParams p;
+        p.n = (int)slots.size(); p.H = LATENT; p.U = lstm_units_per_cta(LATENT); p.pass3 = 1; p.to_lanes = to_lanes;
+        p.state_h = P.lanes->enc_h[l]; p.state_c = P.lanes->enc_c[l];
+        for (int b = 0; b < p.n; ++b) p.slot[b] = P.carry + ((size_t)slots[b] * 2 + l) * kCarryWords;
+        cudaError_t e = launch_lstm2_lane_carry(p, st);
+        if (e != cudaSuccess) { h->err = std::string("pool.carry: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
+    }
+    return FAC_OK;
+}
+
+// One batch of a codes-pool step: sessions slots[b] (equal codes_key) fed T samples each from x[b].
+int codes_pool_batch(fac_handle* h, fac_handle::CodesPool& P, const std::vector<int>& slots, int T, const float* const* x,
+                     int64_t* const* codes_p, int64_t* const* codes_c, int64_t* const* codes_r, cudaStream_t st) {
+    using S = fac_handle::Stream;
+    S& L = *P.lanes;
+    const int nb = (int)slots.size(), n_c = P.n_c;
+    auto sl = [&](int b) -> S& { return P.slot[slots[b]]; };
+    const S& f = sl(0);
+    const long long E = f.emitted, lo = E > kWnCtx ? E - kWnCtx : 0, N = (f.enc_samples + T) / HOP;
+    const int Fout = (int)(N - 1 - E), win = (int)(E - lo), hist = f.x_hist_len, yh = f.ey_hist_len;
+    const size_t pitch = (size_t)L.mel_cap * N_MELS;
+    int rc = FAC_OK;
+    auto mv = [&](long long words, auto src, auto dst, const char* what) {
+        if (rc == FAC_OK) rc = lane_move(h, nb, words, src, dst, st, what);
+    };
+    mv(T, [&](int b) { return x[b]; }, [&](int b) { return P.xin + (size_t)b * T; }, "pool.x");
+    mv(hist, [&](int b) { return sl(b).x_hist; }, [&](int b) { return L.x_hist + (size_t)b * kEncCtx; }, "pool.x_hist");
+    mv((long long)yh * LATENT, [&](int b) { return sl(b).ey_hist; }, [&](int b) { return L.ey_hist + (size_t)b * 2 * LATENT; },
+       "pool.ey_hist");
+    if (f.enc_samples > 0)
+        mv(LATENT, [&](int b) { return sl(b).z_held; }, [&](int b) { return L.z_held + (size_t)b * LATENT; }, "pool.z_held");
+    mv((long long)win * N_MELS, [&](int b) { return sl(b).mel + (size_t)(sl(b).emitted - win) * N_MELS; },
+       [&](int b) { return L.mel + b * pitch; }, "pool.mel");
+    if (rc == FAC_OK) rc = codes_pool_carry(h, P, slots, 1, st);
+    if (rc) return rc;
+    L.B = nb; L.x_hist_len = hist; L.ey_hist_len = yh; L.enc_samples = f.enc_samples; L.emitted = E; L.enc_mode = f.enc_mode;
+    L.mel_base = lo;
+    int64_t *cp = P.cout, *cc = cp + (size_t)nb * Fout, *cr = cc + (size_t)nb * n_c * Fout;
+    rc = stream_encode_codes(h, L, P.xin, T, n_c, cp, cc, cr, st);
+    if (rc < 0) return rc;
+    rc = FAC_OK;
+    mv(L.x_hist_len, [&](int b) { return L.x_hist + (size_t)b * kEncCtx; }, [&](int b) { return sl(b).x_hist; }, "pool.x_hist");
+    mv((long long)L.ey_hist_len * LATENT, [&](int b) { return L.ey_hist + (size_t)b * 2 * LATENT; },
+       [&](int b) { return sl(b).ey_hist; }, "pool.ey_hist");
+    mv(LATENT, [&](int b) { return L.z_held + (size_t)b * LATENT; }, [&](int b) { return sl(b).z_held; }, "pool.z_held");
+    mv((long long)Fout * N_MELS, [&](int b) { return L.mel + b * pitch + (size_t)win * N_MELS; },
+       [&](int b) { return sl(b).mel + (size_t)sl(b).emitted * N_MELS; }, "pool.mel");
+    if (rc == FAC_OK) rc = codes_pool_carry(h, P, slots, 0, st);
+    mv(2LL * Fout, [&](int b) { return cp + (size_t)b * Fout; }, [&](int b) { return codes_p[b]; }, "pool.codes_p");
+    mv(2LL * n_c * Fout, [&](int b) { return cc + (size_t)b * n_c * Fout; }, [&](int b) { return codes_c[b]; }, "pool.codes_c");
+    mv(6LL * Fout, [&](int b) { return cr + (size_t)b * 3 * Fout; }, [&](int b) { return codes_r[b]; }, "pool.codes_r");
+    if (rc) return rc;
+    for (int b = 0; b < nb; ++b) {
+        S& s = sl(b);
+        s.x_hist_len = L.x_hist_len; s.ey_hist_len = L.ey_hist_len; s.enc_mode = L.enc_mode; s.n_c = n_c;
+        s.enc_samples += T; s.emitted += Fout;
+    }
+    return FAC_OK;
+}
+
+// One batch of a vc-pool step: sessions slots[b] (equal vc_key) fed F frames each.
+int vc_pool_batch(fac_handle* h, fac_handle::VcPool& P, const std::vector<int>& slots, int F, const int64_t* const* codes_p,
+                  const int64_t* const* codes_c, float* const* y, cudaStream_t st) {
+    using V = fac_handle::VcStream;
+    V& L = *P.lanes;
+    const int nb = (int)slots.size(), n_c = P.n_c, rows = n_c > 0 ? n_c : 1;
+    auto sl = [&](int b) -> V& { return P.slot[slots[b]]; };
+    const V& f = sl(0);
+    long long Zf1, Yf1;
+    vc_targets(f, F, &Zf1, &Yf1);
+    auto floor0 = [](long long v) { return v > 0 ? v : 0; };
+    const int zhist = (int)(f.Zf - floor0(f.Yf - kVcDecCtx)), k = (int)(Yf1 - f.Yf), keep = (int)(Zf1 - floor0(Yf1 - kVcDecCtx));
+    const size_t gfl = redecoder_cond_floats(h, 1), cpl = 3 * kVcCodesHist, zpl = (size_t)kVcZHist * LATENT;
+    int64_t *cp = P.cin, *cc = cp + (size_t)nb * F;
+    int rc = FAC_OK;
+    auto mv = [&](long long words, auto src, auto dst, const char* what) {
+        if (rc == FAC_OK) rc = lane_move(h, nb, words, src, dst, st, what);
+    };
+    mv((long long)gfl, [&](int b) { return sl(b).g; }, [&](int b) { return L.g + b * gfl; }, "pool.g");
+    mv(2LL * cpl, [&](int b) { return sl(b).codes; }, [&](int b) { return L.codes + b * cpl; }, "pool.codes");
+    mv((long long)zhist * LATENT, [&](int b) { return sl(b).z; }, [&](int b) { return L.z + b * zpl; }, "pool.z");
+    mv(2LL * F, [&](int b) { return codes_p[b]; }, [&](int b) { return cp + (size_t)b * F; }, "pool.codes_p");
+    mv(2LL * n_c * F, [&](int b) { return codes_c[b]; }, [&](int b) { return cc + (size_t)b * rows * F; }, "pool.codes_c");
+    if (rc) return rc;
+    L.B = nb; L.N = f.N; L.Zf = f.Zf; L.Yf = f.Yf;
+    rc = vc_step(h, L, cp, cc, rows, F, Zf1, Yf1, P.yout, st);
+    if (rc) return rc;
+    mv(2LL * cpl, [&](int b) { return L.codes + b * cpl; }, [&](int b) { return sl(b).codes; }, "pool.codes");
+    if (Zf1 > f.Zf) mv((long long)keep * LATENT, [&](int b) { return L.z + b * zpl; }, [&](int b) { return sl(b).z; }, "pool.z");
+    mv((long long)k * HOP, [&](int b) { return P.yout + (size_t)b * k * HOP; }, [&](int b) { return y[b]; }, "pool.y");
+    if (rc) return rc;
+    for (int b = 0; b < nb; ++b) {
+        V& s = sl(b);
+        long long z1, y1;
+        vc_targets(s, F, &z1, &y1);
+        s.N += F; s.Zf = z1; s.Yf = y1;
+    }
+    return FAC_OK;
+}
+
+template <typename T>
+std::vector<T> pick(const T* a, const std::vector<int>& idx) {
+    std::vector<T> out;
+    for (int i : idx) out.push_back(a[i]);
+    return out;
+}
+}  // namespace
+
+extern "C" {
+
+int fac_codes_pool_create(fac_handle* h, int capacity, int n_c) {
+    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    const char* who = "fac_codes_pool_create";
+    if (capacity < 1 || n_c < 1 || n_c > 2) { h->err = "fac_codes_pool_create: bad arguments (capacity >= 1, 1 <= n_c <= 2)"; return FAC_ERR_INVALID; }
+    cudaSetDevice(h->device);
+    auto* P = new fac_handle::CodesPool();
+    P->cap = capacity; P->n_c = n_c;
+    P->lanes = alloc_stream(h, kLaneMax, who);
+    const size_t c = (size_t)capacity;
+    int rc = P->lanes ? FAC_OK : FAC_ERR_CUDA;
+    if (!rc) rc = dev_zeros(h, P->x_hist, c * kEncCtx, who);
+    if (!rc) rc = dev_zeros(h, P->ey_hist, c * 2 * LATENT, who);
+    if (!rc) rc = dev_zeros(h, P->z_held, c * LATENT, who);
+    if (!rc) rc = dev_zeros(h, P->carry, c * 2 * kCarryWords, who);
+    if (rc) { free_codes_pool(P); return rc; }
+    P->slot.resize(c);
+    P->used.assign(c, 0);
+    for (size_t i = 0; i < c; ++i) {
+        fac_handle::Stream& s = P->slot[i];
+        s.B = 1; s.alive = true;
+        s.x_hist = P->x_hist + i * kEncCtx; s.ey_hist = P->ey_hist + i * 2 * LATENT; s.z_held = P->z_held + i * LATENT;
+    }
+    h->codes_pools.push_back(P);
+    return (int)h->codes_pools.size() - 1;
+}
+
+int fac_codes_pool_open(fac_handle* h, int pool_id, void* stream) {
+    fac_handle::CodesPool* P = codes_pool(h, pool_id);
+    if (!P) { if (h) h->err = "fac_codes_pool_open: no such pool"; return FAC_ERR_INVALID; }
+    int i = 0;
+    while (i < P->cap && P->used[i]) ++i;
+    if (i == P->cap) { h->err = "fac_codes_pool_open: the pool is full (capacity " + std::to_string(P->cap) + ")"; return FAC_ERR_STATE; }
+    cudaSetDevice(h->device);
+    cudaError_t e = cudaMemsetAsync(P->carry + (size_t)i * 2 * kCarryWords, 0, sizeof(uint32_t) * 2 * kCarryWords, (cudaStream_t)stream);
+    if (e != cudaSuccess) { h->err = std::string("fac_codes_pool_open: ") + cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
+    fac_handle::Stream& s = P->slot[i];
+    s.enc_samples = 0; s.x_hist_len = 0; s.ey_hist_len = 0; s.emitted = 0; s.n_c = 0;
+    s.enc_mode = fac_handle::Stream::kEncNone;
+    P->used[i] = 1;
+    return i;
+}
+
+int fac_codes_pool_encode_codes(fac_handle* h, int pool_id, int n, const int* sessions, const int* T, const float* const* x,
+                                int64_t* const* codes_p, int64_t* const* codes_c, int64_t* const* codes_r, int* frames,
+                                void* stream) {
+    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    const char* who = "fac_codes_pool_encode_codes";
+    fac_handle::CodesPool* P = codes_pool(h, pool_id);
+    if (!P || n < 0 || (n > 0 && (!sessions || !T || !x || !codes_p || !codes_c || !codes_r || !frames))) {
+        h->err = "fac_codes_pool_encode_codes: bad arguments";
+        return FAC_ERR_INVALID;
+    }
+    int rc = check_sessions(h, *P, n, sessions, who);
+    if (rc) return rc;
+    std::vector<std::vector<long long>> keys(n);
+    long long maxT = 0, maxF = 0, maxWin = 0;
+    for (int i = 0; i < n; ++i) {
+        const fac_handle::Stream& s = P->slot[sessions[i]];
+        if (!x[i] || !codes_p[i] || !codes_c[i] || !codes_r[i]) {
+            h->err = "fac_codes_pool_encode_codes: null buffer of session " + std::to_string(sessions[i]);
+            return FAC_ERR_INVALID;
+        }
+        if ((rc = stream_encode_codes_check(h, s, T[i], P->n_c, who))) return rc;
+        keys[i] = codes_key(s.enc_samples, s.x_hist_len, s.ey_hist_len, s.emitted, T[i]);
+        maxT = std::max(maxT, (long long)T[i]); maxF = std::max(maxF, keys[i][5]); maxWin = std::max(maxWin, keys[i][7]);
+    }
+    if (n == 0) return FAC_OK;
+    // capacities: no session changes before every one of these has succeeded
+    cudaStream_t st = (cudaStream_t)stream;
+    for (int i = 0; i < n; ++i) {
+        fac_handle::Stream& s = P->slot[sessions[i]];
+        if ((rc = grow_mel(h, s, (int)((s.enc_samples + T[i]) / HOP), st))) return rc;
+    }
+    P->lanes->B = kLaneMax; P->lanes->emitted = 0;
+    if ((rc = grow_mel(h, *P->lanes, (int)maxWin, st))) return rc;
+    if ((rc = grow_buf(h, P->xin, P->xin_cap, (size_t)kLaneMax * maxT, st))) return rc;
+    if ((rc = grow_buf(h, P->cout, P->cout_cap, (size_t)kLaneMax * (4 + P->n_c) * maxF, st))) return rc;
+    for (const auto& b : pool_plan(keys, nullptr, nullptr)) {
+        rc = codes_pool_batch(h, *P, pick(sessions, b), T[b[0]], pick(x, b).data(), pick(codes_p, b).data(),
+                              pick(codes_c, b).data(), pick(codes_r, b).data(), st);
+        if (rc) return rc;
+    }
+    for (int i = 0; i < n; ++i) frames[i] = (int)keys[i][5];
+    return FAC_OK;
+}
+
+int fac_codes_pool_finish_codes(fac_handle* h, int pool_id, int n, const int* sessions, int64_t* const* codes_p,
+                                int64_t* const* codes_c, int64_t* const* codes_r, float* const* timbre, void* stream) {
+    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    const char* who = "fac_codes_pool_finish_codes";
+    fac_handle::CodesPool* P = codes_pool(h, pool_id);
+    if (!P || n < 0 || (n > 0 && (!sessions || !codes_p || !codes_c || !codes_r))) {
+        h->err = "fac_codes_pool_finish_codes: bad arguments";
+        return FAC_ERR_INVALID;
+    }
+    int rc = check_sessions(h, *P, n, sessions, who);
+    if (rc) return rc;
+    for (int i = 0; i < n; ++i) {
+        if (!codes_p[i] || !codes_c[i] || !codes_r[i]) {
+            h->err = "fac_codes_pool_finish_codes: null buffer of session " + std::to_string(sessions[i]);
+            return FAC_ERR_INVALID;
+        }
+        if ((rc = stream_finish_codes_check(h, P->slot[sessions[i]], who))) return rc;
+    }
+    for (int i = 0; i < n; ++i) {
+        rc = stream_finish_codes(h, P->slot[sessions[i]], codes_p[i], codes_c[i], codes_r[i], timbre ? timbre[i] : nullptr, stream);
+        if (rc < 0) return rc;
+    }
+    return FAC_OK;
+}
+
+int fac_codes_pool_close(fac_handle* h, int pool_id, int session) {
+    fac_handle::CodesPool* P = codes_pool(h, pool_id);
+    if (!P || session < 0 || session >= P->cap || !P->used[session]) {
+        if (h) h->err = "fac_codes_pool_close: session " + std::to_string(session) + " is not open";
+        return FAC_ERR_INVALID;
+    }
+    P->used[session] = 0;
+    return FAC_OK;
+}
+
+int fac_codes_pool_destroy(fac_handle* h, int pool_id) {
+    fac_handle::CodesPool* P = codes_pool(h, pool_id);
+    if (!P) return FAC_ERR_INVALID;
+    cudaSetDevice(h->device);
+    cudaDeviceSynchronize();
+    free_codes_pool(P);
+    h->codes_pools[pool_id] = nullptr;
+    return FAC_OK;
+}
+
+int fac_vc_pool_create(fac_handle* h, int capacity, int use_p_code, int use_c_code, int n_c) {
+    int rc = check_ready(h, FAC_REDECODER);
+    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    if (rc) return rc;
+    const char* who = "fac_vc_pool_create";
+    if (capacity < 1 || n_c < 0 || n_c > 2) { h->err = "fac_vc_pool_create: bad arguments (capacity >= 1, 0 <= n_c <= 2)"; return FAC_ERR_INVALID; }
+    cudaSetDevice(h->device);
+    auto* P = new fac_handle::VcPool();
+    P->cap = capacity; P->use_p = use_p_code ? 1 : 0; P->use_c = use_c_code ? 1 : 0; P->n_c = n_c;
+    const size_t c = (size_t)capacity, gfl = redecoder_cond_floats(h, 1), cpl = 3 * kVcCodesHist, zpl = (size_t)kVcZHist * LATENT;
+    P->lanes = new fac_handle::VcStream();
+    fac_handle::VcStream& L = *P->lanes;
+    L.B = kLaneMax; L.use_p = P->use_p; L.use_c = P->use_c; L.n_c = n_c; L.alive = true;
+    rc = dev_zeros(h, L.g, kLaneMax * gfl, who);
+    L.all[0] = L.g;
+    if (!rc) { rc = dev_zeros(h, L.codes, kLaneMax * cpl, who); L.all[1] = L.codes; }
+    if (!rc) { rc = dev_zeros(h, L.z, kLaneMax * zpl, who); L.all[2] = L.z; }
+    if (!rc) rc = dev_zeros(h, P->g, c * gfl, who);
+    if (!rc) rc = dev_zeros(h, P->codes, c * cpl, who);
+    if (!rc) rc = dev_zeros(h, P->z, c * zpl, who);
+    if (rc) { free_vc_pool(P); return rc; }
+    P->slot.resize(c);
+    P->used.assign(c, 0);
+    for (size_t i = 0; i < c; ++i) {
+        fac_handle::VcStream& s = P->slot[i];
+        s.B = 1; s.use_p = P->use_p; s.use_c = P->use_c; s.n_c = n_c; s.alive = true;
+        s.g = P->g + i * gfl; s.codes = P->codes + i * cpl; s.z = P->z + i * zpl;
+    }
+    h->vc_pools.push_back(P);
+    return (int)h->vc_pools.size() - 1;
+}
+
+int fac_vc_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream) {
+    int rc = check_ready(h, FAC_REDECODER);
+    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    if (rc) return rc;
+    fac_handle::VcPool* P = vc_pool(h, pool_id);
+    if (!P || !timbre) { h->err = "fac_vc_pool_open: bad arguments"; return FAC_ERR_INVALID; }
+    int i = 0;
+    while (i < P->cap && P->used[i]) ++i;
+    if (i == P->cap) { h->err = "fac_vc_pool_open: the pool is full (capacity " + std::to_string(P->cap) + ")"; return FAC_ERR_STATE; }
+    fac_handle::VcStream& s = P->slot[i];
+    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { redecoder_cond(c, timbre, 1, s.g); });
+    if (rc) return rc;
+    s.N = s.Zf = s.Yf = 0;
+    s.finished = false;
+    P->used[i] = 1;
+    return i;
+}
+
+int fac_vc_pool_convert(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
+                        const int64_t* const* codes_c, const int* n_c_rows, float* const* y, int* frames, void* stream) {
+    int rc = check_ready(h, FAC_REDECODER);
+    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    if (rc) return rc;
+    const char* who = "fac_vc_pool_convert";
+    fac_handle::VcPool* P = vc_pool(h, pool_id);
+    if (!P || n < 0 || (n > 0 && (!sessions || !F || !codes_p || !codes_c || !n_c_rows || !y || !frames))) {
+        h->err = "fac_vc_pool_convert: bad arguments";
+        return FAC_ERR_INVALID;
+    }
+    if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
+    std::vector<std::vector<long long>> keys(n);
+    long long maxF = 0, maxK = 0;
+    for (int i = 0; i < n; ++i) {
+        const fac_handle::VcStream& s = P->slot[sessions[i]];
+        if (!codes_p[i] || !codes_c[i] || !y[i] || F[i] <= 0 || n_c_rows[i] < P->n_c || n_c_rows[i] > 2) {
+            h->err = "fac_vc_pool_convert: bad arguments of session " + std::to_string(sessions[i]) +
+                     " (F >= 1, n_c <= rows of codes_c <= 2)";
+            return FAC_ERR_INVALID;
+        }
+        if (s.finished) { h->err = "fac_vc_pool_convert: session " + std::to_string(sessions[i]) + " was finished"; return FAC_ERR_STATE; }
+        keys[i] = vc_key(s.N, s.Zf, s.Yf, F[i]);
+        maxF = std::max(maxF, (long long)F[i]); maxK = std::max(maxK, keys[i][6]);
+    }
+    if (n == 0) return FAC_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = grow_buf(h, P->cin, P->cin_cap, (size_t)kLaneMax * 3 * maxF, st))) return rc;
+    if ((rc = grow_buf(h, P->yout, P->yout_cap, (size_t)kLaneMax * HOP * (maxK > 0 ? maxK : 1), st))) return rc;
+    for (const auto& b : pool_plan(keys, nullptr, nullptr)) {
+        rc = vc_pool_batch(h, *P, pick(sessions, b), F[b[0]], pick(codes_p, b).data(), pick(codes_c, b).data(), pick(y, b).data(), st);
+        if (rc) return rc;
+    }
+    for (int i = 0; i < n; ++i) frames[i] = (int)keys[i][6];
+    return FAC_OK;
+}
+
+int fac_vc_pool_finish(fac_handle* h, int pool_id, int n, const int* sessions, float* const* y, int* frames, void* stream) {
+    int rc = check_ready(h, FAC_REDECODER);
+    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    if (rc) return rc;
+    const char* who = "fac_vc_pool_finish";
+    fac_handle::VcPool* P = vc_pool(h, pool_id);
+    if (!P || n < 0 || (n > 0 && (!sessions || !y || !frames))) { h->err = "fac_vc_pool_finish: bad arguments"; return FAC_ERR_INVALID; }
+    if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
+    for (int i = 0; i < n; ++i) {
+        const fac_handle::VcStream& s = P->slot[sessions[i]];
+        if (!y[i]) { h->err = "fac_vc_pool_finish: null output of session " + std::to_string(sessions[i]); return FAC_ERR_INVALID; }
+        if (s.finished || s.N == 0) {
+            h->err = "fac_vc_pool_finish: session " + std::to_string(sessions[i]) + (s.finished ? " was finished" : " received no codes");
+            return FAC_ERR_STATE;
+        }
+    }
+    for (int i = 0; i < n; ++i) {
+        fac_handle::VcStream& s = P->slot[sessions[i]];
+        if ((rc = vc_step(h, s, nullptr, nullptr, 0, 0, s.N, s.N, y[i], stream))) return rc;
+        frames[i] = (int)(s.N - s.Yf);
+        s.Zf = s.Yf = s.N;
+        s.finished = true;
+    }
+    return FAC_OK;
+}
+
+int fac_vc_pool_close(fac_handle* h, int pool_id, int session) {
+    fac_handle::VcPool* P = vc_pool(h, pool_id);
+    if (!P || session < 0 || session >= P->cap || !P->used[session]) {
+        if (h) h->err = "fac_vc_pool_close: session " + std::to_string(session) + " is not open";
+        return FAC_ERR_INVALID;
+    }
+    P->used[session] = 0;
+    return FAC_OK;
+}
+
+int fac_vc_pool_destroy(fac_handle* h, int pool_id) {
+    fac_handle::VcPool* P = vc_pool(h, pool_id);
+    if (!P) return FAC_ERR_INVALID;
+    cudaSetDevice(h->device);
+    cudaDeviceSynchronize();
+    free_vc_pool(P);
+    h->vc_pools[pool_id] = nullptr;
+    return FAC_OK;
+}
+
+int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch) {
+    if (n < 0 || (n > 0 && (!counters || !lengths || !group || !batch)) || (kind != 0 && kind != 1)) return FAC_ERR_INVALID;
+    std::vector<std::vector<long long>> keys(n);
+    for (int i = 0; i < n; ++i) {
+        const long long* c = counters + (size_t)i * (kind == 0 ? 4 : 3);
+        keys[i] = kind == 0 ? codes_key(c[0], (int)c[1], (int)c[2], c[3], lengths[i]) : vc_key(c[0], c[1], c[2], lengths[i]);
+    }
+    return (int)pool_plan(keys, group, batch).size();
+}
+
+long long fac_debug_lstm_lane_map(int H, int pass3, int lane, long long* pos, long long capacity) {
+    const int U = lstm_units_per_cta(H);
+    if (U == 0 || lane < 0 || lane >= kLaneMax) return FAC_ERR_INVALID;
+    const long long words = (long long)(pass3 ? 2 : 1) * (H / 2) + H;
+    if (pos && capacity >= words) lstm2_lane_map(H, U, pass3 ? 1 : 0, lane, pos);
+    return words;
 }
 
 // meldataset.py:37-47 preprocess: torchaudio MelSpectrogram(n_mels=80, n_fft=2048, win_length=1200, hop_length=300) with

@@ -98,6 +98,27 @@ size_t lstm2_smem_bytes(int H, int U, int pass3);
 // sizes of one layer's carried stream state: state_h words and state_c floats
 void lstm2_state_sizes(int H, int U, int pass3, size_t* h_words, size_t* c_floats);
 cudaError_t lstm2_read_phase_clocks(long long* out4);
+// One batch lane's carry of one layer is PL * H/2 h words + H c floats (PL = 2 when pass3).  lstm2_lane_map writes, for word
+// j of lane b's carry, its position in [state_h words | state_c floats] (state_h first, then state_c at offset h_words).
+void lstm2_lane_map(int H, int U, int pass3, int b, long long* pos);
+// Moves the carries of lanes [0, n) between state (state_h, state_c) and n packed per-session slots of lstm2_lane_map order
+// (to_lanes = 1: slot[b] -> lane b; 0: lane b -> slot[b]), raw 32-bit words.
+constexpr int kLaneMax = 32;
+struct LaneCarryParams {
+    uint32_t* slot[kLaneMax];
+    uint32_t* state_h = nullptr;
+    float* state_c = nullptr;
+    int n = 0, H = 0, U = 0, pass3 = 0, to_lanes = 0;
+};
+cudaError_t launch_lstm2_lane_carry(const LaneCarryParams& p, cudaStream_t st);
+// dst[b][0, words) = src[b][0, words) for lanes b < n (32-bit words; pool.cu): the slot <-> lane moves of the stream pools
+struct LaneCopyParams {
+    const uint32_t* src[kLaneMax];
+    uint32_t* dst[kLaneMax];
+    int n = 0;
+    long long words = 0;
+};
+cudaError_t launch_lane_copy(const LaneCopyParams& p, cudaStream_t st);
 int lstm_units_per_cta(int H);
 cudaError_t lstm_read_phase_clocks(long long* out4);   // CTA-0 accumulated phase clocks of the last launch  // U such that H % U == 0 and H / U <= resident CTAs
 

@@ -298,6 +298,45 @@ void lstm2_state_sizes(int H, int U, int pass3, size_t* h_words, size_t* c_float
     *c_floats = (size_t)(H / U) * L2_BT * U;
 }
 
+// Position of word j of lane b's carry: h word (plane pl, k pair kp) at pl * H/2 * 32 + kp * 32 + (b ^ lstm2_swz_h(kp)), then
+// the cell state of unit k (CTA k / U) at h_words + (k / U) * 32 * U + b * U + k % U.
+__host__ __device__ __forceinline__ long long lstm2_lane_word(int H, int U, int pl_count, int b, int j) {
+    const int hw = pl_count * (H / 2);
+    if (j < hw) {
+        const int pl = j / (H / 2), kp = j % (H / 2);
+        return (long long)pl * (H / 2) * L2_BT + (long long)kp * L2_BT + (b ^ lstm2_swz_h(kp));
+    }
+    const int k = j - hw;
+    return (long long)hw * L2_BT + (long long)(k / U) * L2_BT * U + (long long)b * U + k % U;
+}
+
+void lstm2_lane_map(int H, int U, int pass3, int b, long long* pos) {
+    const int PL = pass3 ? 2 : 1;
+    for (int j = 0; j < PL * (H / 2) + H; ++j) pos[j] = lstm2_lane_word(H, U, PL, b, j);
+}
+
+__global__ void lstm2_lane_carry_kernel(LaneCarryParams p) {
+    const int b = blockIdx.y;
+    if (b >= p.n) return;
+    const int PL = p.pass3 ? 2 : 1, words = PL * (p.H / 2) + p.H;
+    const long long hw = (long long)PL * (p.H / 2) * L2_BT;
+    uint32_t* slot = p.slot[b];
+    uint32_t* cw = reinterpret_cast<uint32_t*>(p.state_c);
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < words; j += gridDim.x * blockDim.x) {
+        const long long pos = lstm2_lane_word(p.H, p.U, PL, b, j);
+        uint32_t* w = pos < hw ? p.state_h + pos : cw + (pos - hw);
+        if (p.to_lanes) *w = slot[j];
+        else slot[j] = *w;
+    }
+}
+
+cudaError_t launch_lstm2_lane_carry(const LaneCarryParams& p, cudaStream_t st) {
+    if (p.n <= 0) return cudaSuccess;
+    if (p.n > L2_BT || p.U <= 0 || p.H % p.U != 0) return cudaErrorInvalidValue;
+    lstm2_lane_carry_kernel<<<dim3(8, p.n), 256, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
 template <int U, bool PASS3>
 static cudaError_t launch2_u(const LstmParams& p, cudaStream_t st) {
     const size_t smem = lstm2_smem_bytes(p.H, U, PASS3 ? 1 : 0);

@@ -1,0 +1,26 @@
+// Slot <-> lane moves of the stream pools (fac_codes_pool_*, fac_vc_pool_*): each lane of a batch reads or writes its own
+// session's buffer through a pointer table passed as a kernel parameter, so a step needs no host-to-device copy.
+#include "common.cuh"
+#include "kernels.h"
+
+namespace fac {
+
+__global__ void lane_copy_kernel(LaneCopyParams p) {
+    const int b = blockIdx.y;
+    if (b >= p.n) return;
+    const uint32_t* src = p.src[b];
+    uint32_t* dst = p.dst[b];
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.words; i += (long long)gridDim.x * blockDim.x)
+        dst[i] = src[i];
+}
+
+cudaError_t launch_lane_copy(const LaneCopyParams& p, cudaStream_t st) {
+    if (p.n <= 0 || p.words <= 0) return cudaSuccess;
+    if (p.n > kLaneMax) return cudaErrorInvalidValue;
+    long long blocks = (p.words + 255) / 256;
+    if (blocks > 64) blocks = 64;
+    lane_copy_kernel<<<dim3((unsigned)blocks, p.n), 256, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
+}  // namespace fac

@@ -666,6 +666,202 @@ class VoiceConversionStream:
         self.close()
 
 
+def _ptr_array(ctype, items):
+    return (ctype * max(len(items), 1))(*items)
+
+
+class _StreamPool:
+    """Shared plumbing of the stream pools: session bookkeeping, pointer tables and the pool's lifetime."""
+
+    _kind = None
+
+    def _setup(self, engine, pid):
+        self.engine, self.pid = engine, pid
+        self.device = torch.device("cuda", engine.device_index)
+        self._open = set()
+
+    def _sessions(self, sessions):
+        if self.pid is None:
+            raise _lib.FacError("pool is closed")
+        sessions = [int(s) for s in sessions]
+        for s in sessions:
+            if s not in self._open:
+                raise _lib.FacError("session %d is not open in this pool" % s)
+        if len(set(sessions)) != len(sessions):
+            raise ValueError("a step names each session at most once")
+        return sessions
+
+    def _check_device(self, t):
+        if t.device.type != "cuda" or (t.device.index if t.device.index is not None else torch.cuda.current_device()) != self.engine.device_index:
+            raise _lib.FacError("pool inputs must be on cuda:%d (no CPU fallback); got %s" % (self.engine.device_index, t.device))
+
+    def close(self, session=None):
+        """close(s) frees session s's slot; close() frees the pool."""
+        e = self.engine
+        if session is not None:
+            s = self._sessions([session])[0]
+            _lib.check(e.handle, getattr(e.L, "fac_%s_pool_close" % self._kind)(e.handle, self.pid, s), "pool close")
+            self._open.discard(s)
+            return
+        if self.pid is not None and e.handle is not None:
+            getattr(e.L, "fac_%s_pool_destroy" % self._kind)(e.handle, self.pid)
+        self.pid = None
+        self._open = set()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+class CodecStreamPool(_StreamPool):
+    """Many live compression sessions (CodecStream.encode_codes with B = 1 each) stepped in shared launches: each session
+    joins, feeds chunks of its own length and leaves on its own schedule, and its codes and timbre equal those of its own
+    B = 1 CodecStream fed the same chunks, bit for bit (fac_codes_pool_*).  n_c is fixed for the pool."""
+
+    _kind = "codes"
+
+    def __init__(self, model, capacity=256, n_c=2, device=None):
+        engine = model.encoder._engine
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        engine.sync_weights(dev)
+        pid = engine.L.fac_codes_pool_create(engine.handle, int(capacity), int(n_c))
+        _lib.check(engine.handle, pid, "fac_codes_pool_create")
+        self._setup(engine, pid)
+        self.capacity, self.n_c = int(capacity), int(n_c)
+
+    def open(self):
+        """A new session id (a slot, reused after close()); raises FacError when the pool is full."""
+        if self.pid is None:
+            raise _lib.FacError("pool is closed")
+        e = self.engine
+        s = _lib.check(e.handle, e.L.fac_codes_pool_open(e.handle, self.pid, _stream(self.device)), "fac_codes_pool_open")
+        self._open.add(s)
+        return s
+
+    def encode_codes(self, chunks):
+        """{session: x [1,1,T]} (T per session, with the chunk rules of CodecStream.encode_codes) -> {session: [codes_p
+        [1,1,F], codes_c [1,n_c,F], codes_r [1,3,F]]}, F = T/300 - 1 on a session's first chunk and T/300 after.  One
+        rejected entry rejects the whole step and leaves every session as it was."""
+        sessions = self._sessions(chunks.keys())
+        xs, Ts, outs = [], [], []
+        for s in sessions:
+            x = chunks[s]
+            self._check_device(x)
+            if x.dim() != 3 or x.shape[0] != 1 or x.shape[1] != 1:
+                raise ValueError("session %d: x must be [1, 1, T], got %s" % (s, tuple(x.shape)))
+            x = _f32c(x)
+            T = x.shape[2]
+            F = max(T // 300, 1)      # the frames are known after the call: T/300 - 1 on a session's first chunk
+            outs.append([torch.empty(r * F, device=self.device, dtype=torch.int64) for r in (1, self.n_c, 3)])
+            xs.append(x)
+            Ts.append(T)
+        n = len(sessions)
+        frames = (ctypes.c_int * max(n, 1))()
+        P = lambda ts: _ptr_array(ctypes.c_void_p, [t.data_ptr() for t in ts])
+        e = self.engine
+        rc = e.L.fac_codes_pool_encode_codes(e.handle, self.pid, n, _ptr_array(ctypes.c_int, sessions), _ptr_array(ctypes.c_int, Ts),
+                                             P(xs), P([o[0] for o in outs]), P([o[1] for o in outs]), P([o[2] for o in outs]),
+                                             frames, _stream(self.device))
+        _lib.check(e.handle, rc, "fac_codes_pool_encode_codes")
+        return {s: [t[:r * frames[i]].view(1, r, frames[i]) for t, r in zip(outs[i], (1, self.n_c, 3))]
+                for i, s in enumerate(sessions)}
+
+    def finish_codes(self, sessions):
+        """End of the sessions' utterances -> {session: ([codes_p, codes_c, codes_r] of the held-back frame, timbre [1,1024])},
+        as CodecStream.finish_codes."""
+        sessions = self._sessions(sessions)
+        outs = [[torch.empty(1, r, 1, device=self.device, dtype=torch.int64) for r in (1, self.n_c, 3)] for _ in sessions]
+        timbres = [torch.empty(1, 1024, device=self.device) for _ in sessions]
+        P = lambda ts: _ptr_array(ctypes.c_void_p, [t.data_ptr() for t in ts])
+        e = self.engine
+        rc = e.L.fac_codes_pool_finish_codes(e.handle, self.pid, len(sessions), _ptr_array(ctypes.c_int, sessions),
+                                             P([o[0] for o in outs]), P([o[1] for o in outs]), P([o[2] for o in outs]), P(timbres),
+                                             _stream(self.device))
+        _lib.check(e.handle, rc, "fac_codes_pool_finish_codes")
+        return {s: (outs[i], timbres[i]) for i, s in enumerate(sessions)}
+
+
+class VoiceConversionPool(_StreamPool):
+    """Many live voice-conversion sessions (VoiceConversionStream with B = 1 each, every one with its own target timbre)
+    stepped in shared launches; each session's waveform equals that of its own B = 1 VoiceConversionStream fed the same
+    chunks, bit for bit (fac_vc_pool_*).  use_p_code / use_c_code / n_c are fixed for the pool."""
+
+    _kind = "vc"
+
+    def __init__(self, redecoder_model, capacity=256, use_p_code=False, use_c_code=True, n_c=1):
+        engine = redecoder_model.encoder._engine
+        engine.sync_weights(torch.device("cuda", torch.cuda.current_device()))
+        pid = engine.L.fac_vc_pool_create(engine.handle, int(capacity), int(bool(use_p_code)), int(bool(use_c_code)), int(n_c))
+        _lib.check(engine.handle, pid, "fac_vc_pool_create")
+        self._setup(engine, pid)
+        self.capacity = int(capacity)
+        self.lookahead_frames = engine.L.fac_vc_stream_lookahead()
+
+    def open(self, timbre):
+        """A new session converting to ``timbre`` [1,1024]; raises FacError when the pool is full."""
+        if self.pid is None:
+            raise _lib.FacError("pool is closed")
+        self._check_device(timbre)
+        tv = _f32c(timbre)
+        if tuple(tv.shape) != (1, 1024):
+            raise ValueError("timbre must be [1, 1024], got %s" % (tuple(tv.shape),))
+        e = self.engine
+        s = _lib.check(e.handle, e.L.fac_vc_pool_open(e.handle, self.pid, _ptr(tv), _stream(self.device)), "fac_vc_pool_open")
+        self._open.add(s)
+        return s
+
+    def convert(self, chunks):
+        """{session: codes} (codes[0] [1,1,F], codes[1] [1,1|2,F], as VoiceConversionStream.convert takes them) -> {session:
+        y [1,1,300 k]}.  Codes outside [0, 1024) raise IndexError (one device reduction + one host sync for the step); one
+        rejected entry rejects the whole step and leaves every session as it was."""
+        sessions = self._sessions(chunks.keys())
+        cps, ccs, ys, Fs = [], [], [], []
+        for s in sessions:
+            codes = chunks[s]
+            if len(codes) < 2 or codes[0].dim() != 3 or codes[0].shape[0] != 1:
+                raise ValueError("session %d: codes must be [codes_p [1, 1, F], codes_c [1, 1|2, F], ...]" % s)
+            cp, cc, F = self._codes(codes)
+            cps.append(cp); ccs.append(cc); Fs.append(F)
+            ys.append(torch.empty(300 * F, device=self.device))
+        if cps and bool(torch.stack([((t < 0) | (t >= 1024)).any() for t in cps + ccs]).any()):
+            raise IndexError("codes must lie in [0, 1024)")
+        n = len(sessions)
+        frames = (ctypes.c_int * max(n, 1))()
+        P = lambda ts: _ptr_array(ctypes.c_void_p, [t.data_ptr() for t in ts])
+        e = self.engine
+        rc = e.L.fac_vc_pool_convert(e.handle, self.pid, n, _ptr_array(ctypes.c_int, sessions), _ptr_array(ctypes.c_int, Fs),
+                                     P(cps), P(ccs), _ptr_array(ctypes.c_int, [c.shape[1] for c in ccs]), P(ys), frames,
+                                     _stream(self.device))
+        _lib.check(e.handle, rc, "fac_vc_pool_convert")
+        return {s: ys[i][:300 * frames[i]].view(1, 1, 300 * frames[i]) for i, s in enumerate(sessions)}
+
+    def _codes(self, codes):
+        """One session's codes -> (codes_p, codes_c, F), int64 and contiguous."""
+        for t in codes[:2]:
+            self._check_device(t)
+            if t.dim() != 3 or t.is_floating_point() or t.is_complex():
+                raise ValueError("codes must be integer tensors [1, rows, F]; got %s %s" % (t.dtype, tuple(t.shape)))
+        cp, cc = (t.detach().to(torch.int64).contiguous() for t in codes[:2])
+        F = cp.shape[2]
+        if cp.shape[:2] != (1, 1) or cc.shape[0] != 1 or cc.shape[1] not in (1, 2) or cc.shape[2] != F or F < 1:
+            raise ValueError("codes must be [codes_p [1, 1, F], codes_c [1, 1|2, F]] with F >= 1; got %s, %s"
+                             % (tuple(cp.shape), tuple(cc.shape)))
+        return cp, cc, F
+
+    def finish(self, sessions):
+        """End of the sessions' utterances -> {session: y [1,1,300 k]}, the last k <= lookahead_frames frames."""
+        sessions = self._sessions(sessions)
+        ys = [torch.empty(300 * self.lookahead_frames, device=self.device) for _ in sessions]
+        frames = (ctypes.c_int * max(len(sessions), 1))()
+        e = self.engine
+        rc = e.L.fac_vc_pool_finish(e.handle, self.pid, len(sessions), _ptr_array(ctypes.c_int, sessions),
+                                    _ptr_array(ctypes.c_void_p, [y.data_ptr() for y in ys]), frames, _stream(self.device))
+        _lib.check(e.handle, rc, "fac_vc_pool_finish")
+        return {s: ys[i][:300 * frames[i]].view(1, 1, 300 * frames[i]) for i, s in enumerate(sessions)}
+
+
 class _HeadLinear(nn.Module):
     """A plain nn.Linear(indim, outdim) run through the head machinery (kind "linear" of fac_head_finalize)."""
 

@@ -187,6 +187,45 @@ int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int6
                             void* stream);
 int fac_stream_end(fac_handle* h, int stream_id);
 
+/* Stream pools: many live sessions, each behaving exactly like its own B = 1 stream, stepped in shared launches.  A pool
+ * owns the state of up to `capacity` sessions; a step names any subset of them, each at most once, with its own chunk.
+ * Sessions at the same stage of their windows (after a short warm-up, those fed equal chunk lengths) share one launch
+ * sequence, up to 32 per batch (the LSTM's batch tile); larger groups run as several batches.  A session's outputs are
+ * bit-identical to those of a B = 1 stream fed the same chunks, whoever shares its launches.
+ * Every step validates all its arguments before it launches anything: a rejected step returns a negative status and leaves
+ * every session of the pool as it was.  Per-session buffers are device pointers, the arrays holding them host arrays.
+ * FAC_ERR_INVALID: an unknown, closed or repeated session, a null buffer, the chunk rules of the stream entries;
+ * FAC_ERR_STATE: a session in the wrong state for the call (as the stream entries), open on a full pool.
+ *
+ * fac_codes_pool_create(capacity >= 1, n_c = 1 or 2 for every session) -> pool id; needs the encoder and the quantizer.
+ * fac_codes_pool_open -> session id (a slot, reused after close), a fresh fac_stream_encode_codes stream.
+ * fac_codes_pool_encode_codes: for i < n, session sessions[i] takes x[i] [1,1,T[i]] (rules of fac_stream_encode_codes) and
+ * writes codes_p[i] [1,1,F], codes_c[i] [1,n_c,F], codes_r[i] [1,3,F]; frames[i] = F (T/300 - 1 on a first chunk, T/300 after).
+ * fac_codes_pool_finish_codes: fac_stream_finish_codes per session (one frame each; timbre may be NULL, or timbre[i] NULL).
+ * The session's mel rows are kept until the pool is destroyed and reused by the next session of the slot.
+ * fac_vc_pool_create(capacity >= 1, use_p_code, use_c_code, 0 <= n_c <= 2) -> pool id; needs the redecoder and its decoder.
+ * fac_vc_pool_open(timbre [1,1024] device) -> session id; the timbre's cond layer runs once here.
+ * fac_vc_pool_convert: session sessions[i] takes codes_p[i] [1,1,F[i]], codes_c[i] [1,n_c_rows[i],F[i]] (as
+ * fac_vc_stream_convert) and writes frames[i] = k output frames to y[i] [1,1,300*k] (capacity 300*F[i] floats).
+ * fac_vc_pool_finish: fac_vc_stream_finish per session; y[i] holds 300*44 floats.
+ * fac_*_pool_close frees a session's slot; fac_*_pool_destroy frees the pool (and runs at fac_destroy). */
+int fac_codes_pool_create(fac_handle* h, int capacity, int n_c);
+int fac_codes_pool_open(fac_handle* h, int pool_id, void* stream);
+int fac_codes_pool_encode_codes(fac_handle* h, int pool_id, int n, const int* sessions, const int* T, const float* const* x,
+                                int64_t* const* codes_p, int64_t* const* codes_c, int64_t* const* codes_r, int* frames,
+                                void* stream);
+int fac_codes_pool_finish_codes(fac_handle* h, int pool_id, int n, const int* sessions, int64_t* const* codes_p,
+                                int64_t* const* codes_c, int64_t* const* codes_r, float* const* timbre, void* stream);
+int fac_codes_pool_close(fac_handle* h, int pool_id, int session);
+int fac_codes_pool_destroy(fac_handle* h, int pool_id);
+int fac_vc_pool_create(fac_handle* h, int capacity, int use_p_code, int use_c_code, int n_c);
+int fac_vc_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream);
+int fac_vc_pool_convert(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
+                        const int64_t* const* codes_c, const int* n_c_rows, float* const* y, int* frames, void* stream);
+int fac_vc_pool_finish(fac_handle* h, int pool_id, int n, const int* sessions, float* const* y, int* frames, void* stream);
+int fac_vc_pool_close(fac_handle* h, int pool_id, int session);
+int fac_vc_pool_destroy(fac_handle* h, int pool_id);
+
 /* quantize/rvq.py:27-75 ResidualVQ.forward (eval) over quantize/fvq.py FactorizedVectorQuantize,
  * dim=1024, codebook_dim=8, 2^10 entries (BASELINE configs[3]).  Parameters are passed directly
  * (already weight-normed, HOST): per quantizer q: in_w [8,1024], in_b [8], out_w [1024,8],

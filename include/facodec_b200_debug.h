@@ -66,6 +66,17 @@ int fac_debug_tc_trace(fac_handle* h, long long* out80);
  * [G][H/16][hi|lo][8][4U], column of row r of k pair k2 = r ^ swizzle(k2) (conflict-free fragment loads).
  * Returns the number of 32-bit words (G*H*4U) also when out is NULL/too small; info3 = {U, G, 4U}. */
 long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out, long long capacity_floats, int* info3);
+/* Host-only: the launch plan of one stream-pool step.  kind 0 (codes pool): counters[4 i ..] = {samples encoded, x history
+ * length, LSTM-output history length, frames emitted} of session i, lengths[i] = its chunk in samples; kind 1 (voice-conversion
+ * pool): counters[3 i ..] = {code frames received, z frames final, output frames emitted}, lengths[i] = its chunk in frames.
+ * group[i] receives the group of session i (sessions whose launch sequences are identical; groups numbered in order of first
+ * appearance), batch[i] its batch (each group cut into batches of <= 32 in input order).  Returns the number of batches. */
+int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch);
+/* Host-only: where one batch lane's carry of one resident-W LSTM layer (H = 1024 or 1536; pass3 = 1: hi | lo h planes) sits
+ * in a stream's state: pos[j] for word j (h words first, then the c floats) is its index in [state_h words | state_c floats].
+ * The pools move exactly these words between a session's slot and any lane.  Returns the word count (also when pos is
+ * NULL or capacity too small). */
+long long fac_debug_lstm_lane_map(int H, int pass3, int lane, long long* pos, long long capacity);
 /* Host-only: the padding index map every conv kernel applies instead of materialising a padded copy
  * (dac/model/encodec.py:96-113 pad1d incl. the short-input branch): out[i] = source row of padded position
  * i - pad_left, or -1 where the padded value is zero; n must be pad_left + L + pad_right. */
