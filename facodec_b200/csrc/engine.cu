@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <map>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/facodec_b200.h"
@@ -95,6 +96,8 @@ struct fac_handle {
     std::vector<CodesPool*> codes_pools;
     struct VcPool;                  // many B = 1 voice-conversion streams stepped in shared batches (fac_vc_pool_*)
     std::vector<VcPool*> vc_pools;
+    struct DecPool;                 // many B = 1 decode-from-codes streams stepped in shared batches (fac_dec_pool_*)
+    std::vector<DecPool*> dec_pools;
     struct HeadSet;                 // modules/quantize.py:106-125 CNNLSTM instances (fac_head_*)
     std::vector<HeadSet*> heads;
     char* ws = nullptr; size_t ws_bytes = 0;
@@ -841,8 +844,9 @@ bool lstm_resident(const Ctx& c, const LstmW& L) {
 }
 
 // SLSTM (encodec.py:272-288) on channels-last x [B][T][H]; y = lstm2(lstm1(x)) + x.  st (streaming, B <= 32, resident-W
-// kernel only): initial state read from / final state written to st.
-void slstm(Ctx& c, const LstmW& L, const float* x, float* y, int B, int T, LstmState* st = nullptr) {
+// kernel only): initial state read from / final state written to st.  lens (HOST, B entries, with st): row b runs lens[b]
+// steps, and st receives the state after them (rows of y past lens[b] are finite don't-cares).
+void slstm(Ctx& c, const LstmW& L, const float* x, float* y, int B, int T, LstmState* st = nullptr, const int* lens = nullptr) {
     const int H = L.H;
     float* xg = c.alloc<float>((size_t)B * T * 4 * H);
     float* h1 = c.alloc<float>((size_t)B * T * H);
@@ -867,12 +871,16 @@ void slstm(Ctx& c, const LstmW& L, const float* x, float* y, int B, int T, LstmS
             p.hT = hT; p.bar = bar;
             p.B = nb; p.T = T; p.H = H; p.U = L.U; p.G = L.G;
             c.begin("lstm_rec", 2.0 * nb * T * 4.0 * H * H, 4.0 * ((double)nb * T * 5 * H + 4.0 * H * H));
-            if (st && (!v2 || B > 32)) { c.check(cudaErrorNotSupported, "lstm.stream (needs the resident-W kernel and B <= 32)"); c.end(); continue; }
+            if ((st || lens) && (!v2 || B > 32 || !st)) {
+                c.check(cudaErrorNotSupported, "lstm.stream (needs the resident-W kernel and B <= 32)"); c.end(); continue;
+            }
             if (v2) {
                 p.whh_p2 = reinterpret_cast<const uint32_t*>(c.W(L.whh2[l][pass3]));
                 p.h16 = h16; p.pass3 = pass3;
                 if (st) { p.state_h = st->h[l]; p.state_c = st->c[l]; }
-                c.check(launch_lstm2_layer(p, c.st), "lstm.rec2");
+                LstmLaneLens ll = {};
+                for (int b = 0; lens && b < nb; ++b) ll.len[b] = lens[b];
+                c.check(launch_lstm2_layer(p, c.st, lens ? &ll : nullptr), "lstm.rec2");
             } else {
                 c.check(launch_lstm_layer(p, c.st), "lstm.rec");
             }
@@ -1393,6 +1401,7 @@ int fac_destroy(fac_handle* h) {
     for (auto* vs : h->vc_streams) { for (void* p : vs->all) if (p) cudaFree(p); delete vs; }
     for (int i = 0; i < (int)h->codes_pools.size(); ++i) fac_codes_pool_destroy(h, i);
     for (int i = 0; i < (int)h->vc_pools.size(); ++i) fac_vc_pool_destroy(h, i);
+    for (int i = 0; i < (int)h->dec_pools.size(); ++i) fac_dec_pool_destroy(h, i);
     delete h;
     return FAC_OK;
 }
@@ -1997,18 +2006,38 @@ int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int6
 }  // extern "C"
 
 namespace {
-// The body of fac_stream_decode / fac_stream_decode_codes: `latents(c, B)` returns the chunk's channels-last latents
-// [B][Fc][1024] (transposed from the caller's z, or dequantized from codes); the stream state is the same either way.
-template <typename F>
-int stream_decode(fac_handle* h, int stream_id, int Fc, float* y, void* stream, const char* who, F latents) {
-    int rc = check_ready(h, FAC_DECODER);
-    if (rc) return rc;
-    if (stream_id < 0 || stream_id >= (int)h->streams.size() || !h->streams[stream_id]->alive || !y) { h->err = std::string(who) + ": bad arguments"; return FAC_ERR_INVALID; }
-    fac_handle::Stream& s = *h->streams[stream_id];
-    if (Fc <= 0 || (s.dec_frames == 0 && Fc < kStreamMinFirst)) { h->err = std::string(who) + ": the first chunk needs at least 10 frames"; return FAC_ERR_INVALID; }
+// The chunk rules and the decoder support of fac_stream_decode / fac_stream_decode_codes, for a stream row that has decoded
+// `frames` frames and is fed Fc more.
+int stream_decode_check(fac_handle* h, long long frames, int Fc, const char* who) {
+    if (Fc <= 0 || (frames == 0 && Fc < kStreamMinFirst)) { h->err = std::string(who) + ": the first chunk needs at least 10 frames"; return FAC_ERR_INVALID; }
     if (!h->lstm_v2 || !h->dec_bf16 || !h->dec_lstm_fp16 || !h->dec.lstm.has2[0]) { h->err = std::string(who) + ": needs the resident-W LSTM kernel"; return FAC_ERR_UNSUPPORTED; }
+    return FAC_OK;
+}
+
+// Inside a launch sequence: lane b of n copies words(b) 32-bit words from src(b) to dst(b) (launch_lane_copy).
+template <typename W, typename S, typename D>
+void lane_copy(Ctx& c, int n, W words, S src, D dst, const char* what) {
+    if (c.dry) return;
+    LaneCopyParams p;
+    p.n = n;
+    for (int b = 0; b < n; ++b) { p.src[b] = (const uint32_t*)src(b); p.dst[b] = (uint32_t*)dst(b); p.words[b] = words(b); }
+    c.check(launch_lane_copy(p, c.st), what);
+}
+
+// The body of fac_stream_decode / fac_stream_decode_codes on a checked stream: row b takes F[b] new frames (HOST, s.B
+// entries), whose channels-last latents `latents(c, B)` returns as [B][Fmax][1024] (Fmax = the largest F[b]; transposed
+// from the caller's z, or dequantized from codes).  y receives [B][300 Fmax], row b valid for its first 300 F[b] samples.
+// With equal F this is one stream chunk.  With unequal F (a decode pool's batch) each row runs on a window padded past its
+// own end: the decoder after the LSTM is causal (left reflect padding, no right padding, transposed convs trimmed on the
+// right), so no sample before a row's end reads the padding; the LSTM stops each row at its own end, and the histories are
+// cut at each row's own end.  The stream's counters advance by Fmax (a pool keeps its sessions' own).
+template <typename L>
+int stream_decode(fac_handle* h, fac_handle::Stream& s, const int* F, float* y, void* stream, L latents) {
     const int B = s.B, zh = s.z_hist_len, dh = s.dy_hist_len;
-    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    int Fc = 0;
+    bool mixed = false;
+    for (int b = 0; b < B; ++b) { Fc = F[b] > Fc ? F[b] : Fc; mixed = mixed || F[b] != F[0]; }
+    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
         const DecW& d = h->dec;
         const float* znew = latents(c, B);
         float* zw = c.alloc<float>((size_t)B * (zh + Fc) * LATENT);
@@ -2021,7 +2050,7 @@ int stream_decode(fac_handle* h, int stream_id, int Fc, float* y, void* stream, 
         float* ynew = c.alloc<float>((size_t)B * Fc * 1536);
         LstmState st;
         st.h[0] = s.dec_h[0]; st.h[1] = s.dec_h[1]; st.c[0] = s.dec_c[0]; st.c[1] = s.dec_c[1];
-        slstm(c, d.lstm, c0new, ynew, B, Fc, &st);
+        slstm(c, d.lstm, c0new, ynew, B, Fc, &st, mixed ? F : nullptr);
         const int Fw = dh + Fc;
         const size_t stage = decoder_stage_floats(B, Fw);
         float* buf[3] = {c.alloc<float>(stage), c.alloc<float>(stage), c.alloc<float>(stage)};
@@ -2031,6 +2060,17 @@ int stream_decode(fac_handle* h, int stream_id, int Fc, float* y, void* stream, 
         float* yw = c.alloc<float>((size_t)B * Fw * HOP);
         decoder_stack(c, d, yw_in, -1, buf, B, Fw, yw);
         copy_rows(c, y, Fc * HOP, yw, Fw * HOP, dh * HOP, Fc * HOP, 1, B, "stream.ynew");
+        if (mixed) {
+            auto nz = [&](int b) { return zh + F[b] < 6 ? zh + F[b] : 6; };
+            auto nd = [&](int b) { return dh + F[b] < kDecCtx ? dh + F[b] : kDecCtx; };
+            lane_copy(c, B, [&](int b) { return (long long)nz(b) * LATENT; },
+                      [&](int b) { return zw + ((size_t)b * (zh + Fc) + zh + F[b] - nz(b)) * LATENT; },
+                      [&](int b) { return s.z_hist + (size_t)b * 6 * LATENT; }, "stream.zh_lanes");
+            lane_copy(c, B, [&](int b) { return (long long)nd(b) * 1536; },
+                      [&](int b) { return yw_in + ((size_t)b * Fw + dh + F[b] - nd(b)) * 1536; },
+                      [&](int b) { return s.dy_hist + (size_t)b * kDecCtx * 1536; }, "stream.dh_lanes");
+            return;
+        }
         const int nzh = zh + Fc < 6 ? zh + Fc : 6, ndh = Fw < kDecCtx ? Fw : kDecCtx;
         float* tz = c.alloc<float>((size_t)B * 6 * LATENT);
         float* td = c.alloc<float>((size_t)B * kDecCtx * 1536);
@@ -2046,6 +2086,18 @@ int stream_decode(fac_handle* h, int stream_id, int Fc, float* y, void* stream, 
     }
     return rc;
 }
+
+// fac_stream_decode / fac_stream_decode_codes on stream stream_id: the checks, then one chunk of Fc frames on every row.
+template <typename L>
+int stream_decode_chunk(fac_handle* h, int stream_id, int Fc, float* y, void* stream, const char* who, L latents) {
+    int rc = check_ready(h, FAC_DECODER);
+    if (rc) return rc;
+    if (stream_id < 0 || stream_id >= (int)h->streams.size() || !h->streams[stream_id]->alive || !y) { h->err = std::string(who) + ": bad arguments"; return FAC_ERR_INVALID; }
+    fac_handle::Stream& s = *h->streams[stream_id];
+    if ((rc = stream_decode_check(h, s.dec_frames, Fc, who))) return rc;
+    const std::vector<int> F(s.B, Fc);
+    return stream_decode(h, s, F.data(), y, stream, latents);
+}
 }  // namespace
 
 extern "C" {
@@ -2054,7 +2106,7 @@ int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, floa
     int rc = check_ready(h, FAC_DECODER);
     if (rc) return rc;
     if (!z) { h->err = "fac_stream_decode: bad arguments"; return FAC_ERR_INVALID; }
-    return stream_decode(h, stream_id, Fc, y, stream, "fac_stream_decode", [&](Ctx& c, int B) {
+    return stream_decode_chunk(h, stream_id, Fc, y, stream, "fac_stream_decode", [&](Ctx& c, int B) {
         float* znew = c.alloc<float>((size_t)B * Fc * LATENT);
         if (!c.dry) c.check(launch_transpose(z, znew, B, LATENT, Fc, c.st), "dec.z_transpose");
         return znew;
@@ -2070,7 +2122,7 @@ int fac_stream_decode_codes(fac_handle* h, int stream_id, const int64_t* codes_p
         h->err = "fac_stream_decode_codes: bad arguments (1 <= content rows <= 2, 0 <= residual rows <= 3)";
         return FAC_ERR_INVALID;
     }
-    return stream_decode(h, stream_id, Fc, y, stream, "fac_stream_decode_codes", [&](Ctx& c, int B) {
+    return stream_decode_chunk(h, stream_id, Fc, y, stream, "fac_stream_decode_codes", [&](Ctx& c, int B) {
         return (const float*)dequantize_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, Fc, false).outs_cl;
     });
 }
@@ -2266,6 +2318,19 @@ struct fac_handle::VcPool {
     int64_t* cin = nullptr; size_t cin_cap = 0;         // [32][1 + n_c][F] gathered codes
     float* yout = nullptr; size_t yout_cap = 0;         // [32][300 k] output before the scatter
 };
+// The decode pool's sessions are rows of a decode-from-codes stream.  Its launch sequence depends only on the history depth
+// (zh = min(frames, 6) and dh = min(frames, 20) frames; a first chunk has >= 10 frames, so min(frames, 20) fixes both): the
+// chunk lengths and code rows of a batch may differ (stream_decode pads each lane past its own end).
+struct fac_handle::DecPool {
+    int cap = 0;
+    std::vector<long long> frames;          // frames decoded by each slot's session
+    std::vector<char> used;
+    Stream* lanes = nullptr;                // the B = 32 batch
+    float *z_hist = nullptr, *dy_hist = nullptr;        // [cap][6][1024], [cap][kDecCtx][1536]
+    uint32_t* carry = nullptr;              // [cap][2 layers][kDecCarryWords] decoder-LSTM (h, c) in lstm2_lane_map order
+    float* gb = nullptr;                    // [cap][2048] timbre_linear(timbre) of each session
+    float* yout = nullptr; size_t yout_cap = 0;         // [32][300 Fmax] output before the scatter
+};
 
 namespace {
 constexpr int kCarryWords = 2 * (LATENT / 2) + LATENT;   // one encoder-LSTM layer of one lane: hi | lo h planes, c
@@ -2301,12 +2366,16 @@ int grow_buf(fac_handle* h, E*& p, size_t& cap, size_t n, cudaStream_t st) {
     return FAC_OK;
 }
 
-// lane b of a batch of n: `words` 32-bit words from src(b) to dst(b)
-template <typename S, typename D>
-int lane_move(fac_handle* h, int n, long long words, S src, D dst, cudaStream_t st, const char* what) {
+// lane b of a batch of n: `words` (a count, or a function of b) 32-bit words from src(b) to dst(b)
+template <typename W, typename S, typename D>
+int lane_move(fac_handle* h, int n, W words, S src, D dst, cudaStream_t st, const char* what) {
     LaneCopyParams p;
-    p.n = n; p.words = words;
-    for (int b = 0; b < n; ++b) { p.src[b] = (const uint32_t*)src(b); p.dst[b] = (uint32_t*)dst(b); }
+    p.n = n;
+    for (int b = 0; b < n; ++b) {
+        p.src[b] = (const uint32_t*)src(b); p.dst[b] = (uint32_t*)dst(b);
+        if constexpr (std::is_invocable_v<W, int>) p.words[b] = words(b);
+        else p.words[b] = words;
+    }
     cudaError_t e = launch_lane_copy(p, st);
     if (e != cudaSuccess) { h->err = std::string(what) + ": " + cudaGetErrorString(e); return FAC_ERR_CUDA; }
     return FAC_OK;
@@ -2390,17 +2459,24 @@ void free_vc_pool(fac_handle::VcPool* P) {
     delete P;
 }
 
-// Moves the encoder-LSTM carries of a batch between the sessions' slots and the lanes' state tiles.
-int codes_pool_carry(fac_handle* h, fac_handle::CodesPool& P, const std::vector<int>& slots, int to_lanes, cudaStream_t st) {
+// Moves the 2-layer LSTM carries (H, pass3; `words` per layer) of a batch between the sessions' slots in `carry`
+// ([slot][2 layers][words]) and the lanes' state tiles (state_h[l], state_c[l]).
+int pool_carry(fac_handle* h, uint32_t* const* state_h, float* const* state_c, uint32_t* carry, int words, int H, int pass3,
+               const std::vector<int>& slots, int to_lanes, cudaStream_t st) {
     for (int l = 0; l < 2; ++l) {
         LaneCarryParams p;
-        p.n = (int)slots.size(); p.H = LATENT; p.U = lstm_units_per_cta(LATENT); p.pass3 = 1; p.to_lanes = to_lanes;
-        p.state_h = P.lanes->enc_h[l]; p.state_c = P.lanes->enc_c[l];
-        for (int b = 0; b < p.n; ++b) p.slot[b] = P.carry + ((size_t)slots[b] * 2 + l) * kCarryWords;
+        p.n = (int)slots.size(); p.H = H; p.U = lstm_units_per_cta(H); p.pass3 = pass3; p.to_lanes = to_lanes;
+        p.state_h = state_h[l]; p.state_c = state_c[l];
+        for (int b = 0; b < p.n; ++b) p.slot[b] = carry + ((size_t)slots[b] * 2 + l) * words;
         cudaError_t e = launch_lstm2_lane_carry(p, st);
         if (e != cudaSuccess) { h->err = std::string("pool.carry: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
     }
     return FAC_OK;
+}
+
+// ... the encoder-LSTM carries of a codes-pool batch.
+int codes_pool_carry(fac_handle* h, fac_handle::CodesPool& P, const std::vector<int>& slots, int to_lanes, cudaStream_t st) {
+    return pool_carry(h, P.lanes->enc_h, P.lanes->enc_c, P.carry, kCarryWords, LATENT, 1, slots, to_lanes, st);
 }
 
 // One batch of a codes-pool step: sessions slots[b] (equal codes_key) fed T samples each from x[b].
@@ -2498,6 +2574,76 @@ std::vector<T> pick(const T* a, const std::vector<int>& idx) {
     std::vector<T> out;
     for (int i : idx) out.push_back(a[i]);
     return out;
+}
+
+constexpr int kDecCarryWords = 1536 / 2 + 1536;   // one decoder-LSTM layer of one lane: one fp16 h plane, c
+
+// The launch-plan key of a decode-pool session that has decoded `frames` frames: its history depth.
+std::vector<long long> dec_key(long long frames) { return {frames < kDecCtx ? frames : kDecCtx}; }
+
+fac_handle::DecPool* dec_pool(fac_handle* h, int id) {
+    return h && id >= 0 && id < (int)h->dec_pools.size() ? h->dec_pools[id] : nullptr;
+}
+
+void free_dec_pool(fac_handle::DecPool* P) {
+    if (P->lanes) { for (void* p : P->lanes->all) if (p) cudaFree(p); delete P->lanes; }
+    for (void* p : {(void*)P->z_hist, (void*)P->dy_hist, (void*)P->carry, (void*)P->gb, (void*)P->yout}) if (p) cudaFree(p);
+    delete P;
+}
+
+// One batch of a decode-pool step: sessions slots[b] (equal dec_key) fed F[b] frames each, their codes and rows per lane.
+int dec_pool_batch(fac_handle* h, fac_handle::DecPool& P, const std::vector<int>& slots, const std::vector<int>& F,
+                   const int64_t* const* codes_p, const int64_t* const* codes_c, const int* n_c, const int64_t* const* codes_r,
+                   const int* n_r, float* const* y, cudaStream_t st) {
+    using S = fac_handle::Stream;
+    S& L = *P.lanes;
+    const int nb = (int)slots.size();
+    const long long frames = P.frames[slots[0]];
+    const int zh = (int)std::min(frames, 6LL), dh = (int)std::min(frames, (long long)kDecCtx);
+    const int Fmax = *std::max_element(F.begin(), F.end());
+    const size_t zpl = (size_t)6 * LATENT, dpl = (size_t)kDecCtx * 1536;
+    int rc = FAC_OK;
+    auto mv = [&](auto words, auto src, auto dst, const char* what) {
+        if (rc == FAC_OK) rc = lane_move(h, nb, words, src, dst, st, what);
+    };
+    mv((long long)zh * LATENT, [&](int b) { return P.z_hist + slots[b] * zpl; }, [&](int b) { return L.z_hist + b * zpl; }, "pool.z_hist");
+    mv((long long)dh * 1536, [&](int b) { return P.dy_hist + slots[b] * dpl; }, [&](int b) { return L.dy_hist + b * dpl; }, "pool.dy_hist");
+    if (rc == FAC_OK) rc = pool_carry(h, L.dec_h, L.dec_c, P.carry, kDecCarryWords, 1536, 0, slots, 1, st);
+    if (rc) return rc;
+    L.B = nb; L.z_hist_len = zh; L.dy_hist_len = dh; L.dec_frames = frames;
+    rc = stream_decode(h, L, F.data(), P.yout, st, [&](Ctx& c, int B) {
+        float* z = c.alloc<float>((size_t)B * Fmax * LATENT);
+        if (c.dry) return (const float*)z;
+        DeqLaneParams dp;
+        for (int i = 0; i < 6; ++i) {
+            const VqW& v = h->qw.vq[i];
+            dp.vq[i] = VqWeights{c.W(v.w_in), c.W(v.b_in), c.W(v.cb), c.W(v.cbn), c.W(v.cbn2), c.W(v.w_out), c.W(v.b_out)};
+        }
+        double codes = 0;
+        for (int b = 0; b < B; ++b) {
+            dp.codes_p[b] = codes_p[b]; dp.codes_c[b] = codes_c[b]; dp.codes_r[b] = codes_r[b];
+            dp.n_c[b] = n_c[b]; dp.n_r[b] = n_r[b]; dp.F[b] = F[b];
+            dp.gamma_beta[b] = P.gb + (size_t)slots[b] * 2048;
+            codes += (double)F[b] * (1 + n_c[b] + n_r[b]);
+        }
+        dp.outs = z; dp.n = B; dp.Fmax = Fmax;
+        c.begin("dequantize", 2.0 * codes * 8.0 * 1024, 8.0 * codes + 4.0 * 1024 * B * Fmax);
+        c.check(launch_dequantize_lanes(dp, c.st), "dequantize_lanes");
+        c.end();
+        c.tap("dec_pool.latents", z, (size_t)B * Fmax * LATENT);
+        return (const float*)z;
+    });
+    if (rc) return rc;
+    auto nz = [&](int b) { return (long long)std::min(zh + F[b], 6) * LATENT; };
+    auto nd = [&](int b) { return (long long)std::min(dh + F[b], kDecCtx) * 1536; };
+    mv(nz, [&](int b) { return L.z_hist + b * zpl; }, [&](int b) { return P.z_hist + slots[b] * zpl; }, "pool.z_hist");
+    mv(nd, [&](int b) { return L.dy_hist + b * dpl; }, [&](int b) { return P.dy_hist + slots[b] * dpl; }, "pool.dy_hist");
+    if (rc == FAC_OK) rc = pool_carry(h, L.dec_h, L.dec_c, P.carry, kDecCarryWords, 1536, 0, slots, 0, st);
+    mv([&](int b) { return (long long)F[b] * HOP; }, [&](int b) { return P.yout + (size_t)b * Fmax * HOP; },
+       [&](int b) { return y[b]; }, "pool.y");
+    if (rc) return rc;
+    for (int b = 0; b < nb; ++b) P.frames[slots[b]] += F[b];
+    return FAC_OK;
 }
 }  // namespace
 
@@ -2767,12 +2913,117 @@ int fac_vc_pool_destroy(fac_handle* h, int pool_id) {
     return FAC_OK;
 }
 
+int fac_dec_pool_create(fac_handle* h, int capacity) {
+    int rc = check_ready(h, FAC_QUANTIZER);
+    if (!rc) rc = check_ready(h, FAC_DECODER);
+    if (rc) return rc;
+    const char* who = "fac_dec_pool_create";
+    if (capacity < 1) { h->err = "fac_dec_pool_create: bad arguments (capacity >= 1)"; return FAC_ERR_INVALID; }
+    cudaSetDevice(h->device);
+    auto* P = new fac_handle::DecPool();
+    P->cap = capacity;
+    P->lanes = alloc_stream(h, kLaneMax, who);
+    const size_t c = (size_t)capacity;
+    rc = P->lanes ? FAC_OK : FAC_ERR_CUDA;
+    if (!rc) rc = dev_zeros(h, P->z_hist, c * 6 * LATENT, who);
+    if (!rc) rc = dev_zeros(h, P->dy_hist, c * kDecCtx * 1536, who);
+    if (!rc) rc = dev_zeros(h, P->carry, c * 2 * kDecCarryWords, who);
+    if (!rc) rc = dev_zeros(h, P->gb, c * 2048, who);
+    if (rc) { free_dec_pool(P); return rc; }
+    P->frames.assign(c, 0);
+    P->used.assign(c, 0);
+    h->dec_pools.push_back(P);
+    return (int)h->dec_pools.size() - 1;
+}
+
+int fac_dec_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream) {
+    int rc = check_ready(h, FAC_QUANTIZER);
+    if (!rc) rc = check_ready(h, FAC_DECODER);
+    if (rc) return rc;
+    fac_handle::DecPool* P = dec_pool(h, pool_id);
+    if (!P || !timbre) { h->err = "fac_dec_pool_open: bad arguments"; return FAC_ERR_INVALID; }
+    int i = 0;
+    while (i < P->cap && P->used[i]) ++i;
+    if (i == P->cap) { h->err = "fac_dec_pool_open: the pool is full (capacity " + std::to_string(P->cap) + ")"; return FAC_ERR_STATE; }
+    // gamma | beta by the B = 1 launch a stream's decode_codes runs on every chunk, so the bits are the same
+    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        const float* gb = timbre_gamma_beta(c, timbre, 1);
+        if (c.dry) return;
+        c.check_nk(cudaMemcpyAsync(P->gb + (size_t)i * 2048, gb, sizeof(float) * 2048, cudaMemcpyDeviceToDevice, c.st), "pool.gb");
+        c.check_nk(cudaMemsetAsync(P->carry + (size_t)i * 2 * kDecCarryWords, 0, sizeof(uint32_t) * 2 * kDecCarryWords, c.st),
+                   "pool.carry");
+    });
+    if (rc) return rc;
+    P->frames[i] = 0;
+    P->used[i] = 1;
+    return i;
+}
+
+int fac_dec_pool_decode_codes(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
+                              const int64_t* const* codes_c, const int* n_c_rows, const int64_t* const* codes_r,
+                              const int* n_r_rows, float* const* y, void* stream) {
+    int rc = check_ready(h, FAC_QUANTIZER);
+    if (!rc) rc = check_ready(h, FAC_DECODER);
+    if (rc) return rc;
+    const char* who = "fac_dec_pool_decode_codes";
+    fac_handle::DecPool* P = dec_pool(h, pool_id);
+    if (!P || n < 0 || (n > 0 && (!sessions || !F || !codes_p || !codes_c || !n_c_rows || !codes_r || !n_r_rows || !y))) {
+        h->err = "fac_dec_pool_decode_codes: bad arguments";
+        return FAC_ERR_INVALID;
+    }
+    if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
+    std::vector<std::vector<long long>> keys(n);
+    int maxF = 0;
+    for (int i = 0; i < n; ++i) {
+        if (!codes_p[i] || !codes_c[i] || !y[i] || (n_r_rows[i] > 0 && !codes_r[i]) || n_c_rows[i] < 1 || n_c_rows[i] > 2 ||
+            n_r_rows[i] < 0 || n_r_rows[i] > 3) {
+            h->err = "fac_dec_pool_decode_codes: bad arguments of session " + std::to_string(sessions[i]) +
+                     " (null buffer, or not 1 <= content rows <= 2, 0 <= residual rows <= 3)";
+            return FAC_ERR_INVALID;
+        }
+        const long long frames = P->frames[sessions[i]];
+        if ((rc = stream_decode_check(h, frames, F[i], who))) return rc;
+        keys[i] = dec_key(frames);
+        maxF = std::max(maxF, F[i]);
+    }
+    if (n == 0) return FAC_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = grow_buf(h, P->yout, P->yout_cap, (size_t)kLaneMax * HOP * maxF, st))) return rc;
+    for (const auto& b : pool_plan(keys, nullptr, nullptr)) {
+        rc = dec_pool_batch(h, *P, pick(sessions, b), pick(F, b), pick(codes_p, b).data(), pick(codes_c, b).data(),
+                            pick(n_c_rows, b).data(), pick(codes_r, b).data(), pick(n_r_rows, b).data(), pick(y, b).data(), st);
+        if (rc) return rc;
+    }
+    return FAC_OK;
+}
+
+int fac_dec_pool_close(fac_handle* h, int pool_id, int session) {
+    fac_handle::DecPool* P = dec_pool(h, pool_id);
+    if (!P || session < 0 || session >= P->cap || !P->used[session]) {
+        if (h) h->err = "fac_dec_pool_close: session " + std::to_string(session) + " is not open";
+        return FAC_ERR_INVALID;
+    }
+    P->used[session] = 0;
+    return FAC_OK;
+}
+
+int fac_dec_pool_destroy(fac_handle* h, int pool_id) {
+    fac_handle::DecPool* P = dec_pool(h, pool_id);
+    if (!P) return FAC_ERR_INVALID;
+    cudaSetDevice(h->device);
+    cudaDeviceSynchronize();
+    free_dec_pool(P);
+    h->dec_pools[pool_id] = nullptr;
+    return FAC_OK;
+}
+
 int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch) {
-    if (n < 0 || (n > 0 && (!counters || !lengths || !group || !batch)) || (kind != 0 && kind != 1)) return FAC_ERR_INVALID;
+    if (n < 0 || (n > 0 && (!counters || !lengths || !group || !batch)) || kind < 0 || kind > 2) return FAC_ERR_INVALID;
     std::vector<std::vector<long long>> keys(n);
     for (int i = 0; i < n; ++i) {
-        const long long* c = counters + (size_t)i * (kind == 0 ? 4 : 3);
-        keys[i] = kind == 0 ? codes_key(c[0], (int)c[1], (int)c[2], c[3], lengths[i]) : vc_key(c[0], c[1], c[2], lengths[i]);
+        const long long* c = counters + (size_t)i * (kind == 0 ? 4 : kind == 1 ? 3 : 1);
+        keys[i] = kind == 0 ? codes_key(c[0], (int)c[1], (int)c[2], c[3], lengths[i])
+                : kind == 1 ? vc_key(c[0], c[1], c[2], lengths[i]) : dec_key(c[0]);
     }
     return (int)pool_plan(keys, group, batch).size();
 }
@@ -3419,9 +3670,13 @@ int fac_debug_conv(fac_handle* h, const float* x, const float* w_host, const flo
     return FAC_OK;
 }
 
-int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, int upstream,
-                    const int* chunks, int n_chunks, float* y, void* stream) {
-    if (!h || !x || !w_host || !y || B <= 0 || T <= 0 || n_chunks < 0) return FAC_ERR_INVALID;
+}  // extern "C"
+
+namespace {
+// fac_debug_slstm, and with `carry` (DEVICE [B][2 layers][lane-map words], read as the initial state and overwritten with
+// the final one) fac_debug_slstm_lanes: one pass over T with row b stopped after lens[b] steps (lens null: T).
+int debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, int upstream,
+                const int* chunks, int n_chunks, const int* lens, uint32_t* carry, float* y, void* stream) {
     const bool chunked = chunks && n_chunks > 0;
     if (chunked) {
         long long sum = 0;
@@ -3450,14 +3705,16 @@ int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, i
     try { L = pack_lstm(&tmp, 0, "l", upstream != 0); } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_UNSUPPORTED; }
     cudaStream_t st = (cudaStream_t)stream;
     size_t hw = 0, cf = 0;
-    if (chunked) {
+    int pass3 = 0;
+    if (chunked || carry) {
         Ctx probe{&tmp, st, true};
         probe.vq_critical = upstream != 0;
         if (B > 32 || !lstm_resident(probe, L)) {
-            h->err = "fac_debug_slstm: chunks need B <= 32 and the resident-W LSTM kernel";
+            h->err = "fac_debug_slstm: chunks and lanes need B <= 32 and the resident-W LSTM kernel";
             return FAC_ERR_UNSUPPORTED;
         }
-        lstm2_state_sizes(H, L.U, lstm_pass3(probe), &hw, &cf);
+        pass3 = lstm_pass3(probe);
+        lstm2_state_sizes(H, L.U, pass3, &hw, &cf);
     }
     cudaSetDevice(h->device);
     cudaError_t e = cudaMalloc(&tmp.warena, (tmp.pack.size() + 64) * sizeof(float));
@@ -3465,8 +3722,9 @@ int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, i
     if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
     int rc = two_pass(&tmp, st, [&](Ctx& c) {
         c.vq_critical = upstream != 0;
-        if (!chunked) { slstm(c, L, x, y, B, T); return; }
-        // chunk by chunk with the state carried as fac_stream_encode / fac_stream_decode do, from a zero state
+        if (!chunked && !carry) { slstm(c, L, x, y, B, T); return; }
+        // chunk by chunk with the state carried as fac_stream_encode / fac_stream_decode do, from a zero state; or from the
+        // caller's per-lane carry, moved as the stream pools move it
         LstmState s;
         for (int l = 0; l < 2; ++l) {
             s.h[l] = c.alloc<uint32_t>(hw);
@@ -3474,6 +3732,22 @@ int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, i
             if (c.dry) continue;
             c.check_nk(cudaMemsetAsync(s.h[l], 0, sizeof(uint32_t) * hw, c.st), "slstm.state_h");
             c.check_nk(cudaMemsetAsync(s.c[l], 0, sizeof(float) * cf, c.st), "slstm.state_c");
+        }
+        if (carry) {
+            const int words = (pass3 ? 2 : 1) * (H / 2) + H;
+            auto move = [&](int to_lanes) {
+                for (int l = 0; l < 2 && !c.dry; ++l) {
+                    LaneCarryParams p;
+                    p.n = B; p.H = H; p.U = L.U; p.pass3 = pass3; p.to_lanes = to_lanes;
+                    p.state_h = s.h[l]; p.state_c = s.c[l];
+                    for (int b = 0; b < B; ++b) p.slot[b] = carry + ((size_t)b * 2 + l) * words;
+                    c.check(launch_lstm2_lane_carry(p, c.st), "slstm.carry");
+                }
+            };
+            move(1);
+            slstm(c, L, x, y, B, T, &s, lens);
+            move(0);
+            return;
         }
         for (int i = 0, t0 = 0; i < n_chunks; t0 += chunks[i++]) {
             const int n = chunks[i];
@@ -3489,6 +3763,24 @@ int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, i
     cudaFree(tmp.warena);
     if (tmp.ws) cudaFree(tmp.ws);
     return rc;
+}
+}  // namespace
+
+extern "C" {
+
+int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, int upstream,
+                    const int* chunks, int n_chunks, float* y, void* stream) {
+    if (!h || !x || !w_host || !y || B <= 0 || T <= 0 || n_chunks < 0) return FAC_ERR_INVALID;
+    return debug_slstm(h, x, w_host, B, T, H, upstream, chunks, n_chunks, nullptr, nullptr, y, stream);
+}
+
+int fac_debug_slstm_lanes(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, int upstream,
+                          const int* lens, uint32_t* carry, float* y, void* stream) {
+    if (!h || !x || !w_host || !y || !carry || B <= 0 || T <= 0) return FAC_ERR_INVALID;
+    if (lens && upstream) { h->err = "fac_debug_slstm_lanes: per-lane lengths run the decoder's one-pass class only"; return FAC_ERR_UNSUPPORTED; }
+    for (int b = 0; lens && b < B; ++b)
+        if (lens[b] < 0 || lens[b] > T) { h->err = "fac_debug_slstm_lanes: lane lengths must lie in [0, T]"; return FAC_ERR_INVALID; }
+    return debug_slstm(h, x, w_host, B, T, H, upstream, nullptr, 0, lens, carry, y, stream);
 }
 
 int fac_debug_fa_quantize(fac_handle* h, const float* f0, const float* z, const float* const vq_host[6][5],

@@ -90,8 +90,13 @@ struct LstmParams {
     unsigned int* bar = nullptr;  // grid barrier counter (zeroed by the launcher)
     int B = 0, T = 0, H = 0, U = 0, G = 0;
 };
+// Per-lane step counts of the resident-W kernel (a stream chunk whose lanes end at different frames): lane b updates (h, c)
+// for t < len[b] only and then carries them unchanged, so the state left behind is the one after len[b] steps; its output
+// rows t >= len[b] are finite don't-cares.  One-pass class (pass3 = 0) only; launches without them run a kernel
+// instantiation of their own.
+struct LstmLaneLens { int len[32]; };
 cudaError_t launch_lstm_layer(const LstmParams& p, cudaStream_t st);
-cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st);   // lstm2.cu
+cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st, const LstmLaneLens* lens = nullptr);   // lstm2.cu
 size_t lstm2_pack_words(int H, int U, int pass3);
 void lstm2_pack(const float* whh, int H, int U, int pass3, uint32_t* out);
 size_t lstm2_smem_bytes(int H, int U, int pass3);
@@ -111,12 +116,12 @@ struct LaneCarryParams {
     int n = 0, H = 0, U = 0, pass3 = 0, to_lanes = 0;
 };
 cudaError_t launch_lstm2_lane_carry(const LaneCarryParams& p, cudaStream_t st);
-// dst[b][0, words) = src[b][0, words) for lanes b < n (32-bit words; pool.cu): the slot <-> lane moves of the stream pools
+// dst[b][0, words[b]) = src[b][0, words[b]) for lanes b < n (32-bit words; pool.cu): the slot <-> lane moves of the stream pools
 struct LaneCopyParams {
     const uint32_t* src[kLaneMax];
     uint32_t* dst[kLaneMax];
+    long long words[kLaneMax];
     int n = 0;
-    long long words = 0;
 };
 cudaError_t launch_lane_copy(const LaneCopyParams& p, cudaStream_t st);
 int lstm_units_per_cta(int H);
@@ -170,6 +175,19 @@ struct DeqParams {
     int B = 0, T = 0;
 };
 cudaError_t launch_dequantize(const DeqParams& p, cudaStream_t st);
+// the same per lane of a decode-pool batch (n <= 32 lanes): lane b reads codes_p[b] [1][F[b]], codes_c[b] [n_c[b]][F[b]],
+// codes_r[b] [n_r[b]][F[b]] and gamma_beta[b] [2048], and writes outs [n][Fmax][1024] (frames t >= F[b] zero)
+struct DeqLaneParams {
+    const int64_t* codes_p[32];
+    const int64_t* codes_c[32];
+    const int64_t* codes_r[32];
+    const float* gamma_beta[32];
+    int n_c[32], n_r[32], F[32];
+    VqWeights vq[6];
+    float* outs = nullptr;
+    int n = 0, Fmax = 0;
+};
+cudaError_t launch_dequantize_lanes(const DeqLaneParams& p, cudaStream_t st);
 // losses[0] = commitment, losses[1] = codebook (identical in forward), from sqerr
 cudaError_t launch_vq_loss_reduce(const float* sqerr, int nq, int B, int Tq, float* losses2, cudaStream_t st);
 

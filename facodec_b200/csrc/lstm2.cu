@@ -24,6 +24,7 @@
 #include <cuda_fp16.h>
 
 #include <cstring>
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -57,9 +58,12 @@ __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0
 __host__ __device__ __forceinline__ int lstm2_swz_w(int k2, int R) { return R == 32 ? ((k2 & 3) << 3) : (((k2 >> 1) & 1) << 3); }
 __host__ __device__ __forceinline__ int lstm2_swz_h(int kp) { return (kp & 3) << 3; }
 
-// h exchange buffer: [2 parities][PL planes][H/2 k pairs][32] words; PL = 2 (hi, lo') when PASS3 else 1.
-template <int U, bool PASS3>
-__global__ void __launch_bounds__(L2_WARPS * 32, 1) lstm_rec2_kernel(LstmParams p) {
+// h exchange buffer: [2 parities][PL planes][H/2 k pairs][32] words; PL = 2 (hi, lo') when PASS3 else 1.  LENS (one-pass
+// class only): the per-lane step counts of LstmLaneLens apply (LstmLenParams); without them the kernel is the one it always
+// was.
+struct LstmLenParams : LstmParams { LstmLaneLens lens; };
+template <int U, bool PASS3, bool LENS>
+__global__ void __launch_bounds__(L2_WARPS * 32, 1) lstm_rec2_kernel(std::conditional_t<LENS, LstmLenParams, LstmParams> p) {
     constexpr int R = 4 * U;
     constexpr int RP = R + 1;
     constexpr int MT = R / 16, NTL = L2_BT / 8;
@@ -232,6 +236,22 @@ __global__ void __launch_bounds__(L2_WARPS * 32, 1) lstm_rec2_kernel(LstmParams 
             }
             float ig = sigmoid_f(g4[0]), fgt = sigmoid_f(g4[1]), gg = tanhf(g4[2]), og = sigmoid_f(g4[3]);
             float c = fgt * cstate[b * U + u] + ig * gg;
+            if constexpr (LENS) {
+                // the line above spelled out as the no-length kernel compiles it (ig * gg fused onto fgt * c), so that a
+                // lane's bits do not depend on which of the two instantiations runs it
+                c = __fmaf_rn(ig, gg, __fmul_rn(fgt, cstate[b * U + u]));
+                if (t >= p.lens.len[b]) {
+                    // past the lane's length: keep c and re-publish h_{t-1} (this thread's own unit, written by no other
+                    // CTA); the output row is a finite don't-care
+                    const int k = j0 + u, kp = k >> 1;
+                    const size_t widx = (size_t)kp * L2_BT + (size_t)(b ^ lstm2_swz_h(kp));
+                    const __half* hp = reinterpret_cast<const __half*>(hprev);
+                    hcur[widx * 2 + (k & 1)] = hp[widx * 2 + (k & 1)];
+                    if (PASS3) hcur[(plane_words + widx) * 2 + (k & 1)] = hp[(plane_words + widx) * 2 + (k & 1)];
+                    if (b < p.B) p.y[((size_t)b * p.T + t) * H + j0 + u] = skv[pi];
+                    continue;
+                }
+            }
             cstate[b * U + u] = c;
             float h = og * tanhf(c);
             // publish h_t pre-split: word (k pair, batch) holds units 2kp (low half) and 2kp+1
@@ -337,11 +357,11 @@ cudaError_t launch_lstm2_lane_carry(const LaneCarryParams& p, cudaStream_t st) {
     return cudaGetLastError();
 }
 
-template <int U, bool PASS3>
-static cudaError_t launch2_u(const LstmParams& p, cudaStream_t st) {
+template <int U, bool PASS3, bool LENS>
+static cudaError_t launch2_u(const LstmParams& p, const LstmLaneLens* lens, cudaStream_t st) {
     const size_t smem = lstm2_smem_bytes(p.H, U, PASS3 ? 1 : 0);
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
-    cudaError_t e = cudaFuncSetAttribute(lstm_rec2_kernel<U, PASS3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(lstm_rec2_kernel<U, PASS3, LENS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     e = cudaMemsetAsync(p.bar, 0, sizeof(unsigned int), st);
     if (e != cudaSuccess) return e;
@@ -352,20 +372,28 @@ static cudaError_t launch2_u(const LstmParams& p, cudaStream_t st) {
     if (p.state_h) e = cudaMemcpyAsync(p.h16 + (size_t)PL * plane_words, p.state_h, sizeof(uint32_t) * PL * plane_words, cudaMemcpyDeviceToDevice, st);
     else e = cudaMemsetAsync(p.h16 + (size_t)PL * plane_words, 0, sizeof(uint32_t) * PL * plane_words, st);
     if (e != cudaSuccess) return e;
-    LstmParams pp = p;
+    std::conditional_t<LENS, LstmLenParams, LstmParams> pp;
+    static_cast<LstmParams&>(pp) = p;
+    if constexpr (LENS) pp.lens = *lens;
     void* args[] = {&pp};
-    e = cudaLaunchCooperativeKernel((void*)lstm_rec2_kernel<U, PASS3>, dim3(p.G), dim3(L2_WARPS * 32), args, smem, st);
+    e = cudaLaunchCooperativeKernel((void*)lstm_rec2_kernel<U, PASS3, LENS>, dim3(p.G), dim3(L2_WARPS * 32), args, smem, st);
     if (e != cudaSuccess) return e;
     // h_{T-1} was published into parity slot (T-1) & 1
     if (p.state_h) e = cudaMemcpyAsync(p.state_h, p.h16 + (size_t)((p.T - 1) & 1) * PL * plane_words, sizeof(uint32_t) * PL * plane_words, cudaMemcpyDeviceToDevice, st);
     return e;
 }
 
-cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st) {
+cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st, const LstmLaneLens* lens) {
     if (p.B > L2_BT || p.B <= 0 || !p.whh_p2 || !p.h16) return cudaErrorInvalidValue;
     if ((p.H / 16) % L2_WARPS != 0) return cudaErrorInvalidValue;
-    if (p.U == 8) return p.pass3 ? launch2_u<8, true>(p, st) : launch2_u<8, false>(p, st);
-    if (p.U == 12) return p.pass3 ? launch2_u<12, true>(p, st) : launch2_u<12, false>(p, st);
+    if (lens) {   // the one-pass class (the decoder's LSTM) only
+        if (p.pass3) return cudaErrorInvalidValue;
+        if (p.U == 8) return launch2_u<8, false, true>(p, lens, st);
+        if (p.U == 12) return launch2_u<12, false, true>(p, lens, st);
+        return cudaErrorInvalidValue;
+    }
+    if (p.U == 8) return p.pass3 ? launch2_u<8, true, false>(p, lens, st) : launch2_u<8, false, false>(p, lens, st);
+    if (p.U == 12) return p.pass3 ? launch2_u<12, true, false>(p, lens, st) : launch2_u<12, false, false>(p, lens, st);
     return cudaErrorInvalidValue;
 }
 

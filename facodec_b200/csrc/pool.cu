@@ -1,5 +1,6 @@
-// Slot <-> lane moves of the stream pools (fac_codes_pool_*, fac_vc_pool_*): each lane of a batch reads or writes its own
-// session's buffer through a pointer table passed as a kernel parameter, so a step needs no host-to-device copy.
+// Slot <-> lane moves of the stream pools (fac_codes_pool_*, fac_vc_pool_*, fac_dec_pool_*): each lane of a batch reads or
+// writes its own session's buffer through a pointer table passed as a kernel parameter, so a step needs no host-to-device
+// copy.  Each lane moves its own word count (a decode pool's lanes end at their own last frame).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -10,14 +11,18 @@ __global__ void lane_copy_kernel(LaneCopyParams p) {
     if (b >= p.n) return;
     const uint32_t* src = p.src[b];
     uint32_t* dst = p.dst[b];
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.words; i += (long long)gridDim.x * blockDim.x)
+    const long long words = p.words[b];
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < words; i += (long long)gridDim.x * blockDim.x)
         dst[i] = src[i];
 }
 
 cudaError_t launch_lane_copy(const LaneCopyParams& p, cudaStream_t st) {
-    if (p.n <= 0 || p.words <= 0) return cudaSuccess;
+    if (p.n <= 0) return cudaSuccess;
     if (p.n > kLaneMax) return cudaErrorInvalidValue;
-    long long blocks = (p.words + 255) / 256;
+    long long most = 0;
+    for (int b = 0; b < p.n; ++b) most = p.words[b] > most ? p.words[b] : most;
+    if (most <= 0) return cudaSuccess;
+    long long blocks = (most + 255) / 256;
     if (blocks > 64) blocks = 64;
     lane_copy_kernel<<<dim3((unsigned)blocks, p.n), 256, 0, st>>>(p);
     return cudaGetLastError();

@@ -251,6 +251,35 @@ __device__ __forceinline__ void code_stage(const VqWeights& W, long long idx, fl
 // FAquantizer from codes per frame: ResidualVectorQuantize.from_codes (dac/nn/quantize.py:200-220, z_q = 0 + sum of the
 // stages in order) for the prosody, content and residual RVQs, outs = LayerNorm((z_p + z_c) + z_r) * gamma + beta
 // (modules/quantize.py:437-449).  n_r = 0 leaves z_r out (z_r = 0, as res_mask = 0 does).  One warp per frame, as above.
+// One frame of it: cp / cc / cr point at the frame's code in row 0 of each code tensor, `row` codes apart; gb is the
+// utterance's gamma | beta.  The parts go to zpo / zco / zro when those are not null.
+__device__ __forceinline__ void dequantize_frame(const VqWeights (&vq)[6], const int64_t* cp, const int64_t* cc, int n_c,
+                                                 const int64_t* cr, int n_r, size_t row, const float* gb, float* outs,
+                                                 float* zpo, float* zco, float* zro, int lane) {
+    float zp[32], zc[32], zr[32], out[32];
+    code_stage(vq[0], cp[0], zp, lane);
+    if (zpo) store_frame(zpo, zp, lane);
+    code_stage(vq[1], cc[0], zc, lane);
+    if (n_c > 1) {
+        code_stage(vq[2], cc[row], out, lane);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) zc[i] += out[i];
+    }
+    if (zco) store_frame(zco, zc, lane);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) zr[i] = 0.f;
+    for (int q = 0; q < n_r; ++q) {
+        code_stage(vq[3 + q], cr[q * row], out, lane);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) zr[i] += out[i];
+    }
+    if (zro) store_frame(zro, zr, lane);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) out[i] = (zp[i] + zc[i]) + zr[i];
+    adaln(out, gb, lane);
+    store_frame(outs, out, lane);
+}
+
 __global__ void __launch_bounds__(128) dequantize_kernel(DeqParams p) {
     const int lane = threadIdx.x & 31;
     const int frame = blockIdx.x * 4 + (threadIdx.x >> 5);
@@ -258,29 +287,33 @@ __global__ void __launch_bounds__(128) dequantize_kernel(DeqParams p) {
     if (frame >= nframes) return;
     const int b = frame / p.T, t = frame - b * p.T;
     const size_t fo = (size_t)frame * VQ_D;
+    dequantize_frame(p.vq, p.codes_p + (size_t)b * p.T + t, p.codes_c + (size_t)b * p.n_c * p.T + t, p.n_c,
+                     p.codes_r + (size_t)b * p.n_r * p.T + t, p.n_r, (size_t)p.T, p.gamma_beta + (size_t)b * 2 * VQ_D,
+                     p.outs + fo, p.zp ? p.zp + fo : nullptr, p.zc ? p.zc + fo : nullptr, p.zr ? p.zr + fo : nullptr, lane);
+}
 
-    float zp[32], zc[32], zr[32], out[32];
-    code_stage(p.vq[0], p.codes_p[(size_t)b * p.T + t], zp, lane);
-    if (p.zp) store_frame(p.zp + fo, zp, lane);
-    code_stage(p.vq[1], p.codes_c[((size_t)b * p.n_c + 0) * p.T + t], zc, lane);
-    if (p.n_c > 1) {
-        code_stage(p.vq[2], p.codes_c[((size_t)b * p.n_c + 1) * p.T + t], out, lane);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) zc[i] += out[i];
+// The same frames for the lanes of a decode-pool batch, each from its own session's codes, rows, length and gamma | beta:
+// lane b's frame t < F[b] is dequantize_kernel's frame t of that session, bit for bit; frames t >= F[b] are zeros.
+__global__ void __launch_bounds__(128) dequantize_lanes_kernel(DeqLaneParams p) {
+    const int lane = threadIdx.x & 31;
+    const int frame = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (frame >= p.n * p.Fmax) return;
+    const int b = frame / p.Fmax, t = frame - b * p.Fmax;
+    float* out = p.outs + (size_t)frame * VQ_D;
+    const int F = p.F[b];
+    if (t >= F) {
+        for (int i = lane; i < VQ_D; i += 32) out[i] = 0.f;
+        return;
     }
-    if (p.zc) store_frame(p.zc + fo, zc, lane);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) zr[i] = 0.f;
-    for (int q = 0; q < p.n_r; ++q) {
-        code_stage(p.vq[3 + q], p.codes_r[((size_t)b * p.n_r + q) * p.T + t], out, lane);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) zr[i] += out[i];
-    }
-    if (p.zr) store_frame(p.zr + fo, zr, lane);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) out[i] = (zp[i] + zc[i]) + zr[i];
-    adaln(out, p.gamma_beta + (size_t)b * 2 * VQ_D, lane);
-    store_frame(p.outs + fo, out, lane);
+    dequantize_frame(p.vq, p.codes_p[b] + t, p.codes_c[b] + t, p.n_c[b], p.codes_r[b] + t, p.n_r[b], (size_t)F,
+                     p.gamma_beta[b], out, nullptr, nullptr, nullptr, lane);
+}
+
+cudaError_t launch_dequantize_lanes(const DeqLaneParams& p, cudaStream_t st) {
+    if (p.n <= 0 || p.Fmax <= 0) return cudaSuccess;
+    if (p.n > 32) return cudaErrorInvalidValue;
+    dequantize_lanes_kernel<<<(unsigned)((p.n * p.Fmax + 3) / 4), 128, 0, st>>>(p);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_dequantize(const DeqParams& p, cudaStream_t st) {

@@ -862,6 +862,77 @@ class VoiceConversionPool(_StreamPool):
         return {s: ys[i][:300 * frames[i]].view(1, 1, 300 * frames[i]) for i, s in enumerate(sessions)}
 
 
+class CodecDecodePool(_StreamPool):
+    """Many live receivers decoding codes back to audio (CodecStream.decode_codes with B = 1 each, every one with its own
+    timbre) stepped in shared launches; each session's audio equals that of its own B = 1 CodecStream fed the same chunks and
+    timbre, bit for bit (fac_dec_pool_*).  Chunk lengths and code rows (1-2 content, 0-3 residual: the bitrate) may change
+    from step to step and differ between sessions that share a batch.  The decoder is causal, so there is no finish step:
+    every frame is final when it arrives."""
+
+    _kind = "dec"
+
+    def __init__(self, model, capacity=256, device=None):
+        engine = model.decoder._engine
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        engine.sync_weights(dev)
+        pid = engine.L.fac_dec_pool_create(engine.handle, int(capacity))
+        _lib.check(engine.handle, pid, "fac_dec_pool_create")
+        self._setup(engine, pid)
+        self.capacity = int(capacity)
+
+    def open(self, timbre):
+        """A new session decoding with ``timbre`` [1,1024]; raises FacError when the pool is full."""
+        if self.pid is None:
+            raise _lib.FacError("pool is closed")
+        self._check_device(timbre)
+        tv = _f32c(timbre)
+        if tuple(tv.shape) != (1, 1024):
+            raise ValueError("timbre must be [1, 1024], got %s" % (tuple(tv.shape),))
+        e = self.engine
+        s = _lib.check(e.handle, e.L.fac_dec_pool_open(e.handle, self.pid, _ptr(tv), _stream(self.device)), "fac_dec_pool_open")
+        self._open.add(s)
+        return s
+
+    def decode_codes(self, chunks):
+        """{session: [codes_p [1,1,F], codes_c [1,1|2,F], codes_r [1,0..3,F] or None]} (F per session; a session's first
+        chunk >= 10 frames) -> {session: y [1,1,300 F]}.  Codes outside [0, 1024) raise IndexError (one device reduction +
+        one host sync for the step); one rejected entry rejects the whole step and leaves every session as it was."""
+        sessions = self._sessions(chunks.keys())
+        cps, ccs, crs, ys = [], [], [], []
+        for s in sessions:
+            codes = chunks[s]
+            if not isinstance(codes, (list, tuple)) or len(codes) != 3 or codes[0] is None or codes[1] is None:
+                raise ValueError("session %d: codes must be [codes_p [1, 1, F], codes_c [1, 1|2, F], codes_r [1, 0..3, F] or None]" % s)
+            for t in codes:
+                if t is not None:
+                    self._check_device(t)
+                    if t.dim() != 3 or t.is_floating_point() or t.is_complex():
+                        raise ValueError("codes must be integer tensors [1, rows, F]; got %s %s" % (t.dtype, tuple(t.shape)))
+            cp, cc, cr = (None if t is None else t.detach().to(torch.int64).contiguous() for t in codes)
+            F = cp.shape[2]
+            if (cp.shape[:2] != (1, 1) or cc.shape[0] != 1 or cc.shape[1] not in (1, 2) or cc.shape[2] != F or F < 1 or
+                    (cr is not None and (cr.shape[0] != 1 or cr.shape[1] > 3 or cr.shape[2] != F))):
+                raise ValueError("session %d: codes must be [codes_p [1, 1, F], codes_c [1, 1|2, F], codes_r [1, 0..3, F]] with "
+                                 "F >= 1; got %s" % (s, [None if t is None else tuple(t.shape) for t in codes]))
+            if cr is not None and cr.shape[1] == 0:
+                cr = None
+            cps.append(cp); ccs.append(cc); crs.append(cr)
+            ys.append(torch.empty(1, 1, 300 * F, device=self.device))
+        present = [t for t in cps + ccs + crs if t is not None]
+        if present and bool(torch.stack([((t < 0) | (t >= 1024)).any() for t in present]).any()):
+            raise IndexError("codes must lie in [0, 1024)")
+        n = len(sessions)
+        P = lambda ts: _ptr_array(ctypes.c_void_p, [0 if t is None else t.data_ptr() for t in ts])
+        e = self.engine
+        rc = e.L.fac_dec_pool_decode_codes(e.handle, self.pid, n, _ptr_array(ctypes.c_int, sessions),
+                                           _ptr_array(ctypes.c_int, [t.shape[2] for t in cps]), P(cps), P(ccs),
+                                           _ptr_array(ctypes.c_int, [t.shape[1] for t in ccs]), P(crs),
+                                           _ptr_array(ctypes.c_int, [0 if t is None else t.shape[1] for t in crs]), P(ys),
+                                           _stream(self.device))
+        _lib.check(e.handle, rc, "fac_dec_pool_decode_codes")
+        return {s: ys[i] for i, s in enumerate(sessions)}
+
+
 class _HeadLinear(nn.Module):
     """A plain nn.Linear(indim, outdim) run through the head machinery (kind "linear" of fac_head_finalize)."""
 

@@ -208,6 +208,14 @@ int fac_stream_end(fac_handle* h, int stream_id);
  * fac_vc_pool_convert: session sessions[i] takes codes_p[i] [1,1,F[i]], codes_c[i] [1,n_c_rows[i],F[i]] (as
  * fac_vc_stream_convert) and writes frames[i] = k output frames to y[i] [1,1,300*k] (capacity 300*F[i] floats).
  * fac_vc_pool_finish: fac_vc_stream_finish per session; y[i] holds 300*44 floats.
+ * fac_dec_pool_create(capacity >= 1) -> pool id; needs the quantizer and the decoder.
+ * fac_dec_pool_open(timbre [1,1024] device) -> session id, a fresh fac_stream_decode_codes stream decoding with that timbre;
+ * gamma | beta = timbre_linear(timbre) is computed once here.
+ * fac_dec_pool_decode_codes: session sessions[i] takes codes_p[i] [1,1,F[i]], codes_c[i] [1,n_c_rows[i],F[i]] and
+ * codes_r[i] [1,n_r_rows[i],F[i]] (1 <= n_c_rows <= 2, 0 <= n_r_rows <= 3, codes_r[i] unread when 0; a session's first chunk
+ * >= 10 frames) and writes y[i] [1,1,300*F[i]].  The decoder is causal, so every frame is final when it arrives (no finish).
+ * Sessions that have decoded equally many frames (20 or more: any two in steady state) share a batch whatever their chunk
+ * lengths and code rows.  Out-of-range codes give NaN samples, as fac_codes_decode.
  * fac_*_pool_close frees a session's slot; fac_*_pool_destroy frees the pool (and runs at fac_destroy). */
 int fac_codes_pool_create(fac_handle* h, int capacity, int n_c);
 int fac_codes_pool_open(fac_handle* h, int pool_id, void* stream);
@@ -225,6 +233,13 @@ int fac_vc_pool_convert(fac_handle* h, int pool_id, int n, const int* sessions, 
 int fac_vc_pool_finish(fac_handle* h, int pool_id, int n, const int* sessions, float* const* y, int* frames, void* stream);
 int fac_vc_pool_close(fac_handle* h, int pool_id, int session);
 int fac_vc_pool_destroy(fac_handle* h, int pool_id);
+int fac_dec_pool_create(fac_handle* h, int capacity);
+int fac_dec_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream);
+int fac_dec_pool_decode_codes(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
+                              const int64_t* const* codes_c, const int* n_c_rows, const int64_t* const* codes_r,
+                              const int* n_r_rows, float* const* y, void* stream);
+int fac_dec_pool_close(fac_handle* h, int pool_id, int session);
+int fac_dec_pool_destroy(fac_handle* h, int pool_id);
 
 /* quantize/rvq.py:27-75 ResidualVQ.forward (eval) over quantize/fvq.py FactorizedVectorQuantize,
  * dim=1024, codebook_dim=8, 2^10 entries (BASELINE configs[3]).  Parameters are passed directly

@@ -68,7 +68,8 @@ int fac_debug_tc_trace(fac_handle* h, long long* out80);
 long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out, long long capacity_floats, int* info3);
 /* Host-only: the launch plan of one stream-pool step.  kind 0 (codes pool): counters[4 i ..] = {samples encoded, x history
  * length, LSTM-output history length, frames emitted} of session i, lengths[i] = its chunk in samples; kind 1 (voice-conversion
- * pool): counters[3 i ..] = {code frames received, z frames final, output frames emitted}, lengths[i] = its chunk in frames.
+ * pool): counters[3 i ..] = {code frames received, z frames final, output frames emitted}, lengths[i] = its chunk in frames;
+ * kind 2 (decode pool): counters[i] = frames decoded by session i, lengths[i] = its chunk in frames.
  * group[i] receives the group of session i (sessions whose launch sequences are identical; groups numbered in order of first
  * appearance), batch[i] its batch (each group cut into batches of <= 32 in input order).  Returns the number of batches. */
 int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch);
@@ -111,6 +112,14 @@ long long fac_debug_convtr_pack(const float* w_host, int Cin, int Cout, int stri
  * Bad chunk lists return FAC_ERR_INVALID.  Both errors are returned before anything is launched. */
 int fac_debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, int upstream,
                     const int* chunks, int n_chunks, float* y, void* stream);
+/* fac_debug_slstm_lanes (synchronous): the same LSTM over all T steps as a stream chunk with per-lane step counts, B <= 32
+ * (the resident-W kernel).  carry (DEVICE [B][2 layers][words], words = fac_debug_lstm_lane_map's count for H and the
+ * class's pass3) holds each row's (h, c) in lane-map order: read as the initial state, overwritten with the final one.
+ * lens (HOST, B entries in [0, T], or NULL for T each): row b steps lens[b] times and its carry is the state after them;
+ * its rows of y past lens[b] are finite but meaningless.  With lens NULL the kernel runs without per-lane counts.  Lengths
+ * run the decoder's one-pass class only (upstream = 0; FAC_ERR_UNSUPPORTED otherwise). */
+int fac_debug_slstm_lanes(fac_handle* h, const float* x, const float* const* w_host, int B, int T, int H, int upstream,
+                          const int* lens, uint32_t* carry, float* y, void* stream);
 /* fa_quantize_kernel + vq_loss_reduce_kernel on caller-given features, the six VectorQuantizes and the AdaLN of
  * FAquantizer.forward_v2 (synchronous).  DEVICE f0 [B][Tf0][1024], z [B][Tz][1024] (Tf0, Tz >= Tq: frame t of
  * utterance b is row b*Tf0 + t / b*Tz + t), gamma_beta [B][2048].  vq_host[i] = HOST {in_w [8][1024], in_b [8],
@@ -130,7 +139,8 @@ int fac_debug_attention(fac_handle* h, const float* q, const float* k, const flo
                         int heads, const int* valid_len, int force_stream, void* stream);
 /* Registers (dst != NULL) or clears a named tap: the next forward copies that channels-last
  * intermediate into dst (DEVICE, up to capacity_floats).  Names: enc_conv0, enc_block1..4,
- * enc_lstm, mel80, f0_input, gamma_beta, dec_conv0, dec_lstm, dec_block1..4.
+ * enc_lstm, mel80, f0_input, gamma_beta, dec_conv0, dec_lstm, dec_block1..4.  dec_pool.latents: the per-lane dequantized
+ * latents [n][Fmax][1024] of a fac_dec_pool_decode_codes batch (each batch overwrites it; frames past a lane's F are 0).
  * Per scale i of fac_reconstruction_loss ("recon.") and fac_spectral_loss ("spec."): recon.dft.<i> / spec.dft.<i> the
  * DFT GEMM output [2*B*F][ld] (rows [0, B*F) of x, then those of the second signal; Re at column 2k, Im at 2k + 1,
  * columns >= 2*nb zero), recon.terms.<i> / spec.terms.<i> the per-frame terms [B*F][2], and recon.fb.<i> / spec.fb.<i>
