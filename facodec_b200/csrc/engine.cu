@@ -6,7 +6,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <initializer_list>
 #include <map>
+#include <memory>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -75,6 +77,72 @@ struct QuantW {
 };
 struct RvqSet { int nq; VqW vq[8]; };
 
+struct DevFree { void operator()(void* p) const { cudaFree(p); } };
+template <typename E> using DevBuf = std::unique_ptr<E, DevFree>;   // owned device memory
+using DevMem = DevBuf<char>;
+
+struct LstmState { uint32_t* h[2] = {nullptr, nullptr}; float* c[2] = {nullptr, nullptr}; };
+
+// Streaming state of one batch of utterances: the encoder and the decoder are causal (README.md:105-107), so a chunk's
+// outputs depend on the past only through (a) a bounded window of earlier samples / frames of every FIR-like conv stack
+// and (b) the LSTM states.  Histories are kept on the device; chunks are computed on [history | chunk] windows with the
+// ordinary kernels and the history part of the output is dropped.  The encoder and decoder halves are independent: a
+// B-row fac_stream_* stream owns one of each; a pool keeps B = 1 views of one kind in its slots and B = 32 in its lanes.
+// The LSTM state is state tiles (a stream, a pool's lanes), or in a pool slot [2 layers][carry_words] in lstm2_lane_map
+// order.  Device pointers are views into memory owned elsewhere (Stream::mem, Pool::mem), except the mel rows.
+struct EncHalf {
+    // Compression to codes (fac_stream_encode_codes / fac_stream_finish_codes).  Mel frame t reads samples up to 300 t + 600,
+    // so the last frame seen is final only at the end of the stream: codes run one frame behind the encoder.
+    enum Mode { kNone, kLatents, kCodes, kFinished };
+    int B = 0;
+    int mode = kNone;                                       // which call feeds the encoder half
+    int n_c = 0;                                            // content codebooks of the codes calls
+    long long samples = 0;                                  // samples encoded
+    long long emitted = 0;                                  // frames of codes written so far
+    float* x_hist = nullptr; int x_hist_len = 0;            // [B][kEncCtx] last samples
+    float* ey_hist = nullptr; int ey_hist_len = 0;          // [B][2][1024] last encoder-LSTM output frames (conv_out, k = 3)
+    float* z_held = nullptr;                                // [B][1024] latent frame `emitted`, quantized by the next call
+    LstmState lstm; uint32_t* carry = nullptr;
+    DevBuf<float> mel; int mel_cap = 0;                     // [B][mel_cap][80] every mel80 row so far: the timbre pools them all
+    long long mel_base = 0;                                 // frame of mel row 0 (a pool's batch holds only the prosody window)
+};
+struct DecHalf {
+    int B = 0;
+    long long frames = 0;                                   // frames decoded
+    float* z_hist = nullptr;                                // [B][6][1024] last latent frames (decoder conv0, k = 7)
+    float* dy_hist = nullptr;                               // [B][kDecCtx][1536] last decoder-LSTM output frames
+    LstmState lstm; uint32_t* carry = nullptr;
+    float* gb = nullptr;                                    // a decode-pool slot's timbre_linear(timbre), [2048]
+};
+struct Stream { EncHalf enc; DecHalf dec; DevMem mem; };
+
+// Streaming voice conversion: the redecoder and its decoder are non-causal but carry no LSTM, so a chunk's outputs depend
+// only on bounded windows of codes and latents on both sides (kVcRedCtx / kVcDecCtx frames, fac_vc_stream_lookahead).
+// Frames [0, Zf) of z and [0, Yf) of the output are final; the device keeps the codes [max(0, Zf - kVcRedCtx), N) and the
+// channels-last z [max(0, Yf - kVcDecCtx), Zf) those windows still need.
+struct VcStream {
+    int B = 0, use_p = 0, use_c = 0, n_c = 0;
+    bool finished = false;
+    long long N = 0, Zf = 0, Yf = 0;        // code frames received, z frames final, output frames emitted
+    float* g = nullptr;                     // [B][2 * 512 * 16] cond_layer(timbre), computed once at begin
+    int64_t* codes = nullptr;               // [B][3][kVcCodesHist]: row 0 prosody, rows 1..2 content
+    float* z = nullptr;                     // [B][kVcZHist][1024]
+    DevMem mem;                             // a fac_vc_stream_* stream's own state (null in a pool)
+};
+
+// A stream pool: `cap` slots of session state, each a B = 1 view, and the B = 32 lanes a batch runs in.
+template <typename S>
+struct Pool {
+    int cap = 0;
+    std::vector<S> slot;
+    std::vector<char> used;
+    S lanes;                                // a codes pool's n_c, a vc pool's options: those of the lanes and every slot
+    DevMem mem;
+};
+using CodesPool = Pool<EncHalf>;
+using VcPool = Pool<VcStream>;
+using DecPool = Pool<DecHalf>;
+
 }  // namespace
 
 struct fac_handle {
@@ -88,16 +156,12 @@ struct fac_handle {
     EncW enc; DecW dec; QuantW qw;
     RedW red; DecW dec2;            // voice-conversion model: Redecoder + its non-causal, LSTM-free decoder
     std::vector<RvqSet> rvqs; std::vector<float*> rvq_arenas;
-    struct Stream;                  // chunked (streaming) encoder / decoder state (fac_stream_*)
-    std::vector<Stream*> streams;
-    struct VcStream;                // chunked voice conversion through the redecoder (fac_vc_stream_*)
-    std::vector<VcStream*> vc_streams;
-    struct CodesPool;               // many B = 1 compression streams stepped in shared batches (fac_codes_pool_*)
-    std::vector<CodesPool*> codes_pools;
-    struct VcPool;                  // many B = 1 voice-conversion streams stepped in shared batches (fac_vc_pool_*)
-    std::vector<VcPool*> vc_pools;
-    struct DecPool;                 // many B = 1 decode-from-codes streams stepped in shared batches (fac_dec_pool_*)
-    std::vector<DecPool*> dec_pools;
+    // streams and pools by id; an ended stream or a destroyed pool leaves a null entry, so ids are never reused
+    std::vector<std::unique_ptr<Stream>> streams;           // chunked encoder / decoder (fac_stream_*)
+    std::vector<std::unique_ptr<VcStream>> vc_streams;      // chunked voice conversion through the redecoder (fac_vc_stream_*)
+    std::vector<std::unique_ptr<CodesPool>> codes_pools;    // many B = 1 compression streams (fac_codes_pool_*)
+    std::vector<std::unique_ptr<VcPool>> vc_pools;          // many B = 1 voice-conversion streams (fac_vc_pool_*)
+    std::vector<std::unique_ptr<DecPool>> dec_pools;        // many B = 1 decode-from-codes streams (fac_dec_pool_*)
     struct HeadSet;                 // modules/quantize.py:106-125 CNNLSTM instances (fac_head_*)
     std::vector<HeadSet*> heads;
     char* ws = nullptr; size_t ws_bytes = 0;
@@ -136,46 +200,6 @@ struct fac_handle {
     std::map<std::string, ProfAgg> prof_agg;
     // debug taps: named intermediates copied out during a forward (fac_debug_tap)
     std::map<std::string, std::pair<float*, size_t>> taps;
-};
-
-// Streaming state of one batch of utterances: the encoder and the decoder are causal (README.md:105-107), so a chunk's
-// outputs depend on the past only through (a) a bounded window of earlier samples / frames of every FIR-like conv stack
-// and (b) the LSTM states.  Histories are kept on the device; chunks are computed on [history | chunk] windows with the
-// ordinary kernels and the history part of the output is dropped.
-struct fac_handle::Stream {
-    int B = 0;
-    bool alive = false;
-    long long enc_samples = 0, dec_frames = 0;
-    float* x_hist = nullptr; int x_hist_len = 0;            // [B][kEncCtx] last samples
-    float* ey_hist = nullptr; int ey_hist_len = 0;          // [B][2][1024] last encoder-LSTM output frames (conv_out, k = 3)
-    float* z_hist = nullptr; int z_hist_len = 0;            // [B][6][1024] last latent frames (decoder conv0, k = 7)
-    float* dy_hist = nullptr; int dy_hist_len = 0;          // [B][kDecCtx][1536] last decoder-LSTM output frames
-    uint32_t* enc_h[2] = {nullptr, nullptr}; float* enc_c[2] = {nullptr, nullptr};
-    uint32_t* dec_h[2] = {nullptr, nullptr}; float* dec_c[2] = {nullptr, nullptr};
-    // Compression to codes (fac_stream_encode_codes / fac_stream_finish_codes).  Mel frame t reads samples up to 300 t + 600,
-    // so the last frame seen is final only at the end of the stream: codes run one frame behind the encoder.
-    enum EncMode { kEncNone, kEncLatents, kEncCodes, kEncFinished };
-    int enc_mode = kEncNone;                                // which call feeds the encoder half
-    int n_c = 0;                                            // content codebooks of the codes calls
-    long long emitted = 0;                                  // frames of codes written so far
-    float* z_held = nullptr;                                // [B][1024] latent frame `emitted`, quantized by the next call
-    float* mel = nullptr; int mel_cap = 0;                  // [B][mel_cap][80] every mel80 row so far: the timbre pools them all
-    long long mel_base = 0;                                 // frame of mel row 0 (a pool's batch holds only the prosody window)
-    void* all[13] = {nullptr};
-};
-
-// Streaming voice conversion: the redecoder and its decoder are non-causal but carry no LSTM, so a chunk's outputs depend
-// only on bounded windows of codes and latents on both sides (kVcRedCtx / kVcDecCtx frames, fac_vc_stream_lookahead).
-// Frames [0, Zf) of z and [0, Yf) of the output are final; the device keeps the codes [max(0, Zf - kVcRedCtx), N) and the
-// channels-last z [max(0, Yf - kVcDecCtx), Zf) those windows still need.
-struct fac_handle::VcStream {
-    int B = 0, use_p = 0, use_c = 0, n_c = 0;
-    bool alive = false, finished = false;
-    long long N = 0, Zf = 0, Yf = 0;        // code frames received, z frames final, output frames emitted
-    float* g = nullptr;                     // [B][2 * 512 * 16] cond_layer(timbre), computed once at begin
-    int64_t* codes = nullptr;               // [B][3][kVcCodesHist]: row 0 prosody, rows 1..2 content
-    float* z = nullptr;                     // [B][kVcZHist][1024]
-    void* all[3] = {nullptr, nullptr, nullptr};
 };
 
 // One CNNLSTM predictor head (modules/quantize.py:106-125): 3 ResidualUnits (alias-free SnakeBeta, k7 conv dilation
@@ -832,8 +856,6 @@ void residual_unit(Ctx& c, const ResW& r, const float* x, float* tmp, float* y, 
 }
 
 // Carried state of one 2-layer SLSTM (streaming): h in the kernel's published fp16 layout, c per CTA.
-struct LstmState { uint32_t* h[2] = {nullptr, nullptr}; float* c[2] = {nullptr, nullptr}; };
-
 // Precision class of slstm's recurrence: 3-pass fp32-faithful upstream of the VQ (and when "decoder_bf16" is off), one fp16
 // pass downstream.
 int lstm_pass3(const Ctx& c) { return (c.vq_critical || !c.h->dec_bf16) ? 1 : 0; }
@@ -1386,6 +1408,7 @@ int fac_create(fac_handle** out, int device) {
 int fac_destroy(fac_handle* h) {
     if (!h) return FAC_OK;
     cudaSetDevice(h->device);
+    cudaDeviceSynchronize();
     if (h->warena) cudaFree(h->warena);
     if (h->ws) cudaFree(h->ws);
     if (h->side) cudaStreamDestroy(h->side);
@@ -1397,12 +1420,7 @@ int fac_destroy(fac_handle* h) {
     if (h->spec_arena) cudaFree(h->spec_arena);
     for (float* p : h->rvq_arenas) if (p) cudaFree(p);
     for (auto* hs : h->heads) { if (hs->arena) cudaFree(hs->arena); delete hs; }
-    for (auto* ss : h->streams) { for (void* p : ss->all) if (p) cudaFree(p); if (ss->mel) cudaFree(ss->mel); delete ss; }
-    for (auto* vs : h->vc_streams) { for (void* p : vs->all) if (p) cudaFree(p); delete vs; }
-    for (int i = 0; i < (int)h->codes_pools.size(); ++i) fac_codes_pool_destroy(h, i);
-    for (int i = 0; i < (int)h->vc_pools.size(); ++i) fac_vc_pool_destroy(h, i);
-    for (int i = 0; i < (int)h->dec_pools.size(); ++i) fac_dec_pool_destroy(h, i);
-    delete h;
+    delete h;   // and with it the streams' and pools' device state
     return FAC_OK;
 }
 
@@ -1454,21 +1472,22 @@ int fac_encode_frames(int T) {
     return t;
 }
 
-static int check_ready(fac_handle* h, int m) {
+static int check_ready(fac_handle* h, std::initializer_list<int> modules) {
     if (!h) return FAC_ERR_INVALID;
-    if (!h->finalized || !h->have[m]) { h->err = "module weights not loaded/finalized"; return FAC_ERR_STATE; }
+    for (int m : modules)
+        if (!h->finalized || !h->have[m]) { h->err = "module weights not loaded/finalized"; return FAC_ERR_STATE; }
     return FAC_OK;
 }
 
 int fac_encode(fac_handle* h, const float* x, int B, int T, float* z, void* stream) {
-    int rc = check_ready(h, FAC_ENCODER);
+    int rc = check_ready(h, {FAC_ENCODER});
     if (rc) return rc;
     if (!x || !z || B <= 0 || T <= 0) { h->err = "fac_encode: bad arguments"; return FAC_ERR_INVALID; }
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { encoder_forward(c, x, B, T, z, true); });
 }
 
 int fac_decode(fac_handle* h, const float* z, int B, int Tf, float* y, void* stream) {
-    int rc = check_ready(h, FAC_DECODER);
+    int rc = check_ready(h, {FAC_DECODER});
     if (rc) return rc;
     if (!z || !y || B <= 0 || Tf <= 0) { h->err = "fac_decode: bad arguments"; return FAC_ERR_INVALID; }
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
@@ -1482,7 +1501,7 @@ int fac_quantize(fac_handle* h, const float* z, const float* wave, int B, int T,
                  const float* full_waves, int T_full, const int64_t* wave_lens, float* outs, float* zp, float* zc,
                  float* zr, float* losses2, float* timbre, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r,
                  void* stream) {
-    int rc = check_ready(h, FAC_QUANTIZER);
+    int rc = check_ready(h, {FAC_QUANTIZER});
     if (rc) return rc;
     if (!z || !wave || !outs || B <= 0 || Tz <= 0 || n_c < 1 || n_c > 2) { h->err = "fac_quantize: bad arguments"; return FAC_ERR_INVALID; }
     if (T <= N_FFT / 2 || (full_waves && (T_full <= N_FFT / 2 || !wave_lens))) {
@@ -1533,7 +1552,7 @@ extern "C" {
 
 int fac_codec_forward(fac_handle* h, const float* x, int B, int T, int n_c, float* y, int64_t* codes_p,
                       int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream) {
-    for (int m = 0; m < 3; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    if (int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER, FAC_DECODER})) return rc;
     if (!x || !y || B <= 0 || T <= N_FFT / 2 || n_c < 1 || n_c > 2) { h->err = "fac_codec_forward: bad arguments"; return FAC_ERR_INVALID; }
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
         QuantOut o = codec_encode(c, x, B, T, n_c, codes_p, codes_c, codes_r, timbre);
@@ -1543,7 +1562,7 @@ int fac_codec_forward(fac_handle* h, const float* x, int B, int T, int n_c, floa
 
 int fac_codec_encode(fac_handle* h, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
                      int64_t* codes_r, float* timbre, void* stream) {
-    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    if (int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER})) return rc;
     if (!x || !codes_p || !codes_c || !codes_r || B <= 0 || T <= N_FFT / 2 || n_c < 1 || n_c > 2) {
         h->err = "fac_codec_encode: bad arguments";
         return FAC_ERR_INVALID;
@@ -1553,7 +1572,7 @@ int fac_codec_encode(fac_handle* h, const float* x, int B, int T, int n_c, int64
 
 int fac_dequantize(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
                    int n_r_rows, const float* timbre, int B, int T, float* outs, float* zp, float* zc, float* zr, void* stream) {
-    int rc = check_ready(h, FAC_QUANTIZER);
+    int rc = check_ready(h, {FAC_QUANTIZER});
     if (rc) return rc;
     if (!outs || bad_codes_args(codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T)) {
         h->err = "fac_dequantize: bad arguments (1 <= content rows <= 2, 0 <= residual rows <= 3)";
@@ -1571,8 +1590,7 @@ int fac_dequantize(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c
 
 int fac_codes_decode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
                      int n_r_rows, const float* timbre, int B, int T, float* y, void* stream) {
-    int rc = check_ready(h, FAC_QUANTIZER);
-    if (!rc) rc = check_ready(h, FAC_DECODER);
+    int rc = check_ready(h, {FAC_QUANTIZER, FAC_DECODER});
     if (rc) return rc;
     if (!y || bad_codes_args(codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T)) {
         h->err = "fac_codes_decode: bad arguments (1 <= content rows <= 2, 0 <= residual rows <= 3)";
@@ -1586,7 +1604,7 @@ int fac_codes_decode(fac_handle* h, const int64_t* codes_p, const int64_t* codes
 
 int fac_codec_forward_host(fac_handle* h, const float* x_host, int B, int T, int n_c, float* y_host,
                            int64_t* codes_p_host, int64_t* codes_c_host, int64_t* codes_r_host, void* stream) {
-    for (int m = 0; m < 3; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    if (int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER, FAC_DECODER})) return rc;
     if (!x_host || !y_host || B <= 0 || T <= N_FFT / 2 || n_c < 1 || n_c > 2) { h->err = "fac_codec_forward_host: bad arguments"; return FAC_ERR_INVALID; }
     cudaStream_t st = (cudaStream_t)stream;
     int Tq = 0;
@@ -1623,7 +1641,7 @@ int fac_codec_forward_host(fac_handle* h, const float* x_host, int B, int T, int
 
 int fac_redecode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre, int B, int T,
                  int use_p_code, int use_c_code, int n_c, float* z, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER);
+    int rc = check_ready(h, {FAC_REDECODER});
     if (rc) return rc;
     if (!codes_p || !codes_c || !timbre || !z || B <= 0 || T <= 0 || n_c < 0 || n_c > 2 || n_c > n_c_rows) {
         h->err = "fac_redecode: bad arguments (n_c <= rows of codes_c <= 2)";
@@ -1636,7 +1654,7 @@ int fac_redecode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, 
 }
 
 int fac_redecoder_decode(fac_handle* h, const float* z, int B, int Tf, float* y, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER_DECODER});
     if (rc) return rc;
     if (!z || !y || B <= 0 || Tf <= 0) { h->err = "fac_redecoder_decode: bad arguments"; return FAC_ERR_INVALID; }
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
@@ -1648,8 +1666,7 @@ int fac_redecoder_decode(fac_handle* h, const float* z, int B, int Tf, float* y,
 
 int fac_voice_convert(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre, int B,
                       int T, int use_p_code, int use_c_code, int n_c, float* y, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER);
-    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
     if (!codes_p || !codes_c || !timbre || !y || B <= 0 || T <= 0 || n_c < 0 || n_c > 2 || n_c > n_c_rows) {
         h->err = "fac_voice_convert: bad arguments";
@@ -1670,37 +1687,85 @@ constexpr int kWnCtx = 32;   // mel frames of prosody-net history a codes window
 }  // extern "C"
 
 namespace {
-// Device state of a B-row stream (zeroed), or null with h->err set.
-fac_handle::Stream* alloc_stream(fac_handle* h, int B, const char* who) {
-    cudaSetDevice(h->device);
-    auto* s = new fac_handle::Stream();
-    s->B = B;
-    // LSTM states: the encoder's LSTM (H = 1024) runs the 3-pass recurrence, the decoder's (H = 1536) one fp16 pass
-    size_t enc_hw, enc_cf, dec_hw, dec_cf;
-    lstm2_state_sizes(LATENT, lstm_units_per_cta(LATENT), 1, &enc_hw, &enc_cf);
-    lstm2_state_sizes(1536, lstm_units_per_cta(1536), 0, &dec_hw, &dec_cf);
-    const size_t sizes[13] = {
-        sizeof(float) * (size_t)B * kEncCtx, sizeof(float) * (size_t)B * 2 * LATENT, sizeof(float) * (size_t)B * 6 * LATENT,
-        sizeof(float) * (size_t)B * kDecCtx * 1536,
-        sizeof(uint32_t) * enc_hw, sizeof(uint32_t) * enc_hw, sizeof(float) * enc_cf, sizeof(float) * enc_cf,
-        sizeof(uint32_t) * dec_hw, sizeof(uint32_t) * dec_hw, sizeof(float) * dec_cf, sizeof(float) * dec_cf,
-        sizeof(float) * (size_t)B * LATENT};
-    for (int i = 0; i < 13; ++i) {
-        cudaError_t e = cudaMalloc(&s->all[i], sizes[i]);
-        if (e == cudaSuccess) e = cudaMemset(s->all[i], 0, sizes[i]);
-        if (e != cudaSuccess) {
-            h->err = std::string(who) + ": " + cudaGetErrorString(e);
-            cudaGetLastError();
-            for (void* p : s->all) if (p) cudaFree(p);
-            delete s;
-            return nullptr;
-        }
+// Zeroed device memory laid out by `layout(Carve&)`, which runs twice: to size the block, then to hand out its pieces.
+struct Carve {
+    char* base = nullptr;
+    size_t off = 0;
+    template <typename E>
+    E* take(size_t n) {
+        E* p = base ? reinterpret_cast<E*>(base + off) : nullptr;
+        off += (n * sizeof(E) + 255) / 256 * 256;
+        return p;
     }
-    s->x_hist = (float*)s->all[0]; s->ey_hist = (float*)s->all[1]; s->z_hist = (float*)s->all[2]; s->dy_hist = (float*)s->all[3];
-    s->enc_h[0] = (uint32_t*)s->all[4]; s->enc_h[1] = (uint32_t*)s->all[5]; s->enc_c[0] = (float*)s->all[6]; s->enc_c[1] = (float*)s->all[7];
-    s->dec_h[0] = (uint32_t*)s->all[8]; s->dec_h[1] = (uint32_t*)s->all[9]; s->dec_c[0] = (float*)s->all[10]; s->dec_c[1] = (float*)s->all[11];
-    s->z_held = (float*)s->all[12];
-    return s;
+};
+
+template <typename F>
+int dev_block(fac_handle* h, DevMem& mem, const char* who, F layout) {
+    Carve size;
+    layout(size);
+    char* p = nullptr;
+    cudaError_t e = cudaSetDevice(h->device);
+    if (e == cudaSuccess) e = cudaMalloc(&p, size.off);
+    mem.reset(p);
+    if (e == cudaSuccess) e = cudaMemset(p, 0, size.off);
+    if (e != cudaSuccess) {
+        h->err = std::string(who) + ": " + cudaGetErrorString(e);
+        cudaGetLastError();
+        mem.reset();
+        return FAC_ERR_CUDA;
+    }
+    Carve at{p};
+    layout(at);
+    return FAC_OK;
+}
+
+// One LSTM layer of one lane in lstm2_lane_map order: hi | lo h planes (pass3) or one fp16 h plane, then c.
+constexpr int carry_words(int H, int pass3) { return (pass3 ? 2 : 1) * (H / 2) + H; }
+
+// The LSTM state tiles of a stream or a pool's lanes: the encoder's LSTM (H = 1024) runs the 3-pass recurrence, the
+// decoder's (H = 1536) one fp16 pass.
+void take_lstm(Carve& m, LstmState& st, int H, int pass3) {
+    size_t hw, cf;
+    lstm2_state_sizes(H, lstm_units_per_cta(H), pass3, &hw, &cf);
+    for (int l = 0; l < 2; ++l) { st.h[l] = m.take<uint32_t>(hw); st.c[l] = m.take<float>(cf); }
+}
+
+// B rows of encoder-half state; a pool slot (B = 1) keeps its LSTM carry in lane-map order instead of state tiles.
+void take_enc(Carve& m, EncHalf& s, int B, bool slot) {
+    s.B = B;
+    s.x_hist = m.take<float>((size_t)B * kEncCtx);
+    s.ey_hist = m.take<float>((size_t)B * 2 * LATENT);
+    s.z_held = m.take<float>((size_t)B * LATENT);
+    if (slot) s.carry = m.take<uint32_t>(2 * carry_words(LATENT, 1));
+    else take_lstm(m, s.lstm, LATENT, 1);
+}
+
+// ... of decoder-half state; a decode-pool slot also holds its session's gamma | beta.
+void take_dec(Carve& m, DecHalf& s, int B, bool slot) {
+    s.B = B;
+    s.z_hist = m.take<float>((size_t)B * 6 * LATENT);
+    s.dy_hist = m.take<float>((size_t)B * kDecCtx * 1536);
+    if (slot) { s.carry = m.take<uint32_t>(2 * carry_words(1536, 0)); s.gb = m.take<float>(2048); }
+    else take_lstm(m, s.lstm, 1536, 0);
+}
+
+// The handle's streams and pools of one kind, by id.
+template <typename T>
+using List = std::vector<std::unique_ptr<T>> fac_handle::*;
+
+template <typename T>
+T* by_id(fac_handle* h, List<T> list, int id) {
+    return h && id >= 0 && id < (int)(h->*list).size() ? (h->*list)[id].get() : nullptr;
+}
+
+// Frees live entry `id` once the device is idle; its id stays unused.
+template <typename T>
+int free_by_id(fac_handle* h, List<T> list, int id) {
+    if (!by_id(h, list, id)) return FAC_ERR_INVALID;
+    cudaSetDevice(h->device);
+    cudaDeviceSynchronize();
+    (h->*list)[id].reset();
+    return FAC_OK;
 }
 }  // namespace
 
@@ -1709,25 +1774,16 @@ extern "C" {
 int fac_stream_begin(fac_handle* h, int B) {
     if (!h || B < 1 || B > 32) { if (h) h->err = "fac_stream_begin: 1 <= B <= 32"; return FAC_ERR_INVALID; }
     if (!h->finalized) { h->err = "module weights not loaded/finalized"; return FAC_ERR_STATE; }
-    auto* s = alloc_stream(h, B, "fac_stream_begin");
-    if (!s) return FAC_ERR_CUDA;
-    s->alive = true;
-    h->streams.push_back(s);
+    auto s = std::make_unique<Stream>();
+    int rc = dev_block(h, s->mem, "fac_stream_begin", [&](Carve& m) { take_enc(m, s->enc, B, false); take_dec(m, s->dec, B, false); });
+    if (rc) return rc;
+    h->streams.push_back(std::move(s));
     return (int)h->streams.size() - 1;
 }
 
 int fac_stream_end(fac_handle* h, int stream_id) {
     if (!h || stream_id < 0 || stream_id >= (int)h->streams.size()) return FAC_ERR_INVALID;
-    fac_handle::Stream* s = h->streams[stream_id];
-    if (s->alive) {
-        cudaSetDevice(h->device);
-        cudaDeviceSynchronize();
-        for (void*& p : s->all) { if (p) cudaFree(p); p = nullptr; }
-        if (s->mel) cudaFree(s->mel);
-        s->mel = nullptr; s->mel_cap = 0;
-        s->alive = false;
-    }
-    return FAC_OK;
+    return h->streams[stream_id] ? free_by_id(h, &fac_handle::streams, stream_id) : FAC_OK;
 }
 
 }  // extern "C"
@@ -1742,97 +1798,134 @@ void copy_rows(Ctx& c, E* dst, int dst_pitch_rows, const E* src, int src_pitch_r
                                  sizeof(E) * (size_t)src_pitch_rows * w, sizeof(E) * (size_t)n_rows * w, B,
                                  cudaMemcpyDeviceToDevice, c.st), what);
 }
-}  // namespace
 
-namespace {
-bool stream_alive(const fac_handle* h, int stream_id) {
-    return stream_id >= 0 && stream_id < (int)h->streams.size() && h->streams[stream_id]->alive;
+// Inside a launch sequence: lane b of n copies `words` (a count, or a function of b) 32-bit words from src(b) to dst(b)
+// (launch_lane_copy).
+template <typename W, typename S, typename D>
+void lane_copy(Ctx& c, int n, W words, S src, D dst, const char* what) {
+    if (c.dry) return;
+    LaneCopyParams p;
+    p.n = n;
+    for (int b = 0; b < n; ++b) {
+        p.src[b] = (const uint32_t*)src(b); p.dst[b] = (uint32_t*)dst(b);
+        if constexpr (std::is_invocable_v<W, int>) p.words[b] = words(b);
+        else p.words[b] = words;
+    }
+    c.check(launch_lane_copy(p, c.st), what);
 }
 
-// The chunk rules and the encoder-half state of fac_stream_encode (mode kEncLatents) / fac_stream_encode_codes (kEncCodes).
-int stream_encode_check(fac_handle* h, const fac_handle::Stream& s, int T, int mode, const char* who) {
-    using S = fac_handle::Stream;
-    if (T <= 0 || T % HOP != 0 || (s.enc_samples == 0 && T < kStreamMinFirst * HOP)) {
+// Inside a launch sequence: moves the 2-layer LSTM carries (H, pass3) of lanes [0, n) between the state tiles `st` and
+// per-lane carries carry(b) ([2 layers][carry_words]; to_lanes = 1: carry -> lane, 0: lane -> carry).
+template <typename P>
+void lane_carry(Ctx& c, const LstmState& st, int H, int pass3, int n, P carry, int to_lanes) {
+    if (c.dry) return;
+    for (int l = 0; l < 2; ++l) {
+        LaneCarryParams p;
+        p.n = n; p.H = H; p.U = lstm_units_per_cta(H); p.pass3 = pass3; p.to_lanes = to_lanes;
+        p.state_h = st.h[l]; p.state_c = st.c[l];
+        for (int b = 0; b < n; ++b) p.slot[b] = carry(b) + (size_t)l * carry_words(H, pass3);
+        c.check(launch_lstm2_lane_carry(p, c.st), "pool.carry");
+    }
+}
+
+// The chunk rules and the encoder-half state of fac_stream_encode (mode kLatents) / fac_stream_encode_codes (kCodes).
+int stream_encode_check(fac_handle* h, const EncHalf& s, int T, int mode, const char* who) {
+    if (T <= 0 || T % HOP != 0 || (s.samples == 0 && T < kStreamMinFirst * HOP)) {
         h->err = std::string(who) + ": chunks must be multiples of 300 samples, the first one at least 3000";
         return FAC_ERR_INVALID;
     }
-    if (s.enc_mode == S::kEncFinished) {
+    if (s.mode == EncHalf::kFinished) {
         h->err = std::string(who) + ": the stream's encoder was closed by fac_stream_finish_codes";
         return FAC_ERR_STATE;
     }
-    if (s.enc_mode != S::kEncNone && s.enc_mode != mode) {
-        h->err = std::string(who) + (mode == S::kEncCodes ? ": the stream is already fed by fac_stream_encode (latents)"
-                                                           : ": the stream is already fed by fac_stream_encode_codes");
+    if (s.mode != EncHalf::kNone && s.mode != mode) {
+        h->err = std::string(who) + (mode == EncHalf::kCodes ? ": the stream is already fed by fac_stream_encode (latents)"
+                                                             : ": the stream is already fed by fac_stream_encode_codes");
         return FAC_ERR_STATE;
     }
     if (!h->lstm_v2 || !h->enc.lstm.has2[1]) { h->err = std::string(who) + ": needs the resident-W LSTM kernel"; return FAC_ERR_UNSUPPORTED; }
     return FAC_OK;
 }
 
-// What the encoder half of a chunk yields: the [x_hist | chunk] window xw [B][Tw] (global samples [enc_samples - hist,
-// enc_samples + T)) and the chunk's channels-last latents znew [B][T/300][1024], both in workspace.
-struct EncChunk { const float* xw; int Tw, hist; const float* znew; };
+// Every integer the launch sequence of an encoder-half chunk depends on, for a half at (samples, hist, yh, emitted = E) fed T
+// samples, and the histories it leaves.  Codes of frames [E, E + Fout) are final: frame N - 1 reads 300 samples past what
+// has arrived (reflected only at the true end).  Halves with equal keys share one pool batch.
+struct EncPlan {
+    int T, hist, yh;            // chunk, sample history, encoder-LSTM output history
+    int first, f_first, Fout;   // first chunk; frame E within the [x_hist | chunk] window; frames of codes
+    int win, Fw;                // the prosody window [lo, E + Fout): E - lo and its length
+    long long lo;
+    int hist1, yh1;             // the histories after the chunk
+    std::vector<long long> key() const { return {T, hist, yh, first, f_first, Fout, win, Fw}; }
+};
 
-// The body of fac_stream_encode / fac_stream_encode_codes (checked by stream_encode_check): advances the encoder state by one
-// chunk and hands the chunk to `tail(c, chunk)` inside the same launch sequence.
-template <typename F>
-int stream_encode(fac_handle* h, fac_handle::Stream& s, const float* x, int T, void* stream, int mode, F tail) {
-    const int B = s.B, hist = s.x_hist_len, Tw = hist + T, Fc = T / HOP, Fh = hist / HOP;
-    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-        const EncW& e = h->enc;
-        c.vq_critical = true;
-        float* xw = c.alloc<float>((size_t)B * Tw);
-        copy_rows(c, xw, Tw, s.x_hist, kEncCtx, 0, hist, 1, B, "stream.xh");
-        copy_rows(c, xw + hist, Tw, x, T, 0, T, 1, B, "stream.xc");
-        int Fw = 0;
-        float* feats = encoder_front(c, xw, B, Tw, &Fw);                    // [B][Fw][1024], Fw == Fh + Fc
-        float* fnew = c.alloc<float>((size_t)B * Fc * LATENT);
-        copy_rows(c, fnew, Fc, feats, Fw, Fh, Fc, LATENT, B, "stream.fnew");
-        const int yh = s.ey_hist_len;
-        float* yw = c.alloc<float>((size_t)B * (yh + Fc) * LATENT);        // [hist | new] LSTM outputs
-        float* ynew = c.alloc<float>((size_t)B * Fc * LATENT);
-        LstmState st;
-        st.h[0] = s.enc_h[0]; st.h[1] = s.enc_h[1]; st.c[0] = s.enc_c[0]; st.c[1] = s.enc_c[1];
-        slstm(c, e.lstm, fnew, ynew, B, Fc, &st);
-        copy_rows(c, yw, yh + Fc, s.ey_hist, 2, 0, yh, LATENT, B, "stream.yh");
-        copy_rows(c, yw + (size_t)yh * LATENT, yh + Fc, ynew, Fc, 0, Fc, LATENT, B, "stream.yc");
-        float* zw = c.alloc<float>((size_t)B * (yh + Fc) * LATENT);
-        float* znew = c.alloc<float>((size_t)B * Fc * LATENT);
-        ConvOpts o;
-        o.in_snake = &e.snake;
-        sconv(c, e.conv_out, yw, zw, B, yh + Fc, 1, 1, o, "enc.conv_out");
-        copy_rows(c, znew, Fc, zw, yh + Fc, yh, Fc, LATENT, B, "stream.znew");
-        tail(c, EncChunk{xw, Tw, hist, znew});
-        // new histories: the last kEncCtx samples / 2 LSTM-output frames of what has been seen so far
-        const int nh = Tw < kEncCtx ? Tw : kEncCtx, nyh = yh + Fc < 2 ? yh + Fc : 2;
-        float* tmpx = c.alloc<float>((size_t)B * kEncCtx);
-        copy_rows(c, tmpx, kEncCtx, xw, Tw, Tw - nh, nh, 1, B, "stream.xh2");
-        copy_rows(c, s.x_hist, kEncCtx, tmpx, kEncCtx, 0, nh, 1, B, "stream.xh3");
-        copy_rows(c, s.ey_hist, 2, yw, yh + Fc, yh + Fc - nyh, nyh, LATENT, B, "stream.yh2");
-        c.vq_critical = false;
-    });
-    if (rc == FAC_OK) {
-        s.x_hist_len = Tw < kEncCtx ? Tw : kEncCtx;
-        s.ey_hist_len = s.ey_hist_len + Fc < 2 ? s.ey_hist_len + Fc : 2;
-        s.enc_samples += T;
-        s.enc_mode = mode;
-    }
-    return rc;
+EncPlan enc_plan(long long samples, int hist, int yh, long long E, int T) {
+    const long long N = (samples + T) / HOP, lo = E > kWnCtx ? E - kWnCtx : 0;
+    EncPlan p;
+    p.T = T; p.hist = hist; p.yh = yh;
+    p.first = samples == 0; p.f_first = (int)(E - (samples - hist) / HOP); p.Fout = (int)(N - 1 - E);
+    p.win = (int)(E - lo); p.Fw = p.win + p.Fout; p.lo = lo;
+    p.hist1 = std::min(hist + T, kEncCtx); p.yh1 = std::min(yh + T / HOP, 2);
+    return p;
+}
+EncPlan enc_plan(const EncHalf& s, int T) { return enc_plan(s.samples, s.x_hist_len, s.ey_hist_len, s.emitted, T); }
+
+// The counters of s after chunk p fed in `mode` (kLatents or kCodes).
+void enc_commit(EncHalf& s, const EncPlan& p, int mode) {
+    s.samples += p.T; s.x_hist_len = p.hist1; s.ey_hist_len = p.yh1; s.mode = mode;
+    if (mode == EncHalf::kCodes) s.emitted += p.Fout;
 }
 
-// Codes of frames [E, E + Fq) (the kCodesOnly VQ kernel): the prosody net recomputed over the stream's mel rows
-// [max(0, E - 32), E + Fq) -- each of the WN's 8 causal k = 5 convs reflect-pads 4 frames at the window's left edge, so the
-// first 32 frames of a window are not those of the whole utterance unless the window starts at frame 0 -- and the latents
-// zq [B][Fq][1024] (row pitch zpitch frames).  Runs with c.vq_critical set, as the offline quantizer.
-void stream_codes(Ctx& c, const fac_handle::Stream& s, long long E, int Fq, const float* zq, int zpitch, int64_t* codes_p,
+// The encoder half of chunk p on the rows of s: hands the [x_hist | chunk] window xw [B][hist + T] (global samples
+// [samples - hist, samples + T)) and the chunk's channels-last latents znew [B][T/300][1024], both in workspace, to
+// `tail(xw, znew)`, then keeps the new histories.
+template <typename F>
+void stream_encode(Ctx& c, EncHalf& s, const EncPlan& p, const float* x, F tail) {
+    const EncW& e = c.h->enc;
+    const int B = s.B, T = p.T, hist = p.hist, yh = p.yh, Tw = hist + T, Fc = T / HOP, Fh = hist / HOP;
+    c.vq_critical = true;
+    float* xw = c.alloc<float>((size_t)B * Tw);
+    copy_rows(c, xw, Tw, s.x_hist, kEncCtx, 0, hist, 1, B, "stream.xh");
+    copy_rows(c, xw + hist, Tw, x, T, 0, T, 1, B, "stream.xc");
+    int Fw = 0;
+    float* feats = encoder_front(c, xw, B, Tw, &Fw);                    // [B][Fw][1024], Fw == Fh + Fc
+    float* fnew = c.alloc<float>((size_t)B * Fc * LATENT);
+    copy_rows(c, fnew, Fc, feats, Fw, Fh, Fc, LATENT, B, "stream.fnew");
+    float* yw = c.alloc<float>((size_t)B * (yh + Fc) * LATENT);        // [hist | new] LSTM outputs
+    float* ynew = c.alloc<float>((size_t)B * Fc * LATENT);
+    LstmState st = s.lstm;
+    slstm(c, e.lstm, fnew, ynew, B, Fc, &st);
+    copy_rows(c, yw, yh + Fc, s.ey_hist, 2, 0, yh, LATENT, B, "stream.yh");
+    copy_rows(c, yw + (size_t)yh * LATENT, yh + Fc, ynew, Fc, 0, Fc, LATENT, B, "stream.yc");
+    float* zw = c.alloc<float>((size_t)B * (yh + Fc) * LATENT);
+    float* znew = c.alloc<float>((size_t)B * Fc * LATENT);
+    ConvOpts o;
+    o.in_snake = &e.snake;
+    sconv(c, e.conv_out, yw, zw, B, yh + Fc, 1, 1, o, "enc.conv_out");
+    copy_rows(c, znew, Fc, zw, yh + Fc, yh, Fc, LATENT, B, "stream.znew");
+    tail(xw, znew);
+    // new histories: the last kEncCtx samples / 2 LSTM-output frames of what has been seen so far
+    float* tmpx = c.alloc<float>((size_t)B * kEncCtx);
+    copy_rows(c, tmpx, kEncCtx, xw, Tw, Tw - p.hist1, p.hist1, 1, B, "stream.xh2");
+    copy_rows(c, s.x_hist, kEncCtx, tmpx, kEncCtx, 0, p.hist1, 1, B, "stream.xh3");
+    copy_rows(c, s.ey_hist, 2, yw, yh + Fc, yh + Fc - p.yh1, p.yh1, LATENT, B, "stream.yh2");
+    c.vq_critical = false;
+}
+
+// Codes of Fq frames from E = the window's frame win (the kCodesOnly VQ kernel): the prosody net recomputed over the mel
+// rows [m0, m0 + win + Fq) of s, i.e. frames [max(0, E - 32), E + Fq) -- each of the WN's 8 causal k = 5 convs reflect-pads
+// 4 frames at the window's left edge, so the first 32 frames of a window are not those of the whole utterance unless the
+// window starts at frame 0 -- and the latents zq [B][Fq][1024] (row pitch zpitch frames).  Runs with c.vq_critical set, as
+// the offline quantizer.
+void stream_codes(Ctx& c, const EncHalf& s, int m0, int win, int Fq, const float* zq, int zpitch, int64_t* codes_p,
                   int64_t* codes_c, int64_t* codes_r) {
-    const int B = s.B, lo = (int)(E > kWnCtx ? E - kWnCtx : 0), Fw = (int)(E + Fq - lo);
+    const int B = s.B, Fw = win + Fq;
     float* melw = c.alloc<float>((size_t)B * Fw * N_MELS);
-    copy_rows(c, melw, Fw, s.mel, s.mel_cap, (int)(lo - s.mel_base), Fw, N_MELS, B, "stream.melw");
+    copy_rows(c, melw, Fw, s.mel.get(), s.mel_cap, m0, Fw, N_MELS, B, "stream.melw");
     const float* f0 = prosody_forward(c, melw, B, Fw);
     if (c.dry) return;
     FaqParams fp;
-    fp.f0 = f0 + (size_t)(E - lo) * LATENT; fp.Tf0 = Fw;
+    fp.f0 = f0 + (size_t)win * LATENT; fp.Tf0 = Fw;
     fp.z = zq; fp.Tz = zpitch;
     for (int i = 0; i < 6; ++i) {
         const VqW& v = c.h->qw.vq[i];
@@ -1844,27 +1937,26 @@ void stream_codes(Ctx& c, const fac_handle::Stream& s, long long E, int Fq, cons
     c.check(launch_fa_codes(fp, c.st), "fa_codes");
 }
 
-// Grow-only (doubling) capacity of the stream's mel80 rows; the `emitted` rows written so far move along.
-int grow_mel(fac_handle* h, fac_handle::Stream& s, int rows, cudaStream_t st) {
+// Grow-only (doubling) capacity of s.mel for B rows of `rows` frames; the first `keep` rows of each move along.
+int grow_mel(fac_handle* h, EncHalf& s, int B, long long keep, int rows, cudaStream_t st) {
     if (rows <= s.mel_cap) return FAC_OK;
     int cap = s.mel_cap > 0 ? s.mel_cap : 64;
     while (cap < rows) cap *= 2;
     cudaError_t e = cudaSetDevice(h->device);
     float* p = nullptr;
-    if (e == cudaSuccess) e = cudaMalloc(&p, sizeof(float) * (size_t)s.B * cap * N_MELS);
+    if (e == cudaSuccess) e = cudaMalloc(&p, sizeof(float) * (size_t)B * cap * N_MELS);
+    DevBuf<float> grown(p);
     if (e == cudaSuccess && s.mel) {
-        e = cudaMemcpy2DAsync(p, sizeof(float) * (size_t)cap * N_MELS, s.mel, sizeof(float) * (size_t)s.mel_cap * N_MELS,
-                              sizeof(float) * (size_t)s.emitted * N_MELS, s.B, cudaMemcpyDeviceToDevice, st);
+        e = cudaMemcpy2DAsync(p, sizeof(float) * (size_t)cap * N_MELS, s.mel.get(), sizeof(float) * (size_t)s.mel_cap * N_MELS,
+                              sizeof(float) * (size_t)keep * N_MELS, B, cudaMemcpyDeviceToDevice, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     }
     if (e != cudaSuccess) {
         h->err = std::string("stream mel buffer: ") + cudaGetErrorString(e);
         cudaGetLastError();
-        if (p) cudaFree(p);
         return FAC_ERR_CUDA;
     }
-    if (s.mel) cudaFree(s.mel);
-    s.mel = p; s.mel_cap = cap;
+    s.mel = std::move(grown); s.mel_cap = cap;
     return FAC_OK;
 }
 
@@ -1875,132 +1967,127 @@ int stream_codes_supported(fac_handle* h, const char* who) {
     h->err = std::string(who) + ": needs tensor_cores = 2 (the mel path that frames the wave explicitly)";
     return FAC_ERR_UNSUPPORTED;
 }
-}  // namespace
 
-extern "C" {
-
-int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float* z, void* stream) {
-    int rc = check_ready(h, FAC_ENCODER);
+// The argument-independent rules of fac_stream_encode_codes on half s (pointers and the stream id checked by the caller).
+int stream_encode_codes_check(fac_handle* h, const EncHalf& s, int T, int n_c, const char* who) {
+    int rc = stream_encode_check(h, s, T, EncHalf::kCodes, who);
     if (rc) return rc;
-    if (!stream_alive(h, stream_id) || !x || !z) { h->err = "fac_stream_encode: bad arguments"; return FAC_ERR_INVALID; }
-    fac_handle::Stream& s = *h->streams[stream_id];
-    rc = stream_encode_check(h, s, T, fac_handle::Stream::kEncLatents, "fac_stream_encode");
-    if (rc) return rc;
-    const int B = s.B, Fc = T / HOP;
-    return stream_encode(h, s, x, T, stream, fac_handle::Stream::kEncLatents, [&](Ctx& c, const EncChunk& ch) {
-        if (!c.dry) c.check(launch_transpose(ch.znew, z, B, Fc, LATENT, c.st), "enc.z_T");
-    });
-}
-
-}  // extern "C"
-
-namespace {
-// The argument-independent rules of fac_stream_encode_codes on stream s (pointers and the stream id checked by the caller).
-int stream_encode_codes_check(fac_handle* h, const fac_handle::Stream& s, int T, int n_c, const char* who) {
-    using S = fac_handle::Stream;
-    int rc = stream_encode_check(h, s, T, S::kEncCodes, who);
-    if (rc) return rc;
-    if (s.enc_mode == S::kEncCodes && n_c != s.n_c) {
+    if (s.mode == EncHalf::kCodes && n_c != s.n_c) {
         h->err = std::string(who) + ": n_c changed mid-stream (" + std::to_string(s.n_c) + " -> " + std::to_string(n_c) + ")";
         return FAC_ERR_INVALID;
     }
     return stream_codes_supported(h, who);
 }
 
-// The launch sequence of fac_stream_encode_codes on a checked stream whose mel rows reach frame N - 1 (row r at s.mel +
-// (r - s.mel_base) * 80): advances the stream and returns the frames written, or a negative status.
-int stream_encode_codes(fac_handle* h, fac_handle::Stream& s, const float* x, int T, int n_c, int64_t* codes_p,
-                        int64_t* codes_c, int64_t* codes_r, void* stream) {
-    using S = fac_handle::Stream;
-    // frames [E, N - 1) are final: frame N - 1 reads 300 samples past what has arrived (reflected only at the true end)
-    const int B = s.B, Fc = T / HOP, first = s.enc_samples == 0;
-    const long long N = (s.enc_samples + T) / HOP, E = s.emitted;
-    const int Fout = (int)(N - 1 - E);
-    s.n_c = n_c;
-    int rc = stream_encode(h, s, x, T, stream, S::kEncCodes, [&](Ctx& c, const EncChunk& ch) {
+// The launch sequence of a codes chunk p on a checked half whose mel rows reach frame E + Fout - 1 (frame f at row
+// f - s.mel_base).
+void stream_encode_codes(Ctx& c, EncHalf& s, const EncPlan& p, const float* x, int64_t* codes_p, int64_t* codes_c,
+                         int64_t* codes_r) {
+    const int B = s.B, Fc = p.T / HOP, Fout = p.Fout, m0 = (int)(p.lo - s.mel_base);
+    stream_encode(c, s, p, x, [&](const float* xw, const float* znew) {
         c.vq_critical = true;
-        const int f_first = (int)(E - (s.enc_samples - ch.hist) / HOP);   // frame E within the window
-        const float* mel = mel_frames_tc(c, quantizer_mel(h), ch.xw, B, ch.Tw, f_first, Fout);
-        copy_rows(c, s.mel + (size_t)(E - s.mel_base) * N_MELS, s.mel_cap, mel, Fout, 0, Fout, N_MELS, B, "stream.mel");
+        const float* mel = mel_frames_tc(c, quantizer_mel(c.h), xw, B, p.hist + p.T, p.f_first, Fout);
+        copy_rows(c, s.mel.get() + (size_t)(m0 + p.win) * N_MELS, s.mel_cap, mel, Fout, 0, Fout, N_MELS, B, "stream.mel");
         // latents of frames [E, N - 1): the held frame (after the first chunk) then all but the chunk's last frame
-        const float* zq = ch.znew;
-        if (!first) {
+        const float* zq = znew;
+        if (!p.first) {
             float* zcat = c.alloc<float>((size_t)B * Fout * LATENT);
             copy_rows(c, zcat, Fout, s.z_held, 1, 0, 1, LATENT, B, "stream.zheld");
-            copy_rows(c, zcat + LATENT, Fout, ch.znew, Fc, 0, Fc - 1, LATENT, B, "stream.zcat");
+            copy_rows(c, zcat + LATENT, Fout, znew, Fc, 0, Fc - 1, LATENT, B, "stream.zcat");
             zq = zcat;
         }
-        stream_codes(c, s, E, Fout, zq, first ? Fc : Fout, codes_p, codes_c, codes_r);
-        copy_rows(c, s.z_held, 1, ch.znew, Fc, Fc - 1, 1, LATENT, B, "stream.zhold");
+        stream_codes(c, s, m0, p.win, Fout, zq, p.first ? Fc : Fout, codes_p, codes_c, codes_r);
+        copy_rows(c, s.z_held, 1, znew, Fc, Fc - 1, 1, LATENT, B, "stream.zhold");
     });
-    if (rc == FAC_OK) s.emitted = N - 1;
-    return rc == FAC_OK ? Fout : rc;
 }
 
-int stream_finish_codes_check(fac_handle* h, const fac_handle::Stream& s, const char* who) {
-    using S = fac_handle::Stream;
-    if (s.enc_mode != S::kEncCodes) {
-        h->err = std::string(who) + (s.enc_mode == S::kEncFinished ? ": the stream's encoder is already finished"
-                                                                    : ": nothing was encoded with fac_stream_encode_codes");
+int stream_finish_codes_check(fac_handle* h, const EncHalf& s, const char* who) {
+    if (s.mode != EncHalf::kCodes) {
+        h->err = std::string(who) + (s.mode == EncHalf::kFinished ? ": the stream's encoder is already finished"
+                                                                   : ": nothing was encoded with fac_stream_encode_codes");
         return FAC_ERR_STATE;
     }
     return stream_codes_supported(h, who);
 }
 
-// The launch sequence of fac_stream_finish_codes on a checked stream whose mel rows start at frame 0.
-int stream_finish_codes(fac_handle* h, fac_handle::Stream& s, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r,
-                        float* timbre, void* stream) {
-    using S = fac_handle::Stream;
-    const int B = s.B, hist = s.x_hist_len, N = (int)(s.enc_samples / HOP);
+// fac_stream_finish_codes on a checked half whose mel rows start at frame 0 (a stream, or a pool session's B = 1 slot,
+// which keeps all of its mel rows): returns the frames written (1) or a negative status.
+int finish_codes(fac_handle* h, EncHalf& s, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre,
+                 void* stream) {
+    const int B = s.B, hist = s.x_hist_len, N = (int)(s.samples / HOP);
     const long long E = s.emitted;   // == N - 1
+    const int win = (int)(E > kWnCtx ? kWnCtx : E);
     int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
         c.vq_critical = true;
         // frame N - 1 from the last `hist` samples, reflected at the utterance's true end
         float* xw = c.alloc<float>((size_t)B * hist);
         copy_rows(c, xw, hist, s.x_hist, kEncCtx, 0, hist, 1, B, "stream.xfin");
-        const float* mel = mel_frames_tc(c, quantizer_mel(h), xw, B, hist, (int)(E - (s.enc_samples - hist) / HOP), 1);
-        copy_rows(c, s.mel + (size_t)E * N_MELS, s.mel_cap, mel, 1, 0, 1, N_MELS, B, "stream.mel");
-        stream_codes(c, s, E, 1, s.z_held, 1, codes_p, codes_c, codes_r);
+        const float* mel = mel_frames_tc(c, quantizer_mel(h), xw, B, hist, (int)(E - (s.samples - hist) / HOP), 1);
+        copy_rows(c, s.mel.get() + (size_t)E * N_MELS, s.mel_cap, mel, 1, 0, 1, N_MELS, B, "stream.mel");
+        stream_codes(c, s, (int)E - win, win, 1, s.z_held, 1, codes_p, codes_c, codes_r);
         if (timbre) {
             // the offline StyleEncoder input: every mel80 row of the utterance
             float* melall = c.alloc<float>((size_t)B * N * N_MELS);
-            copy_rows(c, melall, N, s.mel, s.mel_cap, 0, N, N_MELS, B, "stream.melall");
+            copy_rows(c, melall, N, s.mel.get(), s.mel_cap, 0, N, N_MELS, B, "stream.melall");
             style_encoder(c, melall, B, N, nullptr, timbre);
         }
         c.vq_critical = false;
     });
     if (rc != FAC_OK) return rc;
     s.emitted = N;
-    s.enc_mode = S::kEncFinished;
+    s.mode = EncHalf::kFinished;
     return 1;
 }
 }  // namespace
 
 extern "C" {
 
+int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float* z, void* stream) {
+    int rc = check_ready(h, {FAC_ENCODER});
+    if (rc) return rc;
+    Stream* st = by_id(h, &fac_handle::streams, stream_id);
+    if (!st || !x || !z) { h->err = "fac_stream_encode: bad arguments"; return FAC_ERR_INVALID; }
+    EncHalf& s = st->enc;
+    if ((rc = stream_encode_check(h, s, T, EncHalf::kLatents, "fac_stream_encode"))) return rc;
+    const EncPlan p = enc_plan(s, T);
+    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        stream_encode(c, s, p, x, [&](const float*, const float* znew) {
+            if (!c.dry) c.check(launch_transpose(znew, z, s.B, T / HOP, LATENT, c.st), "enc.z_T");
+        });
+    });
+    if (rc == FAC_OK) enc_commit(s, p, EncHalf::kLatents);
+    return rc;
+}
+
 int fac_stream_encode_codes(fac_handle* h, int stream_id, const float* x, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
                             int64_t* codes_r, void* stream) {
-    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER});
+    if (rc) return rc;
     const char* who = "fac_stream_encode_codes";
-    if (!stream_alive(h, stream_id) || !x || !codes_p || !codes_c || !codes_r || n_c < 1 || n_c > 2) {
+    Stream* st = by_id(h, &fac_handle::streams, stream_id);
+    if (!st || !x || !codes_p || !codes_c || !codes_r || n_c < 1 || n_c > 2) {
         h->err = "fac_stream_encode_codes: bad arguments (1 <= n_c <= 2)";
         return FAC_ERR_INVALID;
     }
-    fac_handle::Stream& s = *h->streams[stream_id];
-    int rc = stream_encode_codes_check(h, s, T, n_c, who);
+    EncHalf& s = st->enc;
+    if ((rc = stream_encode_codes_check(h, s, T, n_c, who))) return rc;
+    if ((rc = grow_mel(h, s, s.B, s.emitted, (int)((s.samples + T) / HOP), (cudaStream_t)stream))) return rc;
+    const EncPlan p = enc_plan(s, T);
+    s.n_c = n_c;
+    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { stream_encode_codes(c, s, p, x, codes_p, codes_c, codes_r); });
     if (rc) return rc;
-    if ((rc = grow_mel(h, s, (int)((s.enc_samples + T) / HOP), (cudaStream_t)stream))) return rc;
-    return stream_encode_codes(h, s, x, T, n_c, codes_p, codes_c, codes_r, stream);
+    enc_commit(s, p, EncHalf::kCodes);
+    return p.Fout;
 }
 
 int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre,
                             void* stream) {
-    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
-    if (!stream_alive(h, stream_id) || !codes_p || !codes_c || !codes_r) { h->err = "fac_stream_finish_codes: bad arguments"; return FAC_ERR_INVALID; }
-    fac_handle::Stream& s = *h->streams[stream_id];
-    int rc = stream_finish_codes_check(h, s, "fac_stream_finish_codes");
+    int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER});
     if (rc) return rc;
-    return stream_finish_codes(h, s, codes_p, codes_c, codes_r, timbre, stream);
+    Stream* st = by_id(h, &fac_handle::streams, stream_id);
+    if (!st || !codes_p || !codes_c || !codes_r) { h->err = "fac_stream_finish_codes: bad arguments"; return FAC_ERR_INVALID; }
+    if ((rc = stream_finish_codes_check(h, st->enc, "fac_stream_finish_codes"))) return rc;
+    return finish_codes(h, st->enc, codes_p, codes_c, codes_r, timbre, stream);
 }
 
 }  // extern "C"
@@ -2014,99 +2101,88 @@ int stream_decode_check(fac_handle* h, long long frames, int Fc, const char* who
     return FAC_OK;
 }
 
-// Inside a launch sequence: lane b of n copies words(b) 32-bit words from src(b) to dst(b) (launch_lane_copy).
-template <typename W, typename S, typename D>
-void lane_copy(Ctx& c, int n, W words, S src, D dst, const char* what) {
-    if (c.dry) return;
-    LaneCopyParams p;
-    p.n = n;
-    for (int b = 0; b < n; ++b) { p.src[b] = (const uint32_t*)src(b); p.dst[b] = (uint32_t*)dst(b); p.words[b] = words(b); }
-    c.check(launch_lane_copy(p, c.st), what);
-}
+// The decoder half's launch sequence depends only on its history depth: zh = min(frames, 6) latent and dh = min(frames, 20)
+// LSTM-output frames (a first chunk has >= 10 frames, so dh fixes zh).  The chunk lengths of its rows may differ.
+struct DecPlan {
+    int zh, dh;
+    std::vector<long long> key() const { return {zh, dh}; }
+};
+DecPlan dec_plan(long long frames) { return {(int)std::min(frames, 6LL), (int)std::min(frames, (long long)kDecCtx)}; }
 
-// The body of fac_stream_decode / fac_stream_decode_codes on a checked stream: row b takes F[b] new frames (HOST, s.B
-// entries), whose channels-last latents `latents(c, B)` returns as [B][Fmax][1024] (Fmax = the largest F[b]; transposed
-// from the caller's z, or dequantized from codes).  y receives [B][300 Fmax], row b valid for its first 300 F[b] samples.
-// With equal F this is one stream chunk.  With unequal F (a decode pool's batch) each row runs on a window padded past its
-// own end: the decoder after the LSTM is causal (left reflect padding, no right padding, transposed convs trimmed on the
-// right), so no sample before a row's end reads the padding; the LSTM stops each row at its own end, and the histories are
-// cut at each row's own end.  The stream's counters advance by Fmax (a pool keeps its sessions' own).
+// The decoder half of a chunk on the rows of s (plan p): row b takes F[b] new frames (HOST, s.B entries), whose channels-last
+// latents `latents(c, B)` returns as [B][Fmax][1024] (Fmax = the largest F[b]; transposed from the caller's z, or
+// dequantized from codes).  y receives [B][300 Fmax], row b valid for its first 300 F[b] samples.  With equal F this is one
+// stream chunk.  With unequal F (a decode pool's batch) each row runs on a window padded past its own end: the decoder after
+// the LSTM is causal (left reflect padding, no right padding, transposed convs trimmed on the right), so no sample before a
+// row's end reads the padding; the LSTM stops each row at its own end, and the histories are cut at each row's own end.
 template <typename L>
-int stream_decode(fac_handle* h, fac_handle::Stream& s, const int* F, float* y, void* stream, L latents) {
-    const int B = s.B, zh = s.z_hist_len, dh = s.dy_hist_len;
+void stream_decode(Ctx& c, DecHalf& s, const DecPlan& p, const int* F, float* y, L latents) {
+    const DecW& d = c.h->dec;
+    const int B = s.B, zh = p.zh, dh = p.dh;
     int Fc = 0;
     bool mixed = false;
     for (int b = 0; b < B; ++b) { Fc = F[b] > Fc ? F[b] : Fc; mixed = mixed || F[b] != F[0]; }
-    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-        const DecW& d = h->dec;
-        const float* znew = latents(c, B);
-        float* zw = c.alloc<float>((size_t)B * (zh + Fc) * LATENT);
-        copy_rows(c, zw, zh + Fc, s.z_hist, 6, 0, zh, LATENT, B, "stream.zh");
-        copy_rows(c, zw + (size_t)zh * LATENT, zh + Fc, znew, Fc, 0, Fc, LATENT, B, "stream.zc");
-        float* c0w = c.alloc<float>((size_t)B * (zh + Fc) * 1536);
-        sconv(c, d.conv0, zw, c0w, B, zh + Fc, 1, 1, ConvOpts(), "dec.conv0");
-        float* c0new = c.alloc<float>((size_t)B * Fc * 1536);
-        copy_rows(c, c0new, Fc, c0w, zh + Fc, zh, Fc, 1536, B, "stream.c0new");
-        float* ynew = c.alloc<float>((size_t)B * Fc * 1536);
-        LstmState st;
-        st.h[0] = s.dec_h[0]; st.h[1] = s.dec_h[1]; st.c[0] = s.dec_c[0]; st.c[1] = s.dec_c[1];
-        slstm(c, d.lstm, c0new, ynew, B, Fc, &st, mixed ? F : nullptr);
-        const int Fw = dh + Fc;
-        const size_t stage = decoder_stage_floats(B, Fw);
-        float* buf[3] = {c.alloc<float>(stage), c.alloc<float>(stage), c.alloc<float>(stage)};
-        float* yw_in = c.alloc<float>((size_t)B * Fw * 1536);
-        copy_rows(c, yw_in, Fw, s.dy_hist, kDecCtx, 0, dh, 1536, B, "stream.dh");
-        copy_rows(c, yw_in + (size_t)dh * 1536, Fw, ynew, Fc, 0, Fc, 1536, B, "stream.dc");
-        float* yw = c.alloc<float>((size_t)B * Fw * HOP);
-        decoder_stack(c, d, yw_in, -1, buf, B, Fw, yw);
-        copy_rows(c, y, Fc * HOP, yw, Fw * HOP, dh * HOP, Fc * HOP, 1, B, "stream.ynew");
-        if (mixed) {
-            auto nz = [&](int b) { return zh + F[b] < 6 ? zh + F[b] : 6; };
-            auto nd = [&](int b) { return dh + F[b] < kDecCtx ? dh + F[b] : kDecCtx; };
-            lane_copy(c, B, [&](int b) { return (long long)nz(b) * LATENT; },
-                      [&](int b) { return zw + ((size_t)b * (zh + Fc) + zh + F[b] - nz(b)) * LATENT; },
-                      [&](int b) { return s.z_hist + (size_t)b * 6 * LATENT; }, "stream.zh_lanes");
-            lane_copy(c, B, [&](int b) { return (long long)nd(b) * 1536; },
-                      [&](int b) { return yw_in + ((size_t)b * Fw + dh + F[b] - nd(b)) * 1536; },
-                      [&](int b) { return s.dy_hist + (size_t)b * kDecCtx * 1536; }, "stream.dh_lanes");
-            return;
-        }
-        const int nzh = zh + Fc < 6 ? zh + Fc : 6, ndh = Fw < kDecCtx ? Fw : kDecCtx;
-        float* tz = c.alloc<float>((size_t)B * 6 * LATENT);
-        float* td = c.alloc<float>((size_t)B * kDecCtx * 1536);
-        copy_rows(c, tz, 6, zw, zh + Fc, zh + Fc - nzh, nzh, LATENT, B, "stream.zh2");
-        copy_rows(c, s.z_hist, 6, tz, 6, 0, nzh, LATENT, B, "stream.zh3");
-        copy_rows(c, td, kDecCtx, yw_in, Fw, Fw - ndh, ndh, 1536, B, "stream.dh2");
-        copy_rows(c, s.dy_hist, kDecCtx, td, kDecCtx, 0, ndh, 1536, B, "stream.dh3");
-    });
-    if (rc == FAC_OK) {
-        s.z_hist_len = zh + Fc < 6 ? zh + Fc : 6;
-        s.dy_hist_len = dh + Fc < kDecCtx ? dh + Fc : kDecCtx;
-        s.dec_frames += Fc;
+    const float* znew = latents(c, B);
+    float* zw = c.alloc<float>((size_t)B * (zh + Fc) * LATENT);
+    copy_rows(c, zw, zh + Fc, s.z_hist, 6, 0, zh, LATENT, B, "stream.zh");
+    copy_rows(c, zw + (size_t)zh * LATENT, zh + Fc, znew, Fc, 0, Fc, LATENT, B, "stream.zc");
+    float* c0w = c.alloc<float>((size_t)B * (zh + Fc) * 1536);
+    sconv(c, d.conv0, zw, c0w, B, zh + Fc, 1, 1, ConvOpts(), "dec.conv0");
+    float* c0new = c.alloc<float>((size_t)B * Fc * 1536);
+    copy_rows(c, c0new, Fc, c0w, zh + Fc, zh, Fc, 1536, B, "stream.c0new");
+    float* ynew = c.alloc<float>((size_t)B * Fc * 1536);
+    LstmState st = s.lstm;
+    slstm(c, d.lstm, c0new, ynew, B, Fc, &st, mixed ? F : nullptr);
+    const int Fw = dh + Fc;
+    const size_t stage = decoder_stage_floats(B, Fw);
+    float* buf[3] = {c.alloc<float>(stage), c.alloc<float>(stage), c.alloc<float>(stage)};
+    float* yw_in = c.alloc<float>((size_t)B * Fw * 1536);
+    copy_rows(c, yw_in, Fw, s.dy_hist, kDecCtx, 0, dh, 1536, B, "stream.dh");
+    copy_rows(c, yw_in + (size_t)dh * 1536, Fw, ynew, Fc, 0, Fc, 1536, B, "stream.dc");
+    float* yw = c.alloc<float>((size_t)B * Fw * HOP);
+    decoder_stack(c, d, yw_in, -1, buf, B, Fw, yw);
+    copy_rows(c, y, Fc * HOP, yw, Fw * HOP, dh * HOP, Fc * HOP, 1, B, "stream.ynew");
+    if (mixed) {
+        auto nz = [&](int b) { return zh + F[b] < 6 ? zh + F[b] : 6; };
+        auto nd = [&](int b) { return dh + F[b] < kDecCtx ? dh + F[b] : kDecCtx; };
+        lane_copy(c, B, [&](int b) { return (long long)nz(b) * LATENT; },
+                  [&](int b) { return zw + ((size_t)b * (zh + Fc) + zh + F[b] - nz(b)) * LATENT; },
+                  [&](int b) { return s.z_hist + (size_t)b * 6 * LATENT; }, "stream.zh_lanes");
+        lane_copy(c, B, [&](int b) { return (long long)nd(b) * 1536; },
+                  [&](int b) { return yw_in + ((size_t)b * Fw + dh + F[b] - nd(b)) * 1536; },
+                  [&](int b) { return s.dy_hist + (size_t)b * kDecCtx * 1536; }, "stream.dh_lanes");
+        return;
     }
-    return rc;
+    const int nzh = zh + Fc < 6 ? zh + Fc : 6, ndh = Fw < kDecCtx ? Fw : kDecCtx;
+    float* tz = c.alloc<float>((size_t)B * 6 * LATENT);
+    float* td = c.alloc<float>((size_t)B * kDecCtx * 1536);
+    copy_rows(c, tz, 6, zw, zh + Fc, zh + Fc - nzh, nzh, LATENT, B, "stream.zh2");
+    copy_rows(c, s.z_hist, 6, tz, 6, 0, nzh, LATENT, B, "stream.zh3");
+    copy_rows(c, td, kDecCtx, yw_in, Fw, Fw - ndh, ndh, 1536, B, "stream.dh2");
+    copy_rows(c, s.dy_hist, kDecCtx, td, kDecCtx, 0, ndh, 1536, B, "stream.dh3");
 }
 
-// fac_stream_decode / fac_stream_decode_codes on stream stream_id: the checks, then one chunk of Fc frames on every row.
+// fac_stream_decode / fac_stream_decode_codes on a live stream: the checks, then one chunk of Fc frames on every row.
 template <typename L>
-int stream_decode_chunk(fac_handle* h, int stream_id, int Fc, float* y, void* stream, const char* who, L latents) {
-    int rc = check_ready(h, FAC_DECODER);
+int stream_decode_chunk(fac_handle* h, Stream& st, int Fc, float* y, void* stream, const char* who, L latents) {
+    DecHalf& s = st.dec;
+    int rc = stream_decode_check(h, s.frames, Fc, who);
     if (rc) return rc;
-    if (stream_id < 0 || stream_id >= (int)h->streams.size() || !h->streams[stream_id]->alive || !y) { h->err = std::string(who) + ": bad arguments"; return FAC_ERR_INVALID; }
-    fac_handle::Stream& s = *h->streams[stream_id];
-    if ((rc = stream_decode_check(h, s.dec_frames, Fc, who))) return rc;
     const std::vector<int> F(s.B, Fc);
-    return stream_decode(h, s, F.data(), y, stream, latents);
+    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { stream_decode(c, s, dec_plan(s.frames), F.data(), y, latents); });
+    if (rc == FAC_OK) s.frames += Fc;
+    return rc;
 }
 }  // namespace
 
 extern "C" {
 
 int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, float* y, void* stream) {
-    int rc = check_ready(h, FAC_DECODER);
+    int rc = check_ready(h, {FAC_DECODER});
     if (rc) return rc;
-    if (!z) { h->err = "fac_stream_decode: bad arguments"; return FAC_ERR_INVALID; }
-    return stream_decode_chunk(h, stream_id, Fc, y, stream, "fac_stream_decode", [&](Ctx& c, int B) {
+    Stream* st = by_id(h, &fac_handle::streams, stream_id);
+    if (!st || !z || !y) { h->err = "fac_stream_decode: bad arguments"; return FAC_ERR_INVALID; }
+    return stream_decode_chunk(h, *st, Fc, y, stream, "fac_stream_decode", [&](Ctx& c, int B) {
         float* znew = c.alloc<float>((size_t)B * Fc * LATENT);
         if (!c.dry) c.check(launch_transpose(z, znew, B, LATENT, Fc, c.st), "dec.z_transpose");
         return znew;
@@ -2115,14 +2191,14 @@ int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, floa
 
 int fac_stream_decode_codes(fac_handle* h, int stream_id, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows,
                             const int64_t* codes_r, int n_r_rows, const float* timbre, int Fc, float* y, void* stream) {
-    int rc = check_ready(h, FAC_QUANTIZER);
+    int rc = check_ready(h, {FAC_QUANTIZER, FAC_DECODER});
     if (rc) return rc;
-    if (stream_id < 0 || stream_id >= (int)h->streams.size() || !h->streams[stream_id]->alive ||
-        bad_codes_args(codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, h->streams[stream_id]->B, Fc)) {
+    Stream* st = by_id(h, &fac_handle::streams, stream_id);
+    if (!st || !y || bad_codes_args(codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, st->dec.B, Fc)) {
         h->err = "fac_stream_decode_codes: bad arguments (1 <= content rows <= 2, 0 <= residual rows <= 3)";
         return FAC_ERR_INVALID;
     }
-    return stream_decode_chunk(h, stream_id, Fc, y, stream, "fac_stream_decode_codes", [&](Ctx& c, int B) {
+    return stream_decode_chunk(h, *st, Fc, y, stream, "fac_stream_decode_codes", [&](Ctx& c, int B) {
         return (const float*)dequantize_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, Fc, false).outs_cl;
     });
 }
@@ -2154,52 +2230,80 @@ constexpr int kVcDecCtx = vc_decoder_reach();
 // 2 * kVcDecCtx.
 constexpr int kVcCodesHist = 2 * kVcRedCtx, kVcZHist = 2 * kVcDecCtx;
 
-// The frames a convert of F new code frames makes final: z up to Zf1, the output up to Yf1.
-void vc_targets(const fac_handle::VcStream& s, int F, long long* Zf1, long long* Yf1) {
-    const long long N1 = s.N + F;
-    *Zf1 = N1 - kVcRedCtx > s.Zf ? N1 - kVcRedCtx : s.Zf;
-    *Yf1 = *Zf1 - kVcDecCtx > s.Yf ? *Zf1 - kVcDecCtx : s.Yf;
+// B rows of voice-conversion state.
+void take_vc(Carve& m, VcStream& s, int B, size_t gfl) {
+    s.B = B;
+    s.g = m.take<float>((size_t)B * gfl);
+    s.codes = m.take<int64_t>((size_t)B * 3 * kVcCodesHist);
+    s.z = m.take<float>((size_t)B * kVcZHist * LATENT);
 }
 
-fac_handle::VcStream* vc_stream(fac_handle* h, int id) {
-    return id >= 0 && id < (int)h->vc_streams.size() && h->vc_streams[id]->alive ? h->vc_streams[id] : nullptr;
-}
+// Every integer of a voice-conversion step on a stream at (N, Zf, Yf) fed F code frames (F = 0 at finish, which makes every
+// frame final), and the counters it leaves.  The step runs on the codes window [hc0, N1) (Tw frames, hist of them history)
+// and the z window [zh0, Zf1) (Tz frames, zhist of them history).  It makes z final up to Zf1 and the output up to Yf1:
+// both stages reach kVcRedCtx / kVcDecCtx frames past the rows they keep, so those rows never see a window edge except the
+// utterance's own (frame 0, and frame N at finish).  Streams with equal keys share one pool batch.
+struct VcPlan {
+    int F, Tw, hist, Tz, zhist;
+    int zoff, znew;             // z rows [Zf, Zf1) in the codes window
+    int k, yoff;                // output frames [Yf, Yf1) and Yf in the z window
+    int zkeep_at, zkeep;        // z history kept: [zh1, Zf1) in the z window
+    int ckeep_at, ckeep;        // codes history kept: [hc1, N1) in the codes window
+    long long N1, Zf1, Yf1;
+    std::vector<long long> key() const { return {F, Tw, hist, Tz, zhist, zoff, znew, k, yoff, zkeep_at, zkeep, ckeep_at, ckeep}; }
+};
 
-// One step of a voice-conversion stream: append F code frames (codes_p [B][1][F], codes_c [B][n_c_rows][F]; F = 0 at
-// finish), make z final up to frame Zf1 and the output up to frame Yf1, and write output frames [Yf, Yf1) to y as
-// [B][1][300 (Yf1 - Yf)].  Both stages run the offline bodies on windows that reach kVcRedCtx / kVcDecCtx frames past the
-// rows they keep, so those rows never see a window edge except the utterance's own (frame 0, and frame N at finish).
-// The state (N, Zf, Yf) is the caller's to advance on success.
-int vc_step(fac_handle* h, fac_handle::VcStream& s, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, int F,
-            long long Zf1, long long Yf1, float* y, void* stream) {
+VcPlan vc_plan(long long N, long long Zf, long long Yf, int F, bool finish) {
     auto floor0 = [](long long v) { return v > 0 ? v : 0; };
-    const int B = s.B;
-    const long long N1 = s.N + F, hc0 = floor0(s.Zf - kVcRedCtx), zh0 = floor0(s.Yf - kVcDecCtx);
-    const long long hc1 = floor0(Zf1 - kVcRedCtx), zh1 = floor0(Yf1 - kVcDecCtx);
-    const int Tw = (int)(N1 - hc0), hist = (int)(s.N - hc0), Tz = (int)(Zf1 - zh0), zhist = (int)(s.Zf - zh0);
-    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-        // codes [hc0, N1) as [B][3][Tw]: the history, then the new frames
-        int64_t* cw = c.alloc<int64_t>((size_t)B * 3 * Tw);
-        copy_rows(c, cw, Tw, s.codes, kVcCodesHist, 0, hist, 1, 3 * B, "vc.codes_hist");
-        copy_rows(c, cw + hist, 3 * Tw, codes_p, F, 0, F, 1, B, "vc.codes_p");
-        for (int i = 0; i < s.n_c; ++i)
-            copy_rows(c, cw + (size_t)(1 + i) * Tw + hist, 3 * Tw, codes_c + (size_t)i * F, n_c_rows * F, 0, F, 1, B, "vc.codes_c");
-        if (Zf1 > s.Zf) {
-            // z over the codes window, of which rows [Zf, Zf1) are final; the decoder's window is z [zh0, Zf1)
-            float* zc = redecoder_body(c, cw, 3 * Tw, cw + Tw, 3 * Tw, s.g, B, Tw, s.use_p, s.use_c, s.n_c);
-            float* zw = c.alloc<float>((size_t)B * Tz * LATENT);
-            copy_rows(c, zw, Tz, s.z, kVcZHist, 0, zhist, LATENT, B, "vc.z_hist");
-            copy_rows(c, zw + (size_t)zhist * LATENT, Tz, zc, Tw, (int)(s.Zf - hc0), (int)(Zf1 - s.Zf), LATENT, B, "vc.z_new");
-            if (Yf1 > s.Yf) {
-                const int k = (int)(Yf1 - s.Yf);
-                float* yw = c.alloc<float>((size_t)B * Tz * HOP);
-                decoder_forward(c, h->dec2, zw, B, Tz, yw);
-                copy_rows(c, y, k * HOP, yw, Tz * HOP, (int)(s.Yf - zh0) * HOP, k * HOP, 1, B, "vc.y");
-            }
-            copy_rows(c, s.z, kVcZHist, zw, Tz, (int)(zh1 - zh0), (int)(Zf1 - zh1), LATENT, B, "vc.z_keep");
+    VcPlan p;
+    p.N1 = N + F;
+    p.Zf1 = finish ? p.N1 : std::max(p.N1 - kVcRedCtx, Zf);
+    p.Yf1 = finish ? p.N1 : std::max(p.Zf1 - kVcDecCtx, Yf);
+    const long long hc0 = floor0(Zf - kVcRedCtx), zh0 = floor0(Yf - kVcDecCtx);
+    const long long hc1 = floor0(p.Zf1 - kVcRedCtx), zh1 = floor0(p.Yf1 - kVcDecCtx);
+    p.F = F; p.Tw = (int)(p.N1 - hc0); p.hist = (int)(N - hc0); p.Tz = (int)(p.Zf1 - zh0); p.zhist = (int)(Zf - zh0);
+    p.zoff = (int)(Zf - hc0); p.znew = (int)(p.Zf1 - Zf); p.k = (int)(p.Yf1 - Yf); p.yoff = (int)(Yf - zh0);
+    p.zkeep_at = (int)(zh1 - zh0); p.zkeep = (int)(p.Zf1 - zh1); p.ckeep_at = (int)(hc1 - hc0); p.ckeep = (int)(p.N1 - hc1);
+    return p;
+}
+VcPlan vc_plan(const VcStream& s, int F, bool finish) { return vc_plan(s.N, s.Zf, s.Yf, F, finish); }
+
+// The launch sequence of step p on the rows of s: appends F code frames (codes_p [B][1][F], codes_c [B][n_c_rows][F]) and
+// writes output frames [Yf, Yf1) to y as [B][1][300 k].
+void vc_step(Ctx& c, VcStream& s, const VcPlan& p, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, float* y) {
+    const int B = s.B, F = p.F, Tw = p.Tw, hist = p.hist, Tz = p.Tz;
+    // codes [hc0, N1) as [B][3][Tw]: the history, then the new frames
+    int64_t* cw = c.alloc<int64_t>((size_t)B * 3 * Tw);
+    copy_rows(c, cw, Tw, s.codes, kVcCodesHist, 0, hist, 1, 3 * B, "vc.codes_hist");
+    copy_rows(c, cw + hist, 3 * Tw, codes_p, F, 0, F, 1, B, "vc.codes_p");
+    for (int i = 0; i < s.n_c; ++i)
+        copy_rows(c, cw + (size_t)(1 + i) * Tw + hist, 3 * Tw, codes_c + (size_t)i * F, n_c_rows * F, 0, F, 1, B, "vc.codes_c");
+    if (p.znew > 0) {
+        // z over the codes window, of which rows [Zf, Zf1) are final; the decoder's window is z [zh0, Zf1)
+        float* zc = redecoder_body(c, cw, 3 * Tw, cw + Tw, 3 * Tw, s.g, B, Tw, s.use_p, s.use_c, s.n_c);
+        float* zw = c.alloc<float>((size_t)B * Tz * LATENT);
+        copy_rows(c, zw, Tz, s.z, kVcZHist, 0, p.zhist, LATENT, B, "vc.z_hist");
+        copy_rows(c, zw + (size_t)p.zhist * LATENT, Tz, zc, Tw, p.zoff, p.znew, LATENT, B, "vc.z_new");
+        if (p.k > 0) {
+            float* yw = c.alloc<float>((size_t)B * Tz * HOP);
+            decoder_forward(c, c.h->dec2, zw, B, Tz, yw);
+            copy_rows(c, y, p.k * HOP, yw, Tz * HOP, p.yoff * HOP, p.k * HOP, 1, B, "vc.y");
         }
-        copy_rows(c, s.codes, kVcCodesHist, cw, Tw, (int)(hc1 - hc0), (int)(N1 - hc1), 1, 3 * B, "vc.codes_keep");
-    });
+        copy_rows(c, s.z, kVcZHist, zw, Tz, p.zkeep_at, p.zkeep, LATENT, B, "vc.z_keep");
+    }
+    copy_rows(c, s.codes, kVcCodesHist, cw, Tw, p.ckeep_at, p.ckeep, 1, 3 * B, "vc.codes_keep");
+}
+
+void vc_commit(VcStream& s, const VcPlan& p) { s.N = p.N1; s.Zf = p.Zf1; s.Yf = p.Yf1; }
+
+// Step p of a voice-conversion stream (or a pool session's B = 1 slot) in its own launch sequence: returns the output frames
+// written or a negative status.
+int vc_run(fac_handle* h, VcStream& s, const VcPlan& p, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, float* y,
+           void* stream) {
+    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { vc_step(c, s, p, codes_p, codes_c, n_c_rows, y); });
+    if (rc) return rc;
+    vc_commit(s, p);
+    return p.k;
 }
 }  // namespace
 
@@ -2208,179 +2312,62 @@ extern "C" {
 int fac_vc_stream_lookahead(void) { return kVcRedCtx + kVcDecCtx; }
 
 int fac_vc_stream_begin(fac_handle* h, int B, const float* timbre, int use_p_code, int use_c_code, int n_c, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER);
-    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
     if (!timbre || B < 1 || B > 32 || n_c < 0 || n_c > 2) {
         h->err = "fac_vc_stream_begin: bad arguments (1 <= B <= 32, 0 <= n_c <= 2)";
         return FAC_ERR_INVALID;
     }
-    cudaSetDevice(h->device);
-    auto* s = new fac_handle::VcStream();
-    s->B = B; s->use_p = use_p_code ? 1 : 0; s->use_c = use_c_code ? 1 : 0; s->n_c = n_c;
-    const size_t sizes[3] = {sizeof(float) * redecoder_cond_floats(h, B), sizeof(int64_t) * (size_t)B * 3 * kVcCodesHist,
-                             sizeof(float) * (size_t)B * kVcZHist * LATENT};
-    for (int i = 0; i < 3 && rc == FAC_OK; ++i) {
-        cudaError_t e = cudaMalloc(&s->all[i], sizes[i]);
-        if (e != cudaSuccess) {
-            h->err = std::string("fac_vc_stream_begin: ") + cudaGetErrorString(e);
-            cudaGetLastError();
-            rc = FAC_ERR_CUDA;
-        }
-    }
-    s->g = (float*)s->all[0]; s->codes = (int64_t*)s->all[1]; s->z = (float*)s->all[2];
+    auto s = std::make_unique<VcStream>();
+    s->use_p = use_p_code ? 1 : 0; s->use_c = use_c_code ? 1 : 0; s->n_c = n_c;
+    rc = dev_block(h, s->mem, "fac_vc_stream_begin", [&](Carve& m) { take_vc(m, *s, B, redecoder_cond_floats(h, 1)); });
     if (rc == FAC_OK) rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { redecoder_cond(c, timbre, B, s->g); });
-    if (rc != FAC_OK) {
-        for (void* p : s->all) if (p) cudaFree(p);
-        delete s;
-        return rc;
-    }
-    s->alive = true;
-    h->vc_streams.push_back(s);
+    if (rc != FAC_OK) return rc;
+    h->vc_streams.push_back(std::move(s));
     return (int)h->vc_streams.size() - 1;
 }
 
 int fac_vc_stream_convert(fac_handle* h, int stream_id, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, int F,
                           float* y, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER);
-    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
-    fac_handle::VcStream* s = vc_stream(h, stream_id);
+    VcStream* s = by_id(h, &fac_handle::vc_streams, stream_id);
     if (!s || !codes_p || !codes_c || !y || F <= 0 || n_c_rows < s->n_c || n_c_rows > 2) {
         h->err = "fac_vc_stream_convert: bad arguments (F >= 1, n_c <= rows of codes_c <= 2)";
         return FAC_ERR_INVALID;
     }
     if (s->finished) { h->err = "fac_vc_stream_convert: the stream was finished"; return FAC_ERR_STATE; }
-    const long long N1 = s->N + F;
-    long long Zf1, Yf1;
-    vc_targets(*s, F, &Zf1, &Yf1);
-    rc = vc_step(h, *s, codes_p, codes_c, n_c_rows, F, Zf1, Yf1, y, stream);
-    if (rc != FAC_OK) return rc;
-    const int k = (int)(Yf1 - s->Yf);
-    s->N = N1; s->Zf = Zf1; s->Yf = Yf1;
-    return k;
+    return vc_run(h, *s, vc_plan(*s, F, false), codes_p, codes_c, n_c_rows, y, stream);
 }
 
 int fac_vc_stream_finish(fac_handle* h, int stream_id, float* y, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER);
-    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
-    fac_handle::VcStream* s = vc_stream(h, stream_id);
+    VcStream* s = by_id(h, &fac_handle::vc_streams, stream_id);
     if (!s || !y) { h->err = "fac_vc_stream_finish: bad arguments"; return FAC_ERR_INVALID; }
     if (s->finished || s->N == 0) {
         h->err = s->finished ? "fac_vc_stream_finish: the stream was finished" : "fac_vc_stream_finish: no codes were received";
         return FAC_ERR_STATE;
     }
-    rc = vc_step(h, *s, nullptr, nullptr, 0, 0, s->N, s->N, y, stream);
-    if (rc != FAC_OK) return rc;
-    const int k = (int)(s->N - s->Yf);
-    s->Zf = s->Yf = s->N;
-    s->finished = true;
-    return k;
+    rc = vc_run(h, *s, vc_plan(*s, 0, true), nullptr, nullptr, 0, y, stream);
+    if (rc >= 0) s->finished = true;
+    return rc;
 }
 
 int fac_vc_stream_end(fac_handle* h, int stream_id) {
     if (!h || stream_id < 0 || stream_id >= (int)h->vc_streams.size()) return FAC_ERR_INVALID;
-    fac_handle::VcStream* s = h->vc_streams[stream_id];
-    if (s->alive) {
-        cudaSetDevice(h->device);
-        cudaDeviceSynchronize();
-        for (void*& p : s->all) { if (p) cudaFree(p); p = nullptr; }
-        s->alive = false;
-    }
-    return FAC_OK;
+    return h->vc_streams[stream_id] ? free_by_id(h, &fac_handle::vc_streams, stream_id) : FAC_OK;
 }
 
 }  // extern "C"
 
-// ---- stream pools (fac_codes_pool_*, fac_vc_pool_*): many B = 1 streams stepped in shared batches ----
-// A session's state lives in slot arrays with the per-row content of a B = 1 stream, and is presented to the stream bodies
-// as a B = 1 Stream / VcStream whose pointers alias its slot (finishes run there directly).  A step groups its sessions by
-// every integer the launch sequence depends on, gathers each batch of <= 32 into the lanes of a B = 32 stream (pool.cu,
-// lstm2.cu), runs the stream body on it and scatters the state back.  Every lane of the batched kernels computes as a
-// B = 1 launch does (batch invariance), so a session's bits do not depend on who shares its launch.
-struct fac_handle::CodesPool {
-    int cap = 0, n_c = 0;
-    std::vector<Stream> slot;               // B = 1 views: x_hist / ey_hist / z_held alias the arrays below; mel is the slot's own
-    std::vector<char> used;
-    Stream* lanes = nullptr;                // the B = 32 batch
-    float *x_hist = nullptr, *ey_hist = nullptr, *z_held = nullptr;
-    uint32_t* carry = nullptr;              // [cap][2 layers][kCarryWords] encoder-LSTM (h, c) in lstm2_lane_map order
-    float* xin = nullptr; size_t xin_cap = 0;           // [32][T] gathered chunks
-    int64_t* cout = nullptr; size_t cout_cap = 0;       // [32][1 + n_c + 3][F] codes before the scatter
-};
-struct fac_handle::VcPool {
-    int cap = 0, use_p = 0, use_c = 0, n_c = 0;
-    std::vector<VcStream> slot;             // B = 1 views of the arrays below
-    std::vector<char> used;
-    VcStream* lanes = nullptr;
-    float* g = nullptr; int64_t* codes = nullptr; float* z = nullptr;
-    int64_t* cin = nullptr; size_t cin_cap = 0;         // [32][1 + n_c][F] gathered codes
-    float* yout = nullptr; size_t yout_cap = 0;         // [32][300 k] output before the scatter
-};
-// The decode pool's sessions are rows of a decode-from-codes stream.  Its launch sequence depends only on the history depth
-// (zh = min(frames, 6) and dh = min(frames, 20) frames; a first chunk has >= 10 frames, so min(frames, 20) fixes both): the
-// chunk lengths and code rows of a batch may differ (stream_decode pads each lane past its own end).
-struct fac_handle::DecPool {
-    int cap = 0;
-    std::vector<long long> frames;          // frames decoded by each slot's session
-    std::vector<char> used;
-    Stream* lanes = nullptr;                // the B = 32 batch
-    float *z_hist = nullptr, *dy_hist = nullptr;        // [cap][6][1024], [cap][kDecCtx][1536]
-    uint32_t* carry = nullptr;              // [cap][2 layers][kDecCarryWords] decoder-LSTM (h, c) in lstm2_lane_map order
-    float* gb = nullptr;                    // [cap][2048] timbre_linear(timbre) of each session
-    float* yout = nullptr; size_t yout_cap = 0;         // [32][300 Fmax] output before the scatter
-};
-
+// ---- stream pools (fac_codes_pool_*, fac_vc_pool_*, fac_dec_pool_*): many B = 1 streams stepped in shared batches ----
+// A session's state lives in a slot: a B = 1 view of the state its step advances (an encoder half, a VcStream, a decoder
+// half), on which finishes run directly.  A step groups its sessions by their plans' keys (every integer the launch
+// sequence depends on), and runs each batch of <= 32 as one launch sequence: gather the sessions' state into the lanes of a
+// B = 32 state (pool.cu, lstm2.cu), run the stream body on them, scatter the state back.  Every lane of the batched kernels
+// computes as a B = 1 launch does (batch invariance), so a session's bits do not depend on who shares its launch.
 namespace {
-constexpr int kCarryWords = 2 * (LATENT / 2) + LATENT;   // one encoder-LSTM layer of one lane: hi | lo h planes, c
-
-template <typename E>
-int dev_zeros(fac_handle* h, E*& p, size_t n, const char* who) {
-    cudaError_t e = cudaMalloc(&p, sizeof(E) * n);
-    if (e == cudaSuccess) e = cudaMemset(p, 0, sizeof(E) * n);
-    if (e != cudaSuccess) {
-        h->err = std::string(who) + ": " + cudaGetErrorString(e);
-        cudaGetLastError();
-        if (p) cudaFree(p);
-        p = nullptr;
-        return FAC_ERR_CUDA;
-    }
-    return FAC_OK;
-}
-
-// Grow-only scratch of a pool; the old buffer may still be read by queued work, so the stream is drained first.
-template <typename E>
-int grow_buf(fac_handle* h, E*& p, size_t& cap, size_t n, cudaStream_t st) {
-    if (n <= cap) return FAC_OK;
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess && p) { e = cudaFree(p); p = nullptr; cap = 0; }
-    if (e == cudaSuccess) e = cudaMalloc(&p, sizeof(E) * n);
-    if (e != cudaSuccess) {
-        h->err = std::string("pool scratch: ") + cudaGetErrorString(e);
-        cudaGetLastError();
-        p = nullptr; cap = 0;
-        return FAC_ERR_CUDA;
-    }
-    cap = n;
-    return FAC_OK;
-}
-
-// lane b of a batch of n: `words` (a count, or a function of b) 32-bit words from src(b) to dst(b)
-template <typename W, typename S, typename D>
-int lane_move(fac_handle* h, int n, W words, S src, D dst, cudaStream_t st, const char* what) {
-    LaneCopyParams p;
-    p.n = n;
-    for (int b = 0; b < n; ++b) {
-        p.src[b] = (const uint32_t*)src(b); p.dst[b] = (uint32_t*)dst(b);
-        if constexpr (std::is_invocable_v<W, int>) p.words[b] = words(b);
-        else p.words[b] = words;
-    }
-    cudaError_t e = launch_lane_copy(p, st);
-    if (e != cudaSuccess) { h->err = std::string(what) + ": " + cudaGetErrorString(e); return FAC_ERR_CUDA; }
-    return FAC_OK;
-}
-
 // Batches of one pool step: sessions with equal keys form a group (groups in order of first appearance, members in input
 // order), each group cut into batches of at most kLaneMax.  group[i] / batch[i] (optional) receive input i's.
 std::vector<std::vector<int>> pool_plan(const std::vector<std::vector<long long>>& keys, int* group, int* batch) {
@@ -2401,35 +2388,50 @@ std::vector<std::vector<int>> pool_plan(const std::vector<std::vector<long long>
     return batches;
 }
 
-// Every integer the launch sequence of stream_encode_codes depends on, for a stream at (enc_samples, x_hist_len,
-// ey_hist_len, emitted) fed T samples: T, hist, yh, first chunk, f_first, Fout, the prosody window's E - lo and Fw.
-std::vector<long long> codes_key(long long enc_samples, int hist, int yh, long long E, int T) {
-    const long long N = (enc_samples + T) / HOP, Fout = N - 1 - E, lo = E > kWnCtx ? E - kWnCtx : 0;
-    return {T, hist, yh, enc_samples == 0, E - (enc_samples - hist) / HOP, Fout, E - lo, E + Fout - lo};
+// A pool of `capacity` slots: take(m, state, B, slot) lays out the B = 32 lanes and each B = 1 slot.
+template <typename S, typename T>
+int pool_create(fac_handle* h, List<Pool<S>> pools, int capacity, const char* who, T take) {
+    auto P = std::make_unique<Pool<S>>();
+    P->cap = capacity;
+    P->slot.resize(capacity);
+    P->used.assign(capacity, 0);
+    int rc = dev_block(h, P->mem, who, [&](Carve& m) {
+        take(m, P->lanes, kLaneMax, false);
+        for (S& s : P->slot) take(m, s, 1, true);
+    });
+    if (rc) return rc;
+    (h->*pools).push_back(std::move(P));
+    return (int)(h->*pools).size() - 1;
 }
 
-// ... of vc_step for a stream at (N, Zf, Yf) fed F frames: F, Tw, hist, Tz, zhist and the copy offsets and lengths.
-std::vector<long long> vc_key(long long N, long long Zf, long long Yf, int F) {
-    auto floor0 = [](long long v) { return v > 0 ? v : 0; };
-    fac_handle::VcStream s;
-    s.N = N; s.Zf = Zf; s.Yf = Yf;
-    long long Zf1, Yf1;
-    vc_targets(s, F, &Zf1, &Yf1);
-    const long long N1 = N + F, hc0 = floor0(Zf - kVcRedCtx), zh0 = floor0(Yf - kVcDecCtx);
-    const long long hc1 = floor0(Zf1 - kVcRedCtx), zh1 = floor0(Yf1 - kVcDecCtx);
-    return {F, N1 - hc0, N - hc0, Zf1 - zh0, Zf - zh0, Zf1 - Zf, Yf1 - Yf, Yf - zh0, zh1 - zh0, Zf1 - zh1, hc1 - hc0, N1 - hc1};
+// Opens the first free slot after init(slot) succeeds; returns the session id or a status.
+template <typename S, typename I>
+int pool_open(fac_handle* h, List<Pool<S>> pools, int id, const char* who, I init) {
+    Pool<S>* P = by_id(h, pools, id);
+    if (!P) { if (h) h->err = std::string(who) + ": no such pool"; return FAC_ERR_INVALID; }
+    int i = 0;
+    while (i < P->cap && P->used[i]) ++i;
+    if (i == P->cap) { h->err = std::string(who) + ": the pool is full (capacity " + std::to_string(P->cap) + ")"; return FAC_ERR_STATE; }
+    int rc = init(P->slot[i]);
+    if (rc) return rc;
+    P->used[i] = 1;
+    return i;
 }
 
-fac_handle::CodesPool* codes_pool(fac_handle* h, int id) {
-    return h && id >= 0 && id < (int)h->codes_pools.size() ? h->codes_pools[id] : nullptr;
-}
-fac_handle::VcPool* vc_pool(fac_handle* h, int id) {
-    return h && id >= 0 && id < (int)h->vc_pools.size() ? h->vc_pools[id] : nullptr;
+template <typename S>
+int pool_close(fac_handle* h, List<Pool<S>> pools, int id, int session, const char* who) {
+    Pool<S>* P = by_id(h, pools, id);
+    if (!P || session < 0 || session >= P->cap || !P->used[session]) {
+        if (h) h->err = std::string(who) + ": session " + std::to_string(session) + " is not open";
+        return FAC_ERR_INVALID;
+    }
+    P->used[session] = 0;
+    return FAC_OK;
 }
 
 // The sessions of one step: each open and named once.
-template <typename P>
-int check_sessions(fac_handle* h, const P& pool, int n, const int* sessions, const char* who) {
+template <typename S>
+int check_sessions(fac_handle* h, const Pool<S>& pool, int n, const int* sessions, const char* who) {
     std::vector<char> seen(pool.cap, 0);
     for (int i = 0; i < n; ++i) {
         const int sid = sessions[i];
@@ -2445,204 +2447,141 @@ int check_sessions(fac_handle* h, const P& pool, int n, const int* sessions, con
     return FAC_OK;
 }
 
-void free_codes_pool(fac_handle::CodesPool* P) {
-    if (P->lanes) { for (void* p : P->lanes->all) if (p) cudaFree(p); if (P->lanes->mel) cudaFree(P->lanes->mel); delete P->lanes; }
-    for (auto& s : P->slot) if (s.mel) cudaFree(s.mel);
-    for (void* p : {(void*)P->x_hist, (void*)P->ey_hist, (void*)P->z_held, (void*)P->carry, (void*)P->xin, (void*)P->cout})
-        if (p) cudaFree(p);
-    delete P;
-}
-
-void free_vc_pool(fac_handle::VcPool* P) {
-    if (P->lanes) { for (void* p : P->lanes->all) if (p) cudaFree(p); delete P->lanes; }
-    for (void* p : {(void*)P->g, (void*)P->codes, (void*)P->z, (void*)P->cin, (void*)P->yout}) if (p) cudaFree(p);
-    delete P;
-}
-
-// Moves the 2-layer LSTM carries (H, pass3; `words` per layer) of a batch between the sessions' slots in `carry`
-// ([slot][2 layers][words]) and the lanes' state tiles (state_h[l], state_c[l]).
-int pool_carry(fac_handle* h, uint32_t* const* state_h, float* const* state_c, uint32_t* carry, int words, int H, int pass3,
-               const std::vector<int>& slots, int to_lanes, cudaStream_t st) {
-    for (int l = 0; l < 2; ++l) {
-        LaneCarryParams p;
-        p.n = (int)slots.size(); p.H = H; p.U = lstm_units_per_cta(H); p.pass3 = pass3; p.to_lanes = to_lanes;
-        p.state_h = state_h[l]; p.state_c = state_c[l];
-        for (int b = 0; b < p.n; ++b) p.slot[b] = carry + ((size_t)slots[b] * 2 + l) * words;
-        cudaError_t e = launch_lstm2_lane_carry(p, st);
-        if (e != cudaSuccess) { h->err = std::string("pool.carry: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
-    }
-    return FAC_OK;
-}
-
-// ... the encoder-LSTM carries of a codes-pool batch.
-int codes_pool_carry(fac_handle* h, fac_handle::CodesPool& P, const std::vector<int>& slots, int to_lanes, cudaStream_t st) {
-    return pool_carry(h, P.lanes->enc_h, P.lanes->enc_c, P.carry, kCarryWords, LATENT, 1, slots, to_lanes, st);
-}
-
-// One batch of a codes-pool step: sessions slots[b] (equal codes_key) fed T samples each from x[b].
-int codes_pool_batch(fac_handle* h, fac_handle::CodesPool& P, const std::vector<int>& slots, int T, const float* const* x,
-                     int64_t* const* codes_p, int64_t* const* codes_c, int64_t* const* codes_r, cudaStream_t st) {
-    using S = fac_handle::Stream;
-    S& L = *P.lanes;
-    const int nb = (int)slots.size(), n_c = P.n_c;
-    auto sl = [&](int b) -> S& { return P.slot[slots[b]]; };
-    const S& f = sl(0);
-    const long long E = f.emitted, lo = E > kWnCtx ? E - kWnCtx : 0, N = (f.enc_samples + T) / HOP;
-    const int Fout = (int)(N - 1 - E), win = (int)(E - lo), hist = f.x_hist_len, yh = f.ey_hist_len;
+// One batch of a codes-pool step: inputs b (equal plan keys) of the step's sessions, fed T samples each from x.  The lanes'
+// mel rows hold the batch's prosody windows, from frame lo.
+int codes_pool_batch(fac_handle* h, CodesPool& P, const std::vector<int>& b, const int* sessions, const std::vector<EncPlan>& plan,
+                     const float* const* x, int64_t* const* codes_p, int64_t* const* codes_c, int64_t* const* codes_r,
+                     cudaStream_t st) {
+    EncHalf& L = P.lanes;
+    const EncPlan& p = plan[b[0]];
+    const int nb = (int)b.size(), n_c = L.n_c, T = p.T, Fout = p.Fout, win = p.win;
+    auto sl = [&](int j) -> EncHalf& { return P.slot[sessions[b[j]]]; };
     const size_t pitch = (size_t)L.mel_cap * N_MELS;
-    int rc = FAC_OK;
-    auto mv = [&](long long words, auto src, auto dst, const char* what) {
-        if (rc == FAC_OK) rc = lane_move(h, nb, words, src, dst, st, what);
-    };
-    mv(T, [&](int b) { return x[b]; }, [&](int b) { return P.xin + (size_t)b * T; }, "pool.x");
-    mv(hist, [&](int b) { return sl(b).x_hist; }, [&](int b) { return L.x_hist + (size_t)b * kEncCtx; }, "pool.x_hist");
-    mv((long long)yh * LATENT, [&](int b) { return sl(b).ey_hist; }, [&](int b) { return L.ey_hist + (size_t)b * 2 * LATENT; },
-       "pool.ey_hist");
-    if (f.enc_samples > 0)
-        mv(LATENT, [&](int b) { return sl(b).z_held; }, [&](int b) { return L.z_held + (size_t)b * LATENT; }, "pool.z_held");
-    mv((long long)win * N_MELS, [&](int b) { return sl(b).mel + (size_t)(sl(b).emitted - win) * N_MELS; },
-       [&](int b) { return L.mel + b * pitch; }, "pool.mel");
-    if (rc == FAC_OK) rc = codes_pool_carry(h, P, slots, 1, st);
-    if (rc) return rc;
-    L.B = nb; L.x_hist_len = hist; L.ey_hist_len = yh; L.enc_samples = f.enc_samples; L.emitted = E; L.enc_mode = f.enc_mode;
-    L.mel_base = lo;
-    int64_t *cp = P.cout, *cc = cp + (size_t)nb * Fout, *cr = cc + (size_t)nb * n_c * Fout;
-    rc = stream_encode_codes(h, L, P.xin, T, n_c, cp, cc, cr, st);
-    if (rc < 0) return rc;
-    rc = FAC_OK;
-    mv(L.x_hist_len, [&](int b) { return L.x_hist + (size_t)b * kEncCtx; }, [&](int b) { return sl(b).x_hist; }, "pool.x_hist");
-    mv((long long)L.ey_hist_len * LATENT, [&](int b) { return L.ey_hist + (size_t)b * 2 * LATENT; },
-       [&](int b) { return sl(b).ey_hist; }, "pool.ey_hist");
-    mv(LATENT, [&](int b) { return L.z_held + (size_t)b * LATENT; }, [&](int b) { return sl(b).z_held; }, "pool.z_held");
-    mv((long long)Fout * N_MELS, [&](int b) { return L.mel + b * pitch + (size_t)win * N_MELS; },
-       [&](int b) { return sl(b).mel + (size_t)sl(b).emitted * N_MELS; }, "pool.mel");
-    if (rc == FAC_OK) rc = codes_pool_carry(h, P, slots, 0, st);
-    mv(2LL * Fout, [&](int b) { return cp + (size_t)b * Fout; }, [&](int b) { return codes_p[b]; }, "pool.codes_p");
-    mv(2LL * n_c * Fout, [&](int b) { return cc + (size_t)b * n_c * Fout; }, [&](int b) { return codes_c[b]; }, "pool.codes_c");
-    mv(6LL * Fout, [&](int b) { return cr + (size_t)b * 3 * Fout; }, [&](int b) { return codes_r[b]; }, "pool.codes_r");
-    if (rc) return rc;
-    for (int b = 0; b < nb; ++b) {
-        S& s = sl(b);
-        s.x_hist_len = L.x_hist_len; s.ey_hist_len = L.ey_hist_len; s.enc_mode = L.enc_mode; s.n_c = n_c;
-        s.enc_samples += T; s.emitted += Fout;
-    }
-    return FAC_OK;
-}
-
-// One batch of a vc-pool step: sessions slots[b] (equal vc_key) fed F frames each.
-int vc_pool_batch(fac_handle* h, fac_handle::VcPool& P, const std::vector<int>& slots, int F, const int64_t* const* codes_p,
-                  const int64_t* const* codes_c, float* const* y, cudaStream_t st) {
-    using V = fac_handle::VcStream;
-    V& L = *P.lanes;
-    const int nb = (int)slots.size(), n_c = P.n_c, rows = n_c > 0 ? n_c : 1;
-    auto sl = [&](int b) -> V& { return P.slot[slots[b]]; };
-    const V& f = sl(0);
-    long long Zf1, Yf1;
-    vc_targets(f, F, &Zf1, &Yf1);
-    auto floor0 = [](long long v) { return v > 0 ? v : 0; };
-    const int zhist = (int)(f.Zf - floor0(f.Yf - kVcDecCtx)), k = (int)(Yf1 - f.Yf), keep = (int)(Zf1 - floor0(Yf1 - kVcDecCtx));
-    const size_t gfl = redecoder_cond_floats(h, 1), cpl = 3 * kVcCodesHist, zpl = (size_t)kVcZHist * LATENT;
-    int64_t *cp = P.cin, *cc = cp + (size_t)nb * F;
-    int rc = FAC_OK;
-    auto mv = [&](long long words, auto src, auto dst, const char* what) {
-        if (rc == FAC_OK) rc = lane_move(h, nb, words, src, dst, st, what);
-    };
-    mv((long long)gfl, [&](int b) { return sl(b).g; }, [&](int b) { return L.g + b * gfl; }, "pool.g");
-    mv(2LL * cpl, [&](int b) { return sl(b).codes; }, [&](int b) { return L.codes + b * cpl; }, "pool.codes");
-    mv((long long)zhist * LATENT, [&](int b) { return sl(b).z; }, [&](int b) { return L.z + b * zpl; }, "pool.z");
-    mv(2LL * F, [&](int b) { return codes_p[b]; }, [&](int b) { return cp + (size_t)b * F; }, "pool.codes_p");
-    mv(2LL * n_c * F, [&](int b) { return codes_c[b]; }, [&](int b) { return cc + (size_t)b * rows * F; }, "pool.codes_c");
-    if (rc) return rc;
-    L.B = nb; L.N = f.N; L.Zf = f.Zf; L.Yf = f.Yf;
-    rc = vc_step(h, L, cp, cc, rows, F, Zf1, Yf1, P.yout, st);
-    if (rc) return rc;
-    mv(2LL * cpl, [&](int b) { return L.codes + b * cpl; }, [&](int b) { return sl(b).codes; }, "pool.codes");
-    if (Zf1 > f.Zf) mv((long long)keep * LATENT, [&](int b) { return L.z + b * zpl; }, [&](int b) { return sl(b).z; }, "pool.z");
-    mv((long long)k * HOP, [&](int b) { return P.yout + (size_t)b * k * HOP; }, [&](int b) { return y[b]; }, "pool.y");
-    if (rc) return rc;
-    for (int b = 0; b < nb; ++b) {
-        V& s = sl(b);
-        long long z1, y1;
-        vc_targets(s, F, &z1, &y1);
-        s.N += F; s.Zf = z1; s.Yf = y1;
-    }
-    return FAC_OK;
-}
-
-template <typename T>
-std::vector<T> pick(const T* a, const std::vector<int>& idx) {
-    std::vector<T> out;
-    for (int i : idx) out.push_back(a[i]);
-    return out;
-}
-
-constexpr int kDecCarryWords = 1536 / 2 + 1536;   // one decoder-LSTM layer of one lane: one fp16 h plane, c
-
-// The launch-plan key of a decode-pool session that has decoded `frames` frames: its history depth.
-std::vector<long long> dec_key(long long frames) { return {frames < kDecCtx ? frames : kDecCtx}; }
-
-fac_handle::DecPool* dec_pool(fac_handle* h, int id) {
-    return h && id >= 0 && id < (int)h->dec_pools.size() ? h->dec_pools[id] : nullptr;
-}
-
-void free_dec_pool(fac_handle::DecPool* P) {
-    if (P->lanes) { for (void* p : P->lanes->all) if (p) cudaFree(p); delete P->lanes; }
-    for (void* p : {(void*)P->z_hist, (void*)P->dy_hist, (void*)P->carry, (void*)P->gb, (void*)P->yout}) if (p) cudaFree(p);
-    delete P;
-}
-
-// One batch of a decode-pool step: sessions slots[b] (equal dec_key) fed F[b] frames each, their codes and rows per lane.
-int dec_pool_batch(fac_handle* h, fac_handle::DecPool& P, const std::vector<int>& slots, const std::vector<int>& F,
-                   const int64_t* const* codes_p, const int64_t* const* codes_c, const int* n_c, const int64_t* const* codes_r,
-                   const int* n_r, float* const* y, cudaStream_t st) {
-    using S = fac_handle::Stream;
-    S& L = *P.lanes;
-    const int nb = (int)slots.size();
-    const long long frames = P.frames[slots[0]];
-    const int zh = (int)std::min(frames, 6LL), dh = (int)std::min(frames, (long long)kDecCtx);
-    const int Fmax = *std::max_element(F.begin(), F.end());
-    const size_t zpl = (size_t)6 * LATENT, dpl = (size_t)kDecCtx * 1536;
-    int rc = FAC_OK;
-    auto mv = [&](auto words, auto src, auto dst, const char* what) {
-        if (rc == FAC_OK) rc = lane_move(h, nb, words, src, dst, st, what);
-    };
-    mv((long long)zh * LATENT, [&](int b) { return P.z_hist + slots[b] * zpl; }, [&](int b) { return L.z_hist + b * zpl; }, "pool.z_hist");
-    mv((long long)dh * 1536, [&](int b) { return P.dy_hist + slots[b] * dpl; }, [&](int b) { return L.dy_hist + b * dpl; }, "pool.dy_hist");
-    if (rc == FAC_OK) rc = pool_carry(h, L.dec_h, L.dec_c, P.carry, kDecCarryWords, 1536, 0, slots, 1, st);
-    if (rc) return rc;
-    L.B = nb; L.z_hist_len = zh; L.dy_hist_len = dh; L.dec_frames = frames;
-    rc = stream_decode(h, L, F.data(), P.yout, st, [&](Ctx& c, int B) {
-        float* z = c.alloc<float>((size_t)B * Fmax * LATENT);
-        if (c.dry) return (const float*)z;
-        DeqLaneParams dp;
-        for (int i = 0; i < 6; ++i) {
-            const VqW& v = h->qw.vq[i];
-            dp.vq[i] = VqWeights{c.W(v.w_in), c.W(v.b_in), c.W(v.cb), c.W(v.cbn), c.W(v.cbn2), c.W(v.w_out), c.W(v.b_out)};
-        }
-        double codes = 0;
-        for (int b = 0; b < B; ++b) {
-            dp.codes_p[b] = codes_p[b]; dp.codes_c[b] = codes_c[b]; dp.codes_r[b] = codes_r[b];
-            dp.n_c[b] = n_c[b]; dp.n_r[b] = n_r[b]; dp.F[b] = F[b];
-            dp.gamma_beta[b] = P.gb + (size_t)slots[b] * 2048;
-            codes += (double)F[b] * (1 + n_c[b] + n_r[b]);
-        }
-        dp.outs = z; dp.n = B; dp.Fmax = Fmax;
-        c.begin("dequantize", 2.0 * codes * 8.0 * 1024, 8.0 * codes + 4.0 * 1024 * B * Fmax);
-        c.check(launch_dequantize_lanes(dp, c.st), "dequantize_lanes");
-        c.end();
-        c.tap("dec_pool.latents", z, (size_t)B * Fmax * LATENT);
-        return (const float*)z;
+    L.B = nb; L.mel_base = p.lo;
+    int rc = two_pass(h, st, [&](Ctx& c) {
+        float* xin = c.alloc<float>((size_t)nb * T);
+        int64_t* cp = c.alloc<int64_t>((size_t)nb * Fout);
+        int64_t* cc = c.alloc<int64_t>((size_t)nb * n_c * Fout);
+        int64_t* cr = c.alloc<int64_t>((size_t)nb * 3 * Fout);
+        lane_copy(c, nb, T, [&](int j) { return x[b[j]]; }, [&](int j) { return xin + (size_t)j * T; }, "pool.x");
+        lane_copy(c, nb, p.hist, [&](int j) { return sl(j).x_hist; }, [&](int j) { return L.x_hist + (size_t)j * kEncCtx; },
+                  "pool.x_hist");
+        lane_copy(c, nb, (long long)p.yh * LATENT, [&](int j) { return sl(j).ey_hist; },
+                  [&](int j) { return L.ey_hist + (size_t)j * 2 * LATENT; }, "pool.ey_hist");
+        if (!p.first)
+            lane_copy(c, nb, LATENT, [&](int j) { return sl(j).z_held; }, [&](int j) { return L.z_held + (size_t)j * LATENT; },
+                      "pool.z_held");
+        lane_copy(c, nb, (long long)win * N_MELS, [&](int j) { return sl(j).mel.get() + (size_t)(sl(j).emitted - win) * N_MELS; },
+                  [&](int j) { return L.mel.get() + j * pitch; }, "pool.mel");
+        lane_carry(c, L.lstm, LATENT, 1, nb, [&](int j) { return sl(j).carry; }, 1);
+        stream_encode_codes(c, L, p, xin, cp, cc, cr);
+        lane_copy(c, nb, p.hist1, [&](int j) { return L.x_hist + (size_t)j * kEncCtx; }, [&](int j) { return sl(j).x_hist; },
+                  "pool.x_hist");
+        lane_copy(c, nb, (long long)p.yh1 * LATENT, [&](int j) { return L.ey_hist + (size_t)j * 2 * LATENT; },
+                  [&](int j) { return sl(j).ey_hist; }, "pool.ey_hist");
+        lane_copy(c, nb, LATENT, [&](int j) { return L.z_held + (size_t)j * LATENT; }, [&](int j) { return sl(j).z_held; },
+                  "pool.z_held");
+        lane_copy(c, nb, (long long)Fout * N_MELS, [&](int j) { return L.mel.get() + j * pitch + (size_t)win * N_MELS; },
+                  [&](int j) { return sl(j).mel.get() + (size_t)sl(j).emitted * N_MELS; }, "pool.mel");
+        lane_carry(c, L.lstm, LATENT, 1, nb, [&](int j) { return sl(j).carry; }, 0);
+        lane_copy(c, nb, 2LL * Fout, [&](int j) { return cp + (size_t)j * Fout; }, [&](int j) { return codes_p[b[j]]; },
+                  "pool.codes_p");
+        lane_copy(c, nb, 2LL * n_c * Fout, [&](int j) { return cc + (size_t)j * n_c * Fout; },
+                  [&](int j) { return codes_c[b[j]]; }, "pool.codes_c");
+        lane_copy(c, nb, 6LL * Fout, [&](int j) { return cr + (size_t)j * 3 * Fout; }, [&](int j) { return codes_r[b[j]]; },
+                  "pool.codes_r");
     });
     if (rc) return rc;
-    auto nz = [&](int b) { return (long long)std::min(zh + F[b], 6) * LATENT; };
-    auto nd = [&](int b) { return (long long)std::min(dh + F[b], kDecCtx) * 1536; };
-    mv(nz, [&](int b) { return L.z_hist + b * zpl; }, [&](int b) { return P.z_hist + slots[b] * zpl; }, "pool.z_hist");
-    mv(nd, [&](int b) { return L.dy_hist + b * dpl; }, [&](int b) { return P.dy_hist + slots[b] * dpl; }, "pool.dy_hist");
-    if (rc == FAC_OK) rc = pool_carry(h, L.dec_h, L.dec_c, P.carry, kDecCarryWords, 1536, 0, slots, 0, st);
-    mv([&](int b) { return (long long)F[b] * HOP; }, [&](int b) { return P.yout + (size_t)b * Fmax * HOP; },
-       [&](int b) { return y[b]; }, "pool.y");
+    for (int j = 0; j < nb; ++j) enc_commit(sl(j), plan[b[j]], EncHalf::kCodes);
+    return FAC_OK;
+}
+
+// One batch of a vc-pool step: inputs b (equal plan keys) of the step's sessions.
+int vc_pool_batch(fac_handle* h, VcPool& P, const std::vector<int>& b, const int* sessions, const std::vector<VcPlan>& plan,
+                  const int64_t* const* codes_p, const int64_t* const* codes_c, float* const* y, cudaStream_t st) {
+    VcStream& L = P.lanes;
+    const VcPlan& p = plan[b[0]];
+    const int nb = (int)b.size(), n_c = L.n_c, rows = n_c > 0 ? n_c : 1, F = p.F;
+    auto sl = [&](int j) -> VcStream& { return P.slot[sessions[b[j]]]; };
+    const size_t gfl = redecoder_cond_floats(h, 1), cpl = 3 * kVcCodesHist, zpl = (size_t)kVcZHist * LATENT;
+    L.B = nb;
+    int rc = two_pass(h, st, [&](Ctx& c) {
+        int64_t* cp = c.alloc<int64_t>((size_t)nb * F);
+        int64_t* cc = c.alloc<int64_t>((size_t)nb * rows * F);
+        float* yout = c.alloc<float>((size_t)nb * p.k * HOP);
+        lane_copy(c, nb, (long long)gfl, [&](int j) { return sl(j).g; }, [&](int j) { return L.g + j * gfl; }, "pool.g");
+        lane_copy(c, nb, 2LL * cpl, [&](int j) { return sl(j).codes; }, [&](int j) { return L.codes + j * cpl; }, "pool.codes");
+        lane_copy(c, nb, (long long)p.zhist * LATENT, [&](int j) { return sl(j).z; }, [&](int j) { return L.z + j * zpl; }, "pool.z");
+        lane_copy(c, nb, 2LL * F, [&](int j) { return codes_p[b[j]]; }, [&](int j) { return cp + (size_t)j * F; }, "pool.codes_p");
+        lane_copy(c, nb, 2LL * n_c * F, [&](int j) { return codes_c[b[j]]; }, [&](int j) { return cc + (size_t)j * rows * F; },
+                  "pool.codes_c");
+        vc_step(c, L, p, cp, cc, rows, yout);
+        lane_copy(c, nb, 2LL * cpl, [&](int j) { return L.codes + j * cpl; }, [&](int j) { return sl(j).codes; }, "pool.codes");
+        if (p.znew > 0)
+            lane_copy(c, nb, (long long)p.zkeep * LATENT, [&](int j) { return L.z + j * zpl; }, [&](int j) { return sl(j).z; },
+                      "pool.z");
+        lane_copy(c, nb, (long long)p.k * HOP, [&](int j) { return yout + (size_t)j * p.k * HOP; }, [&](int j) { return y[b[j]]; },
+                  "pool.y");
+    });
     if (rc) return rc;
-    for (int b = 0; b < nb; ++b) P.frames[slots[b]] += F[b];
+    for (int j = 0; j < nb; ++j) vc_commit(sl(j), plan[b[j]]);
+    return FAC_OK;
+}
+
+// One batch of a decode-pool step: inputs b (equal plan keys) of the step's sessions, fed F frames each, their codes and
+// rows per lane.
+int dec_pool_batch(fac_handle* h, DecPool& P, const std::vector<int>& b, const int* sessions, const int* F_in,
+                   const int64_t* const* codes_p, const int64_t* const* codes_c, const int* n_c, const int64_t* const* codes_r,
+                   const int* n_r, float* const* y, cudaStream_t st) {
+    DecHalf& L = P.lanes;
+    const int nb = (int)b.size();
+    auto sl = [&](int j) -> DecHalf& { return P.slot[sessions[b[j]]]; };
+    const DecPlan p = dec_plan(sl(0).frames);
+    std::vector<int> F(nb);
+    for (int j = 0; j < nb; ++j) F[j] = F_in[b[j]];
+    const int Fmax = *std::max_element(F.begin(), F.end());
+    const size_t zpl = (size_t)6 * LATENT, dpl = (size_t)kDecCtx * 1536;
+    L.B = nb;
+    int rc = two_pass(h, st, [&](Ctx& c) {
+        float* yout = c.alloc<float>((size_t)nb * Fmax * HOP);
+        lane_copy(c, nb, (long long)p.zh * LATENT, [&](int j) { return sl(j).z_hist; }, [&](int j) { return L.z_hist + j * zpl; },
+                  "pool.z_hist");
+        lane_copy(c, nb, (long long)p.dh * 1536, [&](int j) { return sl(j).dy_hist; }, [&](int j) { return L.dy_hist + j * dpl; },
+                  "pool.dy_hist");
+        lane_carry(c, L.lstm, 1536, 0, nb, [&](int j) { return sl(j).carry; }, 1);
+        stream_decode(c, L, p, F.data(), yout, [&](Ctx& c, int B) {
+            float* z = c.alloc<float>((size_t)B * Fmax * LATENT);
+            if (c.dry) return (const float*)z;
+            DeqLaneParams dp;
+            for (int i = 0; i < 6; ++i) {
+                const VqW& v = h->qw.vq[i];
+                dp.vq[i] = VqWeights{c.W(v.w_in), c.W(v.b_in), c.W(v.cb), c.W(v.cbn), c.W(v.cbn2), c.W(v.w_out), c.W(v.b_out)};
+            }
+            double codes = 0;
+            for (int j = 0; j < B; ++j) {
+                const int i = b[j];
+                dp.codes_p[j] = codes_p[i]; dp.codes_c[j] = codes_c[i]; dp.codes_r[j] = codes_r[i];
+                dp.n_c[j] = n_c[i]; dp.n_r[j] = n_r[i]; dp.F[j] = F[j];
+                dp.gamma_beta[j] = sl(j).gb;
+                codes += (double)F[j] * (1 + n_c[i] + n_r[i]);
+            }
+            dp.outs = z; dp.n = B; dp.Fmax = Fmax;
+            c.begin("dequantize", 2.0 * codes * 8.0 * 1024, 8.0 * codes + 4.0 * 1024 * B * Fmax);
+            c.check(launch_dequantize_lanes(dp, c.st), "dequantize_lanes");
+            c.end();
+            c.tap("dec_pool.latents", z, (size_t)B * Fmax * LATENT);
+            return (const float*)z;
+        });
+        lane_copy(c, nb, [&](int j) { return (long long)std::min(p.zh + F[j], 6) * LATENT; },
+                  [&](int j) { return L.z_hist + j * zpl; }, [&](int j) { return sl(j).z_hist; }, "pool.z_hist");
+        lane_copy(c, nb, [&](int j) { return (long long)std::min(p.dh + F[j], kDecCtx) * 1536; },
+                  [&](int j) { return L.dy_hist + j * dpl; }, [&](int j) { return sl(j).dy_hist; }, "pool.dy_hist");
+        lane_carry(c, L.lstm, 1536, 0, nb, [&](int j) { return sl(j).carry; }, 0);
+        lane_copy(c, nb, [&](int j) { return (long long)F[j] * HOP; }, [&](int j) { return yout + (size_t)j * Fmax * HOP; },
+                  [&](int j) { return y[b[j]]; }, "pool.y");
+    });
+    if (rc) return rc;
+    for (int j = 0; j < nb; ++j) sl(j).frames += F[j];
     return FAC_OK;
 }
 }  // namespace
@@ -2650,102 +2589,77 @@ int dec_pool_batch(fac_handle* h, fac_handle::DecPool& P, const std::vector<int>
 extern "C" {
 
 int fac_codes_pool_create(fac_handle* h, int capacity, int n_c) {
-    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
-    const char* who = "fac_codes_pool_create";
+    int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER});
+    if (rc) return rc;
     if (capacity < 1 || n_c < 1 || n_c > 2) { h->err = "fac_codes_pool_create: bad arguments (capacity >= 1, 1 <= n_c <= 2)"; return FAC_ERR_INVALID; }
-    cudaSetDevice(h->device);
-    auto* P = new fac_handle::CodesPool();
-    P->cap = capacity; P->n_c = n_c;
-    P->lanes = alloc_stream(h, kLaneMax, who);
-    const size_t c = (size_t)capacity;
-    int rc = P->lanes ? FAC_OK : FAC_ERR_CUDA;
-    if (!rc) rc = dev_zeros(h, P->x_hist, c * kEncCtx, who);
-    if (!rc) rc = dev_zeros(h, P->ey_hist, c * 2 * LATENT, who);
-    if (!rc) rc = dev_zeros(h, P->z_held, c * LATENT, who);
-    if (!rc) rc = dev_zeros(h, P->carry, c * 2 * kCarryWords, who);
-    if (rc) { free_codes_pool(P); return rc; }
-    P->slot.resize(c);
-    P->used.assign(c, 0);
-    for (size_t i = 0; i < c; ++i) {
-        fac_handle::Stream& s = P->slot[i];
-        s.B = 1; s.alive = true;
-        s.x_hist = P->x_hist + i * kEncCtx; s.ey_hist = P->ey_hist + i * 2 * LATENT; s.z_held = P->z_held + i * LATENT;
-    }
-    h->codes_pools.push_back(P);
-    return (int)h->codes_pools.size() - 1;
+    return pool_create(h, &fac_handle::codes_pools, capacity, "fac_codes_pool_create", [&](Carve& m, EncHalf& s, int B, bool slot) {
+        take_enc(m, s, B, slot);
+        s.n_c = n_c;
+    });
 }
 
 int fac_codes_pool_open(fac_handle* h, int pool_id, void* stream) {
-    fac_handle::CodesPool* P = codes_pool(h, pool_id);
-    if (!P) { if (h) h->err = "fac_codes_pool_open: no such pool"; return FAC_ERR_INVALID; }
-    int i = 0;
-    while (i < P->cap && P->used[i]) ++i;
-    if (i == P->cap) { h->err = "fac_codes_pool_open: the pool is full (capacity " + std::to_string(P->cap) + ")"; return FAC_ERR_STATE; }
-    cudaSetDevice(h->device);
-    cudaError_t e = cudaMemsetAsync(P->carry + (size_t)i * 2 * kCarryWords, 0, sizeof(uint32_t) * 2 * kCarryWords, (cudaStream_t)stream);
-    if (e != cudaSuccess) { h->err = std::string("fac_codes_pool_open: ") + cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
-    fac_handle::Stream& s = P->slot[i];
-    s.enc_samples = 0; s.x_hist_len = 0; s.ey_hist_len = 0; s.emitted = 0; s.n_c = 0;
-    s.enc_mode = fac_handle::Stream::kEncNone;
-    P->used[i] = 1;
-    return i;
+    return pool_open(h, &fac_handle::codes_pools, pool_id, "fac_codes_pool_open", [&](EncHalf& s) {
+        cudaSetDevice(h->device);
+        cudaError_t e = cudaMemsetAsync(s.carry, 0, sizeof(uint32_t) * 2 * carry_words(LATENT, 1), (cudaStream_t)stream);
+        if (e != cudaSuccess) { h->err = std::string("fac_codes_pool_open: ") + cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
+        s.samples = 0; s.x_hist_len = 0; s.ey_hist_len = 0; s.emitted = 0;
+        s.mode = EncHalf::kNone;
+        return FAC_OK;
+    });
 }
 
 int fac_codes_pool_encode_codes(fac_handle* h, int pool_id, int n, const int* sessions, const int* T, const float* const* x,
                                 int64_t* const* codes_p, int64_t* const* codes_c, int64_t* const* codes_r, int* frames,
                                 void* stream) {
-    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER});
+    if (rc) return rc;
     const char* who = "fac_codes_pool_encode_codes";
-    fac_handle::CodesPool* P = codes_pool(h, pool_id);
+    CodesPool* P = by_id(h, &fac_handle::codes_pools, pool_id);
     if (!P || n < 0 || (n > 0 && (!sessions || !T || !x || !codes_p || !codes_c || !codes_r || !frames))) {
         h->err = "fac_codes_pool_encode_codes: bad arguments";
         return FAC_ERR_INVALID;
     }
-    int rc = check_sessions(h, *P, n, sessions, who);
-    if (rc) return rc;
+    if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
+    std::vector<EncPlan> plan(n);
     std::vector<std::vector<long long>> keys(n);
-    long long maxT = 0, maxF = 0, maxWin = 0;
+    int maxWin = 0;
     for (int i = 0; i < n; ++i) {
-        const fac_handle::Stream& s = P->slot[sessions[i]];
+        const EncHalf& s = P->slot[sessions[i]];
         if (!x[i] || !codes_p[i] || !codes_c[i] || !codes_r[i]) {
             h->err = "fac_codes_pool_encode_codes: null buffer of session " + std::to_string(sessions[i]);
             return FAC_ERR_INVALID;
         }
-        if ((rc = stream_encode_codes_check(h, s, T[i], P->n_c, who))) return rc;
-        keys[i] = codes_key(s.enc_samples, s.x_hist_len, s.ey_hist_len, s.emitted, T[i]);
-        maxT = std::max(maxT, (long long)T[i]); maxF = std::max(maxF, keys[i][5]); maxWin = std::max(maxWin, keys[i][7]);
+        if ((rc = stream_encode_codes_check(h, s, T[i], P->lanes.n_c, who))) return rc;
+        plan[i] = enc_plan(s, T[i]);
+        keys[i] = plan[i].key();
+        maxWin = std::max(maxWin, plan[i].Fw);
     }
     if (n == 0) return FAC_OK;
     // capacities: no session changes before every one of these has succeeded
     cudaStream_t st = (cudaStream_t)stream;
     for (int i = 0; i < n; ++i) {
-        fac_handle::Stream& s = P->slot[sessions[i]];
-        if ((rc = grow_mel(h, s, (int)((s.enc_samples + T[i]) / HOP), st))) return rc;
+        EncHalf& s = P->slot[sessions[i]];
+        if ((rc = grow_mel(h, s, 1, s.emitted, (int)((s.samples + T[i]) / HOP), st))) return rc;
     }
-    P->lanes->B = kLaneMax; P->lanes->emitted = 0;
-    if ((rc = grow_mel(h, *P->lanes, (int)maxWin, st))) return rc;
-    if ((rc = grow_buf(h, P->xin, P->xin_cap, (size_t)kLaneMax * maxT, st))) return rc;
-    if ((rc = grow_buf(h, P->cout, P->cout_cap, (size_t)kLaneMax * (4 + P->n_c) * maxF, st))) return rc;
-    for (const auto& b : pool_plan(keys, nullptr, nullptr)) {
-        rc = codes_pool_batch(h, *P, pick(sessions, b), T[b[0]], pick(x, b).data(), pick(codes_p, b).data(),
-                              pick(codes_c, b).data(), pick(codes_r, b).data(), st);
-        if (rc) return rc;
-    }
-    for (int i = 0; i < n; ++i) frames[i] = (int)keys[i][5];
+    if ((rc = grow_mel(h, P->lanes, kLaneMax, 0, maxWin, st))) return rc;
+    for (const auto& b : pool_plan(keys, nullptr, nullptr))
+        if ((rc = codes_pool_batch(h, *P, b, sessions, plan, x, codes_p, codes_c, codes_r, st))) return rc;
+    for (int i = 0; i < n; ++i) frames[i] = plan[i].Fout;
     return FAC_OK;
 }
 
 int fac_codes_pool_finish_codes(fac_handle* h, int pool_id, int n, const int* sessions, int64_t* const* codes_p,
                                 int64_t* const* codes_c, int64_t* const* codes_r, float* const* timbre, void* stream) {
-    for (int m = 0; m < 2; ++m) { int rc = check_ready(h, m); if (rc) return rc; }
+    int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER});
+    if (rc) return rc;
     const char* who = "fac_codes_pool_finish_codes";
-    fac_handle::CodesPool* P = codes_pool(h, pool_id);
+    CodesPool* P = by_id(h, &fac_handle::codes_pools, pool_id);
     if (!P || n < 0 || (n > 0 && (!sessions || !codes_p || !codes_c || !codes_r))) {
         h->err = "fac_codes_pool_finish_codes: bad arguments";
         return FAC_ERR_INVALID;
     }
-    int rc = check_sessions(h, *P, n, sessions, who);
-    if (rc) return rc;
+    if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
     for (int i = 0; i < n; ++i) {
         if (!codes_p[i] || !codes_c[i] || !codes_r[i]) {
             h->err = "fac_codes_pool_finish_codes: null buffer of session " + std::to_string(sessions[i]);
@@ -2754,129 +2668,79 @@ int fac_codes_pool_finish_codes(fac_handle* h, int pool_id, int n, const int* se
         if ((rc = stream_finish_codes_check(h, P->slot[sessions[i]], who))) return rc;
     }
     for (int i = 0; i < n; ++i) {
-        rc = stream_finish_codes(h, P->slot[sessions[i]], codes_p[i], codes_c[i], codes_r[i], timbre ? timbre[i] : nullptr, stream);
+        rc = finish_codes(h, P->slot[sessions[i]], codes_p[i], codes_c[i], codes_r[i], timbre ? timbre[i] : nullptr, stream);
         if (rc < 0) return rc;
     }
     return FAC_OK;
 }
 
 int fac_codes_pool_close(fac_handle* h, int pool_id, int session) {
-    fac_handle::CodesPool* P = codes_pool(h, pool_id);
-    if (!P || session < 0 || session >= P->cap || !P->used[session]) {
-        if (h) h->err = "fac_codes_pool_close: session " + std::to_string(session) + " is not open";
-        return FAC_ERR_INVALID;
-    }
-    P->used[session] = 0;
-    return FAC_OK;
+    return pool_close(h, &fac_handle::codes_pools, pool_id, session, "fac_codes_pool_close");
 }
 
-int fac_codes_pool_destroy(fac_handle* h, int pool_id) {
-    fac_handle::CodesPool* P = codes_pool(h, pool_id);
-    if (!P) return FAC_ERR_INVALID;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    free_codes_pool(P);
-    h->codes_pools[pool_id] = nullptr;
-    return FAC_OK;
-}
+int fac_codes_pool_destroy(fac_handle* h, int pool_id) { return free_by_id(h, &fac_handle::codes_pools, pool_id); }
 
 int fac_vc_pool_create(fac_handle* h, int capacity, int use_p_code, int use_c_code, int n_c) {
-    int rc = check_ready(h, FAC_REDECODER);
-    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
-    const char* who = "fac_vc_pool_create";
     if (capacity < 1 || n_c < 0 || n_c > 2) { h->err = "fac_vc_pool_create: bad arguments (capacity >= 1, 0 <= n_c <= 2)"; return FAC_ERR_INVALID; }
-    cudaSetDevice(h->device);
-    auto* P = new fac_handle::VcPool();
-    P->cap = capacity; P->use_p = use_p_code ? 1 : 0; P->use_c = use_c_code ? 1 : 0; P->n_c = n_c;
-    const size_t c = (size_t)capacity, gfl = redecoder_cond_floats(h, 1), cpl = 3 * kVcCodesHist, zpl = (size_t)kVcZHist * LATENT;
-    P->lanes = new fac_handle::VcStream();
-    fac_handle::VcStream& L = *P->lanes;
-    L.B = kLaneMax; L.use_p = P->use_p; L.use_c = P->use_c; L.n_c = n_c; L.alive = true;
-    rc = dev_zeros(h, L.g, kLaneMax * gfl, who);
-    L.all[0] = L.g;
-    if (!rc) { rc = dev_zeros(h, L.codes, kLaneMax * cpl, who); L.all[1] = L.codes; }
-    if (!rc) { rc = dev_zeros(h, L.z, kLaneMax * zpl, who); L.all[2] = L.z; }
-    if (!rc) rc = dev_zeros(h, P->g, c * gfl, who);
-    if (!rc) rc = dev_zeros(h, P->codes, c * cpl, who);
-    if (!rc) rc = dev_zeros(h, P->z, c * zpl, who);
-    if (rc) { free_vc_pool(P); return rc; }
-    P->slot.resize(c);
-    P->used.assign(c, 0);
-    for (size_t i = 0; i < c; ++i) {
-        fac_handle::VcStream& s = P->slot[i];
-        s.B = 1; s.use_p = P->use_p; s.use_c = P->use_c; s.n_c = n_c; s.alive = true;
-        s.g = P->g + i * gfl; s.codes = P->codes + i * cpl; s.z = P->z + i * zpl;
-    }
-    h->vc_pools.push_back(P);
-    return (int)h->vc_pools.size() - 1;
+    const size_t gfl = redecoder_cond_floats(h, 1);
+    return pool_create(h, &fac_handle::vc_pools, capacity, "fac_vc_pool_create", [&](Carve& m, VcStream& s, int B, bool) {
+        take_vc(m, s, B, gfl);
+        s.use_p = use_p_code ? 1 : 0; s.use_c = use_c_code ? 1 : 0; s.n_c = n_c;
+    });
 }
 
 int fac_vc_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER);
-    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
-    fac_handle::VcPool* P = vc_pool(h, pool_id);
-    if (!P || !timbre) { h->err = "fac_vc_pool_open: bad arguments"; return FAC_ERR_INVALID; }
-    int i = 0;
-    while (i < P->cap && P->used[i]) ++i;
-    if (i == P->cap) { h->err = "fac_vc_pool_open: the pool is full (capacity " + std::to_string(P->cap) + ")"; return FAC_ERR_STATE; }
-    fac_handle::VcStream& s = P->slot[i];
-    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { redecoder_cond(c, timbre, 1, s.g); });
-    if (rc) return rc;
-    s.N = s.Zf = s.Yf = 0;
-    s.finished = false;
-    P->used[i] = 1;
-    return i;
+    if (!timbre) { h->err = "fac_vc_pool_open: bad arguments"; return FAC_ERR_INVALID; }
+    return pool_open(h, &fac_handle::vc_pools, pool_id, "fac_vc_pool_open", [&](VcStream& s) {
+        s.N = s.Zf = s.Yf = 0;
+        s.finished = false;
+        return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { redecoder_cond(c, timbre, 1, s.g); });
+    });
 }
 
 int fac_vc_pool_convert(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
                         const int64_t* const* codes_c, const int* n_c_rows, float* const* y, int* frames, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER);
-    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
     const char* who = "fac_vc_pool_convert";
-    fac_handle::VcPool* P = vc_pool(h, pool_id);
+    VcPool* P = by_id(h, &fac_handle::vc_pools, pool_id);
     if (!P || n < 0 || (n > 0 && (!sessions || !F || !codes_p || !codes_c || !n_c_rows || !y || !frames))) {
         h->err = "fac_vc_pool_convert: bad arguments";
         return FAC_ERR_INVALID;
     }
     if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
+    std::vector<VcPlan> plan(n);
     std::vector<std::vector<long long>> keys(n);
-    long long maxF = 0, maxK = 0;
     for (int i = 0; i < n; ++i) {
-        const fac_handle::VcStream& s = P->slot[sessions[i]];
-        if (!codes_p[i] || !codes_c[i] || !y[i] || F[i] <= 0 || n_c_rows[i] < P->n_c || n_c_rows[i] > 2) {
+        const VcStream& s = P->slot[sessions[i]];
+        if (!codes_p[i] || !codes_c[i] || !y[i] || F[i] <= 0 || n_c_rows[i] < s.n_c || n_c_rows[i] > 2) {
             h->err = "fac_vc_pool_convert: bad arguments of session " + std::to_string(sessions[i]) +
                      " (F >= 1, n_c <= rows of codes_c <= 2)";
             return FAC_ERR_INVALID;
         }
         if (s.finished) { h->err = "fac_vc_pool_convert: session " + std::to_string(sessions[i]) + " was finished"; return FAC_ERR_STATE; }
-        keys[i] = vc_key(s.N, s.Zf, s.Yf, F[i]);
-        maxF = std::max(maxF, (long long)F[i]); maxK = std::max(maxK, keys[i][6]);
+        plan[i] = vc_plan(s, F[i], false);
+        keys[i] = plan[i].key();
     }
-    if (n == 0) return FAC_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = grow_buf(h, P->cin, P->cin_cap, (size_t)kLaneMax * 3 * maxF, st))) return rc;
-    if ((rc = grow_buf(h, P->yout, P->yout_cap, (size_t)kLaneMax * HOP * (maxK > 0 ? maxK : 1), st))) return rc;
-    for (const auto& b : pool_plan(keys, nullptr, nullptr)) {
-        rc = vc_pool_batch(h, *P, pick(sessions, b), F[b[0]], pick(codes_p, b).data(), pick(codes_c, b).data(), pick(y, b).data(), st);
-        if (rc) return rc;
-    }
-    for (int i = 0; i < n; ++i) frames[i] = (int)keys[i][6];
+    for (const auto& b : pool_plan(keys, nullptr, nullptr))
+        if ((rc = vc_pool_batch(h, *P, b, sessions, plan, codes_p, codes_c, y, (cudaStream_t)stream))) return rc;
+    for (int i = 0; i < n; ++i) frames[i] = plan[i].k;
     return FAC_OK;
 }
 
 int fac_vc_pool_finish(fac_handle* h, int pool_id, int n, const int* sessions, float* const* y, int* frames, void* stream) {
-    int rc = check_ready(h, FAC_REDECODER);
-    if (!rc) rc = check_ready(h, FAC_REDECODER_DECODER);
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
     const char* who = "fac_vc_pool_finish";
-    fac_handle::VcPool* P = vc_pool(h, pool_id);
+    VcPool* P = by_id(h, &fac_handle::vc_pools, pool_id);
     if (!P || n < 0 || (n > 0 && (!sessions || !y || !frames))) { h->err = "fac_vc_pool_finish: bad arguments"; return FAC_ERR_INVALID; }
     if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
     for (int i = 0; i < n; ++i) {
-        const fac_handle::VcStream& s = P->slot[sessions[i]];
+        const VcStream& s = P->slot[sessions[i]];
         if (!y[i]) { h->err = "fac_vc_pool_finish: null output of session " + std::to_string(sessions[i]); return FAC_ERR_INVALID; }
         if (s.finished || s.N == 0) {
             h->err = "fac_vc_pool_finish: session " + std::to_string(sessions[i]) + (s.finished ? " was finished" : " received no codes");
@@ -2884,96 +2748,56 @@ int fac_vc_pool_finish(fac_handle* h, int pool_id, int n, const int* sessions, f
         }
     }
     for (int i = 0; i < n; ++i) {
-        fac_handle::VcStream& s = P->slot[sessions[i]];
-        if ((rc = vc_step(h, s, nullptr, nullptr, 0, 0, s.N, s.N, y[i], stream))) return rc;
-        frames[i] = (int)(s.N - s.Yf);
-        s.Zf = s.Yf = s.N;
+        VcStream& s = P->slot[sessions[i]];
+        if ((rc = vc_run(h, s, vc_plan(s, 0, true), nullptr, nullptr, 0, y[i], stream)) < 0) return rc;
+        frames[i] = rc;
         s.finished = true;
     }
     return FAC_OK;
 }
 
 int fac_vc_pool_close(fac_handle* h, int pool_id, int session) {
-    fac_handle::VcPool* P = vc_pool(h, pool_id);
-    if (!P || session < 0 || session >= P->cap || !P->used[session]) {
-        if (h) h->err = "fac_vc_pool_close: session " + std::to_string(session) + " is not open";
-        return FAC_ERR_INVALID;
-    }
-    P->used[session] = 0;
-    return FAC_OK;
+    return pool_close(h, &fac_handle::vc_pools, pool_id, session, "fac_vc_pool_close");
 }
 
-int fac_vc_pool_destroy(fac_handle* h, int pool_id) {
-    fac_handle::VcPool* P = vc_pool(h, pool_id);
-    if (!P) return FAC_ERR_INVALID;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    free_vc_pool(P);
-    h->vc_pools[pool_id] = nullptr;
-    return FAC_OK;
-}
+int fac_vc_pool_destroy(fac_handle* h, int pool_id) { return free_by_id(h, &fac_handle::vc_pools, pool_id); }
 
 int fac_dec_pool_create(fac_handle* h, int capacity) {
-    int rc = check_ready(h, FAC_QUANTIZER);
-    if (!rc) rc = check_ready(h, FAC_DECODER);
+    int rc = check_ready(h, {FAC_QUANTIZER, FAC_DECODER});
     if (rc) return rc;
-    const char* who = "fac_dec_pool_create";
     if (capacity < 1) { h->err = "fac_dec_pool_create: bad arguments (capacity >= 1)"; return FAC_ERR_INVALID; }
-    cudaSetDevice(h->device);
-    auto* P = new fac_handle::DecPool();
-    P->cap = capacity;
-    P->lanes = alloc_stream(h, kLaneMax, who);
-    const size_t c = (size_t)capacity;
-    rc = P->lanes ? FAC_OK : FAC_ERR_CUDA;
-    if (!rc) rc = dev_zeros(h, P->z_hist, c * 6 * LATENT, who);
-    if (!rc) rc = dev_zeros(h, P->dy_hist, c * kDecCtx * 1536, who);
-    if (!rc) rc = dev_zeros(h, P->carry, c * 2 * kDecCarryWords, who);
-    if (!rc) rc = dev_zeros(h, P->gb, c * 2048, who);
-    if (rc) { free_dec_pool(P); return rc; }
-    P->frames.assign(c, 0);
-    P->used.assign(c, 0);
-    h->dec_pools.push_back(P);
-    return (int)h->dec_pools.size() - 1;
+    return pool_create(h, &fac_handle::dec_pools, capacity, "fac_dec_pool_create", take_dec);
 }
 
 int fac_dec_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream) {
-    int rc = check_ready(h, FAC_QUANTIZER);
-    if (!rc) rc = check_ready(h, FAC_DECODER);
+    int rc = check_ready(h, {FAC_QUANTIZER, FAC_DECODER});
     if (rc) return rc;
-    fac_handle::DecPool* P = dec_pool(h, pool_id);
-    if (!P || !timbre) { h->err = "fac_dec_pool_open: bad arguments"; return FAC_ERR_INVALID; }
-    int i = 0;
-    while (i < P->cap && P->used[i]) ++i;
-    if (i == P->cap) { h->err = "fac_dec_pool_open: the pool is full (capacity " + std::to_string(P->cap) + ")"; return FAC_ERR_STATE; }
-    // gamma | beta by the B = 1 launch a stream's decode_codes runs on every chunk, so the bits are the same
-    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-        const float* gb = timbre_gamma_beta(c, timbre, 1);
-        if (c.dry) return;
-        c.check_nk(cudaMemcpyAsync(P->gb + (size_t)i * 2048, gb, sizeof(float) * 2048, cudaMemcpyDeviceToDevice, c.st), "pool.gb");
-        c.check_nk(cudaMemsetAsync(P->carry + (size_t)i * 2 * kDecCarryWords, 0, sizeof(uint32_t) * 2 * kDecCarryWords, c.st),
-                   "pool.carry");
+    if (!timbre) { h->err = "fac_dec_pool_open: bad arguments"; return FAC_ERR_INVALID; }
+    return pool_open(h, &fac_handle::dec_pools, pool_id, "fac_dec_pool_open", [&](DecHalf& s) {
+        s.frames = 0;
+        // gamma | beta by the B = 1 launch a stream's decode_codes runs on every chunk, so the bits are the same
+        return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+            const float* gb = timbre_gamma_beta(c, timbre, 1);
+            if (c.dry) return;
+            c.check_nk(cudaMemcpyAsync(s.gb, gb, sizeof(float) * 2048, cudaMemcpyDeviceToDevice, c.st), "pool.gb");
+            c.check_nk(cudaMemsetAsync(s.carry, 0, sizeof(uint32_t) * 2 * carry_words(1536, 0), c.st), "pool.carry");
+        });
     });
-    if (rc) return rc;
-    P->frames[i] = 0;
-    P->used[i] = 1;
-    return i;
 }
 
 int fac_dec_pool_decode_codes(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
                               const int64_t* const* codes_c, const int* n_c_rows, const int64_t* const* codes_r,
                               const int* n_r_rows, float* const* y, void* stream) {
-    int rc = check_ready(h, FAC_QUANTIZER);
-    if (!rc) rc = check_ready(h, FAC_DECODER);
+    int rc = check_ready(h, {FAC_QUANTIZER, FAC_DECODER});
     if (rc) return rc;
     const char* who = "fac_dec_pool_decode_codes";
-    fac_handle::DecPool* P = dec_pool(h, pool_id);
+    DecPool* P = by_id(h, &fac_handle::dec_pools, pool_id);
     if (!P || n < 0 || (n > 0 && (!sessions || !F || !codes_p || !codes_c || !n_c_rows || !codes_r || !n_r_rows || !y))) {
         h->err = "fac_dec_pool_decode_codes: bad arguments";
         return FAC_ERR_INVALID;
     }
     if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
     std::vector<std::vector<long long>> keys(n);
-    int maxF = 0;
     for (int i = 0; i < n; ++i) {
         if (!codes_p[i] || !codes_c[i] || !y[i] || (n_r_rows[i] > 0 && !codes_r[i]) || n_c_rows[i] < 1 || n_c_rows[i] > 2 ||
             n_r_rows[i] < 0 || n_r_rows[i] > 3) {
@@ -2981,49 +2805,29 @@ int fac_dec_pool_decode_codes(fac_handle* h, int pool_id, int n, const int* sess
                      " (null buffer, or not 1 <= content rows <= 2, 0 <= residual rows <= 3)";
             return FAC_ERR_INVALID;
         }
-        const long long frames = P->frames[sessions[i]];
+        const long long frames = P->slot[sessions[i]].frames;
         if ((rc = stream_decode_check(h, frames, F[i], who))) return rc;
-        keys[i] = dec_key(frames);
-        maxF = std::max(maxF, F[i]);
+        keys[i] = dec_plan(frames).key();
     }
-    if (n == 0) return FAC_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = grow_buf(h, P->yout, P->yout_cap, (size_t)kLaneMax * HOP * maxF, st))) return rc;
-    for (const auto& b : pool_plan(keys, nullptr, nullptr)) {
-        rc = dec_pool_batch(h, *P, pick(sessions, b), pick(F, b), pick(codes_p, b).data(), pick(codes_c, b).data(),
-                            pick(n_c_rows, b).data(), pick(codes_r, b).data(), pick(n_r_rows, b).data(), pick(y, b).data(), st);
-        if (rc) return rc;
-    }
+    for (const auto& b : pool_plan(keys, nullptr, nullptr))
+        if ((rc = dec_pool_batch(h, *P, b, sessions, F, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, y, (cudaStream_t)stream)))
+            return rc;
     return FAC_OK;
 }
 
 int fac_dec_pool_close(fac_handle* h, int pool_id, int session) {
-    fac_handle::DecPool* P = dec_pool(h, pool_id);
-    if (!P || session < 0 || session >= P->cap || !P->used[session]) {
-        if (h) h->err = "fac_dec_pool_close: session " + std::to_string(session) + " is not open";
-        return FAC_ERR_INVALID;
-    }
-    P->used[session] = 0;
-    return FAC_OK;
+    return pool_close(h, &fac_handle::dec_pools, pool_id, session, "fac_dec_pool_close");
 }
 
-int fac_dec_pool_destroy(fac_handle* h, int pool_id) {
-    fac_handle::DecPool* P = dec_pool(h, pool_id);
-    if (!P) return FAC_ERR_INVALID;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    free_dec_pool(P);
-    h->dec_pools[pool_id] = nullptr;
-    return FAC_OK;
-}
+int fac_dec_pool_destroy(fac_handle* h, int pool_id) { return free_by_id(h, &fac_handle::dec_pools, pool_id); }
 
 int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch) {
     if (n < 0 || (n > 0 && (!counters || !lengths || !group || !batch)) || kind < 0 || kind > 2) return FAC_ERR_INVALID;
     std::vector<std::vector<long long>> keys(n);
     for (int i = 0; i < n; ++i) {
         const long long* c = counters + (size_t)i * (kind == 0 ? 4 : kind == 1 ? 3 : 1);
-        keys[i] = kind == 0 ? codes_key(c[0], (int)c[1], (int)c[2], c[3], lengths[i])
-                : kind == 1 ? vc_key(c[0], c[1], c[2], lengths[i]) : dec_key(c[0]);
+        keys[i] = kind == 0 ? enc_plan(c[0], (int)c[1], (int)c[2], c[3], lengths[i]).key()
+                : kind == 1 ? vc_plan(c[0], c[1], c[2], lengths[i], false).key() : dec_plan(c[0]).key();
     }
     return (int)pool_plan(keys, group, batch).size();
 }
@@ -3031,7 +2835,7 @@ int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* l
 long long fac_debug_lstm_lane_map(int H, int pass3, int lane, long long* pos, long long capacity) {
     const int U = lstm_units_per_cta(H);
     if (U == 0 || lane < 0 || lane >= kLaneMax) return FAC_ERR_INVALID;
-    const long long words = (long long)(pass3 ? 2 : 1) * (H / 2) + H;
+    const long long words = carry_words(H, pass3);
     if (pos && capacity >= words) lstm2_lane_map(H, U, pass3 ? 1 : 0, lane, pos);
     return words;
 }
@@ -3734,19 +3538,10 @@ int debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B
             c.check_nk(cudaMemsetAsync(s.c[l], 0, sizeof(float) * cf, c.st), "slstm.state_c");
         }
         if (carry) {
-            const int words = (pass3 ? 2 : 1) * (H / 2) + H;
-            auto move = [&](int to_lanes) {
-                for (int l = 0; l < 2 && !c.dry; ++l) {
-                    LaneCarryParams p;
-                    p.n = B; p.H = H; p.U = L.U; p.pass3 = pass3; p.to_lanes = to_lanes;
-                    p.state_h = s.h[l]; p.state_c = s.c[l];
-                    for (int b = 0; b < B; ++b) p.slot[b] = carry + ((size_t)b * 2 + l) * words;
-                    c.check(launch_lstm2_lane_carry(p, c.st), "slstm.carry");
-                }
-            };
-            move(1);
+            auto lane = [&](int b) { return carry + (size_t)b * 2 * carry_words(H, pass3); };
+            lane_carry(c, s, H, pass3, B, lane, 1);
             slstm(c, L, x, y, B, T, &s, lens);
-            move(0);
+            lane_carry(c, s, H, pass3, B, lane, 0);
             return;
         }
         for (int i = 0, t0 = 0; i < n_chunks; t0 += chunks[i++]) {
