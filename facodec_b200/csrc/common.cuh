@@ -23,6 +23,11 @@ struct PadMap {
         m.Le = (reflect && L <= mp) ? mp + 1 : L;
         return m;
     }
+    // Lane b of a batch whose lanes have their own lengths (lane_len [B], null: every lane has Tin rows): the map of the
+    // lane's own sequence, so no padded position reads a row at or past the lane's end.
+    __host__ __device__ static PadMap lane(const int* lane_len, int b, int Tin, int pad_left, int pad_right, int reflect) {
+        return make(lane_len ? lane_len[b] : Tin, pad_left, pad_right, reflect);
+    }
     __host__ __device__ __forceinline__ int src(int p) const {
         if (p >= 0 && p < L) return p;
         if (!reflect) return -1;

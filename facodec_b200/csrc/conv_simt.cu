@@ -54,7 +54,7 @@ __global__ void __launch_bounds__(2 * BN) conv_cl_kernel(ConvParams p) {
     const int co0 = blockIdx.y * BN;
 
     const float* __restrict__ xb = p.x + (size_t)b * p.x_bstride;
-    const PadMap pm = PadMap::make(p.Tin, p.pad_left, p.pad_right, p.pad_reflect);
+    const PadMap pm = PadMap::lane(p.lane_len, b, p.Tin, p.pad_left, p.pad_right, p.pad_reflect);
     const int Ktot = p.K * p.Cin;
     const bool vec_a = (p.Cin % 4) == 0;
 
@@ -240,7 +240,7 @@ __global__ void __launch_bounds__(256) conv_cout1_kernel(ConvParams p) {
     float* part = wsm + (size_t)p.K * Cin;      // [C1_TILE] partial sums of the odd pieces
     const int b = blockIdx.y, t0 = blockIdx.x * C1_TILE;
     const float* __restrict__ xb = p.x + (size_t)b * p.x_bstride;
-    const PadMap pm = PadMap::make(p.Tin, p.pad_left, p.pad_right, p.pad_reflect);
+    const PadMap pm = PadMap::lane(p.lane_len, b, p.Tin, p.pad_left, p.pad_right, p.pad_reflect);
     const int c4n = Cin / 4;
     const bool has_alpha = p.in_alpha != nullptr;
     const int total = rows * c4n;
@@ -311,7 +311,7 @@ __global__ void __launch_bounds__(256) conv_cin1_kernel(ConvParams p) {
     const int halo = (p.K - 1) * p.dil;
     const int b = blockIdx.y, t0 = blockIdx.x * C1I_T;
     const float* __restrict__ xb = p.x + (size_t)b * p.x_bstride;
-    const PadMap pm = PadMap::make(p.Tin, p.pad_left, p.pad_right, p.pad_reflect);
+    const PadMap pm = PadMap::lane(p.lane_len, b, p.Tin, p.pad_left, p.pad_right, p.pad_reflect);
     for (int i = threadIdx.x; i < C1I_T + halo; i += 256) {
         const int src = pm.src(t0 + i - p.pad_left);
         float v = src >= 0 ? __ldg(xb + (size_t)src * p.ldx) : 0.f;

@@ -187,7 +187,7 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
     if (tid == 0)
         for (int u = 0; u < S - 1 && u < units; ++u) issue_w(u);
 
-    const PadMap pm = PadMap::make(p.Tin, p.pad_left_s, p.pad_right_s, p.reflect);
+    const PadMap pm = PadMap::lane(p.lane_len, b, p.Tin, p.pad_left_s, p.pad_right_s, p.reflect);
     const float* __restrict__ xb = p.x + (size_t)b * p.x_bstride;
     auto produce = [&](int s) {              // the operand of GEMM-1 step s: chunks s*G .. s*G + G - 1
         uint8_t* ahi = abuf + (size_t)(s & 1) * a_bytes;

@@ -693,6 +693,7 @@ struct ConvOpts {
     int act = ACT_NONE;
     const float* res = nullptr;
     const int* valid_len = nullptr;
+    const int* lane_len = nullptr;   // [B] device: each lane's own input rows (a ragged batch), or null
     int transposed = 0;
     int ldx = 0;            // input row stride (0 = Cin)
     int ldy = 0;            // output row stride (0 = Cout)
@@ -750,7 +751,7 @@ void run_conv(Ctx& c, const ConvW& w, const float* x, float* y, int B, int Tin, 
             tp.res = o.res;
             tp.B = B; tp.Tin = Tin; tp.ldx = w.Cin;
             tp.PLr = o.pad_left / w.vf;
-            tp.pad_left_s = o.pad_left; tp.pad_right_s = o.pad_right; tp.reflect = o.reflect;
+            tp.pad_left_s = o.pad_left; tp.pad_right_s = o.pad_right; tp.reflect = o.reflect; tp.lane_len = o.lane_len;
             tp.Tout = Tout; tp.ldy = w.Cout;
             tp.x_bstride = (size_t)Tin * w.Cin; tp.y_bstride = (size_t)Tout * w.Cout;
             double flops = 2.0 * B * Tout * (double)w.Cout * w.K * w.Cin;
@@ -771,7 +772,7 @@ void run_conv(Ctx& c, const ConvW& w, const float* x, float* y, int B, int Tin, 
     if (o.in_snake) { p.in_alpha = c.W(o.in_snake->a); p.in_inv_alpha = c.W(o.in_snake->ia); }
     p.out_act = o.act;
     if (o.out_snake) { p.out_act = ACT_SNAKE; p.out_alpha = c.W(o.out_snake->a); p.out_inv_alpha = c.W(o.out_snake->ia); }
-    p.res = o.res; p.valid_len = o.valid_len;
+    p.res = o.res; p.valid_len = o.valid_len; p.lane_len = o.lane_len;
     p.B = B; p.Tin = Tin; p.Cin = w.Cin; p.Tout = Tout; p.Cout = w.Cout;
     p.K = w.K; p.dil = o.dil; p.stride = o.stride;
     p.pad_left = o.pad_left; p.pad_right = o.pad_right; p.pad_reflect = o.reflect;
@@ -805,7 +806,7 @@ int sconv(Ctx& c, const ConvW& w, const float* x, float* y, int B, int T, int di
 }
 
 // Whole ResidualUnit in one tensor-core launch (conv_tc_kernel<true>) when every channel fits one CTA tile.
-bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B, int T, bool causal) {
+bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B, int T, bool causal, const int* lane_len) {
     if (c.h->use_tc < 1 || !c.h->fuse_res || c.vq_critical || !r.c7.tc || !r.c1.tc || r.c7.promoted || r.c1.promoted ||
         r.c7.Cin != r.c7.Cout || r.c1.K != 1 || r.c7.vf != 1)
         return false;
@@ -830,7 +831,7 @@ bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B,
     tp.out_act = ACT_SNAKE; tp.out_alpha = c.W(r.s2.a); tp.out_inv_alpha = c.W(r.s2.ia);
     tp.B = B; tp.Tin = T; tp.ldx = r.c7.Cin;
     const int pl = causal ? k_eff - 1 : (k_eff - 1) - (k_eff - 1) / 2;
-    tp.PLr = pl; tp.pad_left_s = pl; tp.pad_right_s = k_eff - 1 - pl; tp.reflect = 1;
+    tp.PLr = pl; tp.pad_left_s = pl; tp.pad_right_s = k_eff - 1 - pl; tp.reflect = 1; tp.lane_len = lane_len;
     tp.Tout = T; tp.ldy = r.c7.Cout;
     tp.x_bstride = (size_t)T * r.c7.Cin; tp.y_bstride = (size_t)T * r.c7.Cout;
     double flops = 2.0 * B * T * (double)r.c7.Cout * r.c7.Cin * (r.c7.K + 1);
@@ -843,12 +844,14 @@ bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B,
     return true;
 }
 
-// ResidualUnit (dac.py:25-42): y = x + conv1(snake2(conv7_d(snake1(x))))
-void residual_unit(Ctx& c, const ResW& r, const float* x, float* tmp, float* y, int B, int T, bool causal = true) {
-    if (residual_unit_fused(c, r, x, y, B, T, causal)) return;
+// ResidualUnit (dac.py:25-42): y = x + conv1(snake2(conv7_d(snake1(x)))); lane_len as ConvOpts::lane_len
+void residual_unit(Ctx& c, const ResW& r, const float* x, float* tmp, float* y, int B, int T, bool causal = true,
+                   const int* lane_len = nullptr) {
+    if (residual_unit_fused(c, r, x, y, B, T, causal, lane_len)) return;
     ConvOpts o1;
     o1.in_snake = &r.s1;
     o1.out_snake = &r.s2;
+    o1.lane_len = lane_len;
     sconv(c, r.c7, x, tmp, B, T, r.dil, 1, o1, "res.conv7", causal);
     ConvOpts o2;
     o2.res = x;
@@ -911,6 +914,20 @@ void slstm(Ctx& c, const LstmW& L, const float* x, float* y, int B, int T, LstmS
     }
 }
 
+// Per-lane lengths of a ragged encode / forward: device rows of B ints (in the workspace) and their host copy.  Rows
+// kEncRows[0..4]: the encoder's input samples and the rows after each down-sampling block (the conv_out_len chain, the
+// last = latent frames); kTmRow: mel frames (samples / 300); kTqRow: code frames, min(mel, latent); kDecRow..+4: lane_rows()
+// of the decoder from the code frames.  A null Lanes* is a batch whose lanes all have its own length.
+constexpr int kTmRow = 5, kTqRow = 6, kDecRow = 7, kLaneRows = 12;
+struct Lanes {
+    const int* d = nullptr;
+    std::vector<int> h;
+    int B = 0;
+    const int* at(int row) const { return d ? d + (size_t)row * B : nullptr; }
+    const int* host(int row) const { return h.data() + (size_t)row * B; }
+};
+const int* lane_at(const Lanes* ln, int row) { return ln ? ln->at(row) : nullptr; }
+
 size_t enc_stage_floats(int B, int T) {
     // largest activation of the encoder: [B][T][64] (== [B][T/2][128])
     return (size_t)B * ((size_t)T + 16) * 64;
@@ -918,22 +935,25 @@ size_t enc_stage_floats(int B, int T) {
 
 // Encoder.forward (dac.py:69-104): x [B][T][1] -> z channels-last [B][Tz][1024] (or NCT when z_nct)
 // Encoder front: conv0 + the four EncoderBlocks (a causal FIR stack) -> features [B][ceil(T/300)][1024] in workspace.
-float* encoder_front(Ctx& c, const float* x, int B, int T, int* frames) {
+float* encoder_front(Ctx& c, const float* x, int B, int T, int* frames, const Lanes* ln = nullptr) {
     const EncW& e = c.h->enc;
     size_t stage = enc_stage_floats(B, T);
     float* buf[3] = {c.alloc<float>(stage), c.alloc<float>(stage), c.alloc<float>(stage)};
     int cur = 0;
-    int t = sconv(c, e.conv0, x, buf[0], B, T, 1, 1, ConvOpts(), "enc.conv0");
+    ConvOpts o0;
+    o0.lane_len = lane_at(ln, 0);
+    int t = sconv(c, e.conv0, x, buf[0], B, T, 1, 1, o0, "enc.conv0");
     c.tap("enc_conv0", buf[0], (size_t)B * t * 64);
     static const char* blk_names[4] = {"enc_block1", "enc_block2", "enc_block3", "enc_block4"};
     for (int i = 0; i < 4; ++i) {
         for (int j = 0; j < 3; ++j) {
             int tmp = (cur + 1) % 3, nxt = (cur + 2) % 3;
-            residual_unit(c, e.blk[i].res[j], buf[cur], buf[tmp], buf[nxt], B, t);
+            residual_unit(c, e.blk[i].res[j], buf[cur], buf[tmp], buf[nxt], B, t, true, lane_at(ln, i));
             cur = nxt;
         }
         ConvOpts o;
         o.in_snake = &e.blk[i].snake;
+        o.lane_len = lane_at(ln, i);    // a down-sampling conv reflects about the lane's own end (its "extra" follows from it)
         int nxt = (cur + 1) % 3;
         t = sconv(c, e.blk[i].down, buf[cur], buf[nxt], B, t, 1, e.blk[i].stride, o, "enc.down");
         cur = nxt;
@@ -944,16 +964,17 @@ float* encoder_front(Ctx& c, const float* x, int B, int T, int* frames) {
 }
 
 // Encoder.forward (dac.py:69-104): x [B][T][1] -> z channels-last [B][Tz][1024] (or NCT when z_nct)
-int encoder_forward(Ctx& c, const float* x, int B, int T, float* z_out, bool z_nct) {
+int encoder_forward(Ctx& c, const float* x, int B, int T, float* z_out, bool z_nct, const Lanes* ln = nullptr) {
     const EncW& e = c.h->enc;
     c.vq_critical = true;
     int t = 0;
-    float* feats = encoder_front(c, x, B, T, &t);
+    float* feats = encoder_front(c, x, B, T, &t, ln);
     float* ylstm = c.alloc<float>((size_t)B * t * LATENT);
     slstm(c, e.lstm, feats, ylstm, B, t);
     c.tap("enc_lstm", ylstm, (size_t)B * t * 1024);
     ConvOpts o;
     o.in_snake = &e.snake;
+    o.lane_len = lane_at(ln, 4);
     if (z_nct) {
         // same kernel as the channels-last path (bit-identical z), then a [B][T][C] -> [B][C][T] transpose
         float* zcl = c.alloc<float>((size_t)B * t * LATENT);
@@ -975,7 +996,9 @@ size_t decoder_stage_floats(int B, int Tf) {
     size_t first = (size_t)B * Tf * 1536;
     return first > stage ? first : stage;
 }
-void decoder_stack(Ctx& c, const DecW& d, const float* in, int in_idx, float* const* buf, int B, int Tf, float* y) {
+// lens (a ragged batch): [5][B] device, lane_rows() of d; null when every lane has Tf frames.
+void decoder_stack(Ctx& c, const DecW& d, const float* in, int in_idx, float* const* buf, int B, int Tf, float* y,
+                   const int* lens = nullptr) {
     int t = Tf;
     const float* cur_p = in;
     int cur = in_idx;
@@ -986,13 +1009,14 @@ void decoder_stack(Ctx& c, const DecW& d, const float* in, int in_idx, float* co
         ConvOpts o;
         o.in_snake = &d.blk[i].snake;
         o.pad_left = 1; o.pad_right = d.causal ? 0 : 1; o.reflect = 0;
+        o.lane_len = lens ? lens + (size_t)i * B : nullptr;
         int nxt = cur < 0 ? 0 : (cur + 1) % 3;
         run_conv(c, d.blk[i].up, cur_p, buf[nxt], B, t, t, o, "dec.up");
         cur = nxt; cur_p = buf[cur];
         t *= d.blk[i].stride;
         for (int j = 0; j < 3; ++j) {
             int tmp = (cur + 1) % 3, nx2 = (cur + 2) % 3;
-            residual_unit(c, d.blk[i].res[j], buf[cur], buf[tmp], buf[nx2], B, t, d.causal);
+            residual_unit(c, d.blk[i].res[j], buf[cur], buf[tmp], buf[nx2], B, t, d.causal, lens ? lens + (size_t)(i + 1) * B : nullptr);
             cur = nx2; cur_p = buf[cur];
         }
         c.tap(dblk_names[i], buf[cur], (size_t)B * t * d.blk[i].cout);
@@ -1000,32 +1024,72 @@ void decoder_stack(Ctx& c, const DecW& d, const float* in, int in_idx, float* co
     ConvOpts o;
     o.in_snake = &d.snake;
     o.act = ACT_TANH;
+    o.lane_len = lens ? lens + (size_t)4 * B : nullptr;
     sconv(c, d.conv_out, buf[cur], y, B, t, 1, 1, o, "dec.conv_out", d.causal);
 }
 
-void decoder_forward(Ctx& c, const DecW& d, const float* z, int B, int Tf, float* y) {
+// Rows of each lane of a ragged batch at every stage of decoder d: [5][B], row 0 the lanes' frames, row i + 1 the rows
+// after DecoderBlock i's up-sampling (300 frames in row 4).  Each conv of the stack pads a lane about its own end.
+std::vector<int> lane_rows(const DecW& d, const int* frames, int B) {
+    std::vector<int> rows((size_t)5 * B);
+    for (int b = 0; b < B; ++b) {
+        rows[b] = frames[b];
+        for (int i = 0; i < 4; ++i) rows[(size_t)(i + 1) * B + b] = rows[(size_t)i * B + b] * d.blk[i].stride;
+    }
+    return rows;
+}
+
+// Host ints -> workspace (null when v is empty).  The copy is queued on the call's stream, ahead of its kernels.
+const int* upload_ints(Ctx& c, const std::vector<int>& v) {
+    if (v.empty()) return nullptr;
+    int* d = c.alloc<int>(v.size());
+    if (!c.dry) c.check_nk(cudaMemcpyAsync(d, v.data(), sizeof(int) * v.size(), cudaMemcpyHostToDevice, c.st), "lanes.h2d");
+    return d;
+}
+
+// y [B][T]: samples [lens[b], T) of lane b set to 0, the output past a ragged lane's end.
+__global__ void zero_tails_kernel(float* __restrict__ y, const int* __restrict__ lens, int T) {
+    float* yb = y + (size_t)blockIdx.y * T;
+    for (int t = lens[blockIdx.y] + blockIdx.x * blockDim.x + threadIdx.x; t < T; t += gridDim.x * blockDim.x) yb[t] = 0.f;
+}
+void zero_tails(Ctx& c, float* y, const int* lens, int B, int T) {
+    if (c.dry || !lens) return;
+    const int blocks = std::min((T + 255) / 256, 64);
+    zero_tails_kernel<<<dim3(blocks, B), 256, 0, c.st>>>(y, lens, T);
+    c.check(cudaGetLastError(), "zero_tails");
+}
+
+void decoder_forward(Ctx& c, const DecW& d, const float* z, int B, int Tf, float* y, const int* lens = nullptr) {
     const size_t stage = decoder_stage_floats(B, Tf);
     float* buf[3] = {c.alloc<float>(stage), c.alloc<float>(stage), c.alloc<float>(stage)};
     int cur = 0;
-    int t = sconv(c, d.conv0, z, buf[0], B, Tf, 1, 1, ConvOpts(), "dec.conv0", d.causal);
+    ConvOpts o0;
+    o0.lane_len = lens;
+    int t = sconv(c, d.conv0, z, buf[0], B, Tf, 1, 1, o0, "dec.conv0", d.causal);
     c.tap("dec_conv0", buf[0], (size_t)B * t * 1536);
     if (d.has_lstm) {
         slstm(c, d.lstm, buf[0], buf[1], B, t);
         cur = 1;
         c.tap("dec_lstm", buf[1], (size_t)B * t * 1536);
     }
-    decoder_stack(c, d, buf[cur], cur, buf, B, t, y);
+    decoder_stack(c, d, buf[cur], cur, buf, B, t, y, lens);
 }
 
 constexpr int kRedCodes = 1024;   // rows of each embedding table (pack_redecoder)
 
 __global__ void embed_sum_kernel(const int64_t* __restrict__ codes_p, int cp_stride, const int64_t* __restrict__ codes_c,
                                  int cc_stride, const float* __restrict__ ep, const float* __restrict__ ec0,
-                                 const float* __restrict__ ec1, float* __restrict__ out, int T, int hidden, int use_p, int n_c) {
+                                 const float* __restrict__ ec1, float* __restrict__ out, int T, int hidden, int use_p, int n_c,
+                                 const int* __restrict__ frames) {
     // one CTA per (b, t): out[b][t][:] = [use_p] E_p[codes_p[b,0,t]] + sum_{i < n_c} E_c[i][codes_c[b,i,t]]  (redecoder.py:36-46)
     // codes_p / codes_c rows of utterance b start at b * cp_stride / b * cc_stride; content row i at + i * T.
-    // A code outside [0, kRedCodes) reads nothing and makes the frame's embedding NaN.
+    // A code outside [0, kRedCodes) reads nothing and makes the frame's embedding NaN.  frames (null: T each): frames
+    // t >= frames[b] of a ragged batch read no code and are 0.
     const int bt = blockIdx.x, b = bt / T, t = bt - b * T;
+    if (frames && t >= frames[b]) {
+        for (int c = threadIdx.x; c < hidden; c += blockDim.x) out[(size_t)bt * hidden + c] = 0.f;
+        return;
+    }
     const long long ip = use_p ? codes_p[(size_t)b * cp_stride + t] : 0;
     const long long i0 = n_c > 0 ? codes_c[(size_t)b * cc_stride + t] : 0;
     const long long i1 = n_c > 1 ? codes_c[(size_t)b * cc_stride + T + t] : 0;
@@ -1052,9 +1116,10 @@ size_t redecoder_cond_floats(const fac_handle* h, int B) { return (size_t)B * 2 
 
 // Redecoder.forward (modules/redecoder.py:35-48) after the cond layer: codes -> embeddings -> WN conditioned on g
 // (redecoder_cond) -> conv_out.  codes_p row b at codes_p + b * cp_stride, codes_c rows at codes_c + b * cc_stride + i * T
-// (int64, device); returns channels-last z [B][T][1024] in workspace.
+// (int64, device); returns channels-last z [B][T][1024] in workspace.  frames (a ragged batch): [B] device, each lane's own
+// frames, or null.
 float* redecoder_body(Ctx& c, const int64_t* codes_p, int cp_stride, const int64_t* codes_c, int cc_stride, const float* g,
-                      int B, int T, int use_p, int use_c, int n_c) {
+                      int B, int T, int use_p, int use_c, int n_c, const int* frames = nullptr) {
     const RedW& r = c.h->red;
     const int Hd = r.hidden;
     float* x = c.alloc<float>((size_t)B * T * Hd);
@@ -1065,14 +1130,16 @@ float* redecoder_body(Ctx& c, const int64_t* codes_p, int cp_stride, const int64
     float* z = c.alloc<float>((size_t)B * T * LATENT);
     if (!c.dry) {
         embed_sum_kernel<<<B * T, 128, 0, c.st>>>(codes_p, cp_stride, codes_c, cc_stride, c.W(r.emb_p), c.W(r.emb_c[0]),
-                                                  c.W(r.emb_c[1]), x, T, Hd, use_p ? 1 : 0, use_c ? n_c : 0);
+                                                  c.W(r.emb_c[1]), x, T, Hd, use_p ? 1 : 0, use_c ? n_c : 0, frames);
         c.check(cudaGetLastError(), "red.embed");
     }
     if (!c.dry) c.check_nk(cudaMemsetAsync(skip, 0, sizeof(float) * (size_t)B * T * Hd, c.st), "red.zero");
+    ConvOpts o;
+    o.lane_len = frames;
     for (int i = 0; i < r.layers; ++i) {
-        sconv(c, r.wn_in[i], x, pin, B, T, 1, 1, ConvOpts(), "red.in", false);
+        sconv(c, r.wn_in[i], x, pin, B, T, 1, 1, o, "red.in", false);
         if (!c.dry) c.check(launch_wn_gate(pin, acts, (size_t)B * T, Hd, c.st, g + (size_t)i * 2 * Hd, (size_t)T, (size_t)2 * Hd * r.layers), "red.gate");
-        sconv(c, r.wn_rs[i], acts, rs, B, T, 1, 1, ConvOpts(), "red.rs", false);
+        sconv(c, r.wn_rs[i], acts, rs, B, T, 1, 1, o, "red.rs", false);
         if (!c.dry) c.check(launch_wn_update(rs, x, skip, (size_t)B * T, Hd, i == r.layers - 1, c.st), "red.upd");
     }
     run_conv(c, r.conv_out, skip, z, B, T, T, ConvOpts(), "red.conv_out");
@@ -1082,30 +1149,31 @@ float* redecoder_body(Ctx& c, const int64_t* codes_p, int cp_stride, const int64
 // Redecoder.forward (modules/redecoder.py:35-48): codes_p [B][1][T], codes_c [B][ncc][T] int64 (device), timbre [B][1024];
 // returns channels-last z [B][T][1024] in workspace.
 float* redecoder_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes_c, int ncc, const float* timbre, int B, int T,
-                         int use_p, int use_c, int n_c) {
+                         int use_p, int use_c, int n_c, const int* frames = nullptr) {
     float* g = c.alloc<float>(redecoder_cond_floats(c.h, B));
     redecoder_cond(c, timbre, B, g);
-    return redecoder_body(c, codes_p, T, codes_c, ncc * T, g, B, T, use_p, use_c, n_c);
+    return redecoder_body(c, codes_p, T, codes_c, ncc * T, g, B, T, use_p, use_c, n_c, frames);
 }
 
 // mel [B][Tm][80] from wave [B][T] (Tm = T/300), preprocess modules/quantize.py:239-242
 struct MelW { const ConvW* dft; const ConvW* dft_tc; size_t fb; };
 // The tensor-core path: mel frames [f_first, f_first + F) of wave [B][T] (reflected at both ends of the T samples) ->
 // [B][F][80].  Frames gather + K=1 GEMM on the promoted tensor-core kernel (the mel feeds the prosody VQ: fp32-grade sums).
-float* mel_frames_tc(Ctx& c, const MelW& q, const float* wave, int B, int T, int f_first, int F) {
+float* mel_frames_tc(Ctx& c, const MelW& q, const float* wave, int B, int T, int f_first, int F, const int* lane_len = nullptr) {
     float* frames = c.alloc<float>((size_t)B * F * WIN);
     float* spec = c.alloc<float>((size_t)B * F * SPEC_TC_LD);
     float* mel = c.alloc<float>((size_t)B * F * N_MELS);
-    if (!c.dry) c.check(launch_stft_frames(wave, frames, B, T, F, HOP, WIN, N_FFT / 2 - (N_FFT - WIN) / 2, c.st, f_first), "mel.frames");
+    if (!c.dry) c.check(launch_stft_frames(wave, frames, B, T, F, HOP, WIN, N_FFT / 2 - (N_FFT - WIN) / 2, c.st, f_first, lane_len), "mel.frames");
     run_conv(c, *q.dft_tc, frames, spec, 1, B * F, B * F, ConvOpts(), "mel.dft");
     if (!c.dry) c.check(launch_mel_from_spec(spec, SPEC_TC_LD, c.W(q.fb), mel, B, F, F, c.st), "mel.fb");
     return mel;
 }
 MelW quantizer_mel(const fac_handle* h) { return MelW{&h->qw.dft, &h->qw.dft_tc, h->qw.fb}; }
-float* mel_forward(Ctx& c, const float* wave, int B, int T, int Tm, const MelW* mw = nullptr) {
+// lane_len (a ragged batch, device [B]): each lane's samples, reflected about their own ends
+float* mel_forward(Ctx& c, const float* wave, int B, int T, int Tm, const MelW* mw = nullptr, const int* lane_len = nullptr) {
     const MelW q = mw ? *mw : quantizer_mel(c.h);
     if (c.h->use_tc >= 2 && q.dft_tc->tc) {
-        float* mel = mel_frames_tc(c, q, wave, B, T, 0, Tm);
+        float* mel = mel_frames_tc(c, q, wave, B, T, 0, Tm, lane_len);
         c.tap("mel80", mel, (size_t)B * Tm * N_MELS);
         return mel;
     }
@@ -1118,6 +1186,7 @@ float* mel_forward(Ctx& c, const float* wave, int B, int T, int Tm, const MelW* 
     o.reflect = 1;
     o.no_bias = true;
     o.ldy = SPEC_LD;
+    o.lane_len = lane_len;
     run_conv(c, *q.dft, wave, spec, B, T, Tm, o, "mel.dft");
     if (!c.dry) c.check(launch_mel_from_spec(spec, SPEC_LD, c.W(q.fb), mel, B, Tm, Tm, c.st), "mel.fb");
     c.tap("mel80", mel, (size_t)B * Tm * N_MELS);
@@ -1125,7 +1194,9 @@ float* mel_forward(Ctx& c, const float* wave, int B, int T, int Tm, const MelW* 
 }
 
 // StyleEncoder.forward (modules/style_encoder.py:63-81): mel80 [B][Tm][80] -> timbre [B][1024]
-void style_encoder(Ctx& c, const float* mel, int B, int Tm, const int* vlen, float* timbre) {
+// ln (a ragged batch): lane b is the StyleEncoder of its own ln mel frames -- GLU convs zero-padded at its end, attention
+// over its own frames in the variant its own call takes, the mean over its own frames.
+void style_encoder(Ctx& c, const float* mel, int B, int Tm, const int* vlen, float* timbre, const Lanes* ln = nullptr) {
     const QuantW& q = c.h->qw;
     float* a = c.alloc<float>((size_t)B * Tm * 512);
     float* x = c.alloc<float>((size_t)B * Tm * 512);
@@ -1142,6 +1213,7 @@ void style_encoder(Ctx& c, const float* mel, int B, int Tm, const int* vlen, flo
     for (int i = 0; i < 2; ++i) {
         ConvOpts g;
         g.pad_left = 2; g.pad_right = 2; g.reflect = 0;
+        g.lane_len = lane_at(ln, kTmRow);
         run_conv(c, q.glu[i], x, y2, B, Tm, Tm, g, "se.glu");
         if (!c.dry) c.check(launch_glu_res(y2, x, B, Tm, 512, i == 1 ? vlen : nullptr, c.st), "se.glu_res");
     }
@@ -1149,12 +1221,14 @@ void style_encoder(Ctx& c, const float* mel, int B, int Tm, const int* vlen, flo
     run_conv(c, q.cq, x, qb, B, Tm, Tm, p, "se.q");
     run_conv(c, q.ck, x, kb, B, Tm, Tm, p, "se.k");
     run_conv(c, q.cv, x, vb, B, Tm, Tm, p, "se.v");
-    if (!c.dry) c.check(launch_attention(qb, kb, vb, ob, B, Tm, 2, 256, vlen, c.st, c.h->attn_stream), "se.attn");
+    if (!c.dry)
+        c.check(launch_attention(qb, kb, vb, ob, B, Tm, 2, 256, vlen, c.st, c.h->attn_stream, lane_at(ln, kTmRow),
+                                 ln ? ln->host(kTmRow) : nullptr), "se.attn");
     ConvOpts r;
     r.res = x;
     run_conv(c, q.co, ob, a, B, Tm, Tm, r, "se.o");          // a = x + conv_o(attn)
     run_conv(c, q.fc, a, y2, B, Tm, Tm, ConvOpts(), "se.fc");
-    if (!c.dry) c.check(launch_mean_pool(y2, timbre, B, Tm, 1024, vlen, c.st), "se.pool");
+    if (!c.dry) c.check(launch_mean_pool(y2, timbre, B, Tm, 1024, vlen, c.st, lane_at(ln, kTmRow)), "se.pool");
 }
 
 __global__ void lens_to_frames_kernel(const int64_t* lens, int* out, int B, int hop, int maxf) {
@@ -1188,7 +1262,7 @@ float* timbre_gamma_beta(Ctx& c, const float* timbre, int B) {
 
 // The prosody branch (modules/quantize.py:399-404): mel[:, :20] -> melspec_linear -> WN (8 causal k = 5 layers) ->
 // melspec_linear2.  mel [B][Tm][80] -> f0 [B][Tm][1024] in workspace; run with c.vq_critical set.
-float* prosody_forward(Ctx& c, const float* mel, int B, int Tm) {
+float* prosody_forward(Ctx& c, const float* mel, int B, int Tm, const int* lane_len = nullptr) {
     const QuantW& q = c.h->qw;
     float* px = c.alloc<float>((size_t)B * Tm * 256);
     float* pin = c.alloc<float>((size_t)B * Tm * 512);
@@ -1201,10 +1275,12 @@ float* prosody_forward(Ctx& c, const float* mel, int B, int Tm) {
     o.ldx = N_MELS;
     run_conv(c, lin, mel, px, B, Tm, Tm, o, "melspec_linear");
     if (!c.dry) c.check_nk(cudaMemsetAsync(skip, 0, sizeof(float) * (size_t)B * Tm * 256, c.st), "wn.zero");
+    ConvOpts ow;
+    ow.lane_len = lane_len;
     for (int i = 0; i < 8; ++i) {
-        sconv(c, q.wn_in[i], px, pin, B, Tm, 1, 1, ConvOpts(), "wn.in");
+        sconv(c, q.wn_in[i], px, pin, B, Tm, 1, 1, ow, "wn.in");
         if (!c.dry) c.check(launch_wn_gate(pin, acts, (size_t)B * Tm, 256, c.st), "wn.gate");
-        sconv(c, q.wn_rs[i], acts, rs, B, Tm, 1, 1, ConvOpts(), "wn.rs");
+        sconv(c, q.wn_rs[i], acts, rs, B, Tm, 1, 1, ow, "wn.rs");
         if (!c.dry) c.check(launch_wn_update(rs, px, skip, (size_t)B * Tm, 256, i == 7, c.st), "wn.upd");
     }
     sconv(c, q.mel_lin2, skip, f0, B, Tm, 1, 1, ConvOpts(), "melspec_linear2");
@@ -1212,12 +1288,12 @@ float* prosody_forward(Ctx& c, const float* mel, int B, int Tm) {
 }
 
 QuantFront quantizer_front(Ctx& c, const float* wave, int B, int T, const float* full_waves, int T_full, const int64_t* wave_lens,
-                           float* timbre) {
+                           float* timbre, const Lanes* ln = nullptr) {
     const int Tm = T / HOP;
     const bool was_critical = c.vq_critical;
     c.vq_critical = true;      // quantizer-side layers are tiny: all of them use the promoted kernel
     // --- timbre ---
-    float* mel = mel_forward(c, wave, B, T, Tm);
+    float* mel = mel_forward(c, wave, B, T, Tm, nullptr, lane_at(ln, 0));
     float* timbre_ws = c.alloc<float>((size_t)B * 1024);
     if (!timbre) timbre = timbre_ws;
     if (full_waves) {
@@ -1230,10 +1306,10 @@ QuantFront quantizer_front(Ctx& c, const float* wave, int B, int T, const float*
         }
         style_encoder(c, melf, B, Tmf, vlen, timbre);
     } else {
-        style_encoder(c, mel, B, Tm, nullptr, timbre);
+        style_encoder(c, mel, B, Tm, nullptr, timbre, ln);
     }
     float* gb = timbre_gamma_beta(c, timbre, B);
-    float* f0 = prosody_forward(c, mel, B, Tm);
+    float* f0 = prosody_forward(c, mel, B, Tm, lane_at(ln, kTmRow));
     c.tap("f0_input", f0, (size_t)B * Tm * 1024);
     c.vq_critical = was_critical;
     QuantFront fr;
@@ -1245,12 +1321,12 @@ QuantFront quantizer_front(Ctx& c, const float* wave, int B, int T, const float*
 QuantOut quantizer_forward(Ctx& c, const float* z_cl, const float* wave, int B, int T, int Tz, int n_c,
                            const float* full_waves, int T_full, const int64_t* wave_lens, float* losses2,
                            float* timbre, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, bool want_parts,
-                           const QuantFront* pre = nullptr) {
+                           const QuantFront* pre = nullptr, const Lanes* ln = nullptr) {
     const QuantW& q = c.h->qw;
     const int Tm = T / HOP;
     const int Tq = Tm < Tz ? Tm : Tz;
     c.vq_critical = true;
-    QuantFront fr = pre ? *pre : quantizer_front(c, wave, B, T, full_waves, T_full, wave_lens, timbre);
+    QuantFront fr = pre ? *pre : quantizer_front(c, wave, B, T, full_waves, T_full, wave_lens, timbre, ln);
     float* gb = fr.gb;
     float* f0 = fr.f0;
     // --- fused per-frame VQ + AdaLN ---
@@ -1320,12 +1396,47 @@ QuantOut dequantize_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes
     return out;
 }
 
+// dequantize_forward for a ragged batch (no parts): lane b reads frames [0, frames[b]) of its codes (rows T apart; host
+// frames) and its frames past them are 0.  Each frame is dequantize_kernel's, bit for bit, in launches of <= 32 lanes.
+QuantOut dequantize_lanes_forward(Ctx& c, const int64_t* codes_p, const int64_t* codes_c, int n_c, const int64_t* codes_r,
+                                  int n_r, const float* timbre, int B, int T, const int* frames) {
+    const QuantW& q = c.h->qw;
+    float* gb = timbre_gamma_beta(c, timbre, B);
+    QuantOut out = {};
+    out.Tq = T;
+    out.outs_cl = c.alloc<float>((size_t)B * T * 1024);
+    if (c.dry) return out;
+    DeqLaneParams dp;
+    for (int i = 0; i < 6; ++i) {
+        const VqW& v = q.vq[i];
+        dp.vq[i] = VqWeights{c.W(v.w_in), c.W(v.b_in), c.W(v.cb), c.W(v.cbn), c.W(v.cbn2), c.W(v.w_out), c.W(v.b_out)};
+    }
+    dp.Fmax = T; dp.ld = T;
+    for (int b0 = 0; b0 < B; b0 += kLaneMax) {
+        dp.n = std::min(B - b0, kLaneMax);
+        double codes = 0;
+        for (int j = 0; j < dp.n; ++j) {
+            const size_t b = (size_t)(b0 + j);
+            dp.codes_p[j] = codes_p + b * T; dp.codes_c[j] = codes_c + b * n_c * T;
+            dp.codes_r[j] = n_r ? codes_r + b * n_r * T : nullptr;
+            dp.n_c[j] = n_c; dp.n_r[j] = n_r; dp.F[j] = frames[b];
+            dp.gamma_beta[j] = gb + b * 2048;
+            codes += (double)frames[b] * (1 + n_c + n_r);
+        }
+        dp.outs = out.outs_cl + (size_t)b0 * T * 1024;
+        c.begin("dequantize", 2.0 * codes * 8.0 * 1024, 8.0 * codes + 4.0 * 1024 * dp.n * T);
+        c.check(launch_dequantize_lanes(dp, c.st), "dequantize_lanes");
+        c.end();
+    }
+    return out;
+}
+
 // Runs the waveform-only half of the quantizer on the handle's side stream, forked after whatever the main stream has
 // queued so far (the input copy) and joined by the caller with join_front() before fa_quantize.
-bool fork_front(Ctx& c, QuantFront& fr, const float* wave, int B, int T, float* timbre) {
+bool fork_front(Ctx& c, QuantFront& fr, const float* wave, int B, int T, float* timbre, const Lanes* ln = nullptr) {
     fac_handle* h = c.h;
     if (!h->overlap_front || h->profiling) { return false; }
-    if (c.dry) { fr = quantizer_front(c, wave, B, T, nullptr, 0, nullptr, timbre); return true; }
+    if (c.dry) { fr = quantizer_front(c, wave, B, T, nullptr, 0, nullptr, timbre, ln); return true; }
     if (!h->side) {
         if (cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
@@ -1339,7 +1450,7 @@ bool fork_front(Ctx& c, QuantFront& fr, const float* wave, int B, int T, float* 
     c.check_nk(cudaEventRecord(h->ev_fork, main_st), "front.fork");
     c.check_nk(cudaStreamWaitEvent(h->side, h->ev_fork, 0), "front.fork_wait");
     c.st = h->side;
-    fr = quantizer_front(c, wave, B, T, nullptr, 0, nullptr, timbre);
+    fr = quantizer_front(c, wave, B, T, nullptr, 0, nullptr, timbre, ln);
     c.check_nk(cudaEventRecord(h->ev_join, h->side), "front.join");
     c.st = main_st;
     return true;
@@ -1526,17 +1637,71 @@ int fac_quantize(fac_handle* h, const float* z, const float* wave, int B, int T,
 namespace {
 // The compress half of reconstruct.py:56-61: encoder -> quantizer(n_c), with the waveform-only quantizer front forked
 // beside the encoder.  Returns the channels-last AdaLN output the decoder reads.
+// ln: a ragged batch (null: every lane has T samples).
 QuantOut codec_encode(Ctx& c, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r,
-                      float* timbre) {
+                      float* timbre, const Lanes* ln = nullptr) {
     int Tz = fac_encode_frames(T);
     float* zcl = c.alloc<float>((size_t)B * Tz * LATENT);
     float* timbre_buf = timbre ? timbre : c.alloc<float>((size_t)B * 1024);
     QuantFront fr;
-    const bool forked = fork_front(c, fr, x, B, T, timbre_buf);
-    encoder_forward(c, x, B, T, zcl, false);
+    const bool forked = fork_front(c, fr, x, B, T, timbre_buf, ln);
+    encoder_forward(c, x, B, T, zcl, false, ln);
     if (forked) join_front(c);
     return quantizer_forward(c, zcl, x, B, T, Tz, n_c, nullptr, 0, nullptr, nullptr, timbre_buf, codes_p, codes_c, codes_r,
-                             false, forked ? &fr : nullptr);
+                             false, forked ? &fr : nullptr, ln);
+}
+
+// The lanes of a ragged encode of B lanes of lens[b] samples (kLaneRows rows, see Lanes), uploaded by the caller's Ctx.
+std::vector<int> encode_lane_rows(const DecW& d, const int* lens, int B) {
+    static const int rates[4] = {2, 5, 5, 6};
+    std::vector<int> rows((size_t)kLaneRows * B);
+    std::vector<int> tq(B);
+    for (int b = 0; b < B; ++b) {
+        rows[b] = lens[b];
+        for (int i = 0; i < 4; ++i) rows[(size_t)(i + 1) * B + b] = conv_out_len(rows[(size_t)i * B + b], 2 * rates[i], rates[i]);
+        rows[(size_t)kTmRow * B + b] = lens[b] / HOP;
+        tq[b] = std::min(lens[b] / HOP, rows[(size_t)4 * B + b]);
+        rows[(size_t)kTqRow * B + b] = tq[b];
+    }
+    const std::vector<int> dec = lane_rows(d, tq.data(), B);
+    std::copy(dec.begin(), dec.end(), rows.begin() + (size_t)kDecRow * B);
+    return rows;
+}
+Lanes upload_lanes(Ctx& c, const std::vector<int>& rows, int B) {
+    Lanes l;
+    l.h = rows; l.B = B;
+    l.d = upload_ints(c, rows);
+    return l;
+}
+
+// codes [B][rows][T]: codes t >= frames[b] of lane b set to -1 (past a ragged lane's end)
+__global__ void code_tails_kernel(int64_t* __restrict__ codes, const int* __restrict__ frames, int rows, int T) {
+    const int b = blockIdx.y;
+    int64_t* cb = codes + (size_t)b * rows * T;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < rows * T; i += gridDim.x * blockDim.x)
+        if (i % T >= frames[b]) cb[i] = -1;
+}
+void code_tails(Ctx& c, int64_t* codes, const int* frames, int B, int rows, int T) {
+    if (c.dry || !frames || !codes) return;
+    code_tails_kernel<<<dim3(std::min((rows * T + 255) / 256, 64), B), 256, 0, c.st>>>(codes, frames, rows, T);
+    c.check(cudaGetLastError(), "code_tails");
+}
+
+// Per-lane counts of a ragged call (host, B entries): each must lie in [lo, hi].  A batch whose every lane has hi is the
+// call without counts, launch for launch, so `counts` is cleared for it.
+int lane_counts(fac_handle* h, const int*& counts, int B, int lo, int hi, const char* who) {
+    if (!counts) return FAC_OK;
+    bool full = true;
+    for (int b = 0; b < B; ++b) {
+        if (counts[b] < lo || counts[b] > hi) {
+            h->err = std::string(who) + ": lane " + std::to_string(b) + " has " + std::to_string(counts[b]) + ", outside [" +
+                     std::to_string(lo) + ", " + std::to_string(hi) + "]";
+            return FAC_ERR_INVALID;
+        }
+        full = full && counts[b] == hi;
+    }
+    if (full) counts = nullptr;
+    return FAC_OK;
 }
 
 // Arguments of the decode-from-codes entry points: 1 prosody row, 1..2 content rows, 0..3 residual rows (codes_r unread
@@ -1550,24 +1715,51 @@ bool bad_codes_args(const int64_t* codes_p, const int64_t* codes_c, int n_c_rows
 
 extern "C" {
 
-int fac_codec_forward(fac_handle* h, const float* x, int B, int T, int n_c, float* y, int64_t* codes_p,
-                      int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream) {
+int fac_codec_forward_lens(fac_handle* h, const float* x, int B, int T, const int* lengths, int n_c, float* y, int64_t* codes_p,
+                           int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream) {
     if (int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER, FAC_DECODER})) return rc;
     if (!x || !y || B <= 0 || T <= N_FFT / 2 || n_c < 1 || n_c > 2) { h->err = "fac_codec_forward: bad arguments"; return FAC_ERR_INVALID; }
+    if (int rc = lane_counts(h, lengths, B, N_FFT / 2 + 1, T, "fac_codec_forward_lens: lengths")) return rc;
+    const std::vector<int> rows = lengths ? encode_lane_rows(h->dec, lengths, B) : std::vector<int>();
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-        QuantOut o = codec_encode(c, x, B, T, n_c, codes_p, codes_c, codes_r, timbre);
-        decoder_forward(c, h->dec, o.outs_cl, B, o.Tq, y);
+        const Lanes ln = upload_lanes(c, rows, B);
+        const Lanes* lp = lengths ? &ln : nullptr;
+        QuantOut o = codec_encode(c, x, B, T, n_c, codes_p, codes_c, codes_r, timbre, lp);
+        decoder_forward(c, h->dec, o.outs_cl, B, o.Tq, y, lane_at(lp, kDecRow));
+        zero_tails(c, y, lane_at(lp, kDecRow + 4), B, o.Tq * HOP);
+        code_tails(c, codes_p, lane_at(lp, kTqRow), B, 1, o.Tq);
+        code_tails(c, codes_c, lane_at(lp, kTqRow), B, n_c, o.Tq);
+        code_tails(c, codes_r, lane_at(lp, kTqRow), B, 3, o.Tq);
     });
 }
 
-int fac_codec_encode(fac_handle* h, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
-                     int64_t* codes_r, float* timbre, void* stream) {
+int fac_codec_forward(fac_handle* h, const float* x, int B, int T, int n_c, float* y, int64_t* codes_p,
+                      int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream) {
+    return fac_codec_forward_lens(h, x, B, T, nullptr, n_c, y, codes_p, codes_c, codes_r, timbre, stream);
+}
+
+int fac_codec_encode_lens(fac_handle* h, const float* x, int B, int T, const int* lengths, int n_c, int64_t* codes_p,
+                          int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream) {
     if (int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER})) return rc;
     if (!x || !codes_p || !codes_c || !codes_r || B <= 0 || T <= N_FFT / 2 || n_c < 1 || n_c > 2) {
         h->err = "fac_codec_encode: bad arguments";
         return FAC_ERR_INVALID;
     }
-    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { codec_encode(c, x, B, T, n_c, codes_p, codes_c, codes_r, timbre); });
+    if (int rc = lane_counts(h, lengths, B, N_FFT / 2 + 1, T, "fac_codec_encode_lens: lengths")) return rc;
+    const std::vector<int> rows = lengths ? encode_lane_rows(h->dec, lengths, B) : std::vector<int>();
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        const Lanes ln = upload_lanes(c, rows, B);
+        const Lanes* lp = lengths ? &ln : nullptr;
+        QuantOut o = codec_encode(c, x, B, T, n_c, codes_p, codes_c, codes_r, timbre, lp);
+        code_tails(c, codes_p, lane_at(lp, kTqRow), B, 1, o.Tq);
+        code_tails(c, codes_c, lane_at(lp, kTqRow), B, n_c, o.Tq);
+        code_tails(c, codes_r, lane_at(lp, kTqRow), B, 3, o.Tq);
+    });
+}
+
+int fac_codec_encode(fac_handle* h, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
+                     int64_t* codes_r, float* timbre, void* stream) {
+    return fac_codec_encode_lens(h, x, B, T, nullptr, n_c, codes_p, codes_c, codes_r, timbre, stream);
 }
 
 int fac_dequantize(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
@@ -1588,18 +1780,28 @@ int fac_dequantize(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c
     });
 }
 
-int fac_codes_decode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
-                     int n_r_rows, const float* timbre, int B, int T, float* y, void* stream) {
+int fac_codes_decode_lens(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
+                          int n_r_rows, const float* timbre, int B, int T, const int* frames, float* y, void* stream) {
     int rc = check_ready(h, {FAC_QUANTIZER, FAC_DECODER});
     if (rc) return rc;
     if (!y || bad_codes_args(codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T)) {
         h->err = "fac_codes_decode: bad arguments (1 <= content rows <= 2, 0 <= residual rows <= 3)";
         return FAC_ERR_INVALID;
     }
+    if ((rc = lane_counts(h, frames, B, 1, T, "fac_codes_decode_lens: frames"))) return rc;
+    const std::vector<int> rows = frames ? lane_rows(h->dec, frames, B) : std::vector<int>();
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-        QuantOut o = dequantize_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T, false);
-        decoder_forward(c, h->dec, o.outs_cl, B, T, y);
+        const int* lens = upload_ints(c, rows);
+        QuantOut o = frames ? dequantize_lanes_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T, frames)
+                            : dequantize_forward(c, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T, false);
+        decoder_forward(c, h->dec, o.outs_cl, B, T, y, lens);
+        zero_tails(c, y, lens ? lens + (size_t)4 * B : nullptr, B, T * HOP);
     });
+}
+
+int fac_codes_decode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
+                     int n_r_rows, const float* timbre, int B, int T, float* y, void* stream) {
+    return fac_codes_decode_lens(h, codes_p, codes_c, n_c_rows, codes_r, n_r_rows, timbre, B, T, nullptr, y, stream);
 }
 
 int fac_codec_forward_host(fac_handle* h, const float* x_host, int B, int T, int n_c, float* y_host,
@@ -1664,18 +1866,27 @@ int fac_redecoder_decode(fac_handle* h, const float* z, int B, int Tf, float* y,
     });
 }
 
-int fac_voice_convert(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre, int B,
-                      int T, int use_p_code, int use_c_code, int n_c, float* y, void* stream) {
+int fac_voice_convert_lens(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre,
+                           int B, int T, int use_p_code, int use_c_code, int n_c, const int* frames, float* y, void* stream) {
     int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
     if (!codes_p || !codes_c || !timbre || !y || B <= 0 || T <= 0 || n_c < 0 || n_c > 2 || n_c > n_c_rows) {
         h->err = "fac_voice_convert: bad arguments";
         return FAC_ERR_INVALID;
     }
+    if ((rc = lane_counts(h, frames, B, 1, T, "fac_voice_convert_lens: frames"))) return rc;
+    const std::vector<int> rows = frames ? lane_rows(h->dec2, frames, B) : std::vector<int>();
     return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-        float* zcl = redecoder_forward(c, codes_p, codes_c, n_c_rows, timbre, B, T, use_p_code, use_c_code, n_c);
-        decoder_forward(c, h->dec2, zcl, B, T, y);
+        const int* lens = upload_ints(c, rows);
+        float* zcl = redecoder_forward(c, codes_p, codes_c, n_c_rows, timbre, B, T, use_p_code, use_c_code, n_c, lens);
+        decoder_forward(c, h->dec2, zcl, B, T, y, lens);
+        zero_tails(c, y, lens ? lens + (size_t)4 * B : nullptr, B, T * HOP);
     });
+}
+
+int fac_voice_convert(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre, int B,
+                      int T, int use_p_code, int use_c_code, int n_c, float* y, void* stream) {
+    return fac_voice_convert_lens(h, codes_p, codes_c, n_c_rows, timbre, B, T, use_p_code, use_c_code, n_c, nullptr, y, stream);
 }
 
 // ---- streaming (SURVEY.md 8f rank 4): chunked encoder / decoder with LSTM-state carry and conv halos ----
@@ -3830,6 +4041,19 @@ int fac_debug_pad_map(int L, int pad_left, int pad_right, int reflect, int* out,
     if (!out || L < 0 || pad_left < 0 || pad_right < 0 || n != pad_left + L + pad_right) return FAC_ERR_INVALID;
     const PadMap pm = PadMap::make(L, pad_left, pad_right, reflect);
     for (int i = 0; i < n; ++i) out[i] = pm.src(i - pad_left);
+    return FAC_OK;
+}
+
+// Host-only: the same map for every lane of a batch of B lanes with their own lengths, as the conv kernels build it
+// (PadMap::lane): out[b * n + i] = source row of padded position i - pad_left of lane b, n = pad_left + Tin + pad_right.
+int fac_debug_lane_pad_map(const int* lane_len, int B, int Tin, int pad_left, int pad_right, int reflect, int* out, int n) {
+    if (!out || B <= 0 || Tin < 0 || pad_left < 0 || pad_right < 0 || n != pad_left + Tin + pad_right) return FAC_ERR_INVALID;
+    for (int b = 0; lane_len && b < B; ++b)
+        if (lane_len[b] < 0 || lane_len[b] > Tin) return FAC_ERR_INVALID;
+    for (int b = 0; b < B; ++b) {
+        const PadMap pm = PadMap::lane(lane_len, b, Tin, pad_left, pad_right, reflect);
+        for (int i = 0; i < n; ++i) out[(size_t)b * n + i] = pm.src(i - pad_left);
+    }
     return FAC_OK;
 }
 

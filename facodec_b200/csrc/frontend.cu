@@ -51,9 +51,10 @@ __global__ void __launch_bounds__(128) mel_from_spec_kernel(const float* __restr
 // window of the utterance with f_first > 0: it only asks for a frame that reaches past a window edge when that edge is the
 // utterance's true start or end, so the reflection is the offline one.
 __global__ void __launch_bounds__(256) stft_frames_kernel(const float* __restrict__ wave, float* __restrict__ frames, int T,
-                                                          int F, int f_first, int hop, int win, int pad) {
+                                                          int F, int f_first, int hop, int win, int pad,
+                                                          const int* __restrict__ lane_len) {
     const int b = blockIdx.y, f = blockIdx.x;
-    const PadMap pm = PadMap::make(T, pad, pad, 1);
+    const PadMap pm = PadMap::lane(lane_len, b, T, pad, pad, 1);
     const float* w = wave + (size_t)b * T;
     float* o = frames + ((size_t)b * F + f) * win;
     for (int j = threadIdx.x; j < win; j += blockDim.x) {
@@ -62,9 +63,9 @@ __global__ void __launch_bounds__(256) stft_frames_kernel(const float* __restric
     }
 }
 cudaError_t launch_stft_frames(const float* wave, float* frames, int B, int T, int F, int hop, int win, int pad, cudaStream_t st,
-                               int f_first) {
+                               int f_first, const int* lane_len) {
     if (B <= 0 || F <= 0) return cudaSuccess;
-    stft_frames_kernel<<<dim3(F, B), 256, 0, st>>>(wave, frames, T, F, f_first, hop, win, pad);
+    stft_frames_kernel<<<dim3(F, B), 256, 0, st>>>(wave, frames, T, F, f_first, hop, win, pad, lane_len);
     return cudaGetLastError();
 }
 

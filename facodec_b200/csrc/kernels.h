@@ -15,6 +15,7 @@ struct ConvParams {
     const float* out_inv_alpha = nullptr;
     const float* res = nullptr;        // residual, same layout as y, or null
     const int* valid_len = nullptr;    // [B] rows >= valid_len[b] are written as 0, or null
+    const int* lane_len = nullptr;     // [B] input rows of each lane (PadMap::lane), or null: Tin for every lane
     float* y = nullptr;                // [B][Tout][ldy] (or [B][Cout][Tout] when y_transposed)
     int B = 0, Tin = 0, Cin = 0, Tout = 0, Cout = 0;
     int K = 1, dil = 1, stride = 1, pad_left = 0, pad_right = 0, pad_reflect = 0;
@@ -40,6 +41,7 @@ struct TcConvParams {
     int vf = 1;                        // samples per A row (down-conv stride; 1 otherwise)
     int Kr = 1, dil = 1, PLr = 0;      // taps / dilation / left pad, in rows
     int pad_left_s = 0, pad_right_s = 0, reflect = 0;   // sample-level padding (PadMap)
+    const int* lane_len = nullptr;     // [B] input samples of each lane (PadMap::lane), or null: Tin for every lane
     int Tout = 0, Cout = 0, ldy = 0;
     int out_act = 0;
     int promoted = 0;                  // 1 = promoted accumulation, windows into a master in shared memory (upstream of the VQ)
@@ -129,9 +131,10 @@ cudaError_t lstm_read_phase_clocks(long long* out4);   // CTA-0 accumulated phas
 
 // ---- mel front-end (frontend.cu) -----------------------------------------------------------
 // spec [B][F][ldspec] (re at 2*bin, im at 2*bin+1) -> mel [B][Tm][80] = (log(1e-5 + |.|^2 fb)+4)/4
-// frames [f_first, f_first + F) of the centred STFT of wave [B][T], reflected at both ends of the T samples
+// frames [f_first, f_first + F) of the centred STFT of wave [B][T], reflected at both ends of the T samples (lane_len [B]
+// device: at both ends of lane b's own lane_len[b] samples)
 cudaError_t launch_stft_frames(const float* wave, float* frames /*[B][F][win]*/, int B, int T, int F, int hop, int win, int pad,
-                               cudaStream_t st, int f_first = 0);
+                               cudaStream_t st, int f_first = 0, const int* lane_len = nullptr);
 cudaError_t launch_mel_from_spec(const float* spec, int ldspec, const float* fb /*[1025][80]*/, float* mel,
                                  int B, int F, int Tm, cudaStream_t st);
 
@@ -176,7 +179,8 @@ struct DeqParams {
 };
 cudaError_t launch_dequantize(const DeqParams& p, cudaStream_t st);
 // the same per lane of a decode-pool batch (n <= 32 lanes): lane b reads codes_p[b] [1][F[b]], codes_c[b] [n_c[b]][F[b]],
-// codes_r[b] [n_r[b]][F[b]] and gamma_beta[b] [2048], and writes outs [n][Fmax][1024] (frames t >= F[b] zero)
+// codes_r[b] [n_r[b]][F[b]] and gamma_beta[b] [2048], and writes outs [n][Fmax][1024] (frames t >= F[b] zero).  ld > 0:
+// every lane's code rows are ld codes apart instead of F[b] (lanes of one [B][rows][ld] tensor, a ragged offline batch).
 struct DeqLaneParams {
     const int64_t* codes_p[32];
     const int64_t* codes_c[32];
@@ -185,7 +189,7 @@ struct DeqLaneParams {
     int n_c[32], n_r[32], F[32];
     VqWeights vq[6];
     float* outs = nullptr;
-    int n = 0, Fmax = 0;
+    int n = 0, Fmax = 0, ld = 0;
 };
 cudaError_t launch_dequantize_lanes(const DeqLaneParams& p, cudaStream_t st);
 // losses[0] = commitment, losses[1] = codebook (identical in forward), from sqerr
@@ -230,9 +234,15 @@ cudaError_t launch_wn_gate(const float* xin, float* acts, size_t n_rows, int hid
                            size_t rows_per_utt = 0, size_t g_stride = 0);
 cudaError_t launch_wn_update(const float* rs, float* x, float* out, size_t n_rows, int hidden, int last, cudaStream_t st);
 cudaError_t launch_glu_res(const float* y, float* x, int B, int T, int C, const int* valid_len, cudaStream_t st);  // x = x + y1*sig(y2) (masked)
+// lane_len (a ragged batch; device [B], with its host copy lane_len_host): lane b is the attention of its own first lane_len[b]
+// rows, as a call with T = lane_len[b] computes it, bit for bit, in the variant that call takes; its other rows of o are 0.
 cudaError_t launch_attention(const float* q, const float* k, const float* v, float* o, int B, int T, int heads,
-                             int dk, const int* valid_len, cudaStream_t st, int force_stream = 0);
-cudaError_t launch_mean_pool(const float* x, float* out, int B, int T, int C, const int* valid_len, cudaStream_t st);
+                             int dk, const int* valid_len, cudaStream_t st, int force_stream = 0, const int* lane_len = nullptr,
+                             const int* lane_len_host = nullptr);
+// mean over T frames (sum over all T / valid_len[b] when valid_len); lane_len [B] device: lane b's first lane_len[b] frames
+// only, summed as a call with T = lane_len[b] sums them
+cudaError_t launch_mean_pool(const float* x, float* out, int B, int T, int C, const int* valid_len, cudaStream_t st,
+                             const int* lane_len = nullptr);
 cudaError_t launch_fill_u32(unsigned int* p, unsigned int v, size_t n, cudaStream_t st);
 
 // alias-free activation (alias_free_torch/act.py:24-29): up x2 -> snake-beta/identity -> down x2

@@ -9,6 +9,8 @@
 // registers (32 per lane), the 1024->8 projection is a warp-shuffle reduction, the 1024-way
 // argmin is lane-strided with a (score, index) shuffle reduction (ties -> lowest index, like
 // torch.max on CPU), and the 8->1024 out-projection updates the residual in place.
+#include <algorithm>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -305,7 +307,7 @@ __global__ void __launch_bounds__(128) dequantize_lanes_kernel(DeqLaneParams p) 
         for (int i = lane; i < VQ_D; i += 32) out[i] = 0.f;
         return;
     }
-    dequantize_frame(p.vq, p.codes_p[b] + t, p.codes_c[b] + t, p.n_c[b], p.codes_r[b] + t, p.n_r[b], (size_t)F,
+    dequantize_frame(p.vq, p.codes_p[b] + t, p.codes_c[b] + t, p.n_c[b], p.codes_r[b] + t, p.n_r[b], (size_t)(p.ld ? p.ld : F),
                      p.gamma_beta[b], out, nullptr, nullptr, nullptr, lane);
 }
 
@@ -595,24 +597,34 @@ cudaError_t launch_glu_res(const float* y, float* x, int B, int T, int C, const 
 }
 
 // MultiHeadAttention.attention (modules/attentions.py:168-199, window_size=None): per (b, head),
-// 16 queries per CTA; K then V tiles of 32 rows staged in shared memory.
+// 16 queries per CTA; K then V tiles of 32 rows staged in shared memory.  Lanes of a ragged batch (lane_len, device [B]) are
+// attended over their own first lane_len[b] rows with the loop bounds a call of that length has, so each is bit-identical
+// to it; a kernel serves lane b when its own call would take that variant: lane_len[b] <= stored_max here, > stored_max in
+// attention_stream_kernel.  ld = row pitch of the score block (>= every served lane's length).
 constexpr int ATT_Q = 16;
 constexpr int ATT_DK = 256;
 __global__ void __launch_bounds__(256) attention_kernel(const float* __restrict__ q, const float* __restrict__ k,
                                                         const float* __restrict__ v, float* __restrict__ o, int T,
-                                                        int heads, const int* __restrict__ valid_len) {
+                                                        int heads, const int* __restrict__ valid_len,
+                                                        const int* __restrict__ lane_len, int stored_max, int ld) {
     extern __shared__ __align__(16) float sm[];
     float* qs = sm;                              // [16][256]
     float* tile = qs + ATT_Q * ATT_DK;           // [32][257]
-    float* sc = tile + 32 * (ATT_DK + 1);        // [16][T]
+    float* sc = tile + 32 * (ATT_DK + 1);        // [16][ld]
     const int C = heads * ATT_DK;
     const int bh = blockIdx.y, b = bh / heads, h = bh % heads;
     const int q0 = blockIdx.x * ATT_Q;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int Tb = T;                            // rows per utterance of the batch: addressing only
+    if (lane_len) {
+        if (lane_len[b] > stored_max) return;    // attention_stream_kernel's lane
+        T = lane_len[b];
+        if (q0 >= T) return;
+    }
     const int vlen = valid_len ? valid_len[b] : T;
-    const float* qb = q + (size_t)b * T * C + h * ATT_DK;
-    const float* kb = k + (size_t)b * T * C + h * ATT_DK;
-    const float* vb = v + (size_t)b * T * C + h * ATT_DK;
+    const float* qb = q + (size_t)b * Tb * C + h * ATT_DK;
+    const float* kb = k + (size_t)b * Tb * C + h * ATT_DK;
+    const float* vb = v + (size_t)b * Tb * C + h * ATT_DK;
     for (int i = tid; i < ATT_Q * ATT_DK; i += 256) {
         int qi = i / ATT_DK, d = i % ATT_DK;
         int t = q0 + qi;
@@ -637,7 +649,7 @@ __global__ void __launch_bounds__(256) attention_kernel(const float* __restrict_
             int s = s0 + lane;
             if (s < T) {
                 bool ok = (q0 + qi < vlen) && (s < vlen);
-                sc[qi * T + s] = ok ? acc : -1e4f;
+                sc[qi * ld + s] = ok ? acc : -1e4f;
             }
         }
     }
@@ -646,7 +658,7 @@ __global__ void __launch_bounds__(256) attention_kernel(const float* __restrict_
 #pragma unroll
     for (int qq = 0; qq < 2; ++qq) {
         int qi = warp * 2 + qq;
-        float* row = sc + qi * T;
+        float* row = sc + qi * ld;
         float mx = -3.0e38f;
         for (int s = lane; s < T; s += 32) mx = fmaxf(mx, row[s]);
 #pragma unroll
@@ -679,7 +691,7 @@ __global__ void __launch_bounds__(256) attention_kernel(const float* __restrict_
             const float* vr = tile + s * (ATT_DK + 1);
 #pragma unroll
             for (int qq = 0; qq < 2; ++qq) {
-                float pw = sc[(warp * 2 + qq) * T + s0 + s];
+                float pw = sc[(warp * 2 + qq) * ld + s0 + s];
 #pragma unroll
                 for (int j = 0; j < 8; ++j) acc[qq][j] = fmaf(pw, vr[lane + 32 * j], acc[qq][j]);
             }
@@ -689,7 +701,7 @@ __global__ void __launch_bounds__(256) attention_kernel(const float* __restrict_
     for (int qq = 0; qq < 2; ++qq) {
         int t = q0 + warp * 2 + qq;
         if (t < T) {
-            float* ob = o + ((size_t)b * T + t) * C + h * ATT_DK;
+            float* ob = o + ((size_t)b * Tb + t) * C + h * ATT_DK;
 #pragma unroll
             for (int j = 0; j < 8; ++j) ob[lane + 32 * j] = acc[qq][j];
         }
@@ -702,7 +714,8 @@ __global__ void __launch_bounds__(256) attention_kernel(const float* __restrict_
 // the rescaling round-off (~1e-7 relative).
 __global__ void __launch_bounds__(256) attention_stream_kernel(const float* __restrict__ q, const float* __restrict__ k,
                                                                const float* __restrict__ v, float* __restrict__ o, int T,
-                                                               int heads, const int* __restrict__ valid_len) {
+                                                               int heads, const int* __restrict__ valid_len,
+                                                               const int* __restrict__ lane_len, int stored_max) {
     extern __shared__ __align__(16) float sm[];
     float* qs = sm;                              // [16][256]
     float* tile = qs + ATT_Q * ATT_DK;           // [32][257]
@@ -711,10 +724,16 @@ __global__ void __launch_bounds__(256) attention_stream_kernel(const float* __re
     const int bh = blockIdx.y, b = bh / heads, h = bh % heads;
     const int q0 = blockIdx.x * ATT_Q;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int Tb = T;                            // rows per utterance of the batch: addressing only
+    if (lane_len) {
+        if (lane_len[b] <= stored_max) return;   // attention_kernel's lane
+        T = lane_len[b];
+        if (q0 >= T) return;
+    }
     const int vlen = valid_len ? valid_len[b] : T;
-    const float* qb = q + (size_t)b * T * C + h * ATT_DK;
-    const float* kb = k + (size_t)b * T * C + h * ATT_DK;
-    const float* vb = v + (size_t)b * T * C + h * ATT_DK;
+    const float* qb = q + (size_t)b * Tb * C + h * ATT_DK;
+    const float* kb = k + (size_t)b * Tb * C + h * ATT_DK;
+    const float* vb = v + (size_t)b * Tb * C + h * ATT_DK;
     for (int i = tid; i < ATT_Q * ATT_DK; i += 256) {
         int qi = i / ATT_DK, d = i % ATT_DK;
         int t = q0 + qi;
@@ -786,38 +805,56 @@ __global__ void __launch_bounds__(256) attention_stream_kernel(const float* __re
     for (int qq = 0; qq < 2; ++qq) {
         int t = q0 + warp * 2 + qq;
         if (t < T) {
-            float* ob = o + ((size_t)b * T + t) * C + h * ATT_DK;
+            float* ob = o + ((size_t)b * Tb + t) * C + h * ATT_DK;
 #pragma unroll
             for (int j = 0; j < 8; ++j) ob[lane + 32 * j] = acc[qq][j];
         }
     }
 }
+static size_t attention_smem(int T) { return sizeof(float) * ((size_t)ATT_Q * ATT_DK + 32 * (ATT_DK + 1) + (size_t)ATT_Q * T); }
 cudaError_t launch_attention(const float* q, const float* k, const float* v, float* o, int B, int T, int heads, int dk,
-                             const int* valid_len, cudaStream_t st, int force_stream) {
+                             const int* valid_len, cudaStream_t st, int force_stream, const int* lane_len,
+                             const int* lane_len_host) {
     if (dk != ATT_DK) return cudaErrorInvalidValue;
     if (B <= 0 || T <= 0) return cudaSuccess;
     if ((long long)B * heads > 65535) return cudaErrorInvalidValue;
-    size_t smem = sizeof(float) * ((size_t)ATT_Q * ATT_DK + 32 * (ATT_DK + 1) + (size_t)ATT_Q * T);
-    dim3 grid((T + ATT_Q - 1) / ATT_Q, B * heads);
-    if (smem > 200 * 1024 || force_stream) {
-        smem = sizeof(float) * ((size_t)ATT_Q * ATT_DK + 32 * (ATT_DK + 1) + (size_t)ATT_Q * 32);
+    if ((lane_len != nullptr) != (lane_len_host != nullptr)) return cudaErrorInvalidValue;
+    // the longest sequence whose score block fits (the variant a call of that length takes)
+    int stored_max = force_stream ? 0 : T;
+    while (stored_max > 0 && attention_smem(stored_max) > 200 * 1024) --stored_max;
+    int Ts = 0, Tr = 0;                          // longest lane of each variant
+    for (int b = 0; lane_len_host && b < B; ++b) {
+        const int L = lane_len_host[b];
+        if (L <= stored_max) Ts = std::max(Ts, L); else Tr = std::max(Tr, L);
+    }
+    if (!lane_len_host) (T <= stored_max ? Ts : Tr) = T;
+    else if (cudaMemsetAsync(o, 0, sizeof(float) * (size_t)B * T * heads * ATT_DK, st) != cudaSuccess) return cudaGetLastError();
+    if (Tr > 0) {
+        const size_t smem = sizeof(float) * ((size_t)ATT_Q * ATT_DK + 32 * (ATT_DK + 1) + (size_t)ATT_Q * 32);
         cudaError_t e = cudaFuncSetAttribute(attention_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        attention_stream_kernel<<<grid, 256, smem, st>>>(q, k, v, o, T, heads, valid_len);
-        return cudaGetLastError();
+        attention_stream_kernel<<<dim3((Tr + ATT_Q - 1) / ATT_Q, B * heads), 256, smem, st>>>(q, k, v, o, T, heads, valid_len,
+                                                                                            lane_len, stored_max);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
-    cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    attention_kernel<<<grid, 256, smem, st>>>(q, k, v, o, T, heads, valid_len);
-    return cudaGetLastError();
+    if (Ts > 0) {
+        const size_t smem = attention_smem(Ts);
+        cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        attention_kernel<<<dim3((Ts + ATT_Q - 1) / ATT_Q, B * heads), 256, smem, st>>>(q, k, v, o, T, heads, valid_len, lane_len,
+                                                                                     stored_max, Ts);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 // StyleEncoder.temporal_avg_pool (modules/style_encoder.py:83-91): sum over ALL frames / len
 __global__ void mean_pool_kernel(const float* __restrict__ x, float* __restrict__ out, int T, int C,
-                                 const int* __restrict__ valid_len) {
+                                 const int* __restrict__ valid_len, const int* __restrict__ lane_len) {
     int b = blockIdx.y, c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
     const float* xb = x + (size_t)b * T * C + c;
+    if (lane_len) T = lane_len[b];               // a ragged lane: its own frames, as a call of that length sums them
     float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
     int t = 0;
     for (; t + 3 < T; t += 4) {
@@ -830,10 +867,11 @@ __global__ void mean_pool_kernel(const float* __restrict__ x, float* __restrict_
     float len = (float)(valid_len ? valid_len[b] : T);
     out[(size_t)b * C + c] = ((a0 + a1) + (a2 + a3)) / len;
 }
-cudaError_t launch_mean_pool(const float* x, float* out, int B, int T, int C, const int* valid_len, cudaStream_t st) {
+cudaError_t launch_mean_pool(const float* x, float* out, int B, int T, int C, const int* valid_len, cudaStream_t st,
+                             const int* lane_len) {
     if (B <= 0) return cudaSuccess;
     dim3 grid((C + 127) / 128, B);
-    mean_pool_kernel<<<grid, 128, 0, st>>>(x, out, T, C, valid_len);
+    mean_pool_kernel<<<grid, 128, 0, st>>>(x, out, T, C, valid_len, lane_len);
     return cudaGetLastError();
 }
 

@@ -13,6 +13,7 @@ Drop-in contract (SURVEY.md section 8b):
 * There is no CPU fallback: CPU tensors or a missing library raise.
 """
 import ctypes
+import operator
 import os
 from collections import OrderedDict
 
@@ -180,12 +181,45 @@ def _engine_inputs(engine, tensors):
                                 % (engine.device_index, t.device))
 
 
-def _codes_args(codes, timbre, check_devices):
+def _int_list(values, what):
+    """Per-lane counts of a ragged batch, given as a sequence of ints or a 1-D integer tensor, read on the host once: a
+    list of ints.  Anything else raises ValueError."""
+    if isinstance(values, torch.Tensor):
+        if values.dim() != 1 or values.is_floating_point() or values.is_complex() or values.dtype == torch.bool:
+            raise ValueError("%s must be a 1-D integer tensor; got %s %s" % (what, values.dtype, tuple(values.shape)))
+        values = values.tolist()
+    try:
+        values = list(values)
+        vals = [operator.index(v) for v in values]
+    except TypeError:
+        raise ValueError("%s must hold integers" % what) from None
+    if any(isinstance(v, bool) for v in values):
+        raise ValueError("%s must hold integers, not booleans" % what)
+    return vals
+
+
+def _lane_counts(values, B, lo, hi, what):
+    """_int_list(values), checked to hold B counts in [lo, hi] (ValueError otherwise)."""
+    vals = _int_list(values, what)
+    if len(vals) != B:
+        raise ValueError("%s holds %d values for a batch of %d" % (what, len(vals), B))
+    for b, v in enumerate(vals):
+        if not lo <= v <= hi:
+            raise ValueError("%s[%d] = %d lies outside [%d, %d]" % (what, b, v, lo, hi))
+    return vals
+
+
+def _c_ints(vals):
+    return None if vals is None else (ctypes.c_int * len(vals))(*vals)
+
+
+def _codes_args(codes, timbre, check_devices, frames=None):
     """Validates the inputs of the decode-from-codes calls: ``codes`` = [codes_p [B,1,T], codes_c [B,1|2,T], codes_r
     [B,0..3,T] or None] integer tensors and ``timbre`` [B,1024]; ``check_devices`` raises FacError for tensors off the
     engine's device.  Returns (codes_p, codes_c, codes_r or None, residual rows, timbre, B, T) ready for the C call.
     Out-of-range codes raise IndexError, as F.embedding does in the reference; that check is one device reduction and
-    one host synchronisation."""
+    one host synchronisation.  ``frames`` (a ragged batch, see _lane_counts) must hold B counts in [1, T], and only codes
+    below each lane's count are checked."""
     if not isinstance(codes, (list, tuple)) or len(codes) != 3 or codes[0] is None or codes[1] is None or timbre is None:
         raise ValueError("codes must be [codes_p, codes_c, codes_r or None] and timbre a [B, 1024] tensor")
     check_devices([t for t in (*codes, timbre) if t is not None])
@@ -203,8 +237,14 @@ def _codes_args(codes, timbre, check_devices):
         raise ValueError("timbre must be [%d, 1024], got %s" % (B, tuple(timbre.shape)))
     if cr is not None and cr.shape[1] == 0:
         cr = None
-    present = [t for t in (cp, cc, cr) if t is not None]
-    if bool(torch.stack([((t < 0) | (t >= 1024)).any() for t in present]).any()):
+    live = None
+    if frames is not None:
+        counts = torch.tensor(_lane_counts(frames, B, 1, T, "frames"), dtype=torch.int64).to(cp.device)
+        live = torch.arange(T, device=cp.device).view(1, 1, T) < counts.view(B, 1, 1)
+    bad = [(t < 0) | (t >= 1024) for t in (cp, cc, cr) if t is not None]
+    if live is not None:
+        bad = [m & live for m in bad]
+    if bool(torch.stack([m.any() for m in bad]).any()):
         raise IndexError("codes must lie in [0, 1024)")
     return cp, cc, cr, 0 if cr is None else cr.shape[1], _f32c(timbre), B, T
 
@@ -363,8 +403,12 @@ class Codec:
         self.model = model
         self.engine = model.encoder._engine
 
-    def forward(self, x, n_c=2):
-        """x [B,1,T] on the GPU -> (y [B,1,T'], [codes_p, codes_c, codes_r], timbre)."""
+    def forward(self, x, n_c=2, lengths=None):
+        """x [B,1,T] on the GPU -> (y [B,1,T'], [codes_p, codes_c, codes_r], timbre).
+        lengths: a batch of utterances of different lengths -- B sample counts in (1024, T] (ints or a 1-D integer
+        tensor).  Utterance b is x[b, :, :lengths[b]]: its F_b = min(lengths[b] // 300, fac_encode_frames(lengths[b]))
+        code frames, timbre and 300 F_b samples are bit-identical to its own B = 1 call; codes past F_b are -1 (a decode
+        without frames rejects them) and y past 300 F_b is 0.  Samples past lengths[b] are never read."""
         e = self.engine
         for m in (self.model.encoder, self.model.quantizer, self.model.decoder):
             if m.training:
@@ -372,6 +416,7 @@ class Codec:
         e.sync_weights(x.device)
         x = _f32c(x)
         B, _, T = x.shape
+        lanes = _c_ints(None if lengths is None else _lane_counts(lengths, B, 1025, T, "lengths"))
         Tq = min(T // 300, e.L.fac_encode_frames(T))
         dev = x.device
         y = torch.empty(B, 1, Tq * 300, device=dev)
@@ -379,13 +424,14 @@ class Codec:
         cc = torch.empty(B, n_c, Tq, device=dev, dtype=torch.int64)
         cr = torch.empty(B, 3, Tq, device=dev, dtype=torch.int64)
         timbre = torch.empty(B, 1024, device=dev)
-        rc = e.L.fac_codec_forward(e.handle, _ptr(x), B, T, n_c, _ptr(y), _ptr(cp), _ptr(cc), _ptr(cr), _ptr(timbre), _stream(dev))
+        rc = e.L.fac_codec_forward_lens(e.handle, _ptr(x), B, T, lanes, n_c, _ptr(y), _ptr(cp), _ptr(cc), _ptr(cr), _ptr(timbre),
+                                        _stream(dev))
         _lib.check(e.handle, rc, "fac_codec_forward")
         return y, [cp, cc, cr], timbre
 
-    def encode(self, x, n_c=2):
+    def encode(self, x, n_c=2, lengths=None):
         """Compress only: x [B,1,T] on the GPU -> ([codes_p, codes_c, codes_r], timbre), bit-identical to what forward()
-        returns, without running the decoder."""
+        returns, without running the decoder.  lengths: per-utterance sample counts, as forward() takes them."""
         e = self.engine
         for m in (self.model.encoder, self.model.quantizer):
             if m.training:
@@ -393,28 +439,36 @@ class Codec:
         e.sync_weights(x.device)
         x = _f32c(x)
         B, _, T = x.shape
+        lanes = _c_ints(None if lengths is None else _lane_counts(lengths, B, 1025, T, "lengths"))
         Tq = min(T // 300, e.L.fac_encode_frames(T))
         dev = x.device
         cp = torch.empty(B, 1, Tq, device=dev, dtype=torch.int64)
         cc = torch.empty(B, n_c, Tq, device=dev, dtype=torch.int64)
         cr = torch.empty(B, 3, Tq, device=dev, dtype=torch.int64)
         timbre = torch.empty(B, 1024, device=dev)
-        rc = e.L.fac_codec_encode(e.handle, _ptr(x), B, T, n_c, _ptr(cp), _ptr(cc), _ptr(cr), _ptr(timbre), _stream(dev))
+        rc = e.L.fac_codec_encode_lens(e.handle, _ptr(x), B, T, lanes, n_c, _ptr(cp), _ptr(cc), _ptr(cr), _ptr(timbre),
+                                       _stream(dev))
         _lib.check(e.handle, rc, "fac_codec_encode")
         return [cp, cc, cr], timbre
 
-    def decode(self, codes, timbre):
+    def decode(self, codes, timbre, frames=None):
         """Decompress: codes ([codes_p, codes_c, codes_r] as forward()/encode() return them, or codefile.DACFile.unpack();
         codes_r may have 0..3 rows or be None) + timbre [B,1024] on the GPU -> y [B,1,300*T].  A timbre from another
         utterance gives that voice (FAquantizer.from_codes).  Out-of-range codes raise IndexError (one device reduction +
-        one host sync)."""
+        one host sync).
+        frames: a batch of utterances of different lengths -- B frame counts in [1, T] (ints or a 1-D integer tensor).
+        Utterance b is codes[..., :frames[b]]: its samples are bit-identical to its own B = 1 decode, codes past its end
+        are neither read nor checked, and y[b, 0, 300 * frames[b]:] is 0."""
         if self.model.decoder.training:
             raise NotImplementedError("eval mode only")
-        cp, cc, cr, n_r, tv, B, T = _codes_args(codes, timbre, lambda ts: self.model.quantizer._prep(*ts))
+        frames = None if frames is None else _int_list(frames, "frames")
+        cp, cc, cr, n_r, tv, B, T = _codes_args(codes, timbre, lambda ts: self.model.quantizer._prep(*ts), frames)
         e = self.engine
         dev = cp.device
         y = torch.empty(B, 1, T * 300, device=dev)
-        rc = e.L.fac_codes_decode(e.handle, _ptr(cp), _ptr(cc), cc.shape[1], _ptr(cr), n_r, _ptr(tv), B, T, _ptr(y), _stream(dev))
+        lanes = _c_ints(frames)
+        rc = e.L.fac_codes_decode_lens(e.handle, _ptr(cp), _ptr(cc), cc.shape[1], _ptr(cr), n_r, _ptr(tv), B, T, lanes,
+                                       _ptr(y), _stream(dev))
         _lib.check(e.handle, rc, "fac_codes_decode")
         return y
 
@@ -588,15 +642,18 @@ class VoiceConverter:
         self.model = model
         self.engine = model.encoder._engine
 
-    def convert(self, codes, timbre, use_p_code=False, use_c_code=True, n_c=1):
+    def convert(self, codes, timbre, use_p_code=False, use_c_code=True, n_c=1, frames=None):
         """codes[0] [B,1,T], codes[1] [B,1|2,T] (codes[2] is not read), timbre [B,1024] -> y [B,1,300 T].  Codes outside
-        [0, 1024) raise IndexError, as F.embedding does (one device reduction + one host sync)."""
+        [0, 1024) raise IndexError, as F.embedding does (one device reduction + one host sync).  frames: utterances of
+        different lengths in one batch, as Codec.decode takes them; each is bit-identical to its own B = 1 convert."""
         e = self.engine
-        cp, cc, _, _, tv, B, T = _codes_args([codes[0], codes[1], None], timbre, lambda ts: _engine_inputs(e, ts))
+        frames = None if frames is None else _int_list(frames, "frames")
+        cp, cc, _, _, tv, B, T = _codes_args([codes[0], codes[1], None], timbre, lambda ts: _engine_inputs(e, ts), frames)
         dev = cp.device
         y = torch.empty(B, 1, T * 300, device=dev)
-        rc = e.L.fac_voice_convert(e.handle, _ptr(cp), _ptr(cc), cc.shape[1], _ptr(tv), B, T, int(bool(use_p_code)),
-                                   int(bool(use_c_code)), int(n_c), _ptr(y), _stream(dev))
+        lanes = _c_ints(frames)
+        rc = e.L.fac_voice_convert_lens(e.handle, _ptr(cp), _ptr(cc), cc.shape[1], _ptr(tv), B, T, int(bool(use_p_code)),
+                                        int(bool(use_c_code)), int(n_c), lanes, _ptr(y), _stream(dev))
         _lib.check(e.handle, rc, "fac_voice_convert")
         return y
 

@@ -96,6 +96,16 @@ int fac_codec_forward_host(fac_handle* h, const float* x_host, int B, int T, int
  * codes_c [B,n_c,Tq], codes_r [B,3,Tq] int64 are required; timbre [B,1024] may be NULL. */
 int fac_codec_encode(fac_handle* h, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
                      int64_t* codes_r, float* timbre, void* stream);
+/* Ragged batches: fac_codec_forward_lens and fac_codec_encode_lens take lengths, a HOST array of B sample counts in
+ * (1024, T] (NULL: T each).  Lane b computes x[b, 0, :lengths[b]] exactly as its own B = 1 call does, bit for bit: its
+ * F_b = min(lengths[b] / 300, fac_encode_frames(lengths[b])) code frames, timbre and 300 * F_b samples.  Outputs keep the
+ * shapes of the call without lengths; codes past F_b are -1 and y past 300 * F_b is 0.  Samples past a lane's length are
+ * never read.  A length out of range is FAC_ERR_INVALID before anything is queued; lengths that all equal T make the
+ * call without them. */
+int fac_codec_forward_lens(fac_handle* h, const float* x, int B, int T, const int* lengths, int n_c, float* y,
+                           int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream);
+int fac_codec_encode_lens(fac_handle* h, const float* x, int B, int T, const int* lengths, int n_c, int64_t* codes_p,
+                          int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream);
 
 /* Decompress.  The reference has no single call for it (FAquantizer.decode, modules/quantize.py:245-254, needs the
  * timbre quantizer that timbre_norm = True leaves out); it is ResidualVectorQuantize.from_codes (dac/nn/quantize.py:200-220:
@@ -111,6 +121,12 @@ int fac_dequantize(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c
                    int n_r_rows, const float* timbre, int B, int T, float* outs, float* zp, float* zc, float* zr, void* stream);
 int fac_codes_decode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
                      int n_r_rows, const float* timbre, int B, int T, float* y, void* stream);
+/* Ragged batches: fac_codes_decode_lens and fac_voice_convert_lens take frames, a HOST array of B frame counts in [1, T]
+ * (NULL: T each).  Lane b decodes its first frames[b] frames exactly as its own B = 1 call on codes[..., :frames[b]] does,
+ * bit for bit; codes past them are neither read nor checked, and y[b, 0, 300 * frames[b]:] is 0.  A count out of range is
+ * FAC_ERR_INVALID before anything is queued.  Counts that all equal T make the call without them. */
+int fac_codes_decode_lens(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
+                          int n_r_rows, const float* timbre, int B, int T, const int* frames, float* y, void* stream);
 
 /* Voice conversion (reconstruct_redecoder.py:108-122, webui.py:68-81).
  * fac_redecode = model.encoder(p_code, c_code, timbre, use_p_code, use_c_code, n_c) of the redecoder model,
@@ -125,6 +141,8 @@ int fac_redecode(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, 
 int fac_redecoder_decode(fac_handle* h, const float* z, int B, int Tf, float* y, void* stream);
 int fac_voice_convert(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre,
                       int B, int T, int use_p_code, int use_c_code, int n_c, float* y, void* stream);
+int fac_voice_convert_lens(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const float* timbre,
+                           int B, int T, int use_p_code, int use_c_code, int n_c, const int* frames, float* y, void* stream);
 
 /* Voice conversion in chunks, bit-identical to fac_voice_convert on the whole utterance.  The redecoder and its decoder are
  * non-causal but hold no LSTM, so the output needs a fixed look-ahead and no recurrent state.  z frame t reads codes

@@ -82,6 +82,10 @@ long long fac_debug_lstm_lane_map(int H, int pass3, int lane, long long* pos, lo
  * (dac/model/encodec.py:96-113 pad1d incl. the short-input branch): out[i] = source row of padded position
  * i - pad_left, or -1 where the padded value is zero; n must be pad_left + L + pad_right. */
 int fac_debug_pad_map(int L, int pad_left, int pad_right, int reflect, int* out, int n);
+/* Host-only: that map for each lane of a ragged batch, as the conv kernels build it from per-lane lengths: lane b (of B)
+ * pads its own lane_len[b] <= Tin rows (lane_len NULL: Tin each).  out [B][n], n = pad_left + Tin + pad_right; positions
+ * past the lane's own padded length hold rows the lane's outputs never read, each -1 or below lane_len[b]. */
+int fac_debug_lane_pad_map(const int* lane_len, int B, int Tin, int pad_left, int pad_right, int reflect, int* out, int n);
 /* Host-only (no GPU, no handle): the tile plan of the wgmma conv kernel for one layer geometry.  mode: 0 TF32,
  * 1 promoted TF32, 2 bf16, 3 promoted fp16 hi + scaled lo, 4 fused ResidualUnit bf16, 5 fused TF32, 6 mode 3 in the
  * transposed formulation, 7 ONE fp16 pass (the k = 7 convs downstream of the VQ), 8 fused ResidualUnit with its k = 7
