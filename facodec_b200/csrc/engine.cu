@@ -3647,10 +3647,33 @@ int fac_alias_free_act(fac_handle* h, const float* x, int B, int C, int T, int a
     return FAC_OK;
 }
 
-int fac_debug_conv(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin, int Cin,
-                   int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
-                   const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
-                   int Tout, void* stream) {
+}  // extern "C"
+
+namespace {
+// The per-lane lengths of a debug conv hook (HOST, B entries, or null) checked and copied to the device: *dev receives
+// the device copy (null when lane_len_host is null; the caller frees it).  Nothing is launched when a length lies
+// outside [1, Tin].
+int debug_upload_lanes(fac_handle* h, const char* who, const int* lane_len_host, int B, int Tin, int** dev) {
+    *dev = nullptr;
+    if (!lane_len_host) return FAC_OK;
+    for (int b = 0; b < B; ++b)
+        if (lane_len_host[b] < 1 || lane_len_host[b] > Tin) {
+            h->err = std::string(who) + ": lane lengths must lie in [1, Tin]";
+            return FAC_ERR_INVALID;
+        }
+    cudaSetDevice(h->device);
+    cudaError_t e = cudaMalloc(dev, sizeof(int) * (size_t)B);
+    if (e == cudaSuccess) e = cudaMemcpy(*dev, lane_len_host, sizeof(int) * (size_t)B, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); cudaFree(*dev); *dev = nullptr; return FAC_ERR_CUDA; }
+    return FAC_OK;
+}
+
+// fac_debug_conv, and fac_debug_conv_lanes' path -1: launch_conv (it picks the cin1 / cout1 / generic kernel) on one
+// layer; lane_len DEVICE [B] (each lane's own input rows) or null.
+int debug_conv(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin, int Cin,
+               int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
+               const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
+               int Tout, const int* lane_len, void* stream) {
     if (!h || !x || !w_host || !y) return FAC_ERR_INVALID;
     cudaSetDevice(h->device);
     cudaStream_t st = (cudaStream_t)stream;
@@ -3673,7 +3696,7 @@ int fac_debug_conv(fac_handle* h, const float* x, const float* w_host, const flo
     if (in_alpha_host) { p.in_alpha = d + o_ia; p.in_inv_alpha = d + o_iia; }
     p.out_act = act;
     if (out_alpha_host) { p.out_act = ACT_SNAKE; p.out_alpha = d + o_oa; p.out_inv_alpha = d + o_oia; }
-    p.res = res;
+    p.res = res; p.lane_len = lane_len;
     p.B = B; p.Tin = Tin; p.Cin = Cin; p.Tout = Tout; p.Cout = Cout; p.K = K; p.dil = dil; p.stride = stride;
     p.pad_left = pad_left; p.pad_right = pad_right; p.pad_reflect = reflect;
     p.ldw = ldw; p.ldy = Cout; p.ldx = Cin;
@@ -3683,6 +3706,17 @@ int fac_debug_conv(fac_handle* h, const float* x, const float* w_host, const flo
     cudaFree(d);
     if (e != cudaSuccess) { h->err = std::string("fac_debug_conv: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
     return FAC_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int fac_debug_conv(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin, int Cin,
+                   int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
+                   const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
+                   int Tout, void* stream) {
+    return debug_conv(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
+                      in_alpha_host, out_alpha_host, act, res, y, Tout, nullptr, stream);
 }
 
 }  // extern "C"
@@ -3857,7 +3891,7 @@ int fac_set_option(fac_handle* h, const char* name, int value) {
 static int debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin, int Cin,
                          int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
                          const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
-                         int Tout, int promoted, void* stream, int* group_out) {
+                         int Tout, int promoted, void* stream, int* group_out, const int* lane_len) {
     if (!h || !x || !w_host || !y) return FAC_ERR_INVALID;
     cudaSetDevice(h->device);
     cudaStream_t st = (cudaStream_t)stream;
@@ -3902,7 +3936,7 @@ static int debug_conv_tc(fac_handle* h, const float* x, const float* w_host, con
     tp.res = res;
     tp.B = B; tp.Tin = Tin; tp.ldx = Cin;
     tp.PLr = pad_left / tp.vf;
-    tp.pad_left_s = pad_left; tp.pad_right_s = pad_right; tp.reflect = reflect;
+    tp.pad_left_s = pad_left; tp.pad_right_s = pad_right; tp.reflect = reflect; tp.lane_len = lane_len;
     tp.Tout = Tout; tp.ldy = Cout;
     tp.x_bstride = (size_t)Tin * Cin; tp.y_bstride = (size_t)Tout * Cout;
     e = launch_conv_tc(tp, st);
@@ -3917,7 +3951,7 @@ int fac_debug_conv_tc(fac_handle* h, const float* x, const float* w_host, const 
                       const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
                       int Tout, int promoted, void* stream) {
     return debug_conv_tc(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
-                         in_alpha_host, out_alpha_host, act, res, y, Tout, promoted, stream, nullptr);
+                         in_alpha_host, out_alpha_host, act, res, y, Tout, promoted, stream, nullptr, nullptr);
 }
 
 int fac_debug_conv_tc_group1(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin,
@@ -3926,13 +3960,42 @@ int fac_debug_conv_tc_group1(fac_handle* h, const float* x, const float* w_host,
                              int Tout, int promoted, void* stream, int* group) {
     if (!group) return FAC_ERR_INVALID;
     return debug_conv_tc(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
-                         in_alpha_host, out_alpha_host, act, res, y, Tout, promoted, stream, group);
+                         in_alpha_host, out_alpha_host, act, res, y, Tout, promoted, stream, group, nullptr);
+}
+
+int fac_debug_conv_lanes(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin,
+                         int Cin, int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
+                         const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
+                         int Tout, int path, const int* lane_len_host, void* stream) {
+    if (!h || !x || !w_host || !y || B <= 0 || Tin <= 0) return FAC_ERR_INVALID;
+    int* lanes = nullptr;
+    int rc = debug_upload_lanes(h, "fac_debug_conv_lanes", lane_len_host, B, Tin, &lanes);
+    if (rc != FAC_OK) return rc;
+    if (path == -1)
+        rc = debug_conv(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
+                        in_alpha_host, out_alpha_host, act, res, y, Tout, lanes, stream);
+    else
+        rc = debug_conv_tc(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
+                           in_alpha_host, out_alpha_host, act, res, y, Tout, path, stream, nullptr, lanes);
+    cudaFree(lanes);
+    return rc;
 }
 
 int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const float* b7_host, const float* w1_host,
                       const float* b1_host, const float* alpha1_host, const float* alpha2_host, int B, int T, int C,
                       int dil, int mode, float* y, void* stream) {
-    if (!h || !x || !y || !w7_host || !w1_host) return FAC_ERR_INVALID;
+    return fac_debug_resunit_lanes(h, x, w7_host, b7_host, w1_host, b1_host, alpha1_host, alpha2_host, B, T, C, dil, mode,
+                                   1, nullptr, y, stream);
+}
+
+int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host, const float* b7_host,
+                            const float* w1_host, const float* b1_host, const float* alpha1_host,
+                            const float* alpha2_host, int B, int T, int C, int dil, int mode, int causal,
+                            const int* lane_len_host, float* y, void* stream) {
+    if (!h || !x || !y || !w7_host || !w1_host || B <= 0 || T <= 0) return FAC_ERR_INVALID;
+    int* lanes = nullptr;
+    int rc0 = debug_upload_lanes(h, "fac_debug_resunit_lanes", lane_len_host, B, T, &lanes);
+    if (rc0 != FAC_OK) return rc0;
     fac_handle tmp;
     tmp.device = h->device;
     tmp.use_tc = mode == 0 ? 0 : 1;          // 0: fp32 FMA, 1: two tensor-core launches, 2: fused launch; 3/4 = 1/2 with bf16 split;
@@ -3954,11 +4017,11 @@ int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const
     put("u.block.3.conv.conv.weight", w1_host, {C, C, 1});
     put("u.block.3.conv.conv.bias", b1_host, {C});
     ResW r;
-    try { r = pack_res(&tmp, 0, "u", dil, false); } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_STATE; }
+    try { r = pack_res(&tmp, 0, "u", dil, false); } catch (const PackError& e) { h->err = e.msg; cudaFree(lanes); return FAC_ERR_STATE; }
     cudaSetDevice(h->device);
     cudaError_t e = cudaMalloc(&tmp.warena, (tmp.pack.size() + 64) * sizeof(float));
     if (e == cudaSuccess) e = cudaMemcpy(tmp.warena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
+    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); cudaFree(lanes); return FAC_ERR_CUDA; }
     cudaStream_t st = (cudaStream_t)stream;
     float* scratch = nullptr;
     e = cudaMalloc(&scratch, sizeof(float) * (size_t)B * T * C);
@@ -3966,7 +4029,7 @@ int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const
     if (e != cudaSuccess) { h->err = cudaGetErrorString(e); rc = FAC_ERR_CUDA; }
     if (rc == FAC_OK) {
         Ctx c{&tmp, st, false};
-        residual_unit(c, r, x, scratch, y, B, T);
+        residual_unit(c, r, x, scratch, y, B, T, causal != 0, lanes);
         rc = finish(&tmp, c);
         cudaError_t e2 = cudaStreamSynchronize(st);
         if (rc == FAC_OK && e2 != cudaSuccess) { tmp.err = cudaGetErrorString(e2); rc = FAC_ERR_CUDA; }
@@ -3975,6 +4038,7 @@ int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const
     if (rc != FAC_OK) h->err = tmp.err;
     if (scratch) cudaFree(scratch);
     cudaFree(tmp.warena);
+    cudaFree(lanes);
     return rc;
 }
 

@@ -41,13 +41,29 @@ int fac_debug_conv_tc_group1(fac_handle* h, const float* x, const float* w_host,
                              int Cin, int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
                              const float* in_alpha_host, const float* out_alpha_host, int act, const float* res,
                              float* y, int Tout, int promoted, void* stream, int* group);
+/* One layer of a ragged batch: fac_debug_conv_tc's arguments with lane_len_host (HOST, B entries, or NULL: Tin each)
+ * the input rows of each lane, each padded about its own end as ConvParams::lane_len / TcConvParams::lane_len do.
+ * path = -1 runs launch_conv (the fp32 FMA kernels: it picks the cin1, cout1 or generic kernel itself), path = 0..5 the
+ * tensor-core classes of fac_debug_conv_tc.  A length outside [1, Tin] returns FAC_ERR_INVALID before anything is
+ * launched. */
+int fac_debug_conv_lanes(fac_handle* h, const float* x, const float* w_host, const float* bias_host, int B, int Tin,
+                         int Cin, int Cout, int K, int dil, int stride, int pad_left, int pad_right, int reflect,
+                         const float* in_alpha_host, const float* out_alpha_host, int act, const float* res,
+                         float* y, int Tout, int path, const int* lane_len_host, void* stream);
 /* One ResidualUnit (dac/model/dac.py:25-42) y = x + conv1(snake(conv7_d(snake(x)))) on DEVICE channels-last
  * x, y [B,T,C] with HOST folded weights w7 [C,C,7], w1 [C,C,1].  mode 0: fp32 FMA kernels, 1: two tensor-core
  * launches, 2: the single fused tensor-core launch (FAC_ERR_UNSUPPORTED if the geometry cannot be fused);
- * 3 / 4: as 1 / 2 with the bf16 hi/lo split. */
+ * 3 / 4: as 1 / 2 with the bf16 hi/lo split; 5 / 6: as 3 / 4 with the k = 7 conv in one fp16 pass.  Causal. */
 int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const float* b7_host, const float* w1_host,
                       const float* b1_host, const float* alpha1_host, const float* alpha2_host, int B, int T, int C,
                       int dil, int mode, float* y, void* stream);
+/* fac_debug_resunit with the unit's padding chosen by causal (0: the non-causal split of the redecoder's decoder,
+ * reflected at both ends) and lane_len_host (HOST, B entries in [1, T], or NULL) each lane's own rows, as the ragged
+ * decoder passes them.  A length outside [1, T] returns FAC_ERR_INVALID before anything is launched. */
+int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host, const float* b7_host,
+                            const float* w1_host, const float* b1_host, const float* alpha1_host,
+                            const float* alpha2_host, int B, int T, int C, int dil, int mode, int causal,
+                            const int* lane_len_host, float* y, void* stream);
 /* clock64() phase timestamps written by one probe CTA of the most recent conv_tc_kernel launch:
  * [0] start, [1] all activation chunks produced, [2] GEMM 1 retired, [3] GEMM-2 operand produced (fused),
  * [4] GEMM 2 retired (fused), [5] epilogue done.  Kernel-tuning aid. */

@@ -1,4 +1,4 @@
-"""GPU: kernel-level parity through the C-ABI test hooks (fac_debug_conv / fac_debug_conv_tc / fac_debug_resunit)
+"""GPU: kernel-level parity through the C-ABI test hooks (fac_debug_conv / fac_debug_conv_tc / fac_debug_resunit_lanes)
 against plain PyTorch on CPU -- the same functional calls the oracle restatement uses.  The LSTM recurrence has its own
 fp64 suite in test_gpu_lstm.py."""
 import ctypes
@@ -165,14 +165,20 @@ def test_conv_tc_kernel_vs_torch(case, promoted, occ2, built_lib):
     assert err <= tol * max(scale, 1.0), f"max err {err} (scale {scale})"
 
 
+UNIT_SHAPES = [(2, 300, 96, 1), (1, 520, 96, 9), (2, 200, 192, 3), (1, 130, 256, 1), (2, 40, 96, 9),
+               (1, 700, 64, 3), (2, 300, 192, 9),     # C = 192, d = 9: single-slot ring
+               (2, 20, 96, 9)]                        # T <= 27: the short-input branch of the non-causal split too
+
+
 @pytest.mark.parametrize("occ2", [0, 256])
 @pytest.mark.parametrize("mode", [0, 1, 2, 3, 4, 5, 6])
-@pytest.mark.parametrize("B,T,C,dil", [(2, 300, 96, 1), (1, 520, 96, 9), (2, 200, 192, 3), (1, 130, 256, 1), (2, 40, 96, 9),
-                                       (1, 700, 64, 3), (2, 300, 192, 9)])   # C = 192, d = 9: single-slot ring
-def test_residual_unit_modes(B, T, C, dil, mode, occ2, built_lib):
+@pytest.mark.parametrize("B,T,C,dil,causal", [pytest.param(*s, cz, id="-".join(map(str, s)) + ("" if cz else "-noncausal"))
+                                              for s in UNIT_SHAPES for cz in (True, False)])
+def test_residual_unit_modes(B, T, C, dil, causal, mode, occ2, built_lib):
     """ResidualUnit (dac.py:25-42) through the fp32 FMA path (0), two tensor-core launches (1 tf32, 3 bf16 split), and the
     fused launch (2 tf32, 4 bf16 split), 5/6 = 3/4 with the k = 7 conv in ONE fp16 pass (the product's default downstream of
-    the VQ); occ2 = tiles planned for two CTAs per SM."""
+    the VQ); occ2 = tiles planned for two CTAs per SM.  causal = False: the redecoder's decoder, reflected at both ends
+    (pad (k_eff - 1) - (k_eff - 1) // 2 on the left, the rest on the right)."""
     from oracle import facodec_oracle as O
     if occ2 and mode == 0:
         pytest.skip("fp32 FMA path has no residency option")
@@ -188,11 +194,11 @@ def test_residual_unit_modes(B, T, C, dil, mode, occ2, built_lib):
     a2 = torch.rand(C, generator=g) + 0.5
     sd = {"u.block.0.alpha": a1.view(1, C, 1), "u.block.1.conv.conv.weight": w7, "u.block.1.conv.conv.bias": b7,
           "u.block.2.alpha": a2.view(1, C, 1), "u.block.3.conv.conv.weight": w1, "u.block.3.conv.conv.bias": b1}
-    ref = O.residual_unit(x, sd, "u", dil)
+    ref = O.residual_unit(x.double(), {k: v.double() for k, v in sd.items()}, "u", dil, causal=causal)
     xd = x.transpose(1, 2).contiguous().cuda()
     yd = torch.full((B, T, C), float("nan"), device="cuda")
-    rc = e.L.fac_debug_resunit(e.handle, _p(xd), _p(w7.contiguous()), _p(b7), _p(w1.contiguous()), _p(b1), _p(a1), _p(a2),
-                               B, T, C, dil, mode, _p(yd), None)
+    rc = e.L.fac_debug_resunit_lanes(e.handle, _p(xd), _p(w7.contiguous()), _p(b7), _p(w1.contiguous()), _p(b1), _p(a1),
+                                     _p(a2), B, T, C, dil, mode, int(causal), None, _p(yd), None)
     if mode == 2 and C > 128:
         # the fused kernel keeps the whole GEMM-2 operand and a chunk's weights in shared memory: with the tf32 split
         # that only fits up to C = 128 (the product runs fused units with the bf16 split, mode 4)
@@ -201,8 +207,8 @@ def test_residual_unit_modes(B, T, C, dil, mode, occ2, built_lib):
     assert rc == 0, e.L.fac_last_error(e.handle)
     y = yd.cpu().transpose(1, 2)
     assert torch.isfinite(y).all()
-    err = (y - ref).abs().max().item()
+    err = (y.double() - ref).abs().max().item()
     scale = ref.abs().max().item()
     tol = 2e-5 if mode == 0 else (8e-5 if mode <= 2 else (3e-4 if mode <= 4 else 2e-3))
-    print(f"RESUNIT mode={mode} C={C} d={dil} T={T} maxerr={err:.3e} scale={scale:.3f}")
+    print(f"RESUNIT mode={mode} C={C} d={dil} T={T} causal={causal} maxerr={err:.3e} scale={scale:.3f}")
     assert err <= tol * max(scale, 1.0), f"max err {err} (scale {scale})"
