@@ -158,8 +158,10 @@ int fac_debug_fa_quantize(fac_handle* h, const float* f0, const float* z, const 
 int fac_debug_attention(fac_handle* h, const float* q, const float* k, const float* v, float* o, int B, int T,
                         int heads, const int* valid_len, int force_stream, void* stream);
 /* Registers (dst != NULL) or clears a named tap: the next forward copies that channels-last
- * intermediate into dst (DEVICE, up to capacity_floats).  Names: enc_conv0, enc_block1..4,
- * enc_lstm, mel80, f0_input, gamma_beta, dec_conv0, dec_lstm, dec_block1..4.  dec_pool.latents: the per-lane dequantized
+ * intermediate into dst (DEVICE, up to capacity_floats).  Names: enc_conv0, enc_block1..4 (after the down-sampling conv),
+ * enc_block<i>.res<j> (after ResidualUnit j = 0..2 of EncoderBlock i), enc_lstm, mel80, f0_input, gamma_beta, dec_conv0,
+ * dec_lstm, dec_block<i>.up (after DecoderBlock i's up-sampling conv), dec_block<i>.res<j>, dec_block1..4 (the block's
+ * output, = dec_block<i>.res2); the dec_* names also fire in the redecoder's decoder.  dec_pool.latents: the per-lane dequantized
  * latents [n][Fmax][1024] of a fac_dec_pool_decode_codes batch (each batch overwrites it; frames past a lane's F are 0).
  * Per scale i of fac_reconstruction_loss ("recon.") and fac_spectral_loss ("spec."): recon.dft.<i> / spec.dft.<i> the
  * DFT GEMM output [2*B*F][ld] (rows [0, B*F) of x, then those of the second signal; Re at column 2k, Im at 2k + 1,

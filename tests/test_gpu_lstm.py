@@ -273,24 +273,28 @@ def reference(H, regime, B, T, kind):
     return _REFS[key]
 
 
-def check_against_reference(y, cfg, H, regime, tag):
-    """Holds the kernel's y [B][T][H] (GPU) to its route's bar; prints every error and ratio."""
+def check_against_reference(y, cfg, H, regime, tag, ref=None):
+    """Holds the kernel's y [B][T][H] (GPU) to its route's bar; prints every error and ratio.  ref(kind) gives the
+    reference for kind = "64", "32" or an emulation pair (slstm_ref's triple); by default the cached reference() of the
+    regime's own weights and inputs."""
     B, T, _ = y.shape
     assert torch.isfinite(y).all(), f"{tag}: non-finite output"
     _, _, factor, emul = CONFIGS[cfg]
-    y64, cmax, gmax = reference(H, regime, B, T, "64")
+    if ref is None:
+        ref = lambda kind: reference(H, regime, B, T, kind)
+    y64, cmax, gmax = ref("64")
     yd = y.double()
     err = (yd - y64).abs().max().item()
     scale = y64.abs().max().item()
     if factor:
-        y32 = reference(H, regime, B, T, "32")[0]
+        y32 = ref("32")[0]
         err32 = (y32.double() - y64).abs().max().item()
         bar = max(factor * err32, 4e-6 * scale)
         print(f"LSTM {tag}: max|y-y64| {err:.3e}  max|y32-y64| {err32:.3e}  scale {scale:.2f}  bar {bar:.3e}  "
               f"ratio {err / bar:.3f}  max|c| {cmax:.1f}  max|gate| {gmax:.1f}")
         assert err <= bar, f"{tag}: max|y - y64| = {err:.3e} > {bar:.3e}"
     else:
-        ye = reference(H, regime, B, T, emul)[0]
+        ye = ref(emul)[0]
         rms = lambda d: d.pow(2).mean().sqrt().item()
         d_kernel, d_model = rms(yd - ye), rms(ye - y64)
         err_e = (ye - y64).abs().max().item()

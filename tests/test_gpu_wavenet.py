@@ -341,14 +341,16 @@ def test_bars_separate_the_classes(regime):
 # ---------------------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------
-def _with_options(eng, opts, fn):
+def _with_options(eng, opts, fn, defaults=None):
+    """fn() with the engine options opts set, each restored to its value in defaults (OPTION_DEFAULTS) afterwards."""
+    defaults = OPTION_DEFAULTS if defaults is None else defaults
     try:
         for k, v in opts.items():
             eng.set_option(k, v)
         return fn()
     finally:
         for k in opts:
-            eng.set_option(k, OPTION_DEFAULTS[k])
+            eng.set_option(k, defaults[k])
 
 
 _CODEC = {}
