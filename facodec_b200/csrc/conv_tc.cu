@@ -29,7 +29,11 @@
 //            start-address offset of tap*dil rows (taps are never re-loaded or im2col'ed);
 //   the next chunk's activations are produced while this chunk's wgmma run (double-buffered operand).
 // Fused mode (a whole ResidualUnit, conv7 -> +b7 -> Snake -> 1x1 conv -> +b1 -> +x): GEMM 1's accumulators go through
-// bias + Snake + split straight into a resident shared-memory operand for GEMM 2.
+// bias + Snake + split straight into a resident shared-memory operand for GEMM 2.  The promoted fp16 hi + scaled-lo class
+// has it too (the encoder's C = 64 and C = 128 units, two CTAs per SM): GEMM 1 is the promoted conv7 with its windows,
+// the split is split_store_f16's, and GEMM 2 runs the unfused 1x1's passes as one window, so the unit's output is the
+// two-launch route's bit for bit without the conv7 output's round trip through global memory.  Its GEMM-2 operand
+// takes the place of the master accumulator, which is dead after GEMM 1's last promotion.
 // Epilogue from the accumulator registers: bias -> Snake/tanh/Mish -> residual -> 8-byte stores.
 // Variants: tiles planned for two resident CTAs per SM (always tried for the promoted class; option "tc_occ2_maxn" for
 // the others), and the transposed formulation of the promoted fp16 class (option "encoder_tt": weights as the wgmma A
@@ -161,8 +165,11 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
     const uint32_t a_plane = (uint32_t)G * T1::KG * Rpad * 16, a_bytes = a_plane * T1::planes;
     uint8_t* abuf = smem + kSmemHdr;
     float4* master = reinterpret_cast<float4*>(abuf + 2 * (size_t)a_bytes);
-    uint8_t* wbuf = abuf + 2 * (size_t)a_bytes + master_bytes(PROMO, nchunk, p.promote_every, NI);
-    uint8_t* a2buf = wbuf + (size_t)S * p.b_slot;
+    const uint32_t m_bytes = master_bytes(PROMO, nchunk, p.promote_every, NI);
+    uint8_t* wbuf = abuf + 2 * (size_t)a_bytes + m_bytes;
+    // a promoted unit's GEMM-2 operand (4 C BM bytes, the master's size at N = C) takes the master's place: the master is
+    // dead after GEMM 1's last promotion
+    uint8_t* a2buf = m_bytes ? reinterpret_cast<uint8_t*>(master) : wbuf + (size_t)S * p.b_slot;
     const uint32_t w_unit1 = (uint32_t)Kr * T1::planes * T1::KG * N * 16;
     const uint32_t w_unit2 = FUSED ? (uint32_t)prec_planes(P2) * prec_kg(P2) * N * 16 : 0;
     const int units = nstep1 + (FUSED ? p.nchunk2 : 0);
@@ -294,6 +301,7 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
                     // GEMM-2 operand snake2(D1 + b7), split, K-major [plane][k-piece][BM rows][16 B]
                     constexpr int KG2 = prec_kg(P2 < 0 ? 0 : P2);
                     const uint32_t a2_plane = (uint32_t)(p.nchunk2 * KG2) * BM2 * 16;
+                    if (m_bytes) __syncthreads();     // every thread has read its master slots before any operand store
                     for_each_pair<NI, 32>(tl, acc, [&](int row, int col, float v0, float v1) {
                         const float2 bi = __ldg(reinterpret_cast<const float2*>(p.bias + col));
                         const float2 al = __ldg(reinterpret_cast<const float2*>(p.out_alpha + col));
@@ -307,6 +315,13 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
                             const uint32_t off = ((uint32_t)(col >> 3) * BM2 + row) * 16 + (col & 7) * 2;
                             *reinterpret_cast<__nv_bfloat162*>(a2buf + off) = h;
                             *reinterpret_cast<__nv_bfloat162*>(a2buf + a2_plane + off) = l;
+                        } else if constexpr (P2 == P_F16X2) {     // split_store_f16's split, in the bf16 layout
+                            const __half2 h = __floats2half2_rn(v0, v1);
+                            const float2 hf = __half22float2(h);
+                            const __half2 l = __floats2half2_rn((v0 - hf.x) * kLoScale, (v1 - hf.y) * kLoScale);
+                            const uint32_t off = ((uint32_t)(col >> 3) * BM2 + row) * 16 + (col & 7) * 2;
+                            *reinterpret_cast<__half2*>(a2buf + off) = h;
+                            *reinterpret_cast<__half2*>(a2buf + a2_plane + off) = l;
                         } else {
                             const float h0 = to_tf32(v0), h1 = to_tf32(v1);
                             const uint32_t off = ((uint32_t)(col >> 2) * BM2 + row) * 16 + (col & 3) * 4;
@@ -325,11 +340,18 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
             const uint32_t a2_plane = (uint32_t)(p.nchunk2 * KG2) * BM2 * 16, a2_lbo = (uint32_t)BM2 * 16;
             const uint32_t ahi = a2base + ((uint32_t)(c2 * KG2) * BM2 + tl.row0) * 16, alo = ahi + a2_plane;
             const uint32_t bhi = wslot + (uint32_t)tl.col0 * 16, blo = bhi + KG2 * b_lbo;
-            mma_pass<P2x, NI>(acc, ahi, a2_lbo, bhi, b_lbo);
-            mma_pass<P2x, NI>(acc, ahi, a2_lbo, blo, b_lbo);
-            mma_pass<P2x, NI>(acc, alo, a2_lbo, bhi, b_lbo);
+            if constexpr (P2x == P_F16X2) {      // the unfused 1x1's passes and order; its K loop is one promotion window
+                mma_pass<P2x, NI>(acc, ahi, a2_lbo, bhi, b_lbo);
+                mma_pass<P2x, NI>(crs, ahi, a2_lbo, blo, b_lbo);
+                mma_pass<P2x, NI>(crs, alo, a2_lbo, bhi, b_lbo);
+            } else {
+                mma_pass<P2x, NI>(acc, ahi, a2_lbo, bhi, b_lbo);
+                mma_pass<P2x, NI>(acc, ahi, a2_lbo, blo, b_lbo);
+                mma_pass<P2x, NI>(acc, alo, a2_lbo, bhi, b_lbo);
+            }
             wg_commit();
             wg_wait_all();
+            if (PROMO && c2 + 1 == p.nchunk2) promote(true, true);
         }
     }
 
@@ -402,11 +424,13 @@ bool tc_conv_plan(TcConvParams& p) {
     if (p.f16x2 && !p.promoted) return false;
     if (p.g1f16 && !p.bf16) return false;
     if (p.tt && !p.f16x2) return false;
-    if (p.fused && (p.promoted || p.Cin != p.Cout || p.vf != 1 || p.Cout > 256)) return false;
-    const int P1 = plan_prec(p), P2 = p.fused ? (p.bf16 ? P_BF16 : P_TF32) : P_NONE;
+    if (p.fused && ((p.promoted && (!p.f16x2 || p.tt)) || p.Cin != p.Cout || p.vf != 1 || p.Cout > 256)) return false;
+    const int P1 = plan_prec(p), P2 = p.fused ? (p.f16x2 ? P_F16X2 : (p.bf16 ? P_BF16 : P_TF32)) : P_NONE;
     p.nchunk = p.Cin * p.vf / kChunk;
     p.nchunk2 = p.fused ? p.Cout / kChunk : 0;
     p.promote_every = p.promoted ? (p.f16x2 ? (48 / p.Kr < 1 ? 1 : 48 / p.Kr) : (8 / p.Kr < 1 ? 1 : 8 / p.Kr)) : 1;
+    // A promoted unit's GEMM 2 (the 1x1) promotes once, at its end, as the unfused 1x1 does: one window of <= 48 chunks.
+    if (p.fused && p.promoted && p.nchunk2 > 48) return false;
     const int nw_max = p.promoted ? 64 : 128;      // accumulator registers per thread: NW / 2 (x 3 when promoted)
     // N depends on the layer's shape and split class only (never on dil, Tout, tt or occ2_maxn): the weight blob is laid
     // out for it once (tc_pack_blob) and every later plan of the layer must find the same N.  It is the widest tile whose
@@ -421,7 +445,7 @@ bool tc_conv_plan(TcConvParams& p) {
         if (kSmemHdr + kAReserve + slot + a2 <= kSmemCap) N = cand;
         else if (p.fused) return false;
     }
-    if (N == 0) return false;
+    if (N == 0 || (p.fused && p.promoted && N != p.Cout)) return false;
     // Two resident CTAs per SM: one CTA's operand production, barriers, promotions and epilogue overlap the other's MMAs;
     // each gets half the shared memory and <= 128 registers per thread.  Always tried for the promoted class, which loses
     // no MMA width to it (NW <= 64 either way); for the others only for tiles of N <= occ2_maxn, which must halve NW.
@@ -456,6 +480,7 @@ bool tc_conv_plan(TcConvParams& p) {
         // transposed: a warpgroup's A operand is always 64 channel rows; rows past its NW read (and discard) whatever
         // follows the weight slot, so the buffer ends with 64 rows of slack
         const size_t master = master_bytes(p.promoted, p.nchunk, p.promote_every, p.tt ? 64 : NW);
+        if (master) a2 = 0;     // a promoted unit's GEMM-2 operand aliases the master: both are 4 C BM bytes at N = C
         l.total = kSmemHdr + 2 * a_bytes + master + S * l.slot + a2 + (p.tt ? 64 * 16 : 0);
         return l;
     };
@@ -471,15 +496,19 @@ bool tc_conv_plan(TcConvParams& p) {
             if (G <= p.max_group && p.nchunk % G == 0 && (!p.promoted || p.promote_every % G == 0) && layout(S, MT, G).total <= cap) return G;
         return 1;
     };
+    // A promoted unit is planned for two CTAs per SM or not at all: at one CTA per SM it would give back more than fusing
+    // saves (two CTAs per SM gave the promoted k = 7 convs 18-43 %).  Its kernel is compiled for NW = 64 only: C = 64 as
+    // 128 rows, C = 128 as 64 rows, the tiles of the unit's two unfused convs.
+    const bool unit2 = p.fused && p.promoted;
     const bool want2 = p.promoted ? !p.tt : (p.occ2_maxn > 0 && N <= p.occ2_maxn);
-    for (int two = want2 ? 1 : 0; two >= 0; --two) {
+    for (int two = want2 ? 1 : 0; two >= (unit2 ? 1 : 0); --two) {
         const size_t cap = two ? kSmemCap2 : kSmemCap;
         const int nwl = two ? 64 : nw_max;
         for (int S = 2; S >= 1; --S)
             for (int MT = 2; MT >= 1; --MT) {
                 const int NW = MT == 2 ? N : N / 2;
                 const bool wide = !two && P1 == P_F16S && NW == f16s_wide_nw(p.fused);
-                if ((NW > nwl && !wide) || NW % 16) continue;
+                if ((NW > nwl && !wide) || NW % 16 || (unit2 && NW != 64)) continue;
                 if (wide && layout(2, 1, 1).total <= kSmemCap2) continue;
                 const Layout l1 = layout(S, MT, 1);
                 if (l1.total > cap) continue;
@@ -647,6 +676,8 @@ cudaError_t launch_conv_tc(const TcConvParams& p, cudaStream_t st) {
     if (grid.y > 65535 || grid.z > 65535) return cudaErrorInvalidValue;
     const int P1 = plan_prec(p);
     if (p.fused) {
+        if (P1 == P_F16X2)
+            return (p.MT == 2 ? p.N : p.N / 2) == 64 ? launch_one<P_F16X2, P_F16X2, true, 64, 2>(p, grid, st) : cudaErrorInvalidValue;
         if (P1 == P_F16S) return launch_occ<P_F16S, P_BF16>(p, grid, st);
         if (P1 == P_BF16) return launch_occ<P_BF16, P_BF16>(p, grid, st);
         return launch_occ<P_TF32, P_TF32>(p, grid, st);

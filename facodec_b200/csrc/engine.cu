@@ -169,8 +169,10 @@ struct fac_handle {
     // tensor-core path (fac_set_option "tensor_cores"): 0 = never, 1 = layers downstream of the VQ only
     // (decoder, timbre branch), 2 = every eligible layer (default; promoted accumulation upstream of the VQ)
     int use_tc = 2;
-    int fuse_res = 1;               // fused ResidualUnit launches (fac_set_option "fuse_resunit"); 2 = only where the
-                                    // fused tile still allows two CTAs per SM (C <= 128)
+    int fuse_res = 1;               // fused ResidualUnit launches (fac_set_option "fuse_resunit"): the decoder's, and the
+                                    // encoder's C = 64 and 128 units in the promoted fp16 hi + scaled-lo class (bit-identical
+                                    // to their two launches); 2 = only where the fused tile still allows two CTAs per SM
+                                    // (C <= 128)
     int lstm_v2 = 1;                // fac_set_option "lstm_v2": resident-W fp16 recurrence kernel (lstm2.cu); 0 = round-1 kernel
     int dec_lstm_fp16 = 1;          // fac_set_option "decoder_lstm_fp16": downstream LSTMs run ONE fp16 pass (0 = bf16 hi/lo 3-pass)
     int attn_stream = 0;            // fac_set_option "attention_stream": 1 forces the recomputing attention kernel (test aid)
@@ -803,14 +805,22 @@ int sconv(Ctx& c, const ConvW& w, const float* x, float* y, int B, int T, int di
     return Tout;
 }
 
-// Whole ResidualUnit in one tensor-core launch (conv_tc_kernel<true>) when every channel fits one CTA tile.
+// Whole ResidualUnit in one tensor-core launch (conv_tc_kernel<true>) when every channel fits one CTA tile.  Upstream of
+// the VQ only where the two launches would run the promoted fp16 hi + scaled-lo class (the fused launch is bit-identical
+// to them there); every other route upstream keeps its two launches.
 bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B, int T, bool causal, const int* lane_len) {
-    if (c.h->use_tc < 1 || !c.h->fuse_res || c.vq_critical || !r.c7.tc || !r.c1.tc || r.c7.promoted || r.c1.promoted ||
-        r.c7.Cin != r.c7.Cout || r.c1.K != 1 || r.c7.vf != 1)
+    const bool promoted = r.c7.promoted && r.c1.promoted;
+    if (!c.h->fuse_res || !r.c7.tc || !r.c1.tc || r.c7.promoted != r.c1.promoted || r.c7.Cin != r.c7.Cout ||
+        r.c1.K != 1 || r.c7.vf != 1)
+        return false;
+    if (c.vq_critical ? (!promoted || c.h->use_tc < 2 || !c.h->enc_f16 || c.h->enc_tt || !r.c7.has16 || !r.c1.has16)
+                      : (promoted || c.h->use_tc < 1))
         return false;
     TcConvParams tp;
     tp.Cin = r.c7.Cin; tp.Cout = r.c7.Cout; tp.vf = 1; tp.Kr = r.c7.K; tp.dil = r.dil; tp.fused = 1;
-    tp.bf16 = (c.h->dec_bf16 && r.c7.has16 && r.c1.has16) ? 1 : 0;
+    tp.promoted = promoted ? 1 : 0;
+    tp.f16x2 = tp.promoted;
+    tp.bf16 = (!promoted && c.h->dec_bf16 && r.c7.has16 && r.c1.has16) ? 1 : 0;
     tp.g1f16 = (tp.bf16 && r.c7.has_f16s && c.h->dec_c7_f16) ? 1 : 0;
     tp.occ2_maxn = c.h->tc_occ2;
     tp.Tout = T;
@@ -823,8 +833,8 @@ bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B,
     if (c.dry) return true;
     const int k_eff = (r.c7.K - 1) * r.dil + 1;
     tp.x = x; tp.y = y; tp.res = x;
-    tp.wblob = c.W(tp.g1f16 ? r.c7.tcw_f16s : (tp.bf16 ? r.c7.tcw16 : r.c7.tcw)); tp.bias = c.W(r.c7.b);
-    tp.wblob2 = c.W(tp.bf16 ? r.c1.tcw16 : r.c1.tcw); tp.bias2 = c.W(r.c1.b);
+    tp.wblob = c.W(tp.g1f16 ? r.c7.tcw_f16s : ((tp.bf16 || tp.f16x2) ? r.c7.tcw16 : r.c7.tcw)); tp.bias = c.W(r.c7.b);
+    tp.wblob2 = c.W((tp.bf16 || tp.f16x2) ? r.c1.tcw16 : r.c1.tcw); tp.bias2 = c.W(r.c1.b);
     tp.in_alpha = c.W(r.s1.a); tp.in_inv_alpha = c.W(r.s1.ia);
     tp.out_act = ACT_SNAKE; tp.out_alpha = c.W(r.s2.a); tp.out_inv_alpha = c.W(r.s2.ia);
     tp.B = B; tp.Tin = T; tp.ldx = r.c7.Cin;
@@ -836,7 +846,7 @@ bool residual_unit_fused(Ctx& c, const ResW& r, const float* x, float* y, int B,
     double bytes = 4.0 * ((double)B * T * r.c7.Cin * 2 + (double)B * T * r.c7.Cout + (double)(r.c7.K + 1) * r.c7.Cin * r.c7.Cout);
     char det[96];
     snprintf(det, sizeof det, "res.fused C%d K%d d%d T%d", r.c7.Cin, r.c7.K, r.dil, T);
-    c.begin("conv_tc", flops, bytes, det);
+    c.begin(tp.promoted ? "conv_tcp" : "conv_tc", flops, bytes, det);
     c.check(launch_conv_tc(tp, c.st), "res.fused");
     c.end();
     return true;
@@ -4006,13 +4016,16 @@ int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host,
     int* lanes = nullptr;
     int rc0 = debug_upload_lanes(h, "fac_debug_resunit_lanes", lane_len_host, B, T, &lanes);
     if (rc0 != FAC_OK) return rc0;
+    if (mode < 0 || mode > 8) { cudaFree(lanes); return FAC_ERR_INVALID; }
     fac_handle tmp;
     tmp.device = h->device;
-    tmp.use_tc = mode == 0 ? 0 : 1;          // 0: fp32 FMA, 1: two tensor-core launches, 2: fused launch; 3/4 = 1/2 with bf16 split;
-                                             // 5/6 = 3/4 with the k = 7 conv in one fp16 pass
-    tmp.fuse_res = (mode == 2 || mode == 4 || mode == 6) ? 1 : 0;
-    tmp.dec_bf16 = mode >= 3;
-    tmp.dec_c7_f16 = mode >= 5;
+    // 0: fp32 FMA, 1: two tensor-core launches, 2: fused launch; 3/4 = 1/2 with bf16 split; 5/6 = 3/4 with the k = 7 conv
+    // in one fp16 pass; 7/8 = 1/2 as an encoder unit (promoted fp16 hi + scaled lo, upstream of the VQ)
+    const bool enc = mode >= 7, fused = mode == 2 || mode == 4 || mode == 6 || mode == 8;
+    tmp.use_tc = mode == 0 ? 0 : (enc ? 2 : 1);
+    tmp.fuse_res = fused ? 1 : 0;
+    tmp.dec_bf16 = mode >= 3 && !enc;
+    tmp.dec_c7_f16 = mode >= 5 && !enc;
     tmp.tc_occ2 = h->tc_occ2;
     auto put = [&](const char* key, const float* d, std::vector<int64_t> shp) {
         HostTensor t;
@@ -4027,7 +4040,7 @@ int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host,
     put("u.block.3.conv.conv.weight", w1_host, {C, C, 1});
     put("u.block.3.conv.conv.bias", b1_host, {C});
     ResW r;
-    try { r = pack_res(&tmp, 0, "u", dil, false); } catch (const PackError& e) { h->err = e.msg; cudaFree(lanes); return FAC_ERR_STATE; }
+    try { r = pack_res(&tmp, 0, "u", dil, enc); } catch (const PackError& e) { h->err = e.msg; cudaFree(lanes); return FAC_ERR_STATE; }
     cudaSetDevice(h->device);
     cudaError_t e = cudaMalloc(&tmp.warena, (tmp.pack.size() + 64) * sizeof(float));
     if (e == cudaSuccess) e = cudaMemcpy(tmp.warena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
@@ -4039,11 +4052,12 @@ int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host,
     if (e != cudaSuccess) { h->err = cudaGetErrorString(e); rc = FAC_ERR_CUDA; }
     if (rc == FAC_OK) {
         Ctx c{&tmp, st, false};
+        c.vq_critical = enc;
         residual_unit(c, r, x, scratch, y, B, T, causal != 0, lanes);
         rc = finish(&tmp, c);
         cudaError_t e2 = cudaStreamSynchronize(st);
         if (rc == FAC_OK && e2 != cudaSuccess) { tmp.err = cudaGetErrorString(e2); rc = FAC_ERR_CUDA; }
-        if (rc == FAC_OK && (mode == 2 || mode == 4 || mode == 6) && tmp.launches != 1) { tmp.err = "fused path not taken for this geometry"; rc = FAC_ERR_UNSUPPORTED; }
+        if (rc == FAC_OK && fused && tmp.launches != 1) { tmp.err = "fused path not taken for this geometry"; rc = FAC_ERR_UNSUPPORTED; }
     }
     if (rc != FAC_OK) h->err = tmp.err;
     if (scratch) cudaFree(scratch);
@@ -4133,12 +4147,12 @@ int fac_debug_lane_pad_map(const int* lane_len, int B, int Tin, int pad_left, in
 
 // Host-only: the tile plan the tensor-core conv kernel would use for a layer geometry (no GPU, no handle).
 static int debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, TcConvParams& tp) {
-    if (Cin <= 0 || Cout <= 0 || K <= 0 || dil <= 0 || stride <= 0 || mode < 0 || mode > 8) return FAC_ERR_INVALID;
+    if (Cin <= 0 || Cout <= 0 || K <= 0 || dil <= 0 || stride <= 0 || mode < 0 || mode > 9) return FAC_ERR_INVALID;
     tp.Cin = Cin; tp.Cout = Cout; tp.Tout = Tout; tp.occ2_maxn = occ2_maxn;
-    tp.promoted = (mode == 1 || mode == 3) ? 1 : 0;
+    tp.promoted = (mode == 1 || mode == 3 || mode == 9) ? 1 : 0;
     tp.bf16 = (mode == 2 || mode == 4 || mode == 7 || mode == 8) ? 1 : 0;
-    tp.f16x2 = mode == 3 ? 1 : 0;
-    tp.fused = (mode == 4 || mode == 5 || mode == 8) ? 1 : 0;
+    tp.f16x2 = (mode == 3 || mode == 9) ? 1 : 0;
+    tp.fused = (mode == 4 || mode == 5 || mode == 8 || mode == 9) ? 1 : 0;     // 9: fused ResidualUnit of mode 3
     tp.g1f16 = (mode == 7 || mode == 8) ? 1 : 0;                     // 7 / 8: one-pass fp16 class, plain / fused
     if (mode == 6) { tp.promoted = 1; tp.f16x2 = 1; tp.tt = 1; }     // 6: transposed formulation of mode 3
     if (stride == 1) { tp.vf = 1; tp.Kr = K; tp.dil = dil; }

@@ -332,8 +332,10 @@ int fac_add3(fac_handle* h, const float* a, const float* b, const float* c, long
  * (encoder, prosody branch); 2 (default) = wgmma everywhere, with the promoted accumulation
  * variant upstream of the VQ where the bit-exact argmin needs fp32-grade sums.
  * "fuse_resunit": 1 (default) runs each decoder ResidualUnit whose channels fit one CTA tile as a single
- * fused launch (conv7 -> Snake -> 1x1 conv -> +x with the intermediate kept in shared memory); 0 = two launches;
- * 2 = fuse only units of at most 128 channels.
+ * fused launch (conv7 -> Snake -> 1x1 conv -> +x with the intermediate kept in shared memory), and so each encoder
+ * ResidualUnit of 64 or 128 channels when it runs the promoted fp16 hi + scaled-lo class ("tensor_cores" 2,
+ * "encoder_f16x2" 1, "encoder_tt" 0; bit-identical to its two launches); 0 = two launches; 2 = fuse only units of at
+ * most 128 channels.
  * "decoder_bf16": 1 (default) = layers downstream of the VQ split operands into bf16 hi + bf16 lo
  * (K = 16 MMAs: half the MMAs and half the operand bytes of the TF32 split; waveform error
  * ~1e-5 RMS against the 1e-4 bar, measured on the oracle), evaluate Snake with the SFU sine and run the LSTM recurrence on bf16 hi/lo

@@ -53,7 +53,9 @@ int fac_debug_conv_lanes(fac_handle* h, const float* x, const float* w_host, con
 /* One ResidualUnit (dac/model/dac.py:25-42) y = x + conv1(snake(conv7_d(snake(x)))) on DEVICE channels-last
  * x, y [B,T,C] with HOST folded weights w7 [C,C,7], w1 [C,C,1].  mode 0: fp32 FMA kernels, 1: two tensor-core
  * launches, 2: the single fused tensor-core launch (FAC_ERR_UNSUPPORTED if the geometry cannot be fused);
- * 3 / 4: as 1 / 2 with the bf16 hi/lo split; 5 / 6: as 3 / 4 with the k = 7 conv in one fp16 pass.  Causal. */
+ * 3 / 4: as 1 / 2 with the bf16 hi/lo split; 5 / 6: as 3 / 4 with the k = 7 conv in one fp16 pass; 7 / 8: as 1 / 2 for
+ * an encoder unit (weights packed for the promoted class, run upstream of the VQ: fp16 hi + 2^11-scaled lo, two CTAs per
+ * SM; 8 only at C = 64 and 128).  Any other mode returns FAC_ERR_INVALID.  Causal. */
 int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const float* b7_host, const float* w1_host,
                       const float* b1_host, const float* alpha1_host, const float* alpha2_host, int B, int T, int C,
                       int dil, int mode, float* y, void* stream);
@@ -105,7 +107,8 @@ int fac_debug_lane_pad_map(const int* lane_len, int B, int Tin, int pad_left, in
 /* Host-only (no GPU, no handle): the tile plan of the wgmma conv kernel for one layer geometry.  mode: 0 TF32,
  * 1 promoted TF32, 2 bf16, 3 promoted fp16 hi + scaled lo, 4 fused ResidualUnit bf16, 5 fused TF32, 6 mode 3 in the
  * transposed formulation, 7 ONE fp16 pass (the k = 7 convs downstream of the VQ), 8 fused ResidualUnit with its k = 7
- * conv in one fp16 pass.  occ2_maxn as the "tc_occ2_maxn" option.  Tout may be 0 (unknown).  out8 = {N, MT (2: warpgroups split 128 rows, 1: they split N over 64 rows),
+ * conv in one fp16 pass, 9 fused ResidualUnit in the class of mode 3 (N = C and two CTAs per SM, or unsupported).
+ * occ2_maxn as the "tc_occ2_maxn" option.  Tout may be 0 (unknown).  out8 = {N, MT (2: warpgroups split 128 rows, 1: they split N over 64 rows),
  * K chunks, weight-ring stages, rows per tile, dynamic shared-memory bytes, padded rows of the operand buffer,
  * chunks per promotion}.  FAC_ERR_UNSUPPORTED when the layer is not eligible. */
 int fac_debug_tc_plan(int Cin, int Cout, int K, int dil, int stride, int Tout, int mode, int occ2_maxn, int* out8);
