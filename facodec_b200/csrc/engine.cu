@@ -17,6 +17,7 @@
 #include "../../include/facodec_b200_debug.h"
 #include "common.cuh"
 #include "kernels.h"
+#include "resample.h"
 
 using namespace fac;
 
@@ -162,6 +163,7 @@ struct fac_handle {
     std::vector<std::unique_ptr<CodesPool>> codes_pools;    // many B = 1 compression streams (fac_codes_pool_*)
     std::vector<std::unique_ptr<VcPool>> vc_pools;          // many B = 1 voice-conversion streams (fac_vc_pool_*)
     std::vector<std::unique_ptr<DecPool>> dec_pools;        // many B = 1 decode-from-codes streams (fac_dec_pool_*)
+    fac::RsHost* rs = nullptr;      // resampler filter tables and session pools (fac_resample*, fac_rs_pool_*), made on use
     struct HeadSet;                 // modules/quantize.py:106-125 CNNLSTM instances (fac_head_*)
     std::vector<HeadSet*> heads;
     char* ws = nullptr; size_t ws_bytes = 0;
@@ -1551,6 +1553,7 @@ int fac_destroy(fac_handle* h) {
     if (h->spec_arena) cudaFree(h->spec_arena);
     for (float* p : h->rvq_arenas) if (p) cudaFree(p);
     for (auto* hs : h->heads) { if (hs->arena) cudaFree(hs->arena); delete hs; }
+    fac::rs_host_free(h->rs);
     delete h;   // and with it the streams' and pools' device state
     return FAC_OK;
 }
@@ -3051,6 +3054,51 @@ int fac_dec_pool_close(fac_handle* h, int pool_id, int session) {
 }
 
 int fac_dec_pool_destroy(fac_handle* h, int pool_id) { return free_by_id(h, &fac_handle::dec_pools, pool_id); }
+
+// Sinc resampling (resample.cu): the handle lends the resampler its device, error text, launch counter and state.
+static fac::RsEnv rs_env(fac_handle* h) { return fac::RsEnv{h->device, h->err, h->launches, h->rs}; }
+
+int fac_resample_geometry(int orig, int new_rate, int* out4) { return fac::rs_geometry(orig, new_rate, out4); }
+long long fac_resample_out_len(int orig, int new_rate, long long n) { return fac::rs_out_len(orig, new_rate, n); }
+long long fac_resample_ready(int orig, int new_rate, int quantum, long long seen, long long emitted) {
+    return fac::rs_ready(orig, new_rate, quantum, seen, emitted);
+}
+
+int fac_resample_table(fac_handle* h, int orig, int new_rate, const float* table_host) {
+    return h ? fac::rs_table(rs_env(h), orig, new_rate, table_host) : FAC_ERR_INVALID;
+}
+
+int fac_resample(fac_handle* h, const float* x, int B, int T, const int* lengths, int orig, int new_rate, float* y, void* stream) {
+    return h ? fac::rs_resample(rs_env(h), x, B, T, lengths, orig, new_rate, y, (cudaStream_t)stream) : FAC_ERR_INVALID;
+}
+
+int fac_rs_pool_create(fac_handle* h, int capacity, int quantum) {
+    return h ? fac::rs_pool_create(rs_env(h), capacity, quantum) : FAC_ERR_INVALID;
+}
+
+int fac_rs_pool_open(fac_handle* h, int pool_id, int orig, int new_rate) {
+    return h ? fac::rs_pool_open(rs_env(h), pool_id, orig, new_rate) : FAC_ERR_INVALID;
+}
+
+int fac_rs_pool_push(fac_handle* h, int pool_id, int n, const int* sessions, const int* T, const float* const* x, float* const* y,
+                     int* counts, void* stream) {
+    return h ? fac::rs_pool_step(rs_env(h), pool_id, n, sessions, T, x, y, counts, false, (cudaStream_t)stream) : FAC_ERR_INVALID;
+}
+
+int fac_rs_pool_finish(fac_handle* h, int pool_id, int n, const int* sessions, const int* T, const float* const* x,
+                       float* const* y, int* counts, void* stream) {
+    return h ? fac::rs_pool_step(rs_env(h), pool_id, n, sessions, T, x, y, counts, true, (cudaStream_t)stream) : FAC_ERR_INVALID;
+}
+
+int fac_rs_pool_undo(fac_handle* h, int pool_id, int n, const int* sessions) {
+    return h ? fac::rs_pool_undo(rs_env(h), pool_id, n, sessions) : FAC_ERR_INVALID;
+}
+
+int fac_rs_pool_close(fac_handle* h, int pool_id, int session) {
+    return h ? fac::rs_pool_close(rs_env(h), pool_id, session) : FAC_ERR_INVALID;
+}
+
+int fac_rs_pool_destroy(fac_handle* h, int pool_id) { return h ? fac::rs_pool_destroy(rs_env(h), pool_id) : FAC_ERR_INVALID; }
 
 int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch) {
     if (n < 0 || (n > 0 && (!counters || !lengths || !group || !batch)) || kind < 0 || kind > 2) return FAC_ERR_INVALID;

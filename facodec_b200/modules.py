@@ -13,6 +13,7 @@ Drop-in contract (SURVEY.md section 8b):
 * There is no CPU fallback: CPU tensors or a missing library raise.
 """
 import ctypes
+import math
 import operator
 import os
 from collections import OrderedDict
@@ -44,6 +45,7 @@ class Engine:
         self.device_index = None
         self.loaded_version = {}
         self.modules = {}
+        self._rs_pairs = set()      # reduced rate pairs whose resampler table this handle holds
 
     def _ensure(self, device):
         if device.type != "cuda":
@@ -736,6 +738,29 @@ class _StreamPool:
         self.engine, self.pid = engine, pid
         self.device = torch.device("cuda", engine.device_index)
         self._open = set()
+        self._rs = None           # sessions at other sample rates: one ResamplePool, made on the first such session
+        self._rate = {}           # session -> its ResamplePool session
+
+    def _rate_open(self, sample_rate, to_24k, quantum, open_session):
+        """Opens a session with open_session(); one at a sample rate other than 24 kHz also gets a resampler session
+        (sample_rate -> 24 kHz when to_24k, else 24 kHz -> sample_rate).  Returns (session, resampler session or None)."""
+        if self.pid is None:
+            raise _lib.FacError("pool is closed")
+        sr = operator.index(sample_rate)
+        rs = None
+        if sr != 24000:
+            if self._rs is None:
+                self._rs = ResamplePool(self.capacity, quantum, device=self.device, engine=self.engine)
+            rs = self._rs.open(sr, 24000) if to_24k else self._rs.open(24000, sr)
+        try:
+            s = open_session()
+        except Exception:
+            if rs is not None:
+                self._rs.close(rs)
+            raise
+        if rs is not None:
+            self._rate[s] = rs
+        return s, rs
 
     def _sessions(self, sessions):
         if self.pid is None:
@@ -759,11 +784,30 @@ class _StreamPool:
             s = self._sessions([session])[0]
             _lib.check(e.handle, getattr(e.L, "fac_%s_pool_close" % self._kind)(e.handle, self.pid, s), "pool close")
             self._open.discard(s)
+            if s in self._rate:
+                self._rs.close(self._rate.pop(s))
+            self._closed(s)
             return
+        if self._rs is not None:
+            self._rs.close()
+            self._rs = None
+        self._rate = {}
         if self.pid is not None and e.handle is not None:
             getattr(e.L, "fac_%s_pool_destroy" % self._kind)(e.handle, self.pid)
         self.pid = None
         self._open = set()
+
+    def _closed(self, s):
+        """Drops a closed session's host-side bookkeeping."""
+
+    def _resampled(self, outs, finish=False):
+        """{session: y [1,1,k]} at 24 kHz -> the same at each rate session's own rate, in one resampler launch (finish: the
+        y are the sessions' last chunks, and the result includes the resampler's flushed tail); 24 kHz sessions pass."""
+        rate = {self._rate[s]: y for s, y in outs.items() if s in self._rate}
+        if not rate:
+            return outs
+        got = self._rs.finish(rate) if finish else self._rs.push(rate)
+        return {s: got[self._rate[s]] if s in self._rate else y for s, y in outs.items()}
 
     def __enter__(self):
         return self
@@ -787,20 +831,81 @@ class CodecStreamPool(_StreamPool):
         _lib.check(engine.handle, pid, "fac_codes_pool_create")
         self._setup(engine, pid)
         self.capacity, self.n_c = int(capacity), int(n_c)
+        self._fed = {}            # session -> 24 kHz samples encoded so far
+        self._held = {}           # rate session -> 24 kHz samples not yet encoded (before its first 3000)
+        self._done = set()        # sessions whose finish_codes ran (open until closed)
 
-    def open(self):
-        """A new session id (a slot, reused after close()); raises FacError when the pool is full."""
-        if self.pid is None:
-            raise _lib.FacError("pool is closed")
+    def open(self, sample_rate=24000):
+        """A new session id (a slot, reused after close()); raises FacError when the pool is full.  A session at another
+        sample_rate (an integer in [8000, 192000], see resample()) takes chunks of any length: they are resampled to
+        24 kHz on the device, and whole 300-sample frames reach the encoder once 3000 samples exist."""
         e = self.engine
-        s = _lib.check(e.handle, e.L.fac_codes_pool_open(e.handle, self.pid, _stream(self.device)), "fac_codes_pool_open")
+
+        def open_session():
+            return _lib.check(e.handle, e.L.fac_codes_pool_open(e.handle, self.pid, _stream(self.device)), "fac_codes_pool_open")
+        s, rs = self._rate_open(sample_rate, True, 300, open_session)
         self._open.add(s)
+        self._fed[s] = 0
+        if rs is not None:
+            self._held[s] = self._empty()
         return s
+
+    def _closed(self, s):
+        self._fed.pop(s, None)
+        self._held.pop(s, None)
+        self._done.discard(s)
+
+    def _empty(self):
+        return torch.empty(0, device=self.device)
+
+    def _no_codes(self):
+        return [torch.empty(1, r, 0, device=self.device, dtype=torch.int64) for r in (1, self.n_c, 3)]
 
     def encode_codes(self, chunks):
         """{session: x [1,1,T]} (T per session, with the chunk rules of CodecStream.encode_codes) -> {session: [codes_p
         [1,1,F], codes_c [1,n_c,F], codes_r [1,3,F]]}, F = T/300 - 1 on a session's first chunk and T/300 after.  One
-        rejected entry rejects the whole step and leaves every session as it was."""
+        rejected entry rejects the whole step and leaves every session as it was.
+        A session opened at another sample rate takes any T >= 0; its chunks are resampled in one launch for the step, and
+        F counts the whole frames its encoder is fed: 0 until its first 3000 samples at 24 kHz, then the frames that
+        accumulated.  Its codes equal Codec.encode(r[..., :L]) with r = resample(x, sample_rate, 24000) of the whole
+        utterance and L = 300 * (len(r) // 300), once finish_codes() has added the rest."""
+        sessions = self._sessions(chunks.keys())
+        rate = [s for s in sessions if s in self._rate]
+        if not rate:
+            return self._encode(chunks)
+        for s in sessions:                  # every rule the encoder checks, before the resampler step
+            x = chunks[s]
+            self._check_device(x)
+            if x.dim() != 3 or x.shape[0] != 1 or x.shape[1] != 1:
+                raise ValueError("session %d: x must be [1, 1, T], got %s" % (s, tuple(x.shape)))
+            if s in self._done:
+                raise _lib.FacError("session %d: its utterance was finished by finish_codes" % s)
+            T = x.shape[2]
+            if s not in self._rate and (T <= 0 or T % 300 or (self._fed[s] == 0 and T < 3000)):
+                raise _lib.FacError("session %d: a chunk of %d samples (a positive multiple of 300, the first >= 3000)" % (s, T))
+        rs = [self._rate[s] for s in rate]
+        got = self._rs.push({self._rate[s]: chunks[s] for s in rate})
+        feed = {s: chunks[s] for s in sessions if s not in self._rate}
+        held = {}
+        for s in rate:
+            y = got[self._rate[s]].view(-1)
+            if self._fed[s] == 0:
+                y = torch.cat([self._held[s], y])
+                if y.numel() < 3000:
+                    held[s] = y
+                    continue
+                held[s] = self._empty()
+            if y.numel():
+                feed[s] = y.view(1, 1, -1)
+        try:
+            codes = self._encode(feed) if feed else {}
+        except Exception:
+            self._rs._undo(rs)              # the encoder rejected the step: give the resampler sessions their samples back
+            raise
+        self._held.update(held)
+        return {s: codes[s] if s in codes else self._no_codes() for s in sessions}
+
+    def _encode(self, chunks):
         sessions = self._sessions(chunks.keys())
         xs, Ts, outs = [], [], []
         for s in sessions:
@@ -822,13 +927,55 @@ class CodecStreamPool(_StreamPool):
                                              P(xs), P([o[0] for o in outs]), P([o[1] for o in outs]), P([o[2] for o in outs]),
                                              frames, _stream(self.device))
         _lib.check(e.handle, rc, "fac_codes_pool_encode_codes")
+        for s, T in zip(sessions, Ts):
+            self._fed[s] += T
         return {s: [t[:r * frames[i]].view(1, r, frames[i]) for t, r in zip(outs[i], (1, self.n_c, 3))]
                 for i, s in enumerate(sessions)}
 
     def finish_codes(self, sessions):
         """End of the sessions' utterances -> {session: ([codes_p, codes_c, codes_r] of the held-back frame, timbre [1,1024])},
-        as CodecStream.finish_codes."""
+        as CodecStream.finish_codes.  A session at another sample rate first flushes its resampler and encodes the whole
+        frames that remain (a tail of fewer than 300 samples is dropped), so its codes hold k >= 1 frames; an utterance
+        that resamples to fewer than 3000 samples raises FacError, as a short first chunk does."""
         sessions = self._sessions(sessions)
+        rate = [s for s in sessions if s in self._rate]
+        if not rate:
+            return self._finish(sessions)
+        for s in sessions:                  # the finish's rules, before the resampler and encoder steps
+            if s in self._done:
+                raise _lib.FacError("session %d: its utterance is already finished" % s)
+            n = self._fed[s]
+            if s in self._rate:
+                n += self._held[s].numel() + self._rs.pending(self._rate[s])
+            if self._fed[s] == 0 and n // 300 * 300 < 3000:
+                raise _lib.FacError("session %d: %d samples at 24 kHz, fewer than the 3000 a stream starts with" % (s, n))
+        rs = [self._rate[s] for s in rate]
+        tails = self._rs.finish(rs)
+        feed = {}
+        for s in rate:
+            y = torch.cat([self._held[s], tails[self._rate[s]].view(-1)])
+            whole = y.numel() // 300 * 300
+            if whole:
+                feed[s] = y[:whole].view(1, 1, whole)
+        try:
+            pre = self._encode(feed) if feed else {}
+        except Exception:
+            self._rs._undo(rs)
+            raise
+        try:
+            out = self._finish(sessions)
+        except Exception:
+            if not pre:                     # nothing reached the encoder: the step can still be taken back whole
+                self._rs._undo(rs)
+            raise
+        for s in rate:
+            self._held[s] = self._empty()
+        for s in pre:
+            codes, timbre = out[s]
+            out[s] = ([torch.cat([a, b], dim=2) for a, b in zip(pre[s], codes)], timbre)
+        return out
+
+    def _finish(self, sessions):
         outs = [[torch.empty(1, r, 1, device=self.device, dtype=torch.int64) for r in (1, self.n_c, 3)] for _ in sessions]
         timbres = [torch.empty(1, 1024, device=self.device) for _ in sessions]
         P = lambda ts: _ptr_array(ctypes.c_void_p, [t.data_ptr() for t in ts])
@@ -837,6 +984,7 @@ class CodecStreamPool(_StreamPool):
                                              P([o[0] for o in outs]), P([o[1] for o in outs]), P([o[2] for o in outs]), P(timbres),
                                              _stream(self.device))
         _lib.check(e.handle, rc, "fac_codes_pool_finish_codes")
+        self._done.update(sessions)
         return {s: (outs[i], timbres[i]) for i, s in enumerate(sessions)}
 
 
@@ -856,8 +1004,9 @@ class VoiceConversionPool(_StreamPool):
         self.capacity = int(capacity)
         self.lookahead_frames = engine.L.fac_vc_stream_lookahead()
 
-    def open(self, timbre):
-        """A new session converting to ``timbre`` [1,1024]; raises FacError when the pool is full."""
+    def open(self, timbre, sample_rate=24000):
+        """A new session converting to ``timbre`` [1,1024]; raises FacError when the pool is full.  A session at another
+        sample_rate gets its audio resampled from 24 kHz on the device (one launch per step for all such sessions)."""
         if self.pid is None:
             raise _lib.FacError("pool is closed")
         self._check_device(timbre)
@@ -865,14 +1014,21 @@ class VoiceConversionPool(_StreamPool):
         if tuple(tv.shape) != (1, 1024):
             raise ValueError("timbre must be [1, 1024], got %s" % (tuple(tv.shape),))
         e = self.engine
-        s = _lib.check(e.handle, e.L.fac_vc_pool_open(e.handle, self.pid, _ptr(tv), _stream(self.device)), "fac_vc_pool_open")
+
+        def open_session():
+            return _lib.check(e.handle, e.L.fac_vc_pool_open(e.handle, self.pid, _ptr(tv), _stream(self.device)), "fac_vc_pool_open")
+        s, _ = self._rate_open(sample_rate, False, 1, open_session)
         self._open.add(s)
         return s
 
     def convert(self, chunks):
         """{session: codes} (codes[0] [1,1,F], codes[1] [1,1|2,F], as VoiceConversionStream.convert takes them) -> {session:
-        y [1,1,300 k]}.  Codes outside [0, 1024) raise IndexError (one device reduction + one host sync for the step); one
+        y [1,1,300 k]}, or [1,1,k'] at a session's own sample rate: concatenated with finish(), resample() of the 24 kHz
+        output.  Codes outside [0, 1024) raise IndexError (one device reduction + one host sync for the step); one
         rejected entry rejects the whole step and leaves every session as it was."""
+        return self._resampled(self._convert(chunks))
+
+    def _convert(self, chunks):
         sessions = self._sessions(chunks.keys())
         cps, ccs, ys, Fs = [], [], [], []
         for s in sessions:
@@ -908,7 +1064,11 @@ class VoiceConversionPool(_StreamPool):
         return cp, cc, F
 
     def finish(self, sessions):
-        """End of the sessions' utterances -> {session: y [1,1,300 k]}, the last k <= lookahead_frames frames."""
+        """End of the sessions' utterances -> {session: y [1,1,300 k]}, the last k <= lookahead_frames frames (at a session's
+        own sample rate: resampled, with the resampler's flushed tail)."""
+        return self._resampled(self._finish(sessions), finish=True)
+
+    def _finish(self, sessions):
         sessions = self._sessions(sessions)
         ys = [torch.empty(300 * self.lookahead_frames, device=self.device) for _ in sessions]
         frames = (ctypes.c_int * max(len(sessions), 1))()
@@ -923,8 +1083,8 @@ class CodecDecodePool(_StreamPool):
     """Many live receivers decoding codes back to audio (CodecStream.decode_codes with B = 1 each, every one with its own
     timbre) stepped in shared launches; each session's audio equals that of its own B = 1 CodecStream fed the same chunks and
     timbre, bit for bit (fac_dec_pool_*).  Chunk lengths and code rows (1-2 content, 0-3 residual: the bitrate) may change
-    from step to step and differ between sessions that share a batch.  The decoder is causal, so there is no finish step:
-    every frame is final when it arrives."""
+    from step to step and differ between sessions that share a batch.  The decoder is causal, so every frame is final when
+    it arrives; finish() only flushes the resampler of a session at another sample rate."""
 
     _kind = "dec"
 
@@ -936,9 +1096,14 @@ class CodecDecodePool(_StreamPool):
         _lib.check(engine.handle, pid, "fac_dec_pool_create")
         self._setup(engine, pid)
         self.capacity = int(capacity)
+        self._finished = set()    # sessions whose finish() ran (open until closed)
 
-    def open(self, timbre):
-        """A new session decoding with ``timbre`` [1,1024]; raises FacError when the pool is full."""
+    def _closed(self, s):
+        self._finished.discard(s)
+
+    def open(self, timbre, sample_rate=24000):
+        """A new session decoding with ``timbre`` [1,1024]; raises FacError when the pool is full.  A session at another
+        sample_rate gets its audio resampled from 24 kHz on the device (one launch per step for all such sessions)."""
         if self.pid is None:
             raise _lib.FacError("pool is closed")
         self._check_device(timbre)
@@ -946,14 +1111,38 @@ class CodecDecodePool(_StreamPool):
         if tuple(tv.shape) != (1, 1024):
             raise ValueError("timbre must be [1, 1024], got %s" % (tuple(tv.shape),))
         e = self.engine
-        s = _lib.check(e.handle, e.L.fac_dec_pool_open(e.handle, self.pid, _ptr(tv), _stream(self.device)), "fac_dec_pool_open")
+
+        def open_session():
+            return _lib.check(e.handle, e.L.fac_dec_pool_open(e.handle, self.pid, _ptr(tv), _stream(self.device)), "fac_dec_pool_open")
+        s, _ = self._rate_open(sample_rate, False, 1, open_session)
         self._open.add(s)
         return s
 
     def decode_codes(self, chunks):
         """{session: [codes_p [1,1,F], codes_c [1,1|2,F], codes_r [1,0..3,F] or None]} (F per session; a session's first
-        chunk >= 10 frames) -> {session: y [1,1,300 F]}.  Codes outside [0, 1024) raise IndexError (one device reduction +
-        one host sync for the step); one rejected entry rejects the whole step and leaves every session as it was."""
+        chunk >= 10 frames) -> {session: y [1,1,300 F]}, or [1,1,k] at a session's own sample rate.  Codes outside [0, 1024)
+        raise IndexError (one device reduction + one host sync for the step); one rejected entry rejects the whole step and
+        leaves every session as it was; so does a session that finish() has ended."""
+        for s in self._sessions(chunks.keys()):
+            if s in self._finished:
+                raise _lib.FacError("session %d: its code stream was ended by finish()" % s)
+        return self._resampled(self._decode(chunks))
+
+    def finish(self, sessions):
+        """End of the sessions' code streams -> {session: y [1,1,k]}: the resampler's flushed tail of a session at another
+        sample rate, empty at 24 kHz (the causal decoder itself holds nothing back).  Concatenated with its decode_codes
+        outputs, a session's audio equals resample() of its 24 kHz audio.  An ended session takes no more codes until
+        close()."""
+        sessions = self._sessions(sessions)
+        for s in sessions:
+            if s in self._finished:
+                raise _lib.FacError("session %d: its code stream is already ended" % s)
+        outs = {s: torch.empty(1, 1, 0, device=self.device) for s in sessions}
+        outs = self._resampled(outs, finish=True)
+        self._finished.update(sessions)
+        return outs
+
+    def _decode(self, chunks):
         sessions = self._sessions(chunks.keys())
         cps, ccs, crs, ys = [], [], [], []
         for s in sessions:
@@ -988,6 +1177,198 @@ class CodecDecodePool(_StreamPool):
                                            _stream(self.device))
         _lib.check(e.handle, rc, "fac_dec_pool_decode_codes")
         return {s: ys[i] for i, s in enumerate(sessions)}
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# Sample-rate conversion (fac_resample*, fac_rs_pool_*): torchaudio.functional.resample with its defaults, on the device.
+# ------------------------------------------------------------------------------------------------------------------------
+
+_RS_ENGINES = {}
+
+
+def _rs_geometry(orig_freq, new_freq):
+    """(orig, new, width, K) of the reduced pair; ValueError for an unsupported one."""
+    g = (ctypes.c_int * 4)()
+    if _lib.load().fac_resample_geometry(operator.index(orig_freq), operator.index(new_freq), g) < 0:
+        raise ValueError("unsupported rate pair %s -> %s: integer rates in [8000, 192000] whose reduced filter table holds "
+                         "at most 65536 floats" % (orig_freq, new_freq))
+    return tuple(g)
+
+
+def resample_table(orig_freq, new_freq):
+    """The float32 filter table [new, K] of the reduced pair, as torchaudio's _get_sinc_resample_kernel(orig_freq, new_freq,
+    gcd, dtype=torch.float32) builds it (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99), step for step with the same
+    torch ops on the CPU: torch's float32 sin and cos are not the C library's, and the table is meant to be torchaudio's bit
+    for bit.  Equal rates give the one-tap table [[1]]."""
+    o, n, width, K = _rs_geometry(orig_freq, new_freq)
+    if o == n:
+        return torch.ones(1, 1)
+    lowpass_filter_width = 6
+    base_freq = min(o, n)
+    base_freq *= 0.99
+    idx = torch.arange(-width, width + o, dtype=torch.float32)[None, None] / o
+    t = torch.arange(0, -n, -1, dtype=torch.float32)[:, None, None] / n + idx
+    t *= base_freq
+    t = t.clamp_(-lowpass_filter_width, lowpass_filter_width)
+    window = torch.cos(t * math.pi / lowpass_filter_width / 2) ** 2
+    t *= math.pi
+    scale = base_freq / o
+    kernels = torch.where(t == 0, torch.tensor(1.0).to(t), t.sin() / t)
+    kernels *= window * scale
+    return kernels.reshape(n, K).contiguous()
+
+
+def _rs_engine(device):
+    """The engine of resample() calls on `device` (no weights: it holds the filter tables)."""
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    e = _RS_ENGINES.get(idx)
+    if e is None:
+        e = _RS_ENGINES[idx] = Engine()
+        e._ensure(torch.device("cuda", idx))
+    return e
+
+
+def _rs_register(engine, orig_freq, new_freq):
+    """Uploads the pair's filter table to the engine's device once."""
+    key = _rs_geometry(orig_freq, new_freq)[:2]
+    if key not in engine._rs_pairs:
+        tab = resample_table(orig_freq, new_freq)
+        _lib.check(engine.handle, engine.L.fac_resample_table(engine.handle, int(orig_freq), int(new_freq), _ptr(tab)),
+                   "fac_resample_table")
+        engine._rs_pairs.add(key)
+
+
+def resample_length(orig_freq, new_freq, n):
+    """Samples that n input samples resample to: ceil(new n / orig) of the reduced pair."""
+    r = _lib.load().fac_resample_out_len(operator.index(orig_freq), operator.index(new_freq), operator.index(n))
+    if r < 0:
+        _rs_geometry(orig_freq, new_freq)
+        raise ValueError("n must be >= 0")
+    return r
+
+
+def resample(x, orig_freq, new_freq, lengths=None):
+    """torchaudio.functional.resample(x, orig_freq, new_freq) (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99) on the
+    GPU: x [B,1,T] or [B,T] float on a CUDA device -> [B,1,T'] or [B,T'], T' = ceil(new T / orig) with the pair reduced by
+    its gcd.  Integer rates in [8000, 192000]; equal rates copy.  Each output sums its K taps in fp32 in a fixed order, so
+    it is the same bit for bit whatever batch or stream it is computed in (ResamplePool equals this call on the
+    concatenated input).  Against torchaudio on the CPU the outputs agree to within float32 rounding of the same sums.
+    lengths: B sample counts in [0, T]; lane b resamples x[b, ..., :lengths[b]] and is 0 past its own ceil(new n_b / orig)
+    samples.  This is not librosa.load(sr=...)'s resampler (soxr, a different filter): audio loaded by librosa at 24 kHz
+    and audio resampled here differ by more than rounding."""
+    if x.device.type != "cuda":
+        raise _lib.FacError("resample runs on CUDA tensors only (no CPU fallback); got " + str(x.device))
+    if x.dim() not in (2, 3) or (x.dim() == 3 and x.shape[1] != 1):
+        raise ValueError("x must be [B, 1, T] or [B, T], got %s" % (tuple(x.shape),))
+    e = _rs_engine(x.device)
+    _rs_register(e, orig_freq, new_freq)
+    B, T = x.shape[0], x.shape[-1]
+    Tout = resample_length(orig_freq, new_freq, T)
+    y = torch.empty(tuple(x.shape[:-1]) + (Tout,), device=x.device)
+    if B == 0 or T == 0:
+        return y
+    lanes = _c_ints(None if lengths is None else _lane_counts(lengths, B, 0, T, "lengths"))
+    xc = _f32c(x)
+    with torch.cuda.device(x.device):
+        rc = e.L.fac_resample(e.handle, _ptr(xc), B, T, lanes, int(orig_freq), int(new_freq), _ptr(y), _stream(x.device))
+    _lib.check(e.handle, rc, "fac_resample")
+    return y
+
+
+class ResamplePool(_StreamPool):
+    """Many live resampler sessions, each with its own rate pair, stepped in one launch per step (fac_rs_pool_*).  A
+    session's outputs, concatenated over its push() steps and finish(), equal resample() of its concatenated input bit for
+    bit, whatever the chunking.  push() returns every output whose window lies inside the input so far, rounded down to a
+    multiple of ``quantum``; finish() returns the rest.  The counts follow from the chunk lengths alone: no step waits for
+    the device."""
+
+    _kind = "rs"
+
+    def __init__(self, capacity=256, quantum=1, device=None, engine=None):
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        engine = engine if engine is not None else _rs_engine(dev)
+        engine._ensure(dev)
+        pid = engine.L.fac_rs_pool_create(engine.handle, int(capacity), int(quantum))
+        _lib.check(engine.handle, pid, "fac_rs_pool_create")
+        self._setup(engine, pid)
+        self.capacity, self.quantum = int(capacity), int(quantum)
+        self._state = {}          # session -> [orig, new, samples pushed, outputs returned]
+        self._prev = {}           # session -> its _state before its last step
+
+    def open(self, orig_freq, new_freq):
+        """A new session resampling orig_freq -> new_freq; ValueError for an unsupported pair, FacError when full."""
+        if self.pid is None:
+            raise _lib.FacError("pool is closed")
+        e = self.engine
+        _rs_register(e, orig_freq, new_freq)
+        s = _lib.check(e.handle, e.L.fac_rs_pool_open(e.handle, self.pid, int(orig_freq), int(new_freq)), "fac_rs_pool_open")
+        self._open.add(s)
+        self._state[s] = [int(orig_freq), int(new_freq), 0, 0]
+        self._prev.pop(s, None)
+        return s
+
+    def _closed(self, s):
+        self._state.pop(s, None)
+        self._prev.pop(s, None)
+
+    def _undo(self, sessions):
+        """Takes back each session's last push or finish (fac_rs_pool_undo): for a caller whose own step on the outputs was
+        rejected.  The outputs that step returned are to be discarded."""
+        sessions = self._sessions(sessions)
+        e = self.engine
+        _lib.check(e.handle, e.L.fac_rs_pool_undo(e.handle, self.pid, len(sessions), _ptr_array(ctypes.c_int, sessions)),
+                   "fac_rs_pool_undo")
+        for s in sessions:
+            self._state[s] = self._prev.pop(s)
+
+    def pending(self, session):
+        """Outputs finish() would return now (known on the host)."""
+        o, n, seen, emitted = self._state[session]
+        return resample_length(o, n, seen) - emitted
+
+    def _chunk(self, s, x):
+        self._check_device(x)
+        if x.dim() > 3 or any(d != 1 for d in x.shape[:-1]):
+            raise ValueError("session %d: a chunk is [T], [1, T] or [1, 1, T], got %s" % (s, tuple(x.shape)))
+        return _f32c(x).view(-1)
+
+    def _step(self, chunks, finish):
+        sessions = self._sessions(chunks.keys())
+        xs = [None if chunks[s] is None else self._chunk(s, chunks[s]) for s in sessions]
+        Ts = [0 if x is None else x.numel() for x in xs]
+        L = self.engine.L
+        counts = []
+        for s, T in zip(sessions, Ts):
+            o, n, seen, emitted = self._state[s]
+            counts.append(resample_length(o, n, seen + T) - emitted if finish else L.fac_resample_ready(o, n, self.quantum, seen + T, emitted))
+        buf = torch.empty(sum(counts), device=self.device)      # one allocation for the step's outputs
+        ys = list(torch.split(buf, counts)) if counts else []
+        got = (ctypes.c_int * max(len(sessions), 1))()
+        P = lambda ts: _ptr_array(ctypes.c_void_p, [0 if t is None or t.numel() == 0 else t.data_ptr() for t in ts])
+        e = self.engine
+        fn = L.fac_rs_pool_finish if finish else L.fac_rs_pool_push
+        rc = fn(e.handle, self.pid, len(sessions), _ptr_array(ctypes.c_int, sessions), _ptr_array(ctypes.c_int, Ts), P(xs), P(ys),
+                got, _stream(self.device))
+        _lib.check(e.handle, rc, "fac_rs_pool_finish" if finish else "fac_rs_pool_push")
+        for i, s in enumerate(sessions):
+            assert got[i] == counts[i], (s, got[i], counts[i])
+            self._prev[s] = list(self._state[s])
+            self._state[s][2] += Ts[i]
+            self._state[s][3] += counts[i]
+        return {s: ys[i].view(1, 1, -1) for i, s in enumerate(sessions)}
+
+    def push(self, chunks):
+        """{session: x} (x [T], [1,T] or [1,1,T] on the pool's device, any T >= 0) -> {session: y [1,1,k]}.  One rejected
+        entry rejects the whole step and leaves every session as it was."""
+        return self._step(chunks, False)
+
+    def finish(self, sessions):
+        """End of the sessions' input -> {session: y [1,1,k]}, the rest of each session's output.  ``sessions`` is a list,
+        or a dict {session: last chunk} to push one last chunk in the same launch.  A finished session takes no more
+        input; close() frees it."""
+        if not isinstance(sessions, dict):
+            sessions = {s: None for s in sessions}
+        return self._step(sessions, True)
 
 
 class _HeadLinear(nn.Module):

@@ -259,6 +259,53 @@ int fac_dec_pool_decode_codes(fac_handle* h, int pool_id, int n, const int* sess
 int fac_dec_pool_close(fac_handle* h, int pool_id, int session);
 int fac_dec_pool_destroy(fac_handle* h, int pool_id);
 
+/* Sample-rate conversion: torchaudio.functional.resample(x, orig, new) with its defaults (sinc_interp_hann,
+ * lowpass_filter_width 6, rolloff 0.99).  Rates are integers in [8000, 192000]; with the pair reduced by its gcd,
+ * width = ceil(6 orig / (min(orig, new) * 0.99)) and the table holds K = 2 width + orig taps for each of `new` phases; pairs
+ * with K * new > 65536 are FAC_ERR_INVALID (every pair between 24 kHz and 8, 11.025, 16, 22.05, 32, 44.1, 48, 96 or 192 kHz
+ * fits).  n input samples give ceil(new n / orig) outputs; output j sums its K taps in fp32 with fmaf in ascending order,
+ * and that order depends on j alone, so a lane of a batch and every session of a pool equal their own offline B = 1 call bit
+ * for bit.  Equal rates copy.
+ * fac_resample_geometry: host only; out4 = {reduced orig, reduced new, width, K}.
+ * fac_resample_out_len: host only; ceil(new n / orig), or a negative status.
+ * fac_resample_table: registers the float32 filter table [new][K] of a pair (reduced, as fac_resample_geometry gives it) and
+ * uploads it once per handle; later calls for the pair are no-ops.  The table is torchaudio's _get_sinc_resample_kernel(...,
+ * dtype=torch.float32) bit for bit, whose sin / cos are torch's own: a C++ build of the same formula with the C library's
+ * sinf / cosf differs in the last bit in about 0.7 % of the taps.  facodec_b200.modules.resample_table builds it (its
+ * recipe, 15 lines of torch ops, is the reference for any other host); a C caller computes it once per pair that way or
+ * takes it from torchaudio, and registers it here.  The other calls return FAC_ERR_STATE for a pair without a table.
+ * fac_resample: x [B,T] (device) -> y [B,ceil(new T / orig)].  lengths: NULL or a HOST array of B counts in [0, T]; lane b
+ * resamples x[b, :lengths[b]] and writes 0 past its ceil(new lengths[b] / orig) outputs.
+ * Resampler pools: live sessions, each with its own rate pair, stepped in one launch (up to 256 lanes per launch).
+ * fac_rs_pool_create(capacity, quantum >= 1) -> pool id.  fac_rs_pool_open(orig, new) -> session id.
+ * fac_rs_pool_push: session sessions[i] takes x[i] [T[i]] (T >= 0) and writes counts[i] outputs to y[i]: every output whose
+ * whole window lies inside the input so far (fac_resample_ready), rounded down to a multiple of the quantum.
+ * fac_resample_ready: host only; that count for a session that has seen `seen` samples and returned `emitted` outputs.
+ * fac_rs_pool_finish: the end of the sessions' input, after an optional last chunk (T / x may be NULL): writes the rest,
+ * counts[i] = ceil(new seen / orig) - emitted, with the input zero-padded as fac_resample pads it.  A finished session takes
+ * no more input until it is closed.  Concatenated, a session's outputs equal fac_resample of its concatenated input.
+ * fac_rs_pool_undo: takes back each named session's last push or finish (the outputs it wrote are to be discarded), for a
+ * caller whose own step on those outputs was rejected; a session can take back one step, and open / close forget it.
+ * A slot keeps the input from the window of its first output not yet returned (at most K + orig ceil((quantum - 1) / new)
+ * samples) in two buffers: a step writes the other one and the slot flips once the launch is queued, so a rejected step
+ * leaves every session as it was.  Counts follow from the pushed lengths alone: no call synchronises with the device.
+ * fac_last_launch_count after fac_resample / fac_rs_pool_push / fac_rs_pool_finish counts that call's launches alone
+ * (1 for up to 256 lanes). */
+int fac_resample_geometry(int orig, int new_rate, int* out4);
+long long fac_resample_out_len(int orig, int new_rate, long long n);
+long long fac_resample_ready(int orig, int new_rate, int quantum, long long seen, long long emitted);
+int fac_resample_table(fac_handle* h, int orig, int new_rate, const float* table_host);
+int fac_resample(fac_handle* h, const float* x, int B, int T, const int* lengths, int orig, int new_rate, float* y, void* stream);
+int fac_rs_pool_create(fac_handle* h, int capacity, int quantum);
+int fac_rs_pool_open(fac_handle* h, int pool_id, int orig, int new_rate);
+int fac_rs_pool_push(fac_handle* h, int pool_id, int n, const int* sessions, const int* T, const float* const* x, float* const* y,
+                     int* counts, void* stream);
+int fac_rs_pool_finish(fac_handle* h, int pool_id, int n, const int* sessions, const int* T, const float* const* x,
+                       float* const* y, int* counts, void* stream);
+int fac_rs_pool_undo(fac_handle* h, int pool_id, int n, const int* sessions);
+int fac_rs_pool_close(fac_handle* h, int pool_id, int session);
+int fac_rs_pool_destroy(fac_handle* h, int pool_id);
+
 /* quantize/rvq.py:27-75 ResidualVQ.forward (eval) over quantize/fvq.py FactorizedVectorQuantize,
  * dim=1024, codebook_dim=8, 2^10 entries (BASELINE configs[3]).  Parameters are passed directly
  * (already weight-normed, HOST): per quantizer q: in_w [8,1024], in_b [8], out_w [1024,8],
