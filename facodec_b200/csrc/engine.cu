@@ -1674,6 +1674,17 @@ QuantOut codec_encode(Ctx& c, const float* x, int B, int T, int n_c, int64_t* co
                              false, forked ? &fr : nullptr, ln);
 }
 
+// The timbre of codec_encode alone: the launches quantizer_front runs for it (mel80 -> StyleEncoder, promoted class, the
+// same lanes), and no encoder, prosody or VQ launch.  timbre [B][1024].
+void codec_timbre(Ctx& c, const float* x, int B, int T, float* timbre, const Lanes* ln = nullptr) {
+    const bool was_critical = c.vq_critical;
+    c.vq_critical = true;
+    const int Tm = T / HOP;
+    const float* mel = mel_forward(c, x, B, T, Tm, nullptr, lane_at(ln, 0));
+    style_encoder(c, mel, B, Tm, nullptr, timbre, ln);
+    c.vq_critical = was_critical;
+}
+
 // The lanes of a ragged encode of B lanes of lens[b] samples (kLaneRows rows, see Lanes), uploaded by the caller's Ctx.
 std::vector<int> encode_lane_rows(const DecW& d, const int* lens, int B) {
     static const int rates[4] = {2, 5, 5, 6};
@@ -1783,6 +1794,17 @@ int fac_codec_encode_lens(fac_handle* h, const float* x, int B, int T, const int
 int fac_codec_encode(fac_handle* h, const float* x, int B, int T, int n_c, int64_t* codes_p, int64_t* codes_c,
                      int64_t* codes_r, float* timbre, void* stream) {
     return fac_codec_encode_lens(h, x, B, T, nullptr, n_c, codes_p, codes_c, codes_r, timbre, stream);
+}
+
+int fac_codec_timbre_lens(fac_handle* h, const float* x, int B, int T, const int* lengths, float* timbre, void* stream) {
+    if (int rc = check_ready(h, {FAC_QUANTIZER})) return rc;
+    if (!x || !timbre || B <= 0 || T <= N_FFT / 2) { h->err = "fac_codec_timbre: bad arguments"; return FAC_ERR_INVALID; }
+    if (int rc = lane_counts(h, lengths, B, N_FFT / 2 + 1, T, "fac_codec_timbre_lens: lengths")) return rc;
+    const std::vector<int> rows = lengths ? encode_lane_rows(h->dec, lengths, B) : std::vector<int>();
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        const Lanes ln = upload_lanes(c, rows, B);
+        codec_timbre(c, x, B, T, timbre, lengths ? &ln : nullptr);
+    });
 }
 
 int fac_dequantize(fac_handle* h, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, const int64_t* codes_r,
@@ -2244,6 +2266,13 @@ int stream_finish_codes_check(fac_handle* h, const EncHalf& s, const char* who) 
     return stream_codes_supported(h, who);
 }
 
+// Mel row N - 1 (N = samples / 300) of a half fed by fac_stream_encode_codes, as if the utterance ended now: cut from
+// the last `hist` samples [B][hist] (x_hist rows) reflected at their end, where the row sits at hist / 300 - 1.
+// [B][1][80] in workspace.
+const float* last_mel_row(Ctx& c, const float* xw, int B, int hist) {
+    return mel_frames_tc(c, quantizer_mel(c.h), xw, B, hist, hist / HOP - 1, 1);
+}
+
 // fac_stream_finish_codes on a checked half whose mel rows start at frame 0 (a stream, or a pool session's B = 1 slot,
 // which keeps all of its mel rows): returns the frames written (1) or a negative status.
 int finish_codes(fac_handle* h, EncHalf& s, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre,
@@ -2256,7 +2285,7 @@ int finish_codes(fac_handle* h, EncHalf& s, int64_t* codes_p, int64_t* codes_c, 
         // frame N - 1 from the last `hist` samples, reflected at the utterance's true end
         float* xw = c.alloc<float>((size_t)B * hist);
         copy_rows(c, xw, hist, s.x_hist, kEncCtx, 0, hist, 1, B, "stream.xfin");
-        const float* mel = mel_frames_tc(c, quantizer_mel(h), xw, B, hist, (int)(E - (s.samples - hist) / HOP), 1);
+        const float* mel = last_mel_row(c, xw, B, hist);
         copy_rows(c, s.mel.get() + (size_t)E * N_MELS, s.mel_cap, mel, 1, 0, 1, N_MELS, B, "stream.mel");
         stream_codes(c, s, (int)E - win, win, 1, s.z_held, 1, codes_p, codes_c, codes_r);
         if (timbre) {
@@ -2271,6 +2300,23 @@ int finish_codes(fac_handle* h, EncHalf& s, int64_t* codes_p, int64_t* codes_c, 
     s.emitted = N;
     s.mode = EncHalf::kFinished;
     return 1;
+}
+
+// The timbre finish_codes would return if the utterance ended now, for a checked half whose mel rows start at frame 0:
+// the StyleEncoder over its N mel rows, the kept N - 1 and the last cut by last_mel_row, gathered in workspace.  s is
+// not changed.
+int stream_timbre(fac_handle* h, const EncHalf& s, float* timbre, void* stream) {
+    const int B = s.B, hist = s.x_hist_len, N = (int)(s.samples / HOP);
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        c.vq_critical = true;
+        float* melall = c.alloc<float>((size_t)B * N * N_MELS);
+        copy_rows(c, melall, N, s.mel.get(), s.mel_cap, 0, N - 1, N_MELS, B, "stream.melall");
+        float* xw = c.alloc<float>((size_t)B * hist);
+        copy_rows(c, xw, hist, s.x_hist, kEncCtx, 0, hist, 1, B, "stream.xfin");
+        copy_rows(c, melall + (size_t)(N - 1) * N_MELS, N, last_mel_row(c, xw, B, hist), 1, 0, 1, N_MELS, B, "stream.mel_last");
+        style_encoder(c, melall, B, N, nullptr, timbre);
+        c.vq_critical = false;
+    });
 }
 }  // namespace
 
@@ -2322,6 +2368,15 @@ int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int6
     if (!st || !codes_p || !codes_c || !codes_r) { h->err = "fac_stream_finish_codes: bad arguments"; return FAC_ERR_INVALID; }
     if ((rc = stream_finish_codes_check(h, st->enc, "fac_stream_finish_codes"))) return rc;
     return finish_codes(h, st->enc, codes_p, codes_c, codes_r, timbre, stream);
+}
+
+int fac_stream_timbre(fac_handle* h, int stream_id, float* timbre, void* stream) {
+    int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER});
+    if (rc) return rc;
+    Stream* st = by_id(h, &fac_handle::streams, stream_id);
+    if (!st || !timbre) { h->err = "fac_stream_timbre: bad arguments"; return FAC_ERR_INVALID; }
+    if ((rc = stream_finish_codes_check(h, st->enc, "fac_stream_timbre"))) return rc;
+    return stream_timbre(h, st->enc, timbre, stream);
 }
 
 }  // extern "C"
@@ -2730,6 +2785,67 @@ int codes_pool_batch(fac_handle* h, CodesPool& P, const std::vector<int>& b, con
     return FAC_OK;
 }
 
+// Lanes x longest lane of one codes-pool timbre batch stay within this many mel frames (~16 KB of StyleEncoder workspace
+// each: ~0.5 GB), so an hour-long session does not grow the workspace by the batch's width; a longer session runs alone.
+constexpr long long kTimbreFrameBudget = 1 << 15;
+
+// Batches of a codes-pool timbre call over sessions of N[i] mel frames: by N (stable), each batch as many sessions as
+// fit kLaneMax lanes and kTimbreFrameBudget frames.
+std::vector<std::vector<int>> timbre_plan(const std::vector<int>& N) {
+    std::vector<int> order(N.size());
+    for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return N[a] < N[b]; });
+    std::vector<std::vector<int>> batches;
+    for (int i : order) {
+        if (batches.empty() || (int)batches.back().size() == kLaneMax ||
+            (long long)(batches.back().size() + 1) * N[i] > kTimbreFrameBudget)
+            batches.emplace_back();
+        batches.back().push_back(i);
+    }
+    return batches;
+}
+
+// One batch of a codes-pool timbre call: inputs b of the step's sessions, each the StyleEncoder lane of its own N mel
+// rows -- the N - 1 its slot keeps and the last one cut by last_mel_row (lanes with equal sample histories share that
+// launch) -- in one ragged StyleEncoder; each lane is the session's B = 1 stream_timbre, bit for bit.
+int codes_pool_timbre_batch(fac_handle* h, CodesPool& P, const std::vector<int>& b, const int* sessions,
+                            float* const* timbre, cudaStream_t st) {
+    const int nb = (int)b.size();
+    auto sl = [&](int j) -> const EncHalf& { return P.slot[sessions[b[j]]]; };
+    std::vector<int> rows((size_t)kLaneRows * nb, 0), N(nb);
+    std::map<int, std::vector<int>> by_hist;     // lanes by sample history
+    int Tm = 0;
+    for (int j = 0; j < nb; ++j) {
+        N[j] = (int)(sl(j).samples / HOP);
+        rows[(size_t)kTmRow * nb + j] = N[j];
+        Tm = std::max(Tm, N[j]);
+        by_hist[sl(j).x_hist_len].push_back(j);
+    }
+    return two_pass(h, st, [&](Ctx& c) {
+        c.vq_critical = true;
+        const Lanes ln = upload_lanes(c, rows, nb);
+        const size_t pitch = (size_t)Tm * N_MELS;
+        float* mel = c.alloc<float>((size_t)nb * pitch);
+        if (!c.dry) c.check_nk(cudaMemsetAsync(mel, 0, sizeof(float) * nb * pitch, c.st), "pool.mel_zero");
+        lane_copy(c, nb, [&](int j) { return (long long)(N[j] - 1) * N_MELS; }, [&](int j) { return sl(j).mel.get(); },
+                  [&](int j) { return mel + j * pitch; }, "pool.mel");
+        for (const auto& kv : by_hist) {
+            const int hist = kv.first, ng = (int)kv.second.size();
+            const std::vector<int>& g = kv.second;
+            float* xw = c.alloc<float>((size_t)ng * hist);
+            lane_copy(c, ng, hist, [&](int k) { return sl(g[k]).x_hist; }, [&](int k) { return xw + (size_t)k * hist; },
+                      "pool.x_hist");
+            const float* last = last_mel_row(c, xw, ng, hist);
+            lane_copy(c, ng, N_MELS, [&](int k) { return last + (size_t)k * N_MELS; },
+                      [&](int k) { return mel + g[k] * pitch + (size_t)(N[g[k]] - 1) * N_MELS; }, "pool.mel_last");
+        }
+        float* tv = c.alloc<float>((size_t)nb * 1024);
+        style_encoder(c, mel, nb, Tm, nullptr, tv, &ln);
+        lane_copy(c, nb, 1024, [&](int j) { return tv + (size_t)j * 1024; }, [&](int j) { return timbre[b[j]]; }, "pool.timbre");
+        c.vq_critical = false;
+    });
+}
+
 // One batch of a vc-pool step: inputs b (equal plan keys) of the step's sessions.
 int vc_pool_batch(fac_handle* h, VcPool& P, const std::vector<int>& b, const int* sessions, const std::vector<VcPlan>& plan,
                   const int64_t* const* codes_p, const int64_t* const* codes_c, float* const* y, cudaStream_t st) {
@@ -2818,6 +2934,13 @@ int dec_pool_batch(fac_handle* h, DecPool& P, const std::vector<int>& b, const i
     for (int j = 0; j < nb; ++j) sl(j).frames += F[j];
     return FAC_OK;
 }
+
+// A decode-pool slot's gamma | beta from timbre [1][1024], by the B = 1 launch a stream's decode_codes runs on every
+// chunk, so the bits are the same.
+void dec_slot_gamma_beta(Ctx& c, DecHalf& s, const float* timbre) {
+    const float* gb = timbre_gamma_beta(c, timbre, 1);
+    if (!c.dry) c.check_nk(cudaMemcpyAsync(s.gb, gb, sizeof(float) * 2048, cudaMemcpyDeviceToDevice, c.st), "pool.gb");
+}
 }  // namespace
 
 extern "C" {
@@ -2905,6 +3028,29 @@ int fac_codes_pool_finish_codes(fac_handle* h, int pool_id, int n, const int* se
         rc = finish_codes(h, P->slot[sessions[i]], codes_p[i], codes_c[i], codes_r[i], timbre ? timbre[i] : nullptr, stream);
         if (rc < 0) return rc;
     }
+    return FAC_OK;
+}
+
+int fac_codes_pool_timbre(fac_handle* h, int pool_id, int n, const int* sessions, float* const* timbre, void* stream) {
+    int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER});
+    if (rc) return rc;
+    const char* who = "fac_codes_pool_timbre";
+    CodesPool* P = by_id(h, &fac_handle::codes_pools, pool_id);
+    if (!P || n < 0 || (n > 0 && (!sessions || !timbre))) { h->err = "fac_codes_pool_timbre: bad arguments"; return FAC_ERR_INVALID; }
+    if ((rc = check_sessions(h, *P, n, sessions, who))) return rc;
+    std::vector<int> N(n);
+    for (int i = 0; i < n; ++i) {
+        const EncHalf& s = P->slot[sessions[i]];
+        if (!timbre[i]) { h->err = "fac_codes_pool_timbre: null output of session " + std::to_string(sessions[i]); return FAC_ERR_INVALID; }
+        if ((rc = stream_finish_codes_check(h, s, who))) return rc;
+        N[i] = (int)(s.samples / HOP);
+    }
+    int launches = 0;
+    for (const auto& b : timbre_plan(N)) {
+        if ((rc = codes_pool_timbre_batch(h, *P, b, sessions, timbre, (cudaStream_t)stream))) return rc;
+        launches += h->launches;
+    }
+    h->launches = launches;
     return FAC_OK;
 }
 
@@ -3009,14 +3155,24 @@ int fac_dec_pool_open(fac_handle* h, int pool_id, const float* timbre, void* str
     if (!timbre) { h->err = "fac_dec_pool_open: bad arguments"; return FAC_ERR_INVALID; }
     return pool_open(h, &fac_handle::dec_pools, pool_id, "fac_dec_pool_open", [&](DecHalf& s) {
         s.frames = 0;
-        // gamma | beta by the B = 1 launch a stream's decode_codes runs on every chunk, so the bits are the same
         return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
-            const float* gb = timbre_gamma_beta(c, timbre, 1);
-            if (c.dry) return;
-            c.check_nk(cudaMemcpyAsync(s.gb, gb, sizeof(float) * 2048, cudaMemcpyDeviceToDevice, c.st), "pool.gb");
-            c.check_nk(cudaMemsetAsync(s.carry, 0, sizeof(uint32_t) * 2 * carry_words(1536, 0), c.st), "pool.carry");
+            dec_slot_gamma_beta(c, s, timbre);
+            if (!c.dry) c.check_nk(cudaMemsetAsync(s.carry, 0, sizeof(uint32_t) * 2 * carry_words(1536, 0), c.st), "pool.carry");
         });
     });
+}
+
+int fac_dec_pool_set_timbre(fac_handle* h, int pool_id, int session, const float* timbre, void* stream) {
+    int rc = check_ready(h, {FAC_QUANTIZER, FAC_DECODER});
+    if (rc) return rc;
+    DecPool* P = by_id(h, &fac_handle::dec_pools, pool_id);
+    if (!P || !timbre) { h->err = "fac_dec_pool_set_timbre: bad arguments"; return FAC_ERR_INVALID; }
+    if (session < 0 || session >= P->cap || !P->used[session]) {
+        h->err = "fac_dec_pool_set_timbre: session " + std::to_string(session) + " is not open";
+        return FAC_ERR_INVALID;
+    }
+    DecHalf& s = P->slot[session];
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { dec_slot_gamma_beta(c, s, timbre); });
 }
 
 int fac_dec_pool_decode_codes(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
@@ -3109,6 +3265,14 @@ int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* l
                 : kind == 1 ? vc_plan(c[0], c[1], c[2], lengths[i], false).key() : dec_plan(c[0]).key();
     }
     return (int)pool_plan(keys, group, batch).size();
+}
+
+int fac_debug_timbre_plan(int n, const int* frames, int* batch) {
+    if (n < 0 || (n > 0 && (!frames || !batch))) return FAC_ERR_INVALID;
+    const auto batches = timbre_plan(std::vector<int>(frames, frames + n));
+    for (size_t k = 0; k < batches.size(); ++k)
+        for (int i : batches[k]) batch[i] = (int)k;
+    return (int)batches.size();
 }
 
 long long fac_debug_lstm_lane_map(int H, int pass3, int lane, long long* pos, long long capacity) {

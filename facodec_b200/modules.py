@@ -453,6 +453,22 @@ class Codec:
         _lib.check(e.handle, rc, "fac_codec_encode")
         return [cp, cc, cr], timbre
 
+    def timbre(self, x, lengths=None):
+        """Timbre only: x [B,1,T] on the GPU -> timbre [B,1024], encode(x, n_c, lengths)[1] bit for bit for any n_c.  It runs
+        the mel front-end and the StyleEncoder alone (no encoder, prosody or VQ launch), so it is the cheap way to get a
+        voice to decode or convert with.  lengths: per-utterance sample counts, as encode() takes them."""
+        e = self.engine
+        if self.model.quantizer.training:
+            raise NotImplementedError("eval mode only")
+        e.sync_weights(x.device)
+        x = _f32c(x)
+        B, _, T = x.shape
+        lanes = _c_ints(None if lengths is None else _lane_counts(lengths, B, 1025, T, "lengths"))
+        timbre = torch.empty(B, 1024, device=x.device)
+        rc = e.L.fac_codec_timbre_lens(e.handle, _ptr(x), B, T, lanes, _ptr(timbre), _stream(x.device))
+        _lib.check(e.handle, rc, "fac_codec_timbre")
+        return timbre
+
     def decode(self, codes, timbre, frames=None):
         """Decompress: codes ([codes_p, codes_c, codes_r] as forward()/encode() return them, or codefile.DACFile.unpack();
         codes_r may have 0..3 rows or be None) + timbre [B,1024] on the GPU -> y [B,1,300*T].  A timbre from another
@@ -623,6 +639,19 @@ class CodecStream:
         rc = e.L.fac_stream_finish_codes(e.handle, self.sid, _ptr(cp), _ptr(cc), _ptr(cr), _ptr(timbre), _stream(dev))
         _lib.check(e.handle, rc, "fac_stream_finish_codes")
         return [cp, cc, cr], timbre
+
+    def timbre(self):
+        """The timbre so far [B,1024], without ending the stream: what finish_codes() would return if the utterance ended
+        now, i.e. Codec.encode(x_so_far)[1] bit for bit with x_so_far every sample fed to encode_codes.  Codes and the
+        timbre emitted later do not change.  Raises FacError before the first encode_codes chunk, on a stream fed by
+        encode(), after finish_codes(), and with tensor_cores < 2; the stream stays as it was."""
+        if self.sid is None:
+            raise _lib.FacError("stream is closed")
+        e = self.engine
+        timbre = torch.empty(self.batch, 1024, device=self.device)
+        rc = e.L.fac_stream_timbre(e.handle, self.sid, _ptr(timbre), _stream(self.device))
+        _lib.check(e.handle, rc, "fac_stream_timbre")
+        return timbre
 
     def close(self):
         if self.sid is not None and self.engine.handle is not None:
@@ -987,6 +1016,26 @@ class CodecStreamPool(_StreamPool):
         self._done.update(sessions)
         return {s: (outs[i], timbres[i]) for i, s in enumerate(sessions)}
 
+    def timbre(self, sessions):
+        """The timbre so far of each session, without ending any -> {session: timbre [1,1024]}, each its own B = 1
+        CodecStream.timbre() fed the same chunks, bit for bit.  For a session at another sample rate, the utterance so far is
+        the whole 24 kHz frames its encoder has been fed: samples still held or pending in its resampler are left out.  The
+        sessions run as lanes of shared StyleEncoder batches.  A session that is finished, or whose encoder has been fed
+        nothing yet (a session at another rate: before its first 3000 samples at 24 kHz), rejects the whole call, and no
+        session changes."""
+        sessions = self._sessions(sessions)
+        for s in sessions:
+            if s in self._done:
+                raise _lib.FacError("session %d: its utterance was finished by finish_codes" % s)
+            if self._fed[s] == 0:
+                raise _lib.FacError("session %d: nothing has been encoded yet" % s)
+        timbres = [torch.empty(1, 1024, device=self.device) for _ in sessions]
+        e = self.engine
+        rc = e.L.fac_codes_pool_timbre(e.handle, self.pid, len(sessions), _ptr_array(ctypes.c_int, sessions),
+                                       _ptr_array(ctypes.c_void_p, [t.data_ptr() for t in timbres]), _stream(self.device))
+        _lib.check(e.handle, rc, "fac_codes_pool_timbre")
+        return dict(zip(sessions, timbres))
+
 
 class VoiceConversionPool(_StreamPool):
     """Many live voice-conversion sessions (VoiceConversionStream with B = 1 each, every one with its own target timbre)
@@ -1127,6 +1176,22 @@ class CodecDecodePool(_StreamPool):
             if s in self._finished:
                 raise _lib.FacError("session %d: its code stream was ended by finish()" % s)
         return self._resampled(self._decode(chunks))
+
+    def set_timbre(self, session, timbre):
+        """Session ``session`` decodes with ``timbre`` [1,1024] from its next decode_codes on, e.g. the sender's own voice
+        from CodecStreamPool.timbre once it exists: its audio then equals its own B = 1 CodecStream.decode_codes given that
+        timbre from the same chunk on.  Its decoder state and the other sessions are untouched.  A wrong shape or device,
+        or a session that is closed or ended by finish(), raises and changes nothing."""
+        s = self._sessions([session])[0]
+        if s in self._finished:
+            raise _lib.FacError("session %d: its code stream was ended by finish()" % s)
+        self._check_device(timbre)
+        tv = _f32c(timbre)
+        if tuple(tv.shape) != (1, 1024):
+            raise ValueError("timbre must be [1, 1024], got %s" % (tuple(tv.shape),))
+        e = self.engine
+        _lib.check(e.handle, e.L.fac_dec_pool_set_timbre(e.handle, self.pid, s, _ptr(tv), _stream(self.device)),
+                   "fac_dec_pool_set_timbre")
 
     def finish(self, sessions):
         """End of the sessions' code streams -> {session: y [1,1,k]}: the resampler's flushed tail of a session at another

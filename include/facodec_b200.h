@@ -106,6 +106,11 @@ int fac_codec_forward_lens(fac_handle* h, const float* x, int B, int T, const in
                            int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream);
 int fac_codec_encode_lens(fac_handle* h, const float* x, int B, int T, const int* lengths, int n_c, int64_t* codes_p,
                           int64_t* codes_c, int64_t* codes_r, float* timbre, void* stream);
+/* Timbre only: the timbre [B,1024] fac_codec_encode_lens writes for the same x and lengths (any n_c), bit for bit, from
+ * the launches it runs for it alone -- the mel front-end and the StyleEncoder (modules/quantize.py:377-379), with the
+ * same lanes -- and no encoder, prosody or VQ launch.  Needs only the quantizer; the rules on T and lengths are those of
+ * fac_codec_encode_lens. */
+int fac_codec_timbre_lens(fac_handle* h, const float* x, int B, int T, const int* lengths, float* timbre, void* stream);
 
 /* Decompress.  The reference has no single call for it (FAquantizer.decode, modules/quantize.py:245-254, needs the
  * timbre quantizer that timbre_norm = True leaves out); it is ResidualVectorQuantize.from_codes (dac/nn/quantize.py:200-220:
@@ -193,7 +198,13 @@ int fac_vc_stream_end(fac_handle* h, int stream_id);
  * Each chunk recomputes the encoder over a 6000-sample history and the prosody net over <= 32 frames of history.
  * FAC_ERR_STATE: encode_codes on a stream fed by fac_stream_encode or the reverse, any encode after finish, finish with
  * nothing encoded; FAC_ERR_INVALID: n_c changed mid-stream; FAC_ERR_UNSUPPORTED unless "tensor_cores" is 2 (the only mel
- * path that cuts the STFT frames explicitly).  A rejected call leaves the stream as it was. */
+ * path that cuts the STFT frames explicitly).  A rejected call leaves the stream as it was.
+ * fac_stream_timbre: the timbre [B,1024] fac_stream_finish_codes would write if the utterance ended now -- fac_codec_encode's
+ * on every sample fed so far, bit for bit -- without ending it: the last mel frame is cut from the sample history reflected
+ * at the current end into workspace, and the StyleEncoder runs over the samples / 300 rows.  Nothing the stream emits
+ * later changes.  Rejected (stream unchanged) as fac_stream_finish_codes is: FAC_ERR_STATE before the first
+ * fac_stream_encode_codes chunk, on a stream fed by fac_stream_encode, after finish; FAC_ERR_UNSUPPORTED unless
+ * "tensor_cores" is 2. */
 int fac_stream_begin(fac_handle* h, int B);
 int fac_stream_encode(fac_handle* h, int stream_id, const float* x, int T, float* z, void* stream);
 int fac_stream_decode(fac_handle* h, int stream_id, const float* z, int Fc, float* y, void* stream);
@@ -203,6 +214,7 @@ int fac_stream_encode_codes(fac_handle* h, int stream_id, const float* x, int T,
                             int64_t* codes_r, void* stream);
 int fac_stream_finish_codes(fac_handle* h, int stream_id, int64_t* codes_p, int64_t* codes_c, int64_t* codes_r, float* timbre,
                             void* stream);
+int fac_stream_timbre(fac_handle* h, int stream_id, float* timbre, void* stream);
 int fac_stream_end(fac_handle* h, int stream_id);
 
 /* Stream pools: many live sessions, each behaving exactly like its own B = 1 stream, stepped in shared launches.  A pool
@@ -221,6 +233,11 @@ int fac_stream_end(fac_handle* h, int stream_id);
  * writes codes_p[i] [1,1,F], codes_c[i] [1,n_c,F], codes_r[i] [1,3,F]; frames[i] = F (T/300 - 1 on a first chunk, T/300 after).
  * fac_codes_pool_finish_codes: fac_stream_finish_codes per session (one frame each; timbre may be NULL, or timbre[i] NULL).
  * The session's mel rows are kept until the pool is destroyed and reused by the next session of the slot.
+ * fac_codes_pool_timbre: fac_stream_timbre per session into timbre[i] [1,1024], without ending any of them.  The sessions
+ * run as lanes of ragged StyleEncoder batches (<= 32 lanes, ordered by frame count, lanes x longest lane <= 32768 mel
+ * frames; a longer session runs alone), each lane bit-identical to its session's own B = 1 fac_stream_timbre.  A session
+ * that is not open, named twice, finished or has nothing encoded rejects the whole call before anything is queued.
+ * fac_last_launch_count counts the launches of all its batches.
  * fac_vc_pool_create(capacity >= 1, use_p_code, use_c_code, 0 <= n_c <= 2) -> pool id; needs the redecoder and its decoder.
  * fac_vc_pool_open(timbre [1,1024] device) -> session id; the timbre's cond layer runs once here.
  * fac_vc_pool_convert: session sessions[i] takes codes_p[i] [1,1,F[i]], codes_c[i] [1,n_c_rows[i],F[i]] (as
@@ -234,6 +251,8 @@ int fac_stream_end(fac_handle* h, int stream_id);
  * >= 10 frames) and writes y[i] [1,1,300*F[i]].  The decoder is causal, so every frame is final when it arrives (no finish).
  * Sessions that have decoded equally many frames (20 or more: any two in steady state) share a batch whatever their chunk
  * lengths and code rows.  Out-of-range codes give NaN samples, as fac_codes_decode.
+ * fac_dec_pool_set_timbre(session, timbre [1,1024] device): the session decodes with this timbre from its next chunk on
+ * (gamma | beta recomputed by fac_dec_pool_open's launch); its decoder state and every other session are untouched.
  * fac_*_pool_close frees a session's slot; fac_*_pool_destroy frees the pool (and runs at fac_destroy). */
 int fac_codes_pool_create(fac_handle* h, int capacity, int n_c);
 int fac_codes_pool_open(fac_handle* h, int pool_id, void* stream);
@@ -242,6 +261,7 @@ int fac_codes_pool_encode_codes(fac_handle* h, int pool_id, int n, const int* se
                                 void* stream);
 int fac_codes_pool_finish_codes(fac_handle* h, int pool_id, int n, const int* sessions, int64_t* const* codes_p,
                                 int64_t* const* codes_c, int64_t* const* codes_r, float* const* timbre, void* stream);
+int fac_codes_pool_timbre(fac_handle* h, int pool_id, int n, const int* sessions, float* const* timbre, void* stream);
 int fac_codes_pool_close(fac_handle* h, int pool_id, int session);
 int fac_codes_pool_destroy(fac_handle* h, int pool_id);
 int fac_vc_pool_create(fac_handle* h, int capacity, int use_p_code, int use_c_code, int n_c);
@@ -256,6 +276,7 @@ int fac_dec_pool_open(fac_handle* h, int pool_id, const float* timbre, void* str
 int fac_dec_pool_decode_codes(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
                               const int64_t* const* codes_c, const int* n_c_rows, const int64_t* const* codes_r,
                               const int* n_r_rows, float* const* y, void* stream);
+int fac_dec_pool_set_timbre(fac_handle* h, int pool_id, int session, const float* timbre, void* stream);
 int fac_dec_pool_close(fac_handle* h, int pool_id, int session);
 int fac_dec_pool_destroy(fac_handle* h, int pool_id);
 

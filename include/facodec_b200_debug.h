@@ -91,6 +91,9 @@ long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out
  * group[i] receives the group of session i (sessions whose launch sequences are identical; groups numbered in order of first
  * appearance), batch[i] its batch (each group cut into batches of <= 32 in input order).  Returns the number of batches. */
 int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch);
+/* Host-only: the StyleEncoder batches of fac_codes_pool_timbre over n sessions of frames[i] mel frames: batch[i] = the
+ * batch of session i (batches in launch order); returns the number of batches. */
+int fac_debug_timbre_plan(int n, const int* frames, int* batch);
 /* Host-only: where one batch lane's carry of one resident-W LSTM layer (H = 1024 or 1536; pass3 = 1: hi | lo h planes) sits
  * in a stream's state: pos[j] for word j (h words first, then the c floats) is its index in [state_h words | state_c floats].
  * The pools move exactly these words between a session's slot and any lane.  Returns the word count (also when pos is
