@@ -119,14 +119,17 @@ struct Stream { EncHalf enc; DecHalf dec; DevMem mem; };
 
 // Streaming voice conversion: the redecoder and its decoder are non-causal but carry no LSTM, so a chunk's outputs depend
 // only on bounded windows of codes and latents on both sides (kVcRedCtx / kVcDecCtx frames, fac_vc_stream_lookahead).
-// Frames [0, Zf) of z and [0, Yf) of the output are final; the device keeps the codes [max(0, Zf - kVcRedCtx), N) and the
-// channels-last z [max(0, Yf - kVcDecCtx), Zf) those windows still need.
+// Frames [0, Zf) of z and [0, Yf) of the output are final; the device keeps the channels-last z [max(0, Yf - kVcDecCtx), Zf)
+// the decoder's windows still need, and the codes [max(0, Yf - kVcDecCtx - kVcRedCtx), N) from which that z can be
+// recomputed under a new timbre (set_timbre; the redecoder's own windows need only [max(0, Zf - kVcRedCtx), N)).
 struct VcStream {
     int B = 0, use_p = 0, use_c = 0, n_c = 0;
     bool finished = false;
+    bool stale = false;                     // g changed since z was computed: the next step recomputes the z history
     long long N = 0, Zf = 0, Yf = 0;        // code frames received, z frames final, output frames emitted
-    float* g = nullptr;                     // [B][2 * 512 * 16] cond_layer(timbre), computed once at begin
-    int64_t* codes = nullptr;               // [B][3][kVcCodesHist]: row 0 prosody, rows 1..2 content
+    float* g = nullptr;                     // [B][2 * 512 * 16] cond_layer(timbre), computed at begin and set_timbre
+    int64_t* codes = nullptr;               // [B][3][kVcCodesHist]: row 0 prosody, rows 1..2 content; frame t of the last
+                                            // kVcCodesHist at column t - N + kVcCodesHist (right-aligned at N)
     float* z = nullptr;                     // [B][kVcZHist][1024]
     DevMem mem;                             // a fac_vc_stream_* stream's own state (null in a pool)
 };
@@ -1102,16 +1105,18 @@ constexpr int kRedCodes = 1024;   // rows of each embedding table (pack_redecode
 __global__ void embed_sum_kernel(const int64_t* __restrict__ codes_p, int cp_stride, const int64_t* __restrict__ codes_c,
                                  int cc_stride, const float* __restrict__ ep, const float* __restrict__ ec0,
                                  const float* __restrict__ ec1, float* __restrict__ out, int T, int hidden, int use_p, int n_c,
-                                 const int* __restrict__ frames) {
+                                 const int* __restrict__ frames, const int* __restrict__ lane_mode) {
     // one CTA per (b, t): out[b][t][:] = [use_p] E_p[codes_p[b,0,t]] + sum_{i < n_c} E_c[i][codes_c[b,i,t]]  (redecoder.py:36-46)
     // codes_p / codes_c rows of utterance b start at b * cp_stride / b * cc_stride; content row i at + i * T.
     // A code outside [0, kRedCodes) reads nothing and makes the frame's embedding NaN.  frames (null: T each): frames
-    // t >= frames[b] of a ragged batch read no code and are 0.
+    // t >= frames[b] of a ragged batch read no code and are 0.  lane_mode (null: use_p and n_c for every b): [B][2] each
+    // row's own use_p and n_c, so a row computes what a launch of its own mode computes.
     const int bt = blockIdx.x, b = bt / T, t = bt - b * T;
     if (frames && t >= frames[b]) {
         for (int c = threadIdx.x; c < hidden; c += blockDim.x) out[(size_t)bt * hidden + c] = 0.f;
         return;
     }
+    if (lane_mode) { use_p = lane_mode[2 * b]; n_c = lane_mode[2 * b + 1]; }
     const long long ip = use_p ? codes_p[(size_t)b * cp_stride + t] : 0;
     const long long i0 = n_c > 0 ? codes_c[(size_t)b * cc_stride + t] : 0;
     const long long i1 = n_c > 1 ? codes_c[(size_t)b * cc_stride + T + t] : 0;
@@ -1139,9 +1144,9 @@ size_t redecoder_cond_floats(const fac_handle* h, int B) { return (size_t)B * 2 
 // Redecoder.forward (modules/redecoder.py:35-48) after the cond layer: codes -> embeddings -> WN conditioned on g
 // (redecoder_cond) -> conv_out.  codes_p row b at codes_p + b * cp_stride, codes_c rows at codes_c + b * cc_stride + i * T
 // (int64, device); returns channels-last z [B][T][1024] in workspace.  frames (a ragged batch): [B] device, each lane's own
-// frames, or null.
+// frames, or null.  lane_mode (a pool batch of mixed modes): [B][2] device, each lane's use_p and effective n_c, or null.
 float* redecoder_body(Ctx& c, const int64_t* codes_p, int cp_stride, const int64_t* codes_c, int cc_stride, const float* g,
-                      int B, int T, int use_p, int use_c, int n_c, const int* frames = nullptr) {
+                      int B, int T, int use_p, int use_c, int n_c, const int* frames = nullptr, const int* lane_mode = nullptr) {
     const RedW& r = c.h->red;
     const int Hd = r.hidden;
     float* x = c.alloc<float>((size_t)B * T * Hd);
@@ -1152,7 +1157,8 @@ float* redecoder_body(Ctx& c, const int64_t* codes_p, int cp_stride, const int64
     float* z = c.alloc<float>((size_t)B * T * LATENT);
     if (!c.dry) {
         embed_sum_kernel<<<B * T, 128, 0, c.st>>>(codes_p, cp_stride, codes_c, cc_stride, c.W(r.emb_p), c.W(r.emb_c[0]),
-                                                  c.W(r.emb_c[1]), x, T, Hd, use_p ? 1 : 0, use_c ? n_c : 0, frames);
+                                                  c.W(r.emb_c[1]), x, T, Hd, use_p ? 1 : 0, use_c ? n_c : 0, frames,
+                                                  lane_mode);
         c.check(cudaGetLastError(), "red.embed");
     }
     if (!c.dry) c.check_nk(cudaMemsetAsync(skip, 0, sizeof(float) * (size_t)B * T * Hd, c.st), "red.zero");
@@ -2515,9 +2521,10 @@ constexpr int vc_decoder_reach() {
     return ahead > behind ? ahead : behind;
 }
 constexpr int kVcDecCtx = vc_decoder_reach();
-// Stream state capacities: after every call the codes history is at most 2 * kVcRedCtx frames and the z history at most
-// 2 * kVcDecCtx.
-constexpr int kVcCodesHist = 2 * kVcRedCtx, kVcZHist = 2 * kVcDecCtx;
+// Stream state capacities.  z history: at most 2 * kVcDecCtx frames after every call.  Codes history: the last
+// kVcCodesHist frames.  A step after set_timbre reads codes from max(0, Yf - kVcDecCtx - kVcRedCtx), and since Yf trails N by
+// at most the look-ahead kVcRedCtx + kVcDecCtx, that start lies at most 2 * (kVcRedCtx + kVcDecCtx) frames back.
+constexpr int kVcCodesHist = 2 * (kVcRedCtx + kVcDecCtx), kVcZHist = 2 * kVcDecCtx;
 
 // B rows of voice-conversion state.
 void take_vc(Carve& m, VcStream& s, int B, size_t gfl) {
@@ -2532,44 +2539,58 @@ void take_vc(Carve& m, VcStream& s, int B, size_t gfl) {
 // and the z window [zh0, Zf1) (Tz frames, zhist of them history).  It makes z final up to Zf1 and the output up to Yf1:
 // both stages reach kVcRedCtx / kVcDecCtx frames past the rows they keep, so those rows never see a window edge except the
 // utterance's own (frame 0, and frame N at finish).  Streams with equal keys share one pool batch.
+// A stale step (the timbre changed since the z history [zh0, Zf) was computed) recomputes it: its codes window starts at
+// hc0 = max(0, zh0 - kVcRedCtx) and every row of the z window comes from it (zhist = 0, zoff = zh0 - hc0).  The same
+// argument holds: z row t in [zh0, Zf1) reads codes [t - kVcRedCtx, t + kVcRedCtx], which lie inside [hc0, N1) except where
+// hc0 = 0 or N1 is the utterance's end -- the edges an offline run reflects at too -- so the rows equal the offline z under
+// the new timbre, bit for bit.  A step whose z history is empty is never stale: the plain step computes every row anew.
 struct VcPlan {
     int F, Tw, hist, Tz, zhist;
-    int zoff, znew;             // z rows [Zf, Zf1) in the codes window
+    int zoff, znew;             // z rows [Zf or zh0 (stale), Zf1) in the codes window
     int k, yoff;                // output frames [Yf, Yf1) and Yf in the z window
     int zkeep_at, zkeep;        // z history kept: [zh1, Zf1) in the z window
-    int ckeep_at, ckeep;        // codes history kept: [hc1, N1) in the codes window
+    int stale;                  // 1: the z history is recomputed from the codes (set_timbre)
     long long N1, Zf1, Yf1;
-    std::vector<long long> key() const { return {F, Tw, hist, Tz, zhist, zoff, znew, k, yoff, zkeep_at, zkeep, ckeep_at, ckeep}; }
+    std::vector<long long> key() const { return {F, Tw, hist, Tz, zhist, zoff, znew, k, yoff, zkeep_at, zkeep, stale}; }
 };
 
-VcPlan vc_plan(long long N, long long Zf, long long Yf, int F, bool finish) {
+VcPlan vc_plan(long long N, long long Zf, long long Yf, int F, bool finish, bool stale = false) {
     auto floor0 = [](long long v) { return v > 0 ? v : 0; };
     VcPlan p;
     p.N1 = N + F;
     p.Zf1 = finish ? p.N1 : std::max(p.N1 - kVcRedCtx, Zf);
     p.Yf1 = finish ? p.N1 : std::max(p.Zf1 - kVcDecCtx, Yf);
-    const long long hc0 = floor0(Zf - kVcRedCtx), zh0 = floor0(Yf - kVcDecCtx);
-    const long long hc1 = floor0(p.Zf1 - kVcRedCtx), zh1 = floor0(p.Yf1 - kVcDecCtx);
-    p.F = F; p.Tw = (int)(p.N1 - hc0); p.hist = (int)(N - hc0); p.Tz = (int)(p.Zf1 - zh0); p.zhist = (int)(Zf - zh0);
-    p.zoff = (int)(Zf - hc0); p.znew = (int)(p.Zf1 - Zf); p.k = (int)(p.Yf1 - Yf); p.yoff = (int)(Yf - zh0);
-    p.zkeep_at = (int)(zh1 - zh0); p.zkeep = (int)(p.Zf1 - zh1); p.ckeep_at = (int)(hc1 - hc0); p.ckeep = (int)(p.N1 - hc1);
+    const long long zh0 = floor0(Yf - kVcDecCtx), zh1 = floor0(p.Yf1 - kVcDecCtx);
+    p.stale = stale && Zf > zh0 ? 1 : 0;
+    const long long hc0 = p.stale ? floor0(zh0 - kVcRedCtx) : floor0(Zf - kVcRedCtx), z0 = p.stale ? zh0 : Zf;
+    p.F = F; p.Tw = (int)(p.N1 - hc0); p.hist = (int)(N - hc0); p.Tz = (int)(p.Zf1 - zh0); p.zhist = (int)(z0 - zh0);
+    p.zoff = (int)(z0 - hc0); p.znew = (int)(p.Zf1 - z0); p.k = (int)(p.Yf1 - Yf); p.yoff = (int)(Yf - zh0);
+    p.zkeep_at = (int)(zh1 - zh0); p.zkeep = (int)(p.Zf1 - zh1);
     return p;
 }
-VcPlan vc_plan(const VcStream& s, int F, bool finish) { return vc_plan(s.N, s.Zf, s.Yf, F, finish); }
+VcPlan vc_plan(const VcStream& s, int F, bool finish) { return vc_plan(s.N, s.Zf, s.Yf, F, finish, s.stale); }
+
+// The conversion mode of a step's rows: one for all (a stream, or a pool batch of one mode), or per lane.
+struct VcMode {
+    int use_p = 0, use_c = 0, n_c = 0;      // n_c: the content rows copied into the codes window
+    const int* lanes = nullptr;             // [B][2] device: each row's use_p and effective n_c (use_c ? n_c : 0), or null
+};
+VcMode vc_mode(const VcStream& s) { return VcMode{s.use_p, s.use_c, s.n_c, nullptr}; }
 
 // The launch sequence of step p on the rows of s: appends F code frames (codes_p [B][1][F], codes_c [B][n_c_rows][F]) and
 // writes output frames [Yf, Yf1) to y as [B][1][300 k].
-void vc_step(Ctx& c, VcStream& s, const VcPlan& p, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, float* y) {
-    const int B = s.B, F = p.F, Tw = p.Tw, hist = p.hist, Tz = p.Tz;
+void vc_step(Ctx& c, VcStream& s, const VcPlan& p, const VcMode& m, const int64_t* codes_p, const int64_t* codes_c,
+             int n_c_rows, float* y) {
+    const int B = s.B, F = p.F, Tw = p.Tw, hist = p.hist, Tz = p.Tz, H = kVcCodesHist;
     // codes [hc0, N1) as [B][3][Tw]: the history, then the new frames
     int64_t* cw = c.alloc<int64_t>((size_t)B * 3 * Tw);
-    copy_rows(c, cw, Tw, s.codes, kVcCodesHist, 0, hist, 1, 3 * B, "vc.codes_hist");
+    copy_rows(c, cw, Tw, s.codes, H, H - hist, hist, 1, 3 * B, "vc.codes_hist");
     copy_rows(c, cw + hist, 3 * Tw, codes_p, F, 0, F, 1, B, "vc.codes_p");
-    for (int i = 0; i < s.n_c; ++i)
+    for (int i = 0; i < m.n_c; ++i)
         copy_rows(c, cw + (size_t)(1 + i) * Tw + hist, 3 * Tw, codes_c + (size_t)i * F, n_c_rows * F, 0, F, 1, B, "vc.codes_c");
     if (p.znew > 0) {
         // z over the codes window, of which rows [Zf, Zf1) are final; the decoder's window is z [zh0, Zf1)
-        float* zc = redecoder_body(c, cw, 3 * Tw, cw + Tw, 3 * Tw, s.g, B, Tw, s.use_p, s.use_c, s.n_c);
+        float* zc = redecoder_body(c, cw, 3 * Tw, cw + Tw, 3 * Tw, s.g, B, Tw, m.use_p, m.use_c, m.n_c, nullptr, m.lanes);
         float* zw = c.alloc<float>((size_t)B * Tz * LATENT);
         copy_rows(c, zw, Tz, s.z, kVcZHist, 0, p.zhist, LATENT, B, "vc.z_hist");
         copy_rows(c, zw + (size_t)p.zhist * LATENT, Tz, zc, Tw, p.zoff, p.znew, LATENT, B, "vc.z_new");
@@ -2580,19 +2601,38 @@ void vc_step(Ctx& c, VcStream& s, const VcPlan& p, const int64_t* codes_p, const
         }
         copy_rows(c, s.z, kVcZHist, zw, Tz, p.zkeep_at, p.zkeep, LATENT, B, "vc.z_keep");
     }
-    copy_rows(c, s.codes, kVcCodesHist, cw, Tw, p.ckeep_at, p.ckeep, 1, 3 * B, "vc.codes_keep");
+    // codes [N1 - H, N1), right-aligned: the frames before the window from the old history (columns [F, H - hist)), the
+    // rest from the window, assembled in workspace (the two ranges of s.codes may overlap)
+    const int fresh = std::min(Tw, H);
+    int64_t* ck = c.alloc<int64_t>((size_t)B * 3 * H);
+    copy_rows(c, ck, H, s.codes, H, F, H - Tw, 1, 3 * B, "vc.codes_old");
+    copy_rows(c, ck + (H - fresh), H, cw, Tw, Tw - fresh, fresh, 1, 3 * B, "vc.codes_new");
+    copy_rows(c, s.codes, H, ck, H, 0, H, 1, 3 * B, "vc.codes_keep");
 }
 
-void vc_commit(VcStream& s, const VcPlan& p) { s.N = p.N1; s.Zf = p.Zf1; s.Yf = p.Yf1; }
+void vc_commit(VcStream& s, const VcPlan& p) { s.N = p.N1; s.Zf = p.Zf1; s.Yf = p.Yf1; s.stale = false; }
 
 // Step p of a voice-conversion stream (or a pool session's B = 1 slot) in its own launch sequence: returns the output frames
 // written or a negative status.
 int vc_run(fac_handle* h, VcStream& s, const VcPlan& p, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, float* y,
            void* stream) {
-    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { vc_step(c, s, p, codes_p, codes_c, n_c_rows, y); });
+    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { vc_step(c, s, p, vc_mode(s), codes_p, codes_c, n_c_rows, y); });
     if (rc) return rc;
     vc_commit(s, p);
     return p.k;
+}
+
+// The target voice of B rows of s from timbre [B][1024]: the cond layer into workspace, then into s.g (nothing of s changes
+// unless the launch sequence is queued); the next step recomputes the z history under it.
+int vc_set_timbre(fac_handle* h, VcStream& s, const float* timbre, void* stream) {
+    const size_t gfl = redecoder_cond_floats(h, s.B);
+    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        float* g = c.alloc<float>(gfl);
+        redecoder_cond(c, timbre, s.B, g);
+        if (!c.dry) c.check_nk(cudaMemcpyAsync(s.g, g, sizeof(float) * gfl, cudaMemcpyDeviceToDevice, c.st), "vc.g");
+    });
+    if (rc == FAC_OK) s.stale = true;
+    return rc;
 }
 }  // namespace
 
@@ -2641,6 +2681,15 @@ int fac_vc_stream_finish(fac_handle* h, int stream_id, float* y, void* stream) {
     rc = vc_run(h, *s, vc_plan(*s, 0, true), nullptr, nullptr, 0, y, stream);
     if (rc >= 0) s->finished = true;
     return rc;
+}
+
+int fac_vc_stream_set_timbre(fac_handle* h, int stream_id, const float* timbre, void* stream) {
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
+    if (rc) return rc;
+    VcStream* s = by_id(h, &fac_handle::vc_streams, stream_id);
+    if (!s || !timbre) { h->err = "fac_vc_stream_set_timbre: bad arguments"; return FAC_ERR_INVALID; }
+    if (s->finished) { h->err = "fac_vc_stream_set_timbre: the stream was finished"; return FAC_ERR_STATE; }
+    return vc_set_timbre(h, *s, timbre, stream);
 }
 
 int fac_vc_stream_end(fac_handle* h, int stream_id) {
@@ -2846,26 +2895,39 @@ int codes_pool_timbre_batch(fac_handle* h, CodesPool& P, const std::vector<int>&
     });
 }
 
-// One batch of a vc-pool step: inputs b (equal plan keys) of the step's sessions.
+// One batch of a vc-pool step: inputs b (equal plan keys) of the step's sessions.  Their modes may differ: a batch of one
+// mode runs the launches of a stream of that mode, a mixed one the same launches with each lane's mode uploaded.
 int vc_pool_batch(fac_handle* h, VcPool& P, const std::vector<int>& b, const int* sessions, const std::vector<VcPlan>& plan,
                   const int64_t* const* codes_p, const int64_t* const* codes_c, float* const* y, cudaStream_t st) {
     VcStream& L = P.lanes;
     const VcPlan& p = plan[b[0]];
-    const int nb = (int)b.size(), n_c = L.n_c, rows = n_c > 0 ? n_c : 1, F = p.F;
+    const int nb = (int)b.size(), F = p.F;
     auto sl = [&](int j) -> VcStream& { return P.slot[sessions[b[j]]]; };
     const size_t gfl = redecoder_cond_floats(h, 1), cpl = 3 * kVcCodesHist, zpl = (size_t)kVcZHist * LATENT;
+    VcMode m = vc_mode(sl(0));
+    std::vector<int> lane_mode(2 * nb);
+    bool mixed = false;
+    for (int j = 0; j < nb; ++j) {
+        const VcStream& s = sl(j);
+        lane_mode[2 * j] = s.use_p; lane_mode[2 * j + 1] = s.use_c ? s.n_c : 0;
+        mixed |= s.use_p != m.use_p || s.use_c != m.use_c || s.n_c != m.n_c;
+        m.n_c = std::max(m.n_c, s.n_c);
+    }
+    const int rows = m.n_c > 0 ? m.n_c : 1;
     L.B = nb;
     int rc = two_pass(h, st, [&](Ctx& c) {
         int64_t* cp = c.alloc<int64_t>((size_t)nb * F);
         int64_t* cc = c.alloc<int64_t>((size_t)nb * rows * F);
         float* yout = c.alloc<float>((size_t)nb * p.k * HOP);
+        VcMode mc = m;
+        if (mixed) mc.lanes = upload_ints(c, lane_mode);
         lane_copy(c, nb, (long long)gfl, [&](int j) { return sl(j).g; }, [&](int j) { return L.g + j * gfl; }, "pool.g");
         lane_copy(c, nb, 2LL * cpl, [&](int j) { return sl(j).codes; }, [&](int j) { return L.codes + j * cpl; }, "pool.codes");
         lane_copy(c, nb, (long long)p.zhist * LATENT, [&](int j) { return sl(j).z; }, [&](int j) { return L.z + j * zpl; }, "pool.z");
         lane_copy(c, nb, 2LL * F, [&](int j) { return codes_p[b[j]]; }, [&](int j) { return cp + (size_t)j * F; }, "pool.codes_p");
-        lane_copy(c, nb, 2LL * n_c * F, [&](int j) { return codes_c[b[j]]; }, [&](int j) { return cc + (size_t)j * rows * F; },
-                  "pool.codes_c");
-        vc_step(c, L, p, cp, cc, rows, yout);
+        lane_copy(c, nb, [&](int j) { return 2LL * sl(j).n_c * F; }, [&](int j) { return codes_c[b[j]]; },
+                  [&](int j) { return cc + (size_t)j * rows * F; }, "pool.codes_c");
+        vc_step(c, L, p, mc, cp, cc, rows, yout);
         lane_copy(c, nb, 2LL * cpl, [&](int j) { return L.codes + j * cpl; }, [&](int j) { return sl(j).codes; }, "pool.codes");
         if (p.znew > 0)
             lane_copy(c, nb, (long long)p.zkeep * LATENT, [&](int j) { return L.z + j * zpl; }, [&](int j) { return sl(j).z; },
@@ -3071,15 +3133,39 @@ int fac_vc_pool_create(fac_handle* h, int capacity, int use_p_code, int use_c_co
     });
 }
 
-int fac_vc_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream) {
+int fac_vc_pool_open_mode(fac_handle* h, int pool_id, const float* timbre, int use_p_code, int use_c_code, int n_c,
+                          void* stream) {
     int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
     if (rc) return rc;
-    if (!timbre) { h->err = "fac_vc_pool_open: bad arguments"; return FAC_ERR_INVALID; }
+    if (!timbre || n_c < 0 || n_c > 2) { h->err = "fac_vc_pool_open: bad arguments (0 <= n_c <= 2)"; return FAC_ERR_INVALID; }
     return pool_open(h, &fac_handle::vc_pools, pool_id, "fac_vc_pool_open", [&](VcStream& s) {
         s.N = s.Zf = s.Yf = 0;
         s.finished = false;
+        s.stale = false;
+        s.use_p = use_p_code ? 1 : 0; s.use_c = use_c_code ? 1 : 0; s.n_c = n_c;
         return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) { redecoder_cond(c, timbre, 1, s.g); });
     });
+}
+
+int fac_vc_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream) {
+    const VcPool* P = h ? by_id(h, &fac_handle::vc_pools, pool_id) : nullptr;
+    if (!P) { if (h) h->err = "fac_vc_pool_open: no such pool"; return FAC_ERR_INVALID; }
+    const VcStream& d = P->lanes;       // the pool's options
+    return fac_vc_pool_open_mode(h, pool_id, timbre, d.use_p, d.use_c, d.n_c, stream);
+}
+
+int fac_vc_pool_set_timbre(fac_handle* h, int pool_id, int session, const float* timbre, void* stream) {
+    int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER});
+    if (rc) return rc;
+    VcPool* P = by_id(h, &fac_handle::vc_pools, pool_id);
+    if (!P || !timbre) { h->err = "fac_vc_pool_set_timbre: bad arguments"; return FAC_ERR_INVALID; }
+    if (session < 0 || session >= P->cap || !P->used[session]) {
+        h->err = "fac_vc_pool_set_timbre: session " + std::to_string(session) + " is not open";
+        return FAC_ERR_INVALID;
+    }
+    VcStream& s = P->slot[session];
+    if (s.finished) { h->err = "fac_vc_pool_set_timbre: session " + std::to_string(session) + " was finished"; return FAC_ERR_STATE; }
+    return vc_set_timbre(h, s, timbre, stream);
 }
 
 int fac_vc_pool_convert(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
@@ -3106,8 +3192,12 @@ int fac_vc_pool_convert(fac_handle* h, int pool_id, int n, const int* sessions, 
         plan[i] = vc_plan(s, F[i], false);
         keys[i] = plan[i].key();
     }
-    for (const auto& b : pool_plan(keys, nullptr, nullptr))
+    int launches = 0;
+    for (const auto& b : pool_plan(keys, nullptr, nullptr)) {
         if ((rc = vc_pool_batch(h, *P, b, sessions, plan, codes_p, codes_c, y, (cudaStream_t)stream))) return rc;
+        launches += h->launches;
+    }
+    h->launches = launches;
     for (int i = 0; i < n; ++i) frames[i] = plan[i].k;
     return FAC_OK;
 }
@@ -3257,14 +3347,24 @@ int fac_rs_pool_close(fac_handle* h, int pool_id, int session) {
 int fac_rs_pool_destroy(fac_handle* h, int pool_id) { return h ? fac::rs_pool_destroy(rs_env(h), pool_id) : FAC_ERR_INVALID; }
 
 int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch) {
-    if (n < 0 || (n > 0 && (!counters || !lengths || !group || !batch)) || kind < 0 || kind > 2) return FAC_ERR_INVALID;
+    if (n < 0 || (n > 0 && (!counters || !lengths || !group || !batch)) || kind < 0 || kind > 3) return FAC_ERR_INVALID;
     std::vector<std::vector<long long>> keys(n);
     for (int i = 0; i < n; ++i) {
-        const long long* c = counters + (size_t)i * (kind == 0 ? 4 : kind == 1 ? 3 : 1);
+        const long long* c = counters + (size_t)i * (kind == 0 ? 4 : kind == 1 ? 3 : kind == 2 ? 1 : 4);
         keys[i] = kind == 0 ? enc_plan(c[0], (int)c[1], (int)c[2], c[3], lengths[i]).key()
-                : kind == 1 ? vc_plan(c[0], c[1], c[2], lengths[i], false).key() : dec_plan(c[0]).key();
+                : kind == 1 ? vc_plan(c[0], c[1], c[2], lengths[i], false).key()
+                : kind == 2 ? dec_plan(c[0]).key() : vc_plan(c[0], c[1], c[2], lengths[i], false, c[3] != 0).key();
     }
     return (int)pool_plan(keys, group, batch).size();
+}
+
+int fac_debug_vc_plan(long long N, long long Zf, long long Yf, int F, int finish, int stale, long long* out16) {
+    if (!out16 || F < 0 || (F == 0) != (finish != 0)) return FAC_ERR_INVALID;
+    const VcPlan p = vc_plan(N, Zf, Yf, F, finish != 0, stale != 0);
+    const long long v[16] = {p.F, p.Tw, p.hist, p.Tz, p.zhist, p.zoff, p.znew, p.k, p.yoff, p.zkeep_at, p.zkeep, p.stale,
+                             p.N1, p.Zf1, p.Yf1, kVcCodesHist};
+    std::copy(v, v + 16, out16);
+    return 16;
 }
 
 int fac_debug_timbre_plan(int n, const int* frames, int* batch) {

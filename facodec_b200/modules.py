@@ -693,7 +693,7 @@ class VoiceConversionStream:
     """Voice conversion in chunks (reconstruct_redecoder.py:118-121 on a live signal): codes in, converted audio out, with
     the concatenated output bit-identical to ONE VoiceConverter.convert(codes, timbre, use_p_code, use_c_code, n_c) on the
     whole utterance.  ``redecoder_model`` is a build_model(stage='redecoder') Munch; ``timbre`` [batch, 1024] (the target
-    voice, e.g. Codec.encode of a reference clip) is fixed for the stream.  The redecoder and its decoder are non-causal, so
+    voice, e.g. Codec.encode of a reference clip) holds until set_timbre() switches it.  The redecoder and its decoder are non-causal, so
     output frame t comes out once code frames up to t + lookahead_frames (44 frames, 550 ms) are in; finish() flushes the
     rest.  The codes and latents those windows need live on the device between calls (fac_vc_stream_*)."""
 
@@ -741,6 +741,25 @@ class VoiceConversionStream:
         k = e.L.fac_vc_stream_finish(e.handle, self.sid, _ptr(y), _stream(self.device))
         _lib.check(e.handle, k, "fac_vc_stream_finish")
         return y[:B * 300 * k].view(B, 1, 300 * k)
+
+    def set_timbre(self, timbre):
+        """Converts to ``timbre`` [batch, 1024] from the next convert() on, e.g. when the caller picks another voice mid-call.
+        Every sample emitted from then on, finish() included, equals VoiceConverter.convert of the whole utterance with the
+        new timbre at the same positions, and everything emitted before equals it with the old one: the next call recomputes
+        the latents the decoder still reads from the codes the stream keeps, so no look-ahead is lost.  A wrong shape or
+        device, or a finished or closed stream, raises and changes nothing."""
+        if self.sid is None:
+            raise _lib.FacError("stream is closed")
+        d = timbre.device
+        if d.type != "cuda" or (d.index if d.index is not None else torch.cuda.current_device()) != self.engine.device_index:
+            raise _lib.FacError("timbre must be on cuda:%d (no CPU fallback); got %s" % (self.engine.device_index, d))
+        tv = _f32c(timbre)
+        if tuple(tv.shape) != (self.batch, 1024):
+            raise ValueError("timbre must be [%d, 1024], got %s" % (self.batch, tuple(tv.shape)))
+        e = self.engine
+        _lib.check(e.handle, e.L.fac_vc_stream_set_timbre(e.handle, self.sid, _ptr(tv), _stream(self.device)),
+                   "fac_vc_stream_set_timbre")
+        self._timbre = tv
 
     def close(self):
         if self.sid is not None and self.engine.handle is not None:
@@ -1040,7 +1059,8 @@ class CodecStreamPool(_StreamPool):
 class VoiceConversionPool(_StreamPool):
     """Many live voice-conversion sessions (VoiceConversionStream with B = 1 each, every one with its own target timbre)
     stepped in shared launches; each session's waveform equals that of its own B = 1 VoiceConversionStream fed the same
-    chunks, bit for bit (fac_vc_pool_*).  use_p_code / use_c_code / n_c are fixed for the pool."""
+    chunks, bit for bit (fac_vc_pool_*).  use_p_code / use_c_code / n_c are the pool's defaults; a session may open with its
+    own, and sessions of different modes still share launches."""
 
     _kind = "vc"
 
@@ -1051,24 +1071,50 @@ class VoiceConversionPool(_StreamPool):
         _lib.check(engine.handle, pid, "fac_vc_pool_create")
         self._setup(engine, pid)
         self.capacity = int(capacity)
+        self.use_p_code, self.use_c_code, self.n_c = bool(use_p_code), bool(use_c_code), int(n_c)
         self.lookahead_frames = engine.L.fac_vc_stream_lookahead()
 
-    def open(self, timbre, sample_rate=24000):
+    def open(self, timbre, sample_rate=24000, use_p_code=None, use_c_code=None, n_c=None):
         """A new session converting to ``timbre`` [1,1024]; raises FacError when the pool is full.  A session at another
-        sample_rate gets its audio resampled from 24 kHz on the device (one launch per step for all such sessions)."""
+        sample_rate gets its audio resampled from 24 kHz on the device (one launch per step for all such sessions).
+        use_p_code / use_c_code / n_c (None: the pool's) set the session's conversion mode; its output equals a B = 1
+        VoiceConversionStream of that mode, and it shares launches with sessions of other modes."""
         if self.pid is None:
             raise _lib.FacError("pool is closed")
         self._check_device(timbre)
         tv = _f32c(timbre)
         if tuple(tv.shape) != (1, 1024):
             raise ValueError("timbre must be [1, 1024], got %s" % (tuple(tv.shape),))
+        mode = (self.use_p_code if use_p_code is None else bool(use_p_code), self.use_c_code if use_c_code is None else bool(use_c_code),
+                self.n_c if n_c is None else operator.index(n_c))
+        if not 0 <= mode[2] <= 2:
+            raise ValueError("n_c must be 0, 1 or 2, got %d" % mode[2])
         e = self.engine
 
         def open_session():
-            return _lib.check(e.handle, e.L.fac_vc_pool_open(e.handle, self.pid, _ptr(tv), _stream(self.device)), "fac_vc_pool_open")
+            if use_p_code is None and use_c_code is None and n_c is None:
+                rc = e.L.fac_vc_pool_open(e.handle, self.pid, _ptr(tv), _stream(self.device))
+            else:
+                rc = e.L.fac_vc_pool_open_mode(e.handle, self.pid, _ptr(tv), int(mode[0]), int(mode[1]), mode[2], _stream(self.device))
+            return _lib.check(e.handle, rc, "fac_vc_pool_open")
         s, _ = self._rate_open(sample_rate, False, 1, open_session)
         self._open.add(s)
         return s
+
+    def set_timbre(self, session, timbre):
+        """Session ``session`` converts to ``timbre`` [1,1024] from its next convert() on: as VoiceConversionStream.set_timbre,
+        its output from then on equals VoiceConverter.convert of its whole utterance with the new timbre, and what it emitted
+        before is unchanged (at another sample rate: resample() of that 24 kHz splice).  Its next step recomputes its recent
+        latents, so until then it shares launches only with other switched sessions.  The other sessions are untouched.  A
+        wrong shape or device, or a session that is closed or ended by finish(), raises and changes nothing."""
+        s = self._sessions([session])[0]
+        self._check_device(timbre)
+        tv = _f32c(timbre)
+        if tuple(tv.shape) != (1, 1024):
+            raise ValueError("timbre must be [1, 1024], got %s" % (tuple(tv.shape),))
+        e = self.engine
+        _lib.check(e.handle, e.L.fac_vc_pool_set_timbre(e.handle, self.pid, s, _ptr(tv), _stream(self.device)),
+                   "fac_vc_pool_set_timbre")
 
     def convert(self, chunks):
         """{session: codes} (codes[0] [1,1,F], codes[1] [1,1|2,F], as VoiceConversionStream.convert takes them) -> {session:

@@ -163,13 +163,20 @@ int fac_voice_convert_lens(fac_handle* h, const int64_t* codes_p, const int64_t*
  * next k output frames to y as [B,1,300*k] (capacity B*300*F floats).
  * fac_vc_stream_finish: the end of the utterance -> returns k <= 44 (k = min(N, 44) for N frames received) and writes the
  * last k frames to y as [B,1,300*k] (capacity B*300*44 floats).  A stream shorter than the look-ahead emits everything here.
- * FAC_ERR_STATE: convert after finish, finish twice, finish with nothing received; FAC_ERR_INVALID: bad B, F <= 0,
- * n_c > n_c_rows.  A rejected call leaves the stream as it was.  Out-of-range codes behave as in fac_voice_convert. */
+ * fac_vc_stream_set_timbre(timbre [B,1024] device): converts to this voice from the next call on; the cond layer runs here.
+ * The next call recomputes the z frames the decoder still reads ([Yf - 12, Zf) of the output frames emitted Yf and z
+ * frames final Zf) from the code history under the new cond, so every sample emitted from then on, finish included, equals
+ * fac_voice_convert of the whole utterance with the new timbre, and everything emitted before equals it with the old one.
+ * The stream keeps the last 2 * (32 + 12) code frames for this.  Switching to the same timbre changes nothing.
+ * FAC_ERR_STATE: convert after finish, finish twice, finish with nothing received, set_timbre after finish;
+ * FAC_ERR_INVALID: bad B, F <= 0, n_c > n_c_rows, a null timbre.  A rejected call leaves the stream as it was (its cond
+ * included: set_timbre computes into workspace, then copies).  Out-of-range codes behave as in fac_voice_convert. */
 int fac_vc_stream_lookahead(void);
 int fac_vc_stream_begin(fac_handle* h, int B, const float* timbre, int use_p_code, int use_c_code, int n_c, void* stream);
 int fac_vc_stream_convert(fac_handle* h, int stream_id, const int64_t* codes_p, const int64_t* codes_c, int n_c_rows, int F,
                           float* y, void* stream);
 int fac_vc_stream_finish(fac_handle* h, int stream_id, float* y, void* stream);
+int fac_vc_stream_set_timbre(fac_handle* h, int stream_id, const float* timbre, void* stream);
 int fac_vc_stream_end(fac_handle* h, int stream_id);
 
 /* Streaming (SURVEY.md section 8f rank 4; README.md:105-107 "causal ... can be used for streaming"): the encoder and the codec's
@@ -239,9 +246,17 @@ int fac_stream_end(fac_handle* h, int stream_id);
  * that is not open, named twice, finished or has nothing encoded rejects the whole call before anything is queued.
  * fac_last_launch_count counts the launches of all its batches.
  * fac_vc_pool_create(capacity >= 1, use_p_code, use_c_code, 0 <= n_c <= 2) -> pool id; needs the redecoder and its decoder.
- * fac_vc_pool_open(timbre [1,1024] device) -> session id; the timbre's cond layer runs once here.
+ * The options are the defaults of fac_vc_pool_open.
+ * fac_vc_pool_open(timbre [1,1024] device) -> session id; the timbre's cond layer runs here.
+ * fac_vc_pool_open_mode(timbre, use_p_code, use_c_code, 0 <= n_c <= 2): fac_vc_pool_open with the session's own mode.
+ * Sessions of different modes share batches: each lane embeds its codes in its own mode, bit for bit as a B = 1 stream of
+ * that mode, and the rest of the launch sequence does not depend on the mode.
+ * fac_vc_pool_set_timbre(session, timbre [1,1024] device): fac_vc_stream_set_timbre on one session.  Until its next step
+ * has run, the session batches only with other switched sessions (that step recomputes its z history on a wider window).
+ * FAC_ERR_INVALID for a session not open, FAC_ERR_STATE after its finish.
  * fac_vc_pool_convert: session sessions[i] takes codes_p[i] [1,1,F[i]], codes_c[i] [1,n_c_rows[i],F[i]] (as
  * fac_vc_stream_convert) and writes frames[i] = k output frames to y[i] [1,1,300*k] (capacity 300*F[i] floats).
+ * fac_last_launch_count counts the launches of all its batches.
  * fac_vc_pool_finish: fac_vc_stream_finish per session; y[i] holds 300*44 floats.
  * fac_dec_pool_create(capacity >= 1) -> pool id; needs the quantizer and the decoder.
  * fac_dec_pool_open(timbre [1,1024] device) -> session id, a fresh fac_stream_decode_codes stream decoding with that timbre;
@@ -266,6 +281,9 @@ int fac_codes_pool_close(fac_handle* h, int pool_id, int session);
 int fac_codes_pool_destroy(fac_handle* h, int pool_id);
 int fac_vc_pool_create(fac_handle* h, int capacity, int use_p_code, int use_c_code, int n_c);
 int fac_vc_pool_open(fac_handle* h, int pool_id, const float* timbre, void* stream);
+int fac_vc_pool_open_mode(fac_handle* h, int pool_id, const float* timbre, int use_p_code, int use_c_code, int n_c,
+                          void* stream);
+int fac_vc_pool_set_timbre(fac_handle* h, int pool_id, int session, const float* timbre, void* stream);
 int fac_vc_pool_convert(fac_handle* h, int pool_id, int n, const int* sessions, const int* F, const int64_t* const* codes_p,
                         const int64_t* const* codes_c, const int* n_c_rows, float* const* y, int* frames, void* stream);
 int fac_vc_pool_finish(fac_handle* h, int pool_id, int n, const int* sessions, float* const* y, int* frames, void* stream);

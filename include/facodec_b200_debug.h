@@ -87,10 +87,17 @@ long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out
 /* Host-only: the launch plan of one stream-pool step.  kind 0 (codes pool): counters[4 i ..] = {samples encoded, x history
  * length, LSTM-output history length, frames emitted} of session i, lengths[i] = its chunk in samples; kind 1 (voice-conversion
  * pool): counters[3 i ..] = {code frames received, z frames final, output frames emitted}, lengths[i] = its chunk in frames;
- * kind 2 (decode pool): counters[i] = frames decoded by session i, lengths[i] = its chunk in frames.
+ * kind 2 (decode pool): counters[i] = frames decoded by session i, lengths[i] = its chunk in frames; kind 3 (voice-conversion
+ * pool with switches): counters[4 i ..] = kind 1's and 1 for a session whose timbre changed since its last step.
  * group[i] receives the group of session i (sessions whose launch sequences are identical; groups numbered in order of first
  * appearance), batch[i] its batch (each group cut into batches of <= 32 in input order).  Returns the number of batches. */
 int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch);
+/* Host-only: the plan of one voice-conversion step on a stream at (N code frames received, Zf z frames final, Yf output
+ * frames emitted) fed F frames (F = 0 exactly when finish), stale = 1 after a timbre switch.  out16 = {F, codes window
+ * frames, of them history, z window frames, of them history, first kept z row in the codes window, kept z rows, output
+ * frames, first output frame in the z window, first z row kept after the step, z rows kept, stale (0 when the z history is
+ * empty), N, Zf and Yf after the step, code frames the stream keeps}.  Returns 16. */
+int fac_debug_vc_plan(long long N, long long Zf, long long Yf, int F, int finish, int stale, long long* out16);
 /* Host-only: the StyleEncoder batches of fac_codes_pool_timbre over n sessions of frames[i] mel frames: batch[i] = the
  * batch of session i (batches in launch order); returns the number of batches. */
 int fac_debug_timbre_plan(int n, const int* frames, int* batch);
