@@ -152,6 +152,18 @@ def load():
                              _c.POINTER(_c.c_double), _c.POINTER(_c.c_longlong)], i32),
         "fac_profile_dump": ([vp, _c.c_char_p, _c.c_size_t], _c.c_size_t),
         "fac_workspace_bytes": ([vp], _c.c_size_t),
+        "fac_codes_pool_export_size": ([vp, i32, i32, _c.POINTER(_c.c_size_t), _c.POINTER(_c.c_size_t)], i32),
+        "fac_codes_pool_export": ([vp, i32, i32, vp, vp, vp, vp], i32),
+        "fac_codes_pool_import": ([vp, i32, vp, _c.c_size_t, vp, _c.c_size_t, vp], i32),
+        "fac_vc_pool_export_size": ([vp, i32, i32, _c.POINTER(_c.c_size_t), _c.POINTER(_c.c_size_t)], i32),
+        "fac_vc_pool_export": ([vp, i32, i32, vp, vp, vp, vp], i32),
+        "fac_vc_pool_import": ([vp, i32, vp, _c.c_size_t, vp, _c.c_size_t, vp], i32),
+        "fac_dec_pool_export_size": ([vp, i32, i32, _c.POINTER(_c.c_size_t), _c.POINTER(_c.c_size_t)], i32),
+        "fac_dec_pool_export": ([vp, i32, i32, vp, vp, vp, vp], i32),
+        "fac_dec_pool_import": ([vp, i32, vp, _c.c_size_t, vp, _c.c_size_t, vp], i32),
+        "fac_rs_pool_export_size": ([vp, i32, i32, _c.POINTER(_c.c_size_t), _c.POINTER(_c.c_size_t)], i32),
+        "fac_rs_pool_export": ([vp, i32, i32, vp, vp, vp, vp], i32),
+        "fac_rs_pool_import": ([vp, i32, vp, _c.c_size_t, vp, _c.c_size_t, vp], i32),
         "fac_last_launch_count": ([vp], i32),
     }
     for name, (args, res) in sigs.items():
@@ -164,8 +176,8 @@ def load():
 
 EXPORTED = ["fac_abi_version", "fac_create", "fac_destroy", "fac_last_error", "fac_load_tensor", "fac_finalize",
             "fac_encode", "fac_encode_frames", "fac_quantize", "fac_decode", "fac_codec_forward",
-            "fac_codec_forward_host", "fac_codec_encode", "fac_codec_encode_lens", "fac_codec_forward_lens", "fac_codec_timbre_lens", "fac_dequantize", "fac_codes_decode", "fac_codes_decode_lens", "fac_redecode", "fac_redecoder_decode", "fac_voice_convert", "fac_voice_convert_lens", "fac_dataset_mel", "fac_reconstruction_loss", "fac_spectral_loss", "fac_l1_loss", "fac_spectral_loss_grad", "fac_l1_loss_grad", "fac_head_begin", "fac_head_tensor", "fac_head_finalize", "fac_head_forward", "fac_add3", "fac_stream_begin", "fac_stream_encode", "fac_stream_decode", "fac_stream_decode_codes", "fac_stream_encode_codes", "fac_stream_finish_codes", "fac_stream_timbre", "fac_stream_end", "fac_vc_stream_lookahead", "fac_vc_stream_begin", "fac_vc_stream_convert", "fac_vc_stream_finish", "fac_vc_stream_set_timbre", "fac_vc_stream_end", "fac_codes_pool_create", "fac_codes_pool_open", "fac_codes_pool_encode_codes", "fac_codes_pool_finish_codes", "fac_codes_pool_timbre", "fac_codes_pool_close", "fac_codes_pool_destroy", "fac_vc_pool_create", "fac_vc_pool_open", "fac_vc_pool_open_mode", "fac_vc_pool_set_timbre", "fac_vc_pool_convert", "fac_vc_pool_finish", "fac_vc_pool_close", "fac_vc_pool_destroy", "fac_dec_pool_create", "fac_dec_pool_open", "fac_dec_pool_decode_codes", "fac_dec_pool_set_timbre", "fac_dec_pool_close", "fac_dec_pool_destroy", "fac_resample_geometry", "fac_resample_out_len", "fac_resample_ready", "fac_resample_table", "fac_resample", "fac_rs_pool_create", "fac_rs_pool_open", "fac_rs_pool_push", "fac_rs_pool_finish", "fac_rs_pool_undo", "fac_rs_pool_close", "fac_rs_pool_destroy", "fac_rvq_create", "fac_rvq_destroy", "fac_rvq_forward", "fac_alias_free_act",
-            "fac_debug_conv", "fac_debug_conv_tc", "fac_debug_conv_tc_group1", "fac_debug_resunit", "fac_debug_conv_lanes", "fac_debug_resunit_lanes", "fac_debug_tc_phase_clocks", "fac_debug_tc_producer_clocks", "fac_debug_tc_trace", "fac_debug_lstm_pack", "fac_debug_pool_plan", "fac_debug_timbre_plan", "fac_debug_vc_plan", "fac_debug_lstm_lane_map", "fac_debug_convtr_pack", "fac_debug_pad_map", "fac_debug_lane_pad_map", "fac_debug_tc_plan", "fac_debug_tc_plan_group", "fac_debug_tc_pack", "fac_debug_lstm_phase_clocks", "fac_set_option", "fac_debug_slstm", "fac_debug_slstm_lanes", "fac_debug_fa_quantize", "fac_debug_attention", "fac_debug_tap", "fac_profile_enable", "fac_profile_reset", "fac_profile_get", "fac_profile_dump",
+            "fac_codec_forward_host", "fac_codec_encode", "fac_codec_encode_lens", "fac_codec_forward_lens", "fac_codec_timbre_lens", "fac_dequantize", "fac_codes_decode", "fac_codes_decode_lens", "fac_redecode", "fac_redecoder_decode", "fac_voice_convert", "fac_voice_convert_lens", "fac_dataset_mel", "fac_reconstruction_loss", "fac_spectral_loss", "fac_l1_loss", "fac_spectral_loss_grad", "fac_l1_loss_grad", "fac_head_begin", "fac_head_tensor", "fac_head_finalize", "fac_head_forward", "fac_add3", "fac_stream_begin", "fac_stream_encode", "fac_stream_decode", "fac_stream_decode_codes", "fac_stream_encode_codes", "fac_stream_finish_codes", "fac_stream_timbre", "fac_stream_end", "fac_vc_stream_lookahead", "fac_vc_stream_begin", "fac_vc_stream_convert", "fac_vc_stream_finish", "fac_vc_stream_set_timbre", "fac_vc_stream_end", "fac_codes_pool_create", "fac_codes_pool_open", "fac_codes_pool_encode_codes", "fac_codes_pool_finish_codes", "fac_codes_pool_timbre", "fac_codes_pool_close", "fac_codes_pool_destroy", "fac_vc_pool_create", "fac_vc_pool_open", "fac_vc_pool_open_mode", "fac_vc_pool_set_timbre", "fac_vc_pool_convert", "fac_vc_pool_finish", "fac_vc_pool_close", "fac_vc_pool_destroy", "fac_dec_pool_create", "fac_dec_pool_open", "fac_dec_pool_decode_codes", "fac_dec_pool_set_timbre", "fac_dec_pool_close", "fac_dec_pool_destroy", "fac_resample_geometry", "fac_resample_out_len", "fac_resample_ready", "fac_resample_table", "fac_resample", "fac_rs_pool_create", "fac_rs_pool_open", "fac_rs_pool_push", "fac_rs_pool_finish", "fac_rs_pool_undo", "fac_rs_pool_close", "fac_rs_pool_destroy", "fac_codes_pool_export_size", "fac_codes_pool_export", "fac_codes_pool_import", "fac_vc_pool_export_size", "fac_vc_pool_export", "fac_vc_pool_import", "fac_dec_pool_export_size", "fac_dec_pool_export", "fac_dec_pool_import", "fac_rs_pool_export_size", "fac_rs_pool_export", "fac_rs_pool_import", "fac_rvq_create", "fac_rvq_destroy", "fac_rvq_forward", "fac_alias_free_act",
+            "fac_debug_conv", "fac_debug_conv_tc", "fac_debug_conv_tc_group1", "fac_debug_resunit", "fac_debug_conv_lanes", "fac_debug_resunit_lanes", "fac_debug_tc_phase_clocks", "fac_debug_tc_producer_clocks", "fac_debug_tc_trace", "fac_debug_lstm_pack", "fac_debug_pool_plan", "fac_debug_timbre_plan", "fac_debug_vc_plan", "fac_debug_state_header", "fac_debug_lstm_lane_map", "fac_debug_convtr_pack", "fac_debug_pad_map", "fac_debug_lane_pad_map", "fac_debug_tc_plan", "fac_debug_tc_plan_group", "fac_debug_tc_pack", "fac_debug_lstm_phase_clocks", "fac_set_option", "fac_debug_slstm", "fac_debug_slstm_lanes", "fac_debug_fa_quantize", "fac_debug_attention", "fac_debug_tap", "fac_profile_enable", "fac_profile_reset", "fac_profile_get", "fac_profile_dump",
             "fac_workspace_bytes", "fac_last_launch_count"]
 
 

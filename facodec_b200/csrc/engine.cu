@@ -2,6 +2,7 @@
 // launch sequences of Encoder.forward (dac/model/dac.py:69-104), FAquantizer.forward_v2
 // (modules/quantize.py:375-454) and Decoder.forward (dac/model/dac.py:131-165).
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -155,6 +156,7 @@ struct fac_handle {
     std::map<std::string, HostTensor> host[FAC_NUM_MODULES];
     bool have[FAC_NUM_MODULES] = {false, false, false, false, false};
     bool finalized = false;
+    uint64_t fp[FAC_NUM_MODULES] = {0, 0, 0, 0, 0};   // weight fingerprints of the modules, taken at fac_finalize (session state)
     std::vector<float> pack;        // host staging of the weight arena
     float* warena = nullptr; size_t wfloats = 0;
     EncW enc; DecW dec; QuantW qw;
@@ -1509,6 +1511,37 @@ int finish(fac_handle* h, Ctx& c) {
     return FAC_OK;
 }
 
+// FNV-1a 64 of n bytes, continuing from h.
+uint64_t fnv1a(const void* p, size_t n, uint64_t h = 14695981039346656037ull) {
+    const unsigned char* b = static_cast<const unsigned char*>(p);
+    for (size_t i = 0; i < n; ++i) { h ^= b[i]; h *= 1099511628211ull; }
+    return h;
+}
+
+// A module's weight fingerprint: every key, shape and float of its host tensors in key order, the floats as raw words over
+// four interleaved FNV-style lanes (a byte-wise hash of ~100 M floats would add seconds to fac_finalize).  Not a secure hash:
+// it tells apart weights, not adversaries.
+uint64_t weights_fingerprint(const std::map<std::string, HostTensor>& m) {
+    uint64_t h = fnv1a("facodec_b200 weights", 20);
+    for (const auto& kv : m) {
+        h = fnv1a(kv.first.c_str(), kv.first.size() + 1, h);
+        h = fnv1a(kv.second.shape.data(), kv.second.shape.size() * sizeof(int64_t), h);
+        uint64_t l[4] = {h, h + 1, h + 2, h + 3};
+        const float* f = kv.second.data.data();
+        const size_t n = kv.second.data.size();
+        size_t i = 0;
+        for (; i + 4 <= n; i += 4)
+            for (int k = 0; k < 4; ++k) {
+                uint32_t w;
+                std::memcpy(&w, f + i + k, 4);
+                l[k] = (l[k] ^ w) * 1099511628211ull;
+            }
+        for (; i < n; ++i) { uint32_t w; std::memcpy(&w, f + i, 4); l[0] = (l[0] ^ w) * 1099511628211ull; }
+        h = fnv1a(l, sizeof l, h);
+    }
+    return h;
+}
+
 // run `body` twice: size pass, then for real
 template <typename F>
 int two_pass(fac_handle* h, cudaStream_t st, F body) {
@@ -1600,6 +1633,7 @@ int fac_finalize(fac_handle* h) {
     if (e != cudaSuccess) { h->err = std::string("weight upload: ") + cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
     h->wfloats = n;
     h->pack.clear(); h->pack.shrink_to_fit();
+    for (int m = 0; m < FAC_NUM_MODULES; ++m) h->fp[m] = h->have[m] ? weights_fingerprint(h->host[m]) : 0;
     for (int m = 0; m < FAC_NUM_MODULES; ++m) h->host[m].clear();
     h->finalized = true;
     return FAC_OK;
@@ -2061,12 +2095,12 @@ void copy_rows(Ctx& c, E* dst, int dst_pitch_rows, const E* src, int src_pitch_r
                                  cudaMemcpyDeviceToDevice, c.st), what);
 }
 
-// Inside a launch sequence: lane b of n copies `words` (a count, or a function of b) 32-bit words from src(b) to dst(b)
+// Inside a launch sequence: lane b of n <= N copies `words` (a count, or a function of b) 32-bit words from src(b) to dst(b)
 // (launch_lane_copy).
-template <typename W, typename S, typename D>
+template <int N = kLaneMax, typename W, typename S, typename D>
 void lane_copy(Ctx& c, int n, W words, S src, D dst, const char* what) {
     if (c.dry) return;
-    LaneCopyParams p;
+    LaneCopyParamsN<N> p;
     p.n = n;
     for (int b = 0; b < n; ++b) {
         p.src[b] = (const uint32_t*)src(b); p.dst[b] = (uint32_t*)dst(b);
@@ -3346,6 +3380,386 @@ int fac_rs_pool_close(fac_handle* h, int pool_id, int session) {
 
 int fac_rs_pool_destroy(fac_handle* h, int pool_id) { return h ? fac::rs_pool_destroy(rs_env(h), pool_id) : FAC_ERR_INVALID; }
 
+}  // extern "C"
+
+// ---- session state (fac_*_pool_export / _import; layout in include/facodec_b200.h) ----
+// A kind adapter binds to one pool and knows its slots: read(session) gives an open session's counters and regions;
+// place(state) checks an imported state's counters and region sizes against the pool, readies a free slot (growing its
+// buffers if need be) and points the state's regions at it, returning the slot; commit(slot, state) opens that slot.  The
+// templates below do the rest, alike for every kind: the header, the checks, and one lane_copy launch per region.
+namespace {
+using fac::SlotState;
+constexpr int kStateOptions = 11;
+
+uint64_t kind_fingerprint(int kind, uint64_t a, uint64_t b) {
+    const uint64_t v[3] = {(uint64_t)kind, a, b};
+    return fnv1a(v, sizeof v);
+}
+
+void state_options(const fac_handle* h, int64_t* o) {
+    const int64_t v[kStateOptions] = {h->use_tc, h->fuse_res, h->lstm_v2, h->dec_lstm_fp16, h->attn_stream, h->dec_c7_f16,
+                                      h->enc_f16, h->enc_tt, h->tc_occ2, h->dec_bf16, h->overlap_front};
+    std::copy(v, v + kStateOptions, o);
+}
+
+uint64_t header_checksum(const fac_state_header& hd) { return fnv1a(&hd, offsetof(fac_state_header, checksum)); }
+
+bool on_device(const void* p, int device) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device;
+}
+
+int state_error(fac_handle* h, const char* who, const std::string& what, int rc) {
+    h->err = std::string(who) + ": " + what;
+    return rc;
+}
+
+void set_regions(SlotState& st, std::initializer_list<std::pair<void*, long long>> r) {
+    st.nreg = 0;
+    for (const auto& x : r) { st.region[st.nreg] = x.first; st.bytes[st.nreg] = x.second; ++st.nreg; }
+}
+
+// Export reads open sessions; import takes the first free slot.
+template <typename S>
+int check_open(fac_handle* h, const Pool<S>& P, int session, const char* who) {
+    if (session < 0 || session >= P.cap || !P.used[session])
+        return state_error(h, who, "session " + std::to_string(session) + " is not open", FAC_ERR_INVALID);
+    return FAC_OK;
+}
+template <typename S>
+int free_slot(fac_handle* h, const Pool<S>& P, const char* who) {
+    int i = 0;
+    while (i < P.cap && P.used[i]) ++i;
+    if (i == P.cap) return state_error(h, who, "the pool is full (capacity " + std::to_string(P.cap) + ")", FAC_ERR_STATE);
+    return i;
+}
+
+// Points an imported state at the regions `want` of its readied slot; their sizes must be the header's.
+int adopt(fac_handle* h, const SlotState& want, SlotState& st, const char* who) {
+    if (!std::equal(want.bytes, want.bytes + FAC_STATE_REGIONS, st.bytes))
+        return state_error(h, who, "the region sizes disagree with the counters", FAC_ERR_INVALID);
+    std::copy(want.region, want.region + FAC_STATE_REGIONS, st.region);
+    st.nreg = want.nreg;
+    return FAC_OK;
+}
+
+// counters {n_c, mode, samples, emitted, x_hist_len, ey_hist_len}; regions {x_hist, ey_hist, z_held, carry, mel rows}
+struct CodesKind {
+    static constexpr int kind = FAC_STATE_CODES;
+    fac_handle* h = nullptr; CodesPool* P = nullptr;
+    int bind(fac_handle* hh, int id, const char* who) {
+        h = hh;
+        if (int rc = check_ready(h, {FAC_ENCODER, FAC_QUANTIZER})) return rc;
+        P = by_id(h, &fac_handle::codes_pools, id);
+        return P ? FAC_OK : state_error(h, who, "no such pool", FAC_ERR_INVALID);
+    }
+    uint64_t fingerprint() const { return kind_fingerprint(kind, h->fp[FAC_ENCODER], h->fp[FAC_QUANTIZER]); }
+    static void regions(const EncHalf& s, long long rows, SlotState& st) {
+        set_regions(st, {{s.x_hist, 4LL * kEncCtx}, {s.ey_hist, 4LL * 2 * LATENT}, {s.z_held, 4LL * LATENT},
+                         {s.carry, 4LL * 2 * carry_words(LATENT, 1)}, {s.mel.get(), 4LL * N_MELS * rows}});
+    }
+    int read(int sid, SlotState& st, const char* who) {
+        if (int rc = check_open(h, *P, sid, who)) return rc;
+        const EncHalf& s = P->slot[sid];
+        if (s.mode == EncHalf::kFinished)
+            return state_error(h, who, "session " + std::to_string(sid) + " was finished by finish_codes", FAC_ERR_STATE);
+        const long long c[6] = {P->lanes.n_c, s.mode, s.samples, s.emitted, s.x_hist_len, s.ey_hist_len};
+        std::copy(c, c + 6, st.counters);
+        regions(s, s.emitted, st);
+        return FAC_OK;
+    }
+    int place(SlotState& st, const char* who, cudaStream_t stream) {
+        const long long* c = st.counters;
+        if (c[0] != P->lanes.n_c)
+            return state_error(h, who, "the state's n_c " + std::to_string(c[0]) + " is not the pool's " + std::to_string(P->lanes.n_c),
+                               FAC_ERR_STATE);
+        const long long S = c[2], frames = S / HOP;
+        if (!((c[1] == EncHalf::kNone && S == 0) || (c[1] == EncHalf::kCodes && S >= kStreamMinFirst * HOP)) || S % HOP ||
+            c[3] != (S ? frames - 1 : 0) || c[4] != std::min<long long>(S, kEncCtx) || c[5] != std::min<long long>(frames, 2) ||
+            frames > (1LL << 30))
+            return state_error(h, who, "the encoder counters are inconsistent", FAC_ERR_INVALID);
+        int i = free_slot(h, *P, who);
+        if (i < 0) return i;
+        EncHalf& s = P->slot[i];
+        if (int rc = grow_mel(h, s, 1, 0, (int)c[3], stream)) return rc;
+        SlotState want;
+        regions(s, c[3], want);
+        return adopt(h, want, st, who) ? FAC_ERR_INVALID : i;
+    }
+    void commit(int i, const SlotState& st) {
+        EncHalf& s = P->slot[i];
+        s.mode = (int)st.counters[1]; s.samples = st.counters[2]; s.emitted = st.counters[3];
+        s.x_hist_len = (int)st.counters[4]; s.ey_hist_len = (int)st.counters[5];
+        P->used[i] = 1;
+    }
+};
+
+// counters {use_p, use_c, n_c, stale, N, Zf, Yf}; regions {g, codes, z}
+struct VcKind {
+    static constexpr int kind = FAC_STATE_VC;
+    fac_handle* h = nullptr; VcPool* P = nullptr;
+    int bind(fac_handle* hh, int id, const char* who) {
+        h = hh;
+        if (int rc = check_ready(h, {FAC_REDECODER, FAC_REDECODER_DECODER})) return rc;
+        P = by_id(h, &fac_handle::vc_pools, id);
+        return P ? FAC_OK : state_error(h, who, "no such pool", FAC_ERR_INVALID);
+    }
+    uint64_t fingerprint() const { return kind_fingerprint(kind, h->fp[FAC_REDECODER], h->fp[FAC_REDECODER_DECODER]); }
+    void regions(const VcStream& s, SlotState& st) const {
+        set_regions(st, {{s.g, 4LL * (long long)redecoder_cond_floats(h, 1)}, {s.codes, 8LL * 3 * kVcCodesHist},
+                         {s.z, 4LL * kVcZHist * LATENT}});
+    }
+    int read(int sid, SlotState& st, const char* who) {
+        if (int rc = check_open(h, *P, sid, who)) return rc;
+        const VcStream& s = P->slot[sid];
+        if (s.finished) return state_error(h, who, "session " + std::to_string(sid) + " was finished", FAC_ERR_STATE);
+        const long long c[7] = {s.use_p, s.use_c, s.n_c, s.stale, s.N, s.Zf, s.Yf};
+        std::copy(c, c + 7, st.counters);
+        regions(s, st);
+        return FAC_OK;
+    }
+    int place(SlotState& st, const char* who, cudaStream_t) {
+        const long long* c = st.counters;
+        if (c[0] < 0 || c[0] > 1 || c[1] < 0 || c[1] > 1 || c[2] < 0 || c[2] > 2 || c[3] < 0 || c[3] > 1 || c[6] < 0 ||
+            c[6] > c[5] || c[5] > c[4])
+            return state_error(h, who, "the conversion counters are inconsistent", FAC_ERR_INVALID);
+        int i = free_slot(h, *P, who);
+        if (i < 0) return i;
+        SlotState want;
+        regions(P->slot[i], want);
+        return adopt(h, want, st, who) ? FAC_ERR_INVALID : i;
+    }
+    void commit(int i, const SlotState& st) {
+        VcStream& s = P->slot[i];
+        const long long* c = st.counters;
+        s.use_p = (int)c[0]; s.use_c = (int)c[1]; s.n_c = (int)c[2]; s.stale = c[3] != 0; s.N = c[4]; s.Zf = c[5]; s.Yf = c[6];
+        s.finished = false;
+        P->used[i] = 1;
+    }
+};
+
+// counters {frames}; regions {z_hist, dy_hist, carry, gamma | beta}
+struct DecKind {
+    static constexpr int kind = FAC_STATE_DEC;
+    fac_handle* h = nullptr; DecPool* P = nullptr;
+    int bind(fac_handle* hh, int id, const char* who) {
+        h = hh;
+        if (int rc = check_ready(h, {FAC_QUANTIZER, FAC_DECODER})) return rc;
+        P = by_id(h, &fac_handle::dec_pools, id);
+        return P ? FAC_OK : state_error(h, who, "no such pool", FAC_ERR_INVALID);
+    }
+    uint64_t fingerprint() const { return kind_fingerprint(kind, h->fp[FAC_QUANTIZER], h->fp[FAC_DECODER]); }
+    static void regions(const DecHalf& s, SlotState& st) {
+        set_regions(st, {{s.z_hist, 4LL * 6 * LATENT}, {s.dy_hist, 4LL * kDecCtx * 1536}, {s.carry, 4LL * 2 * carry_words(1536, 0)},
+                         {s.gb, 4LL * 2048}});
+    }
+    int read(int sid, SlotState& st, const char* who) {
+        if (int rc = check_open(h, *P, sid, who)) return rc;
+        st.counters[0] = P->slot[sid].frames;
+        regions(P->slot[sid], st);
+        return FAC_OK;
+    }
+    int place(SlotState& st, const char* who, cudaStream_t) {
+        if (st.counters[0] < 0) return state_error(h, who, "the decoder counters are inconsistent", FAC_ERR_INVALID);
+        int i = free_slot(h, *P, who);
+        if (i < 0) return i;
+        SlotState want;
+        regions(P->slot[i], want);
+        return adopt(h, want, st, who) ? FAC_ERR_INVALID : i;
+    }
+    void commit(int i, const SlotState& st) {
+        P->slot[i].frames = st.counters[0];
+        P->used[i] = 1;
+    }
+};
+
+// resample.cu keeps the slots; see fac::rs_slot_read / _place / _commit
+struct RsKind {
+    static constexpr int kind = FAC_STATE_RS;
+    fac_handle* h = nullptr; int id = -1;
+    int bind(fac_handle* hh, int pid, const char*) {     // read and place check the pool id
+        h = hh; id = pid;
+        return FAC_OK;
+    }
+    uint64_t fingerprint() const { return 0; }
+    int read(int sid, SlotState& st, const char* who) { return fac::rs_slot_read(rs_env(h), id, sid, st, who); }
+    int place(SlotState& st, const char* who, cudaStream_t) { return fac::rs_slot_place(rs_env(h), id, st, who); }
+    void commit(int i, const SlotState& st) { fac::rs_slot_commit(rs_env(h), id, i, st); }
+};
+
+// Moves region r of n states: src(i, r) -> dst(i, r), one launch per region for up to kMoveLanes states.
+template <typename Src, typename Dst>
+int move_regions(fac_handle* h, int n, int nreg, const std::vector<SlotState>& st, Src src, Dst dst, cudaStream_t stream) {
+    return two_pass(h, stream, [&](Ctx& c) {
+        for (int r = 0; r < nreg; ++r)
+            for (int o = 0; o < n; o += kMoveLanes)
+                lane_copy<kMoveLanes>(c, std::min(n - o, kMoveLanes), [&](int b) { return st[o + b].bytes[r] / 4; },
+                                      [&](int b) { return src(o + b, r); }, [&](int b) { return dst(o + b, r); }, "state.region");
+    });
+}
+
+long long payload_offset(const SlotState& st, int r) {
+    long long off = 0;
+    for (int k = 0; k < r; ++k) off += st.bytes[k];
+    return off;
+}
+
+template <typename K>
+int state_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes, const char* who) {
+    if (!h) return FAC_ERR_INVALID;
+    K k;
+    if (int rc = k.bind(h, pool_id, who)) return rc;
+    if (!header_bytes || !payload_bytes) return state_error(h, who, "null output", FAC_ERR_INVALID);
+    SlotState st;
+    if (int rc = k.read(session, st, who)) return rc;
+    *header_bytes = sizeof(fac_state_header);
+    *payload_bytes = (size_t)payload_offset(st, st.nreg);
+    return FAC_OK;
+}
+
+template <typename K>
+int state_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads, void* stream,
+                 const char* who) {
+    if (!h) return FAC_ERR_INVALID;
+    K k;
+    if (int rc = k.bind(h, pool_id, who)) return rc;
+    if (n < 0 || (n > 0 && (!sessions || !headers || !payloads))) return state_error(h, who, "bad arguments", FAC_ERR_INVALID);
+    std::vector<SlotState> st(n);
+    std::vector<int> seen;
+    for (int i = 0; i < n; ++i) {
+        if (int rc = k.read(sessions[i], st[i], who)) return rc;
+        if (std::find(seen.begin(), seen.end(), sessions[i]) != seen.end())
+            return state_error(h, who, "session " + std::to_string(sessions[i]) + " is named twice", FAC_ERR_INVALID);
+        seen.push_back(sessions[i]);
+        if (!headers[i] || (payload_offset(st[i], st[i].nreg) > 0 &&
+                            (!payloads[i] || (uintptr_t)payloads[i] % 4 || !on_device(payloads[i], h->device))))
+            return state_error(h, who, "session " + std::to_string(sessions[i]) +
+                                       ": a null header, or a payload that is not 4-byte aligned memory of the handle's device",
+                               FAC_ERR_INVALID);
+    }
+    const uint64_t fp = k.fingerprint();
+    for (int i = 0; i < n; ++i) {
+        fac_state_header hd;
+        std::memset(&hd, 0, sizeof hd);
+        hd.magic = FAC_STATE_MAGIC; hd.version = FAC_STATE_VERSION; hd.kind = K::kind; hd.header_bytes = sizeof hd;
+        hd.fingerprint = fp;
+        state_options(h, hd.options);
+        std::copy(st[i].counters, st[i].counters + FAC_STATE_COUNTERS, hd.counters);
+        std::copy(st[i].bytes, st[i].bytes + st[i].nreg, hd.region_bytes);
+        hd.payload_bytes = (uint64_t)payload_offset(st[i], st[i].nreg);
+        hd.checksum = header_checksum(hd);
+        std::memcpy(headers[i], &hd, sizeof hd);
+    }
+    if (n == 0) { h->launches = 0; return FAC_OK; }
+    return move_regions(h, n, st[0].nreg, st, [&](int i, int r) { return st[i].region[r]; },
+                        [&](int i, int r) { return (char*)payloads[i] + payload_offset(st[i], r); }, (cudaStream_t)stream);
+}
+
+// The header checks of an import into a pool of `kind` whose weights give `fp` and whose handle has options `opts`: on
+// success st holds the header's counters and region sizes.  Host only (fac_debug_state_header).
+int check_header(const void* header, size_t header_bytes, int kind, uint64_t fp, const int64_t* opts, size_t payload_bytes,
+                 SlotState& st, std::string& err) {
+    fac_state_header hd;
+    auto fail = [&](const std::string& what, int rc) { err = what; return rc; };
+    if (!header || header_bytes < sizeof hd) return fail("the header is missing or truncated", FAC_ERR_INVALID);
+    std::memcpy(&hd, header, sizeof hd);
+    if (hd.magic != FAC_STATE_MAGIC || hd.header_bytes != sizeof hd || header_bytes != sizeof hd)
+        return fail("not a session-state header", FAC_ERR_INVALID);
+    if (hd.checksum != header_checksum(hd)) return fail("the header is corrupt (checksum)", FAC_ERR_INVALID);
+    if (hd.version != FAC_STATE_VERSION)
+        return fail("state format version " + std::to_string(hd.version) + ", this library reads " + std::to_string(FAC_STATE_VERSION),
+                    FAC_ERR_STATE);
+    if (hd.kind != (uint32_t)kind)
+        return fail("a state of pool kind " + std::to_string(hd.kind) + ", this pool is kind " + std::to_string(kind), FAC_ERR_INVALID);
+    if (hd.fingerprint != fp) return fail("the state comes from other weights", FAC_ERR_STATE);
+    if (!std::equal(opts, opts + FAC_STATE_OPTIONS, hd.options))
+        return fail("the state comes from a handle with other fac_set_option values", FAC_ERR_STATE);
+    std::copy(hd.counters, hd.counters + FAC_STATE_COUNTERS, st.counters);
+    unsigned long long total = 0;
+    for (int r = 0; r < FAC_STATE_REGIONS; ++r) {
+        if (hd.region_bytes[r] < 0 || hd.region_bytes[r] % 4 || hd.region_bytes[r] > (1LL << 40)) return fail("a bad region size", FAC_ERR_INVALID);
+        st.bytes[r] = hd.region_bytes[r];
+        total += (unsigned long long)hd.region_bytes[r];
+    }
+    if (total != hd.payload_bytes || payload_bytes != hd.payload_bytes)
+        return fail("the payload size disagrees with the header", FAC_ERR_INVALID);
+    return FAC_OK;
+}
+
+template <typename K>
+int state_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload, size_t payload_bytes,
+                 void* stream, const char* who) {
+    if (!h) return FAC_ERR_INVALID;
+    K k;
+    if (int rc = k.bind(h, pool_id, who)) return rc;
+    int64_t opts[FAC_STATE_OPTIONS] = {};
+    state_options(h, opts);
+    SlotState st;
+    std::string why;
+    if (int rc = check_header(header, header_bytes, K::kind, k.fingerprint(), opts, payload_bytes, st, why))
+        return state_error(h, who, why, rc);
+    if (payload_bytes > 0 && (!payload || (uintptr_t)payload % 4 || !on_device(payload, h->device)))
+        return state_error(h, who, "the payload is not 4-byte aligned memory of the handle's device (cuda:" +
+                                   std::to_string(h->device) + ")", FAC_ERR_INVALID);
+    const int slot = k.place(st, who, (cudaStream_t)stream);
+    if (slot < 0) return slot;
+    std::vector<SlotState> one{st};
+    int rc = move_regions(h, 1, st.nreg, one, [&](int, int r) { return (const char*)payload + payload_offset(st, r); },
+                          [&](int, int r) { return st.region[r]; }, (cudaStream_t)stream);
+    if (rc) return rc;
+    k.commit(slot, st);
+    return slot;
+}
+}  // namespace
+
+extern "C" {
+
+int fac_codes_pool_export_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes) {
+    return state_size<CodesKind>(h, pool_id, session, header_bytes, payload_bytes, "fac_codes_pool_export_size");
+}
+int fac_codes_pool_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads,
+                          void* stream) {
+    return state_export<CodesKind>(h, pool_id, n, sessions, headers, payloads, stream, "fac_codes_pool_export");
+}
+int fac_codes_pool_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload,
+                          size_t payload_bytes, void* stream) {
+    return state_import<CodesKind>(h, pool_id, header, header_bytes, payload, payload_bytes, stream, "fac_codes_pool_import");
+}
+int fac_vc_pool_export_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes) {
+    return state_size<VcKind>(h, pool_id, session, header_bytes, payload_bytes, "fac_vc_pool_export_size");
+}
+int fac_vc_pool_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads,
+                       void* stream) {
+    return state_export<VcKind>(h, pool_id, n, sessions, headers, payloads, stream, "fac_vc_pool_export");
+}
+int fac_vc_pool_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload,
+                       size_t payload_bytes, void* stream) {
+    return state_import<VcKind>(h, pool_id, header, header_bytes, payload, payload_bytes, stream, "fac_vc_pool_import");
+}
+int fac_dec_pool_export_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes) {
+    return state_size<DecKind>(h, pool_id, session, header_bytes, payload_bytes, "fac_dec_pool_export_size");
+}
+int fac_dec_pool_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads,
+                        void* stream) {
+    return state_export<DecKind>(h, pool_id, n, sessions, headers, payloads, stream, "fac_dec_pool_export");
+}
+int fac_dec_pool_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload,
+                        size_t payload_bytes, void* stream) {
+    return state_import<DecKind>(h, pool_id, header, header_bytes, payload, payload_bytes, stream, "fac_dec_pool_import");
+}
+int fac_rs_pool_export_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes) {
+    return state_size<RsKind>(h, pool_id, session, header_bytes, payload_bytes, "fac_rs_pool_export_size");
+}
+int fac_rs_pool_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads,
+                       void* stream) {
+    return state_export<RsKind>(h, pool_id, n, sessions, headers, payloads, stream, "fac_rs_pool_export");
+}
+int fac_rs_pool_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload,
+                       size_t payload_bytes, void* stream) {
+    return state_import<RsKind>(h, pool_id, header, header_bytes, payload, payload_bytes, stream, "fac_rs_pool_import");
+}
+
 int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* lengths, int* group, int* batch) {
     if (n < 0 || (n > 0 && (!counters || !lengths || !group || !batch)) || kind < 0 || kind > 3) return FAC_ERR_INVALID;
     std::vector<std::vector<long long>> keys(n);
@@ -3356,6 +3770,16 @@ int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* l
                 : kind == 2 ? dec_plan(c[0]).key() : vc_plan(c[0], c[1], c[2], lengths[i], false, c[3] != 0).key();
     }
     return (int)pool_plan(keys, group, batch).size();
+}
+
+int fac_debug_state_header(const void* header, size_t header_bytes, int kind, uint64_t fingerprint, const int64_t* options,
+                           size_t payload_bytes, long long* counters_out) {
+    if (!options) return FAC_ERR_INVALID;
+    SlotState st;
+    std::string why;
+    int rc = check_header(header, header_bytes, kind, fingerprint, options, payload_bytes, st, why);
+    if (rc == FAC_OK && counters_out) std::copy(st.counters, st.counters + FAC_STATE_COUNTERS, counters_out);
+    return rc;
 }
 
 int fac_debug_vc_plan(long long N, long long Zf, long long Yf, int F, int finish, int stale, long long* out16) {

@@ -118,14 +118,20 @@ struct LaneCarryParams {
     int n = 0, H = 0, U = 0, pass3 = 0, to_lanes = 0;
 };
 cudaError_t launch_lstm2_lane_carry(const LaneCarryParams& p, cudaStream_t st);
-// dst[b][0, words[b]) = src[b][0, words[b]) for lanes b < n (32-bit words; pool.cu): the slot <-> lane moves of the stream pools
-struct LaneCopyParams {
-    const uint32_t* src[kLaneMax];
-    uint32_t* dst[kLaneMax];
-    long long words[kLaneMax];
+// dst[b][0, words[b]) = src[b][0, words[b]) for lanes b < n (32-bit words; pool.cu): the slot <-> lane moves of the stream
+// pools (N = kLaneMax), and the slot <-> state-payload moves of a session export or import (N = kMoveLanes, one launch per
+// state region for up to that many sessions; the 24 KB parameter block stays under sm_90's 32 764-byte limit).
+constexpr int kMoveLanes = 1024;
+template <int N>
+struct LaneCopyParamsN {
+    const uint32_t* src[N];
+    uint32_t* dst[N];
+    long long words[N];
     int n = 0;
 };
-cudaError_t launch_lane_copy(const LaneCopyParams& p, cudaStream_t st);
+using LaneCopyParams = LaneCopyParamsN<kLaneMax>;
+cudaError_t launch_lane_copy(const LaneCopyParamsN<kLaneMax>& p, cudaStream_t st);
+cudaError_t launch_lane_copy(const LaneCopyParamsN<kMoveLanes>& p, cudaStream_t st);
 int lstm_units_per_cta(int H);
 cudaError_t lstm_read_phase_clocks(long long* out4);   // CTA-0 accumulated phase clocks of the last launch  // U such that H % U == 0 and H / U <= resident CTAs
 

@@ -327,6 +327,24 @@ int rs_pool_create(RsEnv e, int capacity, int quantum) {
 }
 
 namespace {
+// Grow-only history buffers of a free slot: a reopened slot keeps its buffers.
+int grow_slot(RsEnv& e, RsSlot& s, int cap, const char* who) {
+    if (cap <= s.cap) return FAC_OK;
+    cudaError_t err = cudaSetDevice(e.device);
+    float* b[2] = {nullptr, nullptr};
+    for (int k = 0; k < 2 && err == cudaSuccess; ++k) err = cudaMalloc(&b[k], sizeof(float) * cap);
+    if (err != cudaSuccess) {
+        cudaFree(b[0]); cudaFree(b[1]);
+        e.err = std::string(who) + ": " + cudaGetErrorString(err);
+        cudaGetLastError();
+        return FAC_ERR_CUDA;
+    }
+    cudaDeviceSynchronize();                         // the old buffers may still be read by queued steps
+    cudaFree(s.buf[0]); cudaFree(s.buf[1]);
+    s.buf[0] = b[0]; s.buf[1] = b[1]; s.cap = cap;
+    return FAC_OK;
+}
+
 RsPool* pool_of(RsEnv& e, int id, const char* who) {
     RsHost& H = host_of(e);
     RsPool* P = id >= 0 && id < (int)H.pools.size() ? H.pools[id].get() : nullptr;
@@ -349,21 +367,7 @@ int rs_pool_open(RsEnv e, int pool_id, int orig, int nw) {
         return FAC_ERR_STATE;
     }
     RsSlot& s = P->slot[i];
-    const int cap = hist_cap(t->orig, t->nw, t->K, P->quantum);
-    if (cap > s.cap) {                                   // grow-only: a reopened slot keeps its buffers
-        cudaError_t err = cudaSetDevice(e.device);
-        float* b[2] = {nullptr, nullptr};
-        for (int k = 0; k < 2 && err == cudaSuccess; ++k) err = cudaMalloc(&b[k], sizeof(float) * cap);
-        if (err != cudaSuccess) {
-            cudaFree(b[0]); cudaFree(b[1]);
-            e.err = std::string(who) + ": " + cudaGetErrorString(err);
-            cudaGetLastError();
-            return FAC_ERR_CUDA;
-        }
-        cudaDeviceSynchronize();                         // the old buffers may still be read by queued steps
-        cudaFree(s.buf[0]); cudaFree(s.buf[1]);
-        s.buf[0] = b[0]; s.buf[1] = b[1]; s.cap = cap;
-    }
+    if ((rc = grow_slot(e, s, hist_cap(t->orig, t->nw, t->K, P->quantum), who))) return rc;
     s.used = true; s.finished = false;
     s.orig = t->orig; s.nw = t->nw; s.width = t->width; s.K = t->K; s.tab = t->dev;
     s.seen = s.emitted = s.hs = 0; s.hl = 0; s.cur = 0;
@@ -476,5 +480,74 @@ int rs_pool_destroy(RsEnv e, int pool_id) {
 }
 
 void rs_host_free(RsHost* host) { delete host; }
+
+// counters: {quantum, orig, new, width, K, seen, emitted, hs, hl} (include/facodec_b200.h, FAC_STATE_RS)
+int rs_slot_read(RsEnv e, int pool_id, int session, SlotState& st, const char* who) {
+    RsPool* P = pool_of(e, pool_id, who);
+    if (!P) return FAC_ERR_INVALID;
+    if (session < 0 || session >= (int)P->slot.size() || !P->slot[session].used) {
+        e.err = std::string(who) + ": session " + std::to_string(session) + " is not open";
+        return FAC_ERR_INVALID;
+    }
+    const RsSlot& s = P->slot[session];
+    if (s.finished) { e.err = std::string(who) + ": session " + std::to_string(session) + " is finished"; return FAC_ERR_STATE; }
+    const long long c[9] = {P->quantum, s.orig, s.nw, s.width, s.K, s.seen, s.emitted, s.hs, s.hl};
+    std::copy(c, c + 9, st.counters);
+    st.nreg = 1;
+    st.region[0] = s.buf[s.cur];
+    st.bytes[0] = (long long)sizeof(float) * s.hl;
+    return FAC_OK;
+}
+
+int rs_slot_place(RsEnv e, int pool_id, SlotState& st, const char* who) {
+    RsPool* P = pool_of(e, pool_id, who);
+    if (!P) return FAC_ERR_INVALID;
+    const long long* c = st.counters;
+    if (c[0] != P->quantum) {
+        e.err = std::string(who) + ": the state's quantum " + std::to_string(c[0]) + " is not the pool's " + std::to_string(P->quantum);
+        return FAC_ERR_STATE;
+    }
+    RsHost& H = host_of(e);
+    auto it = H.tables.find({(int)c[1], (int)c[2]});
+    if (it == H.tables.end() && c[1] == 1 && c[2] == 1) {               // equal rates: the one-tap copy table
+        const float one = 1.f;
+        if (int rc = rs_table(e, 24000, 24000, &one)) return rc;
+        it = H.tables.find({1, 1});
+    }
+    if (it == H.tables.end()) {
+        e.err = std::string(who) + ": no filter table for the reduced pair " + std::to_string(c[1]) + " -> " + std::to_string(c[2]) +
+                " (register it with fac_resample_table)";
+        return FAC_ERR_STATE;
+    }
+    const RsTable& t = it->second;
+    const int cap = hist_cap(t.orig, t.nw, t.K, P->quantum);
+    const long long seen = c[5], emitted = c[6], hs = c[7], hl = c[8];
+    if (c[3] != t.width || c[4] != t.K || seen < 0 || emitted < 0 || emitted > out_len_reduced(t.orig, t.nw, seen) || hs < 0 ||
+        hl < 0 || hl > cap || hs + hl != seen || st.bytes[0] != (long long)sizeof(float) * hl ||
+        std::any_of(st.bytes + 1, st.bytes + FAC_STATE_REGIONS, [](long long b) { return b != 0; })) {
+        e.err = std::string(who) + ": the resampler counters are inconsistent";
+        return FAC_ERR_INVALID;
+    }
+    int i = 0;
+    while (i < (int)P->slot.size() && P->slot[i].used) ++i;
+    if (i == (int)P->slot.size()) {
+        e.err = std::string(who) + ": the pool is full (capacity " + std::to_string(P->slot.size()) + ")";
+        return FAC_ERR_STATE;
+    }
+    RsSlot& s = P->slot[i];
+    if (int rc = grow_slot(e, s, cap, who)) return rc;
+    s.orig = t.orig; s.nw = t.nw; s.width = t.width; s.K = t.K; s.tab = t.dev;
+    st.region[0] = s.buf[0];
+    st.nreg = 1;
+    return i;
+}
+
+void rs_slot_commit(RsEnv e, int pool_id, int slot, const SlotState& st) {
+    RsPool* P = pool_of(e, pool_id, "fac_rs_pool_import");
+    RsSlot& s = P->slot[slot];
+    s.used = true; s.finished = false;
+    s.seen = st.counters[5]; s.emitted = st.counters[6]; s.hs = st.counters[7]; s.hl = (int)st.counters[8]; s.cur = 0;
+    P->undo[slot] = 0;
+}
 
 }  // namespace fac

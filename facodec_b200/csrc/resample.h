@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <string>
 
+#include "../../include/facodec_b200.h"
+
 namespace fac {
 
 struct RsHost;
@@ -31,5 +33,22 @@ int rs_pool_undo(RsEnv e, int pool_id, int n, const int* sessions);
 int rs_pool_close(RsEnv e, int pool_id, int session);
 int rs_pool_destroy(RsEnv e, int pool_id);
 void rs_host_free(RsHost* host);
+
+// One pool session's state as fac_*_pool_export / _import move it (engine.cu): the header's counters and the slot's device
+// regions, in payload order.
+struct SlotState {
+    long long counters[FAC_STATE_COUNTERS] = {};
+    void* region[FAC_STATE_REGIONS] = {};
+    long long bytes[FAC_STATE_REGIONS] = {};
+    int nreg = 0;
+};
+// The state of open session `session` of a resampler pool (FAC_ERR_STATE once finished).
+int rs_slot_read(RsEnv e, int pool_id, int session, SlotState& s, const char* who);
+// Checks an imported state's counters and region sizes against the pool and the pair's table, and readies a free slot for
+// it (its buffers grown if need be): s.region[0] becomes the slot's history buffer.  Returns the slot or a status; nothing
+// an open session sees changes.
+int rs_slot_place(RsEnv e, int pool_id, SlotState& s, const char* who);
+// Opens the slot rs_slot_place readied, with the state's counters (no step to take back).
+void rs_slot_commit(RsEnv e, int pool_id, int slot, const SlotState& s);
 
 }  // namespace fac

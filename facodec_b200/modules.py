@@ -13,9 +13,11 @@ Drop-in contract (SURVEY.md section 8b):
 * There is no CPU fallback: CPU tensors or a missing library raise.
 """
 import ctypes
+import json
 import math
 import operator
 import os
+import struct
 from collections import OrderedDict
 
 import torch
@@ -777,10 +779,85 @@ def _ptr_array(ctype, items):
     return (ctype * max(len(items), 1))(*items)
 
 
+class SessionState:
+    """One live pool session taken out of its pool by ``export``: the C header (``header``, bytes), the slot's device state
+    (``payload``, a uint8 tensor) and the pool's Python-side bookkeeping of the session (``info``: counts, and the 24 kHz
+    samples a codes session at another rate holds before its first 3000).  A session opened at another sample rate carries
+    its resampler session's state in ``rate``.  ``import_session`` on any pool of the same kind, model and options (any
+    device, handle or process) continues it bit for bit.  ``kind`` is "codes", "vc", "dec" or "rs"."""
+
+    _MAGIC = b"FACSESS1"
+
+    def __init__(self, kind, header, payload, info=None, rate=None):
+        self.kind = kind
+        self.header = bytes(header)
+        self.payload = payload
+        self.info = dict(info or {})
+        self.rate = rate
+
+    @property
+    def nbytes(self):
+        """Bytes held: header, payload, held samples and the resampler state."""
+        held = self.info.get("held")
+        return (len(self.header) + self.payload.numel() + (0 if held is None else 4 * held.numel()) +
+                (0 if self.rate is None else self.rate.nbytes))
+
+    def to(self, device):
+        """The same state with its tensors on ``device`` (import_session also moves them itself)."""
+        info = {k: v.to(device) if torch.is_tensor(v) else v for k, v in self.info.items()}
+        return SessionState(self.kind, self.header, self.payload.to(device), info, None if self.rate is None else self.rate.to(device))
+
+    def cpu(self):
+        return self.to("cpu")
+
+    def to_bytes(self):
+        """A self-contained byte string (waits for the export to land): for parking a session or handing it to another
+        process.  SessionState.from_bytes reads it back."""
+        held = self.info.get("held")
+        nested = b"" if self.rate is None else self.rate.to_bytes()
+        meta = json.dumps({"kind": self.kind, "info": {k: v for k, v in self.info.items() if not torch.is_tensor(v)},
+                           "header": len(self.header), "payload": self.payload.numel(),
+                           "held": None if held is None else held.numel(), "rate": len(nested)}).encode()
+        parts = [self._MAGIC, struct.pack("<Q", len(meta)), meta, self.header, self.payload.cpu().numpy().tobytes()]
+        if held is not None:
+            parts.append(held.detach().to("cpu", torch.float32).contiguous().numpy().tobytes())
+        parts.append(nested)
+        return b"".join(parts)
+
+    @classmethod
+    def from_bytes(cls, b):
+        """The state to_bytes wrote, its tensors on the CPU; ValueError for anything else or a truncated string."""
+        b = bytes(b)
+        if b[:8] != cls._MAGIC or len(b) < 16:
+            raise ValueError("not a facodec_b200 session state")
+        (n,) = struct.unpack("<Q", b[8:16])
+        try:
+            meta = json.loads(b[16:16 + n].decode())
+            o = 16 + n
+            hb, pb, nh, nr = int(meta["header"]), int(meta["payload"]), meta["held"], int(meta["rate"])
+        except (ValueError, KeyError, TypeError, UnicodeDecodeError) as exc:
+            raise ValueError("corrupt session state: %s" % exc) from None
+        need = o + hb + pb + (0 if nh is None else 4 * int(nh)) + nr
+        if len(b) != need:
+            raise ValueError("session state of %d bytes, its framing says %d" % (len(b), need))
+        header = b[o:o + hb]
+        o += hb
+        payload = torch.frombuffer(bytearray(b[o:o + pb]), dtype=torch.uint8) if pb else torch.empty(0, dtype=torch.uint8)
+        o += pb
+        info = dict(meta["info"])
+        if nh is not None:
+            info["held"] = torch.frombuffer(bytearray(b[o:o + 4 * nh]), dtype=torch.float32) if nh else torch.empty(0)
+            o += 4 * nh
+        rate = cls.from_bytes(b[o:o + nr]) if nr else None
+        return cls(meta["kind"], header, payload, info, rate)
+
+
 class _StreamPool:
-    """Shared plumbing of the stream pools: session bookkeeping, pointer tables and the pool's lifetime."""
+    """Shared plumbing of the stream pools: session bookkeeping, pointer tables, session export / import and the pool's
+    lifetime."""
 
     _kind = None
+    _rs_quantum = 1           # the quantum of the pool's resampler (sessions at other sample rates)
 
     def _setup(self, engine, pid):
         self.engine, self.pid = engine, pid
@@ -824,6 +901,85 @@ class _StreamPool:
     def _check_device(self, t):
         if t.device.type != "cuda" or (t.device.index if t.device.index is not None else torch.cuda.current_device()) != self.engine.device_index:
             raise _lib.FacError("pool inputs must be on cuda:%d (no CPU fallback); got %s" % (self.engine.device_index, t.device))
+
+    def export(self, sessions):
+        """{session: SessionState} of the named sessions, which stay open and unchanged: export, import_session elsewhere,
+        then close(session) moves a session; importing a state twice forks it.  One launch per state region for all the
+        sessions (the payloads are written on the pool's device, in stream order).  A session that is unknown, closed or
+        finished raises, and nothing is exported."""
+        sessions = self._sessions(sessions)
+        for s in sessions:
+            self._check_export(s)
+        states = self._export_states(sessions)
+        rate = [s for s in sessions if s in self._rate]
+        if rate:
+            got = self._rs._export_states([self._rate[s] for s in rate])
+            for s in rate:
+                states[s].rate = got[self._rate[s]]
+        return states
+
+    def import_session(self, state):
+        """Opens a session holding ``state`` (from export on a pool of the same kind, model and options: any device, handle
+        or process) and returns its id.  From then on it produces, bit for bit, what the exported session would have from
+        the same inputs, and it shares batches with the pool's other sessions.  The payload is moved to the pool's device
+        here.  Raises ValueError or FacError, and changes nothing, for a state of another kind, format version, weights,
+        options, pool n_c or quantum, a corrupt or truncated state, or a full pool."""
+        if self.pid is None:
+            raise _lib.FacError("pool is closed")
+        if not isinstance(state, SessionState):
+            raise ValueError("import_session takes a SessionState, got %s" % type(state).__name__)
+        if state.kind != self._kind:
+            raise ValueError("a %r session state cannot join a %r pool" % (state.kind, self._kind))
+        s = self._import_state(state)
+        if state.rate is not None:
+            try:
+                if self._rs is None:
+                    self._rs = ResamplePool(self.capacity, self._rs_quantum, device=self.device, engine=self.engine)
+                r = self._rs.import_session(state.rate)
+            except Exception:
+                e = self.engine
+                getattr(e.L, "fac_%s_pool_close" % self._kind)(e.handle, self.pid, s)
+                raise
+            self._rate[s] = r
+        self._open.add(s)
+        self._adopt(s, state.info)
+        return s
+
+    def _check_export(self, s):
+        """Raises for a session that cannot be exported (the C call checks the rest)."""
+
+    def _info(self, s):
+        """The Python-side bookkeeping of session s, as a SessionState carries it."""
+        return {}
+
+    def _adopt(self, s, info):
+        """Takes over an imported session's Python-side bookkeeping."""
+
+    def _export_states(self, sessions):
+        """{session: SessionState} from one C export call over this pool's own slots."""
+        e, L, n = self.engine, self.engine.L, len(sessions)
+        hb, pb = ctypes.c_size_t(), ctypes.c_size_t()
+        headers, payloads = [], []
+        for s in sessions:
+            _lib.check(e.handle, getattr(L, "fac_%s_pool_export_size" % self._kind)(e.handle, self.pid, s, ctypes.byref(hb),
+                                                                                      ctypes.byref(pb)), "pool export")
+            headers.append(ctypes.create_string_buffer(hb.value))
+            payloads.append(torch.empty(pb.value, dtype=torch.uint8, device=self.device))
+        rc = getattr(L, "fac_%s_pool_export" % self._kind)(
+            e.handle, self.pid, n, _ptr_array(ctypes.c_int, sessions), _ptr_array(ctypes.c_void_p, [ctypes.addressof(h) for h in headers]),
+            _ptr_array(ctypes.c_void_p, [p.data_ptr() if p.numel() else None for p in payloads]), _stream(self.device))
+        _lib.check(e.handle, rc, "fac_%s_pool_export" % self._kind)
+        return {s: SessionState(self._kind, headers[i].raw, payloads[i], self._info(s)) for i, s in enumerate(sessions)}
+
+    def _import_state(self, state):
+        """One C import of state's header and payload (moved to the pool's device) -> the new session id."""
+        payload = state.payload.to(self.device, torch.uint8).contiguous().view(-1)
+        header = ctypes.create_string_buffer(state.header, len(state.header))
+        e = self.engine
+        rc = getattr(e.L, "fac_%s_pool_import" % self._kind)(e.handle, self.pid, header, len(state.header),
+                                                            _ptr(payload) if payload.numel() else None, payload.numel(),
+                                                            _stream(self.device))
+        return _lib.check(e.handle, rc, "fac_%s_pool_import" % self._kind)
 
     def close(self, session=None):
         """close(s) frees session s's slot; close() frees the pool."""
@@ -870,6 +1026,7 @@ class CodecStreamPool(_StreamPool):
     B = 1 CodecStream fed the same chunks, bit for bit (fac_codes_pool_*).  n_c is fixed for the pool."""
 
     _kind = "codes"
+    _rs_quantum = 300
 
     def __init__(self, model, capacity=256, n_c=2, device=None):
         engine = model.encoder._engine
@@ -902,6 +1059,18 @@ class CodecStreamPool(_StreamPool):
         self._fed.pop(s, None)
         self._held.pop(s, None)
         self._done.discard(s)
+
+    def _check_export(self, s):
+        if s in self._done:
+            raise _lib.FacError("session %d: its utterance was finished by finish_codes" % s)
+
+    def _info(self, s):
+        return {"fed": self._fed[s], "held": self._held[s]} if s in self._held else {"fed": self._fed[s]}
+
+    def _adopt(self, s, info):
+        self._fed[s] = int(info["fed"])
+        if s in self._rate:
+            self._held[s] = info["held"].to(self.device, torch.float32) if "held" in info else self._empty()
 
     def _empty(self):
         return torch.empty(0, device=self.device)
@@ -1196,6 +1365,10 @@ class CodecDecodePool(_StreamPool):
     def _closed(self, s):
         self._finished.discard(s)
 
+    def _check_export(self, s):
+        if s in self._finished:
+            raise _lib.FacError("session %d: its code stream was ended by finish()" % s)
+
     def open(self, timbre, sample_rate=24000):
         """A new session decoding with ``timbre`` [1,1024]; raises FacError when the pool is full.  A session at another
         sample_rate gets its audio resampled from 24 kHz on the device (one launch per step for all such sessions)."""
@@ -1421,6 +1594,17 @@ class ResamplePool(_StreamPool):
     def _closed(self, s):
         self._state.pop(s, None)
         self._prev.pop(s, None)
+
+    def _info(self, s):
+        return dict(zip(("orig", "new", "seen", "emitted"), self._state[s]))
+
+    def _import_state(self, state):
+        _rs_register(self.engine, state.info["orig"], state.info["new"])
+        return super()._import_state(state)
+
+    def _adopt(self, s, info):
+        self._state[s] = [int(info[k]) for k in ("orig", "new", "seen", "emitted")]
+        self._prev.pop(s, None)        # an imported session has no step to take back
 
     def _undo(self, sessions):
         """Takes back each session's last push or finish (fac_rs_pool_undo): for a caller whose own step on the outputs was

@@ -345,6 +345,81 @@ int fac_rs_pool_undo(fac_handle* h, int pool_id, int n, const int* sessions);
 int fac_rs_pool_close(fac_handle* h, int pool_id, int session);
 int fac_rs_pool_destroy(fac_handle* h, int pool_id);
 
+/* Session state: a live pool session taken out of its pool and put into another pool of the same kind, model and options,
+ * on the same device or another one, in this process or another.  After import the session continues bit for bit as it
+ * would have in its source pool, and shares batches with native sessions under the usual plan keys.
+ *
+ * A state is a host header (fac_state_header, native little-endian byte order) and one device payload of
+ * header.payload_bytes, which holds the slot's regions back to back in the order listed below, each region_bytes[r] long
+ * (every size a multiple of 4).  Counters and regions per kind:
+ *   FAC_STATE_CODES  counters {n_c of the pool, mode (0 fresh, 2 coding), samples, frames emitted, sample history length,
+ *                    encoder-LSTM output history length}; regions {sample history [6000] f32, LSTM output history
+ *                    [2][1024] f32, held latent [1024] f32, LSTM carry [2][2 048] words, mel rows [emitted][80] f32}.
+ *                    The mel rows make the payload grow with the call: 320 B per frame, about 1.5 MB after 60 s.
+ *   FAC_STATE_VC     counters {use_p_code, use_c_code, n_c, stale, N, Zf, Yf}; regions {cond [16 384] f32, code history
+ *                    [3][88] i64, z history [24][1024] f32}.
+ *   FAC_STATE_DEC    counters {frames}; regions {latent history [6][1024] f32, LSTM output history [20][1536] f32, LSTM
+ *                    carry [2][2 304] words, gamma | beta [2048] f32}.
+ *   FAC_STATE_RS     counters {quantum, reduced orig, reduced new, width, K, samples seen, outputs emitted, first history
+ *                    sample, history length}; regions {history [history length] f32}.
+ * fingerprint: a 64-bit hash of the host weights of the modules a kind runs (codes: encoder + quantizer; dec: quantizer +
+ * decoder; vc: redecoder + its decoder; rs: 0), taken at fac_finalize: the same state dicts give the same value in any
+ * handle, device or process.  options: the fac_set_option values in the order tensor_cores, fuse_resunit, lstm_v2,
+ * decoder_lstm_fp16, attention_stream, decoder_conv7_fp16, encoder_f16x2, encoder_tt, tc_occ2_maxn, decoder_bf16,
+ * overlap_front.  checksum:
+ * FNV-1a 64 of every header byte before it.
+ * FAC_STATE_VERSION moves with any change to a slot struct (EncHalf, VcStream, DecHalf in engine.cu, RsSlot in resample.cu),
+ * to the regions or to the counters; states of another version are refused.
+ *
+ * fac_*_pool_export_size: host only; the header and payload bytes of one open session.
+ * fac_*_pool_export: writes sessions[i]'s header to headers[i] (host, sizeof(fac_state_header)) and its payload to
+ * payloads[i] (device memory of the handle's device, 4-byte aligned, export_size bytes), in one launch per region for up to
+ * 1024 sessions.  The sessions stay open and unchanged: export, import and close moves a session; export and two imports
+ * fork it.  FAC_ERR_INVALID for an unknown, closed or repeated session or a bad buffer; FAC_ERR_STATE for a session
+ * finished by fac_codes_pool_finish_codes, fac_vc_pool_finish or fac_rs_pool_finish.
+ * fac_*_pool_import: opens a slot holding the state and returns its session id.  Everything is checked before anything is
+ * written, and a rejected import changes neither pool: FAC_ERR_INVALID for a short, corrupt or foreign header (magic,
+ * checksum, kind, sizes that disagree with the counters or the payload) or a payload not on the handle's device;
+ * FAC_ERR_STATE for another format version, other weights, other options, another pool n_c or quantum, a full pool or, for
+ * a resampler state, a rate pair without a registered table.  An imported resampler session has no step to take back
+ * (fac_rs_pool_undo).  Bit equality across devices assumes the same GPU model; the SM count is not checked.
+ * fac_last_launch_count after an export or import counts one launch per region. */
+#define FAC_STATE_MAGIC 0x54534346u     /* "FCST" */
+#define FAC_STATE_VERSION 1
+#define FAC_STATE_OPTIONS 12
+#define FAC_STATE_COUNTERS 12
+#define FAC_STATE_REGIONS 6
+enum { FAC_STATE_CODES = 1, FAC_STATE_VC = 2, FAC_STATE_DEC = 3, FAC_STATE_RS = 4 };
+typedef struct fac_state_header {
+    uint32_t magic, version, kind, header_bytes;
+    uint64_t fingerprint;
+    int64_t options[FAC_STATE_OPTIONS];         /* unused entries 0 */
+    int64_t counters[FAC_STATE_COUNTERS];       /* unused entries 0 */
+    int64_t region_bytes[FAC_STATE_REGIONS];    /* unused entries 0 */
+    uint64_t payload_bytes;
+    uint64_t checksum;
+} fac_state_header;
+int fac_codes_pool_export_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes);
+int fac_codes_pool_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads,
+                          void* stream);
+int fac_codes_pool_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload,
+                          size_t payload_bytes, void* stream);
+int fac_vc_pool_export_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes);
+int fac_vc_pool_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads,
+                       void* stream);
+int fac_vc_pool_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload,
+                       size_t payload_bytes, void* stream);
+int fac_dec_pool_export_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes);
+int fac_dec_pool_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads,
+                        void* stream);
+int fac_dec_pool_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload,
+                        size_t payload_bytes, void* stream);
+int fac_rs_pool_export_size(fac_handle* h, int pool_id, int session, size_t* header_bytes, size_t* payload_bytes);
+int fac_rs_pool_export(fac_handle* h, int pool_id, int n, const int* sessions, void* const* headers, void* const* payloads,
+                       void* stream);
+int fac_rs_pool_import(fac_handle* h, int pool_id, const void* header, size_t header_bytes, const void* payload,
+                       size_t payload_bytes, void* stream);
+
 /* quantize/rvq.py:27-75 ResidualVQ.forward (eval) over quantize/fvq.py FactorizedVectorQuantize,
  * dim=1024, codebook_dim=8, 2^10 entries (BASELINE configs[3]).  Parameters are passed directly
  * (already weight-normed, HOST): per quantizer q: in_w [8,1024], in_b [8], out_w [1024,8],

@@ -98,6 +98,12 @@ int fac_debug_pool_plan(int kind, int n, const long long* counters, const int* l
  * frames, first output frame in the z window, first z row kept after the step, z rows kept, stale (0 when the z history is
  * empty), N, Zf and Yf after the step, code frames the stream keeps}.  Returns 16. */
 int fac_debug_vc_plan(long long N, long long Zf, long long Yf, int F, int finish, int stale, long long* out16);
+/* Host-only: the header checks fac_*_pool_import runs before it touches a pool, for a pool of `kind` (FAC_STATE_*) whose
+ * weights give `fingerprint` and whose handle has options[FAC_STATE_OPTIONS], given payload_bytes of payload: the status
+ * the import would return for the header, and on success the header's counters in counters_out[FAC_STATE_COUNTERS] (may
+ * be NULL).  The pool-side checks (counters, n_c, quantum, capacity, device) are not part of it. */
+int fac_debug_state_header(const void* header, size_t header_bytes, int kind, uint64_t fingerprint, const int64_t* options,
+                           size_t payload_bytes, long long* counters_out);
 /* Host-only: the StyleEncoder batches of fac_codes_pool_timbre over n sessions of frames[i] mel frames: batch[i] = the
  * batch of session i (batches in launch order); returns the number of batches. */
 int fac_debug_timbre_plan(int n, const int* frames, int* batch);
