@@ -118,6 +118,12 @@ def load():
                                     _c.c_float, _c.c_float, _c.c_float, _c.c_float, fp, fp, fp, vp], i32),
         "fac_l1_loss_grad": ([vp, fp, fp, _c.c_longlong, fp, fp, fp, vp], i32),
         "fac_add3": ([vp, fp, fp, fp, _c.c_longlong, fp, vp], i32),
+        "fac_jdc_begin": ([vp], i32),
+        "fac_jdc_tensor": ([vp, i32, _c.c_char_p, fp, _c.POINTER(_c.c_int64), i32], i32),
+        "fac_jdc_finalize": ([vp, i32], i32),
+        "fac_jdc_forward": ([vp, i32, fp, i32, i32, vp, fp, fp, fp, vp], i32),
+        "fac_f0_targets": ([vp, fp, i32, i32, vp, fp, fp, vp], i32),
+        "fac_log_norm": ([vp, fp, i32, i32, fp, vp], i32),
         "fac_reconstruction_loss": ([vp, fp, fp, i32, i32, fp, fp, vp], i32),
         "fac_rvq_forward": ([vp, i32, fp, i32, i32, i32, fp, i64p, fp, vp], i32),
         "fac_alias_free_act": ([vp, fp, i32, i32, i32, i32, fp, fp, fp, vp], i32),
@@ -176,7 +182,7 @@ def load():
 
 EXPORTED = ["fac_abi_version", "fac_create", "fac_destroy", "fac_last_error", "fac_load_tensor", "fac_finalize",
             "fac_encode", "fac_encode_frames", "fac_quantize", "fac_decode", "fac_codec_forward",
-            "fac_codec_forward_host", "fac_codec_encode", "fac_codec_encode_lens", "fac_codec_forward_lens", "fac_codec_timbre_lens", "fac_dequantize", "fac_codes_decode", "fac_codes_decode_lens", "fac_redecode", "fac_redecoder_decode", "fac_voice_convert", "fac_voice_convert_lens", "fac_dataset_mel", "fac_reconstruction_loss", "fac_spectral_loss", "fac_l1_loss", "fac_spectral_loss_grad", "fac_l1_loss_grad", "fac_head_begin", "fac_head_tensor", "fac_head_finalize", "fac_head_forward", "fac_add3", "fac_stream_begin", "fac_stream_encode", "fac_stream_decode", "fac_stream_decode_codes", "fac_stream_encode_codes", "fac_stream_finish_codes", "fac_stream_timbre", "fac_stream_end", "fac_vc_stream_lookahead", "fac_vc_stream_begin", "fac_vc_stream_convert", "fac_vc_stream_finish", "fac_vc_stream_set_timbre", "fac_vc_stream_end", "fac_codes_pool_create", "fac_codes_pool_open", "fac_codes_pool_encode_codes", "fac_codes_pool_finish_codes", "fac_codes_pool_timbre", "fac_codes_pool_close", "fac_codes_pool_destroy", "fac_vc_pool_create", "fac_vc_pool_open", "fac_vc_pool_open_mode", "fac_vc_pool_set_timbre", "fac_vc_pool_convert", "fac_vc_pool_finish", "fac_vc_pool_close", "fac_vc_pool_destroy", "fac_dec_pool_create", "fac_dec_pool_open", "fac_dec_pool_decode_codes", "fac_dec_pool_set_timbre", "fac_dec_pool_close", "fac_dec_pool_destroy", "fac_resample_geometry", "fac_resample_out_len", "fac_resample_ready", "fac_resample_table", "fac_resample", "fac_rs_pool_create", "fac_rs_pool_open", "fac_rs_pool_push", "fac_rs_pool_finish", "fac_rs_pool_undo", "fac_rs_pool_close", "fac_rs_pool_destroy", "fac_codes_pool_export_size", "fac_codes_pool_export", "fac_codes_pool_import", "fac_vc_pool_export_size", "fac_vc_pool_export", "fac_vc_pool_import", "fac_dec_pool_export_size", "fac_dec_pool_export", "fac_dec_pool_import", "fac_rs_pool_export_size", "fac_rs_pool_export", "fac_rs_pool_import", "fac_rvq_create", "fac_rvq_destroy", "fac_rvq_forward", "fac_alias_free_act",
+            "fac_codec_forward_host", "fac_codec_encode", "fac_codec_encode_lens", "fac_codec_forward_lens", "fac_codec_timbre_lens", "fac_dequantize", "fac_codes_decode", "fac_codes_decode_lens", "fac_redecode", "fac_redecoder_decode", "fac_voice_convert", "fac_voice_convert_lens", "fac_dataset_mel", "fac_reconstruction_loss", "fac_spectral_loss", "fac_l1_loss", "fac_spectral_loss_grad", "fac_l1_loss_grad", "fac_head_begin", "fac_head_tensor", "fac_head_finalize", "fac_head_forward", "fac_add3", "fac_jdc_begin", "fac_jdc_tensor", "fac_jdc_finalize", "fac_jdc_forward", "fac_f0_targets", "fac_log_norm", "fac_stream_begin", "fac_stream_encode", "fac_stream_decode", "fac_stream_decode_codes", "fac_stream_encode_codes", "fac_stream_finish_codes", "fac_stream_timbre", "fac_stream_end", "fac_vc_stream_lookahead", "fac_vc_stream_begin", "fac_vc_stream_convert", "fac_vc_stream_finish", "fac_vc_stream_set_timbre", "fac_vc_stream_end", "fac_codes_pool_create", "fac_codes_pool_open", "fac_codes_pool_encode_codes", "fac_codes_pool_finish_codes", "fac_codes_pool_timbre", "fac_codes_pool_close", "fac_codes_pool_destroy", "fac_vc_pool_create", "fac_vc_pool_open", "fac_vc_pool_open_mode", "fac_vc_pool_set_timbre", "fac_vc_pool_convert", "fac_vc_pool_finish", "fac_vc_pool_close", "fac_vc_pool_destroy", "fac_dec_pool_create", "fac_dec_pool_open", "fac_dec_pool_decode_codes", "fac_dec_pool_set_timbre", "fac_dec_pool_close", "fac_dec_pool_destroy", "fac_resample_geometry", "fac_resample_out_len", "fac_resample_ready", "fac_resample_table", "fac_resample", "fac_rs_pool_create", "fac_rs_pool_open", "fac_rs_pool_push", "fac_rs_pool_finish", "fac_rs_pool_undo", "fac_rs_pool_close", "fac_rs_pool_destroy", "fac_codes_pool_export_size", "fac_codes_pool_export", "fac_codes_pool_import", "fac_vc_pool_export_size", "fac_vc_pool_export", "fac_vc_pool_import", "fac_dec_pool_export_size", "fac_dec_pool_export", "fac_dec_pool_import", "fac_rs_pool_export_size", "fac_rs_pool_export", "fac_rs_pool_import", "fac_rvq_create", "fac_rvq_destroy", "fac_rvq_forward", "fac_alias_free_act",
             "fac_debug_conv", "fac_debug_conv_tc", "fac_debug_conv_tc_group1", "fac_debug_resunit", "fac_debug_conv_lanes", "fac_debug_resunit_lanes", "fac_debug_tc_phase_clocks", "fac_debug_tc_producer_clocks", "fac_debug_tc_trace", "fac_debug_lstm_pack", "fac_debug_pool_plan", "fac_debug_timbre_plan", "fac_debug_vc_plan", "fac_debug_state_header", "fac_debug_lstm_lane_map", "fac_debug_convtr_pack", "fac_debug_pad_map", "fac_debug_lane_pad_map", "fac_debug_tc_plan", "fac_debug_tc_plan_group", "fac_debug_tc_pack", "fac_debug_lstm_phase_clocks", "fac_set_option", "fac_debug_slstm", "fac_debug_slstm_lanes", "fac_debug_fa_quantize", "fac_debug_attention", "fac_debug_tap", "fac_profile_enable", "fac_profile_reset", "fac_profile_get", "fac_profile_dump",
             "fac_workspace_bytes", "fac_last_launch_count"]
 

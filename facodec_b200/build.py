@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_C")
 LIB = os.path.join(OUT_DIR, "libfacodec_b200.so")
-SOURCES = ["engine.cu", "conv_simt.cu", "conv_tc.cu", "lstm.cu", "lstm2.cu", "frontend.cu", "quant.cu", "altfree.cu", "pool.cu", "resample.cu"]
+SOURCES = ["engine.cu", "conv_simt.cu", "conv_tc.cu", "lstm.cu", "lstm2.cu", "frontend.cu", "quant.cu", "altfree.cu", "pool.cu", "resample.cu", "jdc.cu"]
 HEADERS = ["common.cuh", "kernels.h", "conv_tc_common.cuh", "resample.h", os.path.join("..", "..", "include", "facodec_b200.h"),
            os.path.join("..", "..", "include", "facodec_b200_debug.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",

@@ -125,7 +125,7 @@ __device__ __forceinline__ float mish_f(float x) {
     return x * tanhf(sp);
 }
 
-enum OutAct { ACT_NONE = 0, ACT_TANH = 1, ACT_MISH = 2, ACT_SNAKE = 3 };
+enum OutAct { ACT_NONE = 0, ACT_TANH = 1, ACT_MISH = 2, ACT_SNAKE = 3, ACT_LRELU = 4 };
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -135,10 +135,15 @@ __device__ __forceinline__ float act_out(int act, float v, float al, float ia) {
 template <int P1, int P2, bool TT>
 constexpr bool groupable() { return P1 != P_F16S && P2 == P_NONE && !TT; }
 
-template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false>
-__global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128 ? 2 : MINB) conv_tc_kernel(TcConvParams p) {
+// C2D: the 3x3 Conv2d of conv2d_tc_kernel over a channels-last [T][row2d][C] map, row2d = F + 2 (two zero frequency
+// columns).  Flattened to rows, tap (dt, df) is the row offset dt * row2d + df from PLr = row2d + 1 rows back, so the
+// operand holds BM + 2 row2d + 2 rows and each tap is again a descriptor start-address offset; the epilogue applies
+// LeakyReLU(0.01) and writes the output's pad columns as zeros, so the output is the next layer's input layout.
+template <int P1, int P2, bool PROMO, int NI, int MINB, bool TT, bool C2D>
+__device__ __forceinline__ void conv_tc_body(const TcConvParams& p) {
     constexpr bool FUSED = P2 != P_NONE;
-    constexpr bool GROUPABLE = groupable<P1, P2, TT>();
+    constexpr bool GROUPABLE = groupable<P1, P2, TT>() && !C2D;
+    static_assert(!C2D || (P1 == P_F16X2 && PROMO && !FUSED && !TT), "2-D taps: the promoted fp16 hi + scaled-lo class only");
     static_assert(!TT || (NI == 64 && !FUSED), "transposed tiles: <= 64 channels x 64 time steps per warpgroup");
     static_assert(NI % 16 == 0 && NI <= (PROMO || MINB == 2 ? 64 : (P1 == P_F16S ? 256 : 128)),
                   "accumulator registers: <= 64 / 128 columns (256 in the one-pass fp16 class at one CTA per SM)");
@@ -160,7 +165,7 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
     const int t0 = blockIdx.x * BM, ntile = blockIdx.y, b = blockIdx.z;
     const int Kr = p.Kr, dil = p.dil, Rpad = p.Rpad, nchunk = p.nchunk, S = p.stagesB;
     const int G = GROUPABLE ? p.group : 1;                   // chunks per GEMM-1 step: 1, 2 or 4
-    const int R = BM + (Kr - 1) * dil;
+    const int R = BM + (C2D ? 2 * p.row2d + 2 : (Kr - 1) * dil);
     const int nstep1 = G == 4 ? nchunk >> 2 : (G == 2 ? nchunk >> 1 : nchunk);     // GEMM-1 steps
     const uint32_t a_plane = (uint32_t)G * T1::KG * Rpad * 16, a_bytes = a_plane * T1::planes;
     uint8_t* abuf = smem + kSmemHdr;
@@ -289,7 +294,8 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
             } else {
 #pragma unroll 1
                 for (int tap = 0; tap < Kr; ++tap)
-                    mma_tap(a0 + (uint32_t)(tap * dil) * 16, b0 + (uint32_t)tap * T1::planes * T1::KG * b_lbo);
+                    mma_tap(a0 + (uint32_t)(C2D ? (tap / 3) * p.row2d + tap % 3 : tap * dil) * 16,
+                            b0 + (uint32_t)tap * T1::planes * T1::KG * b_lbo);
             }
             wg_commit();
             if (u + 1 < nstep1) produce(u + 1);         // overlaps the MMAs in flight
@@ -385,6 +391,16 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
     for_each_pair<NI>(tl, acc, [&](int row, int col, float v0, float v1) {
         const int t = t0 + row;
         if (t >= p.Tout) return;
+        if constexpr (C2D) {
+            const float2 bi = __ldg(reinterpret_cast<const float2*>(bi_p + col));
+            v0 += bi.x; v1 += bi.y;
+            if (act == ACT_LRELU) { v0 = v0 >= 0.f ? v0 : 0.01f * v0; v1 = v1 >= 0.f ? v1 : 0.01f * v1; }
+            if (rb) { const float2 r = *reinterpret_cast<const float2*>(rb + (size_t)t * p.ldy + col); v0 += r.x; v1 += r.y; }
+            const int f = t % p.row2d;
+            if (f == 0 || f == p.row2d - 1) { v0 = 0.f; v1 = 0.f; }
+            *reinterpret_cast<float2*>(yb + (size_t)t * p.ldy + col) = make_float2(v0, v1);
+            return;
+        }
         if (bi_p) { const float2 bi = __ldg(reinterpret_cast<const float2*>(bi_p + col)); v0 += bi.x; v1 += bi.y; }
         if (act == ACT_SNAKE) {
             const float2 al = __ldg(reinterpret_cast<const float2*>(al_p + col));
@@ -398,6 +414,17 @@ __global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128
         if (rb) { const float2 r = *reinterpret_cast<const float2*>(rb + (size_t)t * p.ldy + col); v0 += r.x; v1 += r.y; }
         *reinterpret_cast<float2*>(yb + (size_t)t * p.ldy + col) = make_float2(v0, v1);
     });
+}
+
+template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false>
+__global__ void __launch_bounds__(kThreads, groupable<P1, P2, TT>() && NI <= 128 ? 2 : MINB) conv_tc_kernel(TcConvParams p) {
+    conv_tc_body<P1, P2, PROMO, NI, MINB, TT, false>(p);
+}
+
+// 3x3 Conv2d (JDCNet, jdc.cu) in the promoted fp16 hi + scaled-lo class, two CTAs per SM where the plan fits
+template <int NI>
+__global__ void __launch_bounds__(kThreads, 2) conv2d_tc_kernel(TcConvParams p) {
+    conv_tc_body<P_F16X2, P_NONE, true, NI, 2, false, true>(p);
 }
 
 }  // namespace
@@ -424,6 +451,7 @@ bool tc_conv_plan(TcConvParams& p) {
     if (p.f16x2 && !p.promoted) return false;
     if (p.g1f16 && !p.bf16) return false;
     if (p.tt && !p.f16x2) return false;
+    if (p.row2d && (p.Kr != 9 || p.vf != 1 || !p.f16x2 || p.tt || p.fused || p.row2d < 3)) return false;
     if (p.fused && ((p.promoted && (!p.f16x2 || p.tt)) || p.Cin != p.Cout || p.vf != 1 || p.Cout > 256)) return false;
     const int P1 = plan_prec(p), P2 = p.fused ? (p.f16x2 ? P_F16X2 : (p.bf16 ? P_BF16 : P_TF32)) : P_NONE;
     p.nchunk = p.Cin * p.vf / kChunk;
@@ -467,7 +495,7 @@ bool tc_conv_plan(TcConvParams& p) {
         // 4/G in the 16-bit classes at G > 1.  G = 1 keeps Rpad % 8 == 2, right for TF32 (v = 2) and a 2-way conflict
         // in the 16-bit classes (v = 4), as the one-chunk plans have always been laid out.
         const int v = G == 1 ? 2 : (P1 == P_TF32 ? 1 : 4 / G);
-        l.Rpad = BM + (p.Kr - 1) * p.dil;
+        l.Rpad = BM + (p.row2d ? 2 * p.row2d + 2 : (p.Kr - 1) * p.dil);
         while (l.Rpad % 8 != v) ++l.Rpad;
         const size_t a_bytes = (size_t)G * prec_planes(P1) * prec_kg(P1) * l.Rpad * 16;
         l.slot = (size_t)G * p.Kr * prec_planes(P1) * prec_kg(P1) * N * 16;
@@ -626,8 +654,12 @@ void tc_pack_blob(const TcConvParams& p, const float* wp, int ldw, float* blob) 
 }
 
 namespace {
-template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false>
+template <int P1, int P2, bool PROMO, int NI, int MINB = 1, bool TT = false, bool C2D = false>
 cudaError_t launch_one(const TcConvParams& p, dim3 grid, cudaStream_t st) {
+    auto* kern = [] {
+        if constexpr (C2D) return conv2d_tc_kernel<NI>;
+        else return conv_tc_kernel<P1, P2, PROMO, NI, MINB, TT>;
+    }();
     // the > 48 KB dynamic shared-memory opt-in is per device and per kernel
     static bool done[64] = {};
     static std::mutex mu;
@@ -638,24 +670,23 @@ cudaError_t launch_one(const TcConvParams& p, dim3 grid, cudaStream_t st) {
     {
         std::lock_guard<std::mutex> lk(mu);
         if (!done[dev]) {
-            e = cudaFuncSetAttribute(conv_tc_kernel<P1, P2, PROMO, NI, MINB, TT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)kSmemCap);
+            e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap);
             if (e != cudaSuccess) return e;
             done[dev] = true;
         }
     }
-    conv_tc_kernel<P1, P2, PROMO, NI, MINB, TT><<<grid, kThreads, p.smem_bytes, st>>>(p);
+    kern<<<grid, kThreads, p.smem_bytes, st>>>(p);
     return cudaGetLastError();
 }
 // The kernel's wgmma N is the warpgroup's whole channel width NW, so there is one instantiation per width tc_conv_plan
 // can return for the class: 16, 32, ..., 128, or up to 64 when promoted or planned for two CTAs per SM, plus
 // f16s_wide_nw in the one-pass fp16 class.  The promoted class (TT aside) has only the MINB = 2
 // instantiations, whatever residency its plan allows.
-template <int P1, int P2, bool PROMO, int MINB = 1, int NI = (PROMO || MINB == 2 ? 64 : 128)>
+template <int P1, int P2, bool PROMO, int MINB = 1, int NI = (PROMO || MINB == 2 ? 64 : 128), bool C2D = false>
 cudaError_t launch_nw(const TcConvParams& p, dim3 grid, cudaStream_t st) {
     const int NW = p.MT == 2 ? p.N : p.N / 2;
-    if (NW == NI) return launch_one<P1, P2, PROMO, NI, MINB>(p, grid, st);
-    if constexpr (NI > 16) return launch_nw<P1, P2, PROMO, MINB, NI - 16>(p, grid, st);
+    if (NW == NI) return launch_one<P1, P2, PROMO, NI, MINB, false, C2D>(p, grid, st);
+    if constexpr (NI > 16) return launch_nw<P1, P2, PROMO, MINB, NI - 16, C2D>(p, grid, st);
     else return cudaErrorInvalidValue;
 }
 template <int P1, int P2>
@@ -675,6 +706,10 @@ cudaError_t launch_conv_tc(const TcConvParams& p, cudaStream_t st) {
     dim3 grid((p.Tout + BM - 1) / BM, p.Cout / p.N, p.B);
     if (grid.y > 65535 || grid.z > 65535) return cudaErrorInvalidValue;
     const int P1 = plan_prec(p);
+    if (p.row2d) {
+        if (P1 != P_F16X2 || !p.promoted || p.fused || p.tt || p.Kr != 9) return cudaErrorInvalidValue;
+        return launch_nw<P_F16X2, P_NONE, true, 2, 64, true>(p, grid, st);
+    }
     if (p.fused) {
         if (P1 == P_F16X2)
             return (p.MT == 2 ? p.N : p.N / 2) == 64 ? launch_one<P_F16X2, P_F16X2, true, 64, 2>(p, grid, st) : cudaErrorInvalidValue;

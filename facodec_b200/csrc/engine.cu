@@ -171,6 +171,8 @@ struct fac_handle {
     fac::RsHost* rs = nullptr;      // resampler filter tables and session pools (fac_resample*, fac_rs_pool_*), made on use
     struct HeadSet;                 // modules/quantize.py:106-125 CNNLSTM instances (fac_head_*)
     std::vector<HeadSet*> heads;
+    struct JdcSet;                  // modules/JDC/model.py JDCNet instances, eval mode (fac_jdc_*)
+    std::vector<JdcSet*> jdcs;
     char* ws = nullptr; size_t ws_bytes = 0;
     int launches = 0;
     // tensor-core path (fac_set_option "tensor_cores"): 0 = never, 1 = layers downstream of the VQ only
@@ -219,6 +221,23 @@ struct fac_handle::HeadSet {
     struct Unit { size_t a1, b1, a2, b2; ConvW c7, c1; int dil; } unit[3];
     size_t af, bf;                  // final activation exp(alpha), exp(beta)
     ConvW lin[8];
+    std::map<std::string, HostTensor> staged;
+    float* arena = nullptr;
+    bool ready = false;
+};
+
+// One JDCNet(num_class=1) in eval mode (modules/JDC/model.py:102-137).  Every 3x3 conv that a BatchNorm follows carries it
+// folded into its weights and bias; the BatchNorms before a max-pool are per-channel scale / shift pairs.
+struct fac_handle::JdcSet {
+    struct Bn { size_t sc = 0, sh = 0; };
+    size_t conv_in_w = 0, conv_in_b = 0;       // conv_block.0 + .1: [9][64], [64]
+    ConvW c0b;                                 // conv_block.3 (64 -> 64, no BN after it)
+    struct Block { Bn pre; ConvW c1, c2, c11; int F = 0; } blk[3];    // res_block1..3: F = input frequency columns
+    Bn pool;                                   // pool_block.0
+    ConvW ih[2];                               // bilstm_classifier input GEMMs (forward, reverse): 512 -> 1024
+    size_t whh2[2] = {0, 0};                   // their recurrent weights, lstm2_pack(pass3 = 1)
+    int U = 0, G = 0;
+    size_t cls_w = 0, cls_b = 0;               // classifier: [512], [1]
     std::map<std::string, HostTensor> staged;
     float* arena = nullptr;
     bool ready = false;
@@ -1592,6 +1611,7 @@ int fac_destroy(fac_handle* h) {
     if (h->spec_arena) cudaFree(h->spec_arena);
     for (float* p : h->rvq_arenas) if (p) cudaFree(p);
     for (auto* hs : h->heads) { if (hs->arena) cudaFree(hs->arena); delete hs; }
+    for (auto* js : h->jdcs) { if (js->arena) cudaFree(js->arena); delete js; }
     fac::rs_host_free(h->rs);
     delete h;   // and with it the streams' and pools' device state
     return FAC_OK;
@@ -4289,6 +4309,308 @@ int fac_head_forward(fac_handle* h, int head_id, const float* x, int B, int T, f
     });
     h->warena = saved;
     return rc;
+}
+
+// ---- JDCNet pitch extractor (modules/JDC/model.py, eval mode) ----
+int fac_jdc_begin(fac_handle* h) {
+    if (!h) return FAC_ERR_INVALID;
+    h->jdcs.push_back(new fac_handle::JdcSet());
+    return (int)h->jdcs.size() - 1;
+}
+
+int fac_jdc_tensor(fac_handle* h, int jdc_id, const char* key, const float* data_host, const int64_t* shape, int ndim) {
+    if (!h || jdc_id < 0 || jdc_id >= (int)h->jdcs.size() || !key || !data_host || ndim < 0 || ndim > 4) return FAC_ERR_INVALID;
+    HostTensor t;
+    size_t n = 1;
+    for (int i = 0; i < ndim; ++i) { if (shape[i] < 0) return FAC_ERR_INVALID; t.shape.push_back(shape[i]); n *= (size_t)shape[i]; }
+    t.data.assign(data_host, data_host + n);
+    h->jdcs[jdc_id]->staged[key] = std::move(t);
+    h->jdcs[jdc_id]->ready = false;
+    return FAC_OK;
+}
+
+namespace {
+// BatchNorm2d (eval) at `prefix` as y = x * sc + sh, in fp64 then rounded
+void jdc_bn(fac_handle* tmp, const std::string& prefix, int C, std::vector<double>& sc, std::vector<double>& sh) {
+    const HostTensor& g = need(tmp, 0, prefix + ".weight");
+    const HostTensor& b = need(tmp, 0, prefix + ".bias");
+    const HostTensor& m = need(tmp, 0, prefix + ".running_mean");
+    const HostTensor& v = need(tmp, 0, prefix + ".running_var");
+    if ((int)g.numel() != C || (int)b.numel() != C || (int)m.numel() != C || (int)v.numel() != C) throw PackError{"BatchNorm shape at " + prefix};
+    sc.resize(C); sh.resize(C);
+    for (int c = 0; c < C; ++c) {
+        sc[c] = (double)g.data[c] / std::sqrt((double)v.data[c] + 1e-5);
+        sh[c] = (double)b.data[c] - (double)m.data[c] * sc[c];
+    }
+}
+fac_handle::JdcSet::Bn jdc_pack_bn(fac_handle* tmp, const std::string& prefix, int C) {
+    std::vector<double> sc, sh;
+    jdc_bn(tmp, prefix, C, sc, sh);
+    fac_handle::JdcSet::Bn r;
+    r.sc = pack_alloc(tmp, C); r.sh = pack_alloc(tmp, C);
+    for (int c = 0; c < C; ++c) { tmp->pack[r.sc + c] = (float)sc[c]; tmp->pack[r.sh + c] = (float)sh[c]; }
+    return r;
+}
+// nn.Conv2d(Cin, Cout, k, bias=False) at `prefix` (k = 3: 9 row-offset taps tap = kh * 3 + kw; k = 1: one tap), with the
+// BatchNorm at `bn` (or none) folded in, packed [taps * Cin][ldw] with its promoted fp16 hi + scaled-lo blob (conv_tc.cu)
+ConvW jdc_pack_conv(fac_handle* tmp, const std::string& prefix, int Cin, int Cout, int k, const char* bn) {
+    const HostTensor& w = need(tmp, 0, prefix + ".weight");
+    if (w.shape.size() != 4 || w.shape[0] != Cout || w.shape[1] != Cin || w.shape[2] != k || w.shape[3] != k)
+        throw PackError{"Conv2d shape at " + prefix};
+    std::vector<double> sc(Cout, 1.0), sh(Cout, 0.0);
+    if (bn) jdc_bn(tmp, bn, Cout, sc, sh);
+    ConvW c;
+    c.Cin = Cin; c.Cout = Cout; c.K = k * k; c.ldw = (Cout + 3) / 4 * 4;
+    c.w = pack_alloc(tmp, (size_t)c.K * Cin * c.ldw);
+    for (int co = 0; co < Cout; ++co)
+        for (int ci = 0; ci < Cin; ++ci)
+            for (int tap = 0; tap < c.K; ++tap)
+                tmp->pack[c.w + ((size_t)tap * Cin + ci) * c.ldw + co] = (float)(w.data[((size_t)co * Cin + ci) * c.K + tap] * sc[co]);
+    c.b = pack_alloc(tmp, Cout);
+    for (int co = 0; co < Cout; ++co) tmp->pack[c.b + co] = (float)sh[co];
+    TcConvParams tp;
+    tp.Cin = Cin; tp.Cout = Cout; tp.Kr = c.K; tp.vf = 1; tp.dil = 1; tp.promoted = 1; tp.f16x2 = 1; tp.row2d = k == 3 ? 82 : 0;
+    if (!tc_conv_plan(tp)) throw PackError{"no tensor-core plan for " + prefix};
+    c.Kr = c.K; c.promoted = true; c.tcN = tp.N; c.tc = true; c.has16 = true;
+    c.tcw16 = pack_alloc(tmp, tc_blob_floats(tp));
+    tc_pack_blob(tp, tmp->pack.data() + c.w, c.ldw, tmp->pack.data() + c.tcw16);
+    return c;
+}
+
+// 3x3 conv over [B][T][F + 2][Cin] maps (conv2d_tc_kernel): rows = frames x (F + 2), per-lane rows in rows_len
+void jdc_conv3(Ctx& c, const ConvW& w, const float* x, float* y, int B, int T, int F, const int* rows_len, int act,
+               const float* res, const char* name) {
+    if (c.dry) return;
+    TcConvParams tp;
+    tp.Cin = w.Cin; tp.Cout = w.Cout; tp.vf = 1; tp.Kr = 9; tp.dil = 1; tp.promoted = 1; tp.f16x2 = 1; tp.row2d = F + 2;
+    const int rows = T * (F + 2);
+    tp.Tout = rows;
+    if (!tc_conv_plan(tp) || tp.N != w.tcN) { c.check(cudaErrorInvalidValue, name); return; }
+    tp.x = x; tp.y = y; tp.wblob = c.W(w.tcw16); tp.bias = c.W(w.b); tp.res = res; tp.out_act = act;
+    tp.B = B; tp.Tin = rows; tp.ldx = w.Cin; tp.PLr = F + 3; tp.pad_left_s = F + 3; tp.pad_right_s = F + 3; tp.reflect = 0;
+    tp.lane_len = rows_len; tp.ldy = w.Cout;
+    tp.x_bstride = (size_t)rows * w.Cin; tp.y_bstride = (size_t)rows * w.Cout;
+    char det[96];
+    snprintf(det, sizeof det, "%s Cin%d Cout%d F%d T%d", name, w.Cin, w.Cout, F, T);
+    c.begin("conv2d_tc", 2.0 * B * T * F * 9.0 * w.Cin * w.Cout, 4.0 * ((double)B * rows * (w.Cin + w.Cout) + 9.0 * w.Cin * w.Cout), det);
+    c.check(launch_conv_tc(tp, c.st), name);
+    c.end();
+}
+}  // namespace
+
+int fac_jdc_finalize(fac_handle* h, int jdc_id) {
+    if (!h || jdc_id < 0 || jdc_id >= (int)h->jdcs.size()) return FAC_ERR_INVALID;
+    fac_handle::JdcSet& js = *h->jdcs[jdc_id];
+    fac_handle tmp;
+    tmp.device = h->device;
+    tmp.host[0] = js.staged;
+    try {
+        {   // conv_block.0 (1 -> 64) with conv_block.1 folded: SIMT, [9][64]
+            const HostTensor& w = need(&tmp, 0, "conv_block.0.weight");
+            if (w.shape.size() != 4 || w.shape[0] != 64 || w.shape[1] != 1 || w.shape[2] != 3 || w.shape[3] != 3)
+                throw PackError{"Conv2d shape at conv_block.0"};
+            std::vector<double> sc, sh;
+            jdc_bn(&tmp, "conv_block.1", 64, sc, sh);
+            js.conv_in_w = pack_alloc(&tmp, 9 * 64);
+            js.conv_in_b = pack_alloc(&tmp, 64);
+            for (int co = 0; co < 64; ++co) {
+                for (int k = 0; k < 9; ++k) tmp.pack[js.conv_in_w + k * 64 + co] = (float)(w.data[co * 9 + k] * sc[co]);
+                tmp.pack[js.conv_in_b + co] = (float)sh[co];
+            }
+        }
+        js.c0b = jdc_pack_conv(&tmp, "conv_block.3", 64, 64, 3, nullptr);
+        const int cin[3] = {64, 128, 192}, cout[3] = {128, 192, 256}, F[3] = {80, 40, 20};
+        for (int i = 0; i < 3; ++i) {
+            const std::string p = "res_block" + std::to_string(i + 1);
+            auto& b = js.blk[i];
+            b.F = F[i];
+            b.pre = jdc_pack_bn(&tmp, p + ".pre_conv.0", cin[i]);
+            b.c1 = jdc_pack_conv(&tmp, p + ".conv.0", cin[i], cout[i], 3, (p + ".conv.1").c_str());
+            b.c2 = jdc_pack_conv(&tmp, p + ".conv.3", cout[i], cout[i], 3, nullptr);
+            b.c11 = jdc_pack_conv(&tmp, p + ".conv1by1", cin[i], cout[i], 1, nullptr);
+        }
+        js.pool = jdc_pack_bn(&tmp, "pool_block.0", 256);
+        const int H = 256;
+        js.U = lstm_units_per_cta(H);
+        js.G = H / js.U;
+        for (int d = 0; d < 2; ++d) {
+            const std::string sfx = d ? "_l0_reverse" : "_l0";
+            const HostTensor& wih = need(&tmp, 0, "bilstm_classifier.weight_ih" + sfx);
+            const HostTensor& whh = need(&tmp, 0, "bilstm_classifier.weight_hh" + sfx);
+            const HostTensor& bih = need(&tmp, 0, "bilstm_classifier.bias_ih" + sfx);
+            const HostTensor& bhh = need(&tmp, 0, "bilstm_classifier.bias_hh" + sfx);
+            if (wih.numel() != (size_t)4 * H * 512 || whh.numel() != (size_t)4 * H * H || bih.numel() != 4 * H || bhh.numel() != 4 * H)
+                throw PackError{"bilstm_classifier shape"};
+            ConvW c;
+            c.Cin = 512; c.Cout = 4 * H; c.K = 1; c.ldw = 4 * H;
+            c.w = pack_alloc(&tmp, (size_t)512 * c.ldw);
+            for (int row = 0; row < 4 * H; ++row)
+                for (int k = 0; k < 512; ++k) tmp.pack[c.w + (size_t)k * c.ldw + row] = wih.data[(size_t)row * 512 + k];
+            c.b = pack_alloc(&tmp, 4 * H);
+            for (int row = 0; row < 4 * H; ++row) tmp.pack[c.b + row] = bih.data[row] + bhh.data[row];
+            attach_tc(&tmp, c, 1, true);
+            if (!c.tc || !c.has16) throw PackError{"no tensor-core plan for the BiLSTM input GEMM"};
+            js.ih[d] = c;
+            js.whh2[d] = pack_alloc(&tmp, lstm2_pack_words(H, js.U, 1));
+            lstm2_pack(whh.data.data(), H, js.U, 1, reinterpret_cast<uint32_t*>(tmp.pack.data() + js.whh2[d]));
+        }
+        const HostTensor& cw = need(&tmp, 0, "classifier.weight");
+        const HostTensor& cb = need(&tmp, 0, "classifier.bias");
+        if (cw.numel() != 512 || cb.numel() != 1) throw PackError{"classifier shape (num_class must be 1)"};
+        js.cls_w = pack_alloc(&tmp, 512);
+        for (int k = 0; k < 512; ++k) tmp.pack[js.cls_w + k] = cw.data[k];
+        js.cls_b = pack_alloc(&tmp, 1);
+        tmp.pack[js.cls_b] = cb.data[0];
+    } catch (const PackError& e) {
+        h->err = e.msg;
+        return FAC_ERR_STATE;
+    }
+    cudaSetDevice(h->device);
+    if (js.arena) { cudaDeviceSynchronize(); cudaFree(js.arena); js.arena = nullptr; }
+    cudaError_t e = cudaMalloc(&js.arena, (tmp.pack.size() + 64) * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemcpy(js.arena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); js.arena = nullptr; return FAC_ERR_CUDA; }
+    js.staged.clear();
+    js.ready = true;
+    return FAC_OK;
+}
+
+int fac_jdc_forward(fac_handle* h, int jdc_id, const float* mel, int B, int T, const int* lengths, float* f0, float* gan_feature,
+                    float* pool_out, void* stream) {
+    if (!h || jdc_id < 0 || jdc_id >= (int)h->jdcs.size() || !mel || !f0 || !gan_feature || !pool_out || B <= 0 || T <= 0)
+        return FAC_ERR_INVALID;
+    fac_handle::JdcSet& js = *h->jdcs[jdc_id];
+    if (!js.ready) { h->err = "fac_jdc_forward: JDCNet not finalized"; return FAC_ERR_STATE; }
+    std::vector<int> lens(B, T);
+    if (lengths)
+        for (int b = 0; b < B; ++b) {
+            if (lengths[b] < 1 || lengths[b] > T) { h->err = "fac_jdc_forward: lengths must be in [1, T]"; return FAC_ERR_INVALID; }
+            lens[b] = lengths[b];
+        }
+    if (B > 65535) { h->err = "fac_jdc_forward: B > 65535"; return FAC_ERR_UNSUPPORTED; }
+    float* saved = h->warena;
+    h->warena = js.arena;
+    const int H = 256;
+    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        // per-lane frames, then rows of each map width (F + 2 = 82, 42, 22, 12)
+        int* dl = lengths ? c.alloc<int>((size_t)5 * B) : nullptr;
+        const int Fs[4] = {80, 40, 20, 10};
+        if (!c.dry && lengths) {
+            std::vector<int> hl((size_t)5 * B);
+            for (int b = 0; b < B; ++b) {
+                hl[b] = lens[b];
+                for (int i = 0; i < 4; ++i) hl[(size_t)(i + 1) * B + b] = lens[b] * (Fs[i] + 2);
+            }
+            // ordered before the launches that read it on the same stream; a copy from pageable memory has taken the
+            // host data by the time it returns, so hl may go out of scope without a synchronize
+            c.check_nk(cudaMemcpyAsync(dl, hl.data(), hl.size() * sizeof(int), cudaMemcpyHostToDevice, c.st), "jdc.lens");
+        }
+        const int* len_d = lengths ? dl : nullptr;
+        auto rows_of = [&](int i) { return lengths ? dl + (size_t)(i + 1) * B : nullptr; };
+        const size_t big = (size_t)B * T * 42 * 128;      // the largest map: [B][T][42][128] (> [82][64], [22][192], [12][256])
+        float* m0 = c.alloc<float>(big);
+        float* m1 = c.alloc<float>(big);
+        float* m2 = c.alloc<float>(big);
+        float* m3 = c.alloc<float>(big);
+        float* lstm_in = c.alloc<float>((size_t)B * T * 512);
+        float* xg = c.alloc<float>((size_t)B * T * 4 * H);
+        float* yd[2] = {c.alloc<float>((size_t)B * T * H), c.alloc<float>((size_t)B * T * H)};
+        uint32_t* h16 = c.alloc<uint32_t>((size_t)2 * 2 * (H / 2) * 32);
+        unsigned int* bar = c.alloc<unsigned int>(64);
+        if (!c.dry) c.check(launch_jdc_conv_in(mel, c.W(js.conv_in_w), c.W(js.conv_in_b), m0, B, T, len_d, c.st), "jdc.conv_in");
+        c.tap("jdc.conv_in", m0, (size_t)B * T * 82 * 64);
+        jdc_conv3(c, js.c0b, m0, m1, B, T, 80, rows_of(0), ACT_NONE, nullptr, "jdc.conv_block");
+        c.tap("jdc.conv_block", m1, (size_t)B * T * 82 * 64);
+        float* cur = m1;
+        int Cc = 64;
+        for (int i = 0; i < 3; ++i) {
+            const auto& bk = js.blk[i];
+            const int Fo = bk.F / 2;
+            float* xin = cur == m1 ? m0 : m1;         // pre_conv output
+            float* hmid = m2;
+            float* r11 = m3;
+            float* out = cur;                         // cur is dead once pre_conv has read it
+            if (!c.dry) c.check(launch_jdc_pre_pool(cur, c.W(bk.pre.sc), c.W(bk.pre.sh), xin, B, T, bk.F, Cc, c.st), "jdc.pre_conv");
+            const std::string si = std::to_string(i + 1);
+            c.tap(("jdc.res" + si + ".pre").c_str(), xin, (size_t)B * T * (Fo + 2) * Cc);
+            // conv1by1 as a 1-tap row GEMM over the same map: its rows at the pad columns are zeroed by conv2's epilogue
+            if (!c.dry) {
+                TcConvParams tp;
+                tp.Cin = Cc; tp.Cout = bk.c11.Cout; tp.vf = 1; tp.Kr = 1; tp.dil = 1; tp.promoted = 1; tp.f16x2 = 1;
+                const int rows = T * (Fo + 2);
+                tp.Tout = rows;
+                if (!tc_conv_plan(tp) || tp.N != bk.c11.tcN) c.check(cudaErrorInvalidValue, "jdc.conv1by1");
+                else {
+                    tp.x = xin; tp.y = r11; tp.wblob = c.W(bk.c11.tcw16); tp.bias = c.W(bk.c11.b);
+                    tp.B = B; tp.Tin = rows; tp.ldx = Cc; tp.lane_len = rows_of(i + 1); tp.ldy = bk.c11.Cout;
+                    tp.x_bstride = (size_t)rows * Cc; tp.y_bstride = (size_t)rows * bk.c11.Cout;
+                    c.begin("conv_tcp", 2.0 * B * rows * Cc * bk.c11.Cout, 4.0 * ((double)B * rows * (Cc + bk.c11.Cout)), "jdc.conv1by1");
+                    c.check(launch_conv_tc(tp, c.st), "jdc.conv1by1");
+                    c.end();
+                }
+            }
+            jdc_conv3(c, bk.c1, xin, hmid, B, T, Fo, rows_of(i + 1), ACT_LRELU, nullptr, "jdc.conv1");
+            c.tap(("jdc.res" + si + ".conv1").c_str(), hmid, (size_t)B * T * (Fo + 2) * bk.c1.Cout);
+            jdc_conv3(c, bk.c2, hmid, out, B, T, Fo, rows_of(i + 1), ACT_NONE, r11, "jdc.conv2");
+            c.tap(("jdc.res" + si).c_str(), out, (size_t)B * T * (Fo + 2) * bk.c2.Cout);
+            Cc = bk.c2.Cout;
+        }
+        if (!c.dry)
+            c.check(launch_jdc_pool_block(cur, c.W(js.pool.sc), c.W(js.pool.sh), gan_feature, pool_out, lstm_in, B, T, len_d, c.st),
+                    "jdc.pool_block");
+        c.tap("jdc.lstm_in", lstm_in, (size_t)B * T * 512);
+        for (int d = 0; d < 2; ++d) {
+            run_conv(c, js.ih[d], lstm_in, xg, 1, B * T, B * T, ConvOpts(), "jdc.lstm.ih");
+            c.tap(d ? "jdc.lstm.xg_rev" : "jdc.lstm.xg_fwd", xg, (size_t)B * T * 4 * H);
+            if (c.dry) continue;
+            for (int b0 = 0; b0 < B; b0 += 32) {
+                const int nb = B - b0 < 32 ? B - b0 : 32;
+                LstmParams p;
+                p.xg = xg + (size_t)b0 * T * 4 * H;
+                p.whh_p2 = reinterpret_cast<const uint32_t*>(c.W(js.whh2[d]));
+                p.h16 = h16; p.pass3 = 1; p.hT = nullptr; p.bar = bar;
+                p.y = yd[d] + (size_t)b0 * T * H;
+                p.B = nb; p.T = T; p.H = H; p.U = js.U; p.G = js.G;
+                LstmLaneLens ll = {};
+                for (int b = 0; b < nb; ++b) ll.len[b] = lens[b0 + b];
+                c.begin("lstm_rec", 2.0 * nb * T * 4.0 * H * H, 4.0 * ((double)nb * T * 5 * H + 4.0 * H * H));
+                c.check(launch_lstm2_layer(p, c.st, d ? &ll : nullptr, d == 1), d ? "jdc.lstm.rev" : "jdc.lstm.fwd");
+                c.end();
+            }
+        }
+        c.tap("jdc.lstm.fwd", yd[0], (size_t)B * T * H);
+        c.tap("jdc.lstm.rev", yd[1], (size_t)B * T * H);
+        if (!c.dry) c.check(launch_jdc_head(yd[0], yd[1], c.W(js.cls_w), c.W(js.cls_b), f0, B, T, len_d, c.st), "jdc.head");
+    });
+    h->warena = saved;
+    return rc;
+}
+
+int fac_f0_targets(fac_handle* h, const float* f0, int B, int T, const int* lengths, float* targets, float* glob_f0, void* stream) {
+    if (!h || !f0 || !targets || !glob_f0 || B <= 0 || T <= 0) return FAC_ERR_INVALID;
+    std::vector<int> hl;
+    if (lengths) {
+        hl.assign(lengths, lengths + B);
+        for (int b = 0; b < B; ++b)
+            if (hl[b] < 0 || hl[b] > T) { h->err = "fac_f0_targets: lengths must be in [0, T]"; return FAC_ERR_INVALID; }
+    }
+    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        int* dl = lengths ? c.alloc<int>(B) : nullptr;
+        if (c.dry) return;
+        if (dl) {
+            c.check_nk(cudaMemcpyAsync(dl, hl.data(), (size_t)B * sizeof(int), cudaMemcpyHostToDevice, c.st), "f0_targets.lens");
+        }
+        c.check(launch_f0_targets(f0, dl, B, T, targets, glob_f0, c.st), "f0_targets");
+    });
+}
+
+int fac_log_norm(fac_handle* h, const float* mel, int B, int T, float* out, void* stream) {
+    if (!h || !mel || !out || B <= 0 || T <= 0) return FAC_ERR_INVALID;
+    cudaSetDevice(h->device);
+    cudaError_t e = launch_log_norm(mel, B, T, out, (cudaStream_t)stream);
+    if (e != cudaSuccess) { h->err = std::string("CUDA error at log_norm: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
+    h->launches = 1;
+    return FAC_OK;
 }
 
 // out = a + b (+ c): the latent sums FApredictors.forward_v2 feeds its reversal heads (modules/quantize.py:571-586), in the

@@ -66,6 +66,7 @@ struct TcConvParams {
     int R2pad = 0;                     // fused: row pitch (rows) of the resident GEMM-2 operand
     size_t smem_bytes = 0;
     size_t x_bstride = 0, y_bstride = 0;
+    int row2d = 0;                     // > 0: 3x3 Conv2d over [T][row2d][C] maps (Kr = 9, conv2d_tc_kernel); see conv_tc_body
 };
 bool tc_conv_plan(TcConvParams& p);
 size_t tc_blob_floats(const TcConvParams& p);
@@ -98,7 +99,9 @@ struct LstmParams {
 // instantiation of their own.
 struct LstmLaneLens { int len[32]; };
 cudaError_t launch_lstm_layer(const LstmParams& p, cudaStream_t st);
-cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st, const LstmLaneLens* lens = nullptr);   // lstm2.cu
+// reverse = true: the reverse direction of a bidirectional layer, lane b from frame lens->len[b] - 1 down to 0 (pass3, lens
+// required, no stream state); its rows t >= len[b] are finite don't-cares
+cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st, const LstmLaneLens* lens = nullptr, bool reverse = false);
 size_t lstm2_pack_words(int H, int U, int pass3);
 void lstm2_pack(const float* whh, int H, int U, int pass3, uint32_t* out);
 size_t lstm2_smem_bytes(int H, int U, int pass3);
@@ -250,6 +253,18 @@ cudaError_t launch_attention(const float* q, const float* k, const float* v, flo
 cudaError_t launch_mean_pool(const float* x, float* out, int B, int T, int C, const int* valid_len, cudaStream_t st,
                              const int* lane_len = nullptr);
 cudaError_t launch_fill_u32(unsigned int* p, unsigned int v, size_t n, cudaStream_t st);
+
+// JDCNet eval-mode pieces and train.py's targets (jdc.cu); maps are [B][T][F + 2][C] with zero pad columns, lens [B] device
+// frames per lane (null: T each)
+cudaError_t launch_jdc_conv_in(const float* mel /*[B][80][T]*/, const float* w /*[9][64]*/, const float* bias, float* y, int B, int T,
+                               const int* lens, cudaStream_t st);
+cudaError_t launch_jdc_pre_pool(const float* x, const float* sc, const float* sh, float* y, int B, int T, int F, int C, cudaStream_t st);
+cudaError_t launch_jdc_pool_block(const float* x, const float* sc, const float* sh, float* gan, float* pool, float* lstm_in, int B,
+                                  int T, const int* lens, cudaStream_t st);
+cudaError_t launch_jdc_head(const float* yf, const float* yb, const float* w, const float* bias, float* f0, int B, int T,
+                            const int* lens, cudaStream_t st);
+cudaError_t launch_f0_targets(const float* f0, const int* lens, int B, int T, float* out, float* glob, cudaStream_t st);
+cudaError_t launch_log_norm(const float* mel, int B, int T, float* out, cudaStream_t st);
 
 // alias-free activation (alias_free_torch/act.py:24-29): up x2 -> snake-beta/identity -> down x2
 cudaError_t launch_alias_free_act(const float* x, float* y, int B, int C, int T, const float* filt12,

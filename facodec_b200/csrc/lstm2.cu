@@ -58,12 +58,14 @@ __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0
 __host__ __device__ __forceinline__ int lstm2_swz_w(int k2, int R) { return R == 32 ? ((k2 & 3) << 3) : (((k2 >> 1) & 1) << 3); }
 __host__ __device__ __forceinline__ int lstm2_swz_h(int kp) { return (kp & 3) << 3; }
 
-// h exchange buffer: [2 parities][PL planes][H/2 k pairs][32] words; PL = 2 (hi, lo') when PASS3 else 1.  LENS (one-pass
-// class only): the per-lane step counts of LstmLaneLens apply (LstmLenParams); without them the kernel is the one it always
-// was.
+// h exchange buffer: [2 parities][PL planes][H/2 k pairs][32] words; PL = 2 (hi, lo') when PASS3 else 1.  LENS: the per-lane
+// step counts of LstmLaneLens apply (LstmLenParams); without them the kernel is the one it always was.  REV (with LENS): the
+// reverse direction of a bidirectional layer -- step s of lane b reads and writes frame len[b] - 1 - s, so every lane starts
+// at its own last frame.
 struct LstmLenParams : LstmParams { LstmLaneLens lens; };
-template <int U, bool PASS3, bool LENS>
+template <int U, bool PASS3, bool LENS, bool REV = false>
 __global__ void __launch_bounds__(L2_WARPS * 32, 1) lstm_rec2_kernel(std::conditional_t<LENS, LstmLenParams, LstmParams> p) {
+    static_assert(!REV || LENS, "the reverse direction needs the lane lengths");
     constexpr int R = 4 * U;
     constexpr int RP = R + 1;
     constexpr int MT = R / 16, NTL = L2_BT / 8;
@@ -111,10 +113,13 @@ __global__ void __launch_bounds__(L2_WARPS * 32, 1) lstm_rec2_kernel(std::condit
         for (int pi = 0; pi < PAIRS; ++pi) {
             int idx = tid + pi * L2_WARPS * 32;
             int b = idx % L2_BT, u = idx / L2_BT;
-            skv[pi] = (p.skip && idx < L2_BT * U && b < p.B) ? __ldg(p.skip + ((size_t)b * p.T + t) * H + j0 + u) : 0.f;
+            int tx = t;
+            if constexpr (REV) tx = (b < p.B ? p.lens.len[b] : 0) - 1 - t;
+            const bool in = idx < L2_BT * U && b < p.B && tx >= 0;
+            skv[pi] = (p.skip && in) ? __ldg(p.skip + ((size_t)b * p.T + tx) * H + j0 + u) : 0.f;
 #pragma unroll
             for (int g = 0; g < 4; ++g)
-                xgv[pi][g] = (idx < L2_BT * U && b < p.B) ? __ldg(p.xg + ((size_t)b * p.T + t) * (4 * H) + (size_t)g * H + j0 + u) : 0.f;
+                xgv[pi][g] = in ? __ldg(p.xg + ((size_t)b * p.T + tx) * (4 * H) + (size_t)g * H + j0 + u) : 0.f;
         }
         // ---- wait until every CTA has published h_{t-1} ----
         if (t > 0) {
@@ -261,7 +266,9 @@ __global__ void __launch_bounds__(L2_WARPS * 32, 1) lstm_rec2_kernel(std::condit
             hcur[widx * 2 + (k & 1)] = hh;
             if (PASS3) hcur[(plane_words + widx) * 2 + (k & 1)] = __float2half_rn((h - __half2float(hh)) * 2048.0f);
             if (b < p.B) {
-                size_t o = ((size_t)b * p.T + t) * H + j0 + u;
+                int ty = t;
+                if constexpr (REV) ty = p.lens.len[b] - 1 - t;
+                size_t o = ((size_t)b * p.T + ty) * H + j0 + u;
                 p.y[o] = h + skv[pi];
             }
         }
@@ -357,11 +364,11 @@ cudaError_t launch_lstm2_lane_carry(const LaneCarryParams& p, cudaStream_t st) {
     return cudaGetLastError();
 }
 
-template <int U, bool PASS3, bool LENS>
+template <int U, bool PASS3, bool LENS, bool REV = false>
 static cudaError_t launch2_u(const LstmParams& p, const LstmLaneLens* lens, cudaStream_t st) {
     const size_t smem = lstm2_smem_bytes(p.H, U, PASS3 ? 1 : 0);
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
-    cudaError_t e = cudaFuncSetAttribute(lstm_rec2_kernel<U, PASS3, LENS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(lstm_rec2_kernel<U, PASS3, LENS, REV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     e = cudaMemsetAsync(p.bar, 0, sizeof(unsigned int), st);
     if (e != cudaSuccess) return e;
@@ -376,16 +383,24 @@ static cudaError_t launch2_u(const LstmParams& p, const LstmLaneLens* lens, cuda
     static_cast<LstmParams&>(pp) = p;
     if constexpr (LENS) pp.lens = *lens;
     void* args[] = {&pp};
-    e = cudaLaunchCooperativeKernel((void*)lstm_rec2_kernel<U, PASS3, LENS>, dim3(p.G), dim3(L2_WARPS * 32), args, smem, st);
+    e = cudaLaunchCooperativeKernel((void*)lstm_rec2_kernel<U, PASS3, LENS, REV>, dim3(p.G), dim3(L2_WARPS * 32), args, smem, st);
     if (e != cudaSuccess) return e;
     // h_{T-1} was published into parity slot (T-1) & 1
     if (p.state_h) e = cudaMemcpyAsync(p.state_h, p.h16 + (size_t)((p.T - 1) & 1) * PL * plane_words, sizeof(uint32_t) * PL * plane_words, cudaMemcpyDeviceToDevice, st);
     return e;
 }
 
-cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st, const LstmLaneLens* lens) {
+cudaError_t launch_lstm2_layer(const LstmParams& p, cudaStream_t st, const LstmLaneLens* lens, bool reverse) {
     if (p.B > L2_BT || p.B <= 0 || !p.whh_p2 || !p.h16) return cudaErrorInvalidValue;
     if ((p.H / 16) % L2_WARPS != 0) return cudaErrorInvalidValue;
+    if (reverse) {   // the fp32-faithful class (JDCNet's BiLSTM), no carried stream state
+        if (!lens || !p.pass3 || p.state_h || p.state_c) return cudaErrorInvalidValue;
+        for (int b = 0; b < p.B; ++b)
+            if (lens->len[b] < 0 || lens->len[b] > p.T) return cudaErrorInvalidValue;
+        if (p.U == 8) return launch2_u<8, true, true, true>(p, lens, st);
+        if (p.U == 12) return launch2_u<12, true, true, true>(p, lens, st);
+        return cudaErrorInvalidValue;
+    }
     if (lens) {   // the one-pass class (the decoder's LSTM) only
         if (p.pass3) return cudaErrorInvalidValue;
         if (p.U == 8) return launch2_u<8, false, true>(p, lens, st);

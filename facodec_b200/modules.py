@@ -2077,3 +2077,151 @@ class CNNLSTM(nn.Module):
         rc = e.L.fac_head_forward(e.handle, self._head_id, _ptr(x), B, T, arr, _stream(x.device))
         _lib.check(e.handle, rc, "fac_head_forward")
         return outs
+
+
+class _JdcResBlock(nn.Module):
+    """Parameter holder of modules/JDC/model.py ResBlock (state-dict keys only; JDCNet.forward runs on the GPU)."""
+
+    def __init__(self, cin, cout):
+        super().__init__()
+        self.pre_conv = nn.Sequential(nn.BatchNorm2d(cin), nn.LeakyReLU(0.01), nn.MaxPool2d((1, 2)))
+        self.conv = nn.Sequential(nn.Conv2d(cin, cout, 3, padding=1, bias=False), nn.BatchNorm2d(cout), nn.LeakyReLU(0.01),
+                                  nn.Conv2d(cout, cout, 3, padding=1, bias=False))
+        self.conv1by1 = nn.Conv2d(cin, cout, 1, bias=False)
+
+
+class JDCNet(nn.Module):
+    """modules/JDC/model.py JDCNet(num_class=1, seq_len=192) -- the F0 extractor train.py loads -- in eval mode.  Same
+    state-dict keys (the ``['net']`` dict of ``bst.t7``); ``forward(x, lengths=None)`` takes normalized log-mel ``x``
+    [B, 1, 80, T] on a CUDA device and returns ``(F0 [B, T], GAN_feature [B, 256, 10, T], poolblock_out [B, 256, T, 2])``
+    as model.py:102-137 does in eval mode.  The 3x3 convs run on the wgmma conv kernel in its fp32-faithful promoted class,
+    with every BatchNorm folded in; the BiLSTM runs on the resident-weight recurrence kernel.
+
+    ``lengths`` (B ints in [1, T]) makes a ragged batch: lane b is its own first lengths[b] frames, bit for bit what a
+    B = 1 call on them returns, and its outputs past lengths[b] are zero.  The detector branch (maxpool1-3,
+    detector_conv, bilstm_detector, detector) is loaded but, as in the reference forward, never run.  Training mode
+    (batch statistics, dropout) raises NotImplementedError."""
+
+    def __init__(self, num_class=1, seq_len=192, engine=None):
+        super().__init__()
+        if num_class != 1:
+            raise ValueError("JDCNet: only num_class=1 (the F0 regressor train.py loads) is implemented")
+        self.num_class, self.seq_len = num_class, seq_len
+        self.conv_block = nn.Sequential(nn.Conv2d(1, 64, 3, padding=1, bias=False), nn.BatchNorm2d(64), nn.LeakyReLU(0.01),
+                                        nn.Conv2d(64, 64, 3, padding=1, bias=False))
+        self.res_block1 = _JdcResBlock(64, 128)
+        self.res_block2 = _JdcResBlock(128, 192)
+        self.res_block3 = _JdcResBlock(192, 256)
+        self.pool_block = nn.Sequential(nn.BatchNorm2d(256), nn.LeakyReLU(0.01), nn.MaxPool2d((1, 4)), nn.Dropout(0.2))
+        self.maxpool1 = nn.MaxPool2d((1, 40))
+        self.maxpool2 = nn.MaxPool2d((1, 20))
+        self.maxpool3 = nn.MaxPool2d((1, 10))
+        self.detector_conv = nn.Sequential(nn.Conv2d(640, 256, 1, bias=False), nn.BatchNorm2d(256), nn.LeakyReLU(0.01),
+                                           nn.Dropout(0.2))
+        self.bilstm_classifier = nn.LSTM(512, 256, batch_first=True, bidirectional=True)
+        self.bilstm_detector = nn.LSTM(512, 256, batch_first=True, bidirectional=True)
+        self.classifier = nn.Linear(512, num_class)
+        self.detector = nn.Linear(512, 2)
+        for p in self.parameters():
+            p.requires_grad_(False)
+        self._engine = engine if engine is not None else Engine()
+        self._jdc_id = None
+        self._tag = None
+
+    def _sync(self, device):
+        e = self._engine
+        e._ensure(device)
+        sd = self.state_dict()
+        tag = tuple((t._version, t.data_ptr()) for t in sd.values())
+        if self._tag == tag:
+            return
+        L, h = e.L, e.handle
+        if self._jdc_id is None:
+            self._jdc_id = _lib.check(h, L.fac_jdc_begin(h), "fac_jdc_begin")
+        for k, t in sd.items():
+            if k.endswith("num_batches_tracked"):
+                continue
+            t = t.detach().to("cpu", torch.float32).contiguous()
+            shape = (ctypes.c_int64 * max(t.dim(), 1))(*t.shape)
+            _lib.check(h, L.fac_jdc_tensor(h, self._jdc_id, k.encode(), _ptr(t), shape, t.dim()), "fac_jdc_tensor(%s)" % k)
+        _lib.check(h, L.fac_jdc_finalize(h, self._jdc_id), "fac_jdc_finalize")
+        self._tag = tag
+
+    def forward(self, x, lengths=None):
+        if self.training:
+            raise NotImplementedError("facodec_b200.JDCNet implements the eval-mode forward only; call .eval()")
+        if not isinstance(x, torch.Tensor) or x.dim() != 4 or x.shape[1] != 1 or x.shape[2] != 80 or x.shape[3] < 1:
+            raise _lib.FacError("JDCNet expects x [B, 1, 80, T]; got %s" % ((tuple(x.shape) if isinstance(x, torch.Tensor) else type(x)),))
+        B, T = int(x.shape[0]), int(x.shape[3])
+        if B < 1:
+            raise _lib.FacError("JDCNet: empty batch")
+        self._sync(x.device)
+        e = self._engine
+        lens = None if lengths is None else _lane_counts(lengths, B, 1, T, "lengths")
+        x = _f32c(x)
+        f0 = torch.empty(B, T, device=x.device)
+        gan = torch.empty(B, 256, 10, T, device=x.device)
+        pool = torch.empty(B, 256, T, 2, device=x.device)
+        _lib.check(e.handle, e.L.fac_jdc_forward(e.handle, self._jdc_id, _ptr(x), B, T, _c_ints(lens) if lens else None, _ptr(f0),
+                                                 _ptr(gan), _ptr(pool), _stream(x.device)), "fac_jdc_forward")
+        return f0, gan, pool
+
+
+def load_F0_models(path):
+    """modules/commons.py:183-191 load_F0_models: JDCNet(num_class=1, seq_len=192) with ``torch.load(path)['net']``.
+    Returned in eval mode, unlike the reference's ``.train()``: train mode uses batch statistics and dropout, so its F0
+    changes from call to call; eval mode is what this package computes."""
+    model = JDCNet(num_class=1, seq_len=192)
+    params = torch.load(path, map_location="cpu")["net"]
+    model.load_state_dict(params)
+    return model.eval()
+
+
+def _check_cuda(t, what):
+    if not isinstance(t, torch.Tensor) or t.device.type != "cuda":
+        raise _lib.FacError("%s must be a CUDA tensor (no CPU fallback); got %s" % (what, t.device if isinstance(t, torch.Tensor) else type(t)))
+
+
+def f0_targets(F0, lengths=None, norm_f0=True):
+    """train.py:219-251 on F0 [B, T] (CUDA): per lane, voiced = F0 > 5.0, log2, then (x - mean) / std (torch.std's unbiased
+    std) on voiced frames and -10 on the others, NaN / inf replaced by -10; glob_f0 = the mean, 0 without a voiced frame
+    (one voiced frame: std is NaN, so that frame is -10 and the mean is kept).  Returns (targets [B, T], glob_f0 [B]: the
+    torch.stack of train.py's list); with norm_f0=False, (F0, []) as train.py leaves them.  ``lengths``: lane b's statistics cover its first
+    lengths[b] frames only and the rest of its targets are -10.  Fixed-order reductions: the result does not depend on B."""
+    _check_cuda(F0, "F0")
+    if F0.dim() != 2:
+        raise _lib.FacError("f0_targets expects F0 [B, T]; got %s" % (tuple(F0.shape),))
+    if not norm_f0:
+        return F0, []
+    B, T = int(F0.shape[0]), int(F0.shape[1])
+    lens = None if lengths is None else _lane_counts(lengths, B, 0, T, "lengths")
+    x = _f32c(F0)
+    out = torch.empty(B, T, device=x.device)
+    glob = torch.empty(B, device=x.device)
+    if B == 0 or T == 0:
+        return out.fill_(-10.0), glob.zero_()
+    e = _rs_engine(x.device)
+    _lib.check(e.handle, e.L.fac_f0_targets(e.handle, _ptr(x), B, T, _c_ints(lens) if lens else None, _ptr(out), _ptr(glob),
+                                            _stream(x.device)), "fac_f0_targets")
+    return out, glob
+
+
+def log_norm(x, mean=-4, std=4, dim=2):
+    """modules/commons.py:176-181 log_norm: log(||exp(x * std + mean)||_2 over `dim`) for normalized log-mel x [..., 80, T]
+    whose `dim` is the 80-bin axis (train.py:215: x [B, 1, 80, T], dim = 2 -> [B, 1, T]).  Only the reference's mean = -4,
+    std = 4 are implemented."""
+    _check_cuda(x, "x")
+    if mean != -4 or std != 4:
+        raise ValueError("log_norm: only mean=-4, std=4 are implemented")
+    nd = x.dim()
+    if nd < 2 or dim % nd != nd - 2 or x.shape[-2] != 80:
+        raise _lib.FacError("log_norm expects x [..., 80, T] normed over its 80-bin axis; got %s, dim=%d" % (tuple(x.shape), dim))
+    T = int(x.shape[-1])
+    B = x.numel() // (80 * T) if T else 0
+    xc = _f32c(x)
+    out = torch.empty(tuple(x.shape[:-2]) + (T,), device=x.device)
+    if B == 0 or T == 0:
+        return out
+    e = _rs_engine(x.device)
+    _lib.check(e.handle, e.L.fac_log_norm(e.handle, _ptr(xc), B, T, _ptr(out), _stream(x.device)), "fac_log_norm")
+    return out

@@ -25,6 +25,7 @@ reference-like statistics:
 ``synth_waves`` follows meldataset.py:67-68 (PseudoDataset) with fixed length.
 """
 import math
+from collections import OrderedDict
 
 import numpy as np
 import torch
@@ -274,3 +275,30 @@ def synth_waves(batch, n_samples=4 * SR, seed=114514):
         w = w / np.max(np.abs(w))
         out[i, 0] = w.astype(np.float32)
     return torch.from_numpy(out)
+
+
+def synth_jdc(seed=0):
+    """Synthetic weights of JDCNet(num_class=1, seq_len=192) (modules/JDC/model.py) under its state-dict keys: 2-D convs
+    and linears at 1/sqrt(fan_in), BatchNorms with non-trivial affine parameters and running statistics, and a classifier
+    weight of 40 / sqrt(512) and bias of 4.5, so that F0 = |classifier| falls on both sides of train.py's 5.0 voiced threshold."""
+    from .modules import JDCNet
+    g = _Gen(700 + seed)
+    sd = OrderedDict()
+    for k, t in JDCNet().state_dict().items():
+        shape = tuple(t.shape)
+        if k.endswith("num_batches_tracked"):
+            sd[k] = torch.tensor(1000, dtype=torch.long)
+        elif k.endswith("running_mean"):
+            sd[k] = g.uniform(shape, 0.2)
+        elif k.endswith("running_var"):
+            sd[k] = g.scale(shape, 0.5, 1.5)
+        elif len(shape) == 1 and not k.startswith(("bilstm", "classifier", "detector.")):
+            sd[k] = g.scale(shape, 0.8, 1.2) if k.endswith("weight") else g.uniform(shape, 0.1)   # BatchNorm affine
+        elif k.startswith("bilstm"):
+            sd[k] = g.uniform(shape, 1.0 / math.sqrt(256))
+        elif k == "classifier.bias":
+            sd[k] = torch.full(shape, 4.5)
+        else:
+            fan_in = int(np.prod(shape[1:])) if len(shape) > 1 else shape[0]
+            sd[k] = g.uniform(shape, (40.0 if k == "classifier.weight" else 1.0) / math.sqrt(fan_in))
+    return sd

@@ -488,6 +488,25 @@ int fac_head_finalize(fac_handle* h, int head_id, int indim, int outdim, int nhe
 int fac_head_forward(fac_handle* h, int head_id, const float* x, int B, int T, float* const* outs, void* stream);
 int fac_add3(fac_handle* h, const float* a, const float* b, const float* c, long long n, float* out, void* stream);
 
+/* JDCNet pitch extractor (modules/JDC/model.py JDCNet(num_class=1), eval mode; the model train.py's load_F0_models loads).
+ * fac_jdc_begin returns an id; stage the reference state_dict tensors (the ['net'] dict of bst.t7: "conv_block.0.weight",
+ * "res_block1.pre_conv.0.running_mean", "bilstm_classifier.weight_ih_l0_reverse", "classifier.bias", ...; the detector
+ * branch's keys are accepted and unused) with fac_jdc_tensor, then fac_jdc_finalize, which folds every BatchNorm (eval:
+ * running statistics, eps 1e-5).  fac_jdc_forward: mel [B,1,80,T] (device) -> f0 [B,T], gan_feature [B,256,10,T] and
+ * pool_out [B,256,T,2] (caller-allocated device buffers), model.py:102-137 with Dropout as the identity.  lengths (HOST,
+ * B ints in [1, T], or NULL): lane b is its own first lengths[b] frames -- every 3x3 conv zero-pads time at the lane's own
+ * end and the reverse LSTM starts at its last frame -- bit-identical to a B = 1 call on them; outputs past lengths[b] are 0.
+ * fac_f0_targets (train.py:219-251, norm_f0): f0 [B,T] (device) -> targets [B,T] and glob_f0 [B]; lengths (HOST, in [0, T],
+ * or NULL) limits lane b to its first lengths[b] frames (the others are -10).  fac_log_norm (modules/commons.py:176-181,
+ * mean -4, std 4): mel [B,80,T] -> out [B,T] = log(||exp(4 mel - 4)||_2 over the 80 bins). */
+int fac_jdc_begin(fac_handle* h);
+int fac_jdc_tensor(fac_handle* h, int jdc_id, const char* key, const float* data_host, const int64_t* shape, int ndim);
+int fac_jdc_finalize(fac_handle* h, int jdc_id);
+int fac_jdc_forward(fac_handle* h, int jdc_id, const float* mel, int B, int T, const int* lengths, float* f0, float* gan_feature,
+                    float* pool_out, void* stream);
+int fac_f0_targets(fac_handle* h, const float* f0, int B, int T, const int* lengths, float* targets, float* glob_f0, void* stream);
+int fac_log_norm(fac_handle* h, const float* mel, int B, int T, float* out, void* stream);
+
 /* Engine options.  "tensor_cores": 0 = fp32 FMA kernels everywhere; 1 = wgmma split-operand
  * kernel for every eligible layer downstream of the VQ (decoder, timbre branch), fp32 FMA upstream
  * (encoder, prosody branch); 2 (default) = wgmma everywhere, with the promoted accumulation

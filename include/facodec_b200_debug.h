@@ -188,7 +188,10 @@ int fac_debug_attention(fac_handle* h, const float* q, const float* k, const flo
  * (mel scales only) the filterbank [nb][n_mels] as the terms kernel reads it.  fac_spectral_loss_grad adds spec.dframes.<i>:
  * the frames buffer [2*B*F][w] after the transposed DFT GEMM, whose rows of each signal with a requested gradient hold
  * dL/dframes scaled by a per-row power of two (the other signal's rows still hold its frames), and spec.dscale.<i> [2*B*F]
- * the inverse row scales: dL/dframes = row * dscale[row]. */
+ * the inverse row scales: dL/dframes = row * dscale[row].  fac_jdc_forward's taps, maps channels-last [B][T][F + 2][C]
+ * with zero pad columns: jdc.conv_in (conv_block.0-2, F = 80), jdc.conv_block (conv_block.3), jdc.res<i>.pre (res_block<i>
+ * pre_conv), jdc.res<i>.conv1 (conv.0-2), jdc.res<i> (the block's output); jdc.lstm_in [B][T][512], jdc.lstm.xg_fwd /
+ * jdc.lstm.xg_rev [B][T][1024] (input GEMMs, gate order i, f, g, o, b_ih + b_hh added), jdc.lstm.fwd / jdc.lstm.rev [B][T][256]. */
 int fac_debug_tap(fac_handle* h, const char* name, float* dst, size_t capacity_floats);
 
 /* Per-kernel-family device timing for bench.py's roofline object: when enabled, every launch of
