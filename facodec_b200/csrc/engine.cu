@@ -38,6 +38,7 @@ struct HostTensor {
     std::vector<int64_t> shape;
     size_t numel() const { size_t n = 1; for (auto s : shape) n *= (size_t)s; return n; }
 };
+using TensorMap = std::map<std::string, HostTensor>;
 
 struct ConvW {
     size_t w = 0, b = 0; int Cin = 0, Cout = 0, K = 1, ldw = 0;
@@ -77,11 +78,43 @@ struct QuantW {
     ConvW dft; size_t fb = 0;
     ConvW dft_tc;      // same basis as a K=1 GEMM over gathered frames: Cin = 1200, Cout padded to 2176 (17 x 128)
 };
-struct RvqSet { int nq; VqW vq[8]; };
 
 struct DevFree { void operator()(void* p) const { cudaFree(p); } };
 template <typename E> using DevBuf = std::unique_ptr<E, DevFree>;   // owned device memory
 using DevMem = DevBuf<char>;
+
+// One fac_rvq_create set and the arena its offsets point into.
+struct RvqSet { int nq; VqW vq[8]; DevBuf<float> arena; };
+
+// One CNNLSTM predictor head (modules/quantize.py:106-125): 3 ResidualUnits (alias-free SnakeBeta, k7 conv dilation
+// 1/2/3 with zero padding, alias-free SnakeBeta, 1x1 conv, +x), a final alias-free SnakeBeta, nheads Linear layers.
+// Packed with the codec's conv packers; weights live in their own arena.
+struct HeadSet {
+    int indim = 0, outdim = 0, nheads = 0, global_pred = 0;
+    struct Unit { size_t a1, b1, a2, b2; ConvW c7, c1; int dil; } unit[3];
+    size_t af, bf;                  // final activation exp(alpha), exp(beta)
+    ConvW lin[8];
+    TensorMap staged;
+    DevBuf<float> arena;
+    bool ready = false;
+};
+
+// One JDCNet(num_class=1) in eval mode (modules/JDC/model.py:102-137).  Every 3x3 conv that a BatchNorm follows carries it
+// folded into its weights and bias; the BatchNorms before a max-pool are per-channel scale / shift pairs.
+struct JdcSet {
+    struct Bn { size_t sc = 0, sh = 0; };
+    size_t conv_in_w = 0, conv_in_b = 0;       // conv_block.0 + .1: [9][64], [64]
+    ConvW c0b;                                 // conv_block.3 (64 -> 64, no BN after it)
+    struct Block { Bn pre; ConvW c1, c2, c11; int F = 0; } blk[3];    // res_block1..3: F = input frequency columns
+    Bn pool;                                   // pool_block.0
+    ConvW ih[2];                               // bilstm_classifier input GEMMs (forward, reverse): 512 -> 1024
+    size_t whh2[2] = {0, 0};                   // their recurrent weights, lstm2_pack(pass3 = 1)
+    int U = 0, G = 0;
+    size_t cls_w = 0, cls_b = 0;               // classifier: [512], [1]
+    TensorMap staged;
+    DevBuf<float> arena;
+    bool ready = false;
+};
 
 struct LstmState { uint32_t* h[2] = {nullptr, nullptr}; float* c[2] = {nullptr, nullptr}; };
 
@@ -153,27 +186,25 @@ using DecPool = Pool<DecHalf>;
 struct fac_handle {
     int device = 0;
     std::string err;
-    std::map<std::string, HostTensor> host[FAC_NUM_MODULES];
+    TensorMap host[FAC_NUM_MODULES];
     bool have[FAC_NUM_MODULES] = {false, false, false, false, false};
     bool finalized = false;
     uint64_t fp[FAC_NUM_MODULES] = {0, 0, 0, 0, 0};   // weight fingerprints of the modules, taken at fac_finalize (session state)
-    std::vector<float> pack;        // host staging of the weight arena
-    float* warena = nullptr; size_t wfloats = 0;
+    DevBuf<float> warena;           // the codec's weights: the offsets in enc, dec, qw, red and dec2 point into it
     EncW enc; DecW dec; QuantW qw;
     RedW red; DecW dec2;            // voice-conversion model: Redecoder + its non-causal, LSTM-free decoder
-    std::vector<RvqSet> rvqs; std::vector<float*> rvq_arenas;
-    // streams and pools by id; an ended stream or a destroyed pool leaves a null entry, so ids are never reused
+    // weight sets, streams and pools by id; a destroyed set, an ended stream or a destroyed pool leaves a null entry, so ids
+    // are never reused
+    std::vector<std::unique_ptr<RvqSet>> rvqs;              // residual VQ sets (fac_rvq_*)
+    std::vector<std::unique_ptr<HeadSet>> heads;            // modules/quantize.py:106-125 CNNLSTM instances (fac_head_*)
+    std::vector<std::unique_ptr<JdcSet>> jdcs;              // modules/JDC/model.py JDCNet instances, eval mode (fac_jdc_*)
     std::vector<std::unique_ptr<Stream>> streams;           // chunked encoder / decoder (fac_stream_*)
     std::vector<std::unique_ptr<VcStream>> vc_streams;      // chunked voice conversion through the redecoder (fac_vc_stream_*)
     std::vector<std::unique_ptr<CodesPool>> codes_pools;    // many B = 1 compression streams (fac_codes_pool_*)
     std::vector<std::unique_ptr<VcPool>> vc_pools;          // many B = 1 voice-conversion streams (fac_vc_pool_*)
     std::vector<std::unique_ptr<DecPool>> dec_pools;        // many B = 1 decode-from-codes streams (fac_dec_pool_*)
     fac::RsHost* rs = nullptr;      // resampler filter tables and session pools (fac_resample*, fac_rs_pool_*), made on use
-    struct HeadSet;                 // modules/quantize.py:106-125 CNNLSTM instances (fac_head_*)
-    std::vector<HeadSet*> heads;
-    struct JdcSet;                  // modules/JDC/model.py JDCNet instances, eval mode (fac_jdc_*)
-    std::vector<JdcSet*> jdcs;
-    char* ws = nullptr; size_t ws_bytes = 0;
+    DevMem ws; size_t ws_bytes = 0;
     int launches = 0;
     // tensor-core path (fac_set_option "tensor_cores"): 0 = never, 1 = layers downstream of the VQ only
     // (decoder, timbre branch), 2 = every eligible layer (default; promoted accumulation upstream of the VQ)
@@ -192,17 +223,17 @@ struct fac_handle {
     bool dec_bf16 = true;           // decoder-side layers use the bf16x3 split (fac_set_option "decoder_bf16")
     // second stream for the waveform-only half of the quantizer (fac_set_option "overlap_front")
     int overlap_front = 1; cudaStream_t side = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    float* aa_filter = nullptr;
+    DevBuf<float> aa_filter;
     // dataset-side mel (meldataset.py:29-47: MelSpectrogram with its default sample_rate 16000): own constants, built lazily
-    float* mel16_arena = nullptr; ConvW mel16_dft, mel16_dft_tc; size_t mel16_fb = 0;
+    DevBuf<float> mel16_arena; ConvW mel16_dft, mel16_dft_tc; size_t mel16_fb = 0;
     // losses.py:65-89 reconstruction_loss: per scale s = 64 << i the window-folded DFT basis [s][ld] (+ tensor-core blobs)
     // and the 64-band HTK filterbank [n_fft/2 + 1][64]; built on first use
     struct LossScale { ConvW dft; size_t fb = 0; int s = 0, nfft = 0, nb = 0, ld = 0; };
-    float* loss_arena = nullptr; LossScale loss_scale[6];
+    DevBuf<float> loss_arena; LossScale loss_scale[6];
     // dac/nn/loss.py MultiScaleSTFTLoss / MelSpectrogramLoss: one cached configuration (rebuilt when the arguments change);
     // dftT is the same basis transposed ([ld][w]: the gradient GEMM dframes = dspec basis^T)
     struct SpecScale { ConvW dft, dftT; size_t fb = 0; int w = 0, nb = 0, ld = 0, n_out = 0; bool mel = false; };
-    float* spec_arena = nullptr; std::vector<SpecScale> spec_scales; std::vector<double> spec_key;
+    DevBuf<float> spec_arena; std::vector<SpecScale> spec_scales; std::vector<double> spec_key;
     // optional per-kernel-family timing (fac_profile_*): CUDA events around every launch
     bool profiling = false;
     struct ProfRec { std::string name; cudaEvent_t a, b; double flops, bytes; };
@@ -213,67 +244,41 @@ struct fac_handle {
     std::map<std::string, std::pair<float*, size_t>> taps;
 };
 
-// One CNNLSTM predictor head (modules/quantize.py:106-125): 3 ResidualUnits (alias-free SnakeBeta, k7 conv dilation
-// 1/2/3 with zero padding, alias-free SnakeBeta, 1x1 conv, +x), a final alias-free SnakeBeta, nheads Linear layers.
-// Built through a private staging handle so that the conv packing code is shared; weights live in their own arena.
-struct fac_handle::HeadSet {
-    int indim = 0, outdim = 0, nheads = 0, global_pred = 0;
-    struct Unit { size_t a1, b1, a2, b2; ConvW c7, c1; int dil; } unit[3];
-    size_t af, bf;                  // final activation exp(alpha), exp(beta)
-    ConvW lin[8];
-    std::map<std::string, HostTensor> staged;
-    float* arena = nullptr;
-    bool ready = false;
-};
-
-// One JDCNet(num_class=1) in eval mode (modules/JDC/model.py:102-137).  Every 3x3 conv that a BatchNorm follows carries it
-// folded into its weights and bias; the BatchNorms before a max-pool are per-channel scale / shift pairs.
-struct fac_handle::JdcSet {
-    struct Bn { size_t sc = 0, sh = 0; };
-    size_t conv_in_w = 0, conv_in_b = 0;       // conv_block.0 + .1: [9][64], [64]
-    ConvW c0b;                                 // conv_block.3 (64 -> 64, no BN after it)
-    struct Block { Bn pre; ConvW c1, c2, c11; int F = 0; } blk[3];    // res_block1..3: F = input frequency columns
-    Bn pool;                                   // pool_block.0
-    ConvW ih[2];                               // bilstm_classifier input GEMMs (forward, reverse): 512 -> 1024
-    size_t whh2[2] = {0, 0};                   // their recurrent weights, lstm2_pack(pass3 = 1)
-    int U = 0, G = 0;
-    size_t cls_w = 0, cls_b = 0;               // classifier: [512], [1]
-    std::map<std::string, HostTensor> staged;
-    float* arena = nullptr;
-    bool ready = false;
-};
-
 namespace {
 
 // ------------------------------------------------------------------------------------------
 // packing helpers (host)
 // ------------------------------------------------------------------------------------------
-size_t pack_alloc(fac_handle* h, size_t n) {
-    size_t off = (h->pack.size() + 63) / 64 * 64;
-    h->pack.resize(off + n, 0.f);
-    return off;
-}
+// Host staging of one weight arena: every tensor starts on a 64-float boundary.
+struct Packer {
+    std::vector<float> pack;
+    size_t alloc(size_t n) {
+        size_t off = (pack.size() + 63) / 64 * 64;
+        pack.resize(off + n, 0.f);
+        return off;
+    }
+};
 
-const HostTensor* find(fac_handle* h, int m, const std::string& k) {
-    auto it = h->host[m].find(k);
-    return it == h->host[m].end() ? nullptr : &it->second;
+const HostTensor* find(const TensorMap& ts, const std::string& k) {
+    auto it = ts.find(k);
+    return it == ts.end() ? nullptr : &it->second;
 }
 
 struct PackError { std::string msg; };
-const HostTensor& need(fac_handle* h, int m, const std::string& k) {
-    const HostTensor* t = find(h, m, k);
-    if (!t) throw PackError{"missing tensor '" + k + "' in module " + std::to_string(m)};
+const HostTensor& need(const TensorMap& ts, const std::string& k) {
+    const HostTensor* t = find(ts, k);
+    if (!t) throw PackError{"missing tensor '" + k + "'"};
     return *t;
 }
 
 // Folded conv weight in PyTorch layout [d0][d1][K] (weight-norm over dims != 0, encodec.py:42-51).
-std::vector<float> folded_weight(fac_handle* h, int m, const std::string& prefix, std::vector<int64_t>& shape) {
-    if (const HostTensor* w = find(h, m, prefix + ".weight")) {
+std::vector<float> folded_weight(const TensorMap& ts, const std::string& prefix, std::vector<int64_t>& shape) {
+    if (const HostTensor* w = find(ts, prefix + ".weight")) {
         shape = w->shape;
         return w->data;
     }
-    const HostTensor& v = need(h, m, prefix + ".weight_v");
-    const HostTensor& g = need(h, m, prefix + ".weight_g");
+    const HostTensor& v = need(ts, prefix + ".weight_v");
+    const HostTensor& g = need(ts, prefix + ".weight_g");
     shape = v.shape;
     size_t d0 = (size_t)v.shape[0], inner = v.numel() / d0;
     if (g.numel() != d0) throw PackError{"weight_g shape mismatch at " + prefix};
@@ -289,7 +294,7 @@ std::vector<float> folded_weight(fac_handle* h, int m, const std::string& prefix
 
 // Builds the tensor-core weight blob for a packed conv (stride-1 in rows; `stride` > 1 means the
 // kernel-2*stride down-conv viewed as a 2-tap conv over rows of `stride` samples).
-void attach_tc(fac_handle* h, ConvW& c, int stride, bool promoted) {
+void attach_tc(Packer& P, ConvW& c, int stride, bool promoted) {
     TcConvParams tp;
     tp.Cin = c.Cin; tp.Cout = c.Cout; tp.dil = 1; tp.promoted = promoted ? 1 : 0;
     if (stride == 1) { tp.vf = 1; tp.Kr = c.K; }
@@ -298,23 +303,23 @@ void attach_tc(fac_handle* h, ConvW& c, int stride, bool promoted) {
     if (!tc_conv_plan(tp)) return;
     c.vf = tp.vf; c.Kr = tp.Kr; c.promoted = promoted; c.tcN = tp.N;
     size_t n = tc_blob_floats(tp);
-    c.tcw = pack_alloc(h, n);
-    tc_pack_blob(tp, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw);
+    c.tcw = P.alloc(n);
+    tc_pack_blob(tp, P.pack.data() + c.w, c.ldw, P.pack.data() + c.tcw);
     c.tc = true;
     if (promoted) {
         TcConvParams t16 = tp;
         t16.f16x2 = 1;
         if (tc_conv_plan(t16)) {
-            c.tcw16 = pack_alloc(h, tc_blob_floats(t16));
-            tc_pack_blob(t16, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw16);
+            c.tcw16 = P.alloc(tc_blob_floats(t16));
+            tc_pack_blob(t16, P.pack.data() + c.w, c.ldw, P.pack.data() + c.tcw16);
             c.has16 = true;
         }
     } else {
         TcConvParams t16 = tp;
         t16.bf16 = 1;
         if (tc_conv_plan(t16)) {
-            c.tcw16 = pack_alloc(h, tc_blob_floats(t16));
-            tc_pack_blob(t16, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw16);
+            c.tcw16 = P.alloc(tc_blob_floats(t16));
+            tc_pack_blob(t16, P.pack.data() + c.w, c.ldw, P.pack.data() + c.tcw16);
             c.has16 = true;
         }
     }
@@ -322,117 +327,117 @@ void attach_tc(fac_handle* h, ConvW& c, int stride, bool promoted) {
 
 // hi-only fp16 blob of a stride-1 layer downstream of the VQ (conv_tc_kernel's one-pass class; the dilated k = 7 convs of
 // the ResidualUnits: 7/8 of a unit's MACs, 1.4e-5 RMS on the waveform, scripts/cpu_decoder_precision.py)
-void attach_f16_single(fac_handle* h, ConvW& c) {
+void attach_f16_single(Packer& P, ConvW& c) {
     if (!c.tc || c.promoted || !c.has16 || c.vf != 1) return;
     TcConvParams t1;
     t1.Cin = c.Cin; t1.Cout = c.Cout; t1.dil = 1; t1.vf = 1; t1.Kr = c.K; t1.bf16 = 1; t1.g1f16 = 1;
     if (!tc_conv_plan(t1)) return;
-    c.tcw_f16s = pack_alloc(h, tc_blob_floats(t1));
-    tc_pack_blob(t1, h->pack.data() + c.w, c.ldw, h->pack.data() + c.tcw_f16s);
+    c.tcw_f16s = P.alloc(tc_blob_floats(t1));
+    tc_pack_blob(t1, P.pack.data() + c.w, c.ldw, P.pack.data() + c.tcw_f16s);
     c.has_f16s = true;
 }
 
 // nn.Conv1d [Cout][Cin][K] -> packed [K*Cin][ldw]
-ConvW pack_conv(fac_handle* h, int m, const std::string& prefix, int stride = 1, bool promoted = false) {
+ConvW pack_conv(Packer& P, const TensorMap& ts, const std::string& prefix, int stride = 1, bool promoted = false) {
     std::vector<int64_t> shp;
-    std::vector<float> w = folded_weight(h, m, prefix, shp);
+    std::vector<float> w = folded_weight(ts, prefix, shp);
     if (shp.size() == 2) shp.push_back(1);
     if (shp.size() != 3) throw PackError{"conv weight rank at " + prefix};
     ConvW c;
     c.Cout = (int)shp[0]; c.Cin = (int)shp[1]; c.K = (int)shp[2];
     c.ldw = (c.Cout + 3) / 4 * 4;
-    c.w = pack_alloc(h, (size_t)c.K * c.Cin * c.ldw);
+    c.w = P.alloc((size_t)c.K * c.Cin * c.ldw);
     for (int co = 0; co < c.Cout; ++co)
         for (int ci = 0; ci < c.Cin; ++ci)
             for (int k = 0; k < c.K; ++k)
-                h->pack[c.w + ((size_t)k * c.Cin + ci) * c.ldw + co] = w[((size_t)co * c.Cin + ci) * c.K + k];
-    const HostTensor& b = need(h, m, prefix + ".bias");
-    c.b = pack_alloc(h, c.Cout);
-    for (int co = 0; co < c.Cout; ++co) h->pack[c.b + co] = b.data[co];
-    attach_tc(h, c, stride, promoted);
+                P.pack[c.w + ((size_t)k * c.Cin + ci) * c.ldw + co] = w[((size_t)co * c.Cin + ci) * c.K + k];
+    const HostTensor& b = need(ts, prefix + ".bias");
+    c.b = P.alloc(c.Cout);
+    for (int co = 0; co < c.Cout; ++co) P.pack[c.b + co] = b.data[co];
+    attach_tc(P, c, stride, promoted);
     return c;
 }
 
 // nn.ConvTranspose1d [Cin][Cout][2s] stride s + right trim (encodec.py:248-270) -> K=2 conv with
 // Cout*s phase-major output channels: tap0 (x[t-1]) = w[..][r+s], tap1 (x[t]) = w[..][r].
-ConvW pack_convtr(fac_handle* h, int m, const std::string& prefix, int stride, bool promoted = false) {
+ConvW pack_convtr(Packer& P, const TensorMap& ts, const std::string& prefix, int stride, bool promoted = false) {
     std::vector<int64_t> shp;
-    std::vector<float> w = folded_weight(h, m, prefix, shp);
+    std::vector<float> w = folded_weight(ts, prefix, shp);
     if (shp.size() != 3 || shp[2] != 2 * stride) throw PackError{"convtr kernel != 2*stride at " + prefix};
     int Cin = (int)shp[0], Cout = (int)shp[1], K = (int)shp[2];
     ConvW c;
     c.Cin = Cin; c.Cout = Cout * stride; c.K = 2; c.ldw = (c.Cout + 3) / 4 * 4;
-    c.w = pack_alloc(h, (size_t)2 * Cin * c.ldw);
+    c.w = P.alloc((size_t)2 * Cin * c.ldw);
     for (int ci = 0; ci < Cin; ++ci)
         for (int co = 0; co < Cout; ++co)
             for (int r = 0; r < stride; ++r) {
-                h->pack[c.w + ((size_t)0 * Cin + ci) * c.ldw + r * Cout + co] = w[((size_t)ci * Cout + co) * K + r + stride];
-                h->pack[c.w + ((size_t)1 * Cin + ci) * c.ldw + r * Cout + co] = w[((size_t)ci * Cout + co) * K + r];
+                P.pack[c.w + ((size_t)0 * Cin + ci) * c.ldw + r * Cout + co] = w[((size_t)ci * Cout + co) * K + r + stride];
+                P.pack[c.w + ((size_t)1 * Cin + ci) * c.ldw + r * Cout + co] = w[((size_t)ci * Cout + co) * K + r];
             }
-    const HostTensor& b = need(h, m, prefix + ".bias");
-    c.b = pack_alloc(h, c.Cout);
+    const HostTensor& b = need(ts, prefix + ".bias");
+    c.b = P.alloc(c.Cout);
     for (int r = 0; r < stride; ++r)
-        for (int co = 0; co < Cout; ++co) h->pack[c.b + r * Cout + co] = b.data[co];
-    attach_tc(h, c, 1, promoted);
+        for (int co = 0; co < Cout; ++co) P.pack[c.b + r * Cout + co] = b.data[co];
+    attach_tc(P, c, 1, promoted);
     return c;
 }
 
 // Non-causal variant (encodec.py:264-269: trim padding_total - padding_total/2 on the left, padding_total/2 on the right):
 // output sample n = t*s + r reads full[n + pl], pl = s - s/2, i.e. x[t-1]*w[a+s] (a < s) + x[t]*w[a] + x[t+1]*w[a-s] (a >= s)
 // with a = r + pl: a 3-tap conv over (x[t-1], x[t], x[t+1]), zero padding 1 | 1, s*Cout phase-major channels.
-ConvW pack_convtr_noncausal(fac_handle* h, int m, const std::string& prefix, int stride, bool promoted = false) {
+ConvW pack_convtr_noncausal(Packer& P, const TensorMap& ts, const std::string& prefix, int stride, bool promoted = false) {
     std::vector<int64_t> shp;
-    std::vector<float> w = folded_weight(h, m, prefix, shp);
+    std::vector<float> w = folded_weight(ts, prefix, shp);
     if (shp.size() != 3 || shp[2] != 2 * stride) throw PackError{"convtr kernel != 2*stride at " + prefix};
     int Cin = (int)shp[0], Cout = (int)shp[1], K = (int)shp[2];
     const int pl = stride - stride / 2;
     ConvW c;
     c.Cin = Cin; c.Cout = Cout * stride; c.K = 3; c.ldw = (c.Cout + 3) / 4 * 4;
-    c.w = pack_alloc(h, (size_t)3 * Cin * c.ldw);
+    c.w = P.alloc((size_t)3 * Cin * c.ldw);
     for (int ci = 0; ci < Cin; ++ci)
         for (int co = 0; co < Cout; ++co)
             for (int r = 0; r < stride; ++r) {
                 const int a = r + pl;
                 const float* wk = &w[((size_t)ci * Cout + co) * K];
-                h->pack[c.w + ((size_t)0 * Cin + ci) * c.ldw + r * Cout + co] = a < stride ? wk[a + stride] : 0.f;
-                h->pack[c.w + ((size_t)1 * Cin + ci) * c.ldw + r * Cout + co] = wk[a];
-                h->pack[c.w + ((size_t)2 * Cin + ci) * c.ldw + r * Cout + co] = a >= stride ? wk[a - stride] : 0.f;
+                P.pack[c.w + ((size_t)0 * Cin + ci) * c.ldw + r * Cout + co] = a < stride ? wk[a + stride] : 0.f;
+                P.pack[c.w + ((size_t)1 * Cin + ci) * c.ldw + r * Cout + co] = wk[a];
+                P.pack[c.w + ((size_t)2 * Cin + ci) * c.ldw + r * Cout + co] = a >= stride ? wk[a - stride] : 0.f;
             }
-    const HostTensor& b = need(h, m, prefix + ".bias");
-    c.b = pack_alloc(h, c.Cout);
+    const HostTensor& b = need(ts, prefix + ".bias");
+    c.b = P.alloc(c.Cout);
     for (int r = 0; r < stride; ++r)
-        for (int co = 0; co < Cout; ++co) h->pack[c.b + r * Cout + co] = b.data[co];
-    attach_tc(h, c, 1, promoted);
+        for (int co = 0; co < Cout; ++co) P.pack[c.b + r * Cout + co] = b.data[co];
+    attach_tc(P, c, 1, promoted);
     return c;
 }
 
-SnakeW pack_snake(fac_handle* h, int m, const std::string& key) {
-    const HostTensor& a = need(h, m, key);
+SnakeW pack_snake(Packer& P, const TensorMap& ts, const std::string& key) {
+    const HostTensor& a = need(ts, key);
     SnakeW s;
     s.C = (int)a.numel();
-    s.a = pack_alloc(h, s.C);
-    s.ia = pack_alloc(h, s.C);
+    s.a = P.alloc(s.C);
+    s.ia = P.alloc(s.C);
     for (int i = 0; i < s.C; ++i) {
-        h->pack[s.a + i] = a.data[i];
-        h->pack[s.ia + i] = 1.0f / (a.data[i] + 1e-9f);   // (alpha + 1e-9).reciprocal(), fp32
+        P.pack[s.a + i] = a.data[i];
+        P.pack[s.ia + i] = 1.0f / (a.data[i] + 1e-9f);   // (alpha + 1e-9).reciprocal(), fp32
     }
     return s;
 }
 
-ResW pack_res(fac_handle* h, int m, const std::string& prefix, int dil, bool promoted = false) {
+ResW pack_res(Packer& P, const TensorMap& ts, const std::string& prefix, int dil, bool promoted = false) {
     ResW r;
     r.dil = dil;
-    r.s1 = pack_snake(h, m, prefix + ".block.0.alpha");
-    r.c7 = pack_conv(h, m, prefix + ".block.1.conv.conv", 1, promoted);
-    if (!promoted) attach_f16_single(h, r.c7);
-    r.s2 = pack_snake(h, m, prefix + ".block.2.alpha");
-    r.c1 = pack_conv(h, m, prefix + ".block.3.conv.conv", 1, promoted);
+    r.s1 = pack_snake(P, ts, prefix + ".block.0.alpha");
+    r.c7 = pack_conv(P, ts, prefix + ".block.1.conv.conv", 1, promoted);
+    if (!promoted) attach_f16_single(P, r.c7);
+    r.s2 = pack_snake(P, ts, prefix + ".block.2.alpha");
+    r.c1 = pack_conv(P, ts, prefix + ".block.3.conv.conv", 1, promoted);
     return r;
 }
 
-LstmW pack_lstm(fac_handle* h, int m, const std::string& prefix, bool promoted = false) {
+LstmW pack_lstm(Packer& P, const TensorMap& ts, const std::string& prefix, bool promoted = false) {
     LstmW L;
-    const HostTensor& w0 = need(h, m, prefix + ".weight_hh_l0");
+    const HostTensor& w0 = need(ts, prefix + ".weight_hh_l0");
     L.H = (int)w0.shape[1];
     L.U = lstm_units_per_cta(L.H);
     if (L.U == 0) throw PackError{"unsupported LSTM width " + std::to_string(L.H)};
@@ -440,25 +445,25 @@ LstmW pack_lstm(fac_handle* h, int m, const std::string& prefix, bool promoted =
     const int H = L.H, U = L.U, R = 4 * U;
     for (int l = 0; l < 2; ++l) {
         std::string sfx = "_l" + std::to_string(l);
-        const HostTensor& wih = need(h, m, prefix + ".weight_ih" + sfx);
-        const HostTensor& whh = need(h, m, prefix + ".weight_hh" + sfx);
-        const HostTensor& bih = need(h, m, prefix + ".bias_ih" + sfx);
-        const HostTensor& bhh = need(h, m, prefix + ".bias_hh" + sfx);
+        const HostTensor& wih = need(ts, prefix + ".weight_ih" + sfx);
+        const HostTensor& whh = need(ts, prefix + ".weight_hh" + sfx);
+        const HostTensor& bih = need(ts, prefix + ".bias_ih" + sfx);
+        const HostTensor& bhh = need(ts, prefix + ".bias_hh" + sfx);
         ConvW c;
         c.Cin = H; c.Cout = 4 * H; c.K = 1; c.ldw = 4 * H;
-        c.w = pack_alloc(h, (size_t)H * c.ldw);
+        c.w = P.alloc((size_t)H * c.ldw);
         for (int row = 0; row < 4 * H; ++row)
-            for (int k = 0; k < H; ++k) h->pack[c.w + (size_t)k * c.ldw + row] = wih.data[(size_t)row * H + k];
-        c.b = pack_alloc(h, 4 * H);
-        for (int row = 0; row < 4 * H; ++row) h->pack[c.b + row] = bih.data[row] + bhh.data[row];
-        attach_tc(h, c, 1, promoted);
+            for (int k = 0; k < H; ++k) P.pack[c.w + (size_t)k * c.ldw + row] = wih.data[(size_t)row * H + k];
+        c.b = P.alloc(4 * H);
+        for (int row = 0; row < 4 * H; ++row) P.pack[c.b + row] = bih.data[row] + bhh.data[row];
+        attach_tc(P, c, 1, promoted);
         L.ih[l] = c;
-        L.whh[l] = pack_alloc(h, (size_t)L.G * H * R);
+        L.whh[l] = P.alloc((size_t)L.G * H * R);
         for (int cta = 0; cta < L.G; ++cta)
             for (int k = 0; k < H; ++k)
                 for (int g = 0; g < 4; ++g)
                     for (int u = 0; u < U; ++u)
-                        h->pack[L.whh[l] + ((size_t)cta * H + k) * R + g * U + u] =
+                        P.pack[L.whh[l] + ((size_t)cta * H + k) * R + g * U + u] =
                             whh.data[((size_t)g * H + cta * U + u) * H + k];
         for (int p3 = 0; p3 < 2; ++p3) {
             // second-generation kernel: promoted (upstream) layers use the 3-pass pack, the others the one-pass pack; the
@@ -466,15 +471,15 @@ LstmW pack_lstm(fac_handle* h, int m, const std::string& prefix, bool promoted =
             if (p3 == 0 && promoted) continue;
             if ((H / 16) % 8 != 0 || lstm2_smem_bytes(H, U, p3) > 227 * 1024) continue;
             const size_t nw = lstm2_pack_words(H, U, p3);
-            L.whh2[l][p3] = pack_alloc(h, nw);
-            lstm2_pack(whh.data.data(), H, U, p3, reinterpret_cast<uint32_t*>(h->pack.data() + L.whh2[l][p3]));
+            L.whh2[l][p3] = P.alloc(nw);
+            lstm2_pack(whh.data.data(), H, U, p3, reinterpret_cast<uint32_t*>(P.pack.data() + L.whh2[l][p3]));
             L.has2[p3] = true;
         }
         if (!promoted) {
             // bf16 hi/lo words for the recurrence downstream of the VQ: [cta][H/16][hi|lo][8 k-pairs][R]
             auto bf16_rn = [](float f) { uint32_t u; memcpy(&u, &f, 4); u += 0x7FFFu + ((u >> 16) & 1u); return (uint32_t)(u >> 16); };
             auto bf16_f = [](uint32_t b) { uint32_t u = b << 16; float f; memcpy(&f, &u, 4); return f; };
-            L.whh16[l] = pack_alloc(h, (size_t)L.G * H * R);
+            L.whh16[l] = P.alloc((size_t)L.G * H * R);
             for (int cta = 0; cta < L.G; ++cta)
                 for (int sub = 0; sub < H / 16; ++sub)
                     for (int k2 = 0; k2 < 8; ++k2)
@@ -485,8 +490,8 @@ LstmW pack_lstm(fac_handle* h, int m, const std::string& prefix, bool promoted =
                             uint32_t l0 = bf16_rn(wrow[0] - bf16_f(h0)), l1 = bf16_rn(wrow[1] - bf16_f(h1));
                             uint32_t hw = h0 | (h1 << 16), lw = l0 | (l1 << 16);
                             size_t base = L.whh16[l] + ((size_t)cta * (H / 16) + sub) * 16 * R;
-                            memcpy(&h->pack[base + (size_t)k2 * R + r], &hw, 4);
-                            memcpy(&h->pack[base + (size_t)(8 + k2) * R + r], &lw, 4);
+                            memcpy(&P.pack[base + (size_t)k2 * R + r], &hw, 4);
+                            memcpy(&P.pack[base + (size_t)(8 + k2) * R + r], &lw, 4);
                         }
             L.has16 = true;
         }
@@ -494,21 +499,15 @@ LstmW pack_lstm(fac_handle* h, int m, const std::string& prefix, bool promoted =
     return L;
 }
 
-VqW pack_vq_raw(std::vector<float>& pack, const float* in_w, const float* in_b, const float* out_w,
-                const float* out_b, const float* codebook, fac_handle* h = nullptr) {
-    auto alloc = [&](size_t n) {
-        size_t off = (pack.size() + 63) / 64 * 64;
-        pack.resize(off + n, 0.f);
-        return off;
-    };
+VqW pack_vq_raw(Packer& P, const float* in_w, const float* in_b, const float* out_w, const float* out_b, const float* codebook) {
     VqW v;
-    v.w_in = alloc(8 * 1024);
-    for (int i = 0; i < 8 * 1024; ++i) pack[v.w_in + i] = in_w[i];
-    v.b_in = alloc(8);
-    for (int i = 0; i < 8; ++i) pack[v.b_in + i] = in_b[i];
-    v.cb = alloc(1024 * 8);
-    v.cbn = alloc(1024 * 8);
-    v.cbn2 = alloc(1024);
+    v.w_in = P.alloc(8 * 1024);
+    for (int i = 0; i < 8 * 1024; ++i) P.pack[v.w_in + i] = in_w[i];
+    v.b_in = P.alloc(8);
+    for (int i = 0; i < 8; ++i) P.pack[v.b_in + i] = in_b[i];
+    v.cb = P.alloc(1024 * 8);
+    v.cbn = P.alloc(1024 * 8);
+    v.cbn2 = P.alloc(1024);
     for (int j = 0; j < 1024; ++j) {
         float n2 = 0.f;
         for (int k = 0; k < 8; ++k) n2 = fmaf(codebook[j * 8 + k], codebook[j * 8 + k], n2);
@@ -516,156 +515,177 @@ VqW pack_vq_raw(std::vector<float>& pack, const float* in_w, const float* in_b, 
         float c2 = 0.f;
         for (int k = 0; k < 8; ++k) {
             float cn = codebook[j * 8 + k] / nrm;
-            pack[v.cb + j * 8 + k] = codebook[j * 8 + k];
-            pack[v.cbn + j * 8 + k] = cn;
+            P.pack[v.cb + j * 8 + k] = codebook[j * 8 + k];
+            P.pack[v.cbn + j * 8 + k] = cn;
             c2 = fmaf(cn, cn, c2);
         }
-        pack[v.cbn2 + j] = c2;
+        P.pack[v.cbn2 + j] = c2;
     }
-    v.w_out = alloc(8 * 1024);   // transposed [k][c]
+    v.w_out = P.alloc(8 * 1024);   // transposed [k][c]
     for (int c = 0; c < 1024; ++c)
-        for (int k = 0; k < 8; ++k) pack[v.w_out + (size_t)k * 1024 + c] = out_w[c * 8 + k];
-    v.b_out = alloc(1024);
-    for (int c = 0; c < 1024; ++c) pack[v.b_out + c] = out_b[c];
-    (void)h;
+        for (int k = 0; k < 8; ++k) P.pack[v.w_out + (size_t)k * 1024 + c] = out_w[c * 8 + k];
+    v.b_out = P.alloc(1024);
+    for (int c = 0; c < 1024; ++c) P.pack[v.b_out + c] = out_b[c];
     return v;
 }
 
-VqW pack_vq(fac_handle* h, int m, const std::string& prefix) {
+VqW pack_vq(Packer& P, const TensorMap& ts, const std::string& prefix) {
     std::vector<int64_t> s1, s2;
-    std::vector<float> win = folded_weight(h, m, prefix + ".in_proj", s1);
-    std::vector<float> wout = folded_weight(h, m, prefix + ".out_proj", s2);
+    std::vector<float> win = folded_weight(ts, prefix + ".in_proj", s1);
+    std::vector<float> wout = folded_weight(ts, prefix + ".out_proj", s2);
     if (s1[0] != 8 || s1[1] != 1024 || s2[0] != 1024 || s2[1] != 8) throw PackError{"VQ shape at " + prefix};
-    const HostTensor& bi = need(h, m, prefix + ".in_proj.bias");
-    const HostTensor& bo = need(h, m, prefix + ".out_proj.bias");
-    const HostTensor& cb = need(h, m, prefix + ".codebook.weight");
+    const HostTensor& bi = need(ts, prefix + ".in_proj.bias");
+    const HostTensor& bo = need(ts, prefix + ".out_proj.bias");
+    const HostTensor& cb = need(ts, prefix + ".codebook.weight");
     if (cb.shape[0] != 1024 || cb.shape[1] != 8) throw PackError{"codebook shape at " + prefix};
-    return pack_vq_raw(h->pack, win.data(), bi.data.data(), wout.data(), bo.data.data(), cb.data.data());
+    return pack_vq_raw(P, win.data(), bi.data.data(), wout.data(), bo.data.data(), cb.data.data());
 }
 
-void pack_encoder(fac_handle* h) {
-    EncW& e = h->enc;
-    const int m = FAC_ENCODER;
+void pack_encoder(Packer& P, const TensorMap& ts, EncW& e) {
     const int rates[4] = {2, 5, 5, 6};
-    e.conv0 = pack_conv(h, m, "block.0.conv.conv");
+    e.conv0 = pack_conv(P, ts, "block.0.conv.conv");
     for (int i = 0; i < 4; ++i) {
         std::string p = "block." + std::to_string(i + 1);
         const int dils[3] = {1, 3, 9};
-        for (int j = 0; j < 3; ++j) e.blk[i].res[j] = pack_res(h, m, p + ".block." + std::to_string(j), dils[j], true);
-        e.blk[i].snake = pack_snake(h, m, p + ".block.3.alpha");
-        e.blk[i].down = pack_conv(h, m, p + ".block.4.conv.conv", rates[i], true);
+        for (int j = 0; j < 3; ++j) e.blk[i].res[j] = pack_res(P, ts, p + ".block." + std::to_string(j), dils[j], true);
+        e.blk[i].snake = pack_snake(P, ts, p + ".block.3.alpha");
+        e.blk[i].down = pack_conv(P, ts, p + ".block.4.conv.conv", rates[i], true);
         e.blk[i].stride = rates[i];
         if (e.blk[i].down.K != 2 * rates[i]) throw PackError{"encoder stride/kernel mismatch"};
     }
-    e.lstm = pack_lstm(h, m, "block.5.lstm", true);
-    e.snake = pack_snake(h, m, "block.6.alpha");
-    e.conv_out = pack_conv(h, m, "block.7.conv.conv", 1, true);
+    e.lstm = pack_lstm(P, ts, "block.5.lstm", true);
+    e.snake = pack_snake(P, ts, "block.6.alpha");
+    e.conv_out = pack_conv(P, ts, "block.7.conv.conv", 1, true);
 }
 
-void pack_decoder_into(fac_handle* h, int m, DecW& d, bool lstm, bool causal) {
+void pack_decoder(Packer& P, const TensorMap& ts, DecW& d, bool lstm, bool causal) {
     const int rates[4] = {6, 5, 5, 2};
     d.causal = causal; d.has_lstm = lstm;
     // The two layers with the longest chains outside the ResidualUnits (conv0: 1024 x 7 products per output, block 1's
     // up-conv: 1536 x 2) take the promoted packing: on conv_tc_kernel's bf16 hi/lo class the truncating tensor-core
     // accumulation over such a chain reaches 2.4-6x the error of the class's operand rounding
     // (tests/test_gpu_codec_stages.py).  Later up-convs (<= 768 x 2) stay within it; the units keep their classes.
-    d.conv0 = pack_conv(h, m, "model.0.conv.conv", 1, true);
+    d.conv0 = pack_conv(P, ts, "model.0.conv.conv", 1, true);
     int base = 1;
-    if (lstm) { d.lstm = pack_lstm(h, m, "model.1.lstm"); base = 2; }
+    if (lstm) { d.lstm = pack_lstm(P, ts, "model.1.lstm"); base = 2; }
     for (int i = 0; i < 4; ++i) {
         std::string p = "model." + std::to_string(i + base);
-        d.blk[i].snake = pack_snake(h, m, p + ".block.0.alpha");
+        d.blk[i].snake = pack_snake(P, ts, p + ".block.0.alpha");
         const bool long_chain = i == 0;
-        d.blk[i].up = causal ? pack_convtr(h, m, p + ".block.1.convtr.convtr", rates[i], long_chain)
-                             : pack_convtr_noncausal(h, m, p + ".block.1.convtr.convtr", rates[i], long_chain);
+        d.blk[i].up = causal ? pack_convtr(P, ts, p + ".block.1.convtr.convtr", rates[i], long_chain)
+                             : pack_convtr_noncausal(P, ts, p + ".block.1.convtr.convtr", rates[i], long_chain);
         d.blk[i].stride = rates[i];
         d.blk[i].cout = d.blk[i].up.Cout / rates[i];
         const int dils[3] = {1, 3, 9};
-        for (int j = 0; j < 3; ++j) d.blk[i].res[j] = pack_res(h, m, p + ".block." + std::to_string(j + 2), dils[j]);
+        for (int j = 0; j < 3; ++j) d.blk[i].res[j] = pack_res(P, ts, p + ".block." + std::to_string(j + 2), dils[j]);
     }
-    d.snake = pack_snake(h, m, "model." + std::to_string(4 + base) + ".alpha");
-    d.conv_out = pack_conv(h, m, "model." + std::to_string(5 + base) + ".conv.conv");
+    d.snake = pack_snake(P, ts, "model." + std::to_string(4 + base) + ".alpha");
+    d.conv_out = pack_conv(P, ts, "model." + std::to_string(5 + base) + ".conv.conv");
 }
 
-void pack_decoder(fac_handle* h) { pack_decoder_into(h, FAC_DECODER, h->dec, true, true); }
-
 // modules/redecoder.py:5-21 (encoder_type "wavenet"); key names of modules/wavenet.py:103-136 under "encoder."
-void pack_redecoder(fac_handle* h) {
-    RedW& r = h->red;
-    const int m = FAC_REDECODER;
+void pack_redecoder(Packer& P, const TensorMap& ts, RedW& r) {
     auto emb = [&](const std::string& key) {
-        const HostTensor& t = need(h, m, key);
+        const HostTensor& t = need(ts, key);
         if (t.shape.size() != 2 || t.shape[0] != 1024 || t.shape[1] != r.hidden) throw PackError{"embedding shape at " + key};
-        size_t off = pack_alloc(h, t.numel());
-        for (size_t i = 0; i < t.numel(); ++i) h->pack[off + i] = t.data[i];
+        size_t off = P.alloc(t.numel());
+        for (size_t i = 0; i < t.numel(); ++i) P.pack[off + i] = t.data[i];
         return off;
     };
     r.emb_p = emb("prosody_embed.0.weight");
     r.emb_c[0] = emb("content_embed.0.weight");
     r.emb_c[1] = emb("content_embed.1.weight");
-    r.cond = pack_conv(h, m, "encoder.cond_layer.conv.conv");
+    r.cond = pack_conv(P, ts, "encoder.cond_layer.conv.conv");
     for (int i = 0; i < r.layers; ++i) {
-        r.wn_in[i] = pack_conv(h, m, "encoder.in_layers." + std::to_string(i) + ".conv.conv");
-        r.wn_rs[i] = pack_conv(h, m, "encoder.res_skip_layers." + std::to_string(i) + ".conv.conv");
+        r.wn_in[i] = pack_conv(P, ts, "encoder.in_layers." + std::to_string(i) + ".conv.conv");
+        r.wn_rs[i] = pack_conv(P, ts, "encoder.res_skip_layers." + std::to_string(i) + ".conv.conv");
     }
-    r.conv_out = pack_conv(h, m, "conv_out");
+    r.conv_out = pack_conv(P, ts, "conv_out");
     if (r.cond.Cin != LATENT || r.cond.Cout != 2 * r.hidden * r.layers || r.wn_in[0].K != 5 || r.conv_out.Cout != LATENT)
         throw PackError{"redecoder geometry (expects WN(512, kernel 5, 16 layers, gin 1024))"};
 }
 
-// The mel front-end's constants: [1200][2*1025] windowed DFT basis (fp64 -> fp32), its tensor-core variant, the filterbank.
-void pack_mel_frontend(fac_handle* h, ConvW& dft, ConvW& dft_tc, size_t& fb_off, const float* win, const float* fb) {
-    dft.Cin = 1; dft.Cout = 2 * N_BINS; dft.K = WIN; dft.ldw = SPEC_LD;
-    dft.w = pack_alloc(h, (size_t)WIN * SPEC_LD);
-    dft.b = 0;
-    const int left = (N_FFT - WIN) / 2;
-    for (int n = 0; n < WIN; ++n)
-        for (int k = 0; k < N_BINS; ++k) {
-            // reduce the phase index mod N_FFT in integers so the fp64 angle stays small
-            long long ph = ((long long)k * (n + left)) % N_FFT;
-            double ang = 2.0 * M_PI * (double)ph / (double)N_FFT;
-            h->pack[dft.w + (size_t)n * SPEC_LD + 2 * k] = (float)((double)win[n] * std::cos(ang));
-            h->pack[dft.w + (size_t)n * SPEC_LD + 2 * k + 1] = (float)(-(double)win[n] * std::sin(ang));
-        }
-    // tensor-core variant: [1200][2176] with zero columns beyond 2*1025, zero bias
-    dft_tc.Cin = WIN; dft_tc.Cout = SPEC_TC_LD; dft_tc.K = 1; dft_tc.ldw = SPEC_TC_LD;
-    dft_tc.w = pack_alloc(h, (size_t)WIN * SPEC_TC_LD);
-    for (int n = 0; n < WIN; ++n)
-        for (int k = 0; k < 2 * N_BINS; ++k) h->pack[dft_tc.w + (size_t)n * SPEC_TC_LD + k] = h->pack[dft.w + (size_t)n * SPEC_LD + k];
-    dft_tc.b = pack_alloc(h, SPEC_TC_LD);
-    attach_tc(h, dft_tc, 1, true);
-    fb_off = pack_alloc(h, (size_t)N_BINS * N_MELS);
-    for (size_t i = 0; i < (size_t)N_BINS * N_MELS; ++i) h->pack[fb_off + i] = fb[i];
+// Periodic Hann window of n samples (torch.hann_window, scipy.signal.get_window("hann")), fp64.
+std::vector<double> periodic_hann(int n) {
+    std::vector<double> w(n);
+    for (int i = 0; i < n; ++i) w[i] = 0.5 - 0.5 * std::cos(2.0 * M_PI * (double)i / (double)n);
+    return w;
 }
 
-void pack_quantizer(fac_handle* h) {
-    QuantW& q = h->qw;
-    const int m = FAC_QUANTIZER;
-    q.vq[0] = pack_vq(h, m, "prosody_quantizer.quantizers.0");
-    q.vq[1] = pack_vq(h, m, "content_quantizer.quantizers.0");
-    q.vq[2] = pack_vq(h, m, "content_quantizer.quantizers.1");
-    for (int i = 0; i < 3; ++i) q.vq[3 + i] = pack_vq(h, m, "residual_quantizer.quantizers." + std::to_string(i));
-    q.spec0 = pack_conv(h, m, "timbre_encoder.spectral.0", 1, true);
-    q.spec3 = pack_conv(h, m, "timbre_encoder.spectral.3", 1, true);
-    q.glu[0] = pack_conv(h, m, "timbre_encoder.temporal.0.conv1", 1, true);
-    q.glu[1] = pack_conv(h, m, "timbre_encoder.temporal.1.conv1", 1, true);
-    q.cq = pack_conv(h, m, "timbre_encoder.slf_attn.conv_q", 1, true);
-    q.ck = pack_conv(h, m, "timbre_encoder.slf_attn.conv_k", 1, true);
-    q.cv = pack_conv(h, m, "timbre_encoder.slf_attn.conv_v", 1, true);
-    q.co = pack_conv(h, m, "timbre_encoder.slf_attn.conv_o", 1, true);
-    q.fc = pack_conv(h, m, "timbre_encoder.fc", 1, true);
-    q.timbre_linear = pack_conv(h, m, "timbre_linear", 1, true);
-    q.mel_lin = pack_conv(h, m, "melspec_linear.conv.conv");
-    for (int i = 0; i < 8; ++i) {
-        q.wn_in[i] = pack_conv(h, m, "melspec_encoder.in_layers." + std::to_string(i) + ".conv.conv", 1, true);
-        q.wn_rs[i] = pack_conv(h, m, "melspec_encoder.res_skip_layers." + std::to_string(i) + ".conv.conv", 1, true);
+// Window-folded real DFT basis: row n of dst (stride ld) holds win[n] (cos, -sin)(2 pi k (n + left) / n_fft) for k < nb,
+// interleaved (fp64, rounded once to fp32).
+void dft_basis(float* dst, size_t ld, const std::vector<double>& win, int n_fft, int nb, int left) {
+    for (int n = 0; n < (int)win.size(); ++n)
+        for (int k = 0; k < nb; ++k) {
+            // reduce the phase index mod n_fft in integers so the fp64 angle stays small
+            const long long ph = ((long long)k * (n + left)) % n_fft;
+            const double ang = 2.0 * M_PI * (double)ph / (double)n_fft;
+            dst[(size_t)n * ld + 2 * k] = (float)(win[n] * std::cos(ang));
+            dst[(size_t)n * ld + 2 * k + 1] = (float)(-win[n] * std::sin(ang));
+        }
+}
+
+// torchaudio.functional.melscale_fbanks(n_bins, f_min = 0, f_max, n_mels, sample_rate = 2 f_max, norm = None, "htk"):
+// [n_bins][n_mels]
+std::vector<float> htk_fbank(double f_max, int n_bins, int n_mels) {
+    auto hz2mel = [](double f) { return 2595.0 * std::log10(1.0 + f / 700.0); };
+    auto mel2hz = [](double m) { return 700.0 * (std::pow(10.0, m / 2595.0) - 1.0); };
+    std::vector<double> fpts(n_mels + 2);
+    for (int i = 0; i < n_mels + 2; ++i) fpts[i] = mel2hz(hz2mel(0.0) + (hz2mel(f_max) - hz2mel(0.0)) * i / (n_mels + 1));
+    std::vector<float> fb((size_t)n_bins * n_mels);
+    for (int k = 0; k < n_bins; ++k) {
+        const double f = f_max * k / (n_bins - 1);
+        for (int m = 0; m < n_mels; ++m) {
+            const double down = (f - fpts[m]) / (fpts[m + 1] - fpts[m]), up = (fpts[m + 2] - f) / (fpts[m + 2] - fpts[m + 1]);
+            fb[(size_t)k * n_mels + m] = (float)std::max(0.0, std::min(down, up));
+        }
     }
-    q.mel_lin2 = pack_conv(h, m, "melspec_linear2.conv.conv", 1, true);
+    return fb;
+}
+
+// The mel front-end's constants: [1200][2*1025] windowed DFT basis (fp64 -> fp32), its tensor-core variant, the filterbank.
+void pack_mel_frontend(Packer& P, ConvW& dft, ConvW& dft_tc, size_t& fb_off, const float* win, const float* fb) {
+    dft.Cin = 1; dft.Cout = 2 * N_BINS; dft.K = WIN; dft.ldw = SPEC_LD;
+    dft.w = P.alloc((size_t)WIN * SPEC_LD);
+    dft.b = 0;
+    dft_basis(P.pack.data() + dft.w, SPEC_LD, std::vector<double>(win, win + WIN), N_FFT, N_BINS, (N_FFT - WIN) / 2);
+    // tensor-core variant: [1200][2176] with zero columns beyond 2*1025, zero bias
+    dft_tc.Cin = WIN; dft_tc.Cout = SPEC_TC_LD; dft_tc.K = 1; dft_tc.ldw = SPEC_TC_LD;
+    dft_tc.w = P.alloc((size_t)WIN * SPEC_TC_LD);
+    for (int n = 0; n < WIN; ++n)
+        for (int k = 0; k < 2 * N_BINS; ++k) P.pack[dft_tc.w + (size_t)n * SPEC_TC_LD + k] = P.pack[dft.w + (size_t)n * SPEC_LD + k];
+    dft_tc.b = P.alloc(SPEC_TC_LD);
+    attach_tc(P, dft_tc, 1, true);
+    fb_off = P.alloc((size_t)N_BINS * N_MELS);
+    for (size_t i = 0; i < (size_t)N_BINS * N_MELS; ++i) P.pack[fb_off + i] = fb[i];
+}
+
+void pack_quantizer(Packer& P, const TensorMap& ts, QuantW& q) {
+    q.vq[0] = pack_vq(P, ts, "prosody_quantizer.quantizers.0");
+    q.vq[1] = pack_vq(P, ts, "content_quantizer.quantizers.0");
+    q.vq[2] = pack_vq(P, ts, "content_quantizer.quantizers.1");
+    for (int i = 0; i < 3; ++i) q.vq[3 + i] = pack_vq(P, ts, "residual_quantizer.quantizers." + std::to_string(i));
+    q.spec0 = pack_conv(P, ts, "timbre_encoder.spectral.0", 1, true);
+    q.spec3 = pack_conv(P, ts, "timbre_encoder.spectral.3", 1, true);
+    q.glu[0] = pack_conv(P, ts, "timbre_encoder.temporal.0.conv1", 1, true);
+    q.glu[1] = pack_conv(P, ts, "timbre_encoder.temporal.1.conv1", 1, true);
+    q.cq = pack_conv(P, ts, "timbre_encoder.slf_attn.conv_q", 1, true);
+    q.ck = pack_conv(P, ts, "timbre_encoder.slf_attn.conv_k", 1, true);
+    q.cv = pack_conv(P, ts, "timbre_encoder.slf_attn.conv_v", 1, true);
+    q.co = pack_conv(P, ts, "timbre_encoder.slf_attn.conv_o", 1, true);
+    q.fc = pack_conv(P, ts, "timbre_encoder.fc", 1, true);
+    q.timbre_linear = pack_conv(P, ts, "timbre_linear", 1, true);
+    q.mel_lin = pack_conv(P, ts, "melspec_linear.conv.conv");
+    for (int i = 0; i < 8; ++i) {
+        q.wn_in[i] = pack_conv(P, ts, "melspec_encoder.in_layers." + std::to_string(i) + ".conv.conv", 1, true);
+        q.wn_rs[i] = pack_conv(P, ts, "melspec_encoder.res_skip_layers." + std::to_string(i) + ".conv.conv", 1, true);
+    }
+    q.mel_lin2 = pack_conv(P, ts, "melspec_linear2.conv.conv", 1, true);
     // STFT basis with the Hann window folded in: frame sample n+424 of the zero-padded window
-    const HostTensor& win = need(h, m, "to_mel.spectrogram.window");
-    const HostTensor& fb = need(h, m, "to_mel.mel_scale.fb");
+    const HostTensor& win = need(ts, "to_mel.spectrogram.window");
+    const HostTensor& fb = need(ts, "to_mel.mel_scale.fb");
     if ((int)win.numel() != WIN || fb.shape[0] != N_BINS || fb.shape[1] != N_MELS) throw PackError{"mel buffers shape"};
-    pack_mel_frontend(h, q.dft, q.dft_tc, q.fb, win.data.data(), fb.data.data());
+    pack_mel_frontend(P, q.dft, q.dft_tc, q.fb, win.data.data(), fb.data.data());
 }
 
 // ------------------------------------------------------------------------------------------
@@ -675,6 +695,7 @@ struct Ctx {
     fac_handle* h;
     cudaStream_t st;
     bool dry;          // size pass: allocate only
+    const float* wbase = nullptr;   // the weight arena W() reads
     bool vq_critical = false;   // inside the encoder / prosody branch: feeds the bit-exact VQ argmin
     size_t off = 0;
     cudaError_t cerr = cudaSuccess;
@@ -683,11 +704,11 @@ struct Ctx {
     template <typename T>
     T* alloc(size_t n) {
         size_t bytes = (n * sizeof(T) + 255) / 256 * 256;
-        char* p = h->ws ? h->ws + off : nullptr;
+        char* p = h->ws ? h->ws.get() + off : nullptr;
         off += bytes;
         return reinterpret_cast<T*>(p);
     }
-    const float* W(size_t o) const { return h->warena + o; }
+    const float* W(size_t o) const { return wbase + o; }
     bool ok() const { return cerr == cudaSuccess; }
     void check(cudaError_t e, const char* w) {     // a kernel launch
         if (!dry) h->launches++;
@@ -1510,23 +1531,57 @@ void join_front(Ctx& c) {
 
 int ensure_ws(fac_handle* h, size_t bytes) {
     if (bytes <= h->ws_bytes) return FAC_OK;
-    if (h->ws) { cudaDeviceSynchronize(); cudaFree(h->ws); h->ws = nullptr; h->ws_bytes = 0; }
+    if (h->ws) { cudaDeviceSynchronize(); h->ws.reset(); h->ws_bytes = 0; }
     size_t want = bytes + (bytes >> 4) + (1 << 20);
-    cudaError_t e = cudaMalloc(&h->ws, want);
+    char* p = nullptr;
+    cudaError_t e = cudaMalloc(&p, want);
     if (e != cudaSuccess) {
         h->err = std::string("workspace cudaMalloc failed: ") + cudaGetErrorString(e);
         cudaGetLastError();
         return FAC_ERR_CUDA;
     }
+    h->ws.reset(p);
     h->ws_bytes = want;
     return FAC_OK;
 }
+
+// Copies `host` to a new device buffer that replaces `dst` (`slack` more elements allocated past the end, left unset).  A
+// previous buffer is dropped only once the device is idle: kernels in flight may still read it.  On failure dst is empty.
+template <typename T>
+int upload(fac_handle* h, const std::vector<T>& host, DevBuf<T>& dst, const char* who, size_t slack = 0) {
+    cudaError_t e = cudaSetDevice(h->device);
+    if (e == cudaSuccess && dst) { cudaDeviceSynchronize(); dst.reset(); }
+    T* p = nullptr;
+    if (e == cudaSuccess) e = cudaMalloc(&p, (host.size() + slack) * sizeof(T));
+    if (e == cudaSuccess) dst.reset(p);
+    if (e == cudaSuccess) e = cudaMemcpy(p, host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        dst.reset();
+        h->err = std::string(who) + ": " + cudaGetErrorString(e);
+        cudaGetLastError();
+        return FAC_ERR_CUDA;
+    }
+    return FAC_OK;
+}
+
+// A weight arena: the packed floats and 64 floats of slack.
+int upload_weights(fac_handle* h, const Packer& P, DevBuf<float>& dst, const char* who) { return upload(h, P.pack, dst, who, 64); }
 
 int finish(fac_handle* h, Ctx& c) {
     if (c.cerr != cudaSuccess) {
         h->err = std::string("CUDA error at ") + c.where + ": " + cudaGetErrorString(c.cerr);
         return FAC_ERR_CUDA;
     }
+    return FAC_OK;
+}
+
+// Stages one C-ABI tensor (HOST data, 0 <= ndim <= 4 non-negative dimensions) as ts[key].
+int stage_tensor(TensorMap& ts, const char* key, const float* data, const int64_t* shape, int ndim) {
+    if (!key || !data || ndim < 0 || ndim > 4) return FAC_ERR_INVALID;
+    HostTensor t;
+    for (int i = 0; i < ndim; ++i) { if (shape[i] < 0) return FAC_ERR_INVALID; t.shape.push_back(shape[i]); }
+    t.data.assign(data, data + t.numel());
+    ts[key] = std::move(t);
     return FAC_OK;
 }
 
@@ -1540,7 +1595,7 @@ uint64_t fnv1a(const void* p, size_t n, uint64_t h = 14695981039346656037ull) {
 // A module's weight fingerprint: every key, shape and float of its host tensors in key order, the floats as raw words over
 // four interleaved FNV-style lanes (a byte-wise hash of ~100 M floats would add seconds to fac_finalize).  Not a secure hash:
 // it tells apart weights, not adversaries.
-uint64_t weights_fingerprint(const std::map<std::string, HostTensor>& m) {
+uint64_t weights_fingerprint(const TensorMap& m) {
     uint64_t h = fnv1a("facodec_b200 weights", 20);
     for (const auto& kv : m) {
         h = fnv1a(kv.first.c_str(), kv.first.size() + 1, h);
@@ -1561,20 +1616,23 @@ uint64_t weights_fingerprint(const std::map<std::string, HostTensor>& m) {
     return h;
 }
 
-// run `body` twice: size pass, then for real
+// run `body` twice: size pass, then for real, reading the weights of arena `weights`
 template <typename F>
-int two_pass(fac_handle* h, cudaStream_t st, F body) {
+int two_pass(fac_handle* h, cudaStream_t st, const float* weights, F body) {
     cudaError_t e = cudaSetDevice(h->device);
     if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return FAC_ERR_CUDA; }
-    Ctx dry{h, st, true};
+    Ctx dry{h, st, true, weights};
     body(dry);
     int rc = ensure_ws(h, dry.off);
     if (rc != FAC_OK) return rc;
     h->launches = 0;
-    Ctx c{h, st, false};
+    Ctx c{h, st, false, weights};
     body(c);
     return finish(h, c);
 }
+// ... with the codec's own weights
+template <typename F>
+int two_pass(fac_handle* h, cudaStream_t st, F body) { return two_pass(h, st, h->warena.get(), body); }
 
 }  // namespace
 
@@ -1600,59 +1658,39 @@ int fac_destroy(fac_handle* h) {
     if (!h) return FAC_OK;
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
-    if (h->warena) cudaFree(h->warena);
-    if (h->ws) cudaFree(h->ws);
     if (h->side) cudaStreamDestroy(h->side);
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
     if (h->ev_join) cudaEventDestroy(h->ev_join);
-    if (h->aa_filter) cudaFree(h->aa_filter);
-    if (h->mel16_arena) cudaFree(h->mel16_arena);
-    if (h->loss_arena) cudaFree(h->loss_arena);
-    if (h->spec_arena) cudaFree(h->spec_arena);
-    for (float* p : h->rvq_arenas) if (p) cudaFree(p);
-    for (auto* hs : h->heads) { if (hs->arena) cudaFree(hs->arena); delete hs; }
-    for (auto* js : h->jdcs) { if (js->arena) cudaFree(js->arena); delete js; }
     fac::rs_host_free(h->rs);
-    delete h;   // and with it the streams' and pools' device state
+    delete h;   // and with it every arena, the workspace, the weight sets' and the streams' and pools' device state
     return FAC_OK;
 }
 
 const char* fac_last_error(const fac_handle* h) { return h ? h->err.c_str() : "null handle"; }
 
 int fac_load_tensor(fac_handle* h, int module, const char* key, const float* data_host, const int64_t* shape, int ndim) {
-    if (!h || !key || !data_host || module < 0 || module >= FAC_NUM_MODULES || ndim < 0 || ndim > 4) return FAC_ERR_INVALID;
-    HostTensor t;
-    size_t n = 1;
-    for (int i = 0; i < ndim; ++i) { if (shape[i] < 0) return FAC_ERR_INVALID; t.shape.push_back(shape[i]); n *= (size_t)shape[i]; }
-    t.data.assign(data_host, data_host + n);
-    h->host[module][key] = std::move(t);
-    h->have[module] = true;
-    h->finalized = false;
-    return FAC_OK;
+    if (!h || module < 0 || module >= FAC_NUM_MODULES) return FAC_ERR_INVALID;
+    const int rc = stage_tensor(h->host[module], key, data_host, shape, ndim);
+    if (rc == FAC_OK) { h->have[module] = true; h->finalized = false; }
+    return rc;
 }
 
 int fac_finalize(fac_handle* h) {
     if (!h) return FAC_ERR_INVALID;
-    h->pack.clear();
-    h->pack.reserve(160u << 20);
+    Packer P;
+    P.pack.reserve(160u << 20);
     try {
-        if (h->have[FAC_ENCODER]) pack_encoder(h);
-        if (h->have[FAC_QUANTIZER]) pack_quantizer(h);
-        if (h->have[FAC_DECODER]) pack_decoder(h);
-        if (h->have[FAC_REDECODER]) pack_redecoder(h);
-        if (h->have[FAC_REDECODER_DECODER]) pack_decoder_into(h, FAC_REDECODER_DECODER, h->dec2, false, false);
+        if (h->have[FAC_ENCODER]) pack_encoder(P, h->host[FAC_ENCODER], h->enc);
+        if (h->have[FAC_QUANTIZER]) pack_quantizer(P, h->host[FAC_QUANTIZER], h->qw);
+        if (h->have[FAC_DECODER]) pack_decoder(P, h->host[FAC_DECODER], h->dec, true, true);
+        if (h->have[FAC_REDECODER]) pack_redecoder(P, h->host[FAC_REDECODER], h->red);
+        if (h->have[FAC_REDECODER_DECODER]) pack_decoder(P, h->host[FAC_REDECODER_DECODER], h->dec2, false, false);
     } catch (const PackError& e) {
         h->err = e.msg;
         return FAC_ERR_STATE;
     }
-    cudaError_t e = cudaSetDevice(h->device);
-    if (e == cudaSuccess && h->warena) { cudaDeviceSynchronize(); cudaFree(h->warena); h->warena = nullptr; }
-    size_t n = h->pack.size() + 64;
-    if (e == cudaSuccess) e = cudaMalloc(&h->warena, n * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(h->warena, h->pack.data(), h->pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = std::string("weight upload: ") + cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
-    h->wfloats = n;
-    h->pack.clear(); h->pack.shrink_to_fit();
+    const int rc = upload_weights(h, P, h->warena, "weight upload");
+    if (rc != FAC_OK) return rc;
     for (int m = 0; m < FAC_NUM_MODULES; ++m) h->fp[m] = h->have[m] ? weights_fingerprint(h->host[m]) : 0;
     for (int m = 0; m < FAC_NUM_MODULES; ++m) h->host[m].clear();
     h->finalized = true;
@@ -3833,43 +3871,22 @@ long long fac_debug_lstm_lane_map(int H, int pass3, int lane, long long* pos, lo
 int fac_dataset_mel(fac_handle* h, const float* wave, int B, int T, float* mel, void* stream) {
     if (!h || !wave || !mel || B <= 0) return FAC_ERR_INVALID;
     if (T <= N_FFT / 2) { h->err = "fac_dataset_mel: wave shorter than the STFT reflect padding (1024), as torch.stft"; return FAC_ERR_INVALID; }
-    cudaSetDevice(h->device);
     if (!h->mel16_arena) {
-        fac_handle tmp;
-        tmp.device = h->device;
-        std::vector<float> win(WIN), fb((size_t)N_BINS * N_MELS);
-        for (int i = 0; i < WIN; ++i) win[i] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * (double)i / (double)WIN));   // periodic Hann
-        // torchaudio.functional.melscale_fbanks(n_freqs=1025, f_min=0, f_max=8000, n_mels=80, sample_rate=16000, norm=None, "htk")
-        const double sr = 16000.0, f_max = 8000.0;
-        auto hz2mel = [](double f) { return 2595.0 * std::log10(1.0 + f / 700.0); };
-        auto mel2hz = [](double m) { return 700.0 * (std::pow(10.0, m / 2595.0) - 1.0); };
-        std::vector<double> fpts(N_MELS + 2);
-        for (int i = 0; i < N_MELS + 2; ++i) fpts[i] = mel2hz(hz2mel(0.0) + (hz2mel(f_max) - hz2mel(0.0)) * i / (N_MELS + 1));
-        for (int k = 0; k < N_BINS; ++k) {
-            const double f = (sr / 2.0) * k / (N_BINS - 1);
-            for (int m = 0; m < N_MELS; ++m) {
-                const double down = (f - fpts[m]) / (fpts[m + 1] - fpts[m]), up = (fpts[m + 2] - f) / (fpts[m + 2] - fpts[m + 1]);
-                fb[(size_t)k * N_MELS + m] = (float)std::max(0.0, std::min(down, up));
-            }
-        }
-        try { pack_mel_frontend(&tmp, h->mel16_dft, h->mel16_dft_tc, h->mel16_fb, win.data(), fb.data()); }
-        catch (const PackError& e) { h->err = e.msg; return FAC_ERR_STATE; }
-        cudaError_t e = cudaMalloc(&h->mel16_arena, (tmp.pack.size() + 64) * sizeof(float));
-        if (e == cudaSuccess) e = cudaMemcpy(h->mel16_arena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); h->mel16_arena = nullptr; return FAC_ERR_CUDA; }
+        const std::vector<double> hann = periodic_hann(WIN);
+        const std::vector<float> win(hann.begin(), hann.end());
+        Packer P;
+        pack_mel_frontend(P, h->mel16_dft, h->mel16_dft_tc, h->mel16_fb, win.data(), htk_fbank(8000.0, N_BINS, N_MELS).data());
+        const int rc = upload_weights(h, P, h->mel16_arena, "fac_dataset_mel");
+        if (rc != FAC_OK) return rc;
     }
-    float* saved = h->warena;
-    h->warena = h->mel16_arena;
     const int F = T / HOP + 1;
-    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    return two_pass(h, (cudaStream_t)stream, h->mel16_arena.get(), [&](Ctx& c) {
         MelW mw{&h->mel16_dft, &h->mel16_dft_tc, h->mel16_fb};
         c.vq_critical = true;                        // fp32-faithful DFT (the promoted tensor-core kernel)
         float* mel_cl = mel_forward(c, wave, B, T, F, &mw);
         c.vq_critical = false;
         if (!c.dry) c.check(launch_transpose(mel_cl, mel, B, F, N_MELS, c.st), "mel16.T");
     });
-    h->warena = saved;
-    return rc;
 }
 
 // ---- losses.py:65-89 reconstruction_loss (SURVEY.md 8f rank 3: the loss forward of the training step) ----
@@ -3882,54 +3899,27 @@ int fac_reconstruction_loss(fac_handle* h, const float* x, const float* gx, int 
     if (!h || !x || !gx || !loss || B <= 0 || T <= 0) return FAC_ERR_INVALID;
     if (T <= 1024) { h->err = "fac_reconstruction_loss: signals must be longer than the largest STFT reflect padding (1024), as torch.stft"; return FAC_ERR_INVALID; }
     if (B > 32767) { h->err = "fac_reconstruction_loss: B > 32767"; return FAC_ERR_UNSUPPORTED; }
-    cudaSetDevice(h->device);
     if (!h->loss_arena) {
-        fac_handle tmp;
-        tmp.device = h->device;
-        const int NM = 64;
-        auto hz2mel = [](double f) { return 2595.0 * std::log10(1.0 + f / 700.0); };
-        auto mel2hz = [](double m) { return 700.0 * (std::pow(10.0, m / 2595.0) - 1.0); };
-        std::vector<double> fpts(NM + 2);
-        for (int i = 0; i < NM + 2; ++i) fpts[i] = mel2hz(hz2mel(0.0) + (hz2mel(8000.0) - hz2mel(0.0)) * i / (NM + 1));
-        try {
-            for (int i = 0; i < 6; ++i) {
-                fac_handle::LossScale& L = h->loss_scale[i];
-                L.s = 64 << i; L.nfft = L.s < 512 ? 512 : L.s; L.nb = L.nfft / 2 + 1;
-                L.ld = (2 * L.nb + 127) / 128 * 128;            // zero columns beyond 2 * nb: whole 128-channel MMA tiles
-                ConvW& d = L.dft;
-                d = ConvW();
-                d.Cin = L.s; d.Cout = L.ld; d.K = 1; d.ldw = L.ld;
-                d.w = pack_alloc(&tmp, (size_t)L.s * L.ld);
-                d.b = pack_alloc(&tmp, L.ld);
-                const int left = (L.nfft - L.s) / 2;
-                for (int n = 0; n < L.s; ++n) {
-                    const double w = 0.5 - 0.5 * std::cos(2.0 * M_PI * (double)n / (double)L.s);       // periodic Hann(s)
-                    for (int k = 0; k < L.nb; ++k) {
-                        const long long ph = ((long long)k * (n + left)) % L.nfft;
-                        const double ang = 2.0 * M_PI * (double)ph / (double)L.nfft;
-                        tmp.pack[d.w + (size_t)n * L.ld + 2 * k] = (float)(w * std::cos(ang));
-                        tmp.pack[d.w + (size_t)n * L.ld + 2 * k + 1] = (float)(-w * std::sin(ang));
-                    }
-                }
-                attach_tc(&tmp, d, 1, true);
-                // torchaudio.functional.melscale_fbanks(n_freqs, 0, 8000, 64, sample_rate=16000, norm=None, "htk")
-                L.fb = pack_alloc(&tmp, (size_t)L.nb * NM);
-                for (int k = 0; k < L.nb; ++k) {
-                    const double f = 8000.0 * k / (L.nb - 1);
-                    for (int m = 0; m < NM; ++m) {
-                        const double down = (f - fpts[m]) / (fpts[m + 1] - fpts[m]), up = (fpts[m + 2] - f) / (fpts[m + 2] - fpts[m + 1]);
-                        tmp.pack[L.fb + (size_t)k * NM + m] = (float)std::max(0.0, std::min(down, up));
-                    }
-                }
-            }
-        } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_STATE; }
-        cudaError_t e = cudaMalloc(&h->loss_arena, (tmp.pack.size() + 64) * sizeof(float));
-        if (e == cudaSuccess) e = cudaMemcpy(h->loss_arena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); h->loss_arena = nullptr; return FAC_ERR_CUDA; }
+        Packer P;
+        for (int i = 0; i < 6; ++i) {
+            fac_handle::LossScale& L = h->loss_scale[i];
+            L.s = 64 << i; L.nfft = L.s < 512 ? 512 : L.s; L.nb = L.nfft / 2 + 1;
+            L.ld = (2 * L.nb + 127) / 128 * 128;            // zero columns beyond 2 * nb: whole 128-channel MMA tiles
+            ConvW& d = L.dft;
+            d = ConvW();
+            d.Cin = L.s; d.Cout = L.ld; d.K = 1; d.ldw = L.ld;
+            d.w = P.alloc((size_t)L.s * L.ld);
+            d.b = P.alloc(L.ld);
+            dft_basis(P.pack.data() + d.w, L.ld, periodic_hann(L.s), L.nfft, L.nb, (L.nfft - L.s) / 2);
+            attach_tc(P, d, 1, true);
+            const std::vector<float> fb = htk_fbank(8000.0, L.nb, 64);
+            L.fb = P.alloc(fb.size());
+            std::copy(fb.begin(), fb.end(), P.pack.begin() + L.fb);
+        }
+        const int rc = upload_weights(h, P, h->loss_arena, "fac_reconstruction_loss");
+        if (rc != FAC_OK) return rc;
     }
-    float* saved = h->warena;
-    h->warena = h->loss_arena;
-    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    return two_pass(h, (cudaStream_t)stream, h->loss_arena.get(), [&](Ctx& c) {
         double* sums = c.alloc<double>(16);
         const int nblk = 1024;
         float* part = c.alloc<float>(nblk);
@@ -3969,8 +3959,6 @@ int fac_reconstruction_loss(fac_handle* h, const float* x, const float* gx, int 
         c.off = peak;
         if (!c.dry) c.check(launch_loss_combine(sums, loss, terms, c.st), "loss.combine");
     });
-    h->warena = saved;
-    return rc;
 }
 
 // ---- dac/nn/loss.py:142-327 MultiScaleSTFTLoss / MelSpectrogramLoss, :11-47 L1Loss (forward values) ----
@@ -4020,58 +4008,42 @@ static int spectral_loss(fac_handle* h, const float* x, const float* y, int B, i
         const double f1 = (n_mels && mel_fmax && mel_fmax[i] > 0.f) ? mel_fmax[i] : sample_rate / 2.0;
         key.push_back(w); key.push_back(nm); key.push_back(f0); key.push_back(f1);
     }
-    cudaSetDevice(h->device);
     if (!h->spec_arena || h->spec_key != key) {
-        fac_handle tmp;
-        tmp.device = h->device;
+        Packer P;
         std::vector<fac_handle::SpecScale> scales(n_scales);
-        try {
-            for (int i = 0; i < n_scales; ++i) {
-                fac_handle::SpecScale& L = scales[i];
-                L.w = window_lengths[i]; L.nb = L.w / 2 + 1; L.ld = (2 * L.nb + 127) / 128 * 128;
-                const int nm = (int)key[2 + 4 * i + 1];
-                L.mel = nm > 0; L.n_out = L.mel ? nm : L.nb;
-                ConvW& d = L.dft;
-                d = ConvW();
-                d.Cin = L.w; d.Cout = L.ld; d.K = 1; d.ldw = L.ld;
-                d.w = pack_alloc(&tmp, (size_t)L.w * L.ld);
-                d.b = pack_alloc(&tmp, L.ld);
-                for (int n = 0; n < L.w; ++n) {
-                    const double wv = 0.5 - 0.5 * std::cos(2.0 * M_PI * (double)n / (double)L.w);      // periodic Hann
-                    for (int k = 0; k < L.nb; ++k) {
-                        const long long ph = ((long long)k * n) % L.w;
-                        const double ang = 2.0 * M_PI * (double)ph / (double)L.w;
-                        tmp.pack[d.w + (size_t)n * L.ld + 2 * k] = (float)(wv * std::cos(ang));
-                        tmp.pack[d.w + (size_t)n * L.ld + 2 * k + 1] = (float)(-wv * std::sin(ang));
-                    }
-                }
-                attach_tc(&tmp, d, 1, true);
-                ConvW& dt = L.dftT;
-                dt = ConvW();
-                dt.Cin = L.ld; dt.Cout = L.w; dt.K = 1; dt.ldw = L.w;
-                dt.w = pack_alloc(&tmp, (size_t)L.ld * L.w);
-                dt.b = pack_alloc(&tmp, L.w);
-                for (int n = 0; n < L.w; ++n)
-                    for (int col = 0; col < 2 * L.nb; ++col) tmp.pack[dt.w + (size_t)col * L.w + n] = tmp.pack[d.w + (size_t)n * L.ld + col];
-                attach_tc(&tmp, dt, 1, true);
-                if (L.mel) {
-                    std::vector<float> fb;
-                    slaney_mel_fb((double)sample_rate, L.w, nm, key[2 + 4 * i + 2], key[2 + 4 * i + 3], fb);
-                    L.fb = pack_alloc(&tmp, fb.size());
-                    for (size_t j = 0; j < fb.size(); ++j) tmp.pack[L.fb + j] = fb[j];
-                }
+        for (int i = 0; i < n_scales; ++i) {
+            fac_handle::SpecScale& L = scales[i];
+            L.w = window_lengths[i]; L.nb = L.w / 2 + 1; L.ld = (2 * L.nb + 127) / 128 * 128;
+            const int nm = (int)key[2 + 4 * i + 1];
+            L.mel = nm > 0; L.n_out = L.mel ? nm : L.nb;
+            ConvW& d = L.dft;
+            d = ConvW();
+            d.Cin = L.w; d.Cout = L.ld; d.K = 1; d.ldw = L.ld;
+            d.w = P.alloc((size_t)L.w * L.ld);
+            d.b = P.alloc(L.ld);
+            dft_basis(P.pack.data() + d.w, L.ld, periodic_hann(L.w), L.w, L.nb, 0);
+            attach_tc(P, d, 1, true);
+            ConvW& dt = L.dftT;
+            dt = ConvW();
+            dt.Cin = L.ld; dt.Cout = L.w; dt.K = 1; dt.ldw = L.w;
+            dt.w = P.alloc((size_t)L.ld * L.w);
+            dt.b = P.alloc(L.w);
+            for (int n = 0; n < L.w; ++n)
+                for (int col = 0; col < 2 * L.nb; ++col) P.pack[dt.w + (size_t)col * L.w + n] = P.pack[d.w + (size_t)n * L.ld + col];
+            attach_tc(P, dt, 1, true);
+            if (L.mel) {
+                std::vector<float> fb;
+                slaney_mel_fb((double)sample_rate, L.w, nm, key[2 + 4 * i + 2], key[2 + 4 * i + 3], fb);
+                L.fb = P.alloc(fb.size());
+                std::copy(fb.begin(), fb.end(), P.pack.begin() + L.fb);
             }
-        } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_STATE; }
-        if (h->spec_arena) { cudaDeviceSynchronize(); cudaFree(h->spec_arena); h->spec_arena = nullptr; }
-        cudaError_t e = cudaMalloc(&h->spec_arena, (tmp.pack.size() + 64) * sizeof(float));
-        if (e == cudaSuccess) e = cudaMemcpy(h->spec_arena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); h->spec_arena = nullptr; return FAC_ERR_CUDA; }
+        }
+        const int rc = upload_weights(h, P, h->spec_arena, "fac_spectral_loss");
+        if (rc != FAC_OK) return rc;
         h->spec_scales = scales;
         h->spec_key = key;
     }
-    float* saved = h->warena;
-    h->warena = h->spec_arena;
-    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    return two_pass(h, (cudaStream_t)stream, h->spec_arena.get(), [&](Ctx& c) {
         double* sums = c.alloc<double>(2 * 16 + 2);
         const size_t mark = c.off;
         size_t peak = c.off;
@@ -4127,8 +4099,6 @@ static int spectral_loss(fac_handle* h, const float* x, const float* y, int B, i
         c.off = peak;
         if (!c.dry) c.check(launch_spec_loss_combine(sums, n_scales, mag_weight, log_weight, loss, c.st), "spec.combine");
     });
-    h->warena = saved;
-    return rc;
 }
 
 int fac_spectral_loss(fac_handle* h, const float* x, const float* y, int B, int T, int sample_rate, int n_scales, const int* window_lengths,
@@ -4172,42 +4142,39 @@ int fac_l1_loss_grad(fac_handle* h, const float* x, const float* y, long long n,
 // ---- predictor heads (SURVEY.md 8f rank 1; training-side in the reference, forward only here) ----
 int fac_head_begin(fac_handle* h) {
     if (!h) return FAC_ERR_INVALID;
-    h->heads.push_back(new fac_handle::HeadSet());
+    h->heads.push_back(std::make_unique<HeadSet>());
     return (int)h->heads.size() - 1;
 }
 
 int fac_head_tensor(fac_handle* h, int head_id, const char* key, const float* data_host, const int64_t* shape, int ndim) {
-    if (!h || head_id < 0 || head_id >= (int)h->heads.size() || !key || !data_host || ndim < 0 || ndim > 4) return FAC_ERR_INVALID;
-    HostTensor t;
-    size_t n = 1;
-    for (int i = 0; i < ndim; ++i) { if (shape[i] < 0) return FAC_ERR_INVALID; t.shape.push_back(shape[i]); n *= (size_t)shape[i]; }
-    t.data.assign(data_host, data_host + n);
-    h->heads[head_id]->staged[key] = std::move(t);
-    h->heads[head_id]->ready = false;
-    return FAC_OK;
+    HeadSet* hs = by_id(h, &fac_handle::heads, head_id);
+    if (!hs) return FAC_ERR_INVALID;
+    const int rc = stage_tensor(hs->staged, key, data_host, shape, ndim);
+    if (rc == FAC_OK) hs->ready = false;
+    return rc;
 }
 
 int fac_head_finalize(fac_handle* h, int head_id, int indim, int outdim, int nheads, int global_pred) {
-    if (!h || head_id < 0 || head_id >= (int)h->heads.size() || indim <= 0 || outdim <= 0 || nheads < 1 || nheads > 8) return FAC_ERR_INVALID;
+    HeadSet* set = by_id(h, &fac_handle::heads, head_id);
+    if (!set || indim <= 0 || outdim <= 0 || nheads < 1 || nheads > 8) return FAC_ERR_INVALID;
     if (indim % 16 != 0) { h->err = "fac_head_finalize: indim must be a multiple of 16"; return FAC_ERR_UNSUPPORTED; }
-    fac_handle::HeadSet& hs = *h->heads[head_id];
-    fac_handle tmp;                          // staging handle: reuses pack_conv / folded_weight on hs.staged
-    tmp.device = h->device;
-    tmp.host[0] = hs.staged;
+    HeadSet& hs = *set;
+    const TensorMap& ts = hs.staged;
+    Packer P;
     hs.indim = indim; hs.outdim = outdim; hs.nheads = nheads; hs.global_pred = global_pred;
     try {
         if (global_pred == 2) {
             // kind "linear": a plain nn.Linear(indim, outdim) staged as linear.weight [outdim][indim] / linear.bias
             // (FApredictors.timbre_predictor under timbre_norm, modules/quantize.py:470-473)
             if (nheads != 1) throw PackError{"a linear head has exactly one output"};
-            hs.lin[0] = pack_conv(&tmp, 0, "linear");
+            hs.lin[0] = pack_conv(P, ts, "linear");
             if (hs.lin[0].Cin != indim || hs.lin[0].Cout != outdim) throw PackError{"Linear geometry"};
         } else {
         auto expv = [&](const std::string& key) {
-            const HostTensor& t = need(&tmp, 0, key);
+            const HostTensor& t = need(ts, key);
             if ((int)t.numel() != indim) throw PackError{"shape of " + key};
-            size_t off = pack_alloc(&tmp, indim);
-            for (int i = 0; i < indim; ++i) tmp.pack[off + i] = expf(t.data[i]);     // alpha_logscale=True: exp() of the parameter
+            size_t off = P.alloc(indim);
+            for (int i = 0; i < indim; ++i) P.pack[off + i] = expf(t.data[i]);     // alpha_logscale=True: exp() of the parameter
             return off;
         };
         const int dils[3] = {1, 2, 3};
@@ -4216,14 +4183,14 @@ int fac_head_finalize(fac_handle* h, int head_id, int indim, int outdim, int nhe
             auto& u = hs.unit[j];
             u.dil = dils[j];
             u.a1 = expv(p + ".block.0.act.alpha"); u.b1 = expv(p + ".block.0.act.beta");
-            u.c7 = pack_conv(&tmp, 0, p + ".block.1");
+            u.c7 = pack_conv(P, ts, p + ".block.1");
             u.a2 = expv(p + ".block.2.act.alpha"); u.b2 = expv(p + ".block.2.act.beta");
-            u.c1 = pack_conv(&tmp, 0, p + ".block.3");
+            u.c1 = pack_conv(P, ts, p + ".block.3");
             if (u.c7.Cin != indim || u.c7.Cout != indim || u.c7.K != 7 || u.c1.K != 1) throw PackError{"head ResidualUnit geometry"};
         }
         hs.af = expv("model.3.act.alpha"); hs.bf = expv("model.3.act.beta");
         for (int i = 0; i < nheads; ++i) {
-            hs.lin[i] = pack_conv(&tmp, 0, "heads." + std::to_string(i));
+            hs.lin[i] = pack_conv(P, ts, "heads." + std::to_string(i));
             if (hs.lin[i].Cin != indim || hs.lin[i].Cout != outdim) throw PackError{"head Linear geometry"};
         }
         }
@@ -4231,11 +4198,8 @@ int fac_head_finalize(fac_handle* h, int head_id, int indim, int outdim, int nhe
         h->err = e.msg;
         return FAC_ERR_STATE;
     }
-    cudaSetDevice(h->device);
-    if (hs.arena) { cudaDeviceSynchronize(); cudaFree(hs.arena); hs.arena = nullptr; }
-    cudaError_t e = cudaMalloc(&hs.arena, (tmp.pack.size() + 64) * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(hs.arena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
+    const int rc = upload_weights(h, P, hs.arena, "fac_head_finalize");
+    if (rc != FAC_OK) return rc;
     hs.staged.clear();
     hs.ready = true;
     return FAC_OK;
@@ -4244,24 +4208,20 @@ int fac_head_finalize(fac_handle* h, int head_id, int indim, int outdim, int nhe
 static int ensure_aa_filter(fac_handle* h);
 
 int fac_head_forward(fac_handle* h, int head_id, const float* x, int B, int T, float* const* outs, void* stream) {
-    if (!h || head_id < 0 || head_id >= (int)h->heads.size() || !x || !outs || B <= 0 || T <= 0) return FAC_ERR_INVALID;
-    fac_handle::HeadSet& hs = *h->heads[head_id];
+    const HeadSet* set = by_id(h, &fac_handle::heads, head_id);
+    if (!set || !x || !outs || B <= 0 || T <= 0) return FAC_ERR_INVALID;
+    const HeadSet& hs = *set;
     if (!hs.ready) { h->err = "fac_head_forward: head not finalized"; return FAC_ERR_STATE; }
     int rc = ensure_aa_filter(h);
     if (rc) return rc;
-    // the conv launch helpers read weights through h->warena: point it at this head's arena for the duration of the call
-    float* saved = h->warena;
-    h->warena = hs.arena;
     const int C = hs.indim;
     if (hs.global_pred == 2) {
         // kind "linear": x [B*T rows][indim] -> outs[0] [B*T][outdim]
-        rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+        return two_pass(h, (cudaStream_t)stream, hs.arena.get(), [&](Ctx& c) {
             run_conv(c, hs.lin[0], x, outs[0], 1, B * T, B * T, ConvOpts(), "head.linear");
         });
-        h->warena = saved;
-        return rc;
     }
-    rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    return two_pass(h, (cudaStream_t)stream, hs.arena.get(), [&](Ctx& c) {
         const size_t n = (size_t)B * T * C;
         float* a_nct = c.alloc<float>(n);
         float* a_cl = c.alloc<float>(n);
@@ -4271,7 +4231,7 @@ int fac_head_forward(fac_handle* h, int head_id, const float* x, int B, int T, f
         float* x_nct = c.alloc<float>(n);
         float* pooled = c.alloc<float>((size_t)B * C);
         auto act = [&](const float* src, float* dst, size_t al, size_t be, const char* nm) {
-            if (!c.dry) c.check(launch_alias_free_act(src, dst, B, C, T, h->aa_filter, c.W(al), c.W(be), c.st), nm);
+            if (!c.dry) c.check(launch_alias_free_act(src, dst, B, C, T, h->aa_filter.get(), c.W(al), c.W(be), c.st), nm);
         };
         auto tr = [&](const float* src, float* dst, int R, int Cc, const char* nm) {     // [B][R][Cc] -> [B][Cc][R]
             if (!c.dry) c.check(launch_transpose(src, dst, B, R, Cc, c.st), nm);
@@ -4307,35 +4267,30 @@ int fac_head_forward(fac_handle* h, int head_id, const float* x, int B, int T, f
             }
         }
     });
-    h->warena = saved;
-    return rc;
 }
 
 // ---- JDCNet pitch extractor (modules/JDC/model.py, eval mode) ----
 int fac_jdc_begin(fac_handle* h) {
     if (!h) return FAC_ERR_INVALID;
-    h->jdcs.push_back(new fac_handle::JdcSet());
+    h->jdcs.push_back(std::make_unique<JdcSet>());
     return (int)h->jdcs.size() - 1;
 }
 
 int fac_jdc_tensor(fac_handle* h, int jdc_id, const char* key, const float* data_host, const int64_t* shape, int ndim) {
-    if (!h || jdc_id < 0 || jdc_id >= (int)h->jdcs.size() || !key || !data_host || ndim < 0 || ndim > 4) return FAC_ERR_INVALID;
-    HostTensor t;
-    size_t n = 1;
-    for (int i = 0; i < ndim; ++i) { if (shape[i] < 0) return FAC_ERR_INVALID; t.shape.push_back(shape[i]); n *= (size_t)shape[i]; }
-    t.data.assign(data_host, data_host + n);
-    h->jdcs[jdc_id]->staged[key] = std::move(t);
-    h->jdcs[jdc_id]->ready = false;
-    return FAC_OK;
+    JdcSet* js = by_id(h, &fac_handle::jdcs, jdc_id);
+    if (!js) return FAC_ERR_INVALID;
+    const int rc = stage_tensor(js->staged, key, data_host, shape, ndim);
+    if (rc == FAC_OK) js->ready = false;
+    return rc;
 }
 
 namespace {
 // BatchNorm2d (eval) at `prefix` as y = x * sc + sh, in fp64 then rounded
-void jdc_bn(fac_handle* tmp, const std::string& prefix, int C, std::vector<double>& sc, std::vector<double>& sh) {
-    const HostTensor& g = need(tmp, 0, prefix + ".weight");
-    const HostTensor& b = need(tmp, 0, prefix + ".bias");
-    const HostTensor& m = need(tmp, 0, prefix + ".running_mean");
-    const HostTensor& v = need(tmp, 0, prefix + ".running_var");
+void jdc_bn(const TensorMap& ts, const std::string& prefix, int C, std::vector<double>& sc, std::vector<double>& sh) {
+    const HostTensor& g = need(ts, prefix + ".weight");
+    const HostTensor& b = need(ts, prefix + ".bias");
+    const HostTensor& m = need(ts, prefix + ".running_mean");
+    const HostTensor& v = need(ts, prefix + ".running_var");
     if ((int)g.numel() != C || (int)b.numel() != C || (int)m.numel() != C || (int)v.numel() != C) throw PackError{"BatchNorm shape at " + prefix};
     sc.resize(C); sh.resize(C);
     for (int c = 0; c < C; ++c) {
@@ -4343,37 +4298,37 @@ void jdc_bn(fac_handle* tmp, const std::string& prefix, int C, std::vector<doubl
         sh[c] = (double)b.data[c] - (double)m.data[c] * sc[c];
     }
 }
-fac_handle::JdcSet::Bn jdc_pack_bn(fac_handle* tmp, const std::string& prefix, int C) {
+JdcSet::Bn jdc_pack_bn(Packer& P, const TensorMap& ts, const std::string& prefix, int C) {
     std::vector<double> sc, sh;
-    jdc_bn(tmp, prefix, C, sc, sh);
-    fac_handle::JdcSet::Bn r;
-    r.sc = pack_alloc(tmp, C); r.sh = pack_alloc(tmp, C);
-    for (int c = 0; c < C; ++c) { tmp->pack[r.sc + c] = (float)sc[c]; tmp->pack[r.sh + c] = (float)sh[c]; }
+    jdc_bn(ts, prefix, C, sc, sh);
+    JdcSet::Bn r;
+    r.sc = P.alloc(C); r.sh = P.alloc(C);
+    for (int c = 0; c < C; ++c) { P.pack[r.sc + c] = (float)sc[c]; P.pack[r.sh + c] = (float)sh[c]; }
     return r;
 }
 // nn.Conv2d(Cin, Cout, k, bias=False) at `prefix` (k = 3: 9 row-offset taps tap = kh * 3 + kw; k = 1: one tap), with the
 // BatchNorm at `bn` (or none) folded in, packed [taps * Cin][ldw] with its promoted fp16 hi + scaled-lo blob (conv_tc.cu)
-ConvW jdc_pack_conv(fac_handle* tmp, const std::string& prefix, int Cin, int Cout, int k, const char* bn) {
-    const HostTensor& w = need(tmp, 0, prefix + ".weight");
+ConvW jdc_pack_conv(Packer& P, const TensorMap& ts, const std::string& prefix, int Cin, int Cout, int k, const char* bn) {
+    const HostTensor& w = need(ts, prefix + ".weight");
     if (w.shape.size() != 4 || w.shape[0] != Cout || w.shape[1] != Cin || w.shape[2] != k || w.shape[3] != k)
         throw PackError{"Conv2d shape at " + prefix};
     std::vector<double> sc(Cout, 1.0), sh(Cout, 0.0);
-    if (bn) jdc_bn(tmp, bn, Cout, sc, sh);
+    if (bn) jdc_bn(ts, bn, Cout, sc, sh);
     ConvW c;
     c.Cin = Cin; c.Cout = Cout; c.K = k * k; c.ldw = (Cout + 3) / 4 * 4;
-    c.w = pack_alloc(tmp, (size_t)c.K * Cin * c.ldw);
+    c.w = P.alloc((size_t)c.K * Cin * c.ldw);
     for (int co = 0; co < Cout; ++co)
         for (int ci = 0; ci < Cin; ++ci)
             for (int tap = 0; tap < c.K; ++tap)
-                tmp->pack[c.w + ((size_t)tap * Cin + ci) * c.ldw + co] = (float)(w.data[((size_t)co * Cin + ci) * c.K + tap] * sc[co]);
-    c.b = pack_alloc(tmp, Cout);
-    for (int co = 0; co < Cout; ++co) tmp->pack[c.b + co] = (float)sh[co];
+                P.pack[c.w + ((size_t)tap * Cin + ci) * c.ldw + co] = (float)(w.data[((size_t)co * Cin + ci) * c.K + tap] * sc[co]);
+    c.b = P.alloc(Cout);
+    for (int co = 0; co < Cout; ++co) P.pack[c.b + co] = (float)sh[co];
     TcConvParams tp;
     tp.Cin = Cin; tp.Cout = Cout; tp.Kr = c.K; tp.vf = 1; tp.dil = 1; tp.promoted = 1; tp.f16x2 = 1; tp.row2d = k == 3 ? 82 : 0;
     if (!tc_conv_plan(tp)) throw PackError{"no tensor-core plan for " + prefix};
     c.Kr = c.K; c.promoted = true; c.tcN = tp.N; c.tc = true; c.has16 = true;
-    c.tcw16 = pack_alloc(tmp, tc_blob_floats(tp));
-    tc_pack_blob(tp, tmp->pack.data() + c.w, c.ldw, tmp->pack.data() + c.tcw16);
+    c.tcw16 = P.alloc(tc_blob_floats(tp));
+    tc_pack_blob(tp, P.pack.data() + c.w, c.ldw, P.pack.data() + c.tcw16);
     return c;
 }
 
@@ -4399,77 +4354,74 @@ void jdc_conv3(Ctx& c, const ConvW& w, const float* x, float* y, int B, int T, i
 }  // namespace
 
 int fac_jdc_finalize(fac_handle* h, int jdc_id) {
-    if (!h || jdc_id < 0 || jdc_id >= (int)h->jdcs.size()) return FAC_ERR_INVALID;
-    fac_handle::JdcSet& js = *h->jdcs[jdc_id];
-    fac_handle tmp;
-    tmp.device = h->device;
-    tmp.host[0] = js.staged;
+    JdcSet* set = by_id(h, &fac_handle::jdcs, jdc_id);
+    if (!set) return FAC_ERR_INVALID;
+    JdcSet& js = *set;
+    const TensorMap& ts = js.staged;
+    Packer P;
     try {
         {   // conv_block.0 (1 -> 64) with conv_block.1 folded: SIMT, [9][64]
-            const HostTensor& w = need(&tmp, 0, "conv_block.0.weight");
+            const HostTensor& w = need(ts, "conv_block.0.weight");
             if (w.shape.size() != 4 || w.shape[0] != 64 || w.shape[1] != 1 || w.shape[2] != 3 || w.shape[3] != 3)
                 throw PackError{"Conv2d shape at conv_block.0"};
             std::vector<double> sc, sh;
-            jdc_bn(&tmp, "conv_block.1", 64, sc, sh);
-            js.conv_in_w = pack_alloc(&tmp, 9 * 64);
-            js.conv_in_b = pack_alloc(&tmp, 64);
+            jdc_bn(ts, "conv_block.1", 64, sc, sh);
+            js.conv_in_w = P.alloc(9 * 64);
+            js.conv_in_b = P.alloc(64);
             for (int co = 0; co < 64; ++co) {
-                for (int k = 0; k < 9; ++k) tmp.pack[js.conv_in_w + k * 64 + co] = (float)(w.data[co * 9 + k] * sc[co]);
-                tmp.pack[js.conv_in_b + co] = (float)sh[co];
+                for (int k = 0; k < 9; ++k) P.pack[js.conv_in_w + k * 64 + co] = (float)(w.data[co * 9 + k] * sc[co]);
+                P.pack[js.conv_in_b + co] = (float)sh[co];
             }
         }
-        js.c0b = jdc_pack_conv(&tmp, "conv_block.3", 64, 64, 3, nullptr);
+        js.c0b = jdc_pack_conv(P, ts, "conv_block.3", 64, 64, 3, nullptr);
         const int cin[3] = {64, 128, 192}, cout[3] = {128, 192, 256}, F[3] = {80, 40, 20};
         for (int i = 0; i < 3; ++i) {
             const std::string p = "res_block" + std::to_string(i + 1);
             auto& b = js.blk[i];
             b.F = F[i];
-            b.pre = jdc_pack_bn(&tmp, p + ".pre_conv.0", cin[i]);
-            b.c1 = jdc_pack_conv(&tmp, p + ".conv.0", cin[i], cout[i], 3, (p + ".conv.1").c_str());
-            b.c2 = jdc_pack_conv(&tmp, p + ".conv.3", cout[i], cout[i], 3, nullptr);
-            b.c11 = jdc_pack_conv(&tmp, p + ".conv1by1", cin[i], cout[i], 1, nullptr);
+            b.pre = jdc_pack_bn(P, ts, p + ".pre_conv.0", cin[i]);
+            b.c1 = jdc_pack_conv(P, ts, p + ".conv.0", cin[i], cout[i], 3, (p + ".conv.1").c_str());
+            b.c2 = jdc_pack_conv(P, ts, p + ".conv.3", cout[i], cout[i], 3, nullptr);
+            b.c11 = jdc_pack_conv(P, ts, p + ".conv1by1", cin[i], cout[i], 1, nullptr);
         }
-        js.pool = jdc_pack_bn(&tmp, "pool_block.0", 256);
+        js.pool = jdc_pack_bn(P, ts, "pool_block.0", 256);
         const int H = 256;
         js.U = lstm_units_per_cta(H);
         js.G = H / js.U;
         for (int d = 0; d < 2; ++d) {
             const std::string sfx = d ? "_l0_reverse" : "_l0";
-            const HostTensor& wih = need(&tmp, 0, "bilstm_classifier.weight_ih" + sfx);
-            const HostTensor& whh = need(&tmp, 0, "bilstm_classifier.weight_hh" + sfx);
-            const HostTensor& bih = need(&tmp, 0, "bilstm_classifier.bias_ih" + sfx);
-            const HostTensor& bhh = need(&tmp, 0, "bilstm_classifier.bias_hh" + sfx);
+            const HostTensor& wih = need(ts, "bilstm_classifier.weight_ih" + sfx);
+            const HostTensor& whh = need(ts, "bilstm_classifier.weight_hh" + sfx);
+            const HostTensor& bih = need(ts, "bilstm_classifier.bias_ih" + sfx);
+            const HostTensor& bhh = need(ts, "bilstm_classifier.bias_hh" + sfx);
             if (wih.numel() != (size_t)4 * H * 512 || whh.numel() != (size_t)4 * H * H || bih.numel() != 4 * H || bhh.numel() != 4 * H)
                 throw PackError{"bilstm_classifier shape"};
             ConvW c;
             c.Cin = 512; c.Cout = 4 * H; c.K = 1; c.ldw = 4 * H;
-            c.w = pack_alloc(&tmp, (size_t)512 * c.ldw);
+            c.w = P.alloc((size_t)512 * c.ldw);
             for (int row = 0; row < 4 * H; ++row)
-                for (int k = 0; k < 512; ++k) tmp.pack[c.w + (size_t)k * c.ldw + row] = wih.data[(size_t)row * 512 + k];
-            c.b = pack_alloc(&tmp, 4 * H);
-            for (int row = 0; row < 4 * H; ++row) tmp.pack[c.b + row] = bih.data[row] + bhh.data[row];
-            attach_tc(&tmp, c, 1, true);
+                for (int k = 0; k < 512; ++k) P.pack[c.w + (size_t)k * c.ldw + row] = wih.data[(size_t)row * 512 + k];
+            c.b = P.alloc(4 * H);
+            for (int row = 0; row < 4 * H; ++row) P.pack[c.b + row] = bih.data[row] + bhh.data[row];
+            attach_tc(P, c, 1, true);
             if (!c.tc || !c.has16) throw PackError{"no tensor-core plan for the BiLSTM input GEMM"};
             js.ih[d] = c;
-            js.whh2[d] = pack_alloc(&tmp, lstm2_pack_words(H, js.U, 1));
-            lstm2_pack(whh.data.data(), H, js.U, 1, reinterpret_cast<uint32_t*>(tmp.pack.data() + js.whh2[d]));
+            js.whh2[d] = P.alloc(lstm2_pack_words(H, js.U, 1));
+            lstm2_pack(whh.data.data(), H, js.U, 1, reinterpret_cast<uint32_t*>(P.pack.data() + js.whh2[d]));
         }
-        const HostTensor& cw = need(&tmp, 0, "classifier.weight");
-        const HostTensor& cb = need(&tmp, 0, "classifier.bias");
+        const HostTensor& cw = need(ts, "classifier.weight");
+        const HostTensor& cb = need(ts, "classifier.bias");
         if (cw.numel() != 512 || cb.numel() != 1) throw PackError{"classifier shape (num_class must be 1)"};
-        js.cls_w = pack_alloc(&tmp, 512);
-        for (int k = 0; k < 512; ++k) tmp.pack[js.cls_w + k] = cw.data[k];
-        js.cls_b = pack_alloc(&tmp, 1);
-        tmp.pack[js.cls_b] = cb.data[0];
+        js.cls_w = P.alloc(512);
+        for (int k = 0; k < 512; ++k) P.pack[js.cls_w + k] = cw.data[k];
+        js.cls_b = P.alloc(1);
+        P.pack[js.cls_b] = cb.data[0];
     } catch (const PackError& e) {
         h->err = e.msg;
         return FAC_ERR_STATE;
     }
-    cudaSetDevice(h->device);
-    if (js.arena) { cudaDeviceSynchronize(); cudaFree(js.arena); js.arena = nullptr; }
-    cudaError_t e = cudaMalloc(&js.arena, (tmp.pack.size() + 64) * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(js.arena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); js.arena = nullptr; return FAC_ERR_CUDA; }
+    const int rc = upload_weights(h, P, js.arena, "fac_jdc_finalize");
+    if (rc != FAC_OK) return rc;
     js.staged.clear();
     js.ready = true;
     return FAC_OK;
@@ -4477,9 +4429,9 @@ int fac_jdc_finalize(fac_handle* h, int jdc_id) {
 
 int fac_jdc_forward(fac_handle* h, int jdc_id, const float* mel, int B, int T, const int* lengths, float* f0, float* gan_feature,
                     float* pool_out, void* stream) {
-    if (!h || jdc_id < 0 || jdc_id >= (int)h->jdcs.size() || !mel || !f0 || !gan_feature || !pool_out || B <= 0 || T <= 0)
-        return FAC_ERR_INVALID;
-    fac_handle::JdcSet& js = *h->jdcs[jdc_id];
+    const JdcSet* set = by_id(h, &fac_handle::jdcs, jdc_id);
+    if (!set || !mel || !f0 || !gan_feature || !pool_out || B <= 0 || T <= 0) return FAC_ERR_INVALID;
+    const JdcSet& js = *set;
     if (!js.ready) { h->err = "fac_jdc_forward: JDCNet not finalized"; return FAC_ERR_STATE; }
     std::vector<int> lens(B, T);
     if (lengths)
@@ -4488,10 +4440,8 @@ int fac_jdc_forward(fac_handle* h, int jdc_id, const float* mel, int B, int T, c
             lens[b] = lengths[b];
         }
     if (B > 65535) { h->err = "fac_jdc_forward: B > 65535"; return FAC_ERR_UNSUPPORTED; }
-    float* saved = h->warena;
-    h->warena = js.arena;
     const int H = 256;
-    int rc = two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    return two_pass(h, (cudaStream_t)stream, js.arena.get(), [&](Ctx& c) {
         // per-lane frames, then rows of each map width (F + 2 = 82, 42, 22, 12)
         int* dl = lengths ? c.alloc<int>((size_t)5 * B) : nullptr;
         const int Fs[4] = {80, 40, 20, 10};
@@ -4582,8 +4532,6 @@ int fac_jdc_forward(fac_handle* h, int jdc_id, const float* mel, int B, int T, c
         c.tap("jdc.lstm.rev", yd[1], (size_t)B * T * H);
         if (!c.dry) c.check(launch_jdc_head(yd[0], yd[1], c.W(js.cls_w), c.W(js.cls_b), f0, B, T, len_d, c.st), "jdc.head");
     });
-    h->warena = saved;
-    return rc;
 }
 
 int fac_f0_targets(fac_handle* h, const float* f0, int B, int T, const int* lengths, float* targets, float* glob_f0, void* stream) {
@@ -4626,40 +4574,30 @@ int fac_add3(fac_handle* h, const float* a, const float* b, const float* c3, lon
 int fac_rvq_create(fac_handle* h, int nq, const float* const* in_w, const float* const* in_b, const float* const* out_w,
                    const float* const* out_b, const float* const* codebook) {
     if (!h || nq < 1 || nq > 8) return FAC_ERR_INVALID;
-    std::vector<float> pack;
-    RvqSet s;
-    s.nq = nq;
-    for (int q = 0; q < nq; ++q) s.vq[q] = pack_vq_raw(pack, in_w[q], in_b[q], out_w[q], out_b[q], codebook[q]);
-    cudaSetDevice(h->device);
-    float* dev = nullptr;
-    cudaError_t e = cudaMalloc(&dev, (pack.size() + 64) * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(dev, pack.data(), pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
-    h->rvqs.push_back(s);
-    h->rvq_arenas.push_back(dev);
+    auto s = std::make_unique<RvqSet>();
+    s->nq = nq;
+    Packer P;
+    for (int q = 0; q < nq; ++q) s->vq[q] = pack_vq_raw(P, in_w[q], in_b[q], out_w[q], out_b[q], codebook[q]);
+    const int rc = upload_weights(h, P, s->arena, "fac_rvq_create");
+    if (rc != FAC_OK) return rc;
+    h->rvqs.push_back(std::move(s));
     return (int)h->rvqs.size() - 1;
 }
 
-// Frees the device arena of one fac_rvq_create set (ids of other sets stay valid; the id is not reused).
+// Frees the device arena of one fac_rvq_create set (ids of other sets stay valid; the id is not reused; destroying a set
+// twice is a no-op).
 int fac_rvq_destroy(fac_handle* h, int rvq_id) {
     if (!h || rvq_id < 0 || rvq_id >= (int)h->rvqs.size()) return FAC_ERR_INVALID;
-    if (h->rvq_arenas[rvq_id]) {
-        cudaSetDevice(h->device);
-        cudaDeviceSynchronize();
-        cudaFree(h->rvq_arenas[rvq_id]);
-        h->rvq_arenas[rvq_id] = nullptr;
-        h->rvqs[rvq_id].nq = 0;
-    }
-    return FAC_OK;
+    return h->rvqs[rvq_id] ? free_by_id(h, &fac_handle::rvqs, rvq_id) : FAC_OK;
 }
 
 int fac_rvq_forward(fac_handle* h, int rvq_id, const float* x, int B, int T, int x_channels_last, float* quantized_out,
                     int64_t* indices, float* all_quantized, void* stream) {
     if (!h || rvq_id < 0 || rvq_id >= (int)h->rvqs.size() || !x || !quantized_out || !indices || B <= 0 || T <= 0) return FAC_ERR_INVALID;
-    const RvqSet& s = h->rvqs[rvq_id];
-    const float* base = h->rvq_arenas[rvq_id];
-    if (!base || s.nq < 1) { h->err = "fac_rvq_forward: set was destroyed"; return FAC_ERR_STATE; }
-    return two_pass(h, (cudaStream_t)stream, [&](Ctx& c) {
+    const RvqSet* set = by_id(h, &fac_handle::rvqs, rvq_id);
+    if (!set) { h->err = "fac_rvq_forward: set was destroyed"; return FAC_ERR_STATE; }
+    const RvqSet& s = *set;
+    return two_pass(h, (cudaStream_t)stream, s.arena.get(), [&](Ctx& c) {
         size_t n = (size_t)B * T * 1024;
         float* xcl = x_channels_last ? nullptr : c.alloc<float>(n);
         float* qcl = x_channels_last ? nullptr : c.alloc<float>(n);
@@ -4674,7 +4612,7 @@ int fac_rvq_forward(fac_handle* h, int rvq_id, const float* x, int B, int T, int
         p.nq = s.nq; p.B = B; p.T = T;
         for (int q = 0; q < s.nq; ++q) {
             const VqW& v = s.vq[q];
-            p.vq[q] = VqWeights{base + v.w_in, base + v.b_in, base + v.cb, base + v.cbn, base + v.cbn2, base + v.w_out, base + v.b_out};
+            p.vq[q] = VqWeights{c.W(v.w_in), c.W(v.b_in), c.W(v.cb), c.W(v.cbn), c.W(v.cbn2), c.W(v.w_out), c.W(v.b_out)};
         }
         c.check(launch_rvq(p, c.st), "rvq");
         if (!x_channels_last) {
@@ -4694,7 +4632,7 @@ static int ensure_aa_filter(fac_handle* h) {
         double A = 2.285 * (half - 1) * M_PI * delta_f + 7.95;
         double beta_k = A > 50.0 ? 0.1102 * (A - 8.7) : (A >= 21.0 ? 0.5842 * std::pow(A - 21, 0.4) + 0.07886 * (A - 21.0) : 0.0);
         auto i0 = [](double v) { double s = 1, t = 1; for (int k = 1; k < 60; ++k) { t *= (v / (2 * k)) * (v / (2 * k)); s += t; } return s; };
-        float f[12];
+        std::vector<float> f(ks);
         double sum = 0;
         double tmp[12];
         for (int i = 0; i < ks; ++i) {
@@ -4707,9 +4645,7 @@ static int ensure_aa_filter(fac_handle* h) {
             sum += tmp[i];
         }
         for (int i = 0; i < ks; ++i) f[i] = (float)(tmp[i] / sum);
-        cudaError_t e = cudaMalloc(&h->aa_filter, sizeof(f));
-        if (e == cudaSuccess) e = cudaMemcpy(h->aa_filter, f, sizeof(f), cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
+        return upload(h, f, h->aa_filter, "anti-alias filter");
     }
     return FAC_OK;
 }
@@ -4719,7 +4655,7 @@ int fac_alias_free_act(fac_handle* h, const float* x, int B, int C, int T, int a
     if (!h || !x || !y || B <= 0 || C <= 0 || T <= 0 || (act == 1 && (!alpha || !beta))) return FAC_ERR_INVALID;
     int rc0 = ensure_aa_filter(h);
     if (rc0) return rc0;
-    cudaError_t e = launch_alias_free_act(x, y, B, C, T, h->aa_filter, act == 1 ? alpha : nullptr, act == 1 ? beta : nullptr,
+    cudaError_t e = launch_alias_free_act(x, y, B, C, T, h->aa_filter.get(), act == 1 ? alpha : nullptr, act == 1 ? beta : nullptr,
                                           (cudaStream_t)stream);
     if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return FAC_ERR_CUDA; }
     return FAC_OK;
@@ -4728,22 +4664,16 @@ int fac_alias_free_act(fac_handle* h, const float* x, int B, int C, int T, int a
 }  // extern "C"
 
 namespace {
-// The per-lane lengths of a debug conv hook (HOST, B entries, or null) checked and copied to the device: *dev receives
-// the device copy (null when lane_len_host is null; the caller frees it).  Nothing is launched when a length lies
-// outside [1, Tin].
-int debug_upload_lanes(fac_handle* h, const char* who, const int* lane_len_host, int B, int Tin, int** dev) {
-    *dev = nullptr;
+// The per-lane lengths of a debug conv hook (HOST, B entries, or null) checked and copied to the device: dev receives
+// the device copy (empty when lane_len_host is null).  Nothing is launched when a length lies outside [1, Tin].
+int debug_upload_lanes(fac_handle* h, const char* who, const int* lane_len_host, int B, int Tin, DevBuf<int>& dev) {
     if (!lane_len_host) return FAC_OK;
     for (int b = 0; b < B; ++b)
         if (lane_len_host[b] < 1 || lane_len_host[b] > Tin) {
             h->err = std::string(who) + ": lane lengths must lie in [1, Tin]";
             return FAC_ERR_INVALID;
         }
-    cudaSetDevice(h->device);
-    cudaError_t e = cudaMalloc(dev, sizeof(int) * (size_t)B);
-    if (e == cudaSuccess) e = cudaMemcpy(*dev, lane_len_host, sizeof(int) * (size_t)B, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); cudaFree(*dev); *dev = nullptr; return FAC_ERR_CUDA; }
-    return FAC_OK;
+    return upload(h, std::vector<int>(lane_len_host, lane_len_host + B), dev, who);
 }
 
 // fac_debug_conv, and fac_debug_conv_lanes' path -1: launch_conv (it picks the cin1 / cout1 / generic kernel) on one
@@ -4765,10 +4695,10 @@ int debug_conv(fac_handle* h, const float* x, const float* w_host, const float* 
     for (int i = 0; i < Cout; ++i) pk[o_b + i] = bias_host ? bias_host[i] : 0.f;
     for (int i = 0; i < Cin; ++i) { pk[o_ia + i] = in_alpha_host ? in_alpha_host[i] : 1.f; pk[o_iia + i] = 1.0f / (pk[o_ia + i] + 1e-9f); }
     for (int i = 0; i < Cout; ++i) { pk[o_oa + i] = out_alpha_host ? out_alpha_host[i] : 1.f; pk[o_oia + i] = 1.0f / (pk[o_oa + i] + 1e-9f); }
-    float* d = nullptr;
-    cudaError_t e = cudaMalloc(&d, pk.size() * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(d, pk.data(), pk.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
+    DevBuf<float> buf;
+    const int rc = upload(h, pk, buf, "fac_debug_conv");
+    if (rc != FAC_OK) return rc;
+    const float* d = buf.get();
     ConvParams p;
     p.x = x; p.y = y; p.w = d; p.bias = bias_host ? d + o_b : nullptr;
     if (in_alpha_host) { p.in_alpha = d + o_ia; p.in_inv_alpha = d + o_iia; }
@@ -4779,9 +4709,8 @@ int debug_conv(fac_handle* h, const float* x, const float* w_host, const float* 
     p.pad_left = pad_left; p.pad_right = pad_right; p.pad_reflect = reflect;
     p.ldw = ldw; p.ldy = Cout; p.ldx = Cin;
     p.x_bstride = (size_t)Tin * Cin; p.y_bstride = (size_t)Tout * Cout;
-    e = launch_conv(p, st);
+    cudaError_t e = launch_conv(p, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
     if (e != cudaSuccess) { h->err = std::string("fac_debug_conv: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
     return FAC_OK;
 }
@@ -4813,23 +4742,25 @@ int debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B
         }
         if (sum != T) { h->err = "fac_debug_slstm: chunk lengths must sum to T"; return FAC_ERR_INVALID; }
     }
-    // build a private handle holding only this LSTM with the caller's precision options, reuse the packing + slstm code path
+    // a private handle carries the caller's precision options and its own workspace through the slstm code path
     fac_handle tmp;
     tmp.device = h->device;
     tmp.use_tc = h->use_tc; tmp.enc_f16 = h->enc_f16; tmp.enc_tt = h->enc_tt; tmp.tc_occ2 = h->tc_occ2;
     tmp.dec_bf16 = h->dec_bf16; tmp.dec_c7_f16 = h->dec_c7_f16;
     tmp.lstm_v2 = h->lstm_v2; tmp.dec_lstm_fp16 = h->dec_lstm_fp16;
     const char* names[8] = {"weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0", "weight_ih_l1", "weight_hh_l1", "bias_ih_l1", "bias_hh_l1"};
+    TensorMap ts;
     for (int i = 0; i < 8; ++i) {
         HostTensor t;
         bool mat = (i % 4) < 2;
         if (mat) t.shape = {4 * H, H}; else t.shape = {4 * H};
         t.data.assign(w_host[i], w_host[i] + t.numel());
-        tmp.host[0][std::string("l.") + names[i]] = std::move(t);
+        ts[std::string("l.") + names[i]] = std::move(t);
     }
     // upstream: packed and run as the encoder's LSTM (promoted input projection, under vq_critical); else as the decoder's
+    Packer P;
     LstmW L;
-    try { L = pack_lstm(&tmp, 0, "l", upstream != 0); } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_UNSUPPORTED; }
+    try { L = pack_lstm(P, ts, "l", upstream != 0); } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_UNSUPPORTED; }
     cudaStream_t st = (cudaStream_t)stream;
     size_t hw = 0, cf = 0;
     int pass3 = 0;
@@ -4843,11 +4774,10 @@ int debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B
         pass3 = lstm_pass3(probe);
         lstm2_state_sizes(H, L.U, pass3, &hw, &cf);
     }
-    cudaSetDevice(h->device);
-    cudaError_t e = cudaMalloc(&tmp.warena, (tmp.pack.size() + 64) * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(tmp.warena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
-    int rc = two_pass(&tmp, st, [&](Ctx& c) {
+    DevBuf<float> w;
+    int rc = upload_weights(h, P, w, "fac_debug_slstm");
+    if (rc != FAC_OK) return rc;
+    rc = two_pass(&tmp, st, w.get(), [&](Ctx& c) {
         c.vq_critical = upstream != 0;
         if (!chunked && !carry) { slstm(c, L, x, y, B, T); return; }
         // chunk by chunk with the state carried as fac_stream_encode / fac_stream_decode do, from a zero state; or from the
@@ -4878,8 +4808,6 @@ int debug_slstm(fac_handle* h, const float* x, const float* const* w_host, int B
     });
     cudaStreamSynchronize(st);
     if (rc != FAC_OK) h->err = tmp.err;
-    cudaFree(tmp.warena);
-    if (tmp.ws) cudaFree(tmp.ws);
     return rc;
 }
 }  // namespace
@@ -4911,15 +4839,14 @@ int fac_debug_fa_quantize(fac_handle* h, const float* f0, const float* z, const 
     for (int i = 0; i < 6; ++i)
         for (int j = 0; j < 5; ++j)
             if (!vq_host[i][j]) return FAC_ERR_INVALID;
-    std::vector<float> pack;
+    Packer P;
     VqW v[6];
-    for (int i = 0; i < 6; ++i) v[i] = pack_vq_raw(pack, vq_host[i][0], vq_host[i][1], vq_host[i][2], vq_host[i][3], vq_host[i][4]);
-    cudaSetDevice(h->device);
+    for (int i = 0; i < 6; ++i) v[i] = pack_vq_raw(P, vq_host[i][0], vq_host[i][1], vq_host[i][2], vq_host[i][3], vq_host[i][4]);
     cudaStream_t st = (cudaStream_t)stream;
-    float* d = nullptr;
-    cudaError_t e = cudaMalloc(&d, pack.size() * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(d, pack.data(), pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); cudaFree(d); return FAC_ERR_CUDA; }
+    DevBuf<float> buf;
+    const int rc = upload(h, P.pack, buf, "fac_debug_fa_quantize");
+    if (rc != FAC_OK) return rc;
+    const float* d = buf.get();
     FaqParams fp;
     fp.f0 = f0; fp.z = z;
     for (int i = 0; i < 6; ++i)
@@ -4930,10 +4857,9 @@ int fac_debug_fa_quantize(fac_handle* h, const float* f0, const float* z, const 
     fp.codes_p = codes_p; fp.codes_c = codes_c; fp.codes_r = codes_r;
     fp.sqerr = sqerr;
     fp.B = B; fp.Tq = Tq; fp.Tz = Tz; fp.Tf0 = Tf0;
-    e = launch_fa_quantize(fp, st);
+    cudaError_t e = launch_fa_quantize(fp, st);
     if (e == cudaSuccess) e = launch_vq_loss_reduce(sqerr, 6, B, Tq, losses2, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
     if (e != cudaSuccess) { h->err = std::string("fac_debug_fa_quantize: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
     return FAC_OK;
 }
@@ -5003,10 +4929,10 @@ static int debug_conv_tc(fac_handle* h, const float* x, const float* w_host, con
     for (int i = 0; i < Cout; ++i) pk[o_b + i] = bias_host ? bias_host[i] : 0.f;
     for (int i = 0; i < Cin; ++i) { pk[o_ia + i] = in_alpha_host ? in_alpha_host[i] : 1.f; pk[o_iia + i] = 1.0f / (pk[o_ia + i] + 1e-9f); }
     for (int i = 0; i < Cout; ++i) { pk[o_oa + i] = out_alpha_host ? out_alpha_host[i] : 1.f; pk[o_oia + i] = 1.0f / (pk[o_oa + i] + 1e-9f); }
-    float* d = nullptr;
-    cudaError_t e = cudaMalloc(&d, pk.size() * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(d, pk.data(), pk.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
+    DevBuf<float> buf;
+    const int rc = upload(h, pk, buf, "fac_debug_conv_tc");
+    if (rc != FAC_OK) return rc;
+    const float* d = buf.get();
     tp.x = x; tp.y = y; tp.wblob = d; tp.bias = d + o_b;
     if (in_alpha_host) { tp.in_alpha = d + o_ia; tp.in_inv_alpha = d + o_iia; }
     tp.out_act = act;
@@ -5017,9 +4943,8 @@ static int debug_conv_tc(fac_handle* h, const float* x, const float* w_host, con
     tp.pad_left_s = pad_left; tp.pad_right_s = pad_right; tp.reflect = reflect; tp.lane_len = lane_len;
     tp.Tout = Tout; tp.ldy = Cout;
     tp.x_bstride = (size_t)Tin * Cin; tp.y_bstride = (size_t)Tout * Cout;
-    e = launch_conv_tc(tp, st);
+    cudaError_t e = launch_conv_tc(tp, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
     if (e != cudaSuccess) { h->err = std::string("fac_debug_conv_tc: ") + cudaGetErrorString(e); return FAC_ERR_CUDA; }
     return FAC_OK;
 }
@@ -5046,17 +4971,14 @@ int fac_debug_conv_lanes(fac_handle* h, const float* x, const float* w_host, con
                          const float* in_alpha_host, const float* out_alpha_host, int act, const float* res, float* y,
                          int Tout, int path, const int* lane_len_host, void* stream) {
     if (!h || !x || !w_host || !y || B <= 0 || Tin <= 0) return FAC_ERR_INVALID;
-    int* lanes = nullptr;
-    int rc = debug_upload_lanes(h, "fac_debug_conv_lanes", lane_len_host, B, Tin, &lanes);
+    DevBuf<int> lanes;
+    int rc = debug_upload_lanes(h, "fac_debug_conv_lanes", lane_len_host, B, Tin, lanes);
     if (rc != FAC_OK) return rc;
     if (path == -1)
-        rc = debug_conv(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
-                        in_alpha_host, out_alpha_host, act, res, y, Tout, lanes, stream);
-    else
-        rc = debug_conv_tc(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
-                           in_alpha_host, out_alpha_host, act, res, y, Tout, path, stream, nullptr, lanes);
-    cudaFree(lanes);
-    return rc;
+        return debug_conv(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
+                          in_alpha_host, out_alpha_host, act, res, y, Tout, lanes.get(), stream);
+    return debug_conv_tc(h, x, w_host, bias_host, B, Tin, Cin, Cout, K, dil, stride, pad_left, pad_right, reflect,
+                         in_alpha_host, out_alpha_host, act, res, y, Tout, path, stream, nullptr, lanes.get());
 }
 
 int fac_debug_resunit(fac_handle* h, const float* x, const float* w7_host, const float* b7_host, const float* w1_host,
@@ -5071,11 +4993,11 @@ int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host,
                             const float* alpha2_host, int B, int T, int C, int dil, int mode, int causal,
                             const int* lane_len_host, float* y, void* stream) {
     if (!h || !x || !y || !w7_host || !w1_host || B <= 0 || T <= 0) return FAC_ERR_INVALID;
-    int* lanes = nullptr;
-    int rc0 = debug_upload_lanes(h, "fac_debug_resunit_lanes", lane_len_host, B, T, &lanes);
-    if (rc0 != FAC_OK) return rc0;
-    if (mode < 0 || mode > 8) { cudaFree(lanes); return FAC_ERR_INVALID; }
-    fac_handle tmp;
+    DevBuf<int> lanes;
+    int rc = debug_upload_lanes(h, "fac_debug_resunit_lanes", lane_len_host, B, T, lanes);
+    if (rc != FAC_OK) return rc;
+    if (mode < 0 || mode > 8) return FAC_ERR_INVALID;
+    fac_handle tmp;             // carries this call's precision options
     tmp.device = h->device;
     // 0: fp32 FMA, 1: two tensor-core launches, 2: fused launch; 3/4 = 1/2 with bf16 split; 5/6 = 3/4 with the k = 7 conv
     // in one fp16 pass; 7/8 = 1/2 as an encoder unit (promoted fp16 hi + scaled lo, upstream of the VQ)
@@ -5085,11 +5007,12 @@ int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host,
     tmp.dec_bf16 = mode >= 3 && !enc;
     tmp.dec_c7_f16 = mode >= 5 && !enc;
     tmp.tc_occ2 = h->tc_occ2;
+    TensorMap ts;
     auto put = [&](const char* key, const float* d, std::vector<int64_t> shp) {
         HostTensor t;
         t.shape = shp;
         t.data.assign(d, d + t.numel());
-        tmp.host[0][key] = std::move(t);
+        ts[key] = std::move(t);
     };
     put("u.block.0.alpha", alpha1_host, {1, C, 1});
     put("u.block.1.conv.conv.weight", w7_host, {C, C, 7});
@@ -5097,30 +5020,25 @@ int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host,
     put("u.block.2.alpha", alpha2_host, {1, C, 1});
     put("u.block.3.conv.conv.weight", w1_host, {C, C, 1});
     put("u.block.3.conv.conv.bias", b1_host, {C});
+    Packer P;
     ResW r;
-    try { r = pack_res(&tmp, 0, "u", dil, enc); } catch (const PackError& e) { h->err = e.msg; cudaFree(lanes); return FAC_ERR_STATE; }
-    cudaSetDevice(h->device);
-    cudaError_t e = cudaMalloc(&tmp.warena, (tmp.pack.size() + 64) * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(tmp.warena, tmp.pack.data(), tmp.pack.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); cudaFree(lanes); return FAC_ERR_CUDA; }
+    try { r = pack_res(P, ts, "u", dil, enc); } catch (const PackError& e) { h->err = e.msg; return FAC_ERR_STATE; }
+    DevBuf<float> w;
+    rc = upload_weights(h, P, w, "fac_debug_resunit_lanes");
+    if (rc != FAC_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    float* scratch = nullptr;
-    e = cudaMalloc(&scratch, sizeof(float) * (size_t)B * T * C);
-    int rc = FAC_OK;
-    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); rc = FAC_ERR_CUDA; }
-    if (rc == FAC_OK) {
-        Ctx c{&tmp, st, false};
-        c.vq_critical = enc;
-        residual_unit(c, r, x, scratch, y, B, T, causal != 0, lanes);
-        rc = finish(&tmp, c);
-        cudaError_t e2 = cudaStreamSynchronize(st);
-        if (rc == FAC_OK && e2 != cudaSuccess) { tmp.err = cudaGetErrorString(e2); rc = FAC_ERR_CUDA; }
-        if (rc == FAC_OK && fused && tmp.launches != 1) { tmp.err = "fused path not taken for this geometry"; rc = FAC_ERR_UNSUPPORTED; }
-    }
+    float* p = nullptr;
+    cudaError_t e = cudaMalloc(&p, sizeof(float) * (size_t)B * T * C);
+    DevBuf<float> scratch(p);
+    if (e != cudaSuccess) { h->err = cudaGetErrorString(e); cudaGetLastError(); return FAC_ERR_CUDA; }
+    Ctx c{&tmp, st, false, w.get()};
+    c.vq_critical = enc;
+    residual_unit(c, r, x, scratch.get(), y, B, T, causal != 0, lanes.get());
+    rc = finish(&tmp, c);
+    cudaError_t e2 = cudaStreamSynchronize(st);
+    if (rc == FAC_OK && e2 != cudaSuccess) { tmp.err = cudaGetErrorString(e2); rc = FAC_ERR_CUDA; }
+    if (rc == FAC_OK && fused && tmp.launches != 1) { tmp.err = "fused path not taken for this geometry"; rc = FAC_ERR_UNSUPPORTED; }
     if (rc != FAC_OK) h->err = tmp.err;
-    if (scratch) cudaFree(scratch);
-    cudaFree(tmp.warena);
-    cudaFree(lanes);
     return rc;
 }
 
@@ -5129,18 +5047,19 @@ int fac_debug_resunit_lanes(fac_handle* h, const float* x, const float* w7_host,
 // Returns the number of 32-bit words (G*H*4U); info3 = {U, G, 4U}.
 long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out, long long capacity_floats, int* info3) {
     if (!whh_host || H <= 0) return FAC_ERR_INVALID;
-    fac_handle tmp;
     const char* names[8] = {"weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0", "weight_ih_l1", "weight_hh_l1", "bias_ih_l1", "bias_hh_l1"};
+    TensorMap ts;
     for (int i = 0; i < 8; ++i) {
         HostTensor t;
         const bool mat = (i % 4) < 2;
         if (mat) t.shape = {4 * H, H}; else t.shape = {4 * H};
         if (i == 1) t.data.assign(whh_host, whh_host + (size_t)4 * H * H);
         else t.data.assign(t.numel(), 0.f);
-        tmp.host[0][std::string("l.") + names[i]] = std::move(t);
+        ts[std::string("l.") + names[i]] = std::move(t);
     }
+    Packer P;
     LstmW L;
-    try { L = pack_lstm(&tmp, 0, "l"); } catch (const PackError&) { return FAC_ERR_UNSUPPORTED; }
+    try { L = pack_lstm(P, ts, "l"); } catch (const PackError&) { return FAC_ERR_UNSUPPORTED; }
     if (info3) { info3[0] = L.U; info3[1] = L.G; info3[2] = 4 * L.U; }
     if (bf16 == 2 || bf16 == 3) {
         // lstm2.cu layouts: 2 = one fp16 pass [G][H/16][8][4U] words, 3 = fp16 hi + scaled lo [G][H/16][hi|lo][8][4U]
@@ -5153,7 +5072,7 @@ long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out
     const long long n = (long long)L.G * H * 4 * L.U;
     if (bf16 && !L.has16) return FAC_ERR_UNSUPPORTED;
     if (!out || capacity_floats < n) return n;
-    memcpy(out, tmp.pack.data() + (bf16 ? L.whh16[0] : L.whh[0]), sizeof(float) * (size_t)n);
+    memcpy(out, P.pack.data() + (bf16 ? L.whh16[0] : L.whh[0]), sizeof(float) * (size_t)n);
     return n;
 }
 
@@ -5162,22 +5081,23 @@ long long fac_debug_lstm_pack(const float* whh_host, int H, int bf16, float* out
 // [taps][Cin][s*Cout] (phase-major output channels r*Cout + co); returns the number of floats.
 long long fac_debug_convtr_pack(const float* w_host, int Cin, int Cout, int stride, int causal, float* out, long long capacity_floats) {
     if (!w_host || Cin <= 0 || Cout <= 0 || stride <= 0) return FAC_ERR_INVALID;
-    fac_handle tmp;
     HostTensor t, b;
     t.shape = {Cin, Cout, 2 * stride};
     t.data.assign(w_host, w_host + (size_t)Cin * Cout * 2 * stride);
     b.shape = {Cout};
     b.data.assign(Cout, 0.f);
-    tmp.host[0]["c.weight"] = std::move(t);
-    tmp.host[0]["c.bias"] = std::move(b);
+    TensorMap ts;
+    ts["c.weight"] = std::move(t);
+    ts["c.bias"] = std::move(b);
+    Packer P;
     ConvW c;
-    try { c = causal ? pack_convtr(&tmp, 0, "c", stride) : pack_convtr_noncausal(&tmp, 0, "c", stride); }
+    try { c = causal ? pack_convtr(P, ts, "c", stride) : pack_convtr_noncausal(P, ts, "c", stride); }
     catch (const PackError&) { return FAC_ERR_UNSUPPORTED; }
     const long long n = (long long)c.K * Cin * c.Cout;
     if (!out || capacity_floats < n) return n;
     for (int k = 0; k < c.K; ++k)
         for (int ci = 0; ci < Cin; ++ci)
-            for (int co = 0; co < c.Cout; ++co) out[((size_t)k * Cin + ci) * c.Cout + co] = tmp.pack[c.w + ((size_t)k * Cin + ci) * c.ldw + co];
+            for (int co = 0; co < c.Cout; ++co) out[((size_t)k * Cin + ci) * c.Cout + co] = P.pack[c.w + ((size_t)k * Cin + ci) * c.ldw + co];
     return n;
 }
 
